@@ -8,6 +8,7 @@ of the full-resolution scan, vertex append, per-voxel dilation / Delaunay / pull
   python bench.py --gpus 1 --steps K --warmup W               our CUDA path (N>1: launched under torchrun)
   python bench.py --impl reference --gpus 1 --steps K ...     the reference algorithm on the host cores (oracle port)
   python bench.py --config C1|C2|C3|C4|C5|C5s1                the other BASELINE.json configurations (default: the 100k metric config)
+  python bench.py ... --dump-outputs DIR                      also write what the last timed step computed as DIR/<name>.npy
 
 Prints ONE JSON line (rank 0).  `value` = scans/s with the scans already resident in HBM (device-event time, L2
 flushed between scans); `e2e` = scans/s through the C ABI with pinned HOST buffers (H2D of both clouds and D2H of the
@@ -296,6 +297,25 @@ def algorithmic_bytes(kernel, info):
     return None
 
 
+def dump_outputs(out_dir, arrays, budget=64 << 20, seed=0):
+    """Write every array as out_dir/<name>.npy (float32 stays float32, everything else becomes float64).  Arrays of 1 MB and more
+    share what the small ones leave of `budget`: one over its share is replaced by a fixed seeded sample of its rows (in row
+    order), so equal shapes give equal samples from run to run."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float32 if np.asarray(v).dtype == np.float32 else np.float64) for k, v in arrays.items()}
+    small = sum(a.nbytes for a in arrays.values() if a.nbytes < (1 << 20))
+    large = sum(a.nbytes for a in arrays.values() if a.nbytes >= (1 << 20))
+    scale = min(1.0, (budget - small - 4096 * len(arrays)) / large) if large else 1.0    # 4 KB per file for the .npy header
+    written = {}
+    for name, a in arrays.items():
+        if a.nbytes >= (1 << 20) and scale < 1.0:
+            rows = max(1, int(a.shape[0] * scale))
+            a = a[np.sort(np.random.default_rng(seed).choice(a.shape[0], rows, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        written[name] = list(a.shape)
+    return written
+
+
 def pin(a):
     """Page-locked copy of a numpy array (the e2e inputs live in pinned host memory, the C ABI then DMAs straight from them)."""
     import torch
@@ -434,14 +454,14 @@ def run_gpu(args, rank, world):
     MW = wl["map_warm"]
     n_prof = min(K, 10)
     n_stage = min(K, 10)
-    K_raw = 0 if args.no_raw_leg else min(K, 20)
+    K_raw = 0 if args.no_raw_leg else K
     n_scans = 1 + MW + W + 2 * K + K_raw + n_stage + n_prof + 1 + 6 + K + K_raw    # the last K + K_raw: a second pass of a host-buffer leg (below)
     scans = get_stream(wl, n_scans, seed=rank if args.independent_streams else 0)
     lib = api.load_library()
     dev = torch.device("cuda", local_rank)
     d_ds = [torch.from_numpy(s["body_ds"]).to(dev) for s in scans]
     d_full = [torch.from_numpy(s["body_full"]).to(dev) for s in scans]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # 5 x the 50 MB L2 of an H100
     torch.cuda.synchronize()
 
     # ---- parity gate (before anything is timed): a prefix of THIS stream through the timed path -- pipelined entry points,
@@ -515,10 +535,17 @@ def run_gpu(args, rank, world):
     waits = api.host_wait_ms(lio, mesh)
     host_enqueue_ms = (enq_wall_ms - sum(waits)) / K     # host WORK to queue one scan; the waits are back-pressure from the 2-deep staging slots
     total_ms = api.pipeline_mark_end(lio, mesh)
-    lio.wait()
+    state_last, iters_last = lio.wait()
     mesh.wait()
     barrier()
     launches = api.launch_count(lib) - launches0
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        # what a caller of the timed path holds after its last step: the state and iteration count lio.wait() returns, the mesh
+        # (snapshot) and the VoxelMap (dump) as they stand after that scan
+        verts, tris, flips = mesh.snapshot()
+        dumped = dump_outputs(args.dump_outputs, {"state": state_last, "iterations": [iters_last], "mesh_vertices": verts,
+                                                  "mesh_triangles": tris, "mesh_flips": flips, "voxelmap": lio.dump_map()})
     # the flush alone, to report how much of the timed region it is
     api.pipeline_mark_begin(lio)
     for _ in range(K):
@@ -532,10 +559,9 @@ def run_gpu(args, rank, world):
         k += 1
     lio.wait()
     mesh.wait()
-    # The host-buffer legs are wall-clock measurements with the host in the loop; about one pass in fifteen on the shared boxes showed
-    # a millisecond-scale stall per step (1.1-3.4 ms/step against 0.43, same code, same box, the device-timed region before it
-    # unaffected: profiles/bench_history.md).  A pass slower than half the device-timed rate is measured ONCE more on the scans that
-    # follow; both passes are reported (`attempts_ms_per_step`), the value is the later one.
+    # The host-buffer legs are wall-clock measurements with the host in the loop, and a host shared with other work can stall a whole
+    # pass by milliseconds per step while the device-timed region before it is unaffected.  A pass slower than half the device-timed
+    # rate is measured ONCE more on the scans that follow; both passes are reported (`attempts_ms_per_step`), the value is the later one.
     def slow_pass(seconds, steps):
         # slowest rank's ms/step of this pass against the slowest rank's device-timed ms/step: both reduced, so that every rank takes
         # the same decision (a second pass contains barriers)
@@ -650,7 +676,7 @@ def run_gpu(args, rank, world):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "fallback (H100 SXM data sheet, HBM3)"
     roof = None
     roof_all = {}
     for name in sorted(kern_ms, key=kern_ms.get, reverse=True)[:8]:
@@ -668,12 +694,8 @@ def run_gpu(args, rank, world):
     if b is not None:
         per_launch_bytes = b / kern_launches_per_scan[dominant]
         achieved = per_launch_bytes / (kern_launch_ms[dominant] * 1e-3) / 1e9
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tpath) and args.config == "C100k":
-            traffic = json.load(open(tpath)).get(dominant)
         roof = {"kernel": dominant, "bound": "hbm", "achieved": round(achieved, 3), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 6),
-                "traffic": traffic, "peak_source": peak_src, "bytes_per_launch": round(per_launch_bytes), "ms_per_launch": round(kern_launch_ms[dominant], 5),
+                "peak_source": peak_src, "bytes_per_launch": round(per_launch_bytes), "ms_per_launch": round(kern_launch_ms[dominant], 5),
                 "share_of_step": round(kern_ms[dominant] / sum(kern_ms.values()), 4)}
     # whole-step roofline: algorithmic bytes of every modelled kernel of a scan / the pipelined time per scan
     step_bytes = sum(bb for bb in (algorithmic_bytes(n2, info) for n2 in kern_ms) if bb)
@@ -704,6 +726,7 @@ def run_gpu(args, rank, world):
         "gpu_launches": int(launches),
         "clocks": clocks,
         "parity_gate": gate,
+        "dumped_outputs": dumped,
         "timing_detail": {"l2_flush_ms_per_scan": round(flush_ms, 4),
                           "serial_ms_per_scan_blocking": round(float(np.mean(dev_ms)), 4),
                           "serial_ms_per_scan_blocking_median_p95": [round(float(np.median(dev_ms)), 4), round(float(np.percentile(dev_ms, 95)), 4)],
@@ -796,6 +819,8 @@ def main():
     ap.add_argument("--no-parity-gate", action="store_true", help="experiments only: skip the GPU-vs-oracle check that precedes the timed regions")
     ap.add_argument("--streams", type=int, default=None, help="N=1: also measure this many independent streams interleaved on the one GPU (reported as `multi_stream`; 1 = skip)")
     ap.add_argument("--no-sharded-extra", action="store_true", help="N>1, replicas mode: skip the additional sharded single-stream measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the state, mesh and VoxelMap after the last timed step of `value` as DIR/<name>.npy (at most 64 MB in all)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))

@@ -1,4 +1,4 @@
-"""immesh_b200 -- B200-native (sm_100a CUDA) implementation of the ImMesh per-scan
+"""immesh_b200 -- H100-native (sm_90a CUDA) implementation of the ImMesh per-scan
 localization + meshing hot path behind a C ABI (include/immesh_b200.h).
 
 The Python layer is only a ctypes harness for tests and benchmarks; the product is

@@ -1,6 +1,5 @@
-"""In-tree builds: the CUDA C-ABI library (nvcc, sm_100a), the CPU oracle and the host-emulation
-harness used by the CPU-only logic tests.  Artefacts stay next to the sources so that they travel
-with a gpurun snapshot."""
+"""In-tree builds: the CUDA C-ABI library (nvcc, sm_90a), the CPU oracle and the host-emulation
+harness used by the CPU-only logic tests.  Artefacts stay next to the sources."""
 from __future__ import annotations
 
 import os
@@ -14,10 +13,12 @@ LIB = os.path.join(_HERE, "libimmesh_b200.so")
 EMU = os.path.join(_ROOT, "tests", "emu", "libimmesh_emu.so")
 ORACLE = os.path.join(_ROOT, "oracle", "liborc.so")
 REF_IKD = os.path.join(_ROOT, "oracle", "_ref", "libref_ikd.so")
+# where the reference checkout lies (oracle/Makefile.ref compiles its ikd-Tree from there when it is present)
+REFERENCE = os.environ.get("IMMESH_REFERENCE", "/root/reference")
 GXX = "/usr/bin/g++"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-fmad=false",            # numerics contract: no FMA contraction (bit parity with the reference's SSE2 build)
     "-Xcompiler", "-fPIC", "-shared",
 ]
@@ -36,7 +37,8 @@ def _sources(dirpath, exts):
 
 def build_cuda(force=False, verbose=False):
     cu = _sources(CSRC, (".cu",))
-    deps = cu + _sources(CSRC, (".cuh", ".hpp")) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    # this file is a dependency too: a library built with other NVCC_FLAGS (another architecture) is rebuilt
+    deps = cu + _sources(CSRC, (".cuh", ".hpp")) + [os.path.join(_ROOT, "include", "immesh_b200.h"), os.path.abspath(__file__)]
     if force or _newer(LIB, deps):
         cmd = ["nvcc", *NVCC_FLAGS, "-ccbin", GXX, "-o", LIB, *cu]
         if verbose:
@@ -65,10 +67,10 @@ def build_emu(force=False):
 
 
 def build_ref():
-    """oracle/_ref: the reference's own ikd-Tree compiled unmodified from /root/reference (only in the authoring container;
-    the GPU box uses the prebuilt file that travels with the snapshot)."""
-    if os.path.isdir("/root/reference/include/ikd-Tree"):
-        subprocess.check_call(["make", "-s", "-C", os.path.join(_ROOT, "oracle"), "-f", "Makefile.ref"])
+    """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
+    elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
+    if os.path.isdir(os.path.join(REFERENCE, "include", "ikd-Tree")):
+        subprocess.check_call(["make", "-s", "-C", os.path.join(_ROOT, "oracle"), "-f", "Makefile.ref", f"REF={REFERENCE}"])
     return REF_IKD
 
 

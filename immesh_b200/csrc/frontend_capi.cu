@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(VG_THREADS) k_frontend_pack(const float* __res
 }  // namespace
 
 struct immesh_voxelgrid {
-    int max_points = 0, nblocks_max = 0, n_sm = 148;
+    int max_points = 0, nblocks_max = 0, n_sm = 132;
     cudaStream_t stream = nullptr;
     float* d_in = nullptr;       // staging for host input / packed (calibrated) cloud of immesh_frontend_prepare: the current slot of
     float* d_in_ring[8] = {};   // a ring of 8 (a mesh frame may still be reading the cloud of up to IM_SLOTS + 1 scans ago)

@@ -53,7 +53,7 @@ struct immesh_lio {
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     size_t cap = 0;
     int max_nodes = 0, max_chunks = 0, max_scan = 0;
-    int n_sm = 148;
+    int n_sm = 132;
     int last_n = 0;
     immesh::GraphCtx graph;   // replay of the per-scan launch sequence (pipelined API)
     int use_graph = 1;
@@ -103,7 +103,7 @@ struct immesh_mesh {
     int frame_counter = 0;
     int dilate_bps = 3;       // resident blocks per SM of the dilation kernel
     int warp_nmax = 96;       // largest dilated set triangulated by a single warp
-    int n_sm = 148;
+    int n_sm = 132;
     size_t ccap = 0;
     double last_ms[4] = {0, 0, 0, 0};
     int last_cnt[32];

@@ -279,7 +279,7 @@ IM_HD void so3_log3(const double* R, double* out) {
 // (voxel_loc.cpp:62, mesh_rec_geometry.cpp:199).
 // One rotation, pair (p,q) = (0,1), (0,2), (1,2) for PQ = 0, 1, 2; the pair is a template parameter so that every index into the
 // packed matrix and the eigenvector array is a constant: with a run-time pair the arrays lived in local memory and each rotation paid a
-// dozen dependent local loads/stores on top of its 4 divisions and 2 square roots (profiles/stamps_r02*: 27 k cycles per 3x3 problem).
+// dozen dependent local loads/stores on top of its 4 divisions and 2 square roots.
 template <int PQ>
 IM_HD void jacobi3_rotate(int sweep, double (&a)[6], double (&v)[9]) {
     constexpr int p = (PQ == 2) ? 1 : 0, q = (PQ == 0) ? 1 : 2;

@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const
 
 struct immesh_imu {
     ImuParams P;
-    int max_points = 0, max_imu = 0, nblocks_max = 0, n_sm = 148;
+    int max_points = 0, max_imu = 0, nblocks_max = 0, n_sm = 132;
     // ImuProcess members that live on the host (time stamps) ...
     double last_imu[7] = {0, 0, 0, 0, 0, 0, 0};
     double last_lidar_end_time = -1.0, last_update_time = 0.0;

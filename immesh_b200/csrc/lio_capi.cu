@@ -1,4 +1,4 @@
-// immesh_b200 -- CUDA kernels (sm_100a) and C-ABI host orchestration of the localization path.
+// immesh_b200 -- CUDA kernels (sm_90a) and C-ABI host orchestration of the localization path.
 // Kernel bodies live in lio_core.cuh / voxelmap.cuh; this file adds the launch geometry, the
 // block-level integer reduction of the normal equations, stream/event plumbing and the C ABI.
 // There is no CPU path: every entry point needs a CUDA device and fails loudly without one.
@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(128) k_grow_scatter(ScanBuf sb_) {
 // kernel (few registers: many more warps in flight than the general kernel below, which carries the plane fit and the octree
 // split); only the other voxels go on to k_grow_voxel through a compact list.  At the 1M-point / 0.2 m configuration 175 k voxels
 // are touched per scan and nearly all are of the first kind.  (A THREAD per simple voxel was measured and rejected: one thread's
-// 60 dependent moment read-modify-writes take ~5x longer than the warp's two per lane, profiles/README.md.)
+// 60 dependent moment read-modify-writes take longer than the warp's two per lane.)
 #define GROW_SIMPLE_MAX 4
 __global__ void __launch_bounds__(128) k_grow_simple(VoxelMapDev map, LioParams P, ScanBuf sb, int mode, int* complex_list, int* n_complex) {
     const int lane = threadIdx.x & 31;

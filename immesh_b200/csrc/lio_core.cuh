@@ -351,8 +351,7 @@ struct SolveScratch {
 // 6x6 partial-pivot LU (one thread) + substitution (one thread per column); same operation order as orc::lu_inverse<6>.
 // The factorisation runs on a register copy, every loop unrolled through the step template (a row exchange is a chain of selects, no
 // indexed access -- plain `#pragma unroll` loops with a conditional swap left the copy in local memory):
-// through shared memory, as first written, the one thread's dependent load/store chain took 7.8 k cycles (4 us) per IESKF update
-// (profiles/stamps_r02s_*.txt), a quarter of the whole iteration.
+// through shared memory, as first written, the one thread's dependent load/store chain was a large share of the IESKF update.
 template <int K>
 IM_HD void lu_step6(double (&a)[36], int (&piv)[6]) {
     int best = K;

@@ -1,4 +1,4 @@
-// immesh_b200 -- CUDA kernels (sm_100a) and C-ABI host orchestration of the voxel-wise incremental mesher.
+// immesh_b200 -- CUDA kernels (sm_90a) and C-ABI host orchestration of the voxel-wise incremental mesher.
 // Kernel bodies live in mesh_core.cuh / mesh_voxel.cuh.  No CPU path.
 #include <cuda_runtime.h>
 

@@ -343,7 +343,7 @@ IM_HDN inline void cand_init(const MeshDev& M, const MeshParams& P, const FrameB
 #if defined(__CUDA_ARCH__)
     // The lists are only walked by the kernels after this one, so the moment in which the head already names c while c's link is not
     // stored yet is never observed: one exchange, no fence, no retry.  (A next-store / fence / compare-and-swap loop stood here; the
-    // stamps put 28-30 k of this function's ~45 k cycles into it, profiles/mstamps_r02y.txt.)
+    // stamps put most of this function's cycles into it.)
     F.cand_next[c] = atomicExch(&F.chead[cs], c);
 #else
     F.cand_next[c] = F.chead[cs];

@@ -117,7 +117,7 @@ int immesh_kitti_pose_line(const double* state /*[>= 12]: rot_end[9] row-major, 
 }
 
 const char* immesh_last_error(void) { return immesh::last_error_storage().c_str(); }
-const char* immesh_version(void) { return "immesh_b200 0.1.0 (sm_100a)"; }
+const char* immesh_version(void) { return "immesh_b200 0.1.0 (sm_90a)"; }
 
 int immesh_profile_enable(int on) {
     immesh::profiler().enabled = on != 0;

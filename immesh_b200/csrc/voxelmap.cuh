@@ -29,8 +29,8 @@
 #define IM_BCAST_I(x) (x)
 #endif
 // Predicates of the per-node state machine are evaluated by every lane on data that only lane 0 writes, always behind a warp
-// barrier.  (Taking lane 0's value through a shuffle instead was tried and changed results on the B200 -- tools/debug/lio_diff.py,
-// profiles/README.md round 2 -- so the per-lane evaluation, validated bit for bit against the oracle, stays.)
+// barrier.  (Taking lane 0's value through a shuffle instead was tried and changed results -- tools/debug/lio_diff.py -- so the
+// per-lane evaluation, validated bit for bit against the oracle, stays.)
 #define IM_UPRED(x) (x)
 
 namespace immesh {

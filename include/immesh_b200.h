@@ -1,4 +1,4 @@
-/* immesh_b200 -- C ABI of the B200-native ImMesh localization + meshing hot path.
+/* immesh_b200 -- C ABI of the H100-native (sm_90a) ImMesh localization + meshing hot path.
  *
  * The reference (hku-mars/ImMesh) has no plugin / FFI layer; this header cuts the drop-in
  * boundary at the C++ seams its ROS node calls.  Every entry point names the reference

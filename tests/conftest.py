@@ -10,7 +10,7 @@ for p in (_ROOT, os.path.join(_ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 @pytest.fixture(scope="session")

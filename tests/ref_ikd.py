@@ -1,21 +1,20 @@
 """ctypes wrapper over oracle/_ref/libref_ikd.so -- the REFERENCE's own ikd-Tree (include/ikd-Tree/ikd_Tree.{h,cpp}) compiled
-unmodified by oracle/Makefile.ref.  Test infrastructure only.  The library is (re)built when /root/reference is present (this
-container); on the GPU box only the prebuilt file is used.  `available()` is False when neither exists (tests then skip and
-the committed fixtures under tests/golden/ carry the pin)."""
+unmodified by oracle/Makefile.ref.  Test infrastructure only.  The library is (re)built where the reference checkout is
+present (immesh_b200.build.build_ref); elsewhere a library built earlier is used.  `available()` is False when neither exists
+(tests then skip and the committed fixtures under tests/golden/ carry the pin)."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-_ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_SO = os.path.join(_ROOT, "oracle", "_ref", "libref_ikd.so")
+from immesh_b200 import build as _build
+
+_SO = _build.REF_IKD
 _lib = None
 
 
 def build():
-    if os.path.isdir("/root/reference/include/ikd-Tree"):
-        subprocess.check_call(["make", "-s", "-C", os.path.join(_ROOT, "oracle"), "-f", "Makefile.ref"])
+    _build.build_ref()
     return os.path.exists(_SO)
 
 

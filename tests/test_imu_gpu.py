@@ -1,7 +1,5 @@
 """GPU tier: the IMU front-end (immesh_imu_*, SURVEY 8f-2) through the C ABI against the oracle restatement of
-ImuProcess::UndistortPcl.  Same scenario as tests/test_imu_emu.py (which runs the same device bodies on the CPU, bit-exact).
-
-First hardware run: 3 passed on a B200 (last gpurun call of round 1)."""
+ImuProcess::UndistortPcl.  Same scenario as tests/test_imu_emu.py (which runs the same device bodies on the CPU, bit-exact)."""
 import numpy as np
 import pytest
 

@@ -1,5 +1,5 @@
 // FP64 latency / throughput of this GPU, as the kernels of this repo see it (-fmad=false does not matter here: explicit intrinsics).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench/fp64 tools/microbench/fp64.cu && tools/microbench/fp64
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench/fp64 tools/microbench/fp64.cu && tools/microbench/fp64
 #include <cstdio>
 #include <cuda_runtime.h>
 

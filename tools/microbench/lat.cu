@@ -1,5 +1,5 @@
-// Latency micro-benchmarks behind the design of the 18x18 solve (results quoted in profiles/README.md).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o lat lat.cu && ./lat
+// Latency micro-benchmarks behind the design of the 18x18 solve.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o lat lat.cu && ./lat
 #include <cstdio>
 #include <cuda_runtime.h>
 
