@@ -713,7 +713,17 @@ __global__ void __launch_bounds__(256) k_apply_lists(MeshDev M, FrameBuf F_, con
 }
 
 static int mesh_status(int err) {
-    if (err & (IM_MERR_VERT_POOL | IM_MERR_TRI_POOL | IM_MERR_HASH_FULL | IM_MERR_LIST_CAP | IM_MERR_VOXEL_CAP)) return im_fail(IMMESH_E_CAPACITY, "mesh pool / per-voxel working-set overflow");
+    if (err & (IM_MERR_VERT_POOL | IM_MERR_TRI_POOL | IM_MERR_HASH_FULL | IM_MERR_LIST_CAP | IM_MERR_VOXEL_CAP)) {
+        // name every flag that fired: the caller can tell a full pool from a per-voxel working set over its cap
+        std::string m = "mesh pool / per-voxel working-set overflow (flags:";
+        if (err & IM_MERR_VERT_POOL) m += " VERT_POOL";
+        if (err & IM_MERR_TRI_POOL) m += " TRI_POOL";
+        if (err & IM_MERR_HASH_FULL) m += " HASH_FULL";
+        if (err & IM_MERR_LIST_CAP) m += " LIST_CAP";
+        if (err & IM_MERR_VOXEL_CAP) m += " VOXEL_CAP";
+        m += ")";
+        return im_fail(IMMESH_E_CAPACITY, m.c_str());
+    }
     if (err & (IM_MERR_KEY_RANGE | IM_MERR_PRIO_RANGE)) return im_fail(IMMESH_E_RANGE, "mesh key out of range");
     if (err & IM_MERR_PEER_TIMEOUT) return im_fail(IMMESH_E_CUDA, "sharded mesher: a peer rank did not publish its segment in time (peer window epoch flag)");
     return IMMESH_OK;

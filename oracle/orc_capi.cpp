@@ -250,6 +250,18 @@ long orc_mesh_get_voxels(void* h, int* out, long cap) {
             for (int j = 0; j < 4; ++j) out[i * 4 + j] = rows[i][j];
     return (long)rows.size();
 }
+// per voxel meshed in the last frame, ascending key: x, y, z, dilated-set size, largest cavity, seed found, in-circle ties, duplicates
+long orc_mesh_frame_voxel_stats(void* h, long* out, long cap) {
+    MeshOracle* m = (MeshOracle*)h;
+    const long n = (long)m->frame_stats.size();
+    if (out && n <= cap)
+        for (long i = 0; i < n; ++i) {
+            const MeshOracle::VoxStat& s = m->frame_stats[i];
+            const long row[8] = {s.key[0], s.key[1], s.key[2], s.n, s.max_cav, s.seeded, s.n_ties, s.n_dup};
+            std::memcpy(out + i * 8, row, sizeof(row));
+        }
+    return n;
+}
 void orc_mesh_smooth_all(void* h, double smooth_factor, int knn, double* out) {
     std::vector<std::array<double, 3>> r;
     ((MeshOracle*)h)->smooth_all(smooth_factor, knn, r);

@@ -79,6 +79,10 @@ class Delaunay2D {
     std::vector<int> free_list;
     int last = -1;
     std::vector<int> stamp, cav, link_by_start;  // scratch
+    // path statistics of the last run() (test instrumentation: which kernel path the same input takes on the device)
+    int max_cav = 0;           // largest conflict region (triangles, ghosts included) of one insertion
+    int n_dup = 0;             // insertions skipped because the point coincides with a vertex
+    mutable long n_ties = 0;   // in-circle evaluations that returned exactly 0 (cocircular)
 
     const int64_t* pt(int i) const { return P + 2 * i; }
     bool conflict(const T& t, int p) const {
@@ -95,7 +99,9 @@ class Delaunay2D {
                 const int64_t t2 = (q[0] - b[0]) * dx + (q[1] - b[1]) * dy;
                 return t1 > 0 && t2 < 0;
             }
-        return incircle_i(pt(t.v[0]), pt(t.v[1]), pt(t.v[2]), pt(p)) > 0;
+        const int ic = incircle_i(pt(t.v[0]), pt(t.v[1]), pt(t.v[2]), pt(p));
+        if (ic == 0) ++n_ties;
+        return ic > 0;
     }
     int new_tri(int a, int b, int c) {
         int id;
@@ -111,6 +117,7 @@ class Delaunay2D {
     bool run(const int64_t* pts, int n) {
         P = pts; np = n;
         tris.clear(); free_list.clear();
+        max_cav = 0; n_dup = 0; n_ties = 0;
         if (n < 3) return false;
         // seed: first point distinct from p0, then first non-collinear
         int i1 = -1, i2 = -1;
@@ -163,7 +170,7 @@ class Delaunay2D {
             // p coincides with a vertex of t (duplicate), or lies on the hull line without conflict: look around
             const T& tr = tris[t];
             for (int i = 0; i < 3; ++i)
-                if (tr.v[i] != G && pt(tr.v[i])[0] == pt(p)[0] && pt(tr.v[i])[1] == pt(p)[1]) return;  // duplicate point: skipped (CGAL does too)
+                if (tr.v[i] != G && pt(tr.v[i])[0] == pt(p)[0] && pt(tr.v[i])[1] == pt(p)[1]) { ++n_dup; return; }  // duplicate point: skipped (CGAL does too)
             int found = -1;
             for (int i = 0; i < 3 && found < 0; ++i)
                 if (tr.n[i] >= 0 && conflict(tris[tr.n[i]], p)) found = tr.n[i];
@@ -197,6 +204,7 @@ class Delaunay2D {
                 }
             }
         }
+        if ((int)cav.size() > max_cav) max_cav = (int)cav.size();
         for (int ct : cav) { tris[ct].alive = false; free_list.push_back(ct); }
         // ---- re-triangulate: (a,b,p) per boundary edge
         std::vector<int> created;
@@ -473,10 +481,16 @@ class MeshOracle {
         }
     }
 
+    // per meshed voxel of the last frame: key, dilated-set size, largest Bowyer-Watson cavity, seed found, exact in-circle ties,
+    // duplicate (same snapped point) skips.  Test instrumentation: from n and the cavity a test can tell which kernel path ran.
+    struct VoxStat { int key[3] = {0, 0, 0}; int n = 0, max_cav = 0, seeded = 0, n_dup = 0; long n_ties = 0; };
+    std::vector<VoxStat> frame_stats;
+
     // delaunay_triangulation, mesh_rec_geometry.cpp:174-295 (+ is_face_is_ok :31-57)
-    void triangulate(const std::vector<long>& ids, double* short_axis, std::vector<Tri>& faces) const {
+    void triangulate(const std::vector<long>& ids, double* short_axis, std::vector<Tri>& faces, VoxStat* st = nullptr) const {
         faces.clear();
         const int n = (int)ids.size();
+        if (st) st->n = n;
         if (n < 3) return;
         double c[3] = {0, 0, 0};
         for (int i = 0; i < n; ++i)
@@ -516,7 +530,9 @@ class MeshOracle {
             snapped[2 * i + 1] = std::llrint(uv[2 * i + 1] * inv_q);
         }
         Delaunay2D dt;
-        if (!dt.run(snapped.data(), n)) return;
+        const bool seeded = dt.run(snapped.data(), n);
+        if (st) { st->seeded = seeded; st->max_cav = dt.max_cav; st->n_ties = dt.n_ties; st->n_dup = dt.n_dup; }
+        if (!seeded) return;
         for (const auto& t : dt.tris) {
             if (!t.alive || t.v[0] < 0 || t.v[1] < 0 || t.v[2] < 0) continue;
             bool ok = true;
@@ -585,11 +601,13 @@ class MeshOracle {
         // ---- phase B: triangulate, pull, commit, orient
         struct Res { std::vector<Tri> to_add, to_remove, existing; std::vector<int> flip_add, flip_exist; };
         std::vector<Res> res(work.size());
+        frame_stats.assign(work.size(), VoxStat());
 #pragma omp parallel for num_threads(nthr) schedule(dynamic, 8)
         for (int w = 0; w < (int)work.size(); ++w) {
             Voxel& vx = voxels[work[w].vi];
             std::vector<Tri> faces;
-            triangulate(work[w].ids, vx.short_axis, faces);
+            frame_stats[w].key[0] = vx.key.x; frame_stats[w].key[1] = vx.key.y; frame_stats[w].key[2] = vx.key.z;
+            triangulate(work[w].ids, vx.short_axis, faces, &frame_stats[w]);
             // pull: find_relative_triangulation_combination, triangle.hpp:223-246
             std::set<Tri> pulled;
             const std::vector<long>& ids = work[w].ids;

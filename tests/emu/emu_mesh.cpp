@@ -191,6 +191,7 @@ int emu_mesh_xapply_lists(immesh_mesh_t* h, const int* face4, const unsigned lon
     for (int i = 0; i < nr; ++i) apply_remove(h->M, h->F, rem4[i * 4], rem4[i * 4 + 1], rem4[i * 4 + 2]);
     return 0;
 }
+int emu_mesh_error_word(immesh_mesh_t* h) { return h->last_cnt[3]; }   // IM_MERR_* flags of the last frame
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
     const int* c = h->last_cnt;
     out[0] = c[0]; out[1] = c[2]; out[2] = c[10]; out[3] = c[6] + c[17]; out[4] = c[7]; out[5] = c[8]; out[6] = c[4]; out[7] = c[5];

@@ -18,6 +18,26 @@ def world_scans(kind, n_frames, seed, n_points=None):
     return out
 
 
+def run_scene_parity(lib, scene):
+    """A tests/mesh_scenes.py scene through the implementation under test and the oracle, frame by frame, bit-exact as in
+    run_mesh_parity.  Returns (impl, oracle, the oracle's frame_voxel_stats of the last frame)."""
+    cfg = api.MeshConfig(**{**SMALL, **scene.cfg_kw})
+    g, o = api.Mesh(cfg, lib=lib), OracleMesh(cfg)
+    pose = scene.centre + np.array([0.3, -0.2, 1.5])   # the camera: above the scene, as the orientation flags need one
+    for k, pts in enumerate(scene.frames):
+        g.push_frame(pts, pose, k)
+        o.push_frame(pts, pose, k)
+        cg, co = g.counts(), o.counts()
+        assert cg == co, f"{scene} frame {k}: counts {cg} vs {co}"
+        vg, tg, fg = g.snapshot()
+        vo, to, fo = o.snapshot()
+        assert np.array_equal(vg, vo), f"{scene} frame {k}: vertex positions / ids"
+        assert tg.shape == to.shape and np.array_equal(tg, to), f"{scene} frame {k}: facet set"
+        assert np.array_equal(fg, fo), f"{scene} frame {k}: orientation flags"
+    assert g.counts()["n_vertices"] == scene.n_points, f"{scene}: every point must become a vertex"
+    return g, o, o.frame_voxel_stats()
+
+
 def run_mesh_parity(lib, kind, n_frames, seed, cfg_kw=None, n_points=None, check_every=1):
     cfg = api.MeshConfig(**{**SMALL, **(cfg_kw or {})})
     g, o = api.Mesh(cfg, lib=lib), OracleMesh(cfg)

@@ -203,6 +203,15 @@ class OracleMesh:
         self.L.orc_mesh_get_frame_delta(self.h, _p(a), _p(r))
         return a, r
 
+    def frame_voxel_stats(self):
+        """One row per voxel meshed in the last frame, ascending key: dict of arrays key[m,3], n (dilated-set size), max_cav (largest
+        Bowyer-Watson conflict region, ghost triangles included), seeded, ties (in-circle evaluations == 0), dups (same snapped point)."""
+        self.L.orc_mesh_frame_voxel_stats.restype = C.c_long
+        n = self.L.orc_mesh_frame_voxel_stats(self.h, None, C.c_long(0))
+        o = np.zeros((n, 8), dtype=np.int64)
+        self.L.orc_mesh_frame_voxel_stats(self.h, _p(o), C.c_long(n))
+        return dict(key=o[:, 0:3].astype(np.int32), n=o[:, 3], max_cav=o[:, 4], seeded=o[:, 5].astype(bool), ties=o[:, 6], dups=o[:, 7])
+
     def voxels(self):
         n = self.L.orc_mesh_get_voxels(self.h, None, C.c_long(0))
         o = np.zeros((n, 4), dtype=np.int32)

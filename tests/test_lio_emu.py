@@ -3,7 +3,7 @@ harness (tests/emu), against the oracle -- bit-exact voxel keys, octree shape, m
 import numpy as np
 
 from immesh_b200 import api
-from lio_common import run_stream_parity
+from lio_common import run_degenerate_map_parity, run_stream_parity
 
 
 def test_avia_stream_bit_exact(emu_lib):
@@ -29,3 +29,8 @@ def test_other_residual_bodies_bit_exact(emu_lib):
             run_stream_parity(emu_lib, "hdl64", api.VELODYNE, n_scans=3, seed=2, n_points=16384)
     finally:
         emu_lib.emu_lio_set_split(1)
+
+
+def test_degenerate_root_voxels_bit_exact(emu_lib):
+    # pole, repeated point, exact plane, root and child borders at negative coordinates: NaN-aware, each case asserted
+    run_degenerate_map_parity(emu_lib)

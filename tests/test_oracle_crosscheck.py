@@ -385,3 +385,110 @@ def test_imu_oracle_vs_numpy_propagation():
         T_ei = p_h + v_h * dt + 0.5 * a_h * dt * dt - p_end
         ref = R_end.T @ (R_i @ (x[:3] + lT) + T_ei) - lT
         assert np.allclose(out[s, :3], ref, atol=2e-5), (s, out[s, :3], ref)
+
+
+# ---------------------------------------------------------------- the mesher's per-voxel triangulation without the oracle's Delaunay
+IM_COS150 = -8.65928972248464878803e-01
+
+
+def _scene_facets(scene):
+    from mesh_common import SMALL
+    o = oa.OracleMesh(api.MeshConfig(**{**SMALL, **scene.cfg_kw}))
+    for pts in scene.frames:
+        o.push_frame(pts, scene.centre + np.array([0.3, -0.2, 1.5]))
+    v, t, _ = o.snapshot()
+    return v.astype(np.float64), t, o
+
+
+def _pca_uv(v):
+    """mesh_rec_geometry.cpp:193-213 restated: centroid, covariance / n, ascending eigen-pairs, the sign rule on d0.s and d1.m,
+    l = s x m, projection (d.l, d.m)"""
+    c = v.mean(0)
+    d = v - c
+    w, U = np.linalg.eigh(d.T @ d / len(v))
+    s, m = U[:, 0].copy(), U[:, 1].copy()
+    if d[0] @ s < 0:
+        s = -s
+    if d[1] @ m < 0:
+        m = -m
+    return np.stack([d @ np.cross(s, m), d @ m], 1)
+
+
+def _apex_cos(uv, t):
+    out = []
+    for a, b, c in ((0, 1, 2), (1, 2, 0), (2, 0, 1)):
+        u, w = uv[t[:, b]] - uv[t[:, a]], uv[t[:, c]] - uv[t[:, a]]
+        out.append((u * w).sum(1) / (np.linalg.norm(u, axis=1) * np.linalg.norm(w, axis=1)))
+    return np.stack(out, 1)
+
+
+@pytest.mark.parametrize("n,seed", [(40, 10), (96, 3), (97, 4), (256, 5)])
+def test_voxel_triangulation_matches_numpy_qhull(n, seed):
+    """general-position single-voxel scenes (jitter 3 mm >> the snap unit res * 2^-22 = 0.1 um): the oracle's facet set equals
+    numpy PCA + scipy Delaunay + the 150-degree filter"""
+    import mesh_scenes as ms
+    scene = ms.jittered_patch(n, seed=seed)
+    v, t_orc, _ = _scene_facets(scene)
+    uv = _pca_uv(v)
+    tri = np.sort(Delaunay(uv).simplices, axis=1)
+    cos = _apex_cos(uv, tri)
+    near = (np.abs(cos - IM_COS150) < 1e-9).any(1)
+    keep = ~((cos < IM_COS150) & (cos >= -1.0)).any(1)
+    ref = {tuple(f) for f in tri[keep & ~near]}
+    got = {tuple(f) for f in t_orc} - {tuple(f) for f in tri[near]}
+    assert (~keep).sum() > 0 or n < 90          # the filter is exercised by the larger patches
+    assert got == ref
+
+
+def _invariants(scene, tol_units=8):
+    import scipy.spatial
+    v, t, o = _scene_facets(scene)
+    res = scene.cfg_kw["voxel_resolution"]
+    key = np.round(scene.centre / res)
+    inside = np.where((np.round(v / res) == key).all(1))[0]
+    uv = _pca_uv(v[inside])
+    pos = np.full(len(v), -1)
+    pos[inside] = np.arange(len(inside))
+    t = t[(pos[t] >= 0).all(1)]
+    assert len(t) > 0
+    a, b, c = uv[pos[t[:, 0]]], uv[pos[t[:, 1]]], uv[pos[t[:, 2]]]
+    area2 = (b[:, 0] - a[:, 0]) * (c[:, 1] - a[:, 1]) - (b[:, 1] - a[:, 1]) * (c[:, 0] - a[:, 0])
+    assert (np.abs(area2) > 0).all()
+    hull = scipy.spatial.ConvexHull(uv)
+    assert np.abs(area2).sum() / 2 <= hull.volume * (1 + 1e-9)
+    # empty circumcircles (float64 from the world coordinates): no vertex inside by more than a few snap units
+    unit = res * 2.0 ** -22
+    bx, by, cx, cy = b[:, 0] - a[:, 0], b[:, 1] - a[:, 1], c[:, 0] - a[:, 0], c[:, 1] - a[:, 1]
+    d = 2 * (bx * cy - by * cx)
+    ux = (cy * (bx ** 2 + by ** 2) - by * (cx ** 2 + cy ** 2)) / d
+    uy = (bx * (cx ** 2 + cy ** 2) - cx * (bx ** 2 + by ** 2)) / d
+    cen = a + np.stack([ux, uy], 1)
+    r = np.hypot(ux, uy)
+    dist = np.sqrt(((uv[None, :, :] - cen[:, None, :]) ** 2).sum(-1))
+    assert (dist >= r[:, None] - tol_units * unit).all()
+    return o
+
+
+@pytest.mark.parametrize("name", ["lattice8x8", "lattice16x8", "stacked6x6", "stacked8x8", "ring30", "ring100", "ring250"])
+def test_degenerate_voxel_triangulation_invariants(name):
+    """exact ties, duplicate projections, cocircular rings: non-zero projected areas, no overlap beyond the hull, empty
+    circumcircles up to the snap unit; and the oracle's path statistics see the degeneracy"""
+    import mesh_scenes as ms
+    scene = {s.name: s for s, _ in ms.path_scenes()}[name]
+    o = _invariants(scene)
+    st = ms.centre_stats(o.frame_voxel_stats(), scene, scene.cfg_kw["voxel_resolution"])
+    if name.startswith("lattice"):
+        assert st["ties"] > 0
+    if name.startswith("stacked"):
+        assert st["dups"] == scene.n_points // 2
+    if name.startswith("ring"):
+        n_ring = int(name[4:])
+        assert st["max_cav"] == n_ring - 2 and np.array_equal(o.snapshot()[1], ms.ring_fan(n_ring))
+
+
+def test_collinear_voxel_has_no_seed():
+    import mesh_scenes as ms
+    scene = ms.collinear()
+    v, t, o = _scene_facets(scene)
+    st = ms.centre_stats(o.frame_voxel_stats(), scene, 0.4)
+    assert len(t) == 0 and not st["seeded"] and st["n"] == 12
