@@ -13,6 +13,7 @@ _LIB_PATH = os.path.join(_HERE, "libimmesh_b200.so")
 _lib_cache: dict[str, C.CDLL] = {}
 
 STATE_DOUBLES = 348
+PLANE_MARKER_COLS = 16  # IMMESH_PLANE_MARKER_COLS
 
 
 class _LioCfg(C.Structure):
@@ -102,6 +103,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_push_frame_dev", [vp, vp, C.c_int, dp, C.c_int]),
         ("immesh_mesh_push_frame_from_lio", [vp, vp, vp, C.c_int, C.c_int]),
         ("immesh_lio_match_nodes", [vp, ip, C.c_int]),
+        ("immesh_voxelmap_plane_markers", [vp, dp, C.c_int, ip, C.POINTER(C.c_int64)]),
         ("immesh_voxelmap_build_pv", [vp, dp, dp, C.c_int]),
         ("immesh_voxelmap_update_pv", [vp, dp, dp, C.c_int]),
         ("immesh_residual_build_pv", [vp, dp, dp, dp, C.c_int, ip, dp, C.c_int, ip]),
@@ -359,6 +361,25 @@ class Lio:
         o = np.zeros(4, dtype=np.int64)
         self.lib.immesh_voxelmap_counts(self._h, o.ctypes.data_as(C.POINTER(C.c_int64)))
         return dict(roots=int(o[0]), nodes=int(o[1]), chunks=int(o[2]), err=int(o[3]))
+
+    def plane_markers(self, cap=None):
+        """pubPlaneMap: the markers of the planes refitted since the last call, float64[m, PLANE_MARKER_COLS] rows
+        (kx ky kz path layer id | px py pz nx ny nz | radius min_eig trace alpha), and the counters
+        dict(plane, sub_plane, sub_sub_plane, update, roots_walked).  cap=None sizes the buffer with a count query first; with a
+        cap that is too small the call raises and nothing is consumed."""
+        n = C.c_int(0)
+        cnt = np.zeros(5, dtype=np.int64)
+        pc = cnt.ctypes.data_as(C.POINTER(C.c_int64))
+        if cap is None:
+            rc = self.lib.immesh_voxelmap_plane_markers(self._h, None, 0, C.byref(n), pc)
+            if rc not in (0, -3):
+                _check(self.lib, rc, "voxelmap_plane_markers")
+            cap = n.value
+        rows = np.zeros((max(cap, 1), PLANE_MARKER_COLS))
+        _check(self.lib, self.lib.immesh_voxelmap_plane_markers(self._h, rows.ctypes.data_as(C.POINTER(C.c_double)), cap, C.byref(n), pc),
+               "voxelmap_plane_markers")
+        keys = ("plane", "sub_plane", "sub_sub_plane", "update", "roots_walked")
+        return rows[: n.value], dict(zip(keys, (int(v) for v in cnt)))
 
     def work_stats(self):
         o = np.zeros(4, dtype=np.int64)

@@ -66,6 +66,26 @@ def build_emu(force=False):
     return EMU
 
 
+PUBMAP_DIR = os.path.join(_ROOT, "tests", "pubmap")
+EMU_PUB = os.path.join(PUBMAP_DIR, "libimmesh_emu_pub.so")
+ORACLE_PUB = os.path.join(PUBMAP_DIR, "liborc_pub.so")
+
+
+def build_pubmap(force=False):
+    """tests/pubmap: the host emulation with the plane-map publisher state attached, and the oracle extended by pubPlaneMap
+    (each file includes the library it extends and is built on its own, with that library's flags)."""
+    emu_deps = [os.path.join(PUBMAP_DIR, "emu_pub.cpp")] + _sources(os.path.join(_ROOT, "tests", "emu"), (".cpp",)) + _sources(CSRC, (".cuh", ".hpp"))
+    if force or _newer(EMU_PUB, emu_deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_PUB, "-x", "c++", emu_deps[0]])
+    orc_deps = [os.path.join(PUBMAP_DIR, "orc_pub.cpp")] + _sources(os.path.join(_ROOT, "oracle"), (".cpp", ".hpp"))
+    if force or _newer(ORACLE_PUB, orc_deps):
+        # oracle/Makefile's flags
+        subprocess.check_call([GXX, "-O3", "-std=c++17", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wno-unused-variable",
+                               "-shared", "-o", ORACLE_PUB, orc_deps[0]])
+    return EMU_PUB, ORACLE_PUB
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -78,6 +98,7 @@ def build_all(force=False):
     build_cuda(force)
     build_oracle(force)
     build_emu(force)
+    build_pubmap(force)
     build_ref()
 
 

@@ -22,7 +22,11 @@ struct immesh_lio {
     VoxelMapDev map;
     ScanBuf sb;
     LioCtrl* d_ctrl = nullptr;
-    int* d_counters = nullptr;  // node_count, chunk_bump, avail_top, pending_n, err, n_roots, n_touched, seg_top, work_counter
+    int* d_counters = nullptr;  // node_count, chunk_bump, avail_top, pending_n, err, n_roots, n_touched, seg_top, work_counter, .., pub_n (12)
+    int* d_pub_scratch = nullptr;    // immesh_voxelmap_plane_markers: key sort, per-root row counts / offsets (grown on demand)
+    size_t pub_scratch_ints = 0;
+    double* d_pub_rows = nullptr;    // immesh_voxelmap_plane_markers: the rows of one call (grown on demand)
+    size_t pub_rows_cap = 0;
     int* d_sorted = nullptr;
     int* d_complex = nullptr;   // touched root voxels left to the general warp-per-voxel kernel (the others are finished by k_grow_simple)
     double* d_ptpl = nullptr;

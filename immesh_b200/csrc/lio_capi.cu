@@ -489,6 +489,43 @@ __global__ void k_gather_ptpl(VoxelMapDev map, ScanBuf sb, int n, double* out /*
     }
 }
 
+// ---- plane-map publication (immesh_voxelmap_plane_markers): only the roots in the pending list are visited.
+// The listed roots are ordered by their packed key with two stable radix sorts of the 32-bit halves (low half first), which is the
+// signed (kx, ky, kz) order of the map dump; one thread per root then counts its rows (a walk that clears nothing), an exclusive
+// scan places them, and -- once the host has checked the caller's room -- one thread per root writes its rows and settles its mark.
+namespace {
+#include "radix_sort.cuh"
+}
+#define PUB_THREADS 256
+static_assert(IM_PUB_COLS == IMMESH_PLANE_MARKER_COLS, "plane-marker row width");
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_keys(VoxelMapDev map, int n, int hi, const unsigned int* order, unsigned int* kout, unsigned int* vout) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = order ? order[i] : (unsigned int)i;
+        const unsigned long long key = map.keys[map.pub_list[v]];
+        kout[i] = hi ? (unsigned int)(key >> 32) : (unsigned int)key;
+        vout[i] = v;
+    }
+}
+// per root (in key order): slot, row count; the four reference counters summed with integer atomics (order-free)
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_count(VoxelMapDev map, int n, const unsigned int* order, int* slots, int* cnt, int* counts) {
+    int c[4] = {0, 0, 0, 0};
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int slot = map.pub_list[order[i]];
+        const int root = map.root_node[slot];
+        slots[i] = slot;
+        cnt[i] = root >= 0 ? plane_pub_root(map, root, map.keys[slot], nullptr, c) : 0;
+    }
+    for (int k = 0; k < 4; ++k)
+        if (c[k]) atomicAdd(counts + k, c[k]);
+}
+// per root: its rows at its offset, flags cleared; roots that stay pending go back on the (reset) list
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_emit(VoxelMapDev map, int n, const int* slots, const int* off, double* rows) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int slot = slots[i];
+        if (plane_pub_commit(map, slot, rows + (size_t)off[i] * IM_PUB_COLS)) map.pub_list[atomicAdd(map.pub_n, 1)] = slot;
+    }
+}
+
 // ------------------------------------------------------------------ host side
 
 #include "nccl_api.hpp"
@@ -591,6 +628,10 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     m.node_count = h->d_counters + 0; m.chunk_bump = h->d_counters + 1; m.avail_top = h->d_counters + 2; m.pending_n = h->d_counters + 3;
     m.err = h->d_counters + 4; m.n_roots = h->d_counters + 5; m.stat = h->d_counters + 9;
     m.max_nodes = h->max_nodes; m.max_chunks = h->max_chunks;
+    IM_CREATE(dev_alloc(h, &m.pub, (size_t)h->max_nodes));
+    IM_CREATE(dev_alloc(h, &m.pub_mark, h->cap, 0));
+    IM_CREATE(dev_alloc(h, &m.pub_list, h->cap));
+    m.pub_n = h->d_counters + 12;
     ScanBuf& sb = h->sb;
     const size_t ms = (size_t)h->max_scan;
     float* d_body = nullptr;
@@ -643,6 +684,8 @@ int immesh_lio_destroy(immesh_lio_t* h) {
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && nccl().CommDestroy) nccl().CommDestroy(h->nccl_comm);
     for (void* p : h->allocs) cudaFree(p);
+    if (h->d_pub_scratch) cudaFree(h->d_pub_scratch);
+    if (h->d_pub_rows) cudaFree(h->d_pub_rows);
     if (h->h_body) cudaFreeHost(h->h_body);
     if (h->h_state) cudaFreeHost(h->h_state);
     if (h->h_ints) cudaFreeHost(h->h_ints);
@@ -1147,6 +1190,70 @@ int64_t immesh_voxelmap_dump(immesh_lio_t* h, double* rows, int64_t cap_rows) {
         cudaMemcpy(planes.data(), h->map.planes, (size_t)nn * sizeof(PlaneRec), cudaMemcpyDeviceToHost);
     }
     return dump_voxelmap(keys.data(), roots.data(), h->cap, nodes.data(), planes.data(), rows, cap_rows);
+}
+
+int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n_out, int64_t* counts) {
+    if (!h || !n_out || cap < 0 || (cap > 0 && !rows)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    *n_out = 0;
+    if (counts) for (int k = 0; k < 5; ++k) counts[k] = 0;
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // everything queued on the handle, the pipelined steps included
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, h->map.pub_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    const int n = h->h_ints[40];
+    if (counts) counts[4] = n;
+    if (n == 0) return IMMESH_OK;
+    const int nb = (n + VG_TILE - 1) / VG_TILE;
+    const size_t need = (size_t)6 * n + (size_t)256 * nb + 8;
+    if (need > h->pub_scratch_ints) {
+        if (h->d_pub_scratch) cudaFree(h->d_pub_scratch);
+        h->d_pub_scratch = nullptr;
+        h->pub_scratch_ints = 0;
+        IM_CUDA(cudaMalloc((void**)&h->d_pub_scratch, need * sizeof(int)));
+        h->pub_scratch_ints = need;
+    }
+    unsigned int* ku[2] = {(unsigned int*)h->d_pub_scratch, (unsigned int*)h->d_pub_scratch + n};
+    unsigned int* vu[2] = {(unsigned int*)h->d_pub_scratch + 2 * (size_t)n, (unsigned int*)h->d_pub_scratch + 3 * (size_t)n};
+    int* slots = h->d_pub_scratch + 4 * (size_t)n;
+    int* cnt = h->d_pub_scratch + 5 * (size_t)n;
+    int* hist = h->d_pub_scratch + 6 * (size_t)n;
+    int* misc = hist + (size_t)256 * nb;   // [0] rows in all, [1..4] the reference's counters
+    cudaStream_t st = h->stream;
+    const int g = std::min((n + PUB_THREADS - 1) / PUB_THREADS, h->n_sm * 16);
+    IM_CUDA(cudaMemsetAsync(misc, 0, 8 * sizeof(int), st));
+    int cur = 0;
+    for (int half = 0; half < 2; ++half) {
+        IM_LAUNCH(k_pub_keys, g, PUB_THREADS, 0, st, h->map, n, half, half ? (const unsigned int*)vu[cur] : (const unsigned int*)nullptr, ku[cur ^ half], vu[cur ^ half]);
+        cur ^= half;
+        for (int pass = 0; pass < 4; ++pass) {
+            IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], n, 8 * pass, hist, nb);
+            IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
+            IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
+            cur ^= 1;
+        }
+    }
+    IM_LAUNCH(k_pub_count, g, PUB_THREADS, 0, st, h->map, n, (const unsigned int*)vu[cur], slots, cnt, misc + 1);
+    IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, cnt, n, misc);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, misc, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    const int total = h->h_ints[40];
+    *n_out = total;
+    if (counts) for (int k = 0; k < 4; ++k) counts[k] = h->h_ints[41 + k];
+    if (total > cap) return im_fail(IMMESH_E_CAPACITY, "plane markers: more rows than cap (*n_out holds the number needed; nothing was consumed)");
+    if ((size_t)total > h->pub_rows_cap || !h->d_pub_rows) {
+        if (h->d_pub_rows) cudaFree(h->d_pub_rows);
+        h->d_pub_rows = nullptr;
+        h->pub_rows_cap = 0;
+        const size_t rc = std::max<size_t>((size_t)total, 1024);
+        IM_CUDA(cudaMalloc((void**)&h->d_pub_rows, rc * IM_PUB_COLS * sizeof(double)));
+        h->pub_rows_cap = rc;
+    }
+    IM_CUDA(cudaMemsetAsync(h->map.pub_n, 0, sizeof(int), st));
+    IM_LAUNCH(k_pub_emit, g, PUB_THREADS, 0, st, h->map, n, (const int*)slots, (const int*)cnt, h->d_pub_rows);
+    IM_CUDA(cudaGetLastError());
+    if (total > 0) IM_CUDA(cudaMemcpyAsync(rows, h->d_pub_rows, (size_t)total * IM_PUB_COLS * sizeof(double), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    return IMMESH_OK;
 }
 
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out) {

@@ -94,9 +94,18 @@ struct alignas(16) Chunk {
     int pad_[7];
     double var[6][8];
 };
+// What the plane-map publisher (pubPlaneMap, voxel_mapping.cpp:947-1159) reads besides the plane record, kept out of PlaneRec so
+// that the record's first 128-B line stays what k_match reads.
+struct alignas(16) PubRec {
+    float p_center[3];   // Plane::m_p_center x y z: the centre of the last PLANAR fit (voxel_loc.cpp:111-113), zero until there is one
+    float p_normal[3];   // m_p_center.normal_x/y/z, same rule (:114-116)
+    int updated;         // Plane::m_is_update: set by every fit, planar or not (:118, :136), cleared when the plane is published
+    int pad_;
+};
 static_assert(sizeof(PlaneRec) == 256, "PlaneRec must be 256 B");
 static_assert(sizeof(NodeRec) == 656, "NodeRec must be 656 B");
 static_assert(sizeof(Chunk) == 512, "Chunk must be 512 B");
+static_assert(sizeof(PubRec) == 32, "PubRec must be 32 B");
 
 enum : int {
     IM_ERR_KEY_RANGE = 1,
@@ -126,6 +135,13 @@ struct VoxelMapDev {
     int* err;
     int* n_roots;
     int* stat;   // optional work counters of the current scan: [0] plane refits, [1] points read by them (roofline byte model); may be null
+    // plane-map publication: per node PubRec; per hash slot a "pending" mark, and the list of marked slots (pub_n entries).  A root
+    // is marked by the first fit under it after it left the list; the publication walk visits only the listed roots.  pub == null:
+    // a map without the publisher (the library always allocates it; the host emulation of the other entry points does not).
+    PubRec* pub;
+    int* pub_mark;
+    int* pub_list;
+    int* pub_n;
 };
 
 #define IM_EMPTY_KEY 0xFFFFFFFFFFFFFFFFull
@@ -258,6 +274,11 @@ IM_HD void init_node(const VoxelMapDev& m, int id, int layer, const double* vc, 
     for (int i = 0; i < 21; ++i) p.pv[i] = 0.0;
     p.points_size = 0;
     p.plane_inited = 0;
+    if (m.pub) {
+        PubRec& q = m.pub[id];
+        for (int i = 0; i < 3; ++i) { q.p_center[i] = 0.f; q.p_normal[i] = 0.f; }
+        q.updated = 0;
+    }
 }
 // new root voxel, voxel_mapping.cpp:136-141 / :345-350
 IM_HD int make_root(const VoxelMapDev& m, const LioParams& P, unsigned long long key, int slot) {
@@ -456,6 +477,18 @@ IM_HDN inline void init_plane(const VoxelMapDev& m, const LioParams& P, int nd, 
             pl.is_plane = 0;
         }
         pl.plane_inited = 1;
+        if (m.pub) {   // plane-map publisher state (absent from a map built without it)
+            PubRec& q = m.pub[nd];
+            if (planar)
+                for (int i = 0; i < 3; ++i) { q.p_center[i] = (float)c[i]; q.p_normal[i] = (float)U[i * 3 + imin]; }
+            q.updated = 1;
+            // one warp grows a root voxel at a time, so the mark of this root is not contended
+            const int rs = n.root_slot;
+            if (m.pub_mark[rs] == 0) {
+                m.pub_mark[rs] = 1;
+                m.pub_list[im_atomic_add(m.pub_n, 1)] = rs;
+            }
+        }
     }
     IM_SYNCWARP();
 }
@@ -634,6 +667,74 @@ IM_HDN inline void update_octo_tree(const VoxelMapDev& m, const LioParams& P, in
         }
         return;
     }
+}
+
+// ------------------------------------------------------------------ plane-map publication (pubPlaneMap, voxel_mapping.cpp:947-1159)
+// One root voxel of the reference's walk, literally:
+//   root flag set            -> publish the root (radius 1.25 r, alpha = is_plane), clear; its children are not looked at
+//   else each child i        -> flag set: publish (1.25 r, alpha = is_plane), clear; its children are not looked at
+//   else each grandchild j   -> octo_state == 0 and flag set: counted as a sub-sub plane; published (radius r, alpha 1) and
+//                               cleared only when planar, a non-planar one keeps its flag
+//   layers >= 3 are never published.
+// Row (IM_PUB_COLS doubles): kx ky kz path layer id | p_center xyz, p_center normal xyz (floats) | radius (the float pubPlane is
+// given) | min_eig | trace | alpha.  path: the dump's encoding (child l -> path * 9 + l + 1); id: the node record index;
+// trace: (pv00 + pv11) + pv22, the order of Eigen's 3-vector sum.  rows == nullptr: nothing written, no flag cleared (a count).
+// counts (may be null) += plane, sub-plane, sub-sub-plane and update counts of the reference's two log lines.
+#define IM_PUB_COLS 16
+IM_HD void plane_pub_row(const VoxelMapDev& m, int nd, long long kx, long long ky, long long kz, long long path, int layer, bool scaled, double* row) {
+    const PlaneRec& pl = m.planes[nd];
+    const PubRec& q = m.pub[nd];
+    row[0] = (double)kx; row[1] = (double)ky; row[2] = (double)kz;
+    row[3] = (double)path; row[4] = (double)layer; row[5] = (double)nd;
+    for (int i = 0; i < 3; ++i) { row[6 + i] = (double)q.p_center[i]; row[9 + i] = (double)q.p_normal[i]; }
+    row[12] = scaled ? (double)(float)(1.25 * (double)pl.radius) : (double)pl.radius;
+    row[13] = (double)pl.min_eig;
+    row[14] = (pl.pv[0] + pl.pv[6]) + pl.pv[11];
+    row[15] = scaled ? (pl.is_plane ? 1.0 : 0.0) : 1.0;
+}
+IM_HD int plane_pub_root(const VoxelMapDev& m, int root, unsigned long long key, double* rows, int* counts) {
+    long long kx, ky, kz;
+    unpack_key(key, &kx, &ky, &kz);
+    int c[4] = {0, 0, 0, 0};
+    int nrow = 0;
+    if (m.pub[root].updated) {
+        if (rows) { plane_pub_row(m, root, kx, ky, kz, 0, 0, true, rows); m.pub[root].updated = 0; }
+        nrow = 1; c[0] = 1; c[3] = 1;
+    } else {
+        for (int i = 0; i < 8; ++i) {
+            const int ch = m.nodes[root].children[i];
+            if (ch < 0) continue;
+            if (m.pub[ch].updated) {
+                if (rows) { plane_pub_row(m, ch, kx, ky, kz, i + 1, 1, true, rows + (size_t)nrow * IM_PUB_COLS); m.pub[ch].updated = 0; }
+                ++nrow; ++c[1]; ++c[3];
+                continue;
+            }
+            for (int j = 0; j < 8; ++j) {
+                const int g = m.nodes[ch].children[j];
+                if (g < 0 || m.nodes[g].octo_state != 0 || !m.pub[g].updated) continue;
+                if (m.planes[g].is_plane) {
+                    if (rows) { plane_pub_row(m, g, kx, ky, kz, (long long)(i + 1) * 9 + (j + 1), 2, false, rows + (size_t)nrow * IM_PUB_COLS); m.pub[g].updated = 0; }
+                    ++nrow; ++c[3];
+                }
+                ++c[2];
+            }
+        }
+    }
+    if (counts)
+        for (int k = 0; k < 4; ++k) counts[k] += c[k];
+    return nrow;
+}
+// Publish the root listed at `slot` into rows[] (room for what plane_pub_root counted) and settle its mark: the root stays pending
+// while the same walk over what is left would publish something (a child held back by the root's own flag, a grandchild behind a
+// child that was published), and leaves the list otherwise -- flags that can never be published (non-planar or split layer-2 nodes,
+// layers >= 3) do not keep it there; the next fit under it marks it again.  Returns 1 when the root stays pending.
+IM_HD int plane_pub_commit(const VoxelMapDev& m, int slot, double* rows) {
+    const int root = m.root_node[slot];
+    if (root < 0) { m.pub_mark[slot] = 0; return 0; }
+    plane_pub_root(m, root, m.keys[slot], rows, nullptr);
+    const int again = plane_pub_root(m, root, m.keys[slot], nullptr, nullptr) > 0 ? 1 : 0;
+    if (!again) m.pub_mark[slot] = 0;
+    return again;
 }
 
 // ------------------------------------------------------------------ residual selection

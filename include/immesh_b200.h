@@ -144,6 +144,28 @@ int immesh_lio_match_nodes(immesh_lio_t* h, int* plane_node /*[n] plane record i
 /* canonical dump of the VoxelMap (roots by ascending key, nodes in pre-order), 45 doubles per node */
 int64_t immesh_voxelmap_dump(immesh_lio_t* h, double* rows, int64_t cap_rows);
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out /*[4]: roots, nodes, chunks_in_use, error_flags*/);
+
+/* pubPlaneMap(m_feat_map, voxel_pub, state.pos_end) (src/voxel_mapping.cpp:947-1159), called after voxel_map_init and after every
+ * map_incremental_grow (:1899-1900, :1975-1976): the markers of the planes refitted since the last call, one row per pubPlane call
+ * (:919-945), with the reference's walk -- a root whose m_is_update flag is set is published and its children wait for a later
+ * call; else each child with the flag; else each grandchild with octo_state 0 and the flag, published only when planar (radius
+ * not scaled by 1.25), a non-planar one keeping its flag; deeper layers never.  Every flag published is cleared.
+ * Row = IMMESH_PLANE_MARKER_COLS doubles:
+ *   kx ky kz path layer id | px py pz nx ny nz | radius min_eig trace alpha
+ *   key and path as in immesh_voxelmap_dump; id: the node's record index (stable while the node lives, unique per handle; the
+ *   reference's g_plane_id counter is not reproduced); p / n: Plane::m_p_center, the float centre and normal of the node's last
+ *   PLANAR fit (zeros if it never was one); radius: the float pubPlane receives (1.25 m_radius at layers 0 and 1, m_radius at
+ *   layer 2); min_eig: m_min_eigen_value; trace: (pv00 + pv11) + pv22 of m_plane_var (0 for a non-planar fit); alpha: 1 if planar.
+ *   The node colours with mapJet(pow(min(trace, 0.25) / 0.25, 0.2), 0, 1) and builds the marker with its own pubPlane (:978-990).
+ * Rows are in ascending root key (the dump's order), then in the reference's child order.  Only roots under which a plane was
+ * fitted since the last call, or whose markers were held back by it, are visited.  Blocking: waits for the work queued on h.
+ * counts (or NULL) = [plane, sub-plane, sub-sub-plane, update counts as printed by the reference (:1154-1158), roots walked];
+ * they cover the roots walked, so a non-planar layer-2 flag, which the reference counts as a sub-sub plane again on every call,
+ * is counted only while its root is visited.
+ * *n_out > cap: returns IMMESH_E_CAPACITY with *n_out = rows needed and nothing consumed (cap = 0: a pure count query).
+ * A sharded handle publishes the roots it owns. */
+#define IMMESH_PLANE_MARKER_COLS 16
+int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows /*[cap][16] or NULL*/, int cap, int* n_out, int64_t* counts /*[5] or NULL*/);
 /* device time (ms, CUDA events on the handle's stream) of the stages of the last immesh_lio_step call:
  * [0] whole step incl. H2D, [1] residual+solve iterations, [2] map update */
 int immesh_lio_last_timing(immesh_lio_t* h, double* ms /*[3]*/);
