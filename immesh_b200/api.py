@@ -14,6 +14,7 @@ _lib_cache: dict[str, C.CDLL] = {}
 
 STATE_DOUBLES = 348
 PLANE_MARKER_COLS = 16  # IMMESH_PLANE_MARKER_COLS
+SCAN_PUB_COLS = 4       # IMMESH_SCAN_PUB_COLS: x y z intensity
 
 
 class _LioCfg(C.Structure):
@@ -104,6 +105,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_push_frame_from_lio", [vp, vp, vp, C.c_int, C.c_int]),
         ("immesh_lio_match_nodes", [vp, ip, C.c_int]),
         ("immesh_voxelmap_plane_markers", [vp, dp, C.c_int, ip, C.POINTER(C.c_int64)]),
+        ("immesh_lio_effect_cloud", [vp, fp, ip, C.c_int, ip]),
+        ("immesh_lio_registered_cloud", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, fp, C.c_int, ip]),
         ("immesh_voxelmap_build_pv", [vp, dp, dp, C.c_int]),
         ("immesh_voxelmap_update_pv", [vp, dp, dp, C.c_int]),
         ("immesh_residual_build_pv", [vp, dp, dp, dp, C.c_int, ip, dp, C.c_int, ip]),
@@ -380,6 +383,42 @@ class Lio:
                "voxelmap_plane_markers")
         keys = ("plane", "sub_plane", "sub_sub_plane", "update", "roots_walked")
         return rows[: n.value], dict(zip(keys, (int(v) for v in cnt)))
+
+    def effect_cloud(self):
+        """publish_effect_world: the points matched in the last IESKF iteration as float32[m, SCAN_PUB_COLS] rows x y z intensity
+        (world frame, current state; intensity = sqrt(R_inv), the point's IESKF weight) and their scan indices int32[m], ascending."""
+        n = C.c_int(0)
+        rc = self.lib.immesh_lio_effect_cloud(self._h, None, None, 0, C.byref(n))
+        if rc not in (0, -3):
+            _check(self.lib, rc, "lio_effect_cloud")
+        rows = np.zeros((max(n.value, 1), SCAN_PUB_COLS), dtype=np.float32)
+        idx = np.zeros(max(n.value, 1), dtype=np.int32)
+        _check(self.lib, self.lib.immesh_lio_effect_cloud(self._h, rows.ctypes.data_as(C.POINTER(C.c_float)), idx.ctypes.data_as(C.POINTER(C.c_int)),
+                                                          n.value, C.byref(n)), "lio_effect_cloud")
+        return rows[: n.value], idx[: n.value]
+
+    def registered_cloud(self, pts=None, point_skip=1, intensity_col=-1, on_device=False, n=None, stride=3):
+        """publish_frame_world: points 0, point_skip, 2 point_skip, ... in the world frame of the current state, float32[m, 4] rows
+        x y z intensity (intensity = pts[:, intensity_col], 0 when intensity_col < 0).  pts: float32[n, stride] host array, or with
+        on_device a CUDA address of n rows of `stride` floats; None: the down-sampled scan the handle last localised."""
+        if pts is None:
+            ptr, n, stride, dev = None, 0, 3, 0
+        elif on_device:
+            ptr, dev = C.c_void_p(pts), 1
+        else:
+            a = np.ascontiguousarray(pts, dtype=np.float32)
+            a = a.reshape(a.shape[0], -1)
+            ptr, n, stride, dev = a.ctypes.data_as(C.c_void_p), a.shape[0], a.shape[1], 0
+        n_out = C.c_int(0)
+
+        def call(rows, cap):
+            return self.lib.immesh_lio_registered_cloud(self._h, ptr, n, stride, intensity_col, dev, point_skip, rows, cap, C.byref(n_out))
+        rc = call(None, 0)
+        if rc not in (0, -3):
+            _check(self.lib, rc, "lio_registered_cloud")
+        rows = np.zeros((max(n_out.value, 1), SCAN_PUB_COLS), dtype=np.float32)
+        _check(self.lib, call(rows.ctypes.data_as(C.POINTER(C.c_float)), n_out.value), "lio_registered_cloud")
+        return rows[: n_out.value]
 
     def work_stats(self):
         o = np.zeros(4, dtype=np.int64)

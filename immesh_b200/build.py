@@ -71,19 +71,39 @@ EMU_PUB = os.path.join(PUBMAP_DIR, "libimmesh_emu_pub.so")
 ORACLE_PUB = os.path.join(PUBMAP_DIR, "liborc_pub.so")
 
 
-def build_pubmap(force=False):
-    """tests/pubmap: the host emulation with the plane-map publisher state attached, and the oracle extended by pubPlaneMap
-    (each file includes the library it extends and is built on its own, with that library's flags)."""
-    emu_deps = [os.path.join(PUBMAP_DIR, "emu_pub.cpp")] + _sources(os.path.join(_ROOT, "tests", "emu"), (".cpp",)) + _sources(CSRC, (".cuh", ".hpp"))
-    if force or _newer(EMU_PUB, emu_deps):
+def _emu_ext(src, out, force):
+    """a file that includes tests/emu/emu_lio.cpp and extends it, built on its own with the emulation's flags"""
+    deps = [src] + _sources(os.path.join(_ROOT, "tests", "emu"), (".cpp",)) + _sources(CSRC, (".cuh", ".hpp"))
+    if force or _newer(out, deps):
         subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
-                               "-o", EMU_PUB, "-x", "c++", emu_deps[0]])
-    orc_deps = [os.path.join(PUBMAP_DIR, "orc_pub.cpp")] + _sources(os.path.join(_ROOT, "oracle"), (".cpp", ".hpp"))
-    if force or _newer(ORACLE_PUB, orc_deps):
-        # oracle/Makefile's flags
+                               "-o", out, "-x", "c++", src])
+    return out
+
+
+def _oracle_ext(src, out, force):
+    """a file that includes oracle/orc_capi.cpp and extends it, built on its own with oracle/Makefile's flags"""
+    deps = [src] + _sources(os.path.join(_ROOT, "oracle"), (".cpp", ".hpp"))
+    if force or _newer(out, deps):
         subprocess.check_call([GXX, "-O3", "-std=c++17", "-fPIC", "-fopenmp", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-Wno-unused-variable",
-                               "-shared", "-o", ORACLE_PUB, orc_deps[0]])
-    return EMU_PUB, ORACLE_PUB
+                               "-shared", "-o", out, src])
+    return out
+
+
+def build_pubmap(force=False):
+    """tests/pubmap: the host emulation with the plane-map publisher state attached, and the oracle extended by pubPlaneMap"""
+    return (_emu_ext(os.path.join(PUBMAP_DIR, "emu_pub.cpp"), EMU_PUB, force),
+            _oracle_ext(os.path.join(PUBMAP_DIR, "orc_pub.cpp"), ORACLE_PUB, force))
+
+
+EMU_SCANPUB = os.path.join(PUBMAP_DIR, "libimmesh_emu_scanpub.so")
+ORACLE_SCANPUB = os.path.join(PUBMAP_DIR, "liborc_scanpub.so")
+
+
+def build_scanpub(force=False):
+    """tests/pubmap: the host emulation with the IESKF weights kept and the two scan publishers (effect / registered cloud), and
+    the oracle extended by publish_effect_world / publish_frame_world"""
+    return (_emu_ext(os.path.join(PUBMAP_DIR, "emu_scan_pub.cpp"), EMU_SCANPUB, force),
+            _oracle_ext(os.path.join(PUBMAP_DIR, "orc_scan_pub.cpp"), ORACLE_SCANPUB, force))
 
 
 def build_ref():
@@ -99,6 +119,7 @@ def build_all(force=False):
     build_oracle(force)
     build_emu(force)
     build_pubmap(force)
+    build_scanpub(force)
     build_ref()
 
 

@@ -27,6 +27,17 @@ struct immesh_lio {
     size_t pub_scratch_ints = 0;
     double* d_pub_rows = nullptr;    // immesh_voxelmap_plane_markers: the rows of one call (grown on demand)
     size_t pub_rows_cap = 0;
+    // immesh_lio_effect_cloud / immesh_lio_registered_cloud (all grown on demand)
+    float4* d_spub_rows = nullptr;   // x y z intensity rows of one call
+    size_t spub_rows_cap = 0;
+    int* d_spub_idx = nullptr;       // scan index of each effect row
+    size_t spub_idx_cap = 0;
+    int* d_spub_tiles = nullptr;     // per-tile match counts, scanned in place into offsets; the total behind them
+    size_t spub_tiles_cap = 0;
+    float* d_spub_in = nullptr;      // staging of a host dense cloud (never the scan slots, which hold the localised scan)
+    size_t spub_in_cap = 0;
+    int scan_rows = 0;                      // per-scan buffers: 0 no IESKF run since create / voxelmap_build, 1 last run's, -1 overwritten
+    const char* scan_rows_overwritten_by = nullptr;
     int* d_sorted = nullptr;
     int* d_complex = nullptr;   // touched root voxels left to the general warp-per-voxel kernel (the others are finished by k_grow_simple)
     double* d_ptpl = nullptr;

@@ -526,6 +526,56 @@ __global__ void __launch_bounds__(PUB_THREADS) k_pub_emit(VoxelMapDev map, int n
     }
 }
 
+// ---- scan publishers.  immesh_lio_effect_cloud: a scan-order compaction of match_node >= 0 -- per-tile counts, the one-block
+// exclusive scan over the tiles (k_rs_scan), then each tile emits its rows in order.  immesh_lio_registered_cloud: a strided gather.
+// Both transform with the state in LioCtrl when they run (the handle's current state) and read the scan through scan_load_dyn, so a
+// scan whose count is device resident is published as it was localised.
+#define SPUB_THREADS 256   // one tile of the scan per block
+static_assert(IMMESH_SCAN_PUB_COLS == 4, "scan publisher row width");
+__global__ void __launch_bounds__(SPUB_THREADS) k_eff_count(ScanBuf sb_, int* tile_cnt) {
+    const ScanBuf sb = scan_load_dyn(sb_);
+    const int i = blockIdx.x * SPUB_THREADS + threadIdx.x;
+    const int c = __syncthreads_count(i < sb.n && sb.match_node[i] >= 0);
+    if (threadIdx.x == 0) tile_cnt[blockIdx.x] = c;
+}
+__global__ void __launch_bounds__(SPUB_THREADS) k_eff_emit(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const int* tile_off, float4* rows, int* scan_index) {
+    __shared__ int s_warp[SPUB_THREADS / 32];
+    __shared__ double s_state[12];
+    const ScanBuf sb = scan_load_dyn(sb_);
+    if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
+    const int i = blockIdx.x * SPUB_THREADS + threadIdx.x;
+    const bool m = i < sb.n && sb.match_node[i] >= 0;
+    const unsigned int b = __ballot_sync(0xffffffffu, m);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) s_warp[warp] = __popc(b);
+    __syncthreads();
+    if (!m) return;
+    int off = tile_off[blockIdx.x] + __popc(b & ((1u << lane) - 1u));
+    for (int w = 0; w < warp; ++w) off += s_warp[w];
+    float r[4];
+    scan_pub_row(P, s_state, sb.body + (size_t)i * 3, sb.wsqrt[i], r);
+    rows[off] = make_float4(r[0], r[1], r[2], r[3]);
+    if (scan_index) scan_index[off] = i;
+}
+// rows j = 0 .. ceil(n / skip) - 1 from point j * skip; pts == null: the localised scan
+__global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const float* pts, int n, int stride, int col, int skip, float4* rows) {
+    __shared__ double s_state[12];
+    if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
+    if (!pts) {
+        const ScanBuf sb = scan_load_dyn(sb_);
+        pts = sb.body; n = sb.n; stride = 3; col = -1;
+    }
+    __syncthreads();
+    const int m = n > 0 ? (n - 1) / skip + 1 : 0;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
+        const float* p = pts + (size_t)j * skip * stride;
+        float r[4];
+        scan_pub_row(P, s_state, p, col >= 0 ? p[col] : 0.0f, r);
+        rows[j] = make_float4(r[0], r[1], r[2], r[3]);
+    }
+}
+__global__ void k_scan_n(ScanBuf sb_, int* out) { *out = scan_load_dyn(sb_).n; }
+
 // ------------------------------------------------------------------ host side
 
 #include "nccl_api.hpp"
@@ -572,6 +622,24 @@ static int grid_fixed(const immesh_lio* h, int threads, int max_waves = 8) {
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;
+}
+
+// scan publishers (immesh_lio_effect_cloud / immesh_lio_registered_cloud): buffers grown on demand, the validity of the per-scan rows
+template <class T>
+static int spub_grow(T** p, size_t* cap, size_t need) {
+    if (need <= *cap) return IMMESH_OK;
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+    const size_t c = std::max<size_t>(need, 1024);
+    IM_CUDA(cudaMalloc((void**)p, c * sizeof(T)));
+    *cap = c;
+    return IMMESH_OK;
+}
+static int scan_rows_status(const immesh_lio* h, const char* what) {
+    if (h->scan_rows >= 0) return IMMESH_OK;
+    return im_fail(IMMESH_E_INVALID, (std::string(what) + ": the per-scan buffers were overwritten by " + h->scan_rows_overwritten_by +
+                                      " after the last IESKF run (immesh_lio_estimate / immesh_lio_step*)").c_str());
 }
 
 #if defined(IM_DEBUG_STAMPS)
@@ -645,6 +713,7 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     IM_CREATE(dev_alloc(h, &sb.bv_imu, ms * 6));
     IM_CREATE(dev_alloc(h, &sb.match_node, ms, 0xFF));
     IM_CREATE(dev_alloc(h, &sb.match_layer, ms, 0));
+    IM_CREATE(dev_alloc(h, &sb.wsqrt, ms));
     IM_CREATE(dev_alloc(h, &sb.pw, ms * 3));
     IM_CREATE(dev_alloc(h, &sb.var, ms * 6));
     IM_CREATE(dev_alloc(h, &sb.sortkey, ms));
@@ -686,6 +755,8 @@ int immesh_lio_destroy(immesh_lio_t* h) {
     for (void* p : h->allocs) cudaFree(p);
     if (h->d_pub_scratch) cudaFree(h->d_pub_scratch);
     if (h->d_pub_rows) cudaFree(h->d_pub_rows);
+    for (void* p : {(void*)h->d_spub_rows, (void*)h->d_spub_idx, (void*)h->d_spub_tiles, (void*)h->d_spub_in})
+        if (p) cudaFree(p);
     if (h->h_body) cudaFreeHost(h->h_body);
     if (h->h_state) cudaFreeHost(h->h_state);
     if (h->h_ints) cudaFreeHost(h->h_ints);
@@ -821,6 +892,11 @@ static int lio_flags_status(int err) {
     if (err & IM_ERR_PEER_TIMEOUT) return im_fail(IMMESH_E_CUDA, "sharded mode: a peer rank did not publish its data in time (peer window epoch flag)");
     return IMMESH_OK;
 }
+// the calls that reuse the per-scan buffers for their own points: the effect / registered rows of the last run are gone
+static void scan_rows_overwritten(immesh_lio* h, const char* by) {
+    h->scan_rows = -1;
+    h->scan_rows_overwritten_by = by;
+}
 static int check_flags(immesh_lio* h) {
     IM_CUDA(cudaMemcpyAsync(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
@@ -899,6 +975,7 @@ int immesh_voxelmap_build(immesh_lio_t* h, const float* body, int n) {
     IM_CUDA(cudaStreamSynchronize(h->stream));
     int rc = upload_scan(h, body, n);
     if (rc) return rc;
+    h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
     launch_grow(h, 1);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -912,6 +989,7 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
     if (rc) return rc;
     rc = launch_estimate(h);
     if (rc) return rc;
+    h->scan_rows = 1;
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(h->h_ints + 32, &h->d_ctrl->iters_run, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     rc = check_flags(h);
@@ -968,6 +1046,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
         launch_grow(h, 0);
     }
     if (lrc) return lrc;
+    h->scan_rows = 1;
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(h->h_out + s, &h->d_ctrl->out, sizeof(LioOut), cudaMemcpyDeviceToHost, h->stream));
     if (!queued) IM_CUDA(cudaEventRecord(h->ev[3], h->stream));
@@ -1038,6 +1117,7 @@ int immesh_residual_build(immesh_lio_t* h, const float* body, int n, int* index_
     if (!h || !n_out) return im_fail(IMMESH_E_INVALID, "null argument");
     int rc = upload_scan(h, body, n);
     if (rc) return rc;
+    scan_rows_overwritten(h, "immesh_residual_build");
     if (!h->d_ptpl) IM_CUDA(dev_alloc(h, &h->d_ptpl, (size_t)h->max_scan * 31));
     IM_LAUNCH(k_reset_scan, 2, 256, 0, h->stream, h->sb, h->d_ctrl, 0);
     *n_out = 0;
@@ -1086,6 +1166,7 @@ int immesh_voxelmap_build_pv(immesh_lio_t* h, const double* pts_world, const dou
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     int rc = upload_pv(h, pts_world, var9, n);
     if (rc) return rc;
+    scan_rows_overwritten(h, "immesh_voxelmap_build_pv");
     launch_grow(h, 3);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -1094,6 +1175,7 @@ int immesh_voxelmap_update_pv(immesh_lio_t* h, const double* pts_world, const do
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     int rc = upload_pv(h, pts_world, var9, n);
     if (rc) return rc;
+    scan_rows_overwritten(h, "immesh_voxelmap_update_pv");
     launch_grow(h, 2);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -1104,6 +1186,7 @@ int immesh_residual_build_pv(immesh_lio_t* h, const double* pts_body, const doub
     if (n < 0 || n > h->max_scan) return im_fail(IMMESH_E_CAPACITY, "too many points");
     *n_out = 0;
     if (n == 0) return IMMESH_OK;
+    scan_rows_overwritten(h, "immesh_residual_build_pv");
     std::vector<double> v6((size_t)n * 6);
     for (int i = 0; i < n; ++i) var9_to_6(var9 + (size_t)i * 9, v6.data() + (size_t)i * 6);
     IM_CUDA(cudaMemcpyAsync(h->sb.var, v6.data(), v6.size() * 8, cudaMemcpyHostToDevice, h->stream));
@@ -1252,6 +1335,82 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     IM_LAUNCH(k_pub_emit, g, PUB_THREADS, 0, st, h->map, n, (const int*)slots, (const int*)cnt, h->d_pub_rows);
     IM_CUDA(cudaGetLastError());
     if (total > 0) IM_CUDA(cudaMemcpyAsync(rows, h->d_pub_rows, (size_t)total * IM_PUB_COLS * sizeof(double), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    return IMMESH_OK;
+}
+
+int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, int cap, int* n_out) {
+    if (!h || !n_out || cap < 0 || (cap > 0 && !rows)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    *n_out = 0;
+    int rc = scan_rows_status(h, "immesh_lio_effect_cloud");
+    if (rc) return rc;
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // everything queued on the handle, the pipelined steps included
+    const int n_max = h->dyn_last.n;              // the scan's count, or its bound when the count is device resident
+    if (h->scan_rows == 0 || n_max <= 0) return IMMESH_OK;
+    const int nb = (n_max + SPUB_THREADS - 1) / SPUB_THREADS;
+    rc = spub_grow(&h->d_spub_tiles, &h->spub_tiles_cap, (size_t)nb + 1);
+    if (rc) return rc;
+    int* tiles = h->d_spub_tiles;
+    cudaStream_t st = h->stream;
+    IM_LAUNCH(k_eff_count, nb, SPUB_THREADS, 0, st, h->sb, tiles);
+    IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, tiles, nb, tiles + nb);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, tiles + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    const int total = h->h_ints[40];
+    *n_out = total;
+    if (total > cap) return im_fail(IMMESH_E_CAPACITY, "effect cloud: more rows than cap (*n_out holds the number needed)");
+    if (total == 0) return IMMESH_OK;
+    rc = spub_grow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)total);
+    if (!rc && scan_index) rc = spub_grow(&h->d_spub_idx, &h->spub_idx_cap, (size_t)total);
+    if (rc) return rc;
+    IM_LAUNCH(k_eff_emit, nb, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)tiles, h->d_spub_rows, scan_index ? h->d_spub_idx : (int*)nullptr);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
+    if (scan_index) IM_CUDA(cudaMemcpyAsync(scan_index, h->d_spub_idx, (size_t)total * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    return IMMESH_OK;
+}
+
+int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, int point_skip, float* rows, int cap, int* n_out) {
+    if (!h || !n_out || cap < 0 || (cap > 0 && !rows)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (point_skip <= 0) return im_fail(IMMESH_E_INVALID, "registered cloud: point_skip must be positive");
+    if (pts && (n < 0 || stride < 3 || intensity_col >= stride)) return im_fail(IMMESH_E_INVALID, "registered cloud: needs n >= 0, stride >= 3 and intensity_col < stride");
+    *n_out = 0;
+    cudaStream_t st = h->stream;
+    if (!pts) {
+        const int rc = scan_rows_status(h, "immesh_lio_registered_cloud");
+        if (rc) return rc;
+        if (h->scan_rows == 0) return im_fail(IMMESH_E_INVALID, "immesh_lio_registered_cloud: pts == NULL publishes the scan of the last IESKF run, and there is none");
+    }
+    IM_CUDA(cudaStreamSynchronize(st));
+    if (!pts) {
+        const int rc = spub_grow(&h->d_spub_tiles, &h->spub_tiles_cap, 1);
+        if (rc) return rc;
+        IM_LAUNCH(k_scan_n, 1, 1, 0, st, h->sb, h->d_spub_tiles);
+        IM_CUDA(cudaGetLastError());
+        IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, h->d_spub_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaStreamSynchronize(st));
+        n = h->h_ints[40];
+    }
+    const int m = n > 0 ? (n - 1) / point_skip + 1 : 0;
+    *n_out = m;
+    if (m > cap) return im_fail(IMMESH_E_CAPACITY, "registered cloud: more rows than cap (*n_out holds the number needed)");
+    if (m == 0) return IMMESH_OK;
+    const float* src = pts;
+    if (pts && !on_device) {
+        const size_t floats = ((size_t)(m - 1) * point_skip + 1) * stride;   // up to the last point published
+        int rc = spub_grow(&h->d_spub_in, &h->spub_in_cap, floats);
+        if (rc) return rc;
+        IM_CUDA(cudaMemcpyAsync(h->d_spub_in, pts, floats * sizeof(float), cudaMemcpyHostToDevice, st));
+        src = h->d_spub_in;
+    }
+    int rc = spub_grow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)m);
+    if (rc) return rc;
+    const int g = std::min((m + SPUB_THREADS - 1) / SPUB_THREADS, h->n_sm * 16);
+    IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
     return IMMESH_OK;
 }

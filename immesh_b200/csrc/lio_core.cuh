@@ -79,6 +79,8 @@ struct ScanBuf {
     double* bv_imu;      // [n][6]  calcBodyVar at the IMU-frame point of the raw scan point (weights, :1498-1521); state independent
     int* match_node;     // [n] plane node of the accepted match, -1 otherwise (last residual pass)
     int* match_layer;    // [n]
+    float* wsqrt;        // [n] (float)sqrt(R_inv) of the matched points of the last residual pass: the IESKF weight the reference writes
+                         // into m_laserCloudOri's intensity (:1527), kept for immesh_lio_effect_cloud; null: not kept
     float* pw;           // [n][3] world points of the growth pass
     double* var;         // [n][6]
     double* sortkey;     // [n]
@@ -172,6 +174,8 @@ IM_HDN inline bool residual_terms(const VoxelMapDev& map, const LioParams& P, co
     congr6(RRe, Sb, wv);
     const double sigma_l = plane_sigma(pw2, pl.center, pl.normal, pl.pv);
     const double R_inv = 1.0 / (sigma_l + quad6(nv, wv));
+    // stored here, not recomputed at publish time: the weight depends on this iteration's pose and on the planes before the map update
+    if (sb.wsqrt) sb.wsqrt[i] = (float)sqrt(R_inv);
     double CRt[9], A[3];
     m3_mul_bt(C, R, CRt);
     m3_vec(CRt, nv, A);
@@ -709,6 +713,15 @@ IM_HD void recycle_chunks(const VoxelMapDev& map, int tid, int nthreads) {
         *map.avail_top = top + np;
         *map.pending_n = 0;
     }
+}
+
+// ------------------------------------------------------------------ scan publishers (immesh_lio_effect_cloud / _registered_cloud)
+// one published point: RGBpointBodyToWorld (voxel_mapping_common.cpp:168-189) with `state`, x y z stored as the float PointType holds
+IM_HD void scan_pub_row(const LioParams& P, const double* state, const float* p, float intensity, float* row) {
+    const double pb[3] = {(double)p[0], (double)p[1], (double)p[2]};
+    double pw[3];
+    body_to_world(P, state, state + 9, pb, pw);
+    row[0] = (float)pw[0]; row[1] = (float)pw[1]; row[2] = (float)pw[2]; row[3] = intensity;
 }
 
 }  // namespace immesh

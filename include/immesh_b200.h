@@ -166,6 +166,36 @@ int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out /*[4]: roots, nodes, ch
  * A sharded handle publishes the roots it owns. */
 #define IMMESH_PLANE_MARKER_COLS 16
 int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows /*[cap][16] or NULL*/, int cap, int* n_out, int64_t* counts /*[5] or NULL*/);
+
+/* The two point-cloud publishers that follow map_incremental_grow (src/voxel_mapping.cpp:1983-1995).  Rows are float x y z
+ * intensity (PointXYZI as the reference publishes it), world frame = RGBpointBodyToWorld (src/voxel_mapping_common.cpp:168-189):
+ * (float) of R (R_ext p + t_ext) + t in double with the handle's CURRENT state (what the reference's publishers read); the
+ * reference's extra multiply by _gravity_correct_rotM is the identity and is skipped, which can change at most the sign of a zero.
+ * Both calls block: they wait for the work queued on h, the pipelined steps included.  *n_out > cap returns IMMESH_E_CAPACITY with
+ * *n_out = rows needed (cap = 0: a pure count query; rows may then be NULL).
+ * Validity: the rows of immesh_lio_effect_cloud, and those of immesh_lio_registered_cloud with pts == NULL, belong to the last
+ * IESKF run (immesh_lio_estimate or any immesh_lio_step* entry point).  Before any run, and after immesh_voxelmap_build, the effect
+ * cloud has 0 rows (the reference's m_effct_feat_num is 0) and pts == NULL returns IMMESH_E_INVALID.  immesh_residual_build and the
+ * three *_pv calls overwrite the per-scan buffers: the effect cloud and pts == NULL then return IMMESH_E_INVALID, naming the call,
+ * until the next run.  immesh_voxelmap_update changes neither.
+ * A sharded handle returns the effect rows of the matches it contributed (their union over the ranks, ordered by scan index, is the
+ * single-GPU cloud); its registered cloud is the same on every rank. */
+#define IMMESH_SCAN_PUB_COLS 4
+/* publish_effect_world (src/voxel_mapping_common.cpp:535-547, /cloud_effected): the scan points matched in the LAST IESKF iteration
+ * (m_laserCloudOri, ptpl order = ascending scan index, src/voxel_mapping.cpp:1372-1392), intensity = (float)sqrt(R_inv), the
+ * point's IESKF weight (:1527, :1558), as stored when the residual was formed.  scan_index (or NULL): each row's index in the scan. */
+int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows /*[cap][4]*/, int32_t* scan_index /*[cap] or NULL*/, int cap, int* n_out);
+/* publish_frame_world (src/voxel_mapping_common.cpp:595-614, /cloud_registered, publish/pub_point_skip): points 0, point_skip,
+ * 2 point_skip, ... of pts ([n][stride] floats, x y z in the first three columns; on_device != 0: a device pointer) in the world
+ * frame; intensity = pts[i * stride + intensity_col], or 0 when intensity_col < 0.  A host buffer is copied to a staging buffer of
+ * its own; the scan the handle localised is left as it is.
+ * pts == NULL (dense_map_en = 0): the down-sampled scan the handle last localised, read where the run read it (a caller-owned
+ * device scan must still hold it), intensity 0 -- the device VoxelGrid does not carry intensity (PCL's averages it); n, stride,
+ * intensity_col and on_device are then ignored.
+ * point_skip <= 0 (the reference would loop forever), stride < 3 or intensity_col >= stride: IMMESH_E_INVALID. */
+int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device,
+                                int point_skip, float* rows /*[cap][4]*/, int cap, int* n_out);
+
 /* device time (ms, CUDA events on the handle's stream) of the stages of the last immesh_lio_step call:
  * [0] whole step incl. H2D, [1] residual+solve iterations, [2] map update */
 int immesh_lio_last_timing(immesh_lio_t* h, double* ms /*[3]*/);
