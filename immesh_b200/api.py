@@ -145,6 +145,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
         ("immesh_mesh_smooth_all", [vp, C.c_double, C.c_int, dp]),
         ("immesh_mesh_region_stream", [vp, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32), ip]),
+        ("immesh_mesh_region_buffers", [vp, C.c_double, C.POINTER(C.c_int32), C.c_int, C.c_double, C.c_int, fp, C.POINTER(C.c_int32), C.c_int,
+                                        C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, fp, ip, ip, ip]),
         ("immesh_kitti_pose_line", [dp, C.c_double, C.c_char_p, C.c_int]),
         ("immesh_voxelgrid_create", [C.c_int, C.POINTER(vp)]),
         ("immesh_voxelgrid_destroy", [vp]),
@@ -559,6 +561,34 @@ class Mesh:
         i32 = C.POINTER(C.c_int32)
         _check(self.lib, self.lib.immesh_mesh_region_stream(self._h, region_size, keys.ctypes.data_as(i32), offs.ctypes.data_as(i32), cap, tri.ctypes.data_as(i32), C.byref(nr)), "mesh_region_stream")
         return keys[:nr.value].copy(), offs[:nr.value + 1].copy(), tri[:nt].copy()
+
+    def region_buffers(self, region_size=10.0, keys=None, smooth_factor=1.0, knn=20, axis_min_max=None):
+        """The viewer's triangle buffers (synchronize_triangle_list_for_disp -> unparse_triangle_set_to_vector + get_axis_min_max):
+        (tri_xyz float32[n,9], tri_ids int32[n,3], region_keys int32[nr,3], region_offsets int32[nr+1], n_smoothed).  keys: int[k,3]
+        regions in the order wanted, or None for every non-empty region.  axis_min_max: float32[6] (min xyz, max xyz), updated in place.
+        A count query sizes the buffers first; vertices of the returned triangles whose smoothed flag is clear are smoothed."""
+        i32, f32p = C.POINTER(C.c_int32), C.POINTER(C.c_float)
+        kp, nk = None, 0
+        if keys is not None:
+            k = np.ascontiguousarray(keys, dtype=np.int32).reshape(-1, 3)
+            kp, nk = k.ctypes.data_as(i32), k.shape[0]
+        box = None
+        if axis_min_max is not None:
+            assert isinstance(axis_min_max, np.ndarray) and axis_min_max.dtype == np.float32 and axis_min_max.shape == (6,) and axis_min_max.flags.c_contiguous
+            box = axis_min_max.ctypes.data_as(f32p)
+        nr, nt, ns = C.c_int(0), C.c_int(0), C.c_int(0)
+        rc = self.lib.immesh_mesh_region_buffers(self._h, region_size, kp, nk, smooth_factor, knn, None, None, 0, None, None, 0, None,
+                                                 C.byref(nr), C.byref(nt), C.byref(ns))
+        if rc not in (0, -3):
+            _check(self.lib, rc, "mesh_region_buffers")
+        xyz = np.zeros((nt.value, 9), dtype=np.float32)
+        ids = np.zeros((nt.value, 3), dtype=np.int32)
+        rkeys = np.zeros((nr.value, 3), dtype=np.int32)
+        roff = np.zeros(nr.value + 1, dtype=np.int32)
+        _check(self.lib, self.lib.immesh_mesh_region_buffers(self._h, region_size, kp, nk, smooth_factor, knn, xyz.ctypes.data_as(f32p), ids.ctypes.data_as(i32),
+                                                             nt.value, rkeys.ctypes.data_as(i32), roff.ctypes.data_as(i32), nr.value, box,
+                                                             C.byref(nr), C.byref(nt), C.byref(ns)), "mesh_region_buffers")
+        return xyz, ids, rkeys, roff, ns.value
 
     def last_timing(self):
         o = np.zeros(4)

@@ -71,12 +71,16 @@ EMU_PUB = os.path.join(PUBMAP_DIR, "libimmesh_emu_pub.so")
 ORACLE_PUB = os.path.join(PUBMAP_DIR, "liborc_pub.so")
 
 
-def _emu_ext(src, out, force):
-    """a file that includes tests/emu/emu_lio.cpp and extends it, built on its own with the emulation's flags"""
+def _emu_ext(src, out, force, extra=()):
+    """a file that includes a tests/emu/ source and extends it, built on its own with the emulation's flags (extra: further
+    translation units linked in unchanged)"""
     deps = [src] + _sources(os.path.join(_ROOT, "tests", "emu"), (".cpp",)) + _sources(CSRC, (".cuh", ".hpp"))
     if force or _newer(out, deps):
-        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
-                               "-o", out, "-x", "c++", src])
+        cmd = [GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+               "-o", out, "-x", "c++", src]
+        for e in extra:
+            cmd += ["-x", "c++", e]
+        subprocess.check_call(cmd)
     return out
 
 
@@ -106,6 +110,17 @@ def build_scanpub(force=False):
             _oracle_ext(os.path.join(PUBMAP_DIR, "orc_scan_pub.cpp"), ORACLE_SCANPUB, force))
 
 
+EMU_REGIONBUF = os.path.join(PUBMAP_DIR, "libimmesh_emu_regionbuf.so")
+ORACLE_REGIONBUF = os.path.join(PUBMAP_DIR, "liborc_regionbuf.so")
+
+
+def build_regionbuf(force=False):
+    """tests/pubmap: the host emulation of the mesher with the m_smoothed flags and the viewer's region buffers, and the oracle
+    extended by the viewer's walk (unparse_triangle_set_to_vector + get_axis_min_max)"""
+    return (_emu_ext(os.path.join(PUBMAP_DIR, "emu_region_buf.cpp"), EMU_REGIONBUF, force, extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")]),
+            _oracle_ext(os.path.join(PUBMAP_DIR, "orc_region_buf.cpp"), ORACLE_REGIONBUF, force))
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -120,6 +135,7 @@ def build_all(force=False):
     build_emu(force)
     build_pubmap(force)
     build_scanpub(force)
+    build_regionbuf(force)
     build_ref()
 
 

@@ -123,4 +123,6 @@ struct immesh_mesh {
     double last_ms[4] = {0, 0, 0, 0};
     int last_cnt[32];
     std::vector<void*> allocs;
+    void* rb_buf[16] = {};    // scratch of immesh_mesh_region_buffers, grown on demand (freed by destroy)
+    size_t rb_cap[16] = {};
 };

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
@@ -294,20 +295,10 @@ __global__ void __launch_bounds__(128) k_knn(MeshDev M, MeshParams P, const floa
 // are averaged, smoothed = p (1 - f) + sum f / valid; stored as the smoothed position (set_smooth_pos) and written to out.
 __global__ void __launch_bounds__(128) k_smooth_all(MeshDev M, int nv, int k, const int* __restrict__ idx, const float* __restrict__ d2, double sf, double max_dis, double* out) {
     for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < nv; v += gridDim.x * blockDim.x) {
-        const float4 p = M.vpos[v];
-        double s0 = 0.0, s1 = 0.0, s2 = 0.0, valid = 0.0;
-        for (int j = 1; j < k; ++j) {
-            const int id = idx[(size_t)v * k + j];
-            if (id < 0) break;
-            if ((double)sqrtf(d2[(size_t)v * k + j]) < max_dis) {
-                const float4 q = M.vpos[id];
-                s0 = s0 + (double)q.x; s1 = s1 + (double)q.y; s2 = s2 + (double)q.z;
-                valid += 1.0;
-            }
-        }
-        const double r0 = (double)p.x * (1.0 - sf) + s0 * sf / valid, r1 = (double)p.y * (1.0 - sf) + s1 * sf / valid, r2 = (double)p.z * (1.0 - sf) + s2 * sf / valid;
-        M.vsmooth[(size_t)v * 3 + 0] = r0; M.vsmooth[(size_t)v * 3 + 1] = r1; M.vsmooth[(size_t)v * 3 + 2] = r2;
-        if (out) { out[(size_t)v * 3 + 0] = r0; out[(size_t)v * 3 + 1] = r1; out[(size_t)v * 3 + 2] = r2; }
+        double r[3];
+        smooth_vertex(M, v, k, idx + (size_t)v * k, d2 + (size_t)v * k, sf, max_dis, r);
+        store_smooth(M, v, r[0], r[1], r[2]);
+        if (out) { out[(size_t)v * 3 + 0] = r[0]; out[(size_t)v * 3 + 1] = r[1]; out[(size_t)v * 3 + 2] = r[2]; }
     }
 }
 // Triangle_manager::insert_triangle_to_list (triangle.cpp:35-53): region = round(centre / region_size) of every live triangle
@@ -315,12 +306,9 @@ __global__ void __launch_bounds__(128) k_region_keys(MeshDev M, int n_alloc, dou
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
-        const float4 a = M.vpos[r.x], b = M.vpos[r.y], c = M.vpos[r.z];
         const int e = atomicAdd(out_n, 1);
         out_tri[(size_t)e * 3 + 0] = r.x; out_tri[(size_t)e * 3 + 1] = r.y; out_tri[(size_t)e * 3 + 2] = r.z;
-        out_key[(size_t)e * 3 + 0] = (int)round((((double)a.x + (double)b.x) + (double)c.x) / 3.0 / region_size);
-        out_key[(size_t)e * 3 + 1] = (int)round((((double)a.y + (double)b.y) + (double)c.y) / 3.0 / region_size);
-        out_key[(size_t)e * 3 + 2] = (int)round((((double)a.z + (double)b.z) + (double)c.z) / 3.0 / region_size);
+        tri_region_key(M, r, region_size, out_key + (size_t)e * 3);
     }
 }
 
@@ -388,6 +376,114 @@ __global__ void __launch_bounds__(128) k_depth_finish(DepthCam C, const unsigned
             out_pts[(size_t)k * 4 + 3] = __int_as_float(i);   // the pixel the point came from (the order of the list is arbitrary)
         }
     }
+}
+
+// ---- the viewer's region buffers (immesh_mesh_region_buffers, mesh_rec_display.cpp:78-137 + :220-258).  k_rb_select keys the live
+// triangles and keeps those of the requested regions, compacted in any order.  A stable LSD radix sort of the kept positions over
+// 32-bit words -- the triple's ids k, j, i, then the region -- orders them by (region, triple); that order is total (a live triple is
+// unique), so nothing depends on the compaction order.  The vertices of the kept triangles whose m_smoothed is clear are claimed once
+// (bitmap), compacted, searched with k_knn and smoothed from raw positions; k_rb_emit gathers vsmooth into the float rows and reduces
+// the axis box per block.
+namespace {
+#include "radix_sort.cuh"
+}
+#define RB_THREADS 128
+__global__ void __launch_bounds__(RB_THREADS) k_rb_select(MeshDev M, int n_alloc, double region_size, const unsigned long long* qkeys, const int* qval, unsigned int qmask,
+                                                          int use_keys, int* slot, unsigned long long* rk, int* misc) {
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[t];
+        if (!r.w) continue;
+        int k[3];
+        tri_region_key(M, r, region_size, k);
+        if (!ikey_ok(k[0], k[1], k[2])) { atomicOr(&misc[1], 1); continue; }
+        unsigned long long word = pack_ikey(k[0], k[1], k[2]);
+        if (use_keys) {
+            const int s = table_find(qkeys, qmask, word);
+            if (s < 0) continue;
+            word = (unsigned long long)qval[s];   // the region's index in the caller's list
+        }
+        const int e = atomicAdd(&misc[0], 1);
+        slot[e] = t;
+        rk[e] = word;
+    }
+}
+// sort word w of kept position v: 0..2 = the triple's k, j, i; 3 / 4 = low / high half of the region word
+__global__ void __launch_bounds__(RB_THREADS) k_rb_word(MeshDev M, int n, int w, const int* slot, const unsigned long long* rk, const unsigned int* vin, unsigned int* kout, unsigned int* vout) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = vin ? vin[i] : (unsigned int)i;
+        unsigned int x;
+        if (w < 3) { const int4 r = M.tri[slot[v]]; x = (unsigned int)(w == 0 ? r.z : w == 1 ? r.y : r.x); }
+        else x = w == 3 ? (unsigned int)rk[v] : (unsigned int)(rk[v] >> 32);
+        kout[i] = x;
+        vout[i] = v;
+    }
+}
+__global__ void __launch_bounds__(RB_THREADS) k_rb_starts(int n, const unsigned int* order, const unsigned long long* rk, int* flag) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) flag[i] = (i == 0 || rk[order[i]] != rk[order[i - 1]]) ? 1 : 0;
+}
+// all regions: the first row of every region writes its key and offset (scan: exclusive region number of each row)
+__global__ void __launch_bounds__(RB_THREADS) k_rb_regions(int n, const unsigned int* order, const unsigned long long* rk, const int* scan, int* keys, int* off) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        if (i > 0 && rk[order[i]] == rk[order[i - 1]]) continue;
+        const int r = scan[i];
+        unpack_ikey(rk[order[i]], keys + (size_t)r * 3, keys + (size_t)r * 3 + 1, keys + (size_t)r * 3 + 2);
+        off[r] = i;
+    }
+}
+// requested regions (n >= 1 rows): offsets of nk segments, empty ones included
+__global__ void __launch_bounds__(RB_THREADS) k_rb_offsets(int n, int nk, const unsigned int* order, const unsigned long long* rk, int* off) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int cur = (int)rk[order[i]], prev = i > 0 ? (int)rk[order[i - 1]] : -1;
+        for (int r = prev + 1; r <= cur; ++r) off[r] = i;
+        if (i == n - 1) for (int r = cur + 1; r <= nk; ++r) off[r] = n;
+    }
+}
+// vertices of the kept triangles with m_smoothed clear, each claimed once, compacted with its position as a k_knn query
+__global__ void __launch_bounds__(RB_THREADS) k_rb_claim(MeshDev M, int n, const int* slot, unsigned int* bits, int* misc, int* list, float4* q) {
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < 3 * n; e += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[slot[e / 3]];
+        const int v = e % 3 == 0 ? r.x : e % 3 == 1 ? r.y : r.z;
+        if (M.vsmoothed[v]) continue;
+        const unsigned int bit = 1u << (v & 31);
+        if (atomicOr(&bits[v >> 5], bit) & bit) continue;
+        const int k = atomicAdd(&misc[2], 1);
+        list[k] = v;
+        q[k] = M.vpos[v];
+    }
+}
+__global__ void __launch_bounds__(RB_THREADS) k_rb_smooth(MeshDev M, int nq, int k, const int* list, const int* __restrict__ idx, const float* __restrict__ d2, double sf, double max_dis) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += gridDim.x * blockDim.x) {
+        double r[3];
+        smooth_vertex(M, list[i], k, idx + (size_t)i * k, d2 + (size_t)i * k, sf, max_dis, r);
+        store_smooth(M, list[i], r[0], r[1], r[2]);
+    }
+}
+__global__ void __launch_bounds__(RB_THREADS) k_rb_emit(MeshDev M, int n, const unsigned int* order, const int* slot, float* xyz, int* ids, AxisAcc* part) {
+    __shared__ AxisAcc s[RB_THREADS];
+    AxisAcc a;
+    axis_init(a);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[slot[order[i]]];
+        float row[9];
+        region_row(M, r, row);
+        for (int c = 0; c < 9; ++c) xyz[(size_t)i * 9 + c] = row[c];
+        ids[(size_t)i * 3 + 0] = r.x; ids[(size_t)i * 3 + 1] = r.y; ids[(size_t)i * 3 + 2] = r.z;
+        for (int j = 0; j < 3; ++j)
+            for (int d = 0; d < 3; ++d) { axis_take(a, d, row[j * 3 + d], i * 3 + j); axis_take(a, d + 3, row[j * 3 + d], i * 3 + j); }
+    }
+    s[threadIdx.x] = a;
+    __syncthreads();
+    for (int h = RB_THREADS / 2; h > 0; h >>= 1) {
+        if (threadIdx.x < h) axis_merge(s[threadIdx.x], s[threadIdx.x + h]);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) part[blockIdx.x] = s[0];
+}
+__global__ void k_rb_axis(const AxisAcc* part, int nb, float* box) {
+    AxisAcc a;
+    axis_init(a);
+    for (int b = 0; b < nb; ++b) axis_merge(a, part[b]);
+    axis_apply(a, box);
 }
 
 // ------------------------------------------------------------------ host side
@@ -459,6 +555,7 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     M.max_t = max_t;
     IM_CREATE_M(mdev_alloc(h, &M.vpos, (size_t)max_v));
     IM_CREATE_M(mdev_alloc(h, &M.vsmooth, (size_t)max_v * 3));
+    IM_CREATE_M(mdev_alloc(h, &M.vsmoothed, (size_t)max_v, 0));
     IM_CREATE_M(mdev_alloc(h, &M.v_tri_head, (size_t)max_v, 0xFF));
     const size_t gcap = pow2_at_least((size_t)max_v * 2);
     IM_CREATE_M(mdev_alloc(h, &M.gkeys, gcap, 0xFF));
@@ -563,6 +660,7 @@ int immesh_mesh_destroy(immesh_mesh_t* h) {
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && immesh::nccl().CommDestroy) immesh::nccl().CommDestroy(h->nccl_comm);
     for (void* p : h->allocs) cudaFree(p);
+    for (void* p : h->rb_buf) if (p) cudaFree(p);
     if (h->h_pts) cudaFreeHost(h->h_pts);
     if (h->h_cnt) cudaFreeHost(h->h_cnt);
     if (h->h_fp) cudaFreeHost(h->h_fp);
@@ -689,7 +787,7 @@ __global__ void __launch_bounds__(256) k_apply_smooth(MeshDev M, FrameBuf F_, co
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
             const double2 a = __ldcg(e + 2 * (size_t)i), b = __ldcg(e + 2 * (size_t)i + 1);   // {id|pad, x}, {y, z}
             const int id = (int)(__double_as_longlong(a.x) & 0xffffffffLL);
-            M.vsmooth[(size_t)id * 3 + 0] = a.y; M.vsmooth[(size_t)id * 3 + 1] = b.x; M.vsmooth[(size_t)id * 3 + 2] = b.y;
+            store_smooth(M, id, a.y, b.x, b.y);
         }
     }
 }
@@ -1175,6 +1273,197 @@ int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* reg
     if (region_offsets && nr <= cap_regions) region_offsets[nr] = nlive;
     *n_regions = nr;
     return nr <= cap_regions ? IMMESH_OK : im_fail(IMMESH_E_CAPACITY, "more regions than cap_regions");
+}
+
+// scratch buffer i of the region-buffer call, at least `bytes` long (grow-only)
+static cudaError_t rb_scratch(immesh_mesh* h, int i, size_t bytes, void** out) {
+    if (bytes > h->rb_cap[i]) {
+        if (h->rb_buf[i]) cudaFree(h->rb_buf[i]);
+        h->rb_buf[i] = nullptr;
+        h->rb_cap[i] = 0;
+        const cudaError_t e = cudaMalloc(&h->rb_buf[i], std::max<size_t>(bytes, 4096));
+        if (e != cudaSuccess) return e;
+        h->rb_cap[i] = std::max<size_t>(bytes, 4096);
+    }
+    *out = h->rb_buf[i];
+    return cudaSuccess;
+}
+static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
+    int b = 0;
+    while (b < 64 && (max_value >> b)) ++b;
+    return std::max(1, (b + 7) / 8);
+}
+
+int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32_t* keys, int n_keys, double smooth_factor, int knn,
+                               float* tri_xyz, int32_t* tri_ids, int cap, int32_t* region_keys, int32_t* region_offsets, int cap_regions,
+                               float* axis_min_max, int* n_regions, int* n_tris, int* n_smoothed) {
+    if (!h || !n_regions || !n_tris || !(region_size > 0) || knn < 1 || knn > KNN_KMAX || cap < 0 || cap_regions < 0 || (keys && n_keys < 0))
+        return im_fail(IMMESH_E_INVALID, "bad argument (region_size > 0, knn in [1,32], cap >= 0, cap_regions >= 0)");
+    *n_regions = 0;
+    *n_tris = 0;
+    if (n_smoothed) *n_smoothed = 0;
+    const bool use_keys = keys != nullptr;
+    const int nk = use_keys ? n_keys : 0;
+    // the requested keys: a repeat is an error; a key outside the mesh's key range can hold no triangle (an empty segment)
+    std::vector<unsigned long long> qk;
+    std::vector<int> qv;
+    unsigned int qmask = 0;
+    if (use_keys) {
+        std::vector<std::array<int, 3>> sk((size_t)nk);
+        for (int i = 0; i < nk; ++i) sk[i] = {keys[3 * i], keys[3 * i + 1], keys[3 * i + 2]};
+        std::sort(sk.begin(), sk.end());
+        if (std::adjacent_find(sk.begin(), sk.end()) != sk.end()) return im_fail(IMMESH_E_INVALID, "region_buffers: a region key is repeated");
+        const size_t qcap = pow2_at_least((size_t)std::max(nk, 1) * 2);
+        qk.assign(qcap, IM_EMPTY_KEY);
+        qv.assign(qcap, -1);
+        qmask = (unsigned int)(qcap - 1);
+        for (int i = 0; i < nk; ++i) {
+            if (!ikey_ok(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2])) continue;
+            int created = 0;
+            const int s = table_insert(qk.data(), qmask, pack_ikey(keys[3 * i], keys[3 * i + 1], keys[3 * i + 2]), &created);
+            qv[s] = i;
+        }
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // everything queued on the handle, the pipelined frames included
+    cudaStream_t st = h->stream;
+    int cnt[32];
+    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
+    const int nv = cnt[0], nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
+    const size_t nl = (size_t)std::max(nlive, 1);
+    void *p_slot, *p_rk, *p_k, *p_v, *p_flag, *p_misc, *p_q;
+    IM_CUDA(rb_scratch(h, 0, nl * sizeof(int), &p_slot));
+    IM_CUDA(rb_scratch(h, 1, nl * sizeof(unsigned long long), &p_rk));
+    IM_CUDA(rb_scratch(h, 2, nl * 2 * sizeof(unsigned int), &p_k));
+    IM_CUDA(rb_scratch(h, 3, nl * 2 * sizeof(unsigned int), &p_v));
+    IM_CUDA(rb_scratch(h, 4, (nl + 1) * sizeof(int), &p_flag));
+    IM_CUDA(rb_scratch(h, 5, 8 * sizeof(int), &p_misc));
+    IM_CUDA(rb_scratch(h, 6, std::max<size_t>(qk.size(), 1) * (sizeof(unsigned long long) + sizeof(int)), &p_q));
+    int* slot = (int*)p_slot;
+    unsigned long long* rk = (unsigned long long*)p_rk;
+    unsigned int* ku[2] = {(unsigned int*)p_k, (unsigned int*)p_k + nl};
+    unsigned int* vu[2] = {(unsigned int*)p_v, (unsigned int*)p_v + nl};
+    int* flag = (int*)p_flag;
+    int* misc = (int*)p_misc;   // [0] kept triangles, [1] key out of range, [2] vertices claimed, [3] regions
+    unsigned long long* d_qk = (unsigned long long*)p_q;
+    int* d_qv = (int*)(d_qk + std::max<size_t>(qk.size(), 1));
+    int hm[4] = {0, 0, 0, 0};
+    IM_CUDA(cudaMemsetAsync(misc, 0, 8 * sizeof(int), st));
+    if (use_keys) {
+        IM_CUDA(cudaMemcpyAsync(d_qk, qk.data(), qk.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
+        IM_CUDA(cudaMemcpyAsync(d_qv, qv.data(), qv.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    }
+    if (nalloc > 0)
+        IM_LAUNCH(k_rb_select, mesh_grid(h, nalloc, RB_THREADS), RB_THREADS, 0, st, h->M, nalloc, region_size, (const unsigned long long*)d_qk, (const int*)d_qv, qmask,
+                  use_keys ? 1 : 0, slot, rk, misc);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(hm, misc, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    if (hm[1]) return im_fail(IMMESH_E_RANGE, "region_buffers: a region key is out of range (region_size too small for the mesh's extent)");
+    const int n = hm[0];
+    int nr = use_keys ? nk : 0;
+    // (region, triple) order
+    int cur = 0;
+    if (n > 0) {
+        const int nb = (n + VG_TILE - 1) / VG_TILE;
+        void* p_hist;
+        IM_CUDA(rb_scratch(h, 7, (size_t)256 * nb * sizeof(int), &p_hist));
+        int* hist = (int*)p_hist;
+        const int g = mesh_grid(h, n, RB_THREADS);
+        const int tri_passes = rb_passes((unsigned long long)std::max(nv - 1, 0));
+        const int n_words = use_keys ? 4 : 5;   // k, j, i, region (index, or the two halves of the packed key)
+        for (int w = 0; w < n_words; ++w) {
+            const int passes = w < 3 ? tri_passes : use_keys ? rb_passes((unsigned long long)std::max(nk - 1, 0)) : 4;
+            IM_LAUNCH(k_rb_word, g, RB_THREADS, 0, st, h->M, n, w, (const int*)slot, (const unsigned long long*)rk, w == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur],
+                      ku[cur ^ 1], vu[cur ^ 1]);
+            cur ^= 1;
+            for (int pass = 0; pass < passes; ++pass) {
+                IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], n, 8 * pass, hist, nb);
+                IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
+                IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
+                cur ^= 1;
+            }
+        }
+        if (!use_keys) {
+            IM_LAUNCH(k_rb_starts, g, RB_THREADS, 0, st, n, (const unsigned int*)vu[cur], (const unsigned long long*)rk, flag);
+            IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, flag, n, misc + 3);
+            IM_CUDA(cudaGetLastError());
+            IM_CUDA(cudaMemcpyAsync(hm + 3, misc + 3, sizeof(int), cudaMemcpyDeviceToHost, st));
+            IM_CUDA(cudaStreamSynchronize(st));
+            nr = hm[3];
+        }
+    }
+    *n_tris = n;
+    *n_regions = nr;
+    if (n > cap || nr > cap_regions)
+        return im_fail(IMMESH_E_CAPACITY, "region_buffers: more triangles than cap or more regions than cap_regions (*n_tris / *n_regions hold the numbers needed; nothing was smoothed)");
+    const unsigned int* order = vu[cur];
+    void *p_reg, *p_rows, *p_part, *p_box;
+    IM_CUDA(rb_scratch(h, 8, ((size_t)nr * 3 + (size_t)nr + 1) * sizeof(int), &p_reg));
+    int* d_rkeys = (int*)p_reg;
+    int* d_roff = d_rkeys + (size_t)nr * 3;
+    int* h_off_src = nullptr;
+    std::vector<int> zeros;
+    if (n == 0) {
+        zeros.assign((size_t)nr + 1, 0);
+        h_off_src = zeros.data();
+    } else if (use_keys) {
+        IM_LAUNCH(k_rb_offsets, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, nk, order, (const unsigned long long*)rk, d_roff);
+    } else {
+        IM_LAUNCH(k_rb_regions, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, order, (const unsigned long long*)rk, (const int*)flag, d_rkeys, d_roff);
+        IM_CUDA(cudaMemcpyAsync(d_roff + nr, &n, sizeof(int), cudaMemcpyHostToDevice, st));
+    }
+    // lazy smoothing of the kept triangles' vertices (unparse_triangle_set_to_vector, :88-94)
+    int nq = 0;
+    if (n > 0) {
+        void *p_bits, *p_list, *p_qpos;
+        IM_CUDA(rb_scratch(h, 9, (((size_t)nv + 31) / 32) * sizeof(unsigned int), &p_bits));
+        const size_t qmax = (size_t)std::min<long long>((long long)nv, 3LL * n);
+        IM_CUDA(rb_scratch(h, 10, qmax * sizeof(int), &p_list));
+        IM_CUDA(rb_scratch(h, 11, qmax * sizeof(float4), &p_qpos));
+        IM_CUDA(cudaMemsetAsync(p_bits, 0, (((size_t)nv + 31) / 32) * sizeof(unsigned int), st));
+        IM_LAUNCH(k_rb_claim, mesh_grid(h, 3 * n, RB_THREADS), RB_THREADS, 0, st, h->M, n, (const int*)slot, (unsigned int*)p_bits, misc, (int*)p_list, (float4*)p_qpos);
+        IM_CUDA(cudaGetLastError());
+        IM_CUDA(cudaMemcpyAsync(hm + 2, misc + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaStreamSynchronize(st));
+        nq = hm[2];
+        if (nq > 0) {
+            void *p_idx, *p_d2;
+            IM_CUDA(rb_scratch(h, 12, (size_t)nq * knn * sizeof(int), &p_idx));
+            IM_CUDA(rb_scratch(h, 13, (size_t)nq * knn * sizeof(float), &p_d2));
+            IM_LAUNCH(k_knn, mesh_grid(h, nq * 32, 128), 128, 0, st, h->M, h->P, (const float*)p_qpos, 4, nq, knn, (double)INFINITY, (int*)p_idx, (float*)p_d2);
+            IM_LAUNCH(k_rb_smooth, mesh_grid(h, nq, RB_THREADS), RB_THREADS, 0, st, h->M, nq, knn, (const int*)p_list, (const int*)p_idx, (const float*)p_d2, smooth_factor, h->P.accept);
+        }
+    }
+    if (n_smoothed) *n_smoothed = nq;
+    // rows + axis box
+    const int ge = mesh_grid(h, std::max(n, 1), RB_THREADS);
+    IM_CUDA(rb_scratch(h, 14, std::max<size_t>((size_t)n, 1) * 12 * sizeof(float), &p_rows));
+    IM_CUDA(rb_scratch(h, 15, (size_t)ge * sizeof(AxisAcc) + 8 * sizeof(float), &p_part));
+    float* d_rows = (float*)p_rows;
+    int* d_ids = (int*)(d_rows + (size_t)std::max(n, 1) * 9);
+    AxisAcc* part = (AxisAcc*)p_part;
+    p_box = (void*)(part + ge);
+    if (n > 0) {
+        IM_LAUNCH(k_rb_emit, ge, RB_THREADS, 0, st, h->M, n, order, (const int*)slot, d_rows, d_ids, part);
+        if (axis_min_max) {
+            IM_CUDA(cudaMemcpyAsync(p_box, axis_min_max, 6 * sizeof(float), cudaMemcpyHostToDevice, st));
+            IM_LAUNCH(k_rb_axis, 1, 1, 0, st, (const AxisAcc*)part, ge, (float*)p_box);
+            IM_CUDA(cudaMemcpyAsync(axis_min_max, p_box, 6 * sizeof(float), cudaMemcpyDeviceToHost, st));
+        }
+    }
+    IM_CUDA(cudaGetLastError());
+    if (n > 0 && tri_xyz) IM_CUDA(cudaMemcpyAsync(tri_xyz, d_rows, (size_t)n * 9 * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (n > 0 && tri_ids) IM_CUDA(cudaMemcpyAsync(tri_ids, d_ids, (size_t)n * 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (region_offsets) {
+        if (h_off_src) std::memcpy(region_offsets, h_off_src, ((size_t)nr + 1) * sizeof(int));
+        else IM_CUDA(cudaMemcpyAsync(region_offsets, d_roff, ((size_t)nr + 1) * sizeof(int), cudaMemcpyDeviceToHost, st));
+    }
+    if (region_keys) {
+        if (use_keys) std::memcpy(region_keys, keys, (size_t)nk * 3 * sizeof(int));
+        else if (nr > 0) IM_CUDA(cudaMemcpyAsync(region_keys, d_rkeys, (size_t)nr * 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    }
+    IM_CUDA(cudaStreamSynchronize(st));
+    return IMMESH_OK;
 }
 
 // reconstruct_mesh_from_pointcloud (src/ImMesh_mesh_reconstruction.cpp:328-345, the offline entry of config/offline_pointcloud.yaml):

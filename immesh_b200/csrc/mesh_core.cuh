@@ -69,6 +69,7 @@ struct MeshDev {
     // vertices
     float4* vpos;        // xyz, w unused
     double* vsmooth;     // [max_v][3]
+    unsigned char* vsmoothed;  // [max_v] RGB_pts::m_smoothed: cleared at append, set by every store_smooth (null: not kept)
     int* v_tri_head;     // head of the incidence list
     int max_v;
     // xi-grid hash: cell -> vertex id
@@ -427,6 +428,7 @@ IM_HDN inline void cand_commit(const MeshDev& M, const MeshParams& P, const Fram
     M.vsmooth[(size_t)id * 3 + 0] = (double)p[0];
     M.vsmooth[(size_t)id * 3 + 1] = (double)p[1];
     M.vsmooth[(size_t)id * 3 + 2] = (double)p[2];
+    if (M.vsmoothed) M.vsmoothed[id] = 0;
     M.v_tri_head[id] = -1;
     int created = 0;
     const int gs = table_insert(M.gkeys, M.gmask, F.cand_gkey[c], &created);
@@ -737,6 +739,69 @@ IM_HDN inline void tri_add(const MeshDev& M, int a, int b, int c, unsigned long 
 }
 IM_HD void tri_remove(const MeshDev& M, int t) {  // erase_triangle, triangle.hpp:164-210
     if (im_atomic_exch(&M.tri[t].w, 0) == 1) im_atomic_add(&M.cnt[2], -1);
+}
+
+// ------------------------------------------------------------------ smoothed positions and the viewer's region sets
+// RGB_pts::set_smooth_pos (pointcloud_rgbd.cpp:68-75): the smoothed position and m_smoothed.  Every writer of vsmooth except the
+// append goes through here.
+IM_HD void store_smooth(const MeshDev& M, int v, double x, double y, double z) {
+    M.vsmooth[(size_t)v * 3 + 0] = x; M.vsmooth[(size_t)v * 3 + 1] = y; M.vsmooth[(size_t)v * 3 + 2] = z;
+    if (M.vsmoothed) M.vsmoothed[v] = 1;
+}
+// Global_map::smooth_pts (pointcloud_rgbd.cpp:932-958) of vertex v from its k nearest vertices (ascending; the first is v itself and
+// is skipped, a -1 id ends the list): those with sqrt(d2) < max_dis are averaged from their RAW positions (get_pos()), so the result
+// does not depend on which vertices were smoothed before;  r = p (1 - f) + sum f / valid  (valid == 0 divides by zero like the reference)
+IM_HD void smooth_vertex(const MeshDev& M, int v, int k, const int* idx, const float* d2, double sf, double max_dis, double* r) {
+    const float4 p = M.vpos[v];
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0, valid = 0.0;
+    for (int j = 1; j < k; ++j) {
+        const int id = idx[j];
+        if (id < 0) break;
+        if ((double)sqrtf(d2[j]) < max_dis) {
+            const float4 q = M.vpos[id];
+            s0 = s0 + (double)q.x; s1 = s1 + (double)q.y; s2 = s2 + (double)q.z;
+            valid += 1.0;
+        }
+    }
+    r[0] = (double)p.x * (1.0 - sf) + s0 * sf / valid;
+    r[1] = (double)p.y * (1.0 - sf) + s1 * sf / valid;
+    r[2] = (double)p.z * (1.0 - sf) + s2 * sf / valid;
+}
+// Triangle_manager::insert_triangle_to_list (triangle.cpp:35-53): region = round(centre / region_size), centre = mean of the three
+// raw vertex positions (get_triangle_center)
+IM_HD void tri_region_key(const MeshDev& M, const int4& r, double region_size, int* key) {
+    const float4 a = M.vpos[r.x], b = M.vpos[r.y], c = M.vpos[r.z];
+    key[0] = (int)round((((double)a.x + (double)b.x) + (double)c.x) / 3.0 / region_size);
+    key[1] = (int)round((((double)a.y + (double)b.y) + (double)c.y) / 3.0 / region_size);
+    key[2] = (int)round((((double)a.z + (double)b.z) + (double)c.z) / 3.0 / region_size);
+}
+// unparse_triangle_set_to_vector (mesh_rec_display.cpp:78-104): get_pos(1).cast<float>() of the three vertices, ascending ids
+IM_HD void region_row(const MeshDev& M, const int4& r, float* xyz9) {
+    const int v[3] = {r.x, r.y, r.z};
+    for (int j = 0; j < 3; ++j)
+        for (int d = 0; d < 3; ++d) xyz9[j * 3 + d] = (float)M.vsmooth[(size_t)v[j] * 3 + d];
+}
+// get_axis_min_max (mesh_rec_display.cpp:105-137) as an order-free reduction.  The reference walks the emitted floats in order and
+// replaces the bound on a strict < / >: it ends at the FIRST occurrence of the extreme value (+0 and -0 compare equal) when that
+// beats the bound, and NaN never replaces it.  So per axis the accumulator keeps (extreme value, lowest position among its equals),
+// which any reduction order reproduces; axis_apply then makes the reference's single comparison against the caller's bound.
+struct AxisAcc { float v[6]; int p[6]; };   // min x y z, max x y z; p = 0x7fffffff: nothing seen
+IM_HD void axis_init(AxisAcc& a) {
+    for (int j = 0; j < 6; ++j) { a.v[j] = 0.f; a.p[j] = 0x7fffffff; }
+}
+IM_HD void axis_take(AxisAcc& a, int j, float v, int p) {
+    if (!(v == v) || p == 0x7fffffff) return;
+    const bool lo = j < 3;
+    if (a.p[j] == 0x7fffffff || (lo ? v < a.v[j] : v > a.v[j]) || (v == a.v[j] && p < a.p[j])) { a.v[j] = v; a.p[j] = p; }
+}
+IM_HD void axis_merge(AxisAcc& a, const AxisAcc& b) {
+    for (int j = 0; j < 6; ++j) axis_take(a, j, b.v[j], b.p[j]);
+}
+IM_HD void axis_apply(const AxisAcc& a, float* box) {
+    for (int j = 0; j < 3; ++j) {
+        if (a.p[j] != 0x7fffffff && box[j] > a.v[j]) box[j] = a.v[j];
+        if (a.p[j + 3] != 0x7fffffff && box[j + 3] < a.v[j + 3]) box[j + 3] = a.v[j + 3];
+    }
 }
 
 }  // namespace immesh

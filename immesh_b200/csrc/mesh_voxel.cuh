@@ -84,7 +84,7 @@ IM_HD void apply_remove(const MeshDev& M, const FrameBuf& F, int a, int b, int c
     if (e < F.max_list) F.rem_tri[e] = t; else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
 }
 IM_HD void emit_smooth(const MeshDev& M, const FrameBuf& F, int v, double x, double y, double z) {
-    M.vsmooth[(size_t)v * 3 + 0] = x; M.vsmooth[(size_t)v * 3 + 1] = y; M.vsmooth[(size_t)v * 3 + 2] = z;
+    store_smooth(M, v, x, y, z);
     if (F.shard_n > 1) {
         const int e = im_atomic_add(&M.cnt[32], 1);
         if (e < F.x_cap) { XSmooth r; r.id = v; r.pad = 0; r.x = x; r.y = y; r.z = z; F.x_smooth[e] = r; }

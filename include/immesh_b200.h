@@ -259,6 +259,40 @@ int immesh_mesh_smooth_all(immesh_mesh_t* h, double smooth_factor, int knn /*<= 
  * [nr + 1] into `triangles`), triangles [n_live][3] grouped by region, ascending triples inside a region. */
 int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* region_keys /*[cap][3] or NULL*/, int32_t* region_offsets /*[cap+1] or NULL*/,
                               int cap_regions, int32_t* triangles /*[n_live][3] or NULL*/, int* n_regions);
+/* The mesh viewer's triangle buffers: synchronize_triangle_list_for_disp (src/meshing/mesh_rec_display.cpp:220-258, every 100 ms from
+ * service_refresh_and_synchronize_triangle :262-271) -> unparse_triangle_set_to_vector (:78-104) + get_axis_min_max (:105-137) over the
+ * region sets of Triangle_manager::insert_triangle_to_list (src/meshing/r3live/triangle.cpp:35-53).
+ *   Regions: a triangle's region is the key of immesh_mesh_region_stream.  keys == NULL: every non-empty region, ascending key order;
+ *     else exactly the n_keys regions listed, in the caller's order, an empty segment for a region without triangles (a key outside
+ *     the mesh's key range holds none); a repeated key is IMMESH_E_INVALID.  Inside a region, ascending (i<j<k) triples.
+ *     region_keys [n_regions][3] and region_offsets [n_regions + 1] (into the rows) describe the segments.
+ *   Lazy smoothing: before any row is written, every vertex of an emitted triangle whose m_smoothed flag is clear is smoothed as
+ *     Global_map::smooth_pts (src/meshing/r3live/pointcloud_rgbd.cpp:932-958) does it: its knn nearest vertices (ties to the lower id,
+ *     the immesh_knn rule), neighbours 1..knn-1 closer than g_kd_tree_accept_pt_dis = 1.25 voxel_resolution averaged from their RAW
+ *     positions, p (1 - f) + mean f (no neighbour inside the limit: the reference's division by zero, NaN); the result is stored as
+ *     the vertex's smoothed position and the flag is set (set_smooth_pos).  Only vertices of the selected regions are touched.
+ *     The flag is set by the mesher's dilation (retrieve_neighbor_pts_kdtree, src/meshing/mesh_rec_geometry.cpp:336-377), by
+ *     immesh_mesh_smooth_all and by this call; a vertex is appended with it clear.  *n_smoothed (or NULL): vertices smoothed here.
+ *     The viewer uses g_ply_smooth_factor = 1.0 and g_ply_smooth_k = 20.
+ *   Rows: tri_xyz [n_tris][9] = (float) of the three vertices' smoothed positions, ascending ids (get_pos(1).cast<float>()); tri_ids
+ *     [n_tris][3] the triples.  Either may be NULL.
+ *   axis_min_max [6] (min xyz, max xyz; or NULL) is read and updated over the emitted floats with the reference's strict < / >
+ *     comparisons, in row order; start it at +-1e8 as :264 does.
+ *   *n_tris > cap or *n_regions > cap_regions: IMMESH_E_CAPACITY with the counts needed; nothing is written and nothing is smoothed
+ *     (cap = 0: a pure count query).  region_size <= 0 or knn outside [1, 32]: IMMESH_E_INVALID.  A region key outside the mesh's
+ *     key range (+-1048000): IMMESH_E_RANGE.
+ *   Blocking: waits for the work queued on h, the frames of immesh_mesh_push_frame_from_lio_async included.  The smoothed positions
+ *     stored here are the ones later frames' correct_triangle_index (mesh_rec_geometry.cpp:399-433) reads -- in the reference a race
+ *     with the viewer thread, here ordered between frames.
+ *   A sharded handle: every replica holds the same triangle store, smoothed positions and flags, so every rank returns the same rows
+ *     and applies the same write-back, without an exchange. */
+#define IMMESH_REGION_TRI_FLOATS 9
+int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32_t* keys /*[n_keys][3] or NULL*/, int n_keys,
+                               double smooth_factor, int knn /*[1,32]*/,
+                               float* tri_xyz /*[cap][9] or NULL*/, int32_t* tri_ids /*[cap][3] or NULL*/, int cap,
+                               int32_t* region_keys /*[cap_regions][3] or NULL*/, int32_t* region_offsets /*[cap_regions+1] or NULL*/,
+                               int cap_regions, float* axis_min_max /*[6] in/out or NULL*/,
+                               int* n_regions, int* n_tris, int* n_smoothed /*or NULL*/);
 /* reconstruct_mesh_from_pointcloud(frame_pts, minimum_pts_distance) (src/ImMesh_mesh_reconstruction.cpp:328-345; the offline whole-cloud
  * entry of config/offline_pointcloud.yaml): VoxelGrid down-sampling with leaf = minimum_pts_distance, then one
  * incremental_mesh_reconstruction frame with the identity pose.  xyz: [n][3] host array, or device pointer with on_device = 1. */
