@@ -143,6 +143,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_write_pcd", [C.c_char_p, fp, C.c_int]),
         ("immesh_mesh_render_depth", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, dp, fp, fp, C.POINTER(C.c_int32), ip]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
+        ("immesh_mesh_push_frame_batched", [vp, vp, C.c_int64, C.c_int, dp, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_reconstruct_from_pointcloud_batched", [vp, vp, vp, C.c_int64, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_smooth_all", [vp, C.c_double, C.c_int, dp]),
         ("immesh_mesh_region_stream", [vp, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32), ip]),
         ("immesh_mesh_region_buffers", [vp, C.c_double, C.POINTER(C.c_int32), C.c_int, C.c_double, C.c_int, fp, C.POINTER(C.c_int32), C.c_int,
@@ -528,6 +530,31 @@ class Mesh:
         a, p = _f32(pts)
         m = C.c_int(0)
         _check(self.lib, self.lib.immesh_mesh_reconstruct_from_pointcloud(self._h, vg._h, C.cast(p, C.c_void_p), a.shape[0], 0, minimum_pts_distance, C.byref(m)), "mesh_reconstruct_from_pointcloud")
+        return m.value
+
+    def push_frame_batched(self, world_xyz, pose_t, batch_points=0, batch_voxels=0, n=None, on_device=False):
+        """One incremental_mesh_reconstruction frame of any size, run in bounded batches (the same mesh as one push_frame).
+        world_xyz: float32[n][3] host array, or an integer CUDA address with n when on_device.  batch_points / batch_voxels: append
+        candidates per chunk / activated voxels per batch (0: the handle's capacities).  Returns the frame's stats dict."""
+        if on_device:
+            ptr = C.c_void_p(world_xyz)
+        else:
+            a, p = _f32(world_xyz)
+            n = a.shape[0]
+            ptr = C.cast(p, C.c_void_p)
+        t = np.ascontiguousarray(pose_t, dtype=np.float64)
+        st = np.zeros(4, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_mesh_push_frame_batched(self._h, ptr, n, 1 if on_device else 0, t.ctypes.data_as(C.POINTER(C.c_double)), batch_points, batch_voxels,
+                                                               st.ctypes.data_as(C.POINTER(C.c_int64))), "mesh_push_frame_batched")
+        return dict(zip(["append_chunks", "voxel_batches", "scratch_bytes", "facets_added"], (int(v) for v in st)))
+
+    def reconstruct_from_pointcloud_batched(self, vg: "VoxelGrid", pts, minimum_pts_distance: float, batch_points=0, batch_voxels=0) -> int:
+        """reconstruct_mesh_from_pointcloud on a cloud of any size: PCL's VoxelGrid decision on the whole cloud, then one batched frame with
+        the identity pose; returns the number of points meshed (the cloud's size when PCL passes it through)."""
+        a, p = _f32(pts)
+        m = C.c_int64(0)
+        _check(self.lib, self.lib.immesh_mesh_reconstruct_from_pointcloud_batched(self._h, vg._h, C.cast(p, C.c_void_p), a.shape[0], 0, minimum_pts_distance, batch_points,
+                                                                                batch_voxels, C.byref(m)), "mesh_reconstruct_from_pointcloud_batched")
         return m.value
 
     def render_depth(self, intrinsics, width, height, z_near, z_far, cam_R, cam_t):

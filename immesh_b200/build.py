@@ -121,6 +121,15 @@ def build_regionbuf(force=False):
             _oracle_ext(os.path.join(PUBMAP_DIR, "orc_region_buf.cpp"), ORACLE_REGIONBUF, force))
 
 
+EMU_BATCHED = os.path.join(_ROOT, "tests", "batched", "libimmesh_emu_batched.so")
+
+
+def build_batched(force=False):
+    """tests/batched: the host emulation of the mesher with the m_smoothed flags and the batched frame's orchestration (the
+    localization emulation linked in unchanged: api.load_library binds both handles' entry points)"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "batched", "emu_batched.cpp"), EMU_BATCHED, force, extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")])
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -136,6 +145,7 @@ def build_all(force=False):
     build_pubmap(force)
     build_scanpub(force)
     build_regionbuf(force)
+    build_batched(force)
     build_ref()
 
 

@@ -341,6 +341,33 @@ int immesh_voxelgrid_filter(immesh_voxelgrid_t* h, const float* xyz, int n, int 
     return IMMESH_OK;
 }
 
+// PCL's "leaf size too small" decision (k_vg_setup's index-overflow test) on a cloud of any size: the box of its finite points is reduced
+// max_points at a time (host input through the handle's staging) by k_vg_minmax, whose order-free atomics accumulate across chunks, so
+// the decision equals immesh_voxelgrid_filter's on the whole cloud.  Used by immesh_mesh_reconstruct_from_pointcloud_batched.
+int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int64_t n, int on_device, float leaf, int* too_small) {
+    if (!h || (!xyz && n > 0) || n < 0 || !(leaf > 0.f) || !too_small) return im_fail(IMMESH_E_INVALID, "bad argument");
+    cudaStream_t st = h->stream;
+    IM_LAUNCH(k_vg_reset, 1, 32, 0, st, h->d_grid);
+    for (int64_t c0 = 0; c0 < n; c0 += h->max_points) {
+        const int m = (int)std::min<int64_t>(h->max_points, n - c0);
+        const float* d = xyz + (size_t)c0 * 3;
+        if (!on_device) {
+            IM_CUDA(cudaStreamSynchronize(st));   // the previous chunk's copy out of the staging buffer is done
+            std::memcpy(h->h_pts, d, (size_t)m * 3 * sizeof(float));
+            IM_CUDA(cudaMemcpyAsync(h->d_in, h->h_pts, (size_t)m * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+            d = h->d_in;
+        }
+        const int gs = std::min(((m + VG_TILE - 1) / VG_TILE) * (VG_TILE / VG_THREADS), h->n_sm * 8);
+        IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d, m, h->d_grid);
+    }
+    IM_LAUNCH(k_vg_setup, 1, 32, 0, st, h->d_grid, 1.0f / leaf);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(h->h_grid, h->d_grid, sizeof(VgGrid), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    *too_small = h->h_grid->too_small;
+    return IMMESH_OK;
+}
+
 // upload (host input) + pack / calibrate into d_in on stream st
 static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int stride, int on_device, int calib_laser, cudaStream_t st) {
     h->in_idx = (h->in_idx + 1) & 7;

@@ -125,4 +125,17 @@ struct immesh_mesh {
     std::vector<void*> allocs;
     void* rb_buf[16] = {};    // scratch of immesh_mesh_region_buffers, grown on demand (freed by destroy)
     size_t rb_cap[16] = {};
+    // batched frame (immesh_mesh_push_frame_batched), allocated by its first call, sized by the handle's capacities only
+    int max_vox = 0;
+    int* b_act = nullptr;             // [max_vox] the frame's activated voxels (all append chunks)
+    int* b_sel = nullptr;             // [max_vox] the voxels the frame meshes
+    unsigned long long* b_key = nullptr;   // [max_vox] their keys
+    unsigned int *b_ku = nullptr, *b_vu = nullptr;   // [2][max_vox] radix-sort ping-pong (key order -> rank)
+    int* b_hist = nullptr;
+    int* b_rank = nullptr;            // [max_work] rank of the batch's work voxels
+    unsigned char* b_mark = nullptr;  // [max_t] triangle marks (FrameBuf::tri_mark)
+    int* b_fset = nullptr;            // facet set of a batch, 2 x max_list slots
+    unsigned int b_fset_mask = 0;
+    immesh::FramePose* b_fp = nullptr;
+    size_t b_bytes = 0;
 };

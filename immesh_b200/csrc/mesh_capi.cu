@@ -486,6 +486,82 @@ __global__ void k_rb_axis(const AxisAcc* part, int nb, float* box) {
     axis_apply(a, box);
 }
 
+// ---- the batched frame (immesh_mesh_push_frame_batched): one frame, append in chunks, per-voxel stage in batches.  The frame-level
+// counters of the per-frame path are accumulated across chunks / batches in cnt[33] (new vertices), cnt[34] (add entries), cnt[35]
+// (meshed voxels) and written back by k_bat_frame_end; cnt[36] counts the meshed voxels of the selection.
+__global__ void k_bat_chunk_begin(MeshDev M, FrameBuf F) {   // the candidate grid of one append chunk after the first
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    for (unsigned int i = tid; i <= F.cmask; i += nt) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
+    if (tid == 0) { M.cnt[9] = 0; M.cnt[18] = 0; }
+}
+__global__ void k_bat_chunk_end(MeshDev M) {   // the chunk's vertices are in the map before the next chunk is examined
+    M.cnt[0] += M.cnt[10];
+    M.cnt[33] += M.cnt[10];
+    M.cnt[10] = 0;
+}
+// activation rule over every activated voxel of the frame (after the last chunk); the meshed ones with their keys
+__global__ void __launch_bounds__(128) k_bat_select(MeshDev M, FrameBuf F, int* sel, unsigned long long* key) {
+    const int na = min(M.cnt[5], F.max_act);
+    for (int a = blockIdx.x * blockDim.x + threadIdx.x; a < na; a += gridDim.x * blockDim.x) {
+        const int vs = F.act[a];
+        if (!voxel_activate(M, F, vs)) continue;
+        const int k = atomicAdd(&M.cnt[36], 1);
+        sel[k] = vs;
+        key[k] = M.vkeys[vs];
+    }
+}
+// sort word of position i: half 0 / 1 = low / high 32 bits of the key (LSD order)
+__global__ void __launch_bounds__(128) k_bat_word(int n, int half, const unsigned long long* key, const unsigned int* vin, unsigned int* kout, unsigned int* vout) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = vin ? vin[i] : (unsigned int)i;
+        kout[i] = (unsigned int)(key[v] >> (32 * half));
+        vout[i] = v;
+    }
+}
+__global__ void k_bat_reset(MeshDev M, FrameBuf F, int clear_fset) {   // the per-batch lists
+    const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
+    if (clear_fset) for (unsigned int i = tid; i <= F.fset_mask; i += nt) F.fset[i] = -1;
+    if (tid == 0) {
+        M.cnt[6] = 0; M.cnt[7] = 0; M.cnt[17] = 0; M.cnt[19] = 0;
+        M.cnt[24] = 0; M.cnt[25] = 0; M.cnt[26] = 0; M.cnt[28] = 0; M.cnt[29] = 0;
+    }
+}
+// meshed voxels [lo, hi) in key order -> the batch's work list; the rank is the flip priority
+__global__ void __launch_bounds__(128) k_bat_fill(MeshDev M, FrameBuf F, const int* sel, const unsigned int* order, int lo, int hi, int* rank) {
+    for (int r = lo + blockIdx.x * blockDim.x + threadIdx.x; r < hi; r += gridDim.x * blockDim.x) {
+        const int w = voxel_enqueue(M, F, sel[order[r]]);
+        if (w >= 0) rank[w] = r;
+    }
+}
+// the batch's additions, pushed at once; marked so that later batches' pulls and commits do not see them as pre-frame triangles
+__global__ void __launch_bounds__(128) k_bat_push_add(MeshDev M, FrameBuf F) {
+    const int n = min(M.cnt[7], F.max_list);
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
+        const int t = tri_add(M, F.add_tri[(size_t)e * 3 + 0], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
+        if (t >= 0) F.tri_mark[t] = IM_TRI_BORN;
+    }
+}
+__global__ void k_bat_batch_end(MeshDev M) {
+    M.cnt[34] += M.cnt[7];
+    M.cnt[35] += M.cnt[6] + M.cnt[17];
+}
+// after the last batch: the deferred removals; every mark cleared for the next frame
+__global__ void __launch_bounds__(128) k_bat_sweep(MeshDev M, FrameBuf F) {
+    const int n = min(M.cnt[1], M.max_t);
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        const unsigned char m = F.tri_mark[t];
+        if (!m) continue;
+        if (m == IM_TRI_REMOVE) tri_remove(M, t);
+        F.tri_mark[t] = 0;
+    }
+}
+__global__ void k_bat_frame_end(MeshDev M) {
+    M.cnt[10] = M.cnt[33];
+    M.cnt[7] = M.cnt[34];
+    M.cnt[6] = M.cnt[35];
+    M.cnt[17] = 0;
+}
+
 // ------------------------------------------------------------------ host side
 
 template <class T>
@@ -526,6 +602,7 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
         if (im_e_ != cudaSuccess) { immesh_mesh_destroy(h); return immesh::im_fail_cuda(im_e_, __FILE__, __LINE__); } \
     } while (0)
     h->F.shard_rank = 0; h->F.shard_n = 1; h->F.x_cap = 0;
+    h->F.work_rank = nullptr; h->F.tri_mark = nullptr;   // the per-frame path
     h->bps = std::getenv("IMMESH_MESH_BPS") ? std::atoi(std::getenv("IMMESH_MESH_BPS")) : 3;
     h->dilate_bps = std::getenv("IMMESH_DILATE_BPS") ? std::atoi(std::getenv("IMMESH_DILATE_BPS")) : h->bps;
     // dilated sets up to warp_nmax vertices are triangulated by one warp each (side stream), larger ones by a thread block each
@@ -545,6 +622,7 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     const int max_t = cfg->max_triangles ? cfg->max_triangles : (32 << 20);
     const int max_vox = cfg->max_voxels ? cfg->max_voxels : (2 << 20);
     h->max_frame_points = cfg->max_frame_points ? cfg->max_frame_points : (2 << 20);
+    h->max_vox = max_vox;
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
@@ -1477,6 +1555,193 @@ int immesh_mesh_reconstruct_from_pointcloud(immesh_mesh_t* h, immesh_voxelgrid_t
     if (n_downsampled) *n_downsampled = m;
     const double zero[3] = {0.0, 0.0, 0.0};
     return immesh_mesh_push_frame_dev(h, immesh_voxelgrid_device_points(vg), m, zero, 0);
+}
+
+// scratch of the batched frame: sized by max_voxels, max_work, max_triangles and max_list, never by the frame
+static cudaError_t mesh_batched_scratch(immesh_mesh* h) {
+    if (h->b_fp) return cudaSuccess;
+    const size_t nv = (size_t)std::max(h->max_vox, 1), nb = (nv + VG_TILE - 1) / VG_TILE, fcap = pow2_at_least((size_t)h->F.max_list * 2);
+    cudaError_t e;
+    if ((e = mdev_alloc(h, &h->b_act, nv)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_sel, nv)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_key, nv)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_ku, 2 * nv)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_vu, 2 * nv)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_hist, 256 * nb)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_rank, (size_t)h->F.max_work)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_mark, (size_t)h->M.max_t, 0)) != cudaSuccess) return e;
+    if ((e = mdev_alloc(h, &h->b_fset, fcap, 0xFF)) != cudaSuccess) return e;
+    h->b_fset_mask = (unsigned int)(fcap - 1);
+    h->b_bytes = nv * (4 + 4 + 8 + 16) + 256 * nb * 4 + (size_t)h->F.max_work * 4 + (size_t)h->M.max_t + fcap * 4 + sizeof(FramePose);
+    if ((e = mdev_alloc(h, &h->b_fp, 1)) != cudaSuccess) return e;
+    return cudaDeviceSynchronize();   // the initialising memsets ran on the legacy stream, which the handle's non-blocking streams do not wait for
+}
+
+// incremental_mesh_reconstruction (src/ImMesh_mesh_reconstruction.cpp:92-267) as ONE frame of any size: append in chunks of <= B
+// candidates, then the per-voxel stage in batches of <= V meshed voxels (DESIGN.md, batched frame).  Blocking.
+static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels, int64_t* stats) {
+    if (!h || (!xyz && n > 0) || n < 0 || !pose_t || batch_points < 0 || batch_points > h->max_frame_points || batch_voxels < 0 || batch_voxels > h->F.max_work)
+        return im_fail(IMMESH_E_INVALID, "bad argument (batch_points in [0, max_frame_points], batch_voxels in [0, the frame's work capacity])");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "push_frame_batched: a sharded handle is not supported");
+    const int prev = mesh_wait_impl(h, false);   // frames queued before this one
+    if (prev) return prev;
+    IM_CUDA(mesh_batched_scratch(h));
+    const MeshParams& P = h->P;
+    const int B = batch_points ? batch_points : h->max_frame_points, V = batch_voxels ? batch_voxels : h->F.max_work;
+    // append_point_step = max(1, round(N / appending_pts_frame)), integer division first (ImMesh_mesh_reconstruction.cpp:111), 64-bit
+    const int64_t step = std::max<int64_t>(1, (int64_t)std::llround((double)(n / (int64_t)P.append_target)));
+    if (step > 0x7fffffff) return im_fail(IMMESH_E_INVALID, "push_frame_batched: append step out of range");
+    const int64_t m_total = n > 0 ? (n + step - 1) / step : 0;
+    cudaStream_t st = h->stream;
+    FrameBuf F = h->F;
+    F.dyn = nullptr;
+    F.epoch = 0;
+    F.act = h->b_act; F.max_act = h->max_vox;
+    F.work_rank = h->b_rank; F.tri_mark = h->b_mark;
+    F.fset = h->b_fset; F.fset_mask = h->b_fset_mask;
+    F.fp = h->b_fp;
+    F.frame = ++h->frame_counter;   // one frame: one frame number, one vox_frame stamp
+    FramePose fp;
+    for (int j = 0; j < 3; ++j) { fp.pose_t[j] = pose_t[j]; fp.prio_origin[j] = 0; }
+    IM_CUDA(cudaMemcpyAsync(h->b_fp, &fp, sizeof(FramePose), cudaMemcpyHostToDevice, st));
+    IM_CUDA(cudaMemsetAsync(h->M.cnt + 33, 0, 4 * sizeof(int), st));
+    // ---- append, chunk c = candidates [c B, (c + 1) B), candidate i = point i step.  Host input: gathered into the pinned slot c & 1
+    // while the device works on the other one
+    const size_t slot_pts = (size_t)h->max_frame_points * 3;
+    int64_t chunks = 0;
+    for (int64_t c0 = 0; c0 < m_total || chunks == 0; c0 += B, ++chunks) {
+        const int m = (int)std::min<int64_t>(B, m_total - c0);
+        FrameBuf Fc = F;
+        Fc.m = m; Fc.n = m;
+        Fc.cmask = (unsigned)(pow2_at_least((size_t)std::max(m, 1) * 2) - 1);
+        const int s = (int)(chunks & 1);
+        if (m > 0 && !on_device) {
+            float* hs = h->h_pts + s * slot_pts;
+            float* ds = h->d_pts + s * slot_pts;
+            if (chunks >= 2) IM_CUDA(cudaEventSynchronize(h->ev_up[s]));   // the slot's previous upload has left the pinned buffer
+            if (step == 1) std::memcpy(hs, xyz + (size_t)c0 * 3, (size_t)m * 3 * sizeof(float));
+            else for (int i = 0; i < m; ++i) std::memcpy(hs + (size_t)i * 3, xyz + (size_t)(c0 + i) * step * 3, 3 * sizeof(float));
+            if (chunks >= 2) IM_CUDA(cudaStreamWaitEvent(h->stream_up, h->ev_in[s], 0));   // the chunk that read the slot has finished
+            IM_CUDA(cudaMemcpyAsync(ds, hs, (size_t)m * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream_up));
+            IM_CUDA(cudaEventRecord(h->ev_up[s], h->stream_up));
+            IM_CUDA(cudaStreamWaitEvent(st, h->ev_up[s], 0));
+            Fc.pts = ds; Fc.step = 1;
+        } else {
+            Fc.pts = xyz ? xyz + (size_t)c0 * step * 3 : nullptr;
+            Fc.step = (int)step;
+        }
+        if (chunks == 0) IM_LAUNCH(k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, Fc);
+        else IM_LAUNCH(k_bat_chunk_begin, h->n_sm * 8, 256, 0, st, h->M, Fc);
+        if (m > 0) {
+            const int g = mesh_grid(h, m, 128);
+            IM_LAUNCH(k_cand_init, g, 128, 0, st, h->M, P, Fc);
+            IM_LAUNCH(k_cand_conflicts, g, 128, 0, st, h->M, P, Fc);
+            IM_LAUNCH(k_cand_resolve, h->n_sm * 4, 128, 0, st, h->M, P, Fc);
+            IM_LAUNCH(k_cand_scan, 1, 1024, 0, st, h->M, Fc);
+            IM_LAUNCH(k_cand_commit, g, 128, 0, st, h->M, P, Fc);
+            IM_LAUNCH(k_cand_place, g, 128, 0, st, h->M, Fc);
+        }
+        IM_LAUNCH(k_bat_chunk_end, 1, 1, 0, st, h->M);
+        if (m > 0 && !on_device) IM_CUDA(cudaEventRecord(h->ev_in[s], st));
+    }
+    if (m_total == 0) chunks = 0;
+    // ---- the activation rule after the last chunk; the meshed voxels in ascending key order
+    IM_LAUNCH(k_bat_select, mesh_grid(h, h->max_vox, 128), 128, 0, st, h->M, F, h->b_sel, h->b_key);
+    int nsel = 0;
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(&nsel, h->M.cnt + 36, sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    unsigned int* ku[2] = {h->b_ku, h->b_ku + h->max_vox};
+    unsigned int* vu[2] = {h->b_vu, h->b_vu + h->max_vox};
+    int cur = 0;
+    if (nsel > 0) {
+        const int nb = (nsel + VG_TILE - 1) / VG_TILE, g = mesh_grid(h, nsel, 128);
+        for (int half = 0; half < 2; ++half) {
+            IM_LAUNCH(k_bat_word, g, 128, 0, st, nsel, half, (const unsigned long long*)h->b_key, half == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur],
+                      ku[cur ^ 1], vu[cur ^ 1]);
+            cur ^= 1;
+            for (int pass = 0; pass < 4; ++pass) {
+                IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], nsel, 8 * pass, h->b_hist, nb);
+                IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->b_hist, 256 * nb, (int*)nullptr);
+                IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], nsel, 8 * pass,
+                          (const int*)h->b_hist, nb);
+                cur ^= 1;
+            }
+        }
+    }
+    const unsigned int* order = vu[cur];
+    const int nbat = (nsel + V - 1) / V;
+    const int g_fill = mesh_grid(h, V, 128);
+    // ---- pass 1: every dilation of the frame, with its smoothing store, before any orientation
+    for (int b = 0; b < nbat; ++b) {
+        IM_LAUNCH(k_bat_reset, 1, 32, 0, st, h->M, F, 0);
+        IM_LAUNCH(k_bat_fill, g_fill, 128, 0, st, h->M, F, (const int*)h->b_sel, order, b * V, std::min(nsel, (b + 1) * V), h->b_rank);
+        IM_LAUNCH(k_voxel_dilate, h->n_sm * h->dilate_bps, 128, 0, st, h->M, P, F);
+    }
+    // ---- pass 2: the dilation lists again (the smoothing reads raw positions: the re-store writes the same bits), triangulation,
+    // pull + commit against the pre-frame store, the batch's additions pushed at once
+    for (int b = 0; b < nbat; ++b) {
+        IM_LAUNCH(k_bat_reset, h->n_sm * 8, 256, 0, st, h->M, F, 1);
+        IM_LAUNCH(k_bat_fill, g_fill, 128, 0, st, h->M, F, (const int*)h->b_sel, order, b * V, std::min(nsel, (b + 1) * V), h->b_rank);
+        IM_LAUNCH(k_voxel_dilate, h->n_sm * h->dilate_bps, 128, 0, st, h->M, P, F);
+        IM_CUDA(cudaEventRecord(h->ev_fork, st));
+        IM_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
+        IM_CUDA(cudaStreamWaitEvent(h->stream3, h->ev_fork, 0));
+        IM_LAUNCH(k_voxel_tri_warp, h->n_sm * h->bps, 128, 4 * sizeof(MeshWarpSmem<128>), h->stream2, h->M, P, F, h->warp_nmax);
+        IM_CUDA(cudaEventRecord(h->ev_join, h->stream2));
+        IM_LAUNCH(k_pull_vertices, h->n_sm * 8, 128, 0, h->stream3, h->M, P, F);
+        IM_CUDA(cudaEventRecord(h->ev_join3, h->stream3));
+        IM_LAUNCH((k_voxel_mesh<256>), h->n_sm * h->bps, 128, sizeof(MeshSmem<256>), st, h->M, P, F, h->warp_nmax, 1);
+        IM_CUDA(cudaStreamWaitEvent(st, h->ev_join, 0));
+        IM_CUDA(cudaStreamWaitEvent(st, h->ev_join3, 0));
+        IM_LAUNCH((k_voxel_mesh<1024>), h->n_sm * 2, 128, sizeof(MeshSmem<1024>), st, h->M, P, F, 256, 0);
+        IM_LAUNCH(k_commit_faces, h->n_sm * 8, 128, 0, st, h->M, P, F);
+        IM_LAUNCH(k_pull_check, h->n_sm * 8, 128, 0, st, h->M, F);
+        IM_LAUNCH(k_bat_push_add, h->n_sm * 2, 128, 0, st, h->M, F);
+        IM_LAUNCH(k_bat_batch_end, 1, 1, 0, st, h->M);
+    }
+    IM_LAUNCH(k_bat_sweep, h->n_sm * 8, 128, 0, st, h->M, F);
+    IM_LAUNCH(k_bat_frame_end, 1, 1, 0, st, h->M);
+    IM_CUDA(cudaGetLastError());
+    int cnt[32];
+    IM_CUDA(cudaMemcpyAsync(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    std::memcpy(h->last_cnt, cnt, sizeof(cnt));
+    if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->b_bytes; stats[3] = cnt[7]; }
+    return mesh_status(cnt[3]);
+}
+
+int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* world_xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels,
+                                   int64_t* stats) {
+    return mesh_push_batched(h, world_xyz, n, on_device, pose_t, batch_points, batch_voxels, stats);
+}
+
+int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int64_t n, int on_device, float leaf, int* too_small);   // frontend_capi.cu
+
+int immesh_mesh_reconstruct_from_pointcloud_batched(immesh_mesh_t* h, immesh_voxelgrid_t* vg, const float* xyz, int64_t n, int on_device, double minimum_pts_distance,
+                                                    int batch_points, int batch_voxels, int64_t* n_meshed_points) {
+    if (!h || !vg || (!xyz && n > 0) || n < 0 || !(minimum_pts_distance > 0)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "reconstruct_from_pointcloud_batched: a sharded handle is not supported");
+    if (batch_points < 0 || batch_points > h->max_frame_points || batch_voxels < 0 || batch_voxels > h->F.max_work)
+        return im_fail(IMMESH_E_INVALID, "bad argument (batch_points in [0, max_frame_points], batch_voxels in [0, the frame's work capacity])");
+    if (n_meshed_points) *n_meshed_points = 0;
+    const double zero[3] = {0.0, 0.0, 0.0};
+    int small = 0;
+    if (n > 0) {
+        const int rc = immesh_voxelgrid_leaf_too_small(vg, xyz, n, on_device, (float)minimum_pts_distance, &small);
+        if (rc) return rc;
+    }
+    if (small || n == 0) {   // PCL passes the cloud through: every raw point goes into the frame, whatever the VoxelGrid handle holds
+        if (n_meshed_points) *n_meshed_points = n;
+        return mesh_push_batched(h, xyz, n, on_device, zero, batch_points, batch_voxels, nullptr);
+    }
+    int m = 0, small2 = 0;
+    const int rc = n > 0x7fffffff ? IMMESH_E_CAPACITY : immesh_voxelgrid_filter(vg, xyz, (int)n, on_device, (float)minimum_pts_distance, nullptr, &m, &small2);
+    if (rc == IMMESH_E_CAPACITY)
+        return im_fail(IMMESH_E_CAPACITY, "reconstruct_from_pointcloud_batched: PCL down-samples this cloud and it holds more points than the VoxelGrid handle's max_points");
+    if (rc) return rc;
+    if (n_meshed_points) *n_meshed_points = m;
+    return mesh_push_batched(h, immesh_voxelgrid_device_points(vg), m, 1, zero, batch_points, batch_voxels, nullptr);
 }
 
 int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, const double* cam_R, const double* cam_t,

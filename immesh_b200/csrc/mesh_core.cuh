@@ -167,7 +167,13 @@ struct FrameBuf {
     int4* x_face;         // new facets (a, b, c, -) of this rank's voxels             (count: cnt[30])
     unsigned long long* x_word;   // their flip-priority words
     int4* x_rem;          // triangles (a, b, c, -) this rank's voxels want removed    (count: cnt[31])
+    // batched frame (immesh_mesh_push_frame_batched: one frame's per-voxel stage in several batches); null on the per-frame path
+    const int* work_rank; // [max_work] flip priority of the work voxel: its rank among the frame's meshed voxels in (x, y, z) key order
+    unsigned char* tri_mark;   // [max_t] IM_TRI_BORN: made live by an earlier batch of this frame; IM_TRI_REMOVE: removal deferred to the frame's end
 };
+enum : unsigned char { IM_TRI_BORN = 1, IM_TRI_REMOVE = 2 };
+// a live triangle that was live before the frame began (the only ones the frame's pull and commit see)
+IM_HD bool tri_pre_frame(const FrameBuf& F, int t) { return !F.tri_mark || F.tri_mark[t] != IM_TRI_BORN; }
 
 IM_HD FrameBuf frame_load_dyn(const FrameBuf& F) {
     FrameBuf o = F;
@@ -463,28 +469,49 @@ IM_HDN inline void cand_place(const MeshDev& M, const FrameBuf& F, int c, int ba
     M.vchunk_pts[(size_t)ch * 16 + (pos & 15)] = v;
 }
 
-// activation test of ImMesh_mesh_reconstruction.cpp:132-151 (thread per activated voxel)
-IM_HDN inline void voxel_select(const MeshDev& M, const FrameBuf& F, int a) {
-    const int vs = F.act[a];
-    if (M.vox_meshing_times[vs] >= 1 || M.vox_new_added[vs] < 0) return;
+// activation test of ImMesh_mesh_reconstruction.cpp:132-151 on activated voxel vs: true when this rank meshes it in this frame
+IM_HD bool voxel_activate(const MeshDev& M, const FrameBuf& F, int vs) {
+    if (M.vox_meshing_times[vs] >= 1 || M.vox_new_added[vs] < 0) return false;
     M.vox_meshing_times[vs] += 1;
     M.vox_new_added[vs] = 0;
-    if (M.vox_count[vs] < 3) return;
-    if (F.shard_n > 1 && voxel_owner(M.vkeys[vs], F.shard_n) != F.shard_rank) return;   // another rank meshes this voxel
+    if (M.vox_count[vs] < 3) return false;
+    if (F.shard_n > 1 && voxel_owner(M.vkeys[vs], F.shard_n) != F.shard_rank) return false;   // another rank meshes this voxel
+    return true;
+}
+// voxel vs -> work list + dilation items; returns its work slot (-1: the work list is full)
+IM_HDN inline int voxel_enqueue(const MeshDev& M, const FrameBuf& F, int vs) {
     // two-ended work list: populous voxels (the expensive ones) from the front, the rest from the back, so that the
     // per-voxel stages start the long jobs first (cnt[6] = front count, cnt[17] = back count)
     int w;
     if (M.vox_count[vs] >= 20) w = im_atomic_add(&M.cnt[6], 1);
     else w = F.max_work - 1 - im_atomic_add(&M.cnt[17], 1);
-    if (w >= 0 && w < F.max_work && M.cnt[6] + M.cnt[17] <= F.max_work) F.work[w] = vs; else { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return; }
+    if (w >= 0 && w < F.max_work && M.cnt[6] + M.cnt[17] <= F.max_work) F.work[w] = vs; else { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return -1; }
     // dilation items: groups of up to 8 of the voxel's vertices (the kNN queries), so that a populous voxel is spread over
     // several thread blocks instead of serialising on one
     int nq = M.vox_count[vs];
     if (nq > IM_MAXIN) nq = IM_MAXIN;
     const int ng = (nq + 7) >> 3;
     const int base = im_atomic_add(&M.cnt[29], ng);
-    if (base + ng > F.max_ditem) { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return; }
+    if (base + ng > F.max_ditem) { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return w; }
     for (int g = 0; g < ng; ++g) F.ditem[base + g] = (w << 5) | g;
+    return w;
+}
+// thread per activated voxel
+IM_HDN inline void voxel_select(const MeshDev& M, const FrameBuf& F, int a) {
+    const int vs = F.act[a];
+    if (voxel_activate(M, F, vs)) voxel_enqueue(M, F, vs);
+}
+// Flip-priority field (33 bits) of the facets of work voxel w: the frame word keeps the largest, so among a frame's voxels the last
+// in ascending (x, y, z) key order wins.  Per-frame path: the key relative to prio_origin, 11 bits per axis (IM_MERR_PRIO_RANGE
+// beyond 1024 voxels from the sensor).  Batched frame: the voxel's rank among the frame's meshed voxels in the same order -- the same
+// winner wherever the 11-bit field is in range, and no range limit.
+IM_HD unsigned long long voxel_prio(const MeshDev& M, const FrameBuf& F, int w, bool report) {
+    if (F.work_rank) return (unsigned long long)(unsigned int)F.work_rank[w];
+    int kx, ky, kz;
+    unpack_ikey(M.vkeys[F.work[w]], &kx, &ky, &kz);
+    const long long lx = kx - F.fp->prio_origin[0], ly = ky - F.fp->prio_origin[1], lz = kz - F.fp->prio_origin[2];
+    if (report && (lx < 0 || lx >= 2048 || ly < 0 || ly >= 2048 || lz < 0 || lz >= 2048)) im_atomic_or(&M.cnt[3], IM_MERR_PRIO_RANGE);
+    return ((unsigned long long)(lx & 2047) << 22) | ((unsigned long long)(ly & 2047) << 11) | (unsigned long long)(lz & 2047);
 }
 
 // i-th work item (0 <= i < cnt[6] + cnt[17]) -> slot in the two-ended work arrays
@@ -692,8 +719,9 @@ IM_HDN inline int tri_find(const MeshDev& M, int a, int b, int c) {
     }
     return -1;
 }
-// insert_triangle (triangle.hpp:330-395): find-or-create, mark alive, link into the three incidence lists on creation
-IM_HDN inline void tri_add(const MeshDev& M, int a, int b, int c, unsigned long long flipword) {
+// insert_triangle (triangle.hpp:330-395): find-or-create, mark alive, link into the three incidence lists on creation; returns the
+// triangle's index (-1 on a full pool or hash)
+IM_HDN inline int tri_add(const MeshDev& M, int a, int b, int c, unsigned long long flipword) {
     unsigned int s = tri_hash(a, b, c) & M.tmask;
     int mine = -1;
     int t = -1;
@@ -702,7 +730,7 @@ IM_HDN inline void tri_add(const MeshDev& M, int a, int b, int c, unsigned long 
         if (cur < 0) {
             if (mine < 0) {
                 mine = im_atomic_add(&M.cnt[1], 1);
-                if (mine >= M.max_t) { im_atomic_or(&M.cnt[3], IM_MERR_TRI_POOL); return; }
+                if (mine >= M.max_t) { im_atomic_or(&M.cnt[3], IM_MERR_TRI_POOL); return -1; }
                 M.tri[mine] = make_int4(a, b, c, 0);
                 M.tri_flip[mine] = 0ull;
                 M.tri_next[(size_t)mine * 3 + 0] = -1; M.tri_next[(size_t)mine * 3 + 1] = -1; M.tri_next[(size_t)mine * 3 + 2] = -1;
@@ -715,7 +743,7 @@ IM_HDN inline void tri_add(const MeshDev& M, int a, int b, int c, unsigned long 
         if (r.x == a && r.y == b && r.z == c) { t = cur; break; }
         s = (s + 1) & M.tmask;
     }
-    if (t < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); return; }
+    if (t < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); return -1; }
     if (t == mine) {
         const int vs[3] = {a, b, c};
 #if defined(__CUDA_ARCH__)
@@ -736,6 +764,7 @@ IM_HDN inline void tri_add(const MeshDev& M, int a, int b, int c, unsigned long 
     // (a record allocated by a thread that lost the publication race stays unused: a leaked slot, never linked)
     if (im_atomic_exch(&M.tri[t].w, 1) == 0) im_atomic_add(&M.cnt[2], 1);
     im_atomic_max64(&M.tri_flip[t], flipword);
+    return t;
 }
 IM_HD void tri_remove(const MeshDev& M, int t) {  // erase_triangle, triangle.hpp:164-210
     if (im_atomic_exch(&M.tri[t].w, 0) == 1) im_atomic_add(&M.cnt[2], -1);

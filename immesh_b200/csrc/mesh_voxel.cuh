@@ -44,9 +44,9 @@ IM_HD int im_popc(unsigned m) {
 // all-gathered lists of all ranks to its replica (apply_*), so the replicas stay set-identical.
 IM_HD void apply_face(const MeshDev& M, const FrameBuf& F, int a, int b, int c, unsigned long long word) {
     // commit, faces side (triangle_compare): a face already live in the store is "existing" (its flip priority word is
-    // raised), otherwise it goes to the add list
+    // raised), otherwise it goes to the add list.  Batched frame: a triangle an earlier batch added is not "in the store" yet.
     const int t = tri_find(M, a, b, c);
-    if (t >= 0 && M.tri[t].w) {
+    if (t >= 0 && M.tri[t].w && tri_pre_frame(F, t)) {
         im_atomic_max64(&M.tri_flip[t], word);
     } else {
         const int e = im_atomic_add(&M.cnt[7], 1);
@@ -72,6 +72,11 @@ IM_HD void emit_remove(const MeshDev& M, const FrameBuf& F, int t) {
         const int4 tr = M.tri[t];
         const int e = im_atomic_add(&M.cnt[31], 1);
         if (e < F.x_cap) F.x_rem[e] = make_int4(tr.x, tr.y, tr.z, 0); else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        return;
+    }
+    if (F.tri_mark) {   // batched frame: counted now, removed after the last batch (only pre-frame triangles are pulled)
+        im_atomic_add(&M.cnt[8], 1);
+        F.tri_mark[t] = IM_TRI_REMOVE;
         return;
     }
     const int e = im_atomic_add(&M.cnt[8], 1);
@@ -481,16 +486,9 @@ IM_HDN inline void voxel_dilate(const MeshDev& M, const MeshParams& P, const Fra
 // ------------------------------------------------------------------ stage B
 // commit (triangle_compare) + orientation (correct_triangle_index) + pull (find_relative_triangulation_combination) of one
 // voxel, given its ascending dilated id list, its new facets (sorted id triples) and a hash set over them.
-IM_HDN inline void voxel_commit_common(const MeshDev& M, const MeshParams& P, const FrameBuf& F, int vs, int n, const int* ids, int nf,
+IM_HDN inline void voxel_commit_common(const MeshDev& M, const MeshParams& P, const FrameBuf& F, int w, int n, const int* ids, int nf,
                                        const int (*faces)[3], const int* fhash, unsigned int hmask, const double* axes, int tid, int nthreads) {
-    // flip priority of this voxel: its key relative to the frame origin (ascending (x,y,z) order, last one wins)
-    int kx, ky, kz;
-    unpack_ikey(M.vkeys[vs], &kx, &ky, &kz);
-    const long long lx = kx - F.fp->prio_origin[0], ly = ky - F.fp->prio_origin[1], lz = kz - F.fp->prio_origin[2];
-    if (lx < 0 || lx >= 2048 || ly < 0 || ly >= 2048 || lz < 0 || lz >= 2048) {
-        if (tid == 0) im_atomic_or(&M.cnt[3], IM_MERR_PRIO_RANGE);
-    }
-    const unsigned long long prio = ((unsigned long long)(lx & 2047) << 22) | ((unsigned long long)(ly & 2047) << 11) | (unsigned long long)(lz & 2047);
+    const unsigned long long prio = voxel_prio(M, F, w, tid == 0);
     const unsigned long long word_base = ((unsigned long long)F.frame << 34) | (prio << 1);
     // commit, faces side (triangle_compare): a face already live in the store is "existing", otherwise "to add"
     for (int k = tid; k < nf; k += nthreads) {
@@ -507,7 +505,7 @@ IM_HDN inline void voxel_commit_common(const MeshDev& M, const MeshParams& P, co
             const int4 r = M.tri[t];
             const int slot = (r.x == v) ? 0 : ((r.y == v) ? 1 : 2);
             const int nx = M.tri_next[(size_t)t * 3 + slot];
-            if (r.w && r.x == v) {
+            if (r.w && r.x == v && tri_pre_frame(F, t)) {
                 // binary search y and z in the ascending id list
                 bool in_set = true;
                 for (int pass = 0; pass < 2 && in_set; ++pass) {
@@ -561,7 +559,6 @@ IM_HDN inline void voxel_mesh(const MeshDev& M, const MeshParams& P, const Frame
     const int n = nraw < 0 ? -nraw : nraw;   // negative: handed over to the large variant after a capacity overflow
     if (store_only && tid == 0) F.work_nfaces[w] = (n > MAXD) ? -1 : 0;   // -1: left to the large (monolithic) variant
     if (n < 3 || n > MAXD) return;
-    const int vs = F.work[w];
     for (int i = tid; i < n; i += nthreads) {
         const int id = F.work_ids[(size_t)w * IM_MAXD + i];
         S->ids[i] = id;
@@ -656,7 +653,7 @@ IM_HDN inline void voxel_mesh(const MeshDev& M, const MeshParams& P, const Frame
         if (tid == 0) F.work_nfaces[w] = nf;
         return;
     }
-    voxel_commit_common(M, P, F, vs, n, S->ids, nf, S->faces, S->fhash, 4 * MAXD - 1, S->axes, tid, nthreads);
+    voxel_commit_common(M, P, F, w, n, S->ids, nf, S->faces, S->fhash, 4 * MAXD - 1, S->axes, tid, nthreads);
 }
 
 // ------------------------------------------------------------------ stage B, warp-level variant (small dilated sets)
@@ -959,17 +956,17 @@ IM_HD bool face_is(const int4& f, int a, int b, int c, int w) { return f.x == a 
 // C1: orientation + "existing / to add" decision of facet f, and registration in the frame's facet set
 IM_HDN inline void commit_face(const MeshDev& M, const MeshParams& P, const FrameBuf& F, int f) {
     const int4 fc = F.all_faces[f];
-    const int w = fc.w, vs = F.work[w];
-    int kx, ky, kz;
-    unpack_ikey(M.vkeys[vs], &kx, &ky, &kz);
-    const long long lx = kx - F.fp->prio_origin[0], ly = ky - F.fp->prio_origin[1], lz = kz - F.fp->prio_origin[2];
-    if (lx < 0 || lx >= 2048 || ly < 0 || ly >= 2048 || lz < 0 || lz >= 2048) im_atomic_or(&M.cnt[3], IM_MERR_PRIO_RANGE);
-    const unsigned long long prio = ((unsigned long long)(lx & 2047) << 22) | ((unsigned long long)(ly & 2047) << 11) | (unsigned long long)(lz & 2047);
-    const unsigned long long word = ((unsigned long long)F.frame << 34) | (prio << 1) |
+    const int w = fc.w;
+    const unsigned long long word = ((unsigned long long)F.frame << 34) | (voxel_prio(M, F, w, true) << 1) |
                                     (unsigned long long)compute_flip(M, fc.x, fc.y, fc.z, F.fp->pose_t, F.work_axes + (size_t)w * 9);
     emit_face(M, F, fc.x, fc.y, fc.z, word);
+    // bounded probe: a full set is a capacity error, never a spin
     unsigned int hs = (tri_hash(fc.x, fc.y, fc.z) + (unsigned int)w * 0x9E3779B1u) & F.fset_mask;
-    while (im_atomic_cas32(&F.fset[hs], -1, f) != -1) hs = (hs + 1) & F.fset_mask;
+    for (unsigned int probe = 0;; ++probe) {
+        if (probe > F.fset_mask) { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); break; }
+        if (im_atomic_cas32(&F.fset[hs], -1, f) == -1) break;
+        hs = (hs + 1) & F.fset_mask;
+    }
 }
 // C2a: pull (find_relative_triangulation_combination) for vertex reference r = (w, i): every live triangle whose smallest
 // vertex is this one and whose other two vertices are in the voxel's dilated set.  Needs only the dilation result, so it
@@ -985,7 +982,7 @@ IM_HDN inline void pull_vertex(const MeshDev& M, const MeshParams& P, const Fram
         const int4 tr = M.tri[t];
         const int slot = (tr.x == v) ? 0 : ((tr.y == v) ? 1 : 2);
         const int nx = M.tri_next[(size_t)t * 3 + slot];
-        if (tr.w && tr.x == v) {
+        if (tr.w && tr.x == v && tri_pre_frame(F, t)) {
             bool in_set = true;
             for (int pass = 0; pass < 2 && in_set; ++pass) {
                 const int key = pass == 0 ? tr.y : tr.z;

@@ -298,6 +298,32 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
  * incremental_mesh_reconstruction frame with the identity pose.  xyz: [n][3] host array, or device pointer with on_device = 1. */
 int immesh_mesh_reconstruct_from_pointcloud(immesh_mesh_t* h, immesh_voxelgrid_t* vg, const float* xyz, int n, int on_device, double minimum_pts_distance,
                                             int* n_downsampled /*or NULL*/);
+/* One incremental_mesh_reconstruction frame (src/ImMesh_mesh_reconstruction.cpp:92-267) of any size, executed in bounded batches.
+ *   The append (append_points_to_global_map, src/meshing/r3live/pointcloud_rgbd.cpp:411-552, append_point_step = max(1, round(n /
+ *     appending_pts_frame)) with the integer division in 64 bits) runs in chunks of <= batch_points candidates, in scan order; the
+ *     activation test (:132-151) runs once after the last chunk; the meshed voxels are then processed in batches of <= batch_voxels:
+ *     first every batch's dilation with its smoothing (retrieve_neighbor_pts_kdtree), then every batch's triangulation, pull and commit
+ *     against the store as it was before the frame, its new facets pushed at once; removals are applied after the last batch.
+ *   Result: bit-identical to one unbatched frame on the same points (vertices and ids, smoothed positions and m_smoothed flags, facets,
+ *     m_index_flip, immesh_mesh_counts), whatever the batch sizes.  The orientation priority is the voxel's rank among the frame's meshed
+ *     voxels in (x, y, z) key order, so, unlike immesh_mesh_push_frame, no voxel is too far from pose_t (IMMESH_E_RANGE).
+ *   batch_points: <= max_frame_points, 0 = max_frame_points.  batch_voxels: <= the frame's work capacity (max_voxels / 16 clamped to
+ *     [65536, 262144], or max_voxels when smaller), 0 = that capacity.  Other values, or a sharded handle: IMMESH_E_INVALID.  A batch whose
+ *     facets or dilated sets overflow the per-frame lists returns IMMESH_E_CAPACITY (flag LIST_CAP): use smaller batches.
+ *   world_xyz: [n][3] host array, read chunk by chunk through the handle's pinned slots (double-buffered, not copied whole), or a
+ *     device pointer with on_device = 1.  Scratch beyond the mesh pools is allocated by the first call and sized by the handle's
+ *     capacities only.  stats (or NULL): [append chunks, voxel batches, scratch bytes, facet add entries].  Blocking; frames queued
+ *     before the call are drained first. */
+int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* world_xyz /*[n][3]*/, int64_t n, int on_device, const double* pose_t /*[3]*/,
+                                   int batch_points, int batch_voxels, int64_t* stats /*[4] or NULL*/);
+/* reconstruct_mesh_from_pointcloud (src/ImMesh_mesh_reconstruction.cpp:328-345) on a cloud of any size.  PCL's VoxelGrid decision is
+ * made on the whole cloud (its bounding box reduced chunk by chunk with the VoxelGrid's own kernels, so "leaf size too small" matches
+ * immesh_voxelgrid_filter exactly).  Passed through (the usual case at minimum_pts_distance = 0.01 m for clouds wider than about 13 m):
+ * the raw cloud goes into the batched frame and vg's capacity does not matter.  Filtered: vg down-samples it (more than vg's max_points:
+ * IMMESH_E_CAPACITY) and the result goes into the batched frame.  Identity pose.  *n_meshed_points: points given to the frame. */
+int immesh_mesh_reconstruct_from_pointcloud_batched(immesh_mesh_t* h, immesh_voxelgrid_t* vg, const float* xyz, int64_t n, int on_device,
+                                                    double minimum_pts_distance, int batch_points, int batch_voxels,
+                                                    int64_t* n_meshed_points /*or NULL*/);
 /* Depth rasterisation of the live mesh from a camera -- the reference's "LiDAR point-cloud reinforcement" (src/ImMesh_node.cpp:305-329:
  * draw_triangle into the depth camera, Cam_view::read_depth, convert_depth_buffer_to_truth_depth + unproject_point,
  * src/tools/openGL_libs/openGL_camera_view.cpp:316-418) as a CUDA rasteriser over the device-resident triangle store.
