@@ -98,10 +98,41 @@ __global__ void __launch_bounds__(MATCH_THREADS, 8) k_match(VoxelMapDev map, Lio
     IM_STAMP(7, 0);
 }
 
+// Publish a block's normal-equation sums (2^-20 fixed point, DESIGN.md 3) into the (hi, lo) accumulator pairs `dst`: thread, warp and
+// block sums in int64, the block's sum split into its 32-bit halves for the atomics.  The block sum of 128 thread sums cannot leave
+// int64 while every thread sum is below 2^56 in magnitude, and a thread sum stays exact while it holds at most IM_FX_THREAD_TERMS
+// terms (each below 1e10 * 2^20, residual_terms refuses larger ones).  Beyond either bound -- a dense scan with very large weights,
+// where a block's int64 sum used to wrap silently -- the call fails with IMMESH_E_RANGE.  The flag is raised once per block after the
+// warp sums (a global atomic in every thread ahead of the shuffles made k_terms 60 % slower).
+#define IM_FX_THREAD_TERMS 879   // floor(2^63 / (1e10 * 2^20))
+__device__ __forceinline__ void publish_terms(const long long (&acc)[IM_NTERMS], unsigned long long* dst, int* err) {
+    __shared__ long long s_part[RES_THREADS / 32][IM_NTERMS];
+    long long mag = 0;   // bit 56 or above set iff some acc[k] lies outside [-2^56, 2^56) (x ^ (x >> 63) is x, or -x - 1 for negative x)
+#pragma unroll
+    for (int k = 0; k < IM_NTERMS - 1; ++k) mag |= acc[k] ^ (acc[k] >> 63);
+    const int out_of_range = (acc[28] > IM_FX_THREAD_TERMS || mag >= (1LL << 56)) ? 1 : 0;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < IM_NTERMS - 1; ++k) {
+        long long v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) s_part[warp][k] = v;
+    }
+    if (__syncthreads_or(out_of_range) && threadIdx.x == 0) atomicOr(err, IM_ERR_FX_RANGE);
+    if (threadIdx.x < IM_NTERMS - 1) {
+        long long v = 0;
+        for (int w = 0; w < RES_THREADS / 32; ++w) v += s_part[w][threadIdx.x];
+        if (v != 0) {
+            atomicAdd(&dst[2 * threadIdx.x], (unsigned long long)(v >> 32));
+            atomicAdd(&dst[2 * threadIdx.x + 1], (unsigned long long)(v & 0xffffffffLL));
+        }
+    }
+}
+
 template <bool MATCHED>
 __device__ __forceinline__ void residual_block(const VoxelMapDev& map, const LioParams& P, const ScanBuf& sb_, LioCtrl* ctrl, int iter, int fused_solve) {
     __shared__ double s_state[24 + 6 * 18];
-    __shared__ long long s_part[RES_THREADS / 32][IM_NTERMS];
     IM_STAMP(10, 0);
     // the stop flag, the scan's device-resident description and the state -- rot/pos and the 6x6 pose block of the covariance, the only
     // parts this pass reads -- are loaded together (one trip to L2 instead of three)
@@ -127,23 +158,7 @@ __device__ __forceinline__ void residual_block(const VoxelMapDev& map, const Lio
         }
     }
     IM_STAMP(12, acc[0] + acc[27]);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < IM_NTERMS - 1; ++k) {
-        long long v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_part[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < IM_NTERMS - 1) {
-        long long v = 0;
-        for (int w = 0; w < RES_THREADS / 32; ++w) v += s_part[w][threadIdx.x];
-        if (v != 0) {
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x], (unsigned long long)(v >> 32));
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x + 1], (unsigned long long)(v & 0xffffffffLL));
-        }
-    }
+    publish_terms(acc, ctrl->acc[iter], map.err);
     IM_STAMP(13, 0);
     if (!fused_solve) return;
     // the last block to publish its sums runs the IESKF update of this iteration (6x6 form, lio_core.cuh: ieskf_solve)
@@ -180,7 +195,6 @@ __global__ void __launch_bounds__(RES_THREADS) k_shard_pass1(VoxelMapDev map, Li
 }
 __global__ void __launch_bounds__(RES_THREADS) k_shard_pass2(VoxelMapDev map, LioParams P, ScanBuf sb_, LioCtrl* ctrl, int iter, const unsigned int* bits, int words_cap) {
     __shared__ double s_state[24 + 6 * 18];
-    __shared__ long long s_part[RES_THREADS / 32][IM_NTERMS];
     if (ctrl->stop) return;
     const ScanBuf sb = scan_load_dyn(sb_);
     const int n = sb.n;
@@ -198,23 +212,7 @@ __global__ void __launch_bounds__(RES_THREADS) k_shard_pass2(VoxelMapDev map, Li
             for (int k = 0; k < IM_NTERMS; ++k) acc[k] += t[k];
         }
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < IM_NTERMS - 1; ++k) {
-        long long v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_part[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < IM_NTERMS - 1) {
-        long long v = 0;
-        for (int w = 0; w < RES_THREADS / 32; ++w) v += s_part[w][threadIdx.x];
-        if (v != 0) {
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x], (unsigned long long)(v >> 32));
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x + 1], (unsigned long long)(v & 0xffffffffLL));
-        }
-    }
+    publish_terms(acc, ctrl->acc[iter], map.err);
 }
 
 // ---- sharded VoxelMap over peer windows (peer_win.cuh): the two exchanges of an iteration are fused into the kernels.
@@ -266,7 +264,6 @@ __global__ void __launch_bounds__(RES_THREADS) k_shard_pass1_p2p(VoxelMapDev map
 // into row `rank` of every window and raises the pass-2 flag.
 __global__ void __launch_bounds__(RES_THREADS) k_shard_pass2_p2p(VoxelMapDev map, LioParams P, ScanBuf sb_, LioCtrl* ctrl, int iter, LioPeers pe, int epoch_off) {
     __shared__ double s_state[24 + 6 * 18];
-    __shared__ long long s_part[RES_THREADS / 32][IM_NTERMS];
     __shared__ int s_last;
     if (ctrl->stop) return;
     const ScanBuf sb = scan_load_dyn(sb_);
@@ -294,23 +291,7 @@ __global__ void __launch_bounds__(RES_THREADS) k_shard_pass2_p2p(VoxelMapDev map
             for (int k = 0; k < IM_NTERMS; ++k) acc[k] += t[k];
         }
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < IM_NTERMS - 1; ++k) {
-        long long v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_part[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < IM_NTERMS - 1) {
-        long long v = 0;
-        for (int w = 0; w < RES_THREADS / 32; ++w) v += s_part[w][threadIdx.x];
-        if (v != 0) {
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x], (unsigned long long)(v >> 32));
-            atomicAdd(&ctrl->acc[iter][2 * threadIdx.x + 1], (unsigned long long)(v & 0xffffffffLL));
-        }
-    }
+    publish_terms(acc, ctrl->acc[iter], map.err);
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) s_last = (atomicAdd(&ctrl->shard_cnt[1], 1) == (int)gridDim.x - 1);

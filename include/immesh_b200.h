@@ -72,7 +72,9 @@ int immesh_voxelmap_build(immesh_lio_t* h, const float* body_xyz /*[n][3]*/, int
 /* Voxel_mapping::lio_state_estimation (src/voxel_mapping.cpp:1284-1652): all IESKF iterations on the
  * down-sampled body-frame scan; the propagated state is the handle's state on entry.  The whole loop
  * (BuildResidualListOMP + Jacobian + H^T R^-1 H reduction + 18x18 solve + convergence logic) runs on the
- * device without host round trips. */
+ * device without host round trips.  IMMESH_E_RANGE: a coordinate outside the key range, or normal-equation sums beyond the 2^-20 fixed
+ * point (a term of 1e10 or more, or a thread's sum of 2^36 or more -- which threads sum which points depends on the GPU's SM count);
+ * the state is then undefined and should be restored by the caller. */
 int immesh_lio_estimate(immesh_lio_t* h, const float* body_xyz /*[n][3]*/, int n, int* iters_run);
 
 /* Voxel_mapping::map_incremental_grow, VoxelMap part (src/ImMesh_mesh_reconstruction.cpp:387-408 ->
@@ -131,7 +133,10 @@ int immesh_residual_build(immesh_lio_t* h, const float* body_xyz, int n, int* in
 /* The three free functions of src/voxel_mapping.hpp:80-105 on caller-built Point_with_var lists (what the shim in
  * immesh_b200/csrc/immesh_shim.hpp forwards to).  pts_world: m_point (insert path) / m_point_world (lookup path),
  * var9: m_var row-major, pts_body: m_point of the lookup path.  The caller's order is kept (updateVoxelMap expects
- * its input already sorted by var_contrast). */
+ * its input already sorted by var_contrast).
+ * The insert calls (_build_pv, _update_pv) store every world point as float, as the reference's Point_with_var lists are filled
+ * from pcl::PointXYZI clouds at every call site: pts_world is rounded to float on entry, so a map built from doubles equals the map
+ * built from their float roundings.  The lookup call (_residual_build_pv) uses pts_world as given, in double. */
 int immesh_voxelmap_build_pv(immesh_lio_t* h, const double* pts_world /*[n][3]*/, const double* var9 /*[n][9]*/, int n);
 int immesh_voxelmap_update_pv(immesh_lio_t* h, const double* pts_world /*[n][3]*/, const double* var9 /*[n][9]*/, int n);
 int immesh_residual_build_pv(immesh_lio_t* h, const double* pts_body, const double* pts_world, const double* var9, int n,

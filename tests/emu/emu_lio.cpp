@@ -268,8 +268,8 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
     for (int i = 0; i < n; ++i) prepare_point(h->P, h->sb, i);
     SolveScratch S;
     for (int it = 0; it < h->P.max_iter && !c.stop; ++it) {
-        long long sum[IM_NTERMS];
-        for (int k = 0; k < IM_NTERMS; ++k) sum[k] = 0;
+        long long hi[IM_NTERMS], lo[IM_NTERMS];   // each term split into its 32-bit halves as it is added: no partial sum can wrap
+        for (int k = 0; k < IM_NTERMS; ++k) hi[k] = lo[k] = 0;
         if (g_split == 1)
             for (int i = 0; i < n; ++i) match_lanes_point(h, c.state, i);   // k_match, 8 lanes per point
         else if (g_split == 2)
@@ -279,11 +279,11 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
             const bool hit = g_split ? residual_point_matched(h->map, h->P, h->sb, c.state, i, t, h->map.err)   // k_terms
                                      : residual_point(h->map, h->P, h->sb, c.state, i, t, h->map.err);            // k_residual
             if (hit)
-                for (int k = 0; k < IM_NTERMS; ++k) sum[k] += t[k];
+                for (int k = 0; k < IM_NTERMS; ++k) { hi[k] += t[k] >> 32; lo[k] += t[k] & 0xffffffffLL; }
         }
         for (int k = 0; k < IM_NTERMS; ++k) {
-            c.acc[it][2 * k] += (unsigned long long)(sum[k] >> 32);
-            c.acc[it][2 * k + 1] += (unsigned long long)(sum[k] & 0xffffffffLL);
+            c.acc[it][2 * k] += (unsigned long long)hi[k];
+            c.acc[it][2 * k + 1] += (unsigned long long)lo[k];
         }
         ieskf_solve(h->P, &c, it, &S, 0, 1);
     }
@@ -347,16 +347,16 @@ int emu_shard_pass1(immesh_lio_t* h) {
 int emu_shard_pass2(immesh_lio_t* h, int it) {
     const int n = h->sb.n;
     const size_t w = (size_t)(n + 31) / 32 + 1;
-    long long sum[IM_NTERMS];
-    for (int k = 0; k < IM_NTERMS; ++k) sum[k] = 0;
+    long long hi[IM_NTERMS], lo[IM_NTERMS];
+    for (int k = 0; k < IM_NTERMS; ++k) hi[k] = lo[k] = 0;
     for (int i = 0; i < n; ++i) {
         long long t[IM_NTERMS];
         if (shard_pass2_point(h->map, h->P, h->sb, h->ctrl.state, i, h->bits.data(), h->bits.data() + w, t, h->map.err))
-            for (int k = 0; k < IM_NTERMS; ++k) sum[k] += t[k];
+            for (int k = 0; k < IM_NTERMS; ++k) { hi[k] += t[k] >> 32; lo[k] += t[k] & 0xffffffffLL; }
     }
     for (int k = 0; k < IM_NTERMS; ++k) {
-        h->ctrl.acc[it][2 * k] = (unsigned long long)(sum[k] >> 32);
-        h->ctrl.acc[it][2 * k + 1] = (unsigned long long)(sum[k] & 0xffffffffLL);
+        h->ctrl.acc[it][2 * k] = (unsigned long long)hi[k];
+        h->ctrl.acc[it][2 * k + 1] = (unsigned long long)lo[k];
     }
     return 0;
 }
