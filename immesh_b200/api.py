@@ -132,6 +132,12 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_launch_count", []),
         ("immesh_graph_stats", [vp, vp, C.POINTER(C.c_int64)]),
         ("immesh_lio_last_timing", [vp, dp]),
+        ("immesh_lio_capacity", [vp, C.POINTER(C.c_int64)]),
+        ("immesh_lio_reserve", [vp, C.c_int64, C.c_int64, C.c_int64]),
+        ("immesh_lio_set_growth", [vp, C.c_int64]),
+        ("immesh_mesh_capacity", [vp, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_reserve", [vp, C.c_int64, C.c_int64, C.c_int64]),
+        ("immesh_mesh_set_growth", [vp, C.c_int64]),
         ("immesh_mesh_create", [C.POINTER(_MeshCfg), C.POINTER(vp)]),
         ("immesh_mesh_destroy", [vp]),
         ("immesh_mesh_push_frame", [vp, fp, C.c_int, dp, C.c_int]),
@@ -434,6 +440,22 @@ class Lio:
         self.lib.immesh_lio_last_timing(self._h, o.ctypes.data_as(C.POINTER(C.c_double)))
         return o
 
+    # --- long runs: capacities and growth of the map pools
+    def capacity(self):
+        """dict(root_slots, roots, nodes_cap, nodes, chunks_cap, chunks, device_bytes, growths)"""
+        o = np.zeros(8, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_lio_capacity(self._h, o.ctypes.data_as(C.POINTER(C.c_int64))), "lio_capacity")
+        keys = ("root_slots", "roots", "nodes_cap", "nodes", "chunks_cap", "chunks", "device_bytes", "growths")
+        return dict(zip(keys, (int(v) for v in o)))
+
+    def reserve(self, root_slots=0, nodes=0, chunks=0):
+        """Grow the pools to at least these capacities (0: keep); never shrinks."""
+        _check(self.lib, self.lib.immesh_lio_reserve(self._h, root_slots, nodes, chunks), "lio_reserve")
+
+    def set_growth(self, max_bytes):
+        """Automatic growth before every step, up to max_bytes of device memory for the handle (0: off)."""
+        _check(self.lib, self.lib.immesh_lio_set_growth(self._h, max_bytes), "lio_set_growth")
+
 
 class Mesh:
     """Mirror of incremental_mesh_reconstruction + Global_map/Triangle_manager snapshot + KD_TREE::Nearest_Search."""
@@ -616,6 +638,22 @@ class Mesh:
                                                              nt.value, rkeys.ctypes.data_as(i32), roff.ctypes.data_as(i32), nr.value, box,
                                                              C.byref(nr), C.byref(nt), C.byref(ns)), "mesh_region_buffers")
         return xyz, ids, rkeys, roff, ns.value
+
+    # --- long runs: capacities and growth of the mesh pools
+    def capacity(self):
+        """dict(vertices_cap, vertices, triangles_cap, triangles, voxels_cap, voxels, device_bytes, growths)"""
+        o = np.zeros(8, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_mesh_capacity(self._h, o.ctypes.data_as(C.POINTER(C.c_int64))), "mesh_capacity")
+        keys = ("vertices_cap", "vertices", "triangles_cap", "triangles", "voxels_cap", "voxels", "device_bytes", "growths")
+        return dict(zip(keys, (int(v) for v in o)))
+
+    def reserve(self, vertices=0, triangles=0, voxels=0):
+        """Grow the pools to at least these capacities (0: keep); never shrinks."""
+        _check(self.lib, self.lib.immesh_mesh_reserve(self._h, vertices, triangles, voxels), "mesh_reserve")
+
+    def set_growth(self, max_bytes):
+        """Automatic growth before every frame, up to max_bytes of device memory for the handle (0: off)."""
+        _check(self.lib, self.lib.immesh_mesh_set_growth(self._h, max_bytes), "mesh_set_growth")
 
     def last_timing(self):
         o = np.zeros(4)

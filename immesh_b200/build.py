@@ -130,6 +130,15 @@ def build_batched(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "batched", "emu_batched.cpp"), EMU_BATCHED, force, extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")])
 
 
+EMU_GROWTH = os.path.join(_ROOT, "tests", "growth", "libimmesh_emu_growth.so")
+
+
+def build_growth(force=False):
+    """tests/growth: the host emulation with the plane-map publisher's state and the pool growth of immesh_lio_reserve /
+    immesh_lio_set_growth (the migration bodies and the growth policy of immesh_b200/csrc/pool_growth.cuh)"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "growth", "emu_growth.cpp"), EMU_GROWTH, force)
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -146,6 +155,7 @@ def build_all(force=False):
     build_scanpub(force)
     build_regionbuf(force)
     build_batched(force)
+    build_growth(force)
     build_ref()
 
 

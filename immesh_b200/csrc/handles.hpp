@@ -75,6 +75,15 @@ struct immesh_lio {
     int bps = 4;              // (mesh: 3 by default, see immesh_mesh_create) resident blocks per SM of the persistent per-voxel kernels (headroom for the other stream)
     double last_ms[3] = {0, 0, 0};
     std::vector<void*> allocs;
+    size_t dev_bytes = 0;         // device bytes of `allocs` (the create-time buffers, the map pools and what dev_alloc adds later)
+    // growth of the map pools (immesh_lio_reserve / immesh_lio_set_growth)
+    long long growths = 0;        // calls that enlarged at least one pool
+    int64_t grow_max_bytes = 0;   // automatic growth before every step: 0 off, > 0 ceiling on dev_bytes
+    int known[16] = {};           // counters (d_counters layout) of the last step known to have finished
+    long long known_step = 0;     // its number among the map-growing steps (0: the empty map at create)
+    long long map_steps = 0;      // map-growing steps queued so far
+    long long slot_step[IM_SLOTS] = {};   // number of the step that used staging slot s
+    int max_step_nodes = 0, max_step_chunks = 0;   // largest node / chunk use between two noted steps (finished blocks are noted in step order)
 };
 
 struct immesh_mesh {
@@ -138,4 +147,11 @@ struct immesh_mesh {
     unsigned int b_fset_mask = 0;
     immesh::FramePose* b_fp = nullptr;
     size_t b_bytes = 0;
+    size_t dev_bytes = 0;         // device bytes of `allocs`
+    // growth of the mesh pools (immesh_mesh_reserve / immesh_mesh_set_growth)
+    long long growths = 0;
+    int64_t grow_max_bytes = 0;
+    int known[32] = {};           // counters (MeshDev::cnt layout) of the last frame known to have finished
+    int known_frame = 0;          // its frame number (0: the empty mesh at create)
+    int max_step_tris = 0;        // largest triangle allocation between two noted frames (noted oldest first)
 };

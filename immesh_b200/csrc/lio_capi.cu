@@ -10,6 +10,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/immesh_b200.h"
@@ -17,6 +18,7 @@
 #include "peer_win.cuh"
 #include "handles.hpp"
 #include "map_dump.hpp"
+#include "pool_growth.cuh"
 
 using namespace immesh;
 
@@ -557,6 +559,17 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBu
 }
 __global__ void k_scan_n(ScanBuf sb_, int* out) { *out = scan_load_dyn(sb_).n; }
 
+// ---- growth of the map pools (immesh_lio_reserve): rebuild of the root hash into a larger table, then the back-pointers to slots
+#define GROW_THREADS 256
+__global__ void __launch_bounds__(GROW_THREADS) k_rehash_roots(VoxelMapDev from, VoxelMapDev to, int* slot_map) {
+    const unsigned int cap = from.cap_mask + 1u;   // at most 2^30 slots (IM_POOL_LIMIT)
+    for (unsigned int s = blockIdx.x * blockDim.x + threadIdx.x; s < cap; s += gridDim.x * blockDim.x) rehash_root_slot(from, to, s, slot_map);
+}
+__global__ void __launch_bounds__(GROW_THREADS) k_remap_roots(VoxelMapDev to, int n_nodes, const int* from_pub_list, int n_pub, const int* slot_map) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_nodes; i += gridDim.x * blockDim.x) remap_node_root_slot(to, i, slot_map);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_pub; i += gridDim.x * blockDim.x) remap_pub_entry(from_pub_list, to, i, slot_map);
+}
+
 // ------------------------------------------------------------------ host side
 
 #include "nccl_api.hpp"
@@ -589,6 +602,7 @@ static cudaError_t dev_alloc(immesh_lio* h, T** p, size_t count, int memset_byte
     cudaError_t e = cudaMalloc(&q, count * sizeof(T));
     if (e != cudaSuccess) return e;
     h->allocs.push_back(q);
+    h->dev_bytes += count * sizeof(T);
     *p = (T*)q;
     if (memset_byte >= 0) e = cudaMemset(q, memset_byte, count * sizeof(T));
     return e;
@@ -768,6 +782,7 @@ int immesh_lio_shard(immesh_lio_t* h, int rank, int nranks, const char* unique_i
     if (!h || !unique_id128 || nranks < 1 || rank < 0 || rank >= nranks) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (nranks > IM_MAX_RANKS) return im_fail(IMMESH_E_INVALID, "at most 8 ranks (one node)");
     if (nranks == 1) { h->P.shard_rank = 0; h->P.shard_n = 1; return IMMESH_OK; }
+    if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a handle with automatic growth cannot be sharded (immesh_lio_set_growth(h, 0) first)");
     if (!nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -878,10 +893,188 @@ static void scan_rows_overwritten(immesh_lio* h, const char* by) {
     h->scan_rows = -1;
     h->scan_rows_overwritten_by = by;
 }
+// counters of map-growing step number `step`, finished: the use the growth check starts from, and the largest use of one step seen
+// so far (an older block arriving late is skipped)
+static void note_counters(immesh_lio* h, const int* c, long long step) {
+    if (step <= h->known_step) return;
+    // the difference to the last known step; over several steps (their blocks were not all seen) it bounds one step from above
+    h->max_step_nodes = std::max(h->max_step_nodes, c[0] - h->known[0]);
+    h->max_step_chunks = std::max(h->max_step_chunks, c[1] - h->known[1]);
+    std::memcpy(h->known, c, sizeof(h->known));
+    h->known_step = step;
+}
+// the result blocks of the finished steps still in the staging slots, in step order (consecutive steps: one step's use each)
+static void note_slots(immesh_lio* h, bool only_finished) {
+    int order[IM_SLOTS], n = 0;
+    for (int s = 0; s < IM_SLOTS; ++s)
+        if (h->slot_busy[s] && (!only_finished || cudaEventQuery(h->ev_slot[s]) == cudaSuccess)) order[n++] = s;
+    cudaGetLastError();   // cudaErrorNotReady of the queries
+    std::sort(order, order + n, [&](int a, int b) { return h->slot_step[a] < h->slot_step[b]; });
+    for (int i = 0; i < n; ++i) note_counters(h, h->h_out[order[i]].counters, h->slot_step[order[i]]);
+}
 static int check_flags(immesh_lio* h) {
     IM_CUDA(cudaMemcpyAsync(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->grow_max_bytes > 0) note_counters(h, h->h_ints, h->map_steps);
     return lio_flags_status(h->h_ints[4]);
+}
+
+// ---- growth of the map pools.  Bytes per record: root slot 32 (key 8, root_node 4, pub_mark 4, pub_list 4, the per-scan
+// slot_count / slot_offset / slot_cursor 12), node 944 (NodeRec 656, PlaneRec 256, PubRec 32), chunk 520 (Chunk 512, avail 4,
+// pending 4).  Node, chunk and slot ids are 32-bit ints, and the allocating atomics may count past a full pool: every pool stops
+// at 2^30 records.
+#define IM_POOL_LIMIT (1LL << 30)
+static const size_t kSlotBytes = 8 + 4 + 4 + 4 + 3 * 4;
+static const size_t kNodeBytes = sizeof(NodeRec) + sizeof(PlaneRec) + sizeof(PubRec);
+static const size_t kChunkBytes = sizeof(Chunk) + 2 * sizeof(int);
+
+static size_t pool_bytes(long long cap, long long nodes, long long chunks) {
+    return (size_t)cap * kSlotBytes + (size_t)nodes * kNodeBytes + (size_t)chunks * kChunkBytes;
+}
+// Enlarge the pools to (cap slots, nodes, chunks), each >= the current one.  Drains the handle's stream; allocates every new
+// buffer before anything is touched, so that a failure (allocation, ceiling, id limits) leaves the handle as it was; migrates on
+// the stream; frees the old buffers after the migration and drops the captured launch sequence (it holds the old pointers).
+static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chunks) {
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "a sharded handle cannot grow (its replicas would have to grow in lockstep)");
+    const long long cap0 = (long long)h->cap, nodes0 = h->max_nodes, chunks0 = h->max_chunks;
+    if (cap > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "root hash: more than 2^30 slots (32-bit slot ids)");
+    if (nodes > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "node pool: more than 2^30 node records (32-bit node ids)");
+    if (chunks > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "chunk pool: more than 2^30 chunks (32-bit chunk ids)");
+    const bool g_cap = cap > cap0, g_nodes = nodes > nodes0, g_chunks = chunks > chunks0;
+    if (!g_cap && !g_nodes && !g_chunks) return IMMESH_OK;
+    const size_t bytes = h->dev_bytes - pool_bytes(cap0, nodes0, chunks0) + pool_bytes(cap, nodes, chunks);
+    if (h->grow_max_bytes > 0 && bytes > (size_t)h->grow_max_bytes) {
+        const std::string pools = std::string(g_cap ? " root hash" : "") + (g_nodes ? " node pool" : "") + (g_chunks ? " chunk pool" : "");
+        return im_fail(IMMESH_E_CAPACITY, ("growth of the" + pools + " to " + std::to_string(bytes) + " device bytes is above the ceiling of " +
+                                           std::to_string(h->grow_max_bytes) + " (immesh_lio_set_growth)").c_str());
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+    const int n_nodes = std::min(h->h_ints[0], h->max_nodes), n_chunks = std::min(h->h_ints[1], h->max_chunks);
+    const int n_avail = std::max(0, std::min(h->h_ints[2], h->max_chunks)), n_pending = std::min(h->h_ints[3], h->max_chunks);
+    const int n_pub = std::min<long long>(h->h_ints[12], cap0);
+
+    VoxelMapDev nm = h->map;   // the map after the growth
+    ScanBuf nsb = h->sb;
+    int* slot_map = nullptr;
+    std::vector<void*> fresh;
+    const char* pool = "";
+    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
+        void* q = nullptr;
+        const cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
+        if (e == cudaSuccess) { fresh.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
+        return e;
+    };
+    cudaError_t e = cudaSuccess;
+    if (g_nodes && e == cudaSuccess) {
+        pool = "node pool";
+        if ((e = alloc(&nm.nodes, nodes)) == cudaSuccess && (e = alloc(&nm.planes, nodes)) == cudaSuccess) e = alloc(&nm.pub, nodes);
+    }
+    if (g_chunks && e == cudaSuccess) {
+        pool = "chunk pool";
+        if ((e = alloc(&nm.chunks, chunks)) == cudaSuccess && (e = alloc(&nm.avail, chunks)) == cudaSuccess) e = alloc(&nm.pending, chunks);
+    }
+    if (g_cap && e == cudaSuccess) {
+        pool = "root hash";
+        if ((e = alloc(&nm.keys, cap)) == cudaSuccess && (e = alloc(&nm.root_node, cap)) == cudaSuccess && (e = alloc(&nm.pub_mark, cap)) == cudaSuccess &&
+            (e = alloc(&nm.pub_list, cap)) == cudaSuccess && (e = alloc(&nsb.slot_count, cap)) == cudaSuccess &&
+            (e = alloc(&nsb.slot_offset, cap)) == cudaSuccess && (e = alloc(&nsb.slot_cursor, cap)) == cudaSuccess)
+            e = alloc(&slot_map, cap0);
+    }
+    if (e != cudaSuccess) {
+        for (void* q : fresh) cudaFree(q);
+        cudaGetLastError();
+        const int code = e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA;
+        return im_fail(code, (std::string(pool) + ": device allocation for the growth failed (" + cudaGetErrorString(e) + "); the handle is unchanged").c_str());
+    }
+    cudaStream_t st = h->stream;
+    auto migrate = [&]() -> cudaError_t {
+        cudaError_t r = cudaSuccess;
+#define MG(x) do { if ((r = (x)) != cudaSuccess) return r; } while (0)
+        if (g_nodes && n_nodes > 0) {
+            MG(cudaMemcpyAsync(nm.nodes, h->map.nodes, (size_t)n_nodes * sizeof(NodeRec), cudaMemcpyDeviceToDevice, st));
+            MG(cudaMemcpyAsync(nm.planes, h->map.planes, (size_t)n_nodes * sizeof(PlaneRec), cudaMemcpyDeviceToDevice, st));
+            MG(cudaMemcpyAsync(nm.pub, h->map.pub, (size_t)n_nodes * sizeof(PubRec), cudaMemcpyDeviceToDevice, st));
+        }
+        if (g_chunks) {
+            if (n_chunks > 0) MG(cudaMemcpyAsync(nm.chunks, h->map.chunks, (size_t)n_chunks * sizeof(Chunk), cudaMemcpyDeviceToDevice, st));
+            if (n_avail > 0) MG(cudaMemcpyAsync(nm.avail, h->map.avail, (size_t)n_avail * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            if (n_pending > 0) MG(cudaMemcpyAsync(nm.pending, h->map.pending, (size_t)n_pending * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        }
+        if (g_cap) {
+            MG(cudaMemsetAsync(nm.keys, 0xFF, (size_t)cap * 8, st));
+            MG(cudaMemsetAsync(nm.root_node, 0xFF, (size_t)cap * 4, st));
+            MG(cudaMemsetAsync(nm.pub_mark, 0, (size_t)cap * 4, st));
+            for (int* p : {nsb.slot_count, nsb.slot_offset, nsb.slot_cursor}) MG(cudaMemsetAsync(p, 0, (size_t)cap * 4, st));
+            nm.cap_mask = (unsigned)(cap - 1);
+            const int g = (int)std::min<long long>((cap0 + GROW_THREADS - 1) / GROW_THREADS, (long long)h->n_sm * 16);
+            IM_LAUNCH(k_rehash_roots, g, GROW_THREADS, 0, st, h->map, nm, slot_map);
+            // with the node pool kept, root_slot is rewritten in place: the last step of the migration, after every allocation succeeded
+            const int gn = (int)std::min<long long>((std::max(n_nodes, n_pub) + GROW_THREADS - 1) / GROW_THREADS + 1, (long long)h->n_sm * 16);
+            IM_LAUNCH(k_remap_roots, gn, GROW_THREADS, 0, st, nm, n_nodes, (const int*)h->map.pub_list, n_pub, (const int*)slot_map);
+        }
+        MG(cudaGetLastError());
+        MG(cudaStreamSynchronize(st));
+#undef MG
+        return r;
+    };
+    if ((e = migrate()) != cudaSuccess) {   // a sticky CUDA error: nothing new is kept
+        for (void* q : fresh) cudaFree(q);
+        cudaGetLastError();
+        return immesh::im_fail_cuda(e, __FILE__, __LINE__);
+    }
+    // the old buffers go; the new ones take their places in the handle's allocation list
+    auto swap_buf = [&](void* oldp, void* newp) {
+        if (oldp == newp) return;
+        for (void*& p : h->allocs)
+            if (p == oldp) p = newp;
+        cudaFree(oldp);
+    };
+    swap_buf(h->map.nodes, nm.nodes); swap_buf(h->map.planes, nm.planes); swap_buf(h->map.pub, nm.pub);
+    swap_buf(h->map.chunks, nm.chunks); swap_buf(h->map.avail, nm.avail); swap_buf(h->map.pending, nm.pending);
+    swap_buf(h->map.keys, nm.keys); swap_buf(h->map.root_node, nm.root_node); swap_buf(h->map.pub_mark, nm.pub_mark); swap_buf(h->map.pub_list, nm.pub_list);
+    swap_buf(h->sb.slot_count, nsb.slot_count); swap_buf(h->sb.slot_offset, nsb.slot_offset); swap_buf(h->sb.slot_cursor, nsb.slot_cursor);
+    if (slot_map) cudaFree(slot_map);
+    nm.max_nodes = (int)nodes;
+    nm.max_chunks = (int)chunks;
+    h->map = nm;
+    h->sb = nsb;
+    h->cap = (size_t)cap;
+    h->max_nodes = (int)nodes;
+    h->max_chunks = (int)chunks;
+    h->dev_bytes = bytes;
+    h->growths++;
+    h->graph.destroy();   // the next pipelined step captures the launch sequence again, with the new pointers
+    IM_CUDA(cudaGetLastError());
+    return IMMESH_OK;
+}
+// Automatic growth (immesh_lio_set_growth) before a step of n points is queued: growth_targets (pool_growth.cuh) on the use of the
+// last step known to have finished, without waiting for the others.  Only when a pool is short is the handle drained; the decision
+// is then taken again on its exact counters.
+static int lio_growth_check(immesh_lio* h, long long n) {
+    if (h->grow_max_bytes <= 0) return IMMESH_OK;
+    long long steps = 1, n_max = n;
+    note_slots(h, true);
+    for (int s = 0; s < IM_SLOTS; ++s) {
+        if (h->slot_busy[s] && h->slot_step[s] > h->known_step) {   // still in flight
+            ++steps;
+            n_max = std::max<long long>(n_max, h->h_dyn[s].n);
+        }
+    }
+    for (int pass = 0; pass < 2; ++pass) {
+        long long cap = (long long)h->cap, nodes = h->max_nodes, chunks = h->max_chunks;
+        growth_targets(h->known, steps, n_max, h->max_step_nodes, h->max_step_chunks, &cap, &nodes, &chunks);
+        const bool short_pool = cap > (long long)h->cap || nodes > h->max_nodes || chunks > h->max_chunks;
+        if (!short_pool) return IMMESH_OK;
+        if (pass == 1) return lio_grow(h, cap, nodes, chunks);
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        note_slots(h, false);
+        IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+        note_counters(h, h->h_ints, h->map_steps);
+        steps = 1;
+        n_max = n;
+    }
+    return IMMESH_OK;
 }
 // map growth of the scan described by the device-resident ScanDyn
 static void launch_grow(immesh_lio* h, int mode) {
@@ -954,9 +1147,12 @@ int immesh_lio_predict(immesh_lio_t* h, double dt, double cov_gyr, double cov_ac
 int immesh_voxelmap_build(immesh_lio_t* h, const float* body, int n) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int rc = upload_scan(h, body, n);
+    int rc = lio_growth_check(h, n);
+    if (rc) return rc;
+    rc = upload_scan(h, body, n);
     if (rc) return rc;
     h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
+    ++h->map_steps;
     launch_grow(h, 1);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -981,6 +1177,9 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
 
 int immesh_voxelmap_update(immesh_lio_t* h) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    const int rc = lio_growth_check(h, h->last_n);
+    if (rc) return rc;
+    ++h->map_steps;
     launch_grow(h, 0);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -991,6 +1190,8 @@ int immesh_voxelmap_update(immesh_lio_t* h) {
 // ONE cudaGraphLaunch (no node is touched) + ONE D2H of the LioOut block + one event.
 static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device, double dt, double cov_gyr, double cov_acc, bool allow_graph) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    const int grc = lio_growth_check(h, n);
+    if (grc) return grc;
     const int s = (++h->step_counter) & (IM_SLOTS - 1);
     if (h->slot_busy[s]) {
         const auto t0 = std::chrono::steady_clock::now();
@@ -1000,6 +1201,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     }
     h->win.epoch += IM_MAX_ITER + 1;   // epoch base of this scan: advanced exactly once per scan
     ++h->scan_counter;
+    ++h->map_steps;   // (a replayed graph runs no host code of launch_grow: counted here)
     const bool timing = !(allow_graph && h->use_graph && !profiler().enabled && (h->P.shard_n <= 1 || h->win.ok));
     if (timing) IM_CUDA(cudaEventRecord(h->ev[0], h->stream));
     int rc = upload_scan(h, body, n, on_device, s, dt, cov_gyr, cov_acc);
@@ -1033,6 +1235,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     if (!queued) IM_CUDA(cudaEventRecord(h->ev[3], h->stream));
     IM_CUDA(cudaEventRecord(h->ev_slot[s], h->stream));
     h->slot_busy[s] = 1;
+    h->slot_step[s] = h->map_steps;
     h->timed_last = queued ? 0 : 1;
     h->pose_pub_idx = h->scan_counter;
     return IMMESH_OK;
@@ -1041,6 +1244,7 @@ static int lio_wait_impl(immesh_lio_t* h, double* state_out, int* iters_run, boo
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     const int s = h->step_counter & (IM_SLOTS - 1);
     IM_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->grow_max_bytes > 0) note_slots(h, false);
     for (int i = 0; i < IM_SLOTS; ++i) h->slot_busy[i] = 0;
     if (profiler().enabled) profiler().collect();
     const LioOut& o = h->h_out[s];
@@ -1145,18 +1349,24 @@ static int upload_pv(immesh_lio* h, const double* pts_world, const double* var9,
 }
 int immesh_voxelmap_build_pv(immesh_lio_t* h, const double* pts_world, const double* var9, int n) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
-    int rc = upload_pv(h, pts_world, var9, n);
+    int rc = lio_growth_check(h, n);
+    if (rc) return rc;
+    rc = upload_pv(h, pts_world, var9, n);
     if (rc) return rc;
     scan_rows_overwritten(h, "immesh_voxelmap_build_pv");
+    ++h->map_steps;
     launch_grow(h, 3);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
 }
 int immesh_voxelmap_update_pv(immesh_lio_t* h, const double* pts_world, const double* var9, int n) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
-    int rc = upload_pv(h, pts_world, var9, n);
+    int rc = lio_growth_check(h, n);
+    if (rc) return rc;
+    rc = upload_pv(h, pts_world, var9, n);
     if (rc) return rc;
     scan_rows_overwritten(h, "immesh_voxelmap_update_pv");
+    ++h->map_steps;
     launch_grow(h, 2);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -1401,6 +1611,39 @@ int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out) {
     int counters[16];
     IM_CUDA(cudaMemcpy(counters, h->d_counters, sizeof(counters), cudaMemcpyDeviceToHost));
     out[0] = counters[5]; out[1] = counters[0]; out[2] = counters[1]; out[3] = counters[4];
+    return IMMESH_OK;
+}
+
+int immesh_lio_capacity(immesh_lio_t* h, int64_t* out) {
+    if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+    const int* c = h->h_ints;
+    out[0] = (int64_t)h->cap; out[1] = c[5];
+    out[2] = h->max_nodes; out[3] = c[0];
+    out[4] = h->max_chunks; out[5] = (int64_t)c[1] - std::max(c[2], 0);
+    out[6] = (int64_t)h->dev_bytes; out[7] = h->growths;
+    return IMMESH_OK;
+}
+int immesh_lio_reserve(immesh_lio_t* h, int64_t root_slots, int64_t nodes, int64_t chunks) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_reserve: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
+    long long cap = (long long)h->cap;
+    if (root_slots > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "root hash: more than 2^30 slots (32-bit slot ids)");
+    while (cap < root_slots) cap *= 2;
+    const int rc = lio_grow(h, cap, std::max<long long>(nodes, h->max_nodes), std::max<long long>(chunks, h->max_chunks));
+    if (rc == IMMESH_OK) return rc;
+    return im_fail(rc, (std::string("immesh_lio_reserve: ") + immesh::last_error_storage()).c_str());
+}
+int immesh_lio_set_growth(immesh_lio_t* h, int64_t max_bytes) {
+    if (!h || max_bytes < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (max_bytes > 0 && h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_set_growth: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
+    if (max_bytes > 0 && h->grow_max_bytes <= 0) {   // growth starts from the map as it is now
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+        note_counters(h, h->h_ints, ++h->map_steps);   // the map as it is now, under a step number of its own
+    }
+    h->grow_max_bytes = max_bytes;
     return IMMESH_OK;
 }
 

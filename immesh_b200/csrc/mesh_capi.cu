@@ -14,6 +14,7 @@
 #include "../../include/immesh_b200.h"
 #include "common_host.hpp"
 #include "handles.hpp"
+#include "pool_growth.cuh"
 #include "nccl_api.hpp"
 
 using namespace immesh;
@@ -245,7 +246,7 @@ __global__ void __launch_bounds__(128) k_knn(MeshDev M, MeshParams P, const floa
                 int cntv = M.vox_count[s];
                 if (cntv > IM_VCHUNKS * 16) cntv = IM_VCHUNKS * 16;
                 for (int kk = 0; kk < cntv; ++kk) {
-                    const float4 p = M.vchunk_pts[(size_t)M.vox_chunk[(size_t)s * IM_VCHUNKS + (kk >> 4)] * 16 + (kk & 15)];
+                    const float4 p = M.vchunk_pts[(size_t)im_chunk_or0(M.vox_chunk[(size_t)s * IM_VCHUNKS + (kk >> 4)]) * 16 + (kk & 15)];
                     const int v = __float_as_int(p.w);
                     const float d2 = dist2f(qx, qy, qz, p.x, p.y, p.z);
                     if (!((double)d2 <= max_d2)) continue;
@@ -562,6 +563,18 @@ __global__ void k_bat_frame_end(MeshDev M) {
     M.cnt[17] = 0;
 }
 
+// ---- growth of the mesh pools (immesh_mesh_reserve): the three open-addressed tables rebuilt into tables of the new size
+#define MGROW_THREADS 256
+__global__ void __launch_bounds__(MGROW_THREADS) k_rehash_xi(MeshDev from, MeshDev to) {
+    for (unsigned int s = blockIdx.x * blockDim.x + threadIdx.x; s <= from.gmask; s += gridDim.x * blockDim.x) rehash_xi_slot(from, to, s);
+}
+__global__ void __launch_bounds__(MGROW_THREADS) k_rehash_voxels(MeshDev from, MeshDev to) {
+    for (unsigned int s = blockIdx.x * blockDim.x + threadIdx.x; s <= from.vmask; s += gridDim.x * blockDim.x) rehash_voxel_slot(from, to, s);
+}
+__global__ void __launch_bounds__(MGROW_THREADS) k_rehash_tris(MeshDev from, MeshDev to) {
+    for (unsigned int s = blockIdx.x * blockDim.x + threadIdx.x; s <= from.tmask; s += gridDim.x * blockDim.x) rehash_tri_slot(from, to, s);
+}
+
 // ------------------------------------------------------------------ host side
 
 template <class T>
@@ -570,6 +583,7 @@ static cudaError_t mdev_alloc(immesh_mesh* h, T** p, size_t count, int memset_by
     cudaError_t e = cudaMalloc(&q, count * sizeof(T));
     if (e != cudaSuccess) return e;
     h->allocs.push_back(q);
+    h->dev_bytes += count * sizeof(T);
     *p = (T*)q;
     if (memset_byte >= 0) e = cudaMemset(q, memset_byte, count * sizeof(T));
     return e;
@@ -904,6 +918,7 @@ static int mesh_status(int err) {
     if (err & IM_MERR_PEER_TIMEOUT) return im_fail(IMMESH_E_CUDA, "sharded mesher: a peer rank did not publish its segment in time (peer window epoch flag)");
     return IMMESH_OK;
 }
+static void mesh_note(immesh_mesh* h, const int* c, int frame);
 // wait for the frame queued in slot s and take over its counters
 static int mesh_harvest(immesh_mesh* h, int s) {
     if (!h->inflight[s]) return IMMESH_OK;
@@ -915,9 +930,210 @@ static int mesh_harvest(immesh_mesh* h, int s) {
     }
     h->inflight[s] = 0;
     std::memcpy(h->last_cnt, h->h_cnt + 32 * s, 32 * sizeof(int));
+    if (h->grow_max_bytes > 0) mesh_note(h, h->last_cnt, h->h_dyn[s].frame);
     const int rc = mesh_status(h->last_cnt[3]);
     if (rc && !h->pending_rc) h->pending_rc = rc;
     return rc;
+}
+
+// ---- growth of the mesh pools.  Device bytes per record: vertex 109 (vpos 16, vsmooth 24, m_smoothed 1, incidence head 4, its
+// share of the vertex chunks 64 at max_v / 4 chunks of 16 float4), plus the xi-grid at 12 B per slot over 2 max_v rounded up to a
+// power of two; triangle 36 (record 16, incidence links 12, flip word 8) plus the triple hash at 4 B per slot over 2 max_t; mesh
+// voxel 88 B per slot (key 8, 16 chunk ids 64, count / meshing_times / new_added / frame 16) over 2 max_voxels.  Ids are 32-bit:
+// every pool stops at 2^30 records.
+#define IM_MPOOL_LIMIT (1LL << 30)
+static size_t mesh_pool_bytes(const immesh_mesh* h, long long v, long long t, long long x) {
+    const size_t gcap = pow2_at_least((size_t)v * 2), tcap = pow2_at_least((size_t)t * 2), vcap = pow2_at_least((size_t)x * 2);
+    const size_t act = std::min<size_t>((size_t)x, (size_t)h->max_frame_points);
+    return (size_t)v * 45 + gcap * 12 + ((size_t)v / 4 + 1024) * 16 * sizeof(float4) + (size_t)t * 36 + tcap * 4 + vcap * (8 + IM_VCHUNKS * 4 + 16) + act * 4;
+}
+// counters of frame number `frame`, finished (see note_counters of the localization handle)
+static void mesh_note(immesh_mesh* h, const int* c, int frame) {
+    if (frame <= h->known_frame) return;
+    h->max_step_tris = std::max(h->max_step_tris, c[1] - h->known[1]);   // over several frames: an upper bound of one
+    std::memcpy(h->known, c, sizeof(h->known));
+    h->known_frame = frame;
+}
+// Enlarge the pools to (vertices, triangles, voxels), each >= the current one: as lio_grow (lio_capi.cu) -- drain, allocate all,
+// migrate on the stream, free the old buffers, drop the captured launch sequence.  The batched frame's scratch (sized by max_voxels
+// and max_triangles) is freed and allocated again at the new sizes by the next batched frame.
+static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long vox) {
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "a sharded mesh handle cannot grow (its replicas would have to grow in lockstep)");
+    if (verts > IM_MPOOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "vertex pool: more than 2^30 vertices (32-bit vertex ids)");
+    if (tris > IM_MPOOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "triangle pool: more than 2^30 triangles (32-bit triangle ids)");
+    if (vox > IM_MPOOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "voxel hash: more than 2^30 mesh voxels (32-bit voxel ids)");
+    MeshDev& M = h->M;
+    const long long v0 = M.max_v, t0 = M.max_t, x0 = h->max_vox;
+    const bool gv = verts > v0, gt = tris > t0, gx = vox > x0;
+    if (!gv && !gt && !gx) return IMMESH_OK;
+    verts = std::max(verts, v0); tris = std::max(tris, t0); vox = std::max(vox, x0);
+    const size_t drop = h->b_fp ? h->b_bytes : 0;   // the batched frame's scratch goes
+    const size_t bytes = h->dev_bytes - drop - mesh_pool_bytes(h, v0, t0, x0) + mesh_pool_bytes(h, verts, tris, vox);
+    if (h->grow_max_bytes > 0 && bytes > (size_t)h->grow_max_bytes) {
+        const std::string pools = std::string(gv ? " vertex pool" : "") + (gt ? " triangle pool" : "") + (gx ? " voxel hash" : "");
+        return im_fail(IMMESH_E_CAPACITY, ("growth of the" + pools + " to " + std::to_string(bytes) + " device bytes is above the ceiling of " +
+                                           std::to_string(h->grow_max_bytes) + " (immesh_mesh_set_growth)").c_str());
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    int c[64];
+    IM_CUDA(cudaMemcpy(c, M.cnt, sizeof(c), cudaMemcpyDeviceToHost));
+    const int nv = std::min(c[0], M.max_v), nt = std::min(c[1], M.max_t), nch = std::min(c[27], M.max_vchunks);
+    MeshDev nm = M;
+    FrameBuf nf = h->F;
+    std::vector<void*> fresh;
+    const char* pool = "";
+    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
+        void* q = nullptr;
+        const cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
+        if (e == cudaSuccess) { fresh.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
+        return e;
+    };
+    const size_t gcap = pow2_at_least((size_t)verts * 2), tcap = pow2_at_least((size_t)tris * 2), vcap = pow2_at_least((size_t)vox * 2);
+    const int vch = (int)(verts / 4 + 1024), act = (int)std::min<long long>(vox, h->max_frame_points);
+    cudaError_t e = cudaSuccess;
+    if (gv) {
+        pool = "vertex pool";
+        if ((e = alloc(&nm.vpos, verts)) == cudaSuccess && (e = alloc(&nm.vsmooth, verts * 3)) == cudaSuccess && (e = alloc(&nm.vsmoothed, verts)) == cudaSuccess &&
+            (e = alloc(&nm.v_tri_head, verts)) == cudaSuccess && (e = alloc(&nm.vchunk_pts, (size_t)vch * 16)) == cudaSuccess && gcap > (size_t)M.gmask + 1 &&
+            (e = alloc(&nm.gkeys, gcap)) == cudaSuccess)
+            e = alloc(&nm.gval, gcap);
+    }
+    if (gt && e == cudaSuccess) {
+        pool = "triangle pool";
+        if ((e = alloc(&nm.tri, tris)) == cudaSuccess && (e = alloc(&nm.tri_next, tris * 3)) == cudaSuccess && (e = alloc(&nm.tri_flip, tris)) == cudaSuccess &&
+            tcap > (size_t)M.tmask + 1)
+            e = alloc(&nm.thash, tcap);
+    }
+    if (gx && e == cudaSuccess) {
+        pool = "voxel hash";
+        if (vcap > (size_t)M.vmask + 1 && (e = alloc(&nm.vkeys, vcap)) == cudaSuccess && (e = alloc(&nm.vox_chunk, vcap * IM_VCHUNKS)) == cudaSuccess &&
+            (e = alloc(&nm.vox_count, vcap)) == cudaSuccess && (e = alloc(&nm.vox_meshing_times, vcap)) == cudaSuccess &&
+            (e = alloc(&nm.vox_new_added, vcap)) == cudaSuccess)
+            e = alloc(&nm.vox_frame, vcap);
+        if (e == cudaSuccess && act > h->F.max_act) e = alloc(&nf.act, act);
+    }
+    auto fail = [&](cudaError_t err, const char* what) {
+        for (void* q : fresh) cudaFree(q);
+        cudaGetLastError();
+        return im_fail(err == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA,
+                       (std::string(what) + ": " + cudaGetErrorString(err) + " during the growth; the handle is unchanged").c_str());
+    };
+    if (e != cudaSuccess) return fail(e, pool);
+    cudaStream_t st = h->stream;
+    const int g = h->n_sm * 16;
+    auto migrate = [&]() -> cudaError_t {
+        cudaError_t r = cudaSuccess;
+#define MG(x) do { if ((r = (x)) != cudaSuccess) return r; } while (0)
+        if (gv) {
+            MG(cudaMemsetAsync(nm.vsmoothed, 0, (size_t)verts, st));
+            MG(cudaMemsetAsync(nm.v_tri_head, 0xFF, (size_t)verts * 4, st));
+            if (nv > 0) {
+                MG(cudaMemcpyAsync(nm.vpos, M.vpos, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+                MG(cudaMemcpyAsync(nm.vsmooth, M.vsmooth, (size_t)nv * 3 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+                MG(cudaMemcpyAsync(nm.vsmoothed, M.vsmoothed, (size_t)nv, cudaMemcpyDeviceToDevice, st));
+                MG(cudaMemcpyAsync(nm.v_tri_head, M.v_tri_head, (size_t)nv * 4, cudaMemcpyDeviceToDevice, st));
+            }
+            if (nch > 0) MG(cudaMemcpyAsync(nm.vchunk_pts, M.vchunk_pts, (size_t)nch * 16 * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+            nm.max_v = (int)verts;
+            nm.max_vchunks = vch;
+            if (nm.gkeys != M.gkeys) {
+                MG(cudaMemsetAsync(nm.gkeys, 0xFF, gcap * 8, st));
+                MG(cudaMemsetAsync(nm.gval, 0xFF, gcap * 4, st));
+                nm.gmask = (unsigned)(gcap - 1);
+                IM_LAUNCH(k_rehash_xi, g, MGROW_THREADS, 0, st, M, nm);
+            }
+        }
+        if (gt) {
+            if (nt > 0) {
+                MG(cudaMemcpyAsync(nm.tri, M.tri, (size_t)nt * sizeof(int4), cudaMemcpyDeviceToDevice, st));
+                MG(cudaMemcpyAsync(nm.tri_next, M.tri_next, (size_t)nt * 3 * sizeof(int), cudaMemcpyDeviceToDevice, st));
+                MG(cudaMemcpyAsync(nm.tri_flip, M.tri_flip, (size_t)nt * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
+            }
+            nm.max_t = (int)tris;
+            if (nm.thash != M.thash) {
+                MG(cudaMemsetAsync(nm.thash, 0xFF, tcap * 4, st));
+                nm.tmask = (unsigned)(tcap - 1);
+                IM_LAUNCH(k_rehash_tris, g, MGROW_THREADS, 0, st, M, nm);
+            }
+        }
+        if (gx && nm.vkeys != M.vkeys) {
+            MG(cudaMemsetAsync(nm.vkeys, 0xFF, vcap * 8, st));
+            MG(cudaMemsetAsync(nm.vox_chunk, 0xFF, vcap * IM_VCHUNKS * 4, st));
+            for (int* q : {nm.vox_count, nm.vox_meshing_times, nm.vox_new_added}) MG(cudaMemsetAsync(q, 0, vcap * 4, st));
+            MG(cudaMemsetAsync(nm.vox_frame, 0xFF, vcap * 4, st));
+            nm.vmask = (unsigned)(vcap - 1);
+            IM_LAUNCH(k_rehash_voxels, g, MGROW_THREADS, 0, st, M, nm);
+        }
+        MG(cudaGetLastError());
+        MG(cudaStreamSynchronize(st));
+#undef MG
+        return r;
+    };
+    e = migrate();
+    if (e != cudaSuccess) return fail(e, "mesh migration");   // the old buffers were only read: the handle is as it was
+    auto swap_buf = [&](void* oldp, void* newp) {
+        if (oldp == newp) return;
+        for (void*& q : h->allocs)
+            if (q == oldp) q = newp;
+        cudaFree(oldp);
+    };
+    swap_buf(M.vpos, nm.vpos); swap_buf(M.vsmooth, nm.vsmooth); swap_buf(M.vsmoothed, nm.vsmoothed); swap_buf(M.v_tri_head, nm.v_tri_head);
+    swap_buf(M.vchunk_pts, nm.vchunk_pts); swap_buf(M.gkeys, nm.gkeys); swap_buf(M.gval, nm.gval);
+    swap_buf(M.tri, nm.tri); swap_buf(M.tri_next, nm.tri_next); swap_buf(M.tri_flip, nm.tri_flip); swap_buf(M.thash, nm.thash);
+    swap_buf(M.vkeys, nm.vkeys); swap_buf(M.vox_chunk, nm.vox_chunk); swap_buf(M.vox_count, nm.vox_count);
+    swap_buf(M.vox_meshing_times, nm.vox_meshing_times); swap_buf(M.vox_new_added, nm.vox_new_added); swap_buf(M.vox_frame, nm.vox_frame);
+    swap_buf(h->F.act, nf.act);
+    if (h->b_fp) {   // batched-frame scratch: allocated again at the new sizes by the next batched frame
+        for (void* q : {(void*)h->b_act, (void*)h->b_sel, (void*)h->b_key, (void*)h->b_ku, (void*)h->b_vu, (void*)h->b_hist, (void*)h->b_rank,
+                        (void*)h->b_mark, (void*)h->b_fset, (void*)h->b_fp}) {
+            h->allocs.erase(std::remove(h->allocs.begin(), h->allocs.end(), q), h->allocs.end());
+            cudaFree(q);
+        }
+        h->b_act = h->b_sel = h->b_rank = h->b_hist = h->b_fset = nullptr;
+        h->b_key = nullptr; h->b_ku = h->b_vu = nullptr; h->b_mark = nullptr; h->b_fp = nullptr;
+        h->b_bytes = 0;
+    }
+    nf.max_act = std::max(h->F.max_act, act);
+    M = nm;
+    h->F.act = nf.act;
+    h->F.max_act = nf.max_act;
+    h->max_vox = (int)vox;
+    h->dev_bytes = bytes;
+    h->growths++;
+    h->graph.destroy();
+    IM_CUDA(cudaGetLastError());
+    return IMMESH_OK;
+}
+// Automatic growth (immesh_mesh_set_growth) before a frame of m candidates: mesh_growth_targets (pool_growth.cuh) on the counters of
+// the last frame known to have finished; the handle is drained only when a pool is short.
+static int mesh_growth_check(immesh_mesh* h, long long m) {
+    if (h->grow_max_bytes <= 0) return IMMESH_OK;
+    long long steps = 1, m_max = m;
+    for (int i = 1; i <= IM_SLOTS; ++i) {   // oldest frame first: consecutive frames give one frame's use each
+        const int s = (h->frame_counter + i) & (IM_SLOTS - 1);
+        if (!h->inflight[s]) continue;
+        if (cudaEventQuery(h->ev_done[s]) == cudaSuccess) {
+            mesh_note(h, h->h_cnt + 32 * s, h->h_dyn[s].frame);
+        } else {
+            ++steps;
+            m_max = std::max<long long>(m_max, h->h_dyn[s].m);
+        }
+    }
+    cudaGetLastError();   // cudaErrorNotReady of the queries
+    for (int pass = 0; pass < 2; ++pass) {
+        long long v = h->M.max_v, t = h->M.max_t, x = h->max_vox;
+        mesh_growth_targets(h->known, steps, m_max, h->max_step_tris, &v, &t, &x);
+        if (v == h->M.max_v && t == h->M.max_t && x == h->max_vox) return IMMESH_OK;
+        if (pass == 1) return mesh_grow(h, v, t, x);
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        for (int i = 1; i <= IM_SLOTS; ++i) {
+            const int s = (h->frame_counter + i) & (IM_SLOTS - 1);
+            if (h->inflight[s]) mesh_note(h, h->h_cnt + 32 * s, h->h_dyn[s].frame);
+        }
+        steps = 1;
+        m_max = m;
+    }
+    return IMMESH_OK;
 }
 
 static bool mesh_host_ptr_is_pinned(const void* p) {
@@ -941,6 +1157,8 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     const MeshParams& P = h->P;
     // append_point_step = max(1, round(N / appending_pts_frame)), integer division first (ImMesh_mesh_reconstruction.cpp:111)
     const int step = std::max(1, (int)std::lround((double)(n / P.append_target)));
+    const int grc = mesh_growth_check(h, n > 0 ? (n + step - 1) / step : 0);
+    if (grc) return grc;
     F.n = n;
     F.step = step;
     F.m = n > 0 ? (n + step - 1) / step : 0;
@@ -1146,6 +1364,7 @@ int immesh_pipeline_mark_end(immesh_lio_t* lio, immesh_mesh_t* h, double* ms) {
 int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique_id128) {
     if (!h || !unique_id128 || nranks < 1 || rank < 0 || rank >= nranks) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (nranks == 1) { h->F.shard_rank = 0; h->F.shard_n = 1; return IMMESH_OK; }
+    if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a mesh handle with automatic growth cannot be sharded (immesh_mesh_set_growth(h, 0) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -1213,6 +1432,35 @@ int immesh_mesh_wait(immesh_mesh_t* h) {
     return mesh_wait_impl(h, false);
 }
 
+int immesh_mesh_capacity(immesh_mesh_t* h, int64_t* out) {
+    if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    int c[32];
+    IM_CUDA(cudaMemcpy(c, h->M.cnt, sizeof(c), cudaMemcpyDeviceToHost));
+    out[0] = h->M.max_v; out[1] = c[0];
+    out[2] = h->M.max_t; out[3] = c[1];
+    out[4] = h->max_vox; out[5] = c[4];
+    out[6] = (int64_t)h->dev_bytes; out[7] = h->growths;
+    return IMMESH_OK;
+}
+int immesh_mesh_reserve(immesh_mesh_t* h, int64_t vertices, int64_t triangles, int64_t voxels) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_mesh_reserve: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
+    const int rc = mesh_grow(h, std::max<long long>(vertices, h->M.max_v), std::max<long long>(triangles, h->M.max_t), std::max<long long>(voxels, h->max_vox));
+    if (rc == IMMESH_OK) return rc;
+    return im_fail(rc, (std::string("immesh_mesh_reserve: ") + immesh::last_error_storage()).c_str());
+}
+int immesh_mesh_set_growth(immesh_mesh_t* h, int64_t max_bytes) {
+    if (!h || max_bytes < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (max_bytes > 0 && h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_mesh_set_growth: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
+    if (max_bytes > 0 && h->grow_max_bytes <= 0) {   // growth starts from the mesh as it is now
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        IM_CUDA(cudaMemcpy(h->known, h->M.cnt, sizeof(h->known), cudaMemcpyDeviceToHost));
+        h->known_frame = h->frame_counter;
+    }
+    h->grow_max_bytes = max_bytes;
+    return IMMESH_OK;
+}
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const int* c = h->last_cnt;
@@ -1585,6 +1833,11 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "push_frame_batched: a sharded handle is not supported");
     const int prev = mesh_wait_impl(h, false);   // frames queued before this one
     if (prev) return prev;
+    {   // growth before the frame only (m candidates at most); an overflow inside it stays IMMESH_E_CAPACITY
+        const int64_t st0 = std::max<int64_t>(1, (int64_t)std::llround((double)(n / (int64_t)h->P.append_target)));
+        const int grc = mesh_growth_check(h, n > 0 ? (n + st0 - 1) / st0 : 0);
+        if (grc) return grc;
+    }
     IM_CUDA(mesh_batched_scratch(h));
     const MeshParams& P = h->P;
     const int B = batch_points ? batch_points : h->max_frame_points, V = batch_voxels ? batch_voxels : h->F.max_work;
@@ -1707,6 +1960,7 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     IM_CUDA(cudaMemcpyAsync(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
     std::memcpy(h->last_cnt, cnt, sizeof(cnt));
+    if (h->grow_max_bytes > 0) mesh_note(h, cnt, F.frame);
     if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->b_bytes; stats[3] = cnt[7]; }
     return mesh_status(cnt[3]);
 }

@@ -454,6 +454,9 @@ IM_HDN inline void cand_commit(const MeshDev& M, const MeshParams& P, const Fram
     im_atomic_add(&M.cnt[10], 1);
 }
 
+// chunk id of a voxel's chunk table entry for the readers: an entry left at -1 by a chunk-pool overflow (the frame fails with
+// VERT_POOL) reads chunk 0 instead of memory before the pool
+IM_HD int im_chunk_or0(int ch) { return ch < 0 ? 0 : ch; }
 // second half of the append: the vertex goes into its voxel's chunk (the chunk table is complete after cand_commit)
 IM_HDN inline void cand_place(const MeshDev& M, const FrameBuf& F, int c, int base) {
     if (F.cand_status[c] != CAND_ACCEPT || F.cand_pos[c] < 0) return;
@@ -461,6 +464,7 @@ IM_HDN inline void cand_place(const MeshDev& M, const FrameBuf& F, int c, int ba
     if (id >= M.max_v) return;
     const int vs = F.cand_vslot[c], pos = F.cand_pos[c];
     const int ch = M.vox_chunk[(size_t)vs * IM_VCHUNKS + (pos >> 4)];
+    if (ch < 0) return;   // the chunk pool overflowed in cand_commit (VERT_POOL raised): nowhere to put the vertex
     const float* p = F.pts + (size_t)c * F.step * 3;
     float4 v;
     v.x = p[0]; v.y = p[1]; v.z = p[2];

@@ -161,7 +161,7 @@ IM_HDN inline void dilate_gather_ring(const MeshDev& M, DilateSmem* S, int kx, i
         if (slot < 0) continue;
         const int o = S->cell_off[c], cntv = S->cell_off[c + 1] - o;
         for (int k = 0; k < cntv; ++k)
-            if (o + k < IM_MAXG) S->cand[o + k] = M.vchunk_pts[(size_t)M.vox_chunk[(size_t)slot * IM_VCHUNKS + (k >> 4)] * 16 + (k & 15)];
+            if (o + k < IM_MAXG) S->cand[o + k] = M.vchunk_pts[(size_t)im_chunk_or0(M.vox_chunk[(size_t)slot * IM_VCHUNKS + (k >> 4)]) * 16 + (k & 15)];
     }
     IM_SYNCBLOCK_M();
 }
@@ -181,7 +181,7 @@ IM_HDN inline void voxel_dilate(const MeshDev& M, const MeshParams& P, const Fra
     if (nqt > IM_VCHUNKS * 16) nqt = IM_VCHUNKS * 16;
     if (nqt > IM_MAXIN) { nqt = IM_MAXIN; if (tid == 0) S->overflow = 1; }
     for (int k = tid; k < nqt; k += nthreads) {
-        const float4 p = M.vchunk_pts[(size_t)M.vox_chunk[(size_t)vs * IM_VCHUNKS + (k >> 4)] * 16 + (k & 15)];
+        const float4 p = M.vchunk_pts[(size_t)im_chunk_or0(M.vox_chunk[(size_t)vs * IM_VCHUNKS + (k >> 4)]) * 16 + (k & 15)];
         S->q[k] = f2i(p.w);
         S->cand[k] = p;
     }

@@ -150,6 +150,24 @@ int immesh_lio_match_nodes(immesh_lio_t* h, int* plane_node /*[n] plane record i
 int64_t immesh_voxelmap_dump(immesh_lio_t* h, double* rows, int64_t cap_rows);
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out /*[4]: roots, nodes, chunks_in_use, error_flags*/);
 
+/* Long runs: the VoxelMap's pools (root hash, node / plane records, 8-point chunks) are sized at create time by
+ * immesh_lio_config; these calls enlarge them on a live handle.  A grown handle computes exactly what a handle created at the
+ * larger capacities computes.  The per-scan buffers (max_scan_points) do not grow.
+ * capacity: out = [root slots, roots, node records, nodes used, chunks, chunks in use, device bytes of the handle, growths so far].
+ *   Blocking: waits for the work queued on h.
+ * reserve: grow to at least these capacities (<= 0 or below the current one: keep; root slots are rounded up to a power of two).
+ *   Never shrinks.  Blocking: drains the steps queued on h first.  Fails with IMMESH_E_CAPACITY (beyond 2^30 records of a pool --
+ *   the ids are 32-bit --, above the set_growth ceiling, or out of device memory) or IMMESH_E_CUDA, immesh_last_error() naming the
+ *   pool; the handle is then exactly as before.  A sharded handle: IMMESH_E_INVALID.
+ * set_growth: max_bytes > 0 turns on automatic growth -- before every step (immesh_voxelmap_build / _update, the *_pv inserts,
+ *   immesh_lio_step*, immesh_lio_step_async*) the pools are checked against the use of the last finished step and doubled while
+ *   their headroom is short (INTEGRATION.md, "Long runs"); max_bytes is a ceiling on the handle's device bytes.  0: off (the
+ *   default); a step then does nothing it did not do before.  A step that overflows anyway returns IMMESH_E_CAPACITY as without
+ *   growth. */
+int immesh_lio_capacity(immesh_lio_t* h, int64_t* out /*[8]*/);
+int immesh_lio_reserve(immesh_lio_t* h, int64_t root_slots, int64_t nodes, int64_t chunks);
+int immesh_lio_set_growth(immesh_lio_t* h, int64_t max_bytes);
+
 /* pubPlaneMap(m_feat_map, voxel_pub, state.pos_end) (src/voxel_mapping.cpp:947-1159), called after voxel_map_init and after every
  * map_incremental_grow (:1899-1900, :1975-1976): the markers of the planes refitted since the last call, one row per pubPlane call
  * (:919-945), with the reference's walk -- a root whose m_is_update flag is set is published and its children wait for a later
@@ -244,6 +262,15 @@ int immesh_pipeline_mark_begin(immesh_lio_t* lio);
 int immesh_pipeline_mark_end(immesh_lio_t* lio, immesh_mesh_t* h, double* ms);
 /* counts: [n_vertices, n_live_triangles, frame_new_vertices, frame_voxels_meshed, frame_added, frame_removed, n_voxels, n_activated] */
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out /*[8]*/);
+/* Long runs: the same three calls as immesh_lio_capacity / _reserve / _set_growth for the mesh handle's pools -- vertices (with the
+ * xi-grid and the vertex chunks), triangles (with the triple hash) and mesh voxels (max_voxels, with the voxel hash).  capacity:
+ * out = [vertex capacity, vertices, triangle capacity, triangles allocated, voxel capacity, voxels, device bytes, growths].  The
+ * automatic check runs before every immesh_mesh_push_frame* call and before a batched frame (not inside one).  The per-frame capacities
+ * (max_frame_points and the frame's work and list capacities) do not grow.  A grown handle computes what a handle created at the
+ * larger capacities computes. */
+int immesh_mesh_capacity(immesh_mesh_t* h, int64_t* out /*[8]*/);
+int immesh_mesh_reserve(immesh_mesh_t* h, int64_t vertices, int64_t triangles, int64_t voxels);
+int immesh_mesh_set_growth(immesh_mesh_t* h, int64_t max_bytes);
 /* Triangle_manager::get_all_triangle_list (src/meshing/r3live/triangle.cpp:12-33) + the vertex array:
  * live triangles as ascending sorted (i<j<k) id triples with their m_index_flip. */
 int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices /*[nv][3] or NULL*/, int32_t* triangles /*[nt][3] or NULL*/,
