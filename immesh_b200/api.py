@@ -170,6 +170,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_imu_undistort", [vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_double, vp]),
         ("immesh_imu_device_points", [vp]),
         ("immesh_imu_get_poses", [vp, dp, C.c_int]),
+        ("immesh_imu_init_begin", [vp, C.c_int]),
+        ("immesh_lio_step_async_imu", [vp, vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, ip]),
     ):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
@@ -723,6 +725,23 @@ class VoxelGrid:
                                                             dt, cov_gyr, cov_acc), "lio_step_async_raw")
         lio._last_n = cnt
 
+    def step_async_imu(self, lio: "Lio", imu_h: "Imu", batch, pts, lidar_beg_time: float, leaf: float, calib_laser=False, n=None, on_device=False) -> int:
+        """The IMU-enabled scan loop, one queued call per scan (immesh_lio_step_async_imu): batch float64[n_imu,7] (stamp, gyr, acc);
+        pts float32[n,4] (x, y, z, curvature ms) host array, or an integer CUDA address with n when on_device.  Returns the branch taken:
+        1 initialising, 2 map built, 3 localised and grown (then hand the frame to the mesher: input_points(), n, on_device)."""
+        im = np.ascontiguousarray(batch, dtype=np.float64).reshape(-1, 7)
+        if on_device:
+            ptr, cnt = C.c_void_p(int(pts)), int(n)
+        else:
+            a = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 4)
+            ptr, cnt = a.ctypes.data_as(C.c_void_p), a.shape[0]
+        br = C.c_int(0)
+        _check(self.lib, self.lib.immesh_lio_step_async_imu(lio._h, imu_h._h, self._h, im.ctypes.data_as(C.POINTER(C.c_double)), im.shape[0], ptr, cnt,
+                                                            1 if on_device else 0, lidar_beg_time, 1 if calib_laser else 0, C.c_float(leaf), C.byref(br)),
+               "lio_step_async_imu")
+        lio._last_n = cnt
+        return br.value
+
 
 class Imu:
     """ImuProcess::UndistortPcl on the device (immesh_imu_*): forward propagation of the localization handle's state over the IMU
@@ -758,6 +777,10 @@ class Imu:
         dp = C.POINTER(C.c_double)
         f = lambda v: None if v is None else np.ascontiguousarray(v, dtype=np.float64).ctypes.data_as(dp)  # noqa: E731
         _check(self.lib, self.lib.immesh_imu_reset(self._h, a.ctypes.data_as(dp), last_lidar_end_time, last_update_time, f(acc_s_last), f(angvel_last)), "imu_reset")
+
+    def init_begin(self, max_ini_count: int = 3):
+        """Enter the IMU initialisation phase of step_async_imu (first call: a fresh ImuProcess; later calls: the loop's reset)."""
+        _check(self.lib, self.lib.immesh_imu_init_begin(self._h, max_ini_count), "imu_init_begin")
 
     def undistort(self, lio: "Lio", imu, pts_xyzt, lidar_beg_time):
         """imu: float64[n_imu,7] (stamp, gyr, acc); pts_xyzt: float32[n,4] (x, y, z, curvature ms).  Returns the time-sorted, compensated cloud."""

@@ -139,6 +139,14 @@ def build_growth(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "growth", "emu_growth.cpp"), EMU_GROWTH, force)
 
 
+EMU_IMU_CHAIN = os.path.join(_ROOT, "tests", "imu_chain", "libimmesh_emu_imu_chain.so")
+
+
+def build_imu_chain(force=False):
+    """tests/imu_chain: the device interval plan and IMU_init's host body of the IMU-enabled scan loop, built for the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "imu_chain", "emu_imu_chain.cpp"), EMU_IMU_CHAIN, force)
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -156,6 +164,7 @@ def build_all(force=False):
     build_regionbuf(force)
     build_batched(force)
     build_growth(force)
+    build_imu_chain(force)
     build_ref()
 
 

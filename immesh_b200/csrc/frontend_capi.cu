@@ -425,4 +425,16 @@ int immesh_lio_step_async_raw(immesh_lio_t* lio, immesh_voxelgrid_t* h, const fl
 
 const float* immesh_voxelgrid_device_points(immesh_voxelgrid_t* h) { return h ? h->d_out : nullptr; }
 
+// internal (immesh_lio_step_async_imu): capacity of the handle, and voxel_map_init queued on the localization stream from a device
+// cloud -- [calibration] + repack into the input ring (immesh_voxelgrid_input_points), then the build kernels on the packed full scan
+int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h) { return h ? h->max_points : 0; }
+int immesh_voxelmap_build_async_dev(immesh_lio_t* lio, const float* d_body_xyz, int n);   // lio_capi.cu
+int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser) {
+    if (!lio || !h || !d_pts || n < 1 || (stride != 3 && stride != 4)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
+    const int rc = frontend_pack(h, d_pts, n, stride, 1, calib_laser, lio->stream);
+    if (rc) return rc;
+    return immesh_voxelmap_build_async_dev(lio, h->d_in, n);
+}
+
 }  // extern "C"

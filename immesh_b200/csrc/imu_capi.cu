@@ -1,8 +1,11 @@
 // immesh_b200 -- IMU step in front of the hot path (SURVEY 8f-2) on the device: ImuProcess::UndistortPcl
-// (/root/reference/src/IMU_Processing.cpp:755-958), LiDAR-only flow.  The state and its covariance stay in the localization
-// handle's HBM (LioCtrl::state); nothing but time stamps is decided on the host.
-//   k_imu_begin     running quantities (vel, pos, R) <- state, IMUpose[0]
-//   k_imu_forward   one block: all live IMU intervals in sequence (18x18 F P F^T + Q each), scan-end prediction
+// (/root/reference/src/IMU_Processing.cpp:755-958), and the IMU-enabled scan loop of Voxel_mapping::service_LiDAR_update
+// (ImuProcess::Process2 :960-1006 + src/voxel_mapping.cpp:1820-1905) as one queued call per scan.  The state and its covariance
+// stay in the localization handle's HBM (LioCtrl::state), the time stamps the scans carry over in ImuTime; the host decides
+// nothing from device data.
+//   k_imu_forward   one block: thread 0 seeds the running quantities from the state (IMUpose[0]) and works out the interval plan
+//                   (imu_plan) from the staged samples; then all live IMU intervals in sequence (18x18 F P F^T + Q each) and the
+//                   scan-end prediction
 //   k_imu_keys      time-stamp keys (ordered-uint image of the float curvature) for the stable radix sort (radix_sort.cuh)
 //   k_imu_gather    points in time order
 //   k_imu_undistort thread per point: interval lookup + rigid transform into the scan-end frame (16 B in, 16 B out per point)
@@ -10,16 +13,17 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
-#include <vector>
 
 #include "../../include/immesh_b200.h"
 #include "common_host.hpp"
 #include "handles.hpp"
 #include "imu_core.cuh"
 
-using immesh::im_fail; using immesh::ImuParams; using immesh::ImuStep;
+using immesh::im_fail; using immesh::ImuParams; using immesh::ImuStep; using immesh::ImuTime; using immesh::ImuInit;
 
 namespace {
 
@@ -27,19 +31,24 @@ namespace {
 
 #define IMU_FWD_THREADS 352
 
-__global__ void k_imu_begin(const LioCtrl* ctrl, double* run, double* poses) {
+// pts: the scan as given (unsorted), read for its last point's stamp only
+__global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward(ImuParams P, LioCtrl* ctrl, double* run, ImuTime* tm, const double* imu, int n_imu, const float* pts, int n,
+                                                                  double lidar_beg_time, ImuStep* steps, double* poses) {
+    __shared__ double Fx[324], T[324];
+    __shared__ double s_note, s_dt;
+    __shared__ int s_steps;
     if (threadIdx.x == 0) {
         const double* st = ctrl->state;
         for (int i = 0; i < 3; ++i) { run[6 + i] = st[12 + i]; run[9 + i] = st[9 + i]; }
         for (int i = 0; i < 9; ++i) run[12 + i] = st[i];
         immesh::imu_write_pose(poses, 0.0, run);   // IMUpose[0] = (0, acc_s_last, angvel_last, vel_end, pos_end, rot_end), :800
+        s_steps = immesh::imu_plan(*tm, imu, n_imu, pts[4 * (size_t)(n - 1) + 3], lidar_beg_time, steps, &s_note, &s_dt);
     }
-}
-__global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward(ImuParams P, LioCtrl* ctrl, double* run, const ImuStep* steps, int n_steps, double* poses, double note, double dt_end) {
-    __shared__ double Fx[324], T[324];
+    __syncthreads();
+    const int n_steps = s_steps;
     for (int k = 0; k < n_steps; ++k)
         immesh::imu_forward_step(P, ctrl->state, run, steps[k], poses + (size_t)(k + 1) * IM_POSE_DOUBLES, Fx, T, threadIdx.x, blockDim.x);
-    if (threadIdx.x == 0) immesh::imu_predict_end(ctrl->state, run, note, dt_end);
+    if (threadIdx.x == 0) immesh::imu_predict_end(ctrl->state, run, s_note, s_dt);
 }
 __global__ void __launch_bounds__(VG_THREADS) k_imu_keys(const float* __restrict__ pts, int n, unsigned int* keys, unsigned int* vals) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -52,9 +61,11 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_keys(const float* __restrict
 __global__ void __launch_bounds__(VG_THREADS) k_imu_gather(const float4* __restrict__ in, const unsigned int* __restrict__ vals, int n, float4* out) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[vals[i]];
 }
-__global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const LioCtrl* ctrl, const double* __restrict__ poses, int n_pose, float* pts, int n) {
+// the IMUpose count comes from the plan (ImuTime::n_pose); the dynamic shared memory is sized for the batch's upper bound
+__global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm, float* pts, int n) {
     extern __shared__ double s_pose[];
     __shared__ double s_end[12];
+    const int n_pose = tm->n_pose;
     for (int i = threadIdx.x; i < n_pose * IM_POSE_DOUBLES; i += blockDim.x) s_pose[i] = poses[i];
     if (threadIdx.x < 12) s_end[threadIdx.x] = ctrl->state[threadIdx.x];
     __syncthreads();
@@ -66,21 +77,89 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const
 struct immesh_imu {
     ImuParams P;
     int max_points = 0, max_imu = 0, nblocks_max = 0, n_sm = 132;
-    // ImuProcess members that live on the host (time stamps) ...
-    double last_imu[7] = {0, 0, 0, 0, 0, 0, 0};
-    double last_lidar_end_time = -1.0, last_update_time = 0.0;
-    // ... and on the device: run = [acc_s_last 3 | angvel_last 3 | vel 3 | pos 3 | R 9]
+    // ImuProcess members on the device: ImuTime (time stamps) and run = [acc_s_last 3 | angvel_last 3 | vel 3 | pos 3 | R 9]
+    ImuTime* d_time = nullptr;
     double* d_run = nullptr;
     double* d_poses = nullptr;      // [max_imu + 2][22]
-    ImuStep* d_steps = nullptr;
-    ImuStep* h_steps = nullptr;     // pinned
-    float* d_in = nullptr;          // [max_points][4] staging of host input
+    ImuStep* d_steps = nullptr;     // [max_imu] the plan of the last scan
+    double* d_imu = nullptr;        // [max_imu][7] the scan's IMU batch
+    float* d_in = nullptr;          // [max_points][4] the scan, when given in host memory
     float* d_out = nullptr;         // [max_points][4] time-sorted, compensated
     unsigned int *d_k[2] = {nullptr, nullptr}, *d_v[2] = {nullptr, nullptr};
     int* d_hist = nullptr;
-    float* h_pts = nullptr;         // pinned
-    int last_n = 0, last_poses = 0;
+    // pinned staging ring, IM_SLOTS deep: slot s holds a scan's IMU batch and the host words of its copies (h_imu) and a host scan
+    // (h_pts); it is reused only after the event recorded behind its copies (ev_stage)
+    double* h_imu = nullptr;
+    float* h_pts = nullptr;
+    size_t slot_doubles = 0;
+    cudaEvent_t ev_stage[IM_SLOTS] = {};
+    int stage_busy[IM_SLOTS] = {};
+    int stage_idx = 0;
+    // initialisation phase of immesh_lio_step_async_imu (imu_need_init_ ... MAX_INI_COUNT)
+    ImuInit ini = {{0, 0, -1.0}, {0, 0, 0}, 1, 1};
+    int init_phase = 0;     // imu_need_init_ (only after immesh_imu_init_begin)
+    int max_ini = 3;        // MAX_INI_COUNT (mapping/imu_int_frame)
+    int began = 0;          // immesh_imu_init_begin has been called on the handle
+    int pending_reset = 0;  // device members still to be reset in stream order: 1 Reset(), 2 a fresh ImuProcess
+    int map_built = 0;      // m_init_map: the chain has built the VoxelMap
 };
+
+// internal entry points of frontend_capi.cu / lio_capi.cu
+extern "C" int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h);
+extern "C" int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser);
+
+// the next staging slot; blocks (back-pressure, counted in the localization handle's host wait) while its last copies are in flight
+static int imu_stage_slot(immesh_imu* h, immesh_lio* lio) {
+    const int s = (++h->stage_idx) & (IM_SLOTS - 1);
+    if (h->stage_busy[s]) {
+        const auto t0 = std::chrono::steady_clock::now();
+        IM_CUDA(cudaEventSynchronize(h->ev_stage[s]));
+        lio->host_wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        h->stage_busy[s] = 0;
+    }
+    return s;
+}
+static int imu_stage_release(immesh_imu* h, int s, cudaStream_t st) {
+    IM_CUDA(cudaEventRecord(h->ev_stage[s], st));
+    h->stage_busy[s] = 1;
+    return IMMESH_OK;
+}
+
+// UndistortPcl queued on the localization stream through staging slot s: batch (+ host scan) upload, plan + forward propagation,
+// stable time sort, compensation into d_out.  No host synchronisation.
+static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device, double lidar_beg_time, int s) {
+    cudaStream_t st = lio->stream;
+    if (n_imu > 0) {
+        double* hi = h->h_imu + (size_t)s * h->slot_doubles;
+        std::memcpy(hi, imu, (size_t)n_imu * 7 * sizeof(double));
+        IM_CUDA(cudaMemcpyAsync(h->d_imu, hi, (size_t)n_imu * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    const float* d_pts = pts_xyzt;
+    if (!on_device) {
+        float* hp = h->h_pts + (size_t)s * h->max_points * 4;
+        std::memcpy(hp, pts_xyzt, (size_t)n * 4 * sizeof(float));
+        IM_CUDA(cudaMemcpyAsync(h->d_in, hp, (size_t)n * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
+        d_pts = h->d_in;
+    }
+    IM_LAUNCH(k_imu_forward, 1, IMU_FWD_THREADS, 0, st, h->P, lio->d_ctrl, h->d_run, h->d_time, (const double*)h->d_imu, n_imu, d_pts, n, lidar_beg_time, h->d_steps, h->d_poses);
+    const int nb = (n + VG_TILE - 1) / VG_TILE;
+    const int gs = std::min(nb * (VG_TILE / VG_THREADS), h->n_sm * 8);
+    IM_LAUNCH(k_imu_keys, gs, VG_THREADS, 0, st, d_pts, n, h->d_k[0], h->d_v[0]);
+    int cur = 0;
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 8 * pass;
+        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, shift, h->d_hist, nb);
+        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_hist, 256 * nb, (int*)nullptr);
+        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], h->d_k[cur ^ 1], h->d_v[cur ^ 1], n, shift,
+                  (const int*)h->d_hist, nb);
+        cur ^= 1;
+    }
+    IM_LAUNCH(k_imu_gather, gs, VG_THREADS, 0, st, (const float4*)d_pts, (const unsigned int*)h->d_v[cur], n, (float4*)h->d_out);
+    const size_t smem = (size_t)(n_imu + 1) * IM_POSE_DOUBLES * sizeof(double);   // IMUpose holds at most n_imu + 1 entries
+    IM_LAUNCH(k_imu_undistort, gs, VG_THREADS, smem, st, h->P, (const LioCtrl*)lio->d_ctrl, (const double*)h->d_poses, (const ImuTime*)h->d_time, h->d_out, n);
+    IM_CUDA(cudaGetLastError());
+    return IMMESH_OK;
+}
 
 extern "C" {
 
@@ -98,11 +177,18 @@ int immesh_imu_create(const immesh_imu_config* c, immesh_imu_t** out) {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
     const size_t n = (size_t)c->max_points;
+    // the time stamps a handle starts from (immesh_imu_reset sets them; a fresh ImuProcess is immesh_imu_init_begin's)
+    ImuTime t0;
+    std::memset(&t0, 0, sizeof(t0));
+    t0.last_lidar_end_time = -1.0;
+    t0.n_pose = 1;
+    IM_CUDA(cudaMalloc((void**)&h->d_time, sizeof(ImuTime)));
+    IM_CUDA(cudaMemcpy(h->d_time, &t0, sizeof(ImuTime), cudaMemcpyHostToDevice));
     IM_CUDA(cudaMalloc((void**)&h->d_run, IM_IMU_RUN * sizeof(double)));
     IM_CUDA(cudaMemset(h->d_run, 0, IM_IMU_RUN * sizeof(double)));
     IM_CUDA(cudaMalloc((void**)&h->d_poses, ((size_t)c->max_imu + 2) * IM_POSE_DOUBLES * sizeof(double)));
     IM_CUDA(cudaMalloc((void**)&h->d_steps, ((size_t)c->max_imu + 1) * sizeof(ImuStep)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_steps, ((size_t)c->max_imu + 1) * sizeof(ImuStep)));
+    IM_CUDA(cudaMalloc((void**)&h->d_imu, (size_t)c->max_imu * 7 * sizeof(double)));
     IM_CUDA(cudaMalloc((void**)&h->d_in, n * 4 * sizeof(float)));
     IM_CUDA(cudaMalloc((void**)&h->d_out, n * 4 * sizeof(float)));
     for (int i = 0; i < 2; ++i) {
@@ -110,27 +196,36 @@ int immesh_imu_create(const immesh_imu_config* c, immesh_imu_t** out) {
         IM_CUDA(cudaMalloc((void**)&h->d_v[i], n * sizeof(unsigned int)));
     }
     IM_CUDA(cudaMalloc((void**)&h->d_hist, (size_t)256 * h->nblocks_max * sizeof(int)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_pts, n * 4 * sizeof(float)));
+    h->slot_doubles = (size_t)c->max_imu * 7 + 32;   // the batch + the host words of an initialising scan
+    IM_CUDA(cudaMallocHost((void**)&h->h_imu, IM_SLOTS * h->slot_doubles * sizeof(double)));
+    IM_CUDA(cudaMallocHost((void**)&h->h_pts, IM_SLOTS * n * 4 * sizeof(float)));
+    for (int i = 0; i < IM_SLOTS; ++i) IM_CUDA(cudaEventCreateWithFlags(&h->ev_stage[i], cudaEventDisableTiming));
     *out = h;
     return IMMESH_OK;
 }
 int immesh_imu_destroy(immesh_imu_t* h) {
     if (!h) return IMMESH_OK;
     cudaDeviceSynchronize();
-    cudaFree(h->d_run); cudaFree(h->d_poses); cudaFree(h->d_steps); cudaFreeHost(h->h_steps); cudaFree(h->d_in); cudaFree(h->d_out);
+    cudaFree(h->d_time); cudaFree(h->d_run); cudaFree(h->d_poses); cudaFree(h->d_steps); cudaFree(h->d_imu); cudaFree(h->d_in); cudaFree(h->d_out);
     for (int i = 0; i < 2; ++i) { cudaFree(h->d_k[i]); cudaFree(h->d_v[i]); }
-    cudaFree(h->d_hist); cudaFreeHost(h->h_pts);
+    cudaFree(h->d_hist); cudaFreeHost(h->h_imu); cudaFreeHost(h->h_pts);
+    for (int i = 0; i < IM_SLOTS; ++i) if (h->ev_stage[i]) cudaEventDestroy(h->ev_stage[i]);
     delete h;
     return IMMESH_OK;
 }
 int immesh_imu_reset(immesh_imu_t* h, const double* last_imu7, double last_lidar_end_time, double last_update_time, const double* acc_s_last, const double* angvel_last) {
     if (!h || !last_imu7) return im_fail(IMMESH_E_INVALID, "null argument");
-    std::memcpy(h->last_imu, last_imu7, 7 * sizeof(double));
-    h->last_lidar_end_time = last_lidar_end_time;
-    h->last_update_time = last_update_time;
+    ImuTime t;
+    std::memset(&t, 0, sizeof(t));
+    std::memcpy(t.last_imu, last_imu7, 7 * sizeof(double));
+    t.last_lidar_end_time = last_lidar_end_time;
+    t.upd_beg = last_update_time;   // + 0.0f / 1000: exactly last_update_time
+    t.n_pose = 1;
     double run6[6] = {0, 0, 0, 0, 0, 0};
     if (acc_s_last) std::memcpy(run6, acc_s_last, 24);
     if (angvel_last) std::memcpy(run6 + 3, angvel_last, 24);
+    IM_CUDA(cudaDeviceSynchronize());   // nothing queued earlier still reads the members
+    IM_CUDA(cudaMemcpy(h->d_time, &t, sizeof(t), cudaMemcpyHostToDevice));
     IM_CUDA(cudaMemcpy(h->d_run, run6, sizeof(run6), cudaMemcpyHostToDevice));
     return IMMESH_OK;
 }
@@ -138,73 +233,119 @@ int immesh_imu_reset(immesh_imu_t* h, const double* last_imu7, double last_lidar
 int immesh_imu_undistort(immesh_imu_t* h, immesh_lio_t* lio, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device, double lidar_beg_time, float* out_xyzt) {
     if (!h || !lio || (!imu && n_imu > 0) || n_imu < 0 || (!pts_xyzt && n > 0) || n < 1) return im_fail(IMMESH_E_INVALID, "bad argument (the scan must hold at least one point)");
     if (n > h->max_points || n_imu > h->max_imu) return im_fail(IMMESH_E_CAPACITY, "scan / IMU batch larger than the configured capacity");
-    cudaStream_t st = lio->stream;
-    // ---- host: time stamps only (v_imu = last_imu_ + meas.imu, :759-764)
-    std::vector<const double*> v;
-    v.push_back(h->last_imu);
-    for (int i = 0; i < n_imu; ++i) v.push_back(imu + 7 * (size_t)i);
-    const double imu_end_time = v.back()[0];
-    const double pcl_beg_time = std::max(lidar_beg_time, h->last_update_time);
-    float last_curv = 0.f;
-    if (on_device) IM_CUDA(cudaMemcpy(&last_curv, pts_xyzt + 4 * (size_t)(n - 1) + 3, sizeof(float), cudaMemcpyDeviceToHost));
-    else last_curv = pts_xyzt[4 * (size_t)(n - 1) + 3];
-    const double pcl_end_time = lidar_beg_time + (double)last_curv / double(1000);
-    h->last_update_time = pcl_end_time;
-    int n_steps = 0;
-    for (size_t k = 0; k + 1 < v.size(); ++k) {
-        const double *head = v[k], *tail = v[k + 1];
-        if (tail[0] < h->last_lidar_end_time) continue;
-        ImuStep& s = h->h_steps[n_steps++];
-        for (int i = 0; i < 3; ++i) { s.gyr_avg[i] = 0.5 * (head[1 + i] + tail[1 + i]); s.acc_avg[i] = 0.5 * (head[4 + i] + tail[4 + i]); }
-        s.dt = (head[0] < h->last_lidar_end_time) ? tail[0] - h->last_lidar_end_time : tail[0] - head[0];
-        s.offs_t = tail[0] - pcl_beg_time;
-    }
-    double note, dt_end;
-    if (imu_end_time > pcl_beg_time) { note = pcl_end_time > imu_end_time ? 1.0 : -1.0; dt_end = note * (pcl_end_time - imu_end_time); }
-    else { note = pcl_end_time > pcl_beg_time ? 1.0 : -1.0; dt_end = note * (pcl_end_time - pcl_beg_time); }
-    std::memcpy(h->last_imu, v.back(), 7 * sizeof(double));
-    h->last_lidar_end_time = pcl_end_time;
-    // ---- device
-    const float* d_pts = pts_xyzt;
-    if (!on_device) {
-        std::memcpy(h->h_pts, pts_xyzt, (size_t)n * 4 * sizeof(float));
-        IM_CUDA(cudaMemcpyAsync(h->d_in, h->h_pts, (size_t)n * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
-        d_pts = h->d_in;
-    }
-    if (n_steps > 0) IM_CUDA(cudaMemcpyAsync(h->d_steps, h->h_steps, (size_t)n_steps * sizeof(ImuStep), cudaMemcpyHostToDevice, st));
-    IM_LAUNCH(k_imu_begin, 1, 32, 0, st, (const LioCtrl*)lio->d_ctrl, h->d_run, h->d_poses);
-    IM_LAUNCH(k_imu_forward, 1, IMU_FWD_THREADS, 0, st, h->P, lio->d_ctrl, h->d_run, (const ImuStep*)h->d_steps, n_steps, h->d_poses, note, dt_end);
-    const int nb = (n + VG_TILE - 1) / VG_TILE;
-    const int gs = std::min(nb * (VG_TILE / VG_THREADS), h->n_sm * 8);
-    IM_LAUNCH(k_imu_keys, gs, VG_THREADS, 0, st, d_pts, n, h->d_k[0], h->d_v[0]);
-    int cur = 0;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 8 * pass;
-        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, shift, h->d_hist, nb);
-        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_hist, 256 * nb, (int*)nullptr);
-        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], h->d_k[cur ^ 1], h->d_v[cur ^ 1], n, shift,
-                  (const int*)h->d_hist, nb);
-        cur ^= 1;
-    }
-    IM_LAUNCH(k_imu_gather, gs, VG_THREADS, 0, st, (const float4*)d_pts, (const unsigned int*)h->d_v[cur], n, (float4*)h->d_out);
-    const int n_pose = n_steps + 1;
-    IM_LAUNCH(k_imu_undistort, gs, VG_THREADS, (size_t)n_pose * IM_POSE_DOUBLES * sizeof(double), st, h->P, (const LioCtrl*)lio->d_ctrl, (const double*)h->d_poses, n_pose, h->d_out, n);
-    IM_CUDA(cudaGetLastError());
-    h->last_n = n; h->last_poses = n_pose;
+    const int s = imu_stage_slot(h, lio);
+    int rc = imu_enqueue_undistort(h, lio, imu, n_imu, pts_xyzt, n, on_device, lidar_beg_time, s);
+    if (rc) return rc;
+    rc = imu_stage_release(h, s, lio->stream);
+    if (rc) return rc;
+    lio->pose_pub_idx = -1;   // the state moved
     if (out_xyzt) {
-        IM_CUDA(cudaMemcpyAsync(h->h_pts, h->d_out, (size_t)n * 4 * sizeof(float), cudaMemcpyDeviceToHost, st));
-        IM_CUDA(cudaStreamSynchronize(st));
-        std::memcpy(out_xyzt, h->h_pts, (size_t)n * 4 * sizeof(float));
+        float* hp = h->h_pts + (size_t)s * h->max_points * 4;
+        IM_CUDA(cudaMemcpyAsync(hp, h->d_out, (size_t)n * 4 * sizeof(float), cudaMemcpyDeviceToHost, lio->stream));
+        IM_CUDA(cudaStreamSynchronize(lio->stream));
+        std::memcpy(out_xyzt, hp, (size_t)n * 4 * sizeof(float));
     }
     return IMMESH_OK;
 }
 const float* immesh_imu_device_points(immesh_imu_t* h) { return h ? h->d_out : nullptr; }
 int immesh_imu_get_poses(immesh_imu_t* h, double* out, int cap_poses) {   // IMUpose of the last call, 22 doubles each; returns their number
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
-    const int m = std::min(cap_poses, h->last_poses);
     IM_CUDA(cudaDeviceSynchronize());
-    IM_CUDA(cudaMemcpy(out, h->d_poses, (size_t)m * IM_POSE_DOUBLES * sizeof(double), cudaMemcpyDeviceToHost));
-    return h->last_poses;
+    int n_pose = 0;
+    IM_CUDA(cudaMemcpy(&n_pose, &h->d_time->n_pose, sizeof(int), cudaMemcpyDeviceToHost));
+    const int m = std::min(cap_poses, n_pose);
+    if (m > 0) IM_CUDA(cudaMemcpy(out, h->d_poses, (size_t)m * IM_POSE_DOUBLES * sizeof(double), cudaMemcpyDeviceToHost));
+    return n_pose;
+}
+
+int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count) {
+    if (!h || max_ini_count < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    h->init_phase = 1;
+    h->max_ini = max_ini_count;
+    immesh::imu_init_reset(h->ini);
+    if (!h->began) {   // a fresh ImuProcess: b_first_frame_, zero members
+        h->began = 1;
+        h->ini.first_frame = 1;
+        h->pending_reset = 2;
+    } else {           // the loop's reset (m_flg_reset -> Reset()): b_first_frame_ stays false
+        h->pending_reset = std::max(h->pending_reset, 1);
+    }
+    return IMMESH_OK;
+}
+
+int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device,
+                              double lidar_beg_time, int calib_laser, float leaf, int* branch_out) {
+    if (branch_out) *branch_out = 0;
+    if (!lio || !h || !vg || (!imu && n_imu > 0) || n_imu < 0 || !pts_xyzt || n < 1 || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument (the scan must hold at least one point)");
+    if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_imu runs on a single GPU: the localization handle is sharded");
+    if (n_imu > h->max_imu) return im_fail(IMMESH_E_CAPACITY, "IMU batch larger than the IMU handle's max_imu");
+    if (n > h->max_points || n > immesh_voxelgrid_max_points(vg)) return im_fail(IMMESH_E_CAPACITY, "scan larger than the IMU / VoxelGrid handle's max_points");
+    if (n > lio->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than the localization handle's max_scan_points (the map is built from the whole scan, and a scan the VoxelGrid passes through reaches the step whole)");
+    cudaStream_t st = lio->stream;
+    if (h->pending_reset) {
+        if (h->pending_reset == 2) {   // a fresh ImuProcess (last_lidar_end_time_ = 0.0, see the header)
+            IM_CUDA(cudaMemsetAsync(h->d_time, 0, sizeof(ImuTime), st));
+            IM_CUDA(cudaMemsetAsync(h->d_run, 0, 6 * sizeof(double), st));
+        } else {                       // Reset(): last_imu_ and angvel_last; acc_s_last and last_lidar_end_time_ are kept
+            IM_CUDA(cudaMemsetAsync(h->d_time->last_imu, 0, 7 * sizeof(double), st));
+            IM_CUDA(cudaMemsetAsync(h->d_run + 3, 0, 3 * sizeof(double), st));
+        }
+        h->pending_reset = 0;
+    }
+    const int s = imu_stage_slot(h, lio);
+    if (h->init_phase) {
+        // branch 1 (Process2 :973-1003): lidar_meas.last_update_time = pcl_end_time; IMU_init on a non-empty batch
+        double* hw = h->h_imu + (size_t)s * h->slot_doubles + (size_t)h->max_imu * 7;   // host words: [upd_beg, curv | rot 9, bg 3, grav 3 | last_imu 7]
+        hw[0] = lidar_beg_time;
+        IM_CUDA(cudaMemcpyAsync((char*)h->d_time + offsetof(ImuTime, upd_beg), hw, sizeof(double), cudaMemcpyHostToDevice, st));
+        float* curv_dst = (float*)((char*)h->d_time + offsetof(ImuTime, upd_curv));
+        if (on_device) {
+            IM_CUDA(cudaMemcpyAsync(curv_dst, pts_xyzt + 4 * (size_t)(n - 1) + 3, sizeof(float), cudaMemcpyDeviceToDevice, st));
+        } else {
+            std::memcpy(hw + 1, pts_xyzt + 4 * (size_t)(n - 1) + 3, sizeof(float));
+            IM_CUDA(cudaMemcpyAsync(curv_dst, hw + 1, sizeof(float), cudaMemcpyHostToDevice, st));
+        }
+        if (n_imu > 0) {
+            double* sw = hw + 2;
+            double grav[3];
+            const double norm = immesh::imu_init_batch(h->ini, imu, n_imu, grav);
+            for (int i = 0; i < 9; ++i) sw[i] = (i % 4 == 0) ? 1.0 : 0.0;   // rot_end = Eye3d
+            for (int i = 0; i < 3; ++i) { sw[9 + i] = 0.0; sw[12 + i] = grav[i]; }   // bias_g = Zero3d, gravity
+            std::memcpy(sw + 15, imu + 7 * (size_t)(n_imu - 1), 7 * sizeof(double));   // last_imu_ = meas.imu.back()
+            double* dst = lio->d_ctrl->state;
+            IM_CUDA(cudaMemcpyAsync(dst, sw, 9 * sizeof(double), cudaMemcpyHostToDevice, st));
+            IM_CUDA(cudaMemcpyAsync(dst + 15, sw + 9, 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+            IM_CUDA(cudaMemcpyAsync(dst + 21, sw + 12, 3 * sizeof(double), cudaMemcpyHostToDevice, st));
+            IM_CUDA(cudaMemcpyAsync(h->d_time->last_imu, sw + 15, 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+            lio->pose_pub_idx = -1;
+            if (h->ini.N > h->max_ini) {   // init_iter_num > MAX_INI_COUNT: imu_need_init_ = false; UndistortPcl scales by |mean_acc| from now on
+                h->init_phase = 0;
+                h->P.mean_acc_norm = norm;
+            }
+        }
+        const int rc = imu_stage_release(h, s, st);
+        if (rc) return rc;
+        if (branch_out) *branch_out = 1;
+        return IMMESH_OK;
+    }
+    int rc = imu_enqueue_undistort(h, lio, imu, n_imu, pts_xyzt, n, on_device, lidar_beg_time, s);
+    if (rc) return rc;
+    rc = imu_stage_release(h, s, st);
+    if (rc) return rc;
+    lio->pose_pub_idx = -1;
+    if (!h->map_built) {
+        // branch 2: voxel_map_init from the full-resolution, undistorted, calibrated scan (voxel_mapping.cpp:1844-1859, :1894-1904)
+        rc = immesh_frontend_build_async(lio, vg, h->d_out, n, 4, calib_laser);
+        if (rc) return rc;
+        h->map_built = 1;
+        if (branch_out) *branch_out = 2;
+        return IMMESH_OK;
+    }
+    // branch 3: calibration -> VoxelGrid -> IESKF on the propagated state (no Forward_without_imu) -> map_incremental_grow
+    rc = immesh_lio_step_async_raw(lio, vg, h->d_out, n, 4, 1, calib_laser, leaf, 0.0, 0.0, 0.0);
+    if (rc) return rc;
+    if (branch_out) *branch_out = 3;
+    return IMMESH_OK;
 }
 
 }  // extern "C"

@@ -1,6 +1,8 @@
 // immesh_b200 -- IMU step in front of the hot path (SURVEY 8f-2): the device bodies of ImuProcess::UndistortPcl
-// (/root/reference/src/IMU_Processing.cpp:755-958).  Split of the work:
-//   host   (imu_capi.cu)   : time stamps only -- which IMU intervals are live, their dt / offset, the scan-end dt and sign
+// (/root/reference/src/IMU_Processing.cpp:755-958) and the host part of IMU_init (:188-232).  Split of the work:
+//   imu_plan                : time stamps only -- which IMU intervals are live, their dt / offset, the scan-end dt and sign (one thread
+//                             of k_imu_forward, on the members carried in ImuTime)
+//   imu_init_batch          : IMU_init's running means on the host (the samples are host data)
 //   imu_forward_step        : one IMU interval: bias / gravity-scale correction, 18x18 covariance propagation F P F^T + Q,
 //                             attitude / velocity / position integration, IMUpose record (block-cooperative, tid / nthreads)
 //   imu_predict_end         : state at the scan end (:881-896)
@@ -26,6 +28,77 @@ struct ImuStep {          // one live interval (head, tail) of v_imu
 };
 // running quantities of the propagation that are not part of the 348-double state: [acc_imu 3 | angvel_avr 3 | vel 3 | pos 3 | R 9]
 #define IM_IMU_RUN 21
+
+// The ImuProcess members UndistortPcl reads and writes from scan to scan, kept in device memory so that the interval plan of a scan
+// is worked out on the device, in stream order, without reading the scan back.
+struct ImuTime {
+    double last_imu[7];          // last_imu_: stamp, angular_velocity, linear_acceleration
+    double last_lidar_end_time;  // last_lidar_end_time_
+    double upd_beg;              // lidar_meas.last_update_time = upd_beg + (double)upd_curv / 1000, the pcl_end_time of the last scan kept as
+    float upd_curv;              //   its two inputs (lidar_beg_time, last point's curvature), so that a queued copy of the stamp can set it
+    int n_pose;                  // IMUpose entries of the last plan
+};
+
+// The time-stamp logic of UndistortPcl (IMU_Processing.cpp:759-787, :810-836, :881-896): the live intervals of v_imu = last_imu_ +
+// meas.imu with their dt and offset, the scan-end dt and sign, and the members carried to the next scan.  imu: [n_imu][7];
+// last_curv: curvature of the LAST point of the unsorted scan (:786).  Returns the number of live intervals.
+IM_HDN inline int imu_plan(ImuTime& tm, const double* imu, int n_imu, float last_curv, double lidar_beg_time, ImuStep* steps, double* note, double* dt_end) {
+    const double* back = n_imu > 0 ? imu + 7 * (size_t)(n_imu - 1) : tm.last_imu;
+    const double imu_end_time = back[0];
+    const double last_update_time = tm.upd_beg + (double)tm.upd_curv / double(1000);
+    const double pcl_beg_time = (lidar_beg_time < last_update_time) ? last_update_time : lidar_beg_time;   // MAX
+    const double pcl_end_time = lidar_beg_time + (double)last_curv / double(1000);
+    tm.upd_beg = lidar_beg_time;
+    tm.upd_curv = last_curv;
+    int n_steps = 0;
+    for (int k = 0; k < n_imu; ++k) {
+        const double* head = k == 0 ? tm.last_imu : imu + 7 * (size_t)(k - 1);
+        const double* tail = imu + 7 * (size_t)k;
+        if (tail[0] < tm.last_lidar_end_time) continue;
+        ImuStep& s = steps[n_steps++];
+        for (int i = 0; i < 3; ++i) { s.gyr_avg[i] = 0.5 * (head[1 + i] + tail[1 + i]); s.acc_avg[i] = 0.5 * (head[4 + i] + tail[4 + i]); }
+        s.dt = (head[0] < tm.last_lidar_end_time) ? tail[0] - tm.last_lidar_end_time : tail[0] - head[0];
+        s.offs_t = tail[0] - pcl_beg_time;
+    }
+    if (imu_end_time > pcl_beg_time) { *note = pcl_end_time > imu_end_time ? 1.0 : -1.0; *dt_end = *note * (pcl_end_time - imu_end_time); }
+    else { *note = pcl_end_time > pcl_beg_time ? 1.0 : -1.0; *dt_end = *note * (pcl_end_time - pcl_beg_time); }
+    if (back != tm.last_imu)
+        for (int i = 0; i < 7; ++i) tm.last_imu[i] = back[i];
+    tm.last_lidar_end_time = pcl_end_time;
+    tm.n_pose = n_steps + 1;
+    return n_steps;
+}
+
+// IMU_init, StatesGroup version (IMU_Processing.cpp:188-232), on the host: the IMU samples arrive in host memory and nothing else is read.
+// The covariance lines are commented out in the reference and absent here.
+struct ImuInit {
+    double mean_acc[3], mean_gyr[3];
+    int N;             // init_iter_num (counts samples)
+    int first_frame;   // b_first_frame_
+};
+// ImuProcess::Reset() as far as IMU_init's members go (:73-86)
+inline void imu_init_reset(ImuInit& s) {
+    s.mean_acc[0] = 0.0; s.mean_acc[1] = 0.0; s.mean_acc[2] = -1.0;
+    s.mean_gyr[0] = s.mean_gyr[1] = s.mean_gyr[2] = 0.0;
+    s.N = 1;
+}
+// one non-empty batch; returns |mean_acc| and gravity = -mean_acc / |mean_acc| * G_m_s2 (rot_end = I, bias_g = 0 are the caller's)
+inline double imu_init_batch(ImuInit& s, const double* imu, int n_imu, double* gravity) {
+    if (s.first_frame) {
+        imu_init_reset(s);
+        s.first_frame = 0;
+        for (int i = 0; i < 3; ++i) { s.mean_acc[i] = imu[4 + i]; s.mean_gyr[i] = imu[1 + i]; }
+    }
+    for (int k = 0; k < n_imu; ++k) {
+        const double* m = imu + 7 * (size_t)k;
+        const double N = (double)s.N;
+        for (int i = 0; i < 3; ++i) { s.mean_acc[i] = s.mean_acc[i] + (m[4 + i] - s.mean_acc[i]) / N; s.mean_gyr[i] = s.mean_gyr[i] + (m[1 + i] - s.mean_gyr[i]) / N; }
+        s.N++;
+    }
+    const double norm = std::sqrt((s.mean_acc[0] * s.mean_acc[0] + s.mean_acc[1] * s.mean_acc[1]) + s.mean_acc[2] * s.mean_acc[2]);
+    for (int i = 0; i < 3; ++i) gravity[i] = -s.mean_acc[i] / norm * 9.81;
+    return norm;
+}
 
 IM_HDN inline void imu_write_pose(double* pose, double t, const double* run) {
     pose[0] = t;

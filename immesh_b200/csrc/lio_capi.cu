@@ -1277,6 +1277,35 @@ int immesh_lio_step_async_dev_n(immesh_lio_t* h, const float* d_body_xyz, int n_
     h->next_n_dev = d_n;
     return lio_enqueue(h, d_body_xyz, n_max, 1, dt, cov_gyr, cov_acc, true);
 }
+// voxel_map_init queued like a pipelined step (internal: the first scan after the IMU initialisation, immesh_lio_step_async_imu): the
+// build kernels of immesh_voxelmap_build on a device-resident full scan, behind the staging-slot protocol, without a host wait
+int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, int n) {
+    if (!h || !d_body_xyz || n < 1) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (n > h->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than max_scan_points");
+    const int grc = lio_growth_check(h, n);
+    if (grc) return grc;
+    const int s = (++h->step_counter) & (IM_SLOTS - 1);
+    if (h->slot_busy[s]) {
+        const auto t0 = std::chrono::steady_clock::now();
+        IM_CUDA(cudaEventSynchronize(h->ev_slot[s]));
+        h->host_wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        h->slot_busy[s] = 0;
+    }
+    ++h->scan_counter;
+    ++h->map_steps;
+    int rc = upload_scan(h, d_body_xyz, n, 1, s);
+    if (rc) return rc;
+    launch_grow(h, 1);
+    h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(h->h_out + s, &h->d_ctrl->out, sizeof(LioOut), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaEventRecord(h->ev_slot[s], h->stream));
+    h->slot_busy[s] = 1;
+    h->slot_step[s] = h->map_steps;
+    h->timed_last = 0;
+    h->pose_pub_idx = h->scan_counter;
+    return IMMESH_OK;
+}
 int immesh_lio_wait(immesh_lio_t* h, double* state_out, int* iters_run) { return lio_wait_impl(h, state_out, iters_run, false); }
 // queue a write of `bytes` bytes over a caller-provided device buffer on the localization stream (benchmark L2 flush)
 int immesh_lio_enqueue_memset(immesh_lio_t* h, void* d_buf, size_t bytes) {

@@ -435,6 +435,40 @@ const float* immesh_imu_device_points(immesh_imu_t* h);
 /* IMUpose of the last call (Pose6D: offset_time, acc, gyr, vel, pos, rot = 22 doubles each); returns their number */
 int immesh_imu_get_poses(immesh_imu_t* h, double* out, int cap_poses);
 
+/* ---- the IMU-enabled scan loop (imu_en: true; config/avia.yaml, nclt.yaml, ntu.yaml): Voxel_mapping::service_LiDAR_update
+ * (src/voxel_mapping.cpp:1820-1905 and on) with ImuProcess::Process2 (src/IMU_Processing.cpp:960-1006) and IMU_init, StatesGroup
+ * version (src/IMU_Processing.cpp:188-232), as one queued call per scan.  Each scan takes exactly one branch:
+ *   1 initialising (imu_need_init_): lidar_meas.last_update_time = pcl_end_time; on a non-empty batch IMU_init -- running means of the
+ *     samples in the reference's order (on the host: the samples are host data), gravity = -mean_acc / |mean_acc| * 9.81, rot_end = I,
+ *     bias_g = 0 written into the localization handle's state in stream order, last_imu_ = the batch's last sample; once
+ *     init_iter_num (which counts samples) exceeds max_ini_count the phase ends and UndistortPcl scales the accelerations by |mean_acc|
+ *     instead of immesh_imu_config::mean_acc_norm.  Nothing else: the reference's m_feats_undistort is empty and the loop continues.
+ *   2 the first scan after it: UndistortPcl, [KITTI calibration], voxel_map_init from the full-resolution undistorted scan (queued:
+ *     the build kernels of immesh_voxelmap_build read the calibrated scan on the device).  No IESKF, no map growth, no mesh frame.
+ *   3 every later scan: UndistortPcl, [calibration], VoxelGrid(leaf), IESKF on the propagated state (no Forward_without_imu),
+ *     map_incremental_grow -- immesh_lio_step_async_raw on the undistorted scan.  Hand the frame to the mesher after it with
+ *       immesh_mesh_push_frame_from_lio_async(mesh, lio, immesh_voxelgrid_input_points(vg), n, 1)
+ *     before the next call on vg (the input ring of vg keeps the packed scan for the frames still in flight).
+ * *branch_out = the branch taken.  It depends on sample counts and the first-map flag only, so the host knows it without waiting.  The
+ * call waits for the device only on a busy staging slot (immesh_host_wait_ms, localization handle); immesh_lio_wait drains it.
+ * The first-map flag is set by branch 2 and kept across immesh_imu_init_begin (the reference's m_init_map survives its reset).
+ * Defined where the reference is not: last_lidar_end_time_ (src/IMU_Processing.h:146) has no initialiser and nothing sets it before
+ * the first UndistortPcl: it is 0.0 here (what the zero-filled heap the reference runs on gives).
+ * imu: [n_imu][7] host array (stamp, gyr xyz, acc xyz); pts_xyzt: [n][4] as for immesh_imu_undistort (host, or device with on_device).
+ * Errors, returned before anything is queued or any counter moves: n_imu > max_imu, n > the IMU or VoxelGrid handle's max_points, or
+ * n > the localization handle's max_scan_points (the map is built from the whole scan, and a scan the VoxelGrid passes through reaches
+ * the step whole): IMMESH_E_CAPACITY; a sharded localization handle: IMMESH_E_INVALID. */
+/* Enter branch 1.  The first call on a handle starts from a fresh ImuProcess (b_first_frame_: the first batch seeds the means; zero
+ * last_imu_, acc_s_last, angvel_last).  A later call is the loop's reset (m_flg_reset -> Reset(), src/voxel_mapping.cpp:1791-1796):
+ * b_first_frame_ stays false, so the means restart from mean_acc = (0, 0, -1), mean_gyr = 0 with init_iter_num = 1; last_imu_ and
+ * angvel_last are zeroed, acc_s_last and last_lidar_end_time_ kept.  A handle that never calls it has no initialisation phase:
+ * immesh_lio_step_async_imu starts at branch 2 with the configured mean_acc_norm (the caller-initialised flow).
+ * max_ini_count = MAX_INI_COUNT (mapping/imu_int_frame, 3 by default). */
+int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count);
+int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_voxelgrid_t* vg, const double* imu /*[n_imu][7]*/, int n_imu,
+                              const float* pts_xyzt /*[n][4]*/, int n, int on_device, double lidar_beg_time, int calib_laser, float leaf,
+                              int* branch_out /*or NULL*/);
+
 /* optional per-kernel CUDA-event profiler (off by default) and launch accounting, process-wide */
 int immesh_profile_enable(int on);   /* 0 off, 1 per-kernel totals, 2 totals + timeline */
 int immesh_profile_timeline(char* buf, int cap); /* "kernel t0_ms t1_ms\n" per launch; returns bytes needed */
