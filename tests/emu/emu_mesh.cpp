@@ -192,6 +192,16 @@ int emu_mesh_xapply_lists(immesh_mesh_t* h, const int* face4, const unsigned lon
     return 0;
 }
 int emu_mesh_error_word(immesh_mesh_t* h) { return h->last_cnt[3]; }   // IM_MERR_* flags of the last frame
+// keys (x, y, z) of the voxels the last frame meshed (its work list, in work-list order); returns their number
+int emu_mesh_frame_voxels(immesh_mesh_t* h, int32_t* keys) {
+    const int nw = work_total(h->M, h->F);
+    for (int i = 0; keys && i < nw; ++i) {
+        int x, y, z;
+        unpack_ikey(h->M.vkeys[h->F.work[work_slot(h->M, h->F, i)]], &x, &y, &z);
+        keys[i * 3] = x; keys[i * 3 + 1] = y; keys[i * 3 + 2] = z;
+    }
+    return nw;
+}
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
     const int* c = h->last_cnt;
     out[0] = c[0]; out[1] = c[2]; out[2] = c[10]; out[3] = c[6] + c[17]; out[4] = c[7]; out[5] = c[8]; out[6] = c[4]; out[7] = c[5];

@@ -157,6 +157,16 @@ def shell(per_face=(7, 6), cluster=3, key=(3, -2, 5), res=0.4, xi=0.001, spacing
     return Scene(f"shell_c{cluster}", [pts], dict(points_minimum_scale=xi, voxel_resolution=res), c)
 
 
+def xi_tie(xi=0.125, res=0.4):
+    """points exactly xi apart in float (xi and every coordinate binary-exact), in different xi-cells: frame 0 holds two of them
+    (the in-frame test), frame 1 one more at distance xi from the first vertex (the test against the map).  sqrtf(d) == xi, so
+    every one of them is appended: the reference rejects only points strictly closer than xi.  The first point's x / res is 2.5,
+    where std::round (half away from zero) and round-half-to-even disagree."""
+    a = np.array([1.0, 2.0, 0.5])
+    frames = [_f32([a, a + [0.0, xi, 0.0]]), _f32([a + [xi, 0.0, 0.0]])]
+    return Scene("xi_tie", frames, dict(points_minimum_scale=xi, voxel_resolution=res), a)
+
+
 def voxel_key(p, res):
     return np.round(np.asarray(p, np.float64) / res).astype(np.int64)
 
