@@ -172,6 +172,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_imu_get_poses", [vp, dp, C.c_int]),
         ("immesh_imu_init_begin", [vp, C.c_int]),
         ("immesh_lio_step_async_imu", [vp, vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, ip]),
+        ("immesh_voxelgrid_filter_i", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, ip, ip]),
+        ("immesh_lio_step_async_raw_i", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_double, C.c_double, C.c_double]),
+        ("immesh_lio_step_async_imu_i", [vp, vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, ip]),
+        ("immesh_lio_frontend_cloud", [vp, vp, C.c_int, C.c_int, fp, C.c_int, ip]),
     ):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
@@ -430,6 +434,20 @@ class Lio:
             _check(self.lib, rc, "lio_registered_cloud")
         rows = np.zeros((max(n_out.value, 1), SCAN_PUB_COLS), dtype=np.float32)
         _check(self.lib, call(rows.ctypes.data_as(C.POINTER(C.c_float)), n_out.value), "lio_registered_cloud")
+        return rows[: n_out.value]
+
+    def frontend_cloud(self, vg: "VoxelGrid", dense: bool, point_skip=1):
+        """publish_frame_world from the front-end clouds of the last _i step through vg (immesh_lio_frontend_cloud): float32[m, 4] rows
+        world x y z intensity of the calibrated full scan (dense) or of the down-sampled scan the step localised."""
+        n_out = C.c_int(0)
+
+        def call(rows, cap):
+            return self.lib.immesh_lio_frontend_cloud(self._h, vg._h, 1 if dense else 0, point_skip, rows, cap, C.byref(n_out))
+        rc = call(None, 0)
+        if rc not in (0, -3):
+            _check(self.lib, rc, "lio_frontend_cloud")
+        rows = np.zeros((max(n_out.value, 1), SCAN_PUB_COLS), dtype=np.float32)
+        _check(self.lib, call(rows.ctypes.data_as(C.POINTER(C.c_float)), n_out.value), "lio_frontend_cloud")
         return rows[: n_out.value]
 
     def work_stats(self):
@@ -701,6 +719,27 @@ class VoxelGrid:
     def device_points(self) -> int:
         return int(self.lib.immesh_voxelgrid_device_points(self._h) or 0)
 
+    @staticmethod
+    def _records(pts, n, stride, on_device):
+        """(pointer, n, stride) of point records: a float32[n, stride] host array, or an integer CUDA address with n and stride"""
+        if on_device:
+            return C.c_void_p(int(pts)), int(n), int(stride)
+        a = np.ascontiguousarray(pts, dtype=np.float32)
+        if a.ndim != 2:
+            a = a.reshape(a.shape[0], -1)
+        return a, a.shape[0], a.shape[1]
+
+    def filter_i(self, pts, leaf: float, intensity_col: int, n=None, stride=None, on_device=False):
+        """filter() on point records of `stride` floats (x y z, intensity in column intensity_col): float32[m, 4] x y z intensity"""
+        a, cnt, stride = self._records(pts, n, stride, on_device)
+        ptr = a if on_device else a.ctypes.data_as(C.c_void_p)
+        out = np.zeros((max(cnt, 1), 4), dtype=np.float32)
+        m, small = C.c_int(0), C.c_int(0)
+        _check(self.lib, self.lib.immesh_voxelgrid_filter_i(self._h, ptr, cnt, stride, intensity_col, 1 if on_device else 0, C.c_float(leaf),
+                                                            out.ctypes.data_as(C.c_void_p), C.byref(m), C.byref(small)), "voxelgrid_filter_i")
+        self.m, self.leaf_too_small = m.value, bool(small.value)
+        return out[:m.value].copy()
+
     def prepare(self, pts, calib_laser=False, fetch=True):
         """KITTI laser calibration (optional) + repack of a float32[n,3] or [n,4] cloud; the packed cloud stays on the device
         (input_points()).  Returns it as float32[n,3] when fetch."""
@@ -724,6 +763,29 @@ class VoxelGrid:
         _check(self.lib, self.lib.immesh_lio_step_async_raw(lio._h, self._h, ptr, cnt, stride, 1 if on_device else 0, 1 if calib_laser else 0, C.c_float(leaf),
                                                             dt, cov_gyr, cov_acc), "lio_step_async_raw")
         lio._last_n = cnt
+
+    def step_async_raw_i(self, lio: "Lio", pts, leaf: float, intensity_col: int, dt=0.0, calib_laser=False, cov_gyr=0.1, cov_acc=0.1, n=None, stride=None,
+                         on_device=False):
+        """step_async_raw on point records of `stride` floats, the intensity (column intensity_col) kept for lio.frontend_cloud(self, ...)"""
+        a, cnt, stride = self._records(pts, n, stride, on_device)
+        ptr = a if on_device else a.ctypes.data_as(C.c_void_p)
+        _check(self.lib, self.lib.immesh_lio_step_async_raw_i(lio._h, self._h, ptr, cnt, stride, intensity_col, 1 if on_device else 0, 1 if calib_laser else 0,
+                                                              C.c_float(leaf), dt, cov_gyr, cov_acc), "lio_step_async_raw_i")
+        lio._last_n = cnt
+
+    def step_async_imu_i(self, lio: "Lio", imu_h: "Imu", batch, pts, lidar_beg_time: float, leaf: float, time_col: int, intensity_col: int,
+                         calib_laser=False, n=None, stride=None, on_device=False) -> int:
+        """step_async_imu on point records of `stride` floats (time stamp in time_col, intensity in intensity_col; pcl::PointXYZINormal:
+        stride 12, time 9, intensity 8).  Returns the branch; after branch 3, lio.frontend_cloud(self, ...) publishes with intensity."""
+        im = np.ascontiguousarray(batch, dtype=np.float64).reshape(-1, 7)
+        a, cnt, stride = self._records(pts, n, stride, on_device)
+        ptr = a if on_device else a.ctypes.data_as(C.c_void_p)
+        br = C.c_int(0)
+        _check(self.lib, self.lib.immesh_lio_step_async_imu_i(lio._h, imu_h._h, self._h, im.ctypes.data_as(C.POINTER(C.c_double)), im.shape[0], ptr, cnt,
+                                                              stride, time_col, intensity_col, 1 if on_device else 0, lidar_beg_time, 1 if calib_laser else 0,
+                                                              C.c_float(leaf), C.byref(br)), "lio_step_async_imu_i")
+        lio._last_n = cnt
+        return br.value
 
     def step_async_imu(self, lio: "Lio", imu_h: "Imu", batch, pts, lidar_beg_time: float, leaf: float, calib_laser=False, n=None, on_device=False) -> int:
         """The IMU-enabled scan loop, one queued call per scan (immesh_lio_step_async_imu): batch float64[n_imu,7] (stamp, gyr, acc);

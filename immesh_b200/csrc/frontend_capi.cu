@@ -125,8 +125,9 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_heads(const unsigned int* __r
     if (threadIdx.x == 0) tile_heads[blockIdx.x] = s_cnt;
 }
 // head_pos != nullptr: only record where run `slot` starts (the sums are then taken by k_vg_centroid_warp)
+// inten != nullptr: the intensity of every point ([n], same index as pts) is averaged like x y z, into out_i (AccumulatorIntensity)
 __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid(const float* __restrict__ pts, const unsigned int* __restrict__ keys, const unsigned int* __restrict__ vals, int n,
-                                                             const int* __restrict__ tile_base, float* out, int* head_pos) {
+                                                             const int* __restrict__ tile_base, float* out, int* head_pos, const float* __restrict__ inten, float* out_i) {
     __shared__ int s_warp[VG_THREADS / 32];
     __shared__ int s_run;
     if (threadIdx.x == 0) s_run = tile_base[blockIdx.x];
@@ -146,15 +147,17 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid(const float* __restr
         if (head && head_pos) {
             head_pos[slot] = i;
         } else if (head) {   // CentroidPoint: float sums in run order, divided by (float)count
-            float sx = 0.f, sy = 0.f, sz = 0.f;
+            float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
             int e = i;
             while (e < n && keys[e] == k) {
                 const unsigned int p = vals[e];
                 sx += pts[3 * (size_t)p]; sy += pts[3 * (size_t)p + 1]; sz += pts[3 * (size_t)p + 2];
+                if (inten) si += inten[p];
                 ++e;
             }
             const float cnt = (float)(e - i);
             out[3 * (size_t)slot] = sx / cnt; out[3 * (size_t)slot + 1] = sy / cnt; out[3 * (size_t)slot + 2] = sz / cnt;
+            if (inten) out_i[slot] = si / cnt;
         }
         __syncthreads();
         if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < VG_THREADS / 32; ++w) t += s_warp[w]; s_run += t; }
@@ -165,43 +168,62 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid(const float* __restr
 // leaf near the sensor holds hundreds of points, ~1 us of dependent misses each), then every lane adds the 32 values in
 // run order from shuffles -- the float sum keeps the serial order of CentroidPoint, only the memory latency is taken off the chain.
 __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid_warp(const float* __restrict__ pts, const unsigned int* __restrict__ vals, const int* __restrict__ head_pos,
-                                                                  const int* __restrict__ total_heads, const VgGrid* g, float* out) {
+                                                                  const int* __restrict__ total_heads, const VgGrid* g, float* out,
+                                                                  const float* __restrict__ inten, float* out_i) {
     const int lane = threadIdx.x & 31;
     const int m = *total_heads, n_valid = g->n_finite;
     const int nwarps = gridDim.x * (blockDim.x >> 5);
     for (int slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); slot < m; slot += nwarps) {
         const int b = head_pos[slot], e = (slot + 1 < m) ? head_pos[slot + 1] : n_valid;
-        float sx = 0.f, sy = 0.f, sz = 0.f;
+        float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
         for (int c = b; c < e; c += 32) {
             const int i = c + lane;
-            float x = 0.f, y = 0.f, z = 0.f;
-            if (i < e) { const unsigned int p = vals[i]; x = pts[3 * (size_t)p]; y = pts[3 * (size_t)p + 1]; z = pts[3 * (size_t)p + 2]; }
+            float x = 0.f, y = 0.f, z = 0.f, w = 0.f;
+            if (i < e) {
+                const unsigned int p = vals[i];
+                x = pts[3 * (size_t)p]; y = pts[3 * (size_t)p + 1]; z = pts[3 * (size_t)p + 2];
+                if (inten) w = inten[p];
+            }
             const int cnt = min(32, e - c);
-            for (int t = 0; t < cnt; ++t) {
-                sx += __shfl_sync(0xffffffffu, x, t); sy += __shfl_sync(0xffffffffu, y, t); sz += __shfl_sync(0xffffffffu, z, t);
+            if (inten) {
+                for (int t = 0; t < cnt; ++t) {
+                    sx += __shfl_sync(0xffffffffu, x, t); sy += __shfl_sync(0xffffffffu, y, t); sz += __shfl_sync(0xffffffffu, z, t);
+                    si += __shfl_sync(0xffffffffu, w, t);
+                }
+            } else {
+                for (int t = 0; t < cnt; ++t) {
+                    sx += __shfl_sync(0xffffffffu, x, t); sy += __shfl_sync(0xffffffffu, y, t); sz += __shfl_sync(0xffffffffu, z, t);
+                }
             }
         }
         if (lane == 0) {
             const float cnt = (float)(e - b);
             out[3 * (size_t)slot] = sx / cnt; out[3 * (size_t)slot + 1] = sy / cnt; out[3 * (size_t)slot + 2] = sz / cnt;
+            if (inten) out_i[slot] = si / cnt;
         }
     }
 }
 __global__ void k_vg_finish(VgGrid* g, const int* total_heads, int n) {
     if (threadIdx.x == 0) g->m_out = g->too_small ? n : *total_heads;
 }
-__global__ void __launch_bounds__(VG_THREADS) k_vg_copy_if_small(const float* __restrict__ pts, int n, const VgGrid* g, float* out) {
+__global__ void __launch_bounds__(VG_THREADS) k_vg_copy_if_small(const float* __restrict__ pts, int n, const VgGrid* g, float* out, const float* __restrict__ inten, float* out_i) {
     if (!g->too_small) return;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < 3 * (size_t)n; i += (size_t)gridDim.x * blockDim.x) out[i] = pts[i];
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < 3 * (size_t)n; i += (size_t)gridDim.x * blockDim.x) {
+        out[i] = pts[i];
+        if (inten && i < (size_t)n) out_i[i] = inten[i];
+    }
 }
 
-// front of the front-end: strided input (3 floats xyz, or 4 as the IMU stage emits: xyz + curvature) -> packed [n][3], with the
-// KITTI laser calibration (voxel_mapping.cpp:1844-1859) applied on the way when preprocess/calib_laser is set
-__global__ void __launch_bounds__(VG_THREADS) k_frontend_pack(const float* __restrict__ src, int n, int stride, int calib, float* __restrict__ dst) {
+// front of the front-end: strided input (x y z in the first three of `stride` floats) -> packed [n][3], with the KITTI laser
+// calibration (voxel_mapping.cpp:1844-1859) applied on the way when preprocess/calib_laser is set.  dst_i != nullptr: the
+// intensity isrc[i * istride] is packed into dst_i[i] beside it (the calibration copies the whole point, intensity included).
+__global__ void __launch_bounds__(VG_THREADS) k_frontend_pack(const float* __restrict__ src, int n, int stride, int calib, float* __restrict__ dst,
+                                                               const float* __restrict__ isrc, int istride, float* __restrict__ dst_i) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         float x = src[(size_t)i * stride], y = src[(size_t)i * stride + 1], z = src[(size_t)i * stride + 2];
         if (calib) immesh::kitti_calib_point(&x, &y, &z);
         dst[3 * (size_t)i] = x; dst[3 * (size_t)i + 1] = y; dst[3 * (size_t)i + 2] = z;
+        if (dst_i) dst_i[i] = isrc[(size_t)i * istride];
     }
 }
 
@@ -227,6 +249,12 @@ struct immesh_voxelgrid {
     VgGrid* h_grid = nullptr;    // pinned
     float* h_pts = nullptr;      // pinned staging [max_points][3]
     int last_m = 0;
+    int raw_stride = 4;          // floats per point that d_raw / h_raw hold (widened by the first _i call with wider host records)
+    // intensity of the _i entry points, allocated by the first of them
+    float* d_in_i_ring[8] = {};  // intensity of the cloud in d_in_ring[k], same order
+    float* d_out_i = nullptr;    // [max_points] intensity of the down-sampled cloud d_out
+    float* h_out_i = nullptr;    // pinned [max_points]
+    long long calls = 0;         // calls that queued work on the handle (immesh_lio_frontend_cloud: has vg run another call since)
 };
 
 extern "C" {
@@ -273,13 +301,45 @@ int immesh_voxelgrid_destroy(immesh_voxelgrid_t* h) {
     for (int i = 0; i < 2; ++i) { cudaFree(h->d_k[i]); cudaFree(h->d_v[i]); }
     cudaFree(h->d_hist); cudaFree(h->d_tile); cudaFree(h->d_head); cudaFree(h->d_grid);
     cudaFreeHost(h->h_grid); cudaFreeHost(h->h_pts);
+    for (int i = 0; i < 8; ++i) cudaFree(h->d_in_i_ring[i]);
+    cudaFree(h->d_out_i); cudaFreeHost(h->h_out_i);
     cudaStreamDestroy(h->stream);
     delete h;
     return IMMESH_OK;
 }
 
-// queue the filter's launch sequence for the packed device cloud d_pts on stream st (no host synchronisation)
-static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf, cudaStream_t st) {
+// the intensity buffers of the _i entry points, and host staging for records of `host_stride` floats (0: device input only).
+// Allocated on first use, so that a handle that never carries intensity keeps the footprint it has at create.
+static int vg_intensity_alloc(immesh_voxelgrid* h, int host_stride) {
+    const size_t n = (size_t)h->max_points;
+    if (!h->d_out_i) {
+        for (int i = 0; i < 8; ++i) IM_CUDA(cudaMalloc((void**)&h->d_in_i_ring[i], n * sizeof(float)));
+        IM_CUDA(cudaMalloc((void**)&h->d_out_i, n * sizeof(float)));
+        IM_CUDA(cudaMallocHost((void**)&h->h_out_i, n * sizeof(float)));
+    }
+    if (host_stride > h->raw_stride) {
+        IM_CUDA(cudaDeviceSynchronize());   // no queued copy or pack still uses the narrower staging
+        h->raw_pending = 0;
+        cudaFree(h->d_raw); cudaFreeHost(h->h_raw);
+        h->d_raw = nullptr; h->h_raw = nullptr; h->raw_stride = 0;
+        IM_CUDA(cudaMalloc((void**)&h->d_raw, n * host_stride * sizeof(float)));
+        IM_CUDA(cudaMallocHost((void**)&h->h_raw, n * host_stride * sizeof(float)));
+        h->raw_stride = host_stride;
+    }
+    return IMMESH_OK;
+}
+// the point records the _i entry points take: `stride` floats, x y z in 0..2, intensity (and the time stamp, tcol >= 0) in columns
+// of their own beyond them
+static bool records_ok(int stride, int icol, int tcol) {
+    if (stride < 4 || stride > 16 || icol < 3 || icol >= stride) return false;
+    return tcol < 0 || (tcol >= 3 && tcol < stride && tcol != icol);
+}
+
+// queue the filter's launch sequence for the packed device cloud d_pts on stream st (no host synchronisation); inten != nullptr:
+// the points' intensity ([n]), averaged into d_out_i
+static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf, cudaStream_t st, const float* inten = nullptr) {
+    ++h->calls;
+    float* out_i = inten ? h->d_out_i : nullptr;
     const float inv = 1.0f / leaf;
     const int nb = (n + VG_TILE - 1) / VG_TILE;
     const int gs = std::min(nb * (VG_TILE / VG_THREADS), h->n_sm * 8);
@@ -299,14 +359,16 @@ static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf
     IM_LAUNCH(k_vg_heads, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, h->d_tile);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_tile, nb, h->d_tile + h->nblocks_max);
     if (h->warp_centroid) {
-        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, h->d_head);
+        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, h->d_head,
+                  (const float*)nullptr, (float*)nullptr);
         IM_LAUNCH(k_vg_centroid_warp, h->n_sm * 4, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_v[cur], (const int*)h->d_head,
-                  (const int*)(h->d_tile + h->nblocks_max), (const VgGrid*)h->d_grid, h->d_out);
+                  (const int*)(h->d_tile + h->nblocks_max), (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
     } else {
-        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, (int*)nullptr);
+        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, (int*)nullptr,
+                  inten, out_i);
     }
     IM_LAUNCH(k_vg_finish, 1, 32, 0, st, h->d_grid, (const int*)(h->d_tile + h->nblocks_max), n);
-    IM_LAUNCH(k_vg_copy_if_small, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, h->d_out);
+    IM_LAUNCH(k_vg_copy_if_small, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
     IM_CUDA(cudaGetLastError());
     return IMMESH_OK;
 }
@@ -347,6 +409,7 @@ int immesh_voxelgrid_filter(immesh_voxelgrid_t* h, const float* xyz, int n, int 
 int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int64_t n, int on_device, float leaf, int* too_small) {
     if (!h || (!xyz && n > 0) || n < 0 || !(leaf > 0.f) || !too_small) return im_fail(IMMESH_E_INVALID, "bad argument");
     cudaStream_t st = h->stream;
+    ++h->calls;
     IM_LAUNCH(k_vg_reset, 1, 32, 0, st, h->d_grid);
     for (int64_t c0 = 0; c0 < n; c0 += h->max_points) {
         const int m = (int)std::min<int64_t>(h->max_points, n - c0);
@@ -368,8 +431,16 @@ int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int
     return IMMESH_OK;
 }
 
-// upload (host input) + pack / calibrate into d_in on stream st
-static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int stride, int on_device, int calib_laser, cudaStream_t st) {
+// upload (host input) + pack / calibrate into d_in on stream st.  Intensity, packed into the ring slot beside d_in: column icol of
+// the records (icol >= 0), or the separate device array isep ([n]).
+static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int stride, int on_device, int calib_laser, cudaStream_t st, int icol = -1,
+                         const float* isep = nullptr) {
+    const bool with_i = icol >= 0 || isep;
+    if (with_i) {
+        const int rc = vg_intensity_alloc(h, on_device ? 0 : stride);
+        if (rc) return rc;
+    }
+    ++h->calls;
     h->in_idx = (h->in_idx + 1) & 7;
     h->d_in = h->d_in_ring[h->in_idx];
     const float* d_src = pts;
@@ -386,7 +457,9 @@ static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int strid
         if (src == h->h_raw) { IM_CUDA(cudaEventRecord(h->ev_raw, st)); h->raw_pending = 1; }
         d_src = h->d_raw;
     }
-    IM_LAUNCH(k_frontend_pack, std::min((n + VG_THREADS - 1) / VG_THREADS, h->n_sm * 8), VG_THREADS, 0, st, d_src, n, stride, calib_laser, h->d_in);
+    const float* isrc = icol >= 0 ? d_src + icol : isep;
+    IM_LAUNCH(k_frontend_pack, std::min((n + VG_THREADS - 1) / VG_THREADS, h->n_sm * 8), VG_THREADS, 0, st, d_src, n, stride, calib_laser, h->d_in,
+              isrc, icol >= 0 ? stride : 1, with_i ? h->d_in_i_ring[h->in_idx] : (float*)nullptr);
     return IMMESH_OK;
 }
 
@@ -408,19 +481,85 @@ int immesh_frontend_prepare(immesh_voxelgrid_t* h, const float* pts, int n, int 
 }
 const float* immesh_voxelgrid_input_points(immesh_voxelgrid_t* h) { return h ? h->d_in : nullptr; }
 
+int immesh_voxelgrid_filter_i(immesh_voxelgrid_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, float leaf, float* out_xyzi, int* m_out,
+                              int* leaf_too_small) {
+    if (!h || (!pts && n > 0) || n < 0 || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (!records_ok(stride, intensity_col, -1)) return im_fail(IMMESH_E_INVALID, "bad records (stride <= 16; intensity_col >= 3 and < stride)");
+    if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
+    if (m_out) *m_out = 0;
+    if (leaf_too_small) *leaf_too_small = 0;
+    h->last_m = 0;
+    if (n == 0) return IMMESH_OK;
+    cudaStream_t st = h->stream;
+    int rc = frontend_pack(h, pts, n, stride, on_device, 0, st, intensity_col);
+    if (rc) return rc;
+    rc = vg_enqueue(h, h->d_in, n, leaf, st, h->d_in_i_ring[h->in_idx]);
+    if (rc) return rc;
+    IM_CUDA(cudaMemcpyAsync(h->h_grid, h->d_grid, sizeof(VgGrid), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    const int m = h->h_grid->m_out;
+    h->last_m = m;
+    if (m_out) *m_out = m;
+    if (leaf_too_small) *leaf_too_small = h->h_grid->too_small;
+    if (out_xyzi && m > 0) {
+        IM_CUDA(cudaMemcpyAsync(h->h_pts, h->d_out, (size_t)m * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaMemcpyAsync(h->h_out_i, h->d_out_i, (size_t)m * sizeof(float), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaStreamSynchronize(st));
+        for (int j = 0; j < m; ++j) {
+            std::memcpy(out_xyzi + 4 * (size_t)j, h->h_pts + 3 * (size_t)j, 3 * sizeof(float));
+            out_xyzi[4 * (size_t)j + 3] = h->h_out_i[j];
+        }
+    }
+    return IMMESH_OK;
+}
+
 // The device-resident front-end chain of one scan (SURVEY 8f-1), queued on the localization handle's stream with no host round
 // trip: [KITTI laser calibration] -> pcl::VoxelGrid -> predict + IESKF iterations + map update.  The down-sampled cloud and its
 // size never leave the device (the step reads the count from the filter's result block).
+// internal (also immesh_lio_step_async_imu): the chain with the intensity of column icol of the records, or of the separate device
+// array isep, carried beside the clouds; then the step is what immesh_lio_frontend_cloud publishes from
+int immesh_frontend_step_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
+                               double dt, double cov_gyr, double cov_acc, int icol, const float* isep) {
+    const bool with_i = icol >= 0 || isep;
+    lio->fe_vg = nullptr;
+    cudaStream_t st = lio->stream;
+    int rc = frontend_pack(h, pts, n, stride, on_device, calib_laser, st, icol, isep);
+    if (rc) return rc;
+    rc = vg_enqueue(h, h->d_in, n, leaf, st, with_i ? h->d_in_i_ring[h->in_idx] : nullptr);
+    if (rc) return rc;
+    rc = immesh_lio_step_async_dev_n(lio, h->d_out, n < lio->max_scan ? n : lio->max_scan, &h->d_grid->m_out, dt, cov_gyr, cov_acc);
+    if (rc || !with_i) return rc;
+    lio->fe_vg = h;
+    lio->fe_uploads = lio->uploads;
+    lio->fe_vg_calls = h->calls;
+    lio->fe_n = n;
+    return IMMESH_OK;
+}
 int immesh_lio_step_async_raw(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
                               double dt, double cov_gyr, double cov_acc) {
     if (!lio || !h || (!pts && n > 0) || n < 1 || (stride != 3 && stride != 4) || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
-    cudaStream_t st = lio->stream;
-    int rc = frontend_pack(h, pts, n, stride, on_device, calib_laser, st);
-    if (rc) return rc;
-    rc = vg_enqueue(h, h->d_in, n, leaf, st);
-    if (rc) return rc;
-    return immesh_lio_step_async_dev_n(lio, h->d_out, n < lio->max_scan ? n : lio->max_scan, &h->d_grid->m_out, dt, cov_gyr, cov_acc);
+    return immesh_frontend_step_async(lio, h, pts, n, stride, on_device, calib_laser, leaf, dt, cov_gyr, cov_acc, -1, nullptr);
+}
+int immesh_lio_step_async_raw_i(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, int calib_laser,
+                                float leaf, double dt, double cov_gyr, double cov_acc) {
+    if (!lio || !h || !pts || n < 1 || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (!records_ok(stride, intensity_col, -1)) return im_fail(IMMESH_E_INVALID, "bad records (stride <= 16; intensity_col >= 3 and < stride)");
+    if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_raw_i runs on a single GPU: the localization handle is sharded");
+    if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
+    return immesh_frontend_step_async(lio, h, pts, n, stride, on_device, calib_laser, leaf, dt, cov_gyr, cov_acc, intensity_col, nullptr);
+}
+
+int immesh_lio_registered_cloud_sep(immesh_lio_t* h, const float* d_xyz, const float* d_inten, int n, int point_skip, float* rows, int cap, int* n_out);   // lio_capi.cu
+int immesh_lio_frontend_cloud(immesh_lio_t* lio, immesh_voxelgrid_t* vg, int dense, int point_skip, float* rows, int cap, int* n_out) {
+    if (!lio || !vg || !n_out || cap < 0 || (cap > 0 && !rows) || point_skip <= 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    *n_out = 0;
+    if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_frontend_cloud: the localization handle is sharded");
+    if (lio->fe_vg != vg || lio->fe_uploads != lio->uploads || lio->fe_vg_calls != vg->calls)
+        return im_fail(IMMESH_E_INVALID, "immesh_lio_frontend_cloud: the last step on the localization handle was not an intensity-carrying (_i) front-end chain "
+                                         "through this VoxelGrid handle, or the VoxelGrid handle has run another call since");
+    if (dense) return immesh_lio_registered_cloud_sep(lio, vg->d_in, vg->d_in_i_ring[vg->in_idx], lio->fe_n, point_skip, rows, cap, n_out);
+    return immesh_lio_registered_cloud_sep(lio, nullptr, vg->d_out_i, 0, point_skip, rows, cap, n_out);
 }
 
 const float* immesh_voxelgrid_device_points(immesh_voxelgrid_t* h) { return h ? h->d_out : nullptr; }
@@ -429,10 +568,10 @@ const float* immesh_voxelgrid_device_points(immesh_voxelgrid_t* h) { return h ? 
 // cloud -- [calibration] + repack into the input ring (immesh_voxelgrid_input_points), then the build kernels on the packed full scan
 int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h) { return h ? h->max_points : 0; }
 int immesh_voxelmap_build_async_dev(immesh_lio_t* lio, const float* d_body_xyz, int n);   // lio_capi.cu
-int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser) {
+int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser, const float* d_inten) {
     if (!lio || !h || !d_pts || n < 1 || (stride != 3 && stride != 4)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
-    const int rc = frontend_pack(h, d_pts, n, stride, 1, calib_laser, lio->stream);
+    const int rc = frontend_pack(h, d_pts, n, stride, 1, calib_laser, lio->stream, -1, d_inten);
     if (rc) return rc;
     return immesh_voxelmap_build_async_dev(lio, h->d_in, n);
 }

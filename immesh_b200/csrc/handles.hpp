@@ -38,6 +38,12 @@ struct immesh_lio {
     size_t spub_in_cap = 0;
     int scan_rows = 0;                      // per-scan buffers: 0 no IESKF run since create / voxelmap_build, 1 last run's, -1 overwritten
     const char* scan_rows_overwritten_by = nullptr;
+    long long uploads = 0;                  // scans placed in the per-scan buffers (upload_scan), by any call
+    // immesh_lio_frontend_cloud: the front-end that fed the last step, when it was an intensity-carrying (_i) chain
+    const void* fe_vg = nullptr;            // its VoxelGrid handle (nullptr: the last step was not such a chain)
+    long long fe_uploads = 0;               // `uploads` right after that step
+    long long fe_vg_calls = 0;              // the VoxelGrid's call count right after it
+    int fe_n = 0;                           // points of its full-resolution scan
     int* d_sorted = nullptr;
     int* d_complex = nullptr;   // touched root voxels left to the general warp-per-voxel kernel (the others are finished by k_grow_simple)
     double* d_ptpl = nullptr;

@@ -6,6 +6,7 @@
 //   k_imu_forward   one block: thread 0 seeds the running quantities from the state (IMUpose[0]) and works out the interval plan
 //                   (imu_plan) from the staged samples; then all live IMU intervals in sequence (18x18 F P F^T + Q each) and the
 //                   scan-end prediction
+//   k_imu_intake    (the _i entry) point records of `stride` floats -> [n][4] x y z t + [n] intensity
 //   k_imu_keys      time-stamp keys (ordered-uint image of the float curvature) for the stable radix sort (radix_sort.cuh)
 //   k_imu_gather    points in time order
 //   k_imu_undistort thread per point: interval lookup + rigid transform into the scan-end frame (16 B in, 16 B out per point)
@@ -58,8 +59,21 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_keys(const float* __restrict
         vals[i] = (unsigned int)i;
     }
 }
-__global__ void __launch_bounds__(VG_THREADS) k_imu_gather(const float4* __restrict__ in, const unsigned int* __restrict__ vals, int n, float4* out) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[vals[i]];
+__global__ void __launch_bounds__(VG_THREADS) k_imu_intake(const float* __restrict__ rec, int n, int stride, int tcol, int icol, float4* out, float* out_i) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float* r = rec + (size_t)i * stride;
+        out[i] = make_float4(r[0], r[1], r[2], r[tcol]);
+        out_i[i] = r[icol];
+    }
+}
+// in_i != nullptr: the intensity follows its point through the same permutation
+__global__ void __launch_bounds__(VG_THREADS) k_imu_gather(const float4* __restrict__ in, const unsigned int* __restrict__ vals, int n, float4* out,
+                                                            const float* __restrict__ in_i, float* out_i) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = vals[i];
+        out[i] = in[v];
+        if (in_i) out_i[i] = in_i[v];
+    }
 }
 // the IMUpose count comes from the plan (ImuTime::n_pose); the dynamic shared memory is sized for the batch's upper bound
 __global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm, float* pts, int n) {
@@ -102,11 +116,19 @@ struct immesh_imu {
     int began = 0;          // immesh_imu_init_begin has been called on the handle
     int pending_reset = 0;  // device members still to be reset in stream order: 1 Reset(), 2 a fresh ImuProcess
     int map_built = 0;      // m_init_map: the chain has built the VoxelMap
+    // immesh_lio_step_async_imu_i, allocated by its first call: the caller's point records and the intensity beside d_in / d_out
+    int rec_stride = 0;     // floats per record that d_rec / h_rec hold
+    float* d_rec = nullptr; // [max_points][rec_stride] the scan's records, when given in host memory
+    float* h_rec = nullptr; // pinned, IM_SLOTS slots of [max_points][rec_stride]
+    float* d_in_i = nullptr;   // [max_points] intensity in scan order
+    float* d_out_i = nullptr;  // [max_points] intensity in time order (beside d_out)
 };
 
 // internal entry points of frontend_capi.cu / lio_capi.cu
 extern "C" int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h);
-extern "C" int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser);
+extern "C" int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser, const float* d_inten);
+extern "C" int immesh_frontend_step_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
+                                          double dt, double cov_gyr, double cov_acc, int icol, const float* isep);
 
 // the next staging slot; blocks (back-pressure, counted in the localization handle's host wait) while its last copies are in flight
 static int imu_stage_slot(immesh_imu* h, immesh_lio* lio) {
@@ -125,9 +147,29 @@ static int imu_stage_release(immesh_imu* h, int s, cudaStream_t st) {
     return IMMESH_OK;
 }
 
+// the buffers of the _i entry: intensity beside d_in / d_out, and record staging of `stride` floats per point (grown for wider records)
+static int imu_records_alloc(immesh_imu* h, int stride) {
+    const size_t n = (size_t)h->max_points;
+    if (!h->d_in_i) {
+        IM_CUDA(cudaMalloc((void**)&h->d_in_i, n * sizeof(float)));
+        IM_CUDA(cudaMalloc((void**)&h->d_out_i, n * sizeof(float)));
+    }
+    if (stride > h->rec_stride) {
+        IM_CUDA(cudaDeviceSynchronize());   // no queued copy still reads the narrower staging
+        cudaFree(h->d_rec); cudaFreeHost(h->h_rec);
+        h->d_rec = nullptr; h->h_rec = nullptr; h->rec_stride = 0;
+        IM_CUDA(cudaMalloc((void**)&h->d_rec, n * stride * sizeof(float)));
+        IM_CUDA(cudaMallocHost((void**)&h->h_rec, IM_SLOTS * n * stride * sizeof(float)));
+        h->rec_stride = stride;
+    }
+    return IMMESH_OK;
+}
+
 // UndistortPcl queued on the localization stream through staging slot s: batch (+ host scan) upload, plan + forward propagation,
-// stable time sort, compensation into d_out.  No host synchronisation.
-static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device, double lidar_beg_time, int s) {
+// stable time sort, compensation into d_out.  No host synchronisation.  icol >= 0: pts holds records of `stride` floats (time stamp in
+// column tcol, intensity in icol), taken apart into d_in / d_in_i, and the intensity is sorted with the points into d_out_i.
+static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device, double lidar_beg_time, int s,
+                                 int stride = 4, int tcol = 3, int icol = -1) {
     cudaStream_t st = lio->stream;
     if (n_imu > 0) {
         double* hi = h->h_imu + (size_t)s * h->slot_doubles;
@@ -135,7 +177,17 @@ static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* i
         IM_CUDA(cudaMemcpyAsync(h->d_imu, hi, (size_t)n_imu * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
     }
     const float* d_pts = pts_xyzt;
-    if (!on_device) {
+    if (icol >= 0) {
+        const float* d_rec = pts_xyzt;
+        if (!on_device) {
+            float* hr = h->h_rec + (size_t)s * h->max_points * h->rec_stride;
+            std::memcpy(hr, pts_xyzt, (size_t)n * stride * sizeof(float));
+            IM_CUDA(cudaMemcpyAsync(h->d_rec, hr, (size_t)n * stride * sizeof(float), cudaMemcpyHostToDevice, st));
+            d_rec = h->d_rec;
+        }
+        IM_LAUNCH(k_imu_intake, std::min((n + VG_THREADS - 1) / VG_THREADS, h->n_sm * 8), VG_THREADS, 0, st, d_rec, n, stride, tcol, icol, (float4*)h->d_in, h->d_in_i);
+        d_pts = h->d_in;
+    } else if (!on_device) {
         float* hp = h->h_pts + (size_t)s * h->max_points * 4;
         std::memcpy(hp, pts_xyzt, (size_t)n * 4 * sizeof(float));
         IM_CUDA(cudaMemcpyAsync(h->d_in, hp, (size_t)n * 4 * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -154,7 +206,8 @@ static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* i
                   (const int*)h->d_hist, nb);
         cur ^= 1;
     }
-    IM_LAUNCH(k_imu_gather, gs, VG_THREADS, 0, st, (const float4*)d_pts, (const unsigned int*)h->d_v[cur], n, (float4*)h->d_out);
+    IM_LAUNCH(k_imu_gather, gs, VG_THREADS, 0, st, (const float4*)d_pts, (const unsigned int*)h->d_v[cur], n, (float4*)h->d_out,
+              icol >= 0 ? (const float*)h->d_in_i : (const float*)nullptr, icol >= 0 ? h->d_out_i : (float*)nullptr);
     const size_t smem = (size_t)(n_imu + 1) * IM_POSE_DOUBLES * sizeof(double);   // IMUpose holds at most n_imu + 1 entries
     IM_LAUNCH(k_imu_undistort, gs, VG_THREADS, smem, st, h->P, (const LioCtrl*)lio->d_ctrl, (const double*)h->d_poses, (const ImuTime*)h->d_time, h->d_out, n);
     IM_CUDA(cudaGetLastError());
@@ -209,6 +262,7 @@ int immesh_imu_destroy(immesh_imu_t* h) {
     cudaFree(h->d_time); cudaFree(h->d_run); cudaFree(h->d_poses); cudaFree(h->d_steps); cudaFree(h->d_imu); cudaFree(h->d_in); cudaFree(h->d_out);
     for (int i = 0; i < 2; ++i) { cudaFree(h->d_k[i]); cudaFree(h->d_v[i]); }
     cudaFree(h->d_hist); cudaFreeHost(h->h_imu); cudaFreeHost(h->h_pts);
+    cudaFree(h->d_rec); cudaFreeHost(h->h_rec); cudaFree(h->d_in_i); cudaFree(h->d_out_i);
     for (int i = 0; i < IM_SLOTS; ++i) if (h->ev_stage[i]) cudaEventDestroy(h->ev_stage[i]);
     delete h;
     return IMMESH_OK;
@@ -273,8 +327,12 @@ int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count) {
     return IMMESH_OK;
 }
 
-int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device,
-                              double lidar_beg_time, int calib_laser, float leaf, int* branch_out) {
+}  // extern "C"
+
+// the loop of immesh_lio_step_async_imu (icol < 0: [n][4] x y z t) and immesh_lio_step_async_imu_i (records of `stride` floats, the time
+// stamp in column tcol, the intensity in icol, carried through the sort, the calibration and the VoxelGrid)
+static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const float* pts_xyzt, int n, int stride, int tcol,
+                     int icol, int on_device, double lidar_beg_time, int calib_laser, float leaf, int* branch_out) {
     if (branch_out) *branch_out = 0;
     if (!lio || !h || !vg || (!imu && n_imu > 0) || n_imu < 0 || !pts_xyzt || n < 1 || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument (the scan must hold at least one point)");
     if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_imu runs on a single GPU: the localization handle is sharded");
@@ -282,6 +340,11 @@ int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgr
     if (n > h->max_points || n > immesh_voxelgrid_max_points(vg)) return im_fail(IMMESH_E_CAPACITY, "scan larger than the IMU / VoxelGrid handle's max_points");
     if (n > lio->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than the localization handle's max_scan_points (the map is built from the whole scan, and a scan the VoxelGrid passes through reaches the step whole)");
     cudaStream_t st = lio->stream;
+    lio->fe_vg = nullptr;   // branches 1 and 2 publish nothing (voxel_mapping.cpp:1879, :1903)
+    if (icol >= 0) {
+        const int rc = imu_records_alloc(h, on_device ? 0 : stride);
+        if (rc) return rc;
+    }
     if (h->pending_reset) {
         if (h->pending_reset == 2) {   // a fresh ImuProcess (last_lidar_end_time_ = 0.0, see the header)
             IM_CUDA(cudaMemsetAsync(h->d_time, 0, sizeof(ImuTime), st));
@@ -300,9 +363,9 @@ int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgr
         IM_CUDA(cudaMemcpyAsync((char*)h->d_time + offsetof(ImuTime, upd_beg), hw, sizeof(double), cudaMemcpyHostToDevice, st));
         float* curv_dst = (float*)((char*)h->d_time + offsetof(ImuTime, upd_curv));
         if (on_device) {
-            IM_CUDA(cudaMemcpyAsync(curv_dst, pts_xyzt + 4 * (size_t)(n - 1) + 3, sizeof(float), cudaMemcpyDeviceToDevice, st));
+            IM_CUDA(cudaMemcpyAsync(curv_dst, pts_xyzt + (size_t)stride * (n - 1) + tcol, sizeof(float), cudaMemcpyDeviceToDevice, st));
         } else {
-            std::memcpy(hw + 1, pts_xyzt + 4 * (size_t)(n - 1) + 3, sizeof(float));
+            std::memcpy(hw + 1, pts_xyzt + (size_t)stride * (n - 1) + tcol, sizeof(float));
             IM_CUDA(cudaMemcpyAsync(curv_dst, hw + 1, sizeof(float), cudaMemcpyHostToDevice, st));
         }
         if (n_imu > 0) {
@@ -328,24 +391,40 @@ int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgr
         if (branch_out) *branch_out = 1;
         return IMMESH_OK;
     }
-    int rc = imu_enqueue_undistort(h, lio, imu, n_imu, pts_xyzt, n, on_device, lidar_beg_time, s);
+    int rc = imu_enqueue_undistort(h, lio, imu, n_imu, pts_xyzt, n, on_device, lidar_beg_time, s, stride, tcol, icol);
     if (rc) return rc;
     rc = imu_stage_release(h, s, st);
     if (rc) return rc;
     lio->pose_pub_idx = -1;
+    const float* d_out_i = icol >= 0 ? h->d_out_i : nullptr;
     if (!h->map_built) {
         // branch 2: voxel_map_init from the full-resolution, undistorted, calibrated scan (voxel_mapping.cpp:1844-1859, :1894-1904)
-        rc = immesh_frontend_build_async(lio, vg, h->d_out, n, 4, calib_laser);
+        rc = immesh_frontend_build_async(lio, vg, h->d_out, n, 4, calib_laser, d_out_i);
         if (rc) return rc;
         h->map_built = 1;
         if (branch_out) *branch_out = 2;
         return IMMESH_OK;
     }
     // branch 3: calibration -> VoxelGrid -> IESKF on the propagated state (no Forward_without_imu) -> map_incremental_grow
-    rc = immesh_lio_step_async_raw(lio, vg, h->d_out, n, 4, 1, calib_laser, leaf, 0.0, 0.0, 0.0);
+    rc = immesh_frontend_step_async(lio, vg, h->d_out, n, 4, 1, calib_laser, leaf, 0.0, 0.0, 0.0, -1, d_out_i);
     if (rc) return rc;
     if (branch_out) *branch_out = 3;
     return IMMESH_OK;
+}
+
+extern "C" {
+
+int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const float* pts_xyzt, int n, int on_device,
+                              double lidar_beg_time, int calib_laser, float leaf, int* branch_out) {
+    return imu_chain(lio, h, vg, imu, n_imu, pts_xyzt, n, 4, 3, -1, on_device, lidar_beg_time, calib_laser, leaf, branch_out);
+}
+int immesh_lio_step_async_imu_i(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const float* pts, int n, int stride,
+                                int time_col, int intensity_col, int on_device, double lidar_beg_time, int calib_laser, float leaf, int* branch_out) {
+    if (branch_out) *branch_out = 0;
+    if (stride < 4 || stride > 16 || time_col < 3 || time_col >= stride || intensity_col < 3 || intensity_col >= stride || time_col == intensity_col)
+        return im_fail(IMMESH_E_INVALID, "bad records (stride <= 16; time_col and intensity_col distinct, >= 3 and < stride)");
+    if (lio && lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_imu_i runs on a single GPU: the localization handle is sharded");
+    return imu_chain(lio, h, vg, imu, n_imu, pts, n, stride, time_col, intensity_col, on_device, lidar_beg_time, calib_laser, leaf, branch_out);
 }
 
 }  // extern "C"

@@ -540,8 +540,10 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_eff_emit(LioParams P, ScanBuf 
     rows[off] = make_float4(r[0], r[1], r[2], r[3]);
     if (scan_index) scan_index[off] = i;
 }
-// rows j = 0 .. ceil(n / skip) - 1 from point j * skip; pts == null: the localised scan
-__global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const float* pts, int n, int stride, int col, int skip, float4* rows) {
+// rows j = 0 .. ceil(n / skip) - 1 from point j * skip; pts == null: the localised scan.  inten != null: the intensity of point i is
+// inten[i] (the front-end's clouds keep it beside the packed points) instead of column col
+__global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const float* pts, int n, int stride, int col, int skip, float4* rows,
+                                                             const float* __restrict__ inten) {
     __shared__ double s_state[12];
     if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
     if (!pts) {
@@ -553,7 +555,7 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBu
     for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < m; j += gridDim.x * blockDim.x) {
         const float* p = pts + (size_t)j * skip * stride;
         float r[4];
-        scan_pub_row(P, s_state, p, col >= 0 ? p[col] : 0.0f, r);
+        scan_pub_row(P, s_state, p, inten ? inten[(size_t)j * skip] : col >= 0 ? p[col] : 0.0f, r);
         rows[j] = make_float4(r[0], r[1], r[2], r[3]);
     }
 }
@@ -866,6 +868,7 @@ static int upload_scan(immesh_lio* h, const float* body, int n, int on_device = 
     return push_dyn(h, n, slot, dt, cov_gyr, cov_acc);
 }
 static int push_dyn(immesh_lio* h, int n, int slot, double dt, double cov_gyr, double cov_acc) {
+    ++h->uploads;
     h->sb.n = n;
     h->last_n = n;
     ScanDyn& d = h->h_dyn[slot];
@@ -1592,7 +1595,9 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, i
     return IMMESH_OK;
 }
 
-int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, int point_skip, float* rows, int cap, int* n_out) {
+// inten (device, or null): the points' intensity as a separate array (immesh_lio_frontend_cloud)
+static int registered_rows(immesh_lio_t* h, const float* pts, const float* inten, int n, int stride, int intensity_col, int on_device, int point_skip, float* rows,
+                           int cap, int* n_out) {
     if (!h || !n_out || cap < 0 || (cap > 0 && !rows)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (point_skip <= 0) return im_fail(IMMESH_E_INVALID, "registered cloud: point_skip must be positive");
     if (pts && (n < 0 || stride < 3 || intensity_col >= stride)) return im_fail(IMMESH_E_INVALID, "registered cloud: needs n >= 0, stride >= 3 and intensity_col < stride");
@@ -1628,11 +1633,18 @@ int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int st
     int rc = spub_grow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)m);
     if (rc) return rc;
     const int g = std::min((m + SPUB_THREADS - 1) / SPUB_THREADS, h->n_sm * 16);
-    IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows);
+    IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows, inten);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
     return IMMESH_OK;
+}
+int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, int point_skip, float* rows, int cap, int* n_out) {
+    return registered_rows(h, pts, nullptr, n, stride, intensity_col, on_device, point_skip, rows, cap, n_out);
+}
+// internal (immesh_lio_frontend_cloud): rows of the packed device cloud d_xyz ([n][3]; null: the localised scan) with intensity d_inten
+int immesh_lio_registered_cloud_sep(immesh_lio_t* h, const float* d_xyz, const float* d_inten, int n, int point_skip, float* rows, int cap, int* n_out) {
+    return registered_rows(h, d_xyz, d_inten, n, 3, -1, 1, point_skip, rows, cap, n_out);
 }
 
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out) {

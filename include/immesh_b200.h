@@ -213,8 +213,8 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows /*[cap][4]*/, int32_t* 
  * frame; intensity = pts[i * stride + intensity_col], or 0 when intensity_col < 0.  A host buffer is copied to a staging buffer of
  * its own; the scan the handle localised is left as it is.
  * pts == NULL (dense_map_en = 0): the down-sampled scan the handle last localised, read where the run read it (a caller-owned
- * device scan must still hold it), intensity 0 -- the device VoxelGrid does not carry intensity (PCL's averages it); n, stride,
- * intensity_col and on_device are then ignored.
+ * device scan must still hold it), intensity 0 -- the plain front-end chains do not carry intensity (PCL's VoxelGrid averages it;
+ * immesh_lio_frontend_cloud publishes it after the _i chains); n, stride, intensity_col and on_device are then ignored.
  * point_skip <= 0 (the reference would loop forever), stride < 3 or intensity_col >= stride: IMMESH_E_INVALID. */
 int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device,
                                 int point_skip, float* rows /*[cap][4]*/, int cap, int* n_out);
@@ -403,6 +403,40 @@ const float* immesh_voxelgrid_input_points(immesh_voxelgrid_t* h);
 int immesh_lio_step_async_raw(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
                               double dt, double cov_gyr, double cov_acc);
 
+/* ---- point intensity through the front-end.  The reference keeps every PointType field through the front-end: the KITTI
+ * calibration copies the whole point (src/voxel_mapping.cpp:1844-1859), and pcl::VoxelGrid (:1888-1889) runs with PCL's default
+ * downsample_all_data_ = true, so each leaf's intensity is CentroidPoint's AccumulatorIntensity: the float sum over the leaf, in the
+ * order of its x y z sums (ascending scan index here, see immesh_voxelgrid_filter), divided by (float)count.
+ * The _i entry points take the caller's point records as `stride` floats per point: x y z in columns 0..2, the intensity in column
+ * intensity_col (and, for the IMU chain, the time stamp, curvature in ms, in time_col) -- pcl::PointXYZINormal as it is: stride 12,
+ * intensity 8, curvature 9.  stride <= 16, the columns distinct, >= 3 and < stride; host pointer, or device pointer with on_device.
+ * Anything else: IMMESH_E_INVALID.  The intensity never enters what the localization or the mesher computes: the _i chains give the
+ * state, map, effect rows and mesh of their plain counterparts fed the same x y z (and stamps).  The intensity buffers (and host
+ * staging for wider records) are allocated by the first _i call on a handle.
+ * A sharded localization handle: IMMESH_E_INVALID (the _i chains and immesh_lio_frontend_cloud run on a single GPU). */
+/* immesh_voxelgrid_filter with intensity: same leaves, same order, bit-identical x y z; rows [m][4] = x y z intensity.  Non-finite
+ * points are dropped with their intensity; in the leaf-too-small branch the output is the input, intensity included.
+ * Replaces m_downSizeFilterSurf.filter(*m_feats_down_body) on PointXYZINormal clouds (src/voxel_mapping.cpp:1888-1889). */
+int immesh_voxelgrid_filter_i(immesh_voxelgrid_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, float leaf,
+                              float* out_xyzi /*[m][4] or NULL*/, int* m_out, int* leaf_too_small /*or NULL*/);
+/* immesh_lio_step_async_raw on point records, the intensity carried beside the clouds (src/voxel_mapping.cpp:1844-1859, :1888-1889):
+ * immesh_voxelgrid_input_points(vg) stays the packed [n][3] scan (hand it to the mesher as after the plain chain); vg keeps its
+ * intensity, and that of the down-sampled cloud, for immesh_lio_frontend_cloud. */
+int immesh_lio_step_async_raw_i(immesh_lio_t* lio, immesh_voxelgrid_t* vg, const float* pts, int n, int stride, int intensity_col,
+                                int on_device, int calib_laser, float leaf, double dt, double cov_gyr, double cov_acc);
+/* publish_frame_world (src/voxel_mapping_common.cpp:595-614, pointBodyToWorld :121-131 with po.intensity = pi.intensity) from the
+ * front-end's own clouds: dense != 0 -> the calibrated (undistorted, for the IMU chain time-sorted) full scan, m_feats_undistort;
+ * else the down-sampled scan the last step localised, m_feats_down_body.  Rows [n][4] = world x y z, intensity
+ * (IMMESH_SCAN_PUB_COLS) of points 0, point_skip, 2 point_skip, ..., transformed as immesh_lio_registered_cloud does, with the
+ * handle's current state: the dense = 0 rows are those of immesh_lio_registered_cloud(lio, NULL, ...) with the intensity filled in.
+ * transformLidar (:709-726) is the same arithmetic, so the viewer's current-scan points (g_eigen_vec_vec,
+ * src/ImMesh_mesh_reconstruction.cpp:102-106) are the dense = 1, point_skip = 1 rows.  Blocking: waits for the work queued on lio;
+ * the counts are read from the device.  *n_out > cap: IMMESH_E_CAPACITY with *n_out = rows needed (cap = 0: a count query).
+ * IMMESH_E_INVALID, besides bad arguments, when the last step on lio did not come through immesh_lio_step_async_raw_i or branch 3 of
+ * immesh_lio_step_async_imu_i with this vg (branches 1 and 2 publish nothing: the loop continues at src/voxel_mapping.cpp:1879,
+ * :1903), or when vg has run any other call since. */
+int immesh_lio_frontend_cloud(immesh_lio_t* lio, immesh_voxelgrid_t* vg, int dense, int point_skip, float* rows /*[cap][4]*/, int cap, int* n_out);
+
 /* ---- front-end (SURVEY 8f-2): IMU forward propagation + per-point motion compensation on the device.  Replaces
  *   ImuProcess::UndistortPcl(lidar_meas, state_inout, pcl_out)            (src/IMU_Processing.cpp:755-958)
  * for the LiDAR-only flow (is_lidar_end == true).  The handle carries the ImuProcess members the function reads and writes
@@ -468,6 +502,13 @@ int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count);
 int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_voxelgrid_t* vg, const double* imu /*[n_imu][7]*/, int n_imu,
                               const float* pts_xyzt /*[n][4]*/, int n, int on_device, double lidar_beg_time, int calib_laser, float leaf,
                               int* branch_out /*or NULL*/);
+/* immesh_lio_step_async_imu on point records (see immesh_voxelgrid_filter_i): lidar_meas.lidar as it is, the time stamp in time_col.
+ * UndistortPcl sorts and compensates whole PointType records (src/IMU_Processing.cpp:784, time_list :48): the intensity follows its
+ * point through the same stable time sort, then through the calibration and the VoxelGrid as in immesh_lio_step_async_raw_i.
+ * Branches, state, map and mesh hand-off are those of immesh_lio_step_async_imu fed the same x y z t. */
+int immesh_lio_step_async_imu_i(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_voxelgrid_t* vg, const double* imu /*[n_imu][7]*/, int n_imu,
+                                const float* pts, int n, int stride, int time_col, int intensity_col, int on_device,
+                                double lidar_beg_time, int calib_laser, float leaf, int* branch_out /*or NULL*/);
 
 /* optional per-kernel CUDA-event profiler (off by default) and launch accounting, process-wide */
 int immesh_profile_enable(int on);   /* 0 off, 1 per-kernel totals, 2 totals + timeline */
