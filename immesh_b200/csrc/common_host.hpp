@@ -8,7 +8,6 @@
 #include <map>
 #include <string>
 #include <tuple>
-#include <cstdlib>
 #include <vector>
 
 #include "../../include/immesh_b200.h"
@@ -94,23 +93,21 @@ Profiler& profiler();  // defined in misc_capi.cu
     } while (0)
 
 // ---- CUDA-graph replay of a fixed launch sequence.  The per-scan work is ~40 short kernels, so queueing them one by
-// one is host-launch-bound.  The same host code path runs in three modes: direct launch; capture (first pipelined call:
-// the launches are recorded into a graph and the node of every launch is remembered); update (later calls: every
-// "launch" only rewrites the parameters / grid of its node in the instantiated graph, then ONE cudaGraphLaunch replays it).
+// one is host-launch-bound.  The first pipelined call runs the host code path under stream capture, recording its launches
+// into a graph; every later call replays that graph with ONE cudaGraphLaunch and runs no host code of the sequence.  Outside
+// a capture (graph_ctx() null), IM_LAUNCH launches directly.
 namespace immesh {
 struct GraphCtx {
-    int mode = 0;                      // 0 direct, 1 capturing, 2 updating node parameters
     cudaGraphExec_t exec = nullptr;
     cudaGraph_t graph = nullptr;
-    std::vector<cudaGraphNode_t> nodes;
-    size_t cursor = 0;
+    long long kernels = 0;             // kernel launches recorded into the graph
     unsigned sig = 0;                  // control-flow signature the graph was captured with
     cudaError_t err = cudaSuccess;
     long long captures = 0, replays = 0, failures = 0;
     void destroy() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
-        exec = nullptr; graph = nullptr; nodes.clear();
+        exec = nullptr; graph = nullptr; kernels = 0;
     }
 };
 inline GraphCtx*& graph_ctx() {
@@ -128,79 +125,29 @@ inline void im_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 
         std::apply([&](auto&... v) { ((ptrs[k++] = (void*)&v), ...); }, vals);
     }
     GraphCtx* g = graph_ctx();
-    if (g && g->mode == 2) {
-        cudaKernelNodeParams kp{};
-        kp.func = (void*)kern; kp.gridDim = grid; kp.blockDim = block; kp.sharedMemBytes = (unsigned)smem;
-        kp.kernelParams = ptrs; kp.extra = nullptr;
-        cudaError_t e = (g->cursor < g->nodes.size()) ? cudaGraphExecKernelNodeSetParams(g->exec, g->nodes[g->cursor], &kp) : cudaErrorInvalidValue;
-        g->cursor++;
-        if (e != cudaSuccess && g->err == cudaSuccess) g->err = e;
-        return;
-    }
     if (pr.enabled) pr.begin(name, st);
     cudaError_t e = cudaLaunchKernel((const void*)kern, grid, block, ptrs, smem, st);
     if (pr.enabled) pr.end(st);
-    if (g && g->mode == 1) {
+    if (g) {   // capturing: the launch must have been recorded on a stream of the capture
         cudaStreamCaptureStatus status;
-        const cudaGraphNode_t* deps = nullptr;
-        size_t ndeps = 0;
-        cudaError_t e2 = cudaStreamGetCaptureInfo(st, &status, nullptr, nullptr, &deps, &ndeps);
-        if (e == cudaSuccess && e2 == cudaSuccess && status == cudaStreamCaptureStatusActive && ndeps == 1) g->nodes.push_back(deps[0]);
+        cudaError_t e2 = cudaStreamGetCaptureInfo(st, &status);
+        if (e == cudaSuccess && e2 == cudaSuccess && status == cudaStreamCaptureStatusActive) g->kernels++;
         else if (g->err == cudaSuccess) g->err = (e != cudaSuccess) ? e : (e2 != cudaSuccess ? e2 : cudaErrorUnknown);
     }
 }
-inline bool im_replaying() { GraphCtx* g = graph_ctx(); return g && g->mode == 2; }
-// queue `body` (a fixed sequence of IM_LAUNCH + fork/join event calls guarded by !im_replaying()) on `st` through graph `g`.
-// Returns cudaSuccess when the work was queued by a graph launch; on any failure the graph is dropped and the caller
-// queues the work directly.
-template <typename Body>
-inline cudaError_t run_graphed(GraphCtx& g, unsigned sig, cudaStream_t st, Body&& body) {
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        if (g.exec && g.sig != sig) g.destroy();
-        g.err = cudaSuccess;
-        graph_ctx() = &g;
-        if (!g.exec) {
-            g.nodes.clear();
-            cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
-            if (e != cudaSuccess) { graph_ctx() = nullptr; return e; }
-            g.mode = 1;
-            body();
-            g.mode = 0;
-            graph_ctx() = nullptr;
-            e = cudaStreamEndCapture(st, &g.graph);
-            if (e == cudaSuccess && g.err != cudaSuccess) e = g.err;
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&g.exec, g.graph, 0);
-            if (e != cudaSuccess) { g.destroy(); cudaGetLastError(); g.failures++; return e; }
-            g.sig = sig;
-            g.captures++;
-        } else {
-            g.mode = 2;
-            g.cursor = 0;
-            body();
-            g.mode = 0;
-            graph_ctx() = nullptr;
-            if (g.err != cudaSuccess || g.cursor != g.nodes.size()) { g.destroy(); cudaGetLastError(); g.failures++; continue; }  // re-capture
-            g.replays++;
-        }
-        return cudaGraphLaunch(g.exec, st);
-    }
-    return cudaErrorUnknown;
-}
-// Static form: the body's launches take every per-call value from device memory, so once captured the graph is replayed by a
-// bare cudaGraphLaunch -- the body is not run again and no node is touched.  `sig` must cover everything that changes the
-// sequence or its arguments (handle pointers, modes, iteration counts).
+// The body's launches take every per-call value from device memory, so once captured the graph is replayed by a bare
+// cudaGraphLaunch -- the body is not run again.  `sig` must cover everything that changes the sequence or its arguments
+// (handle pointers, modes, iteration counts).
 template <typename Body>
 inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st, Body&& body) {
     if (g.exec && g.sig != sig) g.destroy();
     if (!g.exec) {
         g.err = cudaSuccess;
-        g.nodes.clear();
+        g.kernels = 0;
         graph_ctx() = &g;
         cudaError_t e = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal);
         if (e != cudaSuccess) { graph_ctx() = nullptr; return e; }
-        g.mode = 1;
         body();
-        g.mode = 0;
         graph_ctx() = nullptr;
         e = cudaStreamEndCapture(st, &g.graph);
         if (e == cudaSuccess && g.err != cudaSuccess) e = g.err;
@@ -210,7 +157,7 @@ inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st
         g.captures++;
     } else {
         g.replays++;
-        profiler().launches += (long long)g.nodes.size();   // launch accounting: every kernel node of the graph runs
+        profiler().launches += g.kernels;   // launch accounting: every kernel of the graph runs
     }
     return cudaGraphLaunch(g.exec, st);
 }
@@ -218,11 +165,3 @@ inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st
 
 // kernel launch with accounting; wrap template kernels in parentheses: IM_LAUNCH((k<256>), grid, block, smem, stream, args...)
 #define IM_LAUNCH(KERN, GRID, BLOCK, SMEM, STREAM, ...) immesh::im_launch(#KERN, KERN, dim3(GRID), dim3(BLOCK), (SMEM), (STREAM), ##__VA_ARGS__)
-
-// stream priority from the environment (experiments): 0 = default (lowest), 1 = highest
-inline int im_stream_priority(const char* env) {
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    const char* e = getenv(env);
-    return (e && atoi(e) == 1) ? hi : lo;
-}

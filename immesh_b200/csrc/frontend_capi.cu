@@ -12,13 +12,13 @@
 //   k_vg_keys     idx per point (0xFFFFFFFF for non-finite points, sorted last and dropped)  12 n in, 8 n out
 //   k_rs_hist / k_rs_scan / k_rs_scatter  x4   stable LSD radix sort of (idx, point index), 8-bit digits, 2048-element tiles;
 //                 ranks inside a tile from __match_any_sync (warp) + per-warp digit counts (shared memory)   16 n in+out per pass
-//   k_vg_heads / k_rs_scan / k_vg_centroid   run heads -> output slots (tile counts + scan), serial float sums per run
+//   k_vg_heads / k_rs_scan / k_vg_head_pos   run heads -> output slots (tile counts + scan) -> start of every run
+//   k_vg_centroid_warp   one warp per run: serial float sums in run order
 // There is no CPU path: the entry points need a CUDA device.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -124,10 +124,8 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_heads(const unsigned int* __r
     __syncthreads();
     if (threadIdx.x == 0) tile_heads[blockIdx.x] = s_cnt;
 }
-// head_pos != nullptr: only record where run `slot` starts (the sums are then taken by k_vg_centroid_warp)
-// inten != nullptr: the intensity of every point ([n], same index as pts) is averaged like x y z, into out_i (AccumulatorIntensity)
-__global__ void __launch_bounds__(VG_THREADS) k_vg_centroid(const float* __restrict__ pts, const unsigned int* __restrict__ keys, const unsigned int* __restrict__ vals, int n,
-                                                             const int* __restrict__ tile_base, float* out, int* head_pos, const float* __restrict__ inten, float* out_i) {
+// record where every run starts: head_pos[slot] (the sums are then taken by k_vg_centroid_warp)
+__global__ void __launch_bounds__(VG_THREADS) k_vg_head_pos(const unsigned int* __restrict__ keys, int n, const int* __restrict__ tile_base, int* head_pos) {
     __shared__ int s_warp[VG_THREADS / 32];
     __shared__ int s_run;
     if (threadIdx.x == 0) s_run = tile_base[blockIdx.x];
@@ -144,27 +142,13 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid(const float* __restr
         __syncthreads();
         int slot = s_run + __popc(hb & ((1u << lane) - 1u));
         for (int w = 0; w < warp; ++w) slot += s_warp[w];
-        if (head && head_pos) {
-            head_pos[slot] = i;
-        } else if (head) {   // CentroidPoint: float sums in run order, divided by (float)count
-            float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-            int e = i;
-            while (e < n && keys[e] == k) {
-                const unsigned int p = vals[e];
-                sx += pts[3 * (size_t)p]; sy += pts[3 * (size_t)p + 1]; sz += pts[3 * (size_t)p + 2];
-                if (inten) si += inten[p];
-                ++e;
-            }
-            const float cnt = (float)(e - i);
-            out[3 * (size_t)slot] = sx / cnt; out[3 * (size_t)slot + 1] = sy / cnt; out[3 * (size_t)slot + 2] = sz / cnt;
-            if (inten) out_i[slot] = si / cnt;
-        }
+        if (head) head_pos[slot] = i;
         __syncthreads();
         if (threadIdx.x == 0) { int t = 0; for (int w = 0; w < VG_THREADS / 32; ++w) t += s_warp[w]; s_run += t; }
         __syncthreads();
     }
 }
-// one warp per run: the lanes fetch 32 points of the run at once (the loads are what made the thread-per-run loop slow: a dense
+// one warp per run: the lanes fetch 32 points of the run at once (the loads are what makes a thread-per-run loop slow: a dense
 // leaf near the sensor holds hundreds of points, ~1 us of dependent misses each), then every lane adds the 32 values in
 // run order from shuffles -- the float sum keeps the serial order of CentroidPoint, only the memory latency is taken off the chain.
 __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid_warp(const float* __restrict__ pts, const unsigned int* __restrict__ vals, const int* __restrict__ head_pos,
@@ -244,7 +228,6 @@ struct immesh_voxelgrid {
     int* d_hist = nullptr;       // [256 * nblocks_max]
     int* d_tile = nullptr;       // [nblocks_max + 1]
     int* d_head = nullptr;       // [max_points] start of every run in the sorted order
-    int warp_centroid = 1;       // 1: warp-per-run sums (k_vg_centroid_warp); 0: thread-per-run loop (IMMESH_VG_WARP_CENTROID=0)
     VgGrid* d_grid = nullptr;
     VgGrid* h_grid = nullptr;    // pinned
     float* h_pts = nullptr;      // pinned staging [max_points][3]
@@ -284,7 +267,6 @@ int immesh_voxelgrid_create(int max_points, immesh_voxelgrid_t** out) {
     IM_CUDA(cudaMalloc((void**)&h->d_hist, (size_t)256 * h->nblocks_max * sizeof(int)));
     IM_CUDA(cudaMalloc((void**)&h->d_tile, ((size_t)h->nblocks_max + 1) * sizeof(int)));
     IM_CUDA(cudaMalloc((void**)&h->d_head, n * sizeof(int)));
-    if (const char* e = std::getenv("IMMESH_VG_WARP_CENTROID")) h->warp_centroid = (e[0] == '1') ? 1 : 0;
     IM_CUDA(cudaMalloc((void**)&h->d_grid, sizeof(VgGrid)));
     IM_CUDA(cudaMallocHost((void**)&h->h_grid, sizeof(VgGrid)));
     IM_CUDA(cudaMallocHost((void**)&h->h_pts, n * 3 * sizeof(float)));
@@ -358,15 +340,9 @@ static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf
     }
     IM_LAUNCH(k_vg_heads, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, h->d_tile);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_tile, nb, h->d_tile + h->nblocks_max);
-    if (h->warp_centroid) {
-        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, h->d_head,
-                  (const float*)nullptr, (float*)nullptr);
-        IM_LAUNCH(k_vg_centroid_warp, h->n_sm * 4, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_v[cur], (const int*)h->d_head,
-                  (const int*)(h->d_tile + h->nblocks_max), (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
-    } else {
-        IM_LAUNCH(k_vg_centroid, nb, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], n, (const int*)h->d_tile, h->d_out, (int*)nullptr,
-                  inten, out_i);
-    }
+    IM_LAUNCH(k_vg_head_pos, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, (const int*)h->d_tile, h->d_head);
+    IM_LAUNCH(k_vg_centroid_warp, h->n_sm * 4, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_v[cur], (const int*)h->d_head,
+              (const int*)(h->d_tile + h->nblocks_max), (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
     IM_LAUNCH(k_vg_finish, 1, 32, 0, st, h->d_grid, (const int*)(h->d_tile + h->nblocks_max), n);
     IM_LAUNCH(k_vg_copy_if_small, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
     IM_CUDA(cudaGetLastError());

@@ -78,7 +78,6 @@ struct immesh_lio {
     int last_n = 0;
     immesh::GraphCtx graph;   // replay of the per-scan launch sequence (pipelined API)
     int use_graph = 1;
-    int bps = 4;              // (mesh: 3 by default, see immesh_mesh_create) resident blocks per SM of the persistent per-voxel kernels (headroom for the other stream)
     double last_ms[3] = {0, 0, 0};
     std::vector<void*> allocs;
     size_t dev_bytes = 0;         // device bytes of `allocs` (the create-time buffers, the map pools and what dev_alloc adds later)
@@ -129,9 +128,7 @@ struct immesh_mesh {
     int max_frame_points = 0;
     immesh::GraphCtx graph;   // replay of the per-frame launch sequence (pipelined API)
     int use_graph = 1;
-    int bps = 4;              // (mesh: 3 by default, see immesh_mesh_create) resident blocks per SM of the persistent per-voxel kernels (headroom for the other stream)
     int frame_counter = 0;
-    int dilate_bps = 3;       // resident blocks per SM of the dilation kernel
     int warp_nmax = 96;       // largest dilated set triangulated by a single warp
     int n_sm = 132;
     size_t ccap = 0;

@@ -51,7 +51,7 @@ __global__ void k_reset_scan(ScanBuf sb, LioCtrl* ctrl, int copy_prop) {
 //   k_terms : one thread per scan point: the 29 fixed-point normal-equation terms of the matched points; the block's sums are reduced
 //             with warp shuffles (integer adds: exact, order-free) and folded into the iteration's global accumulators with 60
 //             atomics; the last block to finish runs the 6x6 IESKF update (ieskf_solve).
-// k_residual is the two steps in one thread per point (used by immesh_lio_residual_build; IMMESH_LIO_SPLIT=0 selects it everywhere).
+// k_residual is the two steps in one thread per point (used by immesh_residual_build).
 #define RES_THREADS 128
 #define MATCH_THREADS 128
 #define MATCH_LANES 8
@@ -613,8 +613,7 @@ static cudaError_t dev_alloc(immesh_lio* h, T** p, size_t count, int memset_byte
 // Grids are fixed per handle (sized for max_scan_points, at most 8 waves of blocks; every per-point kernel is a grid-stride
 // loop over the n it reads from the device-resident ScanDyn), so that the captured launch sequence is identical for every scan.
 static int grid_fixed(const immesh_lio* h, int threads, int max_waves = 8) {
-    static const int by_n = std::getenv("IMMESH_DEBUG_GRID_N") ? std::atoi(std::getenv("IMMESH_DEBUG_GRID_N")) : 0;   // experiments: size the grids by the scan
-    long long g = ((long long)(by_n ? (h->last_n > 0 ? h->last_n : 1) : h->max_scan) + threads - 1) / threads;
+    long long g = ((long long)h->max_scan + threads - 1) / threads;
     const long long cap = (long long)h->n_sm * max_waves;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
@@ -666,7 +665,6 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
         if (im_e_ != cudaSuccess) { immesh_lio_destroy(h); return immesh::im_fail_cuda(im_e_, __FILE__, __LINE__); } \
     } while (0)
     fill_params(cfg, h->P);
-    h->bps = std::getenv("IMMESH_LIO_BPS") ? std::atoi(std::getenv("IMMESH_LIO_BPS")) : 4;
     h->use_graph = std::getenv("IMMESH_GRAPH") ? std::atoi(std::getenv("IMMESH_GRAPH")) : 1;
     const int caplog = cfg->hash_capacity_log2 ? cfg->hash_capacity_log2 : 22;
     h->cap = (size_t)1 << caplog;
@@ -676,7 +674,7 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
-    IM_CREATE(cudaStreamCreateWithPriority(&h->stream, cudaStreamNonBlocking, im_stream_priority("IMMESH_LIO_PRIO")));
+    IM_CREATE(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     for (auto& e : h->ev) IM_CREATE(cudaEventCreate(&e));
     for (int i = 0; i < IM_SLOTS; ++i) IM_CREATE(cudaEventCreateWithFlags(&h->ev_slot[i], cudaEventDisableTiming));
     IM_CREATE(cudaEventCreateWithFlags(&h->ev_pose, cudaEventDisableTiming));
@@ -1079,6 +1077,8 @@ static int lio_growth_check(immesh_lio* h, long long n) {
     }
     return IMMESH_OK;
 }
+// resident blocks per SM of the persistent per-voxel map update k_grow_voxel (headroom for the kernels on the other streams)
+#define GROW_VOXEL_BPS 4
 // map growth of the scan described by the device-resident ScanDyn
 static void launch_grow(immesh_lio* h, int mode) {
     const int g = grid_fixed(h, 128);
@@ -1086,10 +1086,10 @@ static void launch_grow(immesh_lio* h, int mode) {
     IM_LAUNCH(k_grow_segment, grid_fixed(h, 128, 2), 128, 0, h->stream, h->sb);
     IM_LAUNCH(k_grow_scatter, g, 128, 0, h->stream, h->sb);
     IM_LAUNCH(k_grow_simple, h->n_sm * 16, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_complex, h->d_counters + 11);
-    IM_LAUNCH(k_grow_voxel, h->n_sm * h->bps, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + 8, (const int*)h->d_complex, (const int*)(h->d_counters + 11));
+    IM_LAUNCH(k_grow_voxel, h->n_sm * GROW_VOXEL_BPS, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + 8, (const int*)h->d_complex, (const int*)(h->d_counters + 11));
     IM_LAUNCH(k_grow_finish, 1, 256, 0, h->stream, h->map, h->sb, h->d_counters + 8, h->d_ctrl, (const int*)h->d_counters);
 }
-// IESKF iterations.  One GPU: per iteration ONE kernel -- the residual pass; its last block runs the 6x6 IESKF update.
+// IESKF iterations.  One GPU: per iteration k_match then k_terms; the last block of k_terms runs the 6x6 IESKF update.
 // Sharded over peer windows: pass1(+publish bits) -> pass2(wait bits, +publish sums) -> solve(wait sums), exchanges fused in.
 // Sharded over NCCL (baseline): pass1 -> all-reduce(bit words) -> pass2 -> all-reduce(58 int64 sums) -> solve.
 static int launch_estimate(immesh_lio* h) {
@@ -1118,11 +1118,6 @@ static int launch_estimate(immesh_lio* h) {
             if (nccl().AllReduce(&h->d_ctrl->acc[it][0], &h->d_ctrl->acc[it][0], (size_t)IM_NTERMS * 2, kNcclUint64, kNcclSum, h->nccl_comm, h->stream)) return im_fail(IMMESH_E_CUDA, "ncclAllReduce(acc) failed");
             IM_LAUNCH(k_solve, 1, SOLVE_THREADS, 0, h->stream, h->P, h->d_ctrl, it);
         }
-        return IMMESH_OK;
-    }
-    static const int split = std::getenv("IMMESH_LIO_SPLIT") ? std::atoi(std::getenv("IMMESH_LIO_SPLIT")) : 1;
-    if (!split) {
-        for (int it = 0; it < h->P.max_iter; ++it) IM_LAUNCH(k_residual, g, RES_THREADS, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, it, 1);
         return IMMESH_OK;
     }
     const int gm = h->n_sm * 8;   // one resident wave of k_match blocks (__launch_bounds__(128, 8)); k_match picks the lanes per point from n

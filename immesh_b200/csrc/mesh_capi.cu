@@ -617,8 +617,6 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     } while (0)
     h->F.shard_rank = 0; h->F.shard_n = 1; h->F.x_cap = 0;
     h->F.work_rank = nullptr; h->F.tri_mark = nullptr;   // the per-frame path
-    h->bps = std::getenv("IMMESH_MESH_BPS") ? std::atoi(std::getenv("IMMESH_MESH_BPS")) : 3;
-    h->dilate_bps = std::getenv("IMMESH_DILATE_BPS") ? std::atoi(std::getenv("IMMESH_DILATE_BPS")) : h->bps;
     // dilated sets up to warp_nmax vertices are triangulated by one warp each (side stream), larger ones by a thread block each
     // (main stream, concurrently): the split balances the two kernels' longest serial insertion chains
     h->warp_nmax = std::getenv("IMMESH_WARP_NMAX") ? std::atoi(std::getenv("IMMESH_WARP_NMAX")) : IM_WARP_NMAX;
@@ -640,7 +638,7 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
-    IM_CREATE_M(cudaStreamCreateWithPriority(&h->stream, cudaStreamNonBlocking, im_stream_priority("IMMESH_MESH_PRIO")));
+    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     for (auto& e : h->ev) IM_CREATE_M(cudaEventCreate(&e));
     MeshDev& M = h->M;
     M.max_v = max_v;
@@ -731,8 +729,8 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     IM_CREATE_M(cudaFuncSetAttribute(k_voxel_mesh<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<1024>)));
     IM_CREATE_M(cudaFuncSetAttribute(k_voxel_tri_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * sizeof(MeshWarpSmem<128>))));
     IM_CREATE_M(cudaFuncSetAttribute(k_voxel_mesh<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<256>)));
-    IM_CREATE_M(cudaStreamCreateWithPriority(&h->stream2, cudaStreamNonBlocking, im_stream_priority("IMMESH_MESH_PRIO")));
-    IM_CREATE_M(cudaStreamCreateWithPriority(&h->stream3, cudaStreamNonBlocking, im_stream_priority("IMMESH_MESH_PRIO")));
+    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
+    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream3, cudaStreamNonBlocking));
     IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream_up, cudaStreamNonBlocking));
     for (int i = 0; i < IM_SLOTS; ++i) IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_up[i], cudaEventDisableTiming));
     IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
@@ -776,6 +774,9 @@ static int mesh_grid(const immesh_mesh* h, int n, int threads, int waves = 8) {
     if (g > h->n_sm * waves) g = h->n_sm * waves;
     return g < 1 ? 1 : g;
 }
+// resident blocks per SM of the persistent per-voxel kernels (headroom for the kernels on the other streams)
+#define MESH_TRI_BPS 3      // k_voxel_tri_warp, k_voxel_mesh<256>
+#define MESH_DILATE_BPS 3   // k_voxel_dilate
 
 // transformLidar of the full-resolution scan with the converged state (ImMesh_mesh_reconstruction.cpp:413 ->
 // voxel_mapping_common.cpp:709-726): p_w = (float)( R (R_ext p + t_ext) + t ).  First kernel of a frame handed over by the
@@ -1248,7 +1249,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         IM_LAUNCH(k_cand_place, g_cand, 128, 0, st, h->M, F);
         IM_LAUNCH(k_voxel_select, g_cand, 128, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[2], st);
-        IM_LAUNCH(k_voxel_dilate, h->n_sm * h->dilate_bps, 128, 0, st, h->M, P, F);
+        IM_LAUNCH(k_voxel_dilate, h->n_sm * MESH_DILATE_BPS, 128, 0, st, h->M, P, F);
         if (F.shard_n > 1 && h->win.ok) {   // smoothed positions of the other ranks' voxels, pushed into their windows
             IM_LAUNCH(k_xpush, h->n_sm, 256, 0, st, h->M, F, (const unsigned char*)h->d_seg1, 0, pe, h->d_xdone);
             IM_LAUNCH(k_apply_smooth, h->n_sm * 2, 256, 0, st, h->M, F, (const unsigned char*)h->d_recv1, h->seg1_bytes, pe);
@@ -1262,11 +1263,11 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         cudaEventRecord(h->ev_fork, st);
         cudaStreamWaitEvent(h->stream2, h->ev_fork, 0);
         cudaStreamWaitEvent(h->stream3, h->ev_fork, 0);
-        IM_LAUNCH(k_voxel_tri_warp, h->n_sm * h->bps, 128, 4 * sizeof(MeshWarpSmem<128>), h->stream2, h->M, P, F, h->warp_nmax);
+        IM_LAUNCH(k_voxel_tri_warp, h->n_sm * MESH_TRI_BPS, 128, 4 * sizeof(MeshWarpSmem<128>), h->stream2, h->M, P, F, h->warp_nmax);
         cudaEventRecord(h->ev_join, h->stream2);
         IM_LAUNCH(k_pull_vertices, h->n_sm * 8, 128, 0, h->stream3, h->M, P, F);   // incidence-list walk: only needs the dilation
         cudaEventRecord(h->ev_join3, h->stream3);
-        IM_LAUNCH((k_voxel_mesh<256>), h->n_sm * h->bps, 128, sizeof(MeshSmem<256>), st, h->M, P, F, h->warp_nmax, 1);
+        IM_LAUNCH((k_voxel_mesh<256>), h->n_sm * MESH_TRI_BPS, 128, sizeof(MeshSmem<256>), st, h->M, P, F, h->warp_nmax, 1);
         cudaStreamWaitEvent(st, h->ev_join, 0);
         cudaStreamWaitEvent(st, h->ev_join3, 0);
         IM_LAUNCH((k_voxel_mesh<1024>), h->n_sm * 2, 128, sizeof(MeshSmem<1024>), st, h->M, P, F, 256, 0);
@@ -1929,22 +1930,22 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     for (int b = 0; b < nbat; ++b) {
         IM_LAUNCH(k_bat_reset, 1, 32, 0, st, h->M, F, 0);
         IM_LAUNCH(k_bat_fill, g_fill, 128, 0, st, h->M, F, (const int*)h->b_sel, order, b * V, std::min(nsel, (b + 1) * V), h->b_rank);
-        IM_LAUNCH(k_voxel_dilate, h->n_sm * h->dilate_bps, 128, 0, st, h->M, P, F);
+        IM_LAUNCH(k_voxel_dilate, h->n_sm * MESH_DILATE_BPS, 128, 0, st, h->M, P, F);
     }
     // ---- pass 2: the dilation lists again (the smoothing reads raw positions: the re-store writes the same bits), triangulation,
     // pull + commit against the pre-frame store, the batch's additions pushed at once
     for (int b = 0; b < nbat; ++b) {
         IM_LAUNCH(k_bat_reset, h->n_sm * 8, 256, 0, st, h->M, F, 1);
         IM_LAUNCH(k_bat_fill, g_fill, 128, 0, st, h->M, F, (const int*)h->b_sel, order, b * V, std::min(nsel, (b + 1) * V), h->b_rank);
-        IM_LAUNCH(k_voxel_dilate, h->n_sm * h->dilate_bps, 128, 0, st, h->M, P, F);
+        IM_LAUNCH(k_voxel_dilate, h->n_sm * MESH_DILATE_BPS, 128, 0, st, h->M, P, F);
         IM_CUDA(cudaEventRecord(h->ev_fork, st));
         IM_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
         IM_CUDA(cudaStreamWaitEvent(h->stream3, h->ev_fork, 0));
-        IM_LAUNCH(k_voxel_tri_warp, h->n_sm * h->bps, 128, 4 * sizeof(MeshWarpSmem<128>), h->stream2, h->M, P, F, h->warp_nmax);
+        IM_LAUNCH(k_voxel_tri_warp, h->n_sm * MESH_TRI_BPS, 128, 4 * sizeof(MeshWarpSmem<128>), h->stream2, h->M, P, F, h->warp_nmax);
         IM_CUDA(cudaEventRecord(h->ev_join, h->stream2));
         IM_LAUNCH(k_pull_vertices, h->n_sm * 8, 128, 0, h->stream3, h->M, P, F);
         IM_CUDA(cudaEventRecord(h->ev_join3, h->stream3));
-        IM_LAUNCH((k_voxel_mesh<256>), h->n_sm * h->bps, 128, sizeof(MeshSmem<256>), st, h->M, P, F, h->warp_nmax, 1);
+        IM_LAUNCH((k_voxel_mesh<256>), h->n_sm * MESH_TRI_BPS, 128, sizeof(MeshSmem<256>), st, h->M, P, F, h->warp_nmax, 1);
         IM_CUDA(cudaStreamWaitEvent(st, h->ev_join, 0));
         IM_CUDA(cudaStreamWaitEvent(st, h->ev_join3, 0));
         IM_LAUNCH((k_voxel_mesh<1024>), h->n_sm * 2, 128, sizeof(MeshSmem<1024>), st, h->M, P, F, 256, 0);

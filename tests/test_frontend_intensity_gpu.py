@@ -5,9 +5,6 @@ state, map, effect rows, mesh; immesh_lio_frontend_cloud against the oracle's pu
 the validity, capacity and argument rules."""
 import ctypes as C
 import dataclasses
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -20,7 +17,6 @@ from lio_common import init_velocity
 from scan_pub_common import ScanPubOracle
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_CAPACITY = -1, -3
 MESH_CFG = api.MeshConfig(max_vertices=1 << 19, max_triangles=1 << 20, max_voxels=1 << 17, max_frame_points=1 << 17)
 RAW_CFG = dataclasses.replace(api.VELODYNE, calib_laser=1)
@@ -62,17 +58,6 @@ def test_filter_i_edge_cases(cuda_lib):
     out = check_filter_i(vg, wide, inten, 0.01, 5, 4, True)                   # leaf too small: output = input, intensity included
     assert vg.leaf_too_small and np.array_equal(out[:, 3], inten)
     run_filter_i_cases(cuda_lib)
-
-
-def test_filter_i_thread_per_run_in_own_process():
-    """IMMESH_VG_WARP_CENTROID=0 (read when a handle is created): the intensity sums of k_vg_centroid's thread-per-run loop"""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "from immesh_b200 import api\n"
-            "from frontend_intensity_common import run_filter_i_cases\n"
-            "run_filter_i_cases(api.load_library())\n"
-            "print('thread-per-run ok')\n") % (ROOT, os.path.join(ROOT, "tests"))
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env={**os.environ, "IMMESH_VG_WARP_CENTROID": "0"}, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "thread-per-run ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
 
 
 # ---- the raw chain (velodyne.yaml with calib_laser, HDL-64 stream)

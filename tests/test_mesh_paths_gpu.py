@@ -2,10 +2,6 @@
 the path table are in tests/mesh_scenes.py and test_mesh_paths_emu.py; on the device the warp kernel's one_pass boundary search
 runs for every insertion whose cavity has at most 10 triangles), the capacity errors, the run-time knobs that select other code
 (INTEGRATION.md), and immesh_knn at its largest k."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
@@ -15,7 +11,6 @@ from mesh_common import SMALL, run_mesh_parity, run_scene_parity
 from oracle_api import OracleMesh
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SCENES = ms.path_scenes()
 
 
@@ -57,24 +52,6 @@ def test_knob_graph_off(cuda_lib, monkeypatch):
     import test_mesh_gpu
     monkeypatch.setenv("IMMESH_GRAPH", "0")
     test_mesh_gpu.test_pipelined_equals_sequential(cuda_lib)
-
-
-def test_knob_voxelgrid_block_centroid(cuda_lib, monkeypatch):
-    """IMMESH_VG_WARP_CENTROID=0: the VoxelGrid centroids are summed by the block-level code"""
-    import test_frontend_gpu
-    monkeypatch.setenv("IMMESH_VG_WARP_CENTROID", "0")
-    test_frontend_gpu.test_edge_cases(cuda_lib)
-
-
-def test_knob_lio_split_off():
-    """IMMESH_LIO_SPLIT=0 (read once per process): the fused k_residual instead of k_match + k_terms, in a fresh process"""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "from immesh_b200 import api\n"
-            "from lio_common import run_stream_parity\n"
-            "s = run_stream_parity(api.load_library(), 'avia', api.AVIA, n_scans=4, seed=3)\n"
-            "print('split0 ok', s[-1]['n_match'])\n") % (ROOT, os.path.join(ROOT, "tests"))
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env={**os.environ, "IMMESH_LIO_SPLIT": "0"}, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "split0 ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
 
 
 # ---------------------------------------------------------------- kNN at KNN_KMAX

@@ -1,13 +1,9 @@
 """GPU tier: immesh_lio_effect_cloud / immesh_lio_registered_cloud (publish_effect_world / publish_frame_world) through the C ABI
 against the oracle on every path that forms the IESKF weights: the staged calls, the fused step, the pipelined graph-replayed step
-and its direct launches, IMMESH_LIO_SPLIT=0, k_match at 8 and at 1 lane per point, the raw device chain; the dense cloud from the
-device (the calibrated input of the raw chain, the IMU chain's [n][4] output); the capacity contract, the validity rules and an
-empty scan."""
+and its direct launches, k_match at 8 and at 1 lane per point, the raw device chain; the dense cloud from the device (the
+calibrated input of the raw chain, the IMU chain's [n][4] output); the capacity contract, the validity rules and an empty scan."""
 import ctypes as C
 import dataclasses
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -18,7 +14,6 @@ from lio_common import init_velocity
 from scan_pub_common import ScanPubOracle, run_scan_pub_parity
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_INVALID, E_CAPACITY = -1, -3
 
 
@@ -39,18 +34,6 @@ def test_pipelined_graph_path(cuda_lib):
 def test_pipelined_direct_launches(cuda_lib, monkeypatch):
     monkeypatch.setenv("IMMESH_GRAPH", "0")    # read when a handle is created
     run_scan_pub_parity(cuda_lib, "avia", api.AVIA, n_scans=6, seed=7, mode="async", oracle_checks=False)
-
-
-def test_lio_split0_in_own_process():
-    """IMMESH_LIO_SPLIT=0 (read once per process): the weights come from k_residual instead of k_terms"""
-    code = ("import sys; sys.path[:0] = [%r, %r]\n"
-            "from immesh_b200 import api\n"
-            "from scan_pub_common import run_scan_pub_parity\n"
-            "c = run_scan_pub_parity(api.load_library(), 'avia', api.AVIA, n_scans=5, seed=3, oracle_checks=False)\n"
-            "c += run_scan_pub_parity(api.load_library(), 'avia', api.AVIA, n_scans=4, seed=4, mode='async', oracle_checks=False)\n"
-            "print('split0 ok', min(c))\n") % (ROOT, os.path.join(ROOT, "tests"))
-    r = subprocess.run([sys.executable, "-c", code], cwd=ROOT, env={**os.environ, "IMMESH_LIO_SPLIT": "0"}, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "split0 ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
 
 
 def test_k_match_both_lane_modes(cuda_lib):
