@@ -148,6 +148,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_write_ply", [C.c_char_p, fp, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int]),
         ("immesh_write_pcd", [C.c_char_p, fp, C.c_int]),
         ("immesh_mesh_render_depth", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, dp, fp, fp, C.POINTER(C.c_int32), ip]),
+        ("immesh_mesh_reinforce_enable", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int]),
+        ("immesh_mesh_reinforce_pose", [vp, dp, dp]),
+        ("immesh_mesh_reinforced_cloud", [vp, fp, fp, C.POINTER(C.c_int32), C.c_int, ip, dp]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
         ("immesh_mesh_push_frame_batched", [vp, vp, C.c_int64, C.c_int, dp, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud_batched", [vp, vp, vp, C.c_int64, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
@@ -193,6 +196,13 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         lib.immesh_version.restype = C.c_char_p
     _lib_cache[path] = lib
     return lib
+
+
+def reinforce_intrinsics(width=640, height=480, focus=400.0):
+    """Cam_view::set_gl_projection (openGL_camera_view.cpp:83-101): the width rounded up to a multiple of 4, then
+    m_camera_intrinsic = [focus 0 w/2; 0 focus h/2] with integer halves; focus 400 for the reinforcement camera (ImMesh_node.cpp:291)."""
+    w = width + (4 - width % 4) % 4
+    return (float(focus), float(focus), float(w // 2), float(height // 2))
 
 
 def _f32(a):
@@ -613,6 +623,42 @@ class Mesh:
                                                            depth.ctypes.data_as(C.POINTER(C.c_float)), pts.ctypes.data_as(C.POINTER(C.c_float)),
                                                            pix.ctypes.data_as(C.POINTER(C.c_int32)), C.byref(n)), "mesh_render_depth")
         return depth, pts[:n.value].copy(), pix[:n.value].copy()
+
+    def reinforce_enable(self, intrinsics=None, width=640, height=480, z_near=0.1, z_far=1500.0, win=1):
+        """Queue the LiDAR point-cloud reinforcement behind every frame (intrinsics None: the reference's camera, reinforce_intrinsics)."""
+        if intrinsics is None:
+            intrinsics = reinforce_intrinsics(width, height)
+        K = np.ascontiguousarray(intrinsics, dtype=np.float64)
+        self._rf_shape = (height, width)
+        _check(self.lib, self.lib.immesh_mesh_reinforce_enable(self._h, K.ctypes.data_as(C.POINTER(C.c_double)), width, height, z_near, z_far, win), "mesh_reinforce_enable")
+
+    def reinforce_disable(self):
+        _check(self.lib, self.lib.immesh_mesh_reinforce_enable(self._h, None, 0, 0, 0.0, 0.0, 0), "mesh_reinforce_enable")
+
+    def reinforce_pose(self, cam_R=None, cam_t=None):
+        """The caller's camera pose from the next frame on (None: back to the pose bound to the sensor)."""
+        if cam_R is None:
+            _check(self.lib, self.lib.immesh_mesh_reinforce_pose(self._h, None, None), "mesh_reinforce_pose")
+            return
+        R = np.ascontiguousarray(cam_R, dtype=np.float64).reshape(9)
+        t = np.ascontiguousarray(cam_t, dtype=np.float64).reshape(3)
+        dp = C.POINTER(C.c_double)
+        _check(self.lib, self.lib.immesh_mesh_reinforce_pose(self._h, R.ctypes.data_as(dp), t.ctypes.data_as(dp)), "mesh_reinforce_pose")
+
+    def reinforced_cloud(self):
+        """(depth float32[h,w], points float32[n,3], pixel int32[n], cam_R float64[3,3], cam_t float64[3]) of the newest queued frame."""
+        n = C.c_int(0)
+        pose = np.zeros(12)
+        dp = C.POINTER(C.c_double)
+        rc = self.lib.immesh_mesh_reinforced_cloud(self._h, None, None, None, 0, C.byref(n), pose.ctypes.data_as(dp))
+        if rc not in (0, -3):
+            _check(self.lib, rc, "mesh_reinforced_cloud")
+        depth = np.zeros(self._rf_shape, dtype=np.float32)
+        pts = np.zeros((max(n.value, 1), 3), dtype=np.float32)
+        pix = np.zeros(max(n.value, 1), dtype=np.int32)
+        _check(self.lib, self.lib.immesh_mesh_reinforced_cloud(self._h, depth.ctypes.data_as(C.POINTER(C.c_float)), pts.ctypes.data_as(C.POINTER(C.c_float)),
+                                                               pix.ctypes.data_as(C.POINTER(C.c_int32)), n.value, C.byref(n), pose.ctypes.data_as(dp)), "mesh_reinforced_cloud")
+        return depth, pts[:n.value].copy(), pix[:n.value].copy(), pose[:9].reshape(3, 3).copy(), pose[9:].copy()
 
     def smooth_all(self, smooth_factor=0.1, knn=20):
         """smooth_all_pts: returns the smoothed positions float64[nv,3] (and stores them as the vertices' smoothed positions)."""

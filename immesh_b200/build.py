@@ -147,6 +147,14 @@ def build_imu_chain(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "imu_chain", "emu_imu_chain.cpp"), EMU_IMU_CHAIN, force)
 
 
+EMU_REINFORCE = os.path.join(_ROOT, "tests", "reinforce", "libimmesh_emu_reinforce.so")
+
+
+def build_reinforce(force=False):
+    """tests/reinforce: the reinforcement's camera pose and tiled rasteriser bodies (immesh_b200/csrc/reinforce.cuh), built for the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "reinforce", "emu_reinforce.cpp"), EMU_REINFORCE, force)
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -165,6 +173,7 @@ def build_all(force=False):
     build_batched(force)
     build_growth(force)
     build_imu_chain(force)
+    build_reinforce(force)
     build_ref()
 
 

@@ -8,6 +8,7 @@
 #include "lio_core.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
+#include "reinforce.cuh"
 
 using immesh::LioParams; using immesh::VoxelMapDev; using immesh::ScanBuf; using immesh::LioCtrl;
 using immesh::MeshParams; using immesh::MeshDev; using immesh::FrameBuf; using immesh::FramePose;
@@ -157,4 +158,21 @@ struct immesh_mesh {
     int known[32] = {};           // counters (MeshDev::cnt layout) of the last frame known to have finished
     int known_frame = 0;          // its frame number (0: the empty mesh at create)
     int max_step_tris = 0;        // largest triangle allocation between two noted frames (noted oldest first)
+    // LiDAR point-cloud reinforcement (immesh_mesh_reinforce_enable)
+    double (*cam_ring)[12] = nullptr;   // [IM_RF_RING] rot_end, pos_end of the frames handed over by the localization handle
+    int* cam_ring_frame = nullptr;      // [IM_RF_RING] frame number each ring entry belongs to (0: none)
+    struct Reinforce {
+        int on = 0, win = 1, ntiles = 0, nb = 0, bin_cap = 0;
+        int last_frame = 0;               // newest frame queued with the reinforcement (0: none since enable)
+        int explicit_pose = 0;            // immesh_mesh_reinforce_pose: the caller's pose from the next frame on
+        double R[9] = {}, t[3] = {};
+        immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
+        std::vector<void*> bufs;          // device buffers below, freed by disable / destroy
+        void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
+        void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
+        immesh::DepthCam* cam = nullptr;
+        int *tile_cnt = nullptr, *tile_off = nullptr, *bin = nullptr, *misc = nullptr, *blk = nullptr, *blk_off = nullptr;
+        unsigned int* depth_bits = nullptr;
+        float* depth[2] = {}; float* pts[2] = {}; int* pix[2] = {}; int* n[2] = {}; double* pose[2] = {};
+    } rf;
 };

@@ -16,6 +16,7 @@
 #include "handles.hpp"
 #include "pool_growth.cuh"
 #include "nccl_api.hpp"
+#include "reinforce.cuh"
 
 using namespace immesh;
 
@@ -319,17 +320,8 @@ __global__ void __launch_bounds__(128) k_region_keys(MeshDev M, int n_alloc, dou
 // camera frame x right / y down / z forward (the frame unproject_point inverts: world = R diag(1,-1,-1) p + t), pixel (u, v) =
 // (fx x / z + cx, fy y / z + cy), samples at integer pixel coordinates, a sample is covered when the three edge functions have one
 // sign (zero included), depth interpolated perspective-correctly (1/z is affine in the image), nearest surface wins (atomicMin on the
-// float bits).  Triangles with a vertex outside (z_near, z_far) are skipped (GL would clip them).
-struct DepthCam { double fx, fy, cx, cy, z_near, z_far; double R[9], t[3]; int w, h; };
-__device__ __forceinline__ void depth_project(const DepthCam& C, const float4& p, double* u, double* v, double* z) {
-    const double d[3] = {(double)p.x - C.t[0], (double)p.y - C.t[1], (double)p.z - C.t[2]};
-    const double xc = (C.R[0] * d[0] + C.R[3] * d[1]) + C.R[6] * d[2];     // R^T d
-    const double yc = -((C.R[1] * d[0] + C.R[4] * d[1]) + C.R[7] * d[2]);
-    const double zc = -((C.R[2] * d[0] + C.R[5] * d[1]) + C.R[8] * d[2]);
-    *z = zc;
-    *u = C.fx * xc / zc + C.cx;
-    *v = C.fy * yc / zc + C.cy;
-}
+// float bits).  Triangles with a vertex outside (z_near, z_far) are skipped (GL would clip them).  DepthCam, the triangle set-up and
+// the sample are in reinforce.cuh; k_depth_raster (one thread per triangle) is the reference the tiled rasteriser below is tested against.
 __global__ void __launch_bounds__(128) k_depth_clear(unsigned int* depth, int n) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) depth[i] = 0x7f800000u;   // +inf
 }
@@ -337,26 +329,12 @@ __global__ void __launch_bounds__(128) k_depth_raster(MeshDev M, int n_alloc, De
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
-        double u0, v0, z0, u1, v1, z1, u2, v2, z2;
-        depth_project(C, M.vpos[r.x], &u0, &v0, &z0);
-        depth_project(C, M.vpos[r.y], &u1, &v1, &z1);
-        depth_project(C, M.vpos[r.z], &u2, &v2, &z2);
-        if (!(z0 > C.z_near && z0 < C.z_far && z1 > C.z_near && z1 < C.z_far && z2 > C.z_near && z2 < C.z_far)) continue;
-        const double area = (u1 - u0) * (v2 - v0) - (v1 - v0) * (u2 - u0);
-        if (area == 0.0) continue;
-        const int x_lo = max(0, (int)ceil(fmin(u0, fmin(u1, u2)))), x_hi = min(C.w - 1, (int)floor(fmax(u0, fmax(u1, u2))));
-        const int y_lo = max(0, (int)ceil(fmin(v0, fmin(v1, v2)))), y_hi = min(C.h - 1, (int)floor(fmax(v0, fmax(v1, v2))));
-        const double iz0 = 1.0 / z0, iz1 = 1.0 / z1, iz2 = 1.0 / z2;
-        for (int y = y_lo; y <= y_hi; ++y)
-            for (int x = x_lo; x <= x_hi; ++x) {
-                const double px = (double)x, py = (double)y;
-                const double e0 = (u2 - u1) * (py - v1) - (v2 - v1) * (px - u1);   // weight of vertex 0
-                const double e1 = (u0 - u2) * (py - v2) - (v0 - v2) * (px - u2);
-                const double e2 = (u1 - u0) * (py - v0) - (v1 - v0) * (px - u0);
-                if (!((e0 >= 0 && e1 >= 0 && e2 >= 0) || (e0 <= 0 && e1 <= 0 && e2 <= 0))) continue;
-                const double iz = ((e0 * iz0 + e1 * iz1) + e2 * iz2) / area;
-                const float zf = (float)(1.0 / iz);
-                if (zf > 0.f) atomicMin(&depth[(size_t)y * C.w + x], __float_as_uint(zf));
+        DepthTri T;
+        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
+        for (int y = T.y_lo; y <= T.y_hi; ++y)
+            for (int x = T.x_lo; x <= T.x_hi; ++x) {
+                float zf;
+                if (depth_sample(T, x, y, &zf)) atomicMin(&depth[(size_t)y * C.w + x], __float_as_uint(zf));
             }
     }
 }
@@ -365,18 +343,176 @@ __global__ void __launch_bounds__(128) k_depth_finish(DepthCam C, const unsigned
     const int n = C.w * C.h;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float val = __uint_as_float(depth[i]);
-        const bool ok = (double)val < C.z_far * 0.99;
+        const bool ok = depth_valid(C, val);
         out_depth[i] = ok ? val : -1.0f;
         if (ok && out_pts) {
-            const int x = i % C.w, y = i / C.w;
-            // m_camera_intrinsic_inv * (x, y, 1), scaled to depth val, GL camera axes (x, -y, -z), then R p + t
-            const double sx = ((double)x - C.cx) / C.fx, sy = ((double)y - C.cy) / C.fy;
-            const double g[3] = {sx * (double)val, -(sy * (double)val), -(double)val};
             const int k = atomicAdd(n_pts, 1);
-            for (int a = 0; a < 3; ++a) out_pts[(size_t)k * 4 + a] = (float)(((C.R[a * 3 + 0] * g[0] + C.R[a * 3 + 1] * g[1]) + C.R[a * 3 + 2] * g[2]) + C.t[a]);
+            depth_unproject(C, i % C.w, i / C.w, val, out_pts + (size_t)k * 4);
             out_pts[(size_t)k * 4 + 3] = __int_as_float(i);   // the pixel the point came from (the order of the list is arbitrary)
         }
     }
+}
+
+// ---- the queued reinforcement (immesh_mesh_reinforce_enable): behind every frame, on the mesh stream and inside its graph, the
+// camera pose (k_rf_pose), the tiled rasteriser (k_rf_count -> k_rf_scan -> k_rf_fill -> k_rf_tile) and the compaction of the valid
+// pixels in ascending pixel order (k_rf_fcount -> k_rf_scan -> k_rf_emit) into result buffer (frame & 1).
+struct RfDyn { int mode, pad; double R[9], t[3]; };   // per frame: mode 1 = the caller's pose (immesh_mesh_reinforce_pose)
+struct RfOut { float* depth; float* pts; int* pix; int* n; double* pose; };
+// one block: the frame's camera (sensor-bound or the caller's), the tile counters cleared
+__global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const int* ring_frame, const FrameDyn* dyn, const RfDyn* rd, int win, DepthCam base,
+                                                 DepthCam* cam, RfOut o0, RfOut o1, int* tile_cnt, int ntiles) {
+    for (int i = threadIdx.x; i < ntiles; i += blockDim.x) tile_cnt[i] = 0;
+    if (threadIdx.x != 0) return;
+    const int frame = dyn->frame;
+    double R[9], t[3];
+    if (rd->mode == 1) {
+        for (int i = 0; i < 9; ++i) R[i] = rd->R[i];
+        for (int i = 0; i < 3; ++i) t[i] = rd->t[i];
+    } else {
+        rf_avr_pose(ring, ring_frame, frame, win, R, t);
+    }
+    for (int i = 0; i < 9; ++i) base.R[i] = R[i];
+    for (int i = 0; i < 3; ++i) base.t[i] = t[i];
+    *cam = base;
+    double* pose = (frame & 1) ? o1.pose : o0.pose;
+    for (int i = 0; i < 9; ++i) pose[i] = R[i];
+    for (int i = 0; i < 3; ++i) pose[9 + i] = t[i];
+}
+// the screen tiles a triangle's pixel box touches
+__device__ __forceinline__ void rf_tiles(const DepthTri& T, int* tx0, int* tx1, int* ty0, int* ty1) {
+    *tx0 = T.x_lo / IM_RT_TILE; *tx1 = T.x_hi / IM_RT_TILE; *ty0 = T.y_lo / IM_RT_TILE; *ty1 = T.y_hi / IM_RT_TILE;
+}
+// count pass: bin entries per tile
+__global__ void __launch_bounds__(128) k_rf_count(MeshDev M, const DepthCam* cam, int* tile_cnt) {
+    const DepthCam C = *cam;
+    const int n_alloc = min(M.cnt[1], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[t];
+        if (!r.w) continue;
+        DepthTri T;
+        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
+        int tx0, tx1, ty0, ty1;
+        rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
+        for (int ty = ty0; ty <= ty1; ++ty)
+            for (int tx = tx0; tx <= tx1; ++tx) atomicAdd(&tile_cnt[ty * ntx + tx], 1);
+    }
+}
+// one block: exclusive scan of cnt[0, n) into off[0, n] (off[n] = total), in one pass over contiguous chunks (as k_cand_scan);
+// cur (or null) gets a copy of the offsets, the fill cursors; misc[0] (or null) = total > cap, the bins' overflow flag
+__global__ void __launch_bounds__(1024) k_rf_scan(const int* cnt, int n, int* off, int* cur, int cap, int* misc) {
+    __shared__ int s_warp[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int per = (n + 1023) / 1024;
+    const int lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
+    int mine = 0;
+    for (int c = lo; c < hi; ++c) mine += cnt[c];
+    int v = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, v, o);
+        if (lane >= o) v += u;
+    }
+    if (lane == 31) s_warp[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+        int wv = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, wv, o);
+            if (lane >= o) wv += u;
+        }
+        s_warp[lane] = wv;
+    }
+    __syncthreads();
+    int run = (warp ? s_warp[warp - 1] : 0) + v - mine;
+    for (int c = lo; c < hi; ++c) {
+        const int k = cnt[c];
+        off[c] = run;
+        if (cur) cur[c] = run;
+        run += k;
+    }
+    if (threadIdx.x == 1023) {
+        off[n] = run;
+        if (misc) misc[0] = run > cap ? 1 : 0;
+    }
+}
+// fill pass: triangle slots into the bins (order inside a bin is free: the tile takes the minimum)
+__global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, const DepthCam* cam, int* cur, int* bin, const int* misc) {
+    if (misc[0]) return;
+    const DepthCam C = *cam;
+    const int n_alloc = min(M.cnt[1], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[t];
+        if (!r.w) continue;
+        DepthTri T;
+        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
+        int tx0, tx1, ty0, ty1;
+        rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
+        for (int ty = ty0; ty <= ty1; ++ty)
+            for (int tx = tx0; tx <= tx1; ++tx) bin[atomicAdd(&cur[ty * ntx + tx], 1)] = t;
+    }
+}
+// one block per tile, one thread per pixel: the bin's triangles are set up IM_RT_THREADS at a time into shared memory, each thread
+// keeps its pixel's nearest sample in a register and writes it once.  Bins over capacity (misc[0]): every triangle slot instead.
+__global__ void __launch_bounds__(IM_RT_THREADS) k_rf_tile(MeshDev M, const DepthCam* cam, const int* tile_off, const int* bin, const int* misc, unsigned int* depth) {
+    __shared__ DepthTri S[IM_RT_THREADS];
+    const DepthCam C = *cam;
+    const int ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    const int x = (blockIdx.x % ntx) * IM_RT_TILE + (int)(threadIdx.x % IM_RT_TILE), y = (blockIdx.x / ntx) * IM_RT_TILE + (int)(threadIdx.x / IM_RT_TILE);
+    const bool all = misc[0] != 0;
+    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[1], M.max_t) : tile_off[blockIdx.x + 1];
+    unsigned int acc = 0x7f800000u;   // +inf
+    for (int b = lo; b < hi; b += IM_RT_THREADS) {
+        const int i = b + (int)threadIdx.x;
+        bool ok = false;
+        if (i < hi) {
+            const int4 r = M.tri[all ? i : bin[i]];
+            ok = r.w && depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &S[threadIdx.x]);
+        }
+        if (!ok) { S[threadIdx.x].x_lo = 1; S[threadIdx.x].x_hi = 0; }   // an empty box
+        __syncthreads();
+        acc = rt_pixel_min(S, min(IM_RT_THREADS, hi - b), x, y, acc);
+        __syncthreads();
+    }
+    if (x < C.w && y < C.h) depth[(size_t)y * C.w + x] = acc;
+}
+#define RF_FIN 1024
+// valid pixels per block of RF_FIN consecutive pixels
+__global__ void __launch_bounds__(RF_FIN) k_rf_fcount(const DepthCam* cam, const unsigned int* depth, int* blk) {
+    const DepthCam C = *cam;
+    const int i = blockIdx.x * RF_FIN + threadIdx.x;
+    const int c = __syncthreads_count(i < C.w * C.h && depth_valid(C, __uint_as_float(depth[i])));
+    if (threadIdx.x == 0) blk[blockIdx.x] = c;
+}
+// depth image and the valid pixels' points in ascending pixel order: block offset + rank inside the block
+__global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const FrameDyn* dyn, const unsigned int* depth, const int* blk_off, int nb, RfOut o0, RfOut o1) {
+    __shared__ int s_warp[RF_FIN / 32];
+    const DepthCam C = *cam;
+    const RfOut o = (dyn->frame & 1) ? o1 : o0;
+    const int i = blockIdx.x * RF_FIN + threadIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const float val = i < C.w * C.h ? __uint_as_float(depth[i]) : 0.f;
+    const bool ok = i < C.w * C.h && depth_valid(C, val);
+    const unsigned int ball = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0) s_warp[warp] = __popc(ball);
+    __syncthreads();
+    if (warp == 0) {
+        const int mine = s_warp[lane];
+        int v = mine;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, v, d);
+            if (lane >= d) v += u;
+        }
+        s_warp[lane] = v - mine;   // exclusive
+    }
+    __syncthreads();
+    if (i < C.w * C.h) o.depth[i] = ok ? val : -1.0f;
+    if (ok) {
+        const int k = blk_off[blockIdx.x] + s_warp[warp] + __popc(ball & ((1u << lane) - 1u));
+        depth_unproject(C, i % C.w, i / C.w, val, o.pts + (size_t)k * 3);
+        o.pix[k] = i;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *o.n = blk_off[nb];
 }
 
 // ---- the viewer's region buffers (immesh_mesh_region_buffers, mesh_rec_display.cpp:78-137 + :220-258).  k_rb_select keys the live
@@ -724,6 +860,8 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     IM_CREATE_M(cudaMallocHost((void**)&h->h_fp, IM_SLOTS * sizeof(FramePose)));
     IM_CREATE_M(cudaMallocHost((void**)&h->h_dyn, IM_SLOTS * sizeof(FrameDyn)));
     IM_CREATE_M(mdev_alloc(h, &h->d_dyn, 1, 0));
+    IM_CREATE_M(mdev_alloc(h, &h->cam_ring, IM_RF_RING, 0));
+    IM_CREATE_M(mdev_alloc(h, &h->cam_ring_frame, IM_RF_RING, 0));
     F.dyn = h->d_dyn;
     F.epoch = 0;
     IM_CREATE_M(cudaFuncSetAttribute(k_voxel_mesh<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<1024>)));
@@ -751,6 +889,8 @@ int immesh_mesh_destroy(immesh_mesh_t* h) {
     if (h->nccl_comm && immesh::nccl().CommDestroy) immesh::nccl().CommDestroy(h->nccl_comm);
     for (void* p : h->allocs) cudaFree(p);
     for (void* p : h->rb_buf) if (p) cudaFree(p);
+    for (void* p : h->rf.bufs) cudaFree(p);
+    if (h->rf.h_rd) cudaFreeHost(h->rf.h_rd);
     if (h->h_pts) cudaFreeHost(h->h_pts);
     if (h->h_cnt) cudaFreeHost(h->h_cnt);
     if (h->h_fp) cudaFreeHost(h->h_fp);
@@ -782,8 +922,8 @@ static int mesh_grid(const immesh_mesh* h, int n, int threads, int waves = 8) {
 // voxel_mapping_common.cpp:709-726): p_w = (float)( R (R_ext p + t_ext) + t ).  First kernel of a frame handed over by the
 // localization handle: the pose is the one that scan converged to (LioCtrl::pose_ring, written by the last kernel of the
 // scan's sequence; the localization stream may already be working on later scans).  Block 0 also derives the frame's sensor
-// position + the origin of the flip-priority rank.
-__global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCtrl* ctrl, FrameBuf F_, double res) {
+// position + the origin of the flip-priority rank, and records the pose in the handle's camera ring (reinforce.cuh, rf_avr_pose).
+__global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCtrl* ctrl, FrameBuf F_, double res, double (*cam_ring)[12], int* cam_ring_frame) {
     __shared__ double s[12];
     const FrameDyn d = *F_.dyn;
     if (threadIdx.x < 12) s[threadIdx.x] = ctrl->pose_ring[d.pose_idx][threadIdx.x];
@@ -792,6 +932,10 @@ __global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCt
         const double t = s[9 + threadIdx.x];
         d.fp->pose_t[threadIdx.x] = t;
         d.fp->prio_origin[threadIdx.x] = (long long)floor(t / res) - 1024;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < 12) {
+        cam_ring[d.frame % IM_RF_RING][threadIdx.x] = s[threadIdx.x];
+        if (threadIdx.x == 0) cam_ring_frame[d.frame % IM_RF_RING] = d.frame;
     }
     const float* body = d.body;
     float* world = const_cast<float*>(d.pts);
@@ -1147,6 +1291,23 @@ static int mesh_grid_fixed(const immesh_mesh* h, long long n_cap, int threads, i
     if (g > (long long)h->n_sm * waves) g = (long long)h->n_sm * waves;
     return g < 1 ? 1 : (int)g;
 }
+static RfOut rf_out(const immesh_mesh* h, int b) { return RfOut{h->rf.depth[b], h->rf.pts[b], h->rf.pix[b], h->rf.n[b], h->rf.pose[b]}; }
+// the reinforcement of the frame just queued (fixed grids: every per-frame value is read on the device)
+static void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st) {
+    auto& r = h->rf;
+    IM_LAUNCH(k_rf_pose, 1, 256, 0, st, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame, (const FrameDyn*)h->d_dyn, (const RfDyn*)r.rd, r.win, r.base,
+              r.cam, rf_out(h, 0), rf_out(h, 1), r.tile_cnt, r.ntiles);
+    const int g = h->n_sm * 8;
+    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, (const DepthCam*)r.cam, r.tile_cnt);
+    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)r.tile_cnt, r.ntiles, r.tile_off, r.tile_cnt, r.bin_cap, r.misc);
+    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, (const DepthCam*)r.cam, r.tile_cnt, r.bin, (const int*)r.misc);
+    IM_LAUNCH(k_rf_tile, r.ntiles, IM_RT_THREADS, 0, st, h->M, (const DepthCam*)r.cam, (const int*)r.tile_off, (const int*)r.bin, (const int*)r.misc, r.depth_bits);
+    IM_LAUNCH(k_rf_fcount, r.nb, RF_FIN, 0, st, (const DepthCam*)r.cam, (const unsigned int*)r.depth_bits, r.blk);
+    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)r.blk, r.nb, r.blk_off, (int*)nullptr, 0, (int*)nullptr);
+    IM_LAUNCH(k_rf_emit, r.nb, RF_FIN, 0, st, (const DepthCam*)r.cam, (const FrameDyn*)h->d_dyn, (const unsigned int*)r.depth_bits, (const int*)r.blk_off, r.nb,
+              rf_out(h, 0), rf_out(h, 1));
+}
+
 // src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state.
 // Queues one frame (no host synchronisation except when both staging slots are still busy).  Host work per frame in the
 // pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D FrameDyn + one stream
@@ -1233,12 +1394,20 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         d.n = F.n; d.step = F.step; d.m = F.m; d.frame = F.frame; d.cmask = F.cmask; d.pose_idx = pose_idx; d.epoch = epoch;
         IM_CUDA(cudaMemcpyAsync(h->d_dyn, &d, sizeof(FrameDyn), cudaMemcpyHostToDevice, st));
     }
+    const bool rf_on = h->rf.on != 0;
+    if (rf_on) {   // the camera source of this frame
+        RfDyn* r = (RfDyn*)h->rf.h_rd + s;
+        r->mode = h->rf.explicit_pose;
+        for (int i = 0; i < 9; ++i) r->R[i] = h->rf.R[i];
+        for (int i = 0; i < 3; ++i) r->t[i] = h->rf.t[i];
+        IM_CUDA(cudaMemcpyAsync(h->rf.rd, r, sizeof(RfDyn), cudaMemcpyHostToDevice, st));
+    }
     // the frame's launch sequence (fixed grids: grid-stride loops over the counts the kernels read on the device)
     bool nccl_failed = false;
     const int g_pts = mesh_grid_fixed(h, h->max_frame_points, 128);
     const int g_cand = mesh_grid_fixed(h, std::min<long long>(h->max_frame_points, 2LL * P.append_target), 128);
     auto launch_frame = [&](bool timing) {
-        if (src_mode >= 2) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res);
+        if (src_mode >= 2) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
         IM_LAUNCH(k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[1], st);
         IM_LAUNCH(k_cand_init, g_cand, 128, 0, st, h->M, P, F);
@@ -1285,6 +1454,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         IM_LAUNCH(k_push_remove, h->n_sm * 2, 128, 0, st, h->M, F);
         IM_LAUNCH(k_push_add, h->n_sm * 2, 128, 0, st, h->M, F);
         IM_LAUNCH(k_frame_end, 1, 1, 0, st, h->M);
+        if (rf_on) mesh_reinforce_launch(h, st);
     };
     bool queued = false;
     if (graphed) {
@@ -1302,6 +1472,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     IM_CUDA(cudaEventRecord(h->ev_done[s], st));
     h->inflight[s] = 1;
     h->timed_last = queued ? 0 : 1;
+    if (rf_on) h->rf.last_frame = F.frame;
     return IMMESH_OK;
 }
 // drain the queue; returns the status of the frames harvested since the last call
@@ -1366,6 +1537,7 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (!h || !unique_id128 || nranks < 1 || rank < 0 || rank >= nranks) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (nranks == 1) { h->F.shard_rank = 0; h->F.shard_n = 1; return IMMESH_OK; }
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a mesh handle with automatic growth cannot be sharded (immesh_mesh_set_growth(h, 0) first)");
+    if (h->rf.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the reinforcement enabled cannot be sharded (immesh_mesh_reinforce_enable(h, NULL, ...) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -2048,6 +2220,87 @@ int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int wid
     }
     if (n_points) *n_points = np;
     cudaFree(d_depth); cudaFree(d_out); if (d_pts) cudaFree(d_pts); cudaFree(d_n);
+    return IMMESH_OK;
+}
+
+static void mesh_reinforce_free(immesh_mesh* h) {
+    for (void* p : h->rf.bufs) cudaFree(p);
+    if (h->rf.h_rd) cudaFreeHost(h->rf.h_rd);
+    h->rf = immesh_mesh::Reinforce();
+}
+int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, int win) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "reinforce_enable: a sharded mesh handle is not supported (the reinforcement runs on a single GPU)");
+    if (intrinsics) {
+        const double* K = intrinsics;
+        if (width < 1 || height < 1 || (long long)width * height > (1 << 26) || !(z_near > 0) || !(z_far > z_near) || !std::isfinite(z_far) || win < 1 ||
+            win > IM_RF_RING - 1 || !std::isfinite(K[0]) || !std::isfinite(K[1]) || !std::isfinite(K[2]) || !std::isfinite(K[3]) || K[0] == 0.0 || K[1] == 0.0)
+            return im_fail(IMMESH_E_INVALID, "reinforce_enable: bad argument (finite intrinsics with fx, fy != 0; 1 <= width * height <= 2^26; 0 < z_near < z_far; 1 <= win <= 63)");
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
+    h->graph.destroy();                          // the captured sequence changes
+    mesh_reinforce_free(h);
+    if (!intrinsics) return IMMESH_OK;
+    auto& r = h->rf;
+    DepthCam& C = r.base;
+    C.fx = intrinsics[0]; C.fy = intrinsics[1]; C.cx = intrinsics[2]; C.cy = intrinsics[3]; C.z_near = z_near; C.z_far = z_far;
+    C.w = width; C.h = height;
+    const size_t n = (size_t)width * height;
+    r.ntiles = ((width + IM_RT_TILE - 1) / IM_RT_TILE) * ((height + IM_RT_TILE - 1) / IM_RT_TILE);
+    r.nb = (int)((n + RF_FIN - 1) / RF_FIN);
+    r.bin_cap = std::max(1 << 22, 16 * r.ntiles);   // beyond it a frame's tiles walk every triangle slot (same image, slower)
+    r.win = win;
+    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
+        void* q = nullptr;
+        const cudaError_t e = cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(**p));
+        if (e == cudaSuccess) { r.bufs.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
+        return e;
+    };
+    RfDyn* rd = nullptr;
+    cudaError_t e = cudaSuccess;
+    auto step = [&](cudaError_t x) { if (e == cudaSuccess) e = x; };
+    step(alloc(&rd, 1)); step(alloc(&r.cam, 1));
+    step(alloc(&r.tile_cnt, (size_t)r.ntiles)); step(alloc(&r.tile_off, (size_t)r.ntiles + 1)); step(alloc(&r.bin, (size_t)r.bin_cap)); step(alloc(&r.misc, 4));
+    step(alloc(&r.blk, (size_t)r.nb)); step(alloc(&r.blk_off, (size_t)r.nb + 1)); step(alloc(&r.depth_bits, n));
+    for (int b = 0; b < 2; ++b) { step(alloc(&r.depth[b], n)); step(alloc(&r.pts[b], n * 3)); step(alloc(&r.pix[b], n)); step(alloc(&r.n[b], 1)); step(alloc(&r.pose[b], 12)); }
+    step(cudaMallocHost(&r.h_rd, IM_SLOTS * sizeof(RfDyn)));
+    if (e != cudaSuccess) {
+        mesh_reinforce_free(h);
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "reinforce_enable: allocation of the reinforcement buffers failed");
+    }
+    std::memset(r.h_rd, 0, IM_SLOTS * sizeof(RfDyn));
+    r.rd = rd;
+    r.on = 1;
+    return IMMESH_OK;
+}
+int immesh_mesh_reinforce_pose(immesh_mesh_t* h, const double* cam_R, const double* cam_t) {
+    if (!h || (!cam_R) != (!cam_t)) return im_fail(IMMESH_E_INVALID, "bad argument (cam_R and cam_t both given or both NULL)");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "reinforce_pose: a sharded mesh handle is not supported");
+    h->rf.explicit_pose = cam_R ? 1 : 0;
+    for (int i = 0; i < 9; ++i) h->rf.R[i] = cam_R ? cam_R[i] : 0.0;
+    for (int i = 0; i < 3; ++i) h->rf.t[i] = cam_t ? cam_t[i] : 0.0;
+    return IMMESH_OK;
+}
+int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth, float* points, int32_t* point_pixel, int cap, int* n_out, double* pose_out) {
+    if (!h || !n_out || cap < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    *n_out = 0;
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "reinforced_cloud: a sharded mesh handle is not supported");
+    if (!h->rf.on) return im_fail(IMMESH_E_INVALID, "reinforced_cloud: the reinforcement is not enabled (immesh_mesh_reinforce_enable)");
+    if (!h->rf.last_frame) return im_fail(IMMESH_E_INVALID, "reinforced_cloud: no frame has been queued since immesh_mesh_reinforce_enable");
+    // the newest frame's result; the next queued frame writes the other buffer, so these copies (legacy stream) do not wait for it
+    const int f = h->rf.last_frame, b = f & 1;
+    IM_CUDA(cudaEventSynchronize(h->ev_done[f & (IM_SLOTS - 1)]));
+    int n = 0;
+    double pose[12];
+    IM_CUDA(cudaMemcpy(&n, h->rf.n[b], sizeof(int), cudaMemcpyDeviceToHost));
+    IM_CUDA(cudaMemcpy(pose, h->rf.pose[b], sizeof(pose), cudaMemcpyDeviceToHost));
+    *n_out = n;
+    if (n > cap) return im_fail(IMMESH_E_CAPACITY, "reinforced_cloud: more points than cap (*n_out holds the number needed; nothing was written)");
+    if (depth) IM_CUDA(cudaMemcpy(depth, h->rf.depth[b], (size_t)h->rf.base.w * h->rf.base.h * sizeof(float), cudaMemcpyDeviceToHost));
+    if (points && n > 0) IM_CUDA(cudaMemcpy(points, h->rf.pts[b], (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    if (point_pixel && n > 0) IM_CUDA(cudaMemcpy(point_pixel, h->rf.pix[b], (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+    if (pose_out) std::memcpy(pose_out, pose, sizeof(pose));
     return IMMESH_OK;
 }
 

@@ -366,6 +366,40 @@ int immesh_mesh_reconstruct_from_pointcloud_batched(immesh_mesh_t* h, immesh_vox
  * the three edge functions share a sign, 1/z interpolated affinely, triangles with a vertex outside (z_near, z_far) skipped. */
 int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics /*[4]*/, int width, int height, double z_near, double z_far,
                              const double* cam_R /*[9]*/, const double* cam_t /*[3]*/, float* depth, float* points, int32_t* point_pixel, int* n_points);
+/* The LiDAR point-cloud reinforcement with the depth camera bound to the sensor (src/ImMesh_node.cpp:302-329, g_if_draw_depth with
+ * g_if_depth_bind_cam), queued behind every mesh frame.  Per frame the reference takes the camera pose from the last meshed frames
+ * (get_last_avr_pose, :169-206), rasterises the live mesh into the depth camera (draw_triangle, Cam_view::read_depth) and unprojects
+ * every valid pixel (convert_depth_buffer_to_truth_depth + unproject_point, src/tools/openGL_libs/openGL_camera_view.cpp:316-418); the
+ * points are drawn beside the current scan (display_reinforced_LiDAR_pts, src/meshing/mesh_rec_display.cpp:178-196).
+ *   immesh_mesh_reinforce_enable: allocates the buffers once for the image and from then on every frame of immesh_mesh_push_frame,
+ *     _dev, _from_lio, _from_lio_async (and reconstruct_from_pointcloud) queues, on the mesh stream right behind the frame and inside
+ *     its captured graph, the camera pose, the depth image of the mesh as the frame left it and its points -- no host
+ *     synchronisation, no allocation.  The batched frames (push_frame_batched) are not followed.  intrinsics = NULL turns it off and
+ *     frees the buffers.  Either call drains the frames in flight.  Bad intrinsics (non-finite, fx or fy = 0), image size outside
+ *     [1, 2^26] pixels, z range not 0 < z_near < z_far < inf, win outside [1, 63], or a sharded handle: IMMESH_E_INVALID.
+ *   The reference's camera (ImMesh_node.cpp:285-293): 640 x 480, m_camera_focus = 400, the z range of the GL camera (z_near 0.1,
+ *     z_far 1500), win_ssd = 1.  Cam_view::set_gl_projection (openGL_camera_view.cpp:83-101) rounds the width up to a multiple of 4
+ *     and sets m_camera_intrinsic = [focus 0 w/2; 0 focus h/2; 0 0 1] with integer halves: intrinsics = (focus, focus, w / 2, h / 2),
+ *     (400, 400, 320, 240) for the defaults.
+ *   Camera pose of frame n (the handle's frames counted from 1; the reference's current frame is n - 1): the frames
+ *     [max(1, n - win), n) that were handed over by the localization handle (they recorded rot_end, pos_end of the pose they were
+ *     transformed with) give q_first exp(mean_i log(q_first^-1 q_i)) * lidar_frame_to_camera_frame = [0 0 -1; -1 0 0; 0 1 0] (quaternions
+ *     from the rotation matrices as Eigen::Quaterniond does it, Sophus SO3 log / exp) and the mean position; the result is
+ *     m_camera_rot / m_camera_pos as in immesh_mesh_render_depth.  The first frame (the reference's cur < 1) gets the identity pose;
+ *     so does a window holding no frame with a pose (world-frame frames carry none; the reference divides by zero there).
+ *   immesh_mesh_reinforce_pose(h, cam_R, cam_t): the caller's camera pose instead, from the next queued frame on, for every frame
+ *     (the form for frames pushed with world points); NULL, NULL returns to the sensor-bound pose.  Enabling starts sensor-bound.
+ *   Result: exactly immesh_mesh_render_depth at that pose -- same depth image bit for bit, same points and pixels in ascending pixel
+ *     order -- computed by a tiled rasteriser (16 x 16 pixel tiles; the triangles binned by their pixel boxes).
+ *   immesh_mesh_reinforced_cloud: blocking read of the newest queued frame's result (waits for that frame only).  The result is
+ *     double-buffered: a frame queued after the read started writes the other buffer.  depth [height][width] (-1 where empty),
+ *     points [n][3], point_pixel [n] (y * width + x), pose_out [12] = R row-major, t; each may be NULL.  *n_out > cap:
+ *     IMMESH_E_CAPACITY with *n_out = points needed, nothing written (cap = 0: a count query).  Not enabled, no frame queued since
+ *     enable, or a sharded handle: IMMESH_E_INVALID. */
+int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics /*[4] or NULL*/, int width, int height, double z_near, double z_far, int win);
+int immesh_mesh_reinforce_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/);
+int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth /*[h][w] or NULL*/, float* points /*[cap][3] or NULL*/, int32_t* point_pixel /*[cap] or NULL*/,
+                                 int cap, int* n_out, double* pose_out /*[12] or NULL*/);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
