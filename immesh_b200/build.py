@@ -155,6 +155,19 @@ def build_reinforce(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "reinforce", "emu_reinforce.cpp"), EMU_REINFORCE, force)
 
 
+DEV_MEM_DIR = os.path.join(_ROOT, "tests", "dev_mem")
+EMU_DEV_MEM = os.path.join(DEV_MEM_DIR, "libdev_mem_emu.so")
+
+
+def build_dev_mem(force=False):
+    """tests/dev_mem: the handles' memory owner (immesh_b200/csrc/dev_mem.hpp) built for the host against allocation stubs that
+    can fail on demand (-Bsymbolic: the stubs, not a CUDA runtime loaded earlier in the process, serve its calls)"""
+    src = os.path.join(DEV_MEM_DIR, "emu_dev_mem.cpp")
+    if force or _newer(EMU_DEV_MEM, [src, os.path.join(CSRC, "dev_mem.hpp")]):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-Wall", "-I/usr/local/cuda/include", "-shared", "-Wl,-Bsymbolic", "-o", EMU_DEV_MEM, src])
+    return EMU_DEV_MEM
+
+
 def build_ref():
     """oracle/_ref: the reference's own ikd-Tree compiled unmodified from the reference checkout, where one is present;
     elsewhere a library built earlier is used, and the tests that need it skip when there is none."""
@@ -174,6 +187,7 @@ def build_all(force=False):
     build_growth(force)
     build_imu_chain(force)
     build_reinforce(force)
+    build_dev_mem(force)
     build_ref()
 
 

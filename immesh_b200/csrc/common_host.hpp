@@ -6,13 +6,28 @@
 
 #include <cstdio>
 #include <map>
+#include <memory>
 #include <string>
 #include <tuple>
 #include <vector>
 
 #include "../../include/immesh_b200.h"
+#include "dev_mem.hpp"
 
 namespace immesh {
+// a handle under construction: every return before release() hands it to its destroy function, which copes with a handle built
+// only in part (its memory is held by MemSet members)
+template <class H>
+using Building = std::unique_ptr<H, int (*)(H*)>;
+
+// true when `p` is page-locked host memory the device can read directly (allocated pinned, or registered): such an input is
+// copied straight from the caller's buffer, without the staging memcpy
+inline bool host_ptr_is_pinned(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeHost;
+}
+
 inline std::string& last_error_storage() {
     static thread_local std::string s;
     return s;

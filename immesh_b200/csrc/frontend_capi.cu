@@ -238,6 +238,7 @@ struct immesh_voxelgrid {
     float* d_out_i = nullptr;    // [max_points] intensity of the down-sampled cloud d_out
     float* h_out_i = nullptr;    // pinned [max_points]
     long long calls = 0;         // calls that queued work on the handle (immesh_lio_frontend_cloud: has vg run another call since)
+    immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // every buffer above
 };
 
 extern "C" {
@@ -246,7 +247,8 @@ int immesh_voxelgrid_create(int max_points, immesh_voxelgrid_t** out) {
     if (!out || max_points < 1) return im_fail(IMMESH_E_INVALID, "bad argument");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return im_fail(IMMESH_E_NO_DEVICE, "no CUDA device: immesh_b200 has no CPU path"); }
-    immesh_voxelgrid* h = new immesh_voxelgrid();
+    immesh::Building<immesh_voxelgrid> owner(new immesh_voxelgrid(), immesh_voxelgrid_destroy);   // every failure below releases what was created
+    immesh_voxelgrid* h = owner.get();
     h->max_points = max_points;
     h->nblocks_max = (max_points + VG_TILE - 1) / VG_TILE;
     int dev = 0;
@@ -254,59 +256,63 @@ int immesh_voxelgrid_create(int max_points, immesh_voxelgrid_t** out) {
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
     IM_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     const size_t n = (size_t)max_points;
-    for (int i = 0; i < 8; ++i) IM_CUDA(cudaMalloc((void**)&h->d_in_ring[i], n * 3 * sizeof(float)));
+    for (int i = 0; i < 8; ++i) IM_CUDA(h->dev.alloc(&h->d_in_ring[i], n * 3));
     h->d_in = h->d_in_ring[0];
-    IM_CUDA(cudaMalloc((void**)&h->d_out, n * 3 * sizeof(float)));
-    IM_CUDA(cudaMalloc((void**)&h->d_raw, n * 4 * sizeof(float)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_raw, n * 4 * sizeof(float)));
+    IM_CUDA(h->dev.alloc(&h->d_out, n * 3));
+    IM_CUDA(h->dev.alloc(&h->d_raw, n * 4));
+    IM_CUDA(h->pinned.alloc(&h->h_raw, n * 4));
     IM_CUDA(cudaEventCreateWithFlags(&h->ev_raw, cudaEventDisableTiming));
     for (int i = 0; i < 2; ++i) {
-        IM_CUDA(cudaMalloc((void**)&h->d_k[i], n * sizeof(unsigned int)));
-        IM_CUDA(cudaMalloc((void**)&h->d_v[i], n * sizeof(unsigned int)));
+        IM_CUDA(h->dev.alloc(&h->d_k[i], n));
+        IM_CUDA(h->dev.alloc(&h->d_v[i], n));
     }
-    IM_CUDA(cudaMalloc((void**)&h->d_hist, (size_t)256 * h->nblocks_max * sizeof(int)));
-    IM_CUDA(cudaMalloc((void**)&h->d_tile, ((size_t)h->nblocks_max + 1) * sizeof(int)));
-    IM_CUDA(cudaMalloc((void**)&h->d_head, n * sizeof(int)));
-    IM_CUDA(cudaMalloc((void**)&h->d_grid, sizeof(VgGrid)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_grid, sizeof(VgGrid)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_pts, n * 3 * sizeof(float)));
-    *out = h;
+    IM_CUDA(h->dev.alloc(&h->d_hist, (size_t)256 * h->nblocks_max));
+    IM_CUDA(h->dev.alloc(&h->d_tile, (size_t)h->nblocks_max + 1));
+    IM_CUDA(h->dev.alloc(&h->d_head, n));
+    IM_CUDA(h->dev.alloc(&h->d_grid, 1));
+    IM_CUDA(h->pinned.alloc(&h->h_grid, 1));
+    IM_CUDA(h->pinned.alloc(&h->h_pts, n * 3));
+    *out = owner.release();
     return IMMESH_OK;
 }
 
 int immesh_voxelgrid_destroy(immesh_voxelgrid_t* h) {
     if (!h) return IMMESH_OK;
     cudaStreamSynchronize(h->stream);
-    for (int i = 0; i < 8; ++i) cudaFree(h->d_in_ring[i]);
-    cudaFree(h->d_out); cudaFree(h->d_raw); cudaFreeHost(h->h_raw);
     if (h->ev_raw) cudaEventDestroy(h->ev_raw);
-    for (int i = 0; i < 2; ++i) { cudaFree(h->d_k[i]); cudaFree(h->d_v[i]); }
-    cudaFree(h->d_hist); cudaFree(h->d_tile); cudaFree(h->d_head); cudaFree(h->d_grid);
-    cudaFreeHost(h->h_grid); cudaFreeHost(h->h_pts);
-    for (int i = 0; i < 8; ++i) cudaFree(h->d_in_i_ring[i]);
-    cudaFree(h->d_out_i); cudaFreeHost(h->h_out_i);
-    cudaStreamDestroy(h->stream);
+    if (h->stream) cudaStreamDestroy(h->stream);
     delete h;
     return IMMESH_OK;
 }
 
 // the intensity buffers of the _i entry points, and host staging for records of `host_stride` floats (0: device input only).
-// Allocated on first use, so that a handle that never carries intensity keeps the footprint it has at create.
+// Allocated on first use, so that a handle that never carries intensity keeps the footprint it has at create.  Each of the two
+// steps is all or nothing: after a failure the handle is as it was.
 static int vg_intensity_alloc(immesh_voxelgrid* h, int host_stride) {
     const size_t n = (size_t)h->max_points;
     if (!h->d_out_i) {
-        for (int i = 0; i < 8; ++i) IM_CUDA(cudaMalloc((void**)&h->d_in_i_ring[i], n * sizeof(float)));
-        IM_CUDA(cudaMalloc((void**)&h->d_out_i, n * sizeof(float)));
-        IM_CUDA(cudaMallocHost((void**)&h->h_out_i, n * sizeof(float)));
+        immesh::MemSet dev, pinned(immesh::MemSet::Pinned);
+        float *ring[8], *d_out_i, *h_out_i;
+        for (int i = 0; i < 8; ++i) IM_CUDA(dev.alloc(&ring[i], n));
+        IM_CUDA(dev.alloc(&d_out_i, n));
+        IM_CUDA(pinned.alloc(&h_out_i, n));
+        std::copy(ring, ring + 8, h->d_in_i_ring);
+        h->d_out_i = d_out_i;
+        h->h_out_i = h_out_i;
+        h->dev.take(std::move(dev));
+        h->pinned.take(std::move(pinned));
     }
     if (host_stride > h->raw_stride) {
+        immesh::MemSet dev, pinned(immesh::MemSet::Pinned);
+        float *d_raw, *h_raw;
+        IM_CUDA(dev.alloc(&d_raw, n * host_stride));
+        IM_CUDA(pinned.alloc(&h_raw, n * host_stride));
         IM_CUDA(cudaDeviceSynchronize());   // no queued copy or pack still uses the narrower staging
         h->raw_pending = 0;
-        cudaFree(h->d_raw); cudaFreeHost(h->h_raw);
-        h->d_raw = nullptr; h->h_raw = nullptr; h->raw_stride = 0;
-        IM_CUDA(cudaMalloc((void**)&h->d_raw, n * host_stride * sizeof(float)));
-        IM_CUDA(cudaMallocHost((void**)&h->h_raw, n * host_stride * sizeof(float)));
-        h->raw_stride = host_stride;
+        h->dev.free(h->d_raw); h->pinned.free(h->h_raw);
+        h->d_raw = d_raw; h->h_raw = h_raw; h->raw_stride = host_stride;
+        h->dev.take(std::move(dev));
+        h->pinned.take(std::move(pinned));
     }
     return IMMESH_OK;
 }
@@ -421,10 +427,8 @@ static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int strid
     h->d_in = h->d_in_ring[h->in_idx];
     const float* d_src = pts;
     if (!on_device) {
-        cudaPointerAttributes a;
         const float* src = pts;
-        if (cudaPointerGetAttributes(&a, pts) != cudaSuccess || a.type != cudaMemoryTypeHost) {
-            cudaGetLastError();
+        if (!immesh::host_ptr_is_pinned(pts)) {
             if (h->raw_pending) { IM_CUDA(cudaEventSynchronize(h->ev_raw)); h->raw_pending = 0; }   // the previous copy out of the staging buffer
             std::memcpy(h->h_raw, pts, (size_t)n * stride * sizeof(float));
             src = h->h_raw;

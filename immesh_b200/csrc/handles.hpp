@@ -2,8 +2,6 @@
 #pragma once
 #include <cuda_runtime.h>
 
-#include <vector>
-
 #include "common_host.hpp"
 #include "lio_core.cuh"
 #include "mesh_voxel.cuh"
@@ -24,11 +22,12 @@ struct immesh_lio {
     ScanBuf sb;
     LioCtrl* d_ctrl = nullptr;
     int* d_counters = nullptr;  // node_count, chunk_bump, avail_top, pending_n, err, n_roots, n_touched, seg_top, work_counter, .., pub_n (12)
-    int* d_pub_scratch = nullptr;    // immesh_voxelmap_plane_markers: key sort, per-root row counts / offsets (grown on demand)
+    // grow-only scratch of the publishers, in `scratch`
+    int* d_pub_scratch = nullptr;    // immesh_voxelmap_plane_markers: key sort, per-root row counts / offsets
     size_t pub_scratch_ints = 0;
-    double* d_pub_rows = nullptr;    // immesh_voxelmap_plane_markers: the rows of one call (grown on demand)
-    size_t pub_rows_cap = 0;
-    // immesh_lio_effect_cloud / immesh_lio_registered_cloud (all grown on demand)
+    double* d_pub_rows = nullptr;    // immesh_voxelmap_plane_markers: the rows of one call
+    size_t pub_rows_doubles = 0;
+    // immesh_lio_effect_cloud / immesh_lio_registered_cloud
     float4* d_spub_rows = nullptr;   // x y z intensity rows of one call
     size_t spub_rows_cap = 0;
     int* d_spub_idx = nullptr;       // scan index of each effect row
@@ -48,17 +47,17 @@ struct immesh_lio {
     int* d_sorted = nullptr;
     int* d_complex = nullptr;   // touched root voxels left to the general warp-per-voxel kernel (the others are finished by k_grow_simple)
     double* d_ptpl = nullptr;
-    float* d_body_own = nullptr;  // scan buffers owned by the handle, 2 slots of max_scan*3 (sb.body points into them unless the caller passed a device pointer)
+    float* d_body_own = nullptr;  // scan buffers owned by the handle, IM_SLOTS slots of max_scan*3 (sb.body points into them unless the caller passed a device pointer)
     cudaStream_t stream_up = nullptr;   // upload stream: the H2D copy of scan k+1 overlaps the kernels of scan k
     cudaEvent_t ev_up[IM_SLOTS] = {};
     float* h_body = nullptr;   // pinned staging, IM_SLOTS slots
-    double* h_state = nullptr; // pinned, 2 slots of (IM_STATE_DOUBLES + 64)
+    double* h_state = nullptr; // pinned, IM_STATE_DOUBLES + 64
     cudaEvent_t ev_slot[IM_SLOTS] = {};  // completion of the step that used staging slot s
     int slot_busy[IM_SLOTS] = {};
     int step_counter = 0;
-    immesh::ScanDyn* h_dyn = nullptr;   // pinned, 2 slots: per-scan inputs of the launch sequence (one H2D per scan)
+    immesh::ScanDyn* h_dyn = nullptr;   // pinned, IM_SLOTS slots: per-scan inputs of the launch sequence (one H2D per scan)
     immesh::ScanDyn dyn_last = {};         // host copy of the block last uploaded
-    immesh::LioOut* h_out = nullptr;    // pinned, 2 slots: what a scan returns to the host (one D2H per scan)
+    immesh::LioOut* h_out = nullptr;    // pinned, IM_SLOTS slots: what a scan returns to the host (one D2H per scan)
     const int* next_n_dev = nullptr;    // device-resident point count for the next upload (immesh_lio_step_async_dev_n)
     int scan_counter = 0;               // scans queued through the step entry points; pose ring slot = scan_counter & 7
     int pose_pub_idx = -1;              // scan index whose converged pose is in LioCtrl::pose_ring (-1: not published)
@@ -80,11 +79,12 @@ struct immesh_lio {
     immesh::GraphCtx graph;   // replay of the per-scan launch sequence (pipelined API)
     int use_graph = 1;
     double last_ms[3] = {0, 0, 0};
-    std::vector<void*> allocs;
-    size_t dev_bytes = 0;         // device bytes of `allocs` (the create-time buffers, the map pools and what dev_alloc adds later)
+    immesh::MemSet dev;           // device memory counted in immesh_lio_capacity: the create-time buffers, the map pools, d_ptpl, d_bits
+    immesh::MemSet scratch;       // device memory not counted: the publishers' scratch
+    immesh::MemSet pinned{immesh::MemSet::Pinned};
     // growth of the map pools (immesh_lio_reserve / immesh_lio_set_growth)
     long long growths = 0;        // calls that enlarged at least one pool
-    int64_t grow_max_bytes = 0;   // automatic growth before every step: 0 off, > 0 ceiling on dev_bytes
+    int64_t grow_max_bytes = 0;   // automatic growth before every step: 0 off, > 0 ceiling on dev.bytes()
     int known[16] = {};           // counters (d_counters layout) of the last step known to have finished
     long long known_step = 0;     // its number among the map-growing steps (0: the empty map at create)
     long long map_steps = 0;      // map-growing steps queued so far
@@ -98,13 +98,13 @@ struct immesh_mesh {
     FrameBuf F;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    float* d_pts = nullptr;   // 2 slots of max_frame_points*3
-    float* d_body = nullptr;  // 2 slots, staging for body-frame scans handed over by the localization handle
-    float* h_pts = nullptr;   // pinned, 2 slots
-    int* h_cnt = nullptr;     // pinned, 2 slots of 32
-    FramePose* d_fp = nullptr;  // 2 slots
-    FramePose* h_fp = nullptr;  // pinned, 2 slots
-    immesh::FrameDyn* h_dyn = nullptr;  // pinned, 2 slots: per-frame inputs of the launch sequence
+    float* d_pts = nullptr;   // IM_SLOTS slots of max_frame_points*3
+    float* d_body = nullptr;  // IM_SLOTS slots, staging for body-frame scans handed over by the localization handle
+    float* h_pts = nullptr;   // pinned, IM_SLOTS slots
+    int* h_cnt = nullptr;     // pinned, IM_SLOTS slots of 32
+    FramePose* d_fp = nullptr;  // IM_SLOTS slots
+    FramePose* h_fp = nullptr;  // pinned, IM_SLOTS slots
+    immesh::FrameDyn* h_dyn = nullptr;  // pinned, IM_SLOTS slots: per-frame inputs of the launch sequence
     immesh::FrameDyn* d_dyn = nullptr;  // device copy read by every kernel of the frame (F.dyn)
     int timed_last = 0;
     double host_wait_ms = 0;
@@ -135,10 +135,13 @@ struct immesh_mesh {
     size_t ccap = 0;
     double last_ms[4] = {0, 0, 0, 0};
     int last_cnt[32];
-    std::vector<void*> allocs;
-    void* rb_buf[16] = {};    // scratch of immesh_mesh_region_buffers, grown on demand (freed by destroy)
-    size_t rb_cap[16] = {};
-    // batched frame (immesh_mesh_push_frame_batched), allocated by its first call, sized by the handle's capacities only
+    immesh::MemSet dev;       // device memory counted in immesh_mesh_capacity (with `batch`): the create-time buffers, the pools and the shard segments
+    immesh::MemSet scratch;   // device memory not counted: the region buffers' scratch
+    immesh::MemSet pinned{immesh::MemSet::Pinned};
+    unsigned char* region_scratch[16] = {};   // immesh_mesh_region_buffers, grow-only, in `scratch`
+    size_t region_scratch_cap[16] = {};
+    // batched frame (immesh_mesh_push_frame_batched), allocated by its first call into `batch`, sized by the handle's capacities only
+    immesh::MemSet batch;
     int max_vox = 0;
     int* b_act = nullptr;             // [max_vox] the frame's activated voxels (all append chunks)
     int* b_sel = nullptr;             // [max_vox] the voxels the frame meshes
@@ -150,8 +153,6 @@ struct immesh_mesh {
     int* b_fset = nullptr;            // facet set of a batch, 2 x max_list slots
     unsigned int b_fset_mask = 0;
     immesh::FramePose* b_fp = nullptr;
-    size_t b_bytes = 0;
-    size_t dev_bytes = 0;         // device bytes of `allocs`
     // growth of the mesh pools (immesh_mesh_reserve / immesh_mesh_set_growth)
     long long growths = 0;
     int64_t grow_max_bytes = 0;
@@ -167,12 +168,12 @@ struct immesh_mesh {
         int explicit_pose = 0;            // immesh_mesh_reinforce_pose: the caller's pose from the next frame on
         double R[9] = {}, t[3] = {};
         immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
-        std::vector<void*> bufs;          // device buffers below, freed by disable / destroy
         void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
         void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
         immesh::DepthCam* cam = nullptr;
         int *tile_cnt = nullptr, *tile_off = nullptr, *bin = nullptr, *misc = nullptr, *blk = nullptr, *blk_off = nullptr;
         unsigned int* depth_bits = nullptr;
         float* depth[2] = {}; float* pts[2] = {}; int* pix[2] = {}; int* n[2] = {}; double* pose[2] = {};
+        immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
     } rf;
 };

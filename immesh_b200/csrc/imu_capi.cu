@@ -122,6 +122,7 @@ struct immesh_imu {
     float* h_rec = nullptr; // pinned, IM_SLOTS slots of [max_points][rec_stride]
     float* d_in_i = nullptr;   // [max_points] intensity in scan order
     float* d_out_i = nullptr;  // [max_points] intensity in time order (beside d_out)
+    immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // every buffer above
 };
 
 // internal entry points of frontend_capi.cu / lio_capi.cu
@@ -147,20 +148,29 @@ static int imu_stage_release(immesh_imu* h, int s, cudaStream_t st) {
     return IMMESH_OK;
 }
 
-// the buffers of the _i entry: intensity beside d_in / d_out, and record staging of `stride` floats per point (grown for wider records)
+// the buffers of the _i entry: intensity beside d_in / d_out, and record staging of `stride` floats per point (grown for wider
+// records).  Each of the two steps is all or nothing: after a failure the handle is as it was.
 static int imu_records_alloc(immesh_imu* h, int stride) {
     const size_t n = (size_t)h->max_points;
     if (!h->d_in_i) {
-        IM_CUDA(cudaMalloc((void**)&h->d_in_i, n * sizeof(float)));
-        IM_CUDA(cudaMalloc((void**)&h->d_out_i, n * sizeof(float)));
+        immesh::MemSet dev;
+        float *d_in_i, *d_out_i;
+        IM_CUDA(dev.alloc(&d_in_i, n));
+        IM_CUDA(dev.alloc(&d_out_i, n));
+        h->d_in_i = d_in_i;
+        h->d_out_i = d_out_i;
+        h->dev.take(std::move(dev));
     }
     if (stride > h->rec_stride) {
+        immesh::MemSet dev, pinned(immesh::MemSet::Pinned);
+        float *d_rec, *h_rec;
+        IM_CUDA(dev.alloc(&d_rec, n * stride));
+        IM_CUDA(pinned.alloc(&h_rec, IM_SLOTS * n * stride));
         IM_CUDA(cudaDeviceSynchronize());   // no queued copy still reads the narrower staging
-        cudaFree(h->d_rec); cudaFreeHost(h->h_rec);
-        h->d_rec = nullptr; h->h_rec = nullptr; h->rec_stride = 0;
-        IM_CUDA(cudaMalloc((void**)&h->d_rec, n * stride * sizeof(float)));
-        IM_CUDA(cudaMallocHost((void**)&h->h_rec, IM_SLOTS * n * stride * sizeof(float)));
-        h->rec_stride = stride;
+        h->dev.free(h->d_rec); h->pinned.free(h->h_rec);
+        h->d_rec = d_rec; h->h_rec = h_rec; h->rec_stride = stride;
+        h->dev.take(std::move(dev));
+        h->pinned.take(std::move(pinned));
     }
     return IMMESH_OK;
 }
@@ -220,7 +230,8 @@ int immesh_imu_create(const immesh_imu_config* c, immesh_imu_t** out) {
     if (!c || !out || c->max_points < 1 || c->max_imu < 1 || c->max_imu > 256) return im_fail(IMMESH_E_INVALID, "bad argument (max_imu must be in [1, 256])");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return im_fail(IMMESH_E_NO_DEVICE, "no CUDA device: immesh_b200 has no CPU path"); }
-    immesh_imu* h = new immesh_imu();
+    immesh::Building<immesh_imu> owner(new immesh_imu(), immesh_imu_destroy);   // every failure below releases what was created
+    immesh_imu* h = owner.get();
     for (int i = 0; i < 3; ++i) { h->P.cov_gyr[i] = c->cov_gyr[i]; h->P.cov_acc[i] = c->cov_acc[i]; h->P.cov_bias_gyr[i] = c->cov_bias_gyr[i]; h->P.cov_bias_acc[i] = c->cov_bias_acc[i]; h->P.lid_T[i] = c->lid_T[i]; }
     for (int i = 0; i < 9; ++i) h->P.lid_R[i] = c->lid_R[i];
     h->P.mean_acc_norm = c->mean_acc_norm;
@@ -235,34 +246,29 @@ int immesh_imu_create(const immesh_imu_config* c, immesh_imu_t** out) {
     std::memset(&t0, 0, sizeof(t0));
     t0.last_lidar_end_time = -1.0;
     t0.n_pose = 1;
-    IM_CUDA(cudaMalloc((void**)&h->d_time, sizeof(ImuTime)));
+    IM_CUDA(h->dev.alloc(&h->d_time, 1));
     IM_CUDA(cudaMemcpy(h->d_time, &t0, sizeof(ImuTime), cudaMemcpyHostToDevice));
-    IM_CUDA(cudaMalloc((void**)&h->d_run, IM_IMU_RUN * sizeof(double)));
-    IM_CUDA(cudaMemset(h->d_run, 0, IM_IMU_RUN * sizeof(double)));
-    IM_CUDA(cudaMalloc((void**)&h->d_poses, ((size_t)c->max_imu + 2) * IM_POSE_DOUBLES * sizeof(double)));
-    IM_CUDA(cudaMalloc((void**)&h->d_steps, ((size_t)c->max_imu + 1) * sizeof(ImuStep)));
-    IM_CUDA(cudaMalloc((void**)&h->d_imu, (size_t)c->max_imu * 7 * sizeof(double)));
-    IM_CUDA(cudaMalloc((void**)&h->d_in, n * 4 * sizeof(float)));
-    IM_CUDA(cudaMalloc((void**)&h->d_out, n * 4 * sizeof(float)));
+    IM_CUDA(h->dev.alloc(&h->d_run, IM_IMU_RUN, 0));
+    IM_CUDA(h->dev.alloc(&h->d_poses, ((size_t)c->max_imu + 2) * IM_POSE_DOUBLES));
+    IM_CUDA(h->dev.alloc(&h->d_steps, (size_t)c->max_imu + 1));
+    IM_CUDA(h->dev.alloc(&h->d_imu, (size_t)c->max_imu * 7));
+    IM_CUDA(h->dev.alloc(&h->d_in, n * 4));
+    IM_CUDA(h->dev.alloc(&h->d_out, n * 4));
     for (int i = 0; i < 2; ++i) {
-        IM_CUDA(cudaMalloc((void**)&h->d_k[i], n * sizeof(unsigned int)));
-        IM_CUDA(cudaMalloc((void**)&h->d_v[i], n * sizeof(unsigned int)));
+        IM_CUDA(h->dev.alloc(&h->d_k[i], n));
+        IM_CUDA(h->dev.alloc(&h->d_v[i], n));
     }
-    IM_CUDA(cudaMalloc((void**)&h->d_hist, (size_t)256 * h->nblocks_max * sizeof(int)));
+    IM_CUDA(h->dev.alloc(&h->d_hist, (size_t)256 * h->nblocks_max));
     h->slot_doubles = (size_t)c->max_imu * 7 + 32;   // the batch + the host words of an initialising scan
-    IM_CUDA(cudaMallocHost((void**)&h->h_imu, IM_SLOTS * h->slot_doubles * sizeof(double)));
-    IM_CUDA(cudaMallocHost((void**)&h->h_pts, IM_SLOTS * n * 4 * sizeof(float)));
+    IM_CUDA(h->pinned.alloc(&h->h_imu, IM_SLOTS * h->slot_doubles));
+    IM_CUDA(h->pinned.alloc(&h->h_pts, IM_SLOTS * n * 4));
     for (int i = 0; i < IM_SLOTS; ++i) IM_CUDA(cudaEventCreateWithFlags(&h->ev_stage[i], cudaEventDisableTiming));
-    *out = h;
+    *out = owner.release();
     return IMMESH_OK;
 }
 int immesh_imu_destroy(immesh_imu_t* h) {
     if (!h) return IMMESH_OK;
     cudaDeviceSynchronize();
-    cudaFree(h->d_time); cudaFree(h->d_run); cudaFree(h->d_poses); cudaFree(h->d_steps); cudaFree(h->d_imu); cudaFree(h->d_in); cudaFree(h->d_out);
-    for (int i = 0; i < 2; ++i) { cudaFree(h->d_k[i]); cudaFree(h->d_v[i]); }
-    cudaFree(h->d_hist); cudaFreeHost(h->h_imu); cudaFreeHost(h->h_pts);
-    cudaFree(h->d_rec); cudaFreeHost(h->h_rec); cudaFree(h->d_in_i); cudaFree(h->d_out_i);
     for (int i = 0; i < IM_SLOTS; ++i) if (h->ev_stage[i]) cudaEventDestroy(h->ev_stage[i]);
     delete h;
     return IMMESH_OK;

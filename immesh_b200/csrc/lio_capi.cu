@@ -598,18 +598,6 @@ static void fill_params(const immesh_lio_config* c, LioParams& P) {
     for (int i = 0; i < 3; ++i) P.extT[i] = c->ext_T[i];
 }
 
-template <class T>
-static cudaError_t dev_alloc(immesh_lio* h, T** p, size_t count, int memset_byte = -1) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return e;
-    h->allocs.push_back(q);
-    h->dev_bytes += count * sizeof(T);
-    *p = (T*)q;
-    if (memset_byte >= 0) e = cudaMemset(q, memset_byte, count * sizeof(T));
-    return e;
-}
-
 // Grids are fixed per handle (sized for max_scan_points, at most 8 waves of blocks; every per-point kernel is a grid-stride
 // loop over the n it reads from the device-resident ScanDyn), so that the captured launch sequence is identical for every scan.
 static int grid_fixed(const immesh_lio* h, int threads, int max_waves = 8) {
@@ -620,18 +608,7 @@ static int grid_fixed(const immesh_lio* h, int threads, int max_waves = 8) {
     return (int)g;
 }
 
-// scan publishers (immesh_lio_effect_cloud / immesh_lio_registered_cloud): buffers grown on demand, the validity of the per-scan rows
-template <class T>
-static int spub_grow(T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return IMMESH_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    const size_t c = std::max<size_t>(need, 1024);
-    IM_CUDA(cudaMalloc((void**)p, c * sizeof(T)));
-    *cap = c;
-    return IMMESH_OK;
-}
+// scan publishers (immesh_lio_effect_cloud / immesh_lio_registered_cloud): the validity of the per-scan rows
 static int scan_rows_status(const immesh_lio* h, const char* what) {
     if (h->scan_rows >= 0) return IMMESH_OK;
     return im_fail(IMMESH_E_INVALID, (std::string(what) + ": the per-scan buffers were overwritten by " + h->scan_rows_overwritten_by +
@@ -657,13 +634,8 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     if (cfg->max_nodes < 0 || cfg->max_chunks < 0 || cfg->max_scan_points < 0) return im_fail(IMMESH_E_INVALID, "capacities must be non-negative (0 = default)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return im_fail(IMMESH_E_NO_DEVICE, "no CUDA device: immesh_b200 has no CPU path");
-    immesh_lio* h = new immesh_lio();
-    // every failure below releases what has been created so far (immesh_lio_destroy copes with a partially built handle)
-#define IM_CREATE(expr)                                                                     \
-    do {                                                                                    \
-        cudaError_t im_e_ = (expr);                                                         \
-        if (im_e_ != cudaSuccess) { immesh_lio_destroy(h); return immesh::im_fail_cuda(im_e_, __FILE__, __LINE__); } \
-    } while (0)
+    immesh::Building<immesh_lio> owner(new immesh_lio(), immesh_lio_destroy);   // every failure below releases what was created
+    immesh_lio* h = owner.get();
     fill_params(cfg, h->P);
     h->use_graph = std::getenv("IMMESH_GRAPH") ? std::atoi(std::getenv("IMMESH_GRAPH")) : 1;
     const int caplog = cfg->hash_capacity_log2 ? cfg->hash_capacity_log2 : 22;
@@ -674,70 +646,69 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
-    IM_CREATE(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    for (auto& e : h->ev) IM_CREATE(cudaEventCreate(&e));
-    for (int i = 0; i < IM_SLOTS; ++i) IM_CREATE(cudaEventCreateWithFlags(&h->ev_slot[i], cudaEventDisableTiming));
-    IM_CREATE(cudaEventCreateWithFlags(&h->ev_pose, cudaEventDisableTiming));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    for (auto& e : h->ev) IM_CUDA(cudaEventCreate(&e));
+    for (int i = 0; i < IM_SLOTS; ++i) IM_CUDA(cudaEventCreateWithFlags(&h->ev_slot[i], cudaEventDisableTiming));
+    IM_CUDA(cudaEventCreateWithFlags(&h->ev_pose, cudaEventDisableTiming));
     VoxelMapDev& m = h->map;
-    IM_CREATE(dev_alloc(h, &m.keys, h->cap, 0xFF));
-    IM_CREATE(dev_alloc(h, &m.root_node, h->cap, 0xFF));
+    IM_CUDA(h->dev.alloc(&m.keys, h->cap, 0xFF));
+    IM_CUDA(h->dev.alloc(&m.root_node, h->cap, 0xFF));
     m.cap_mask = (unsigned)(h->cap - 1);
-    IM_CREATE(dev_alloc(h, &m.nodes, (size_t)h->max_nodes));
-    IM_CREATE(dev_alloc(h, &m.planes, (size_t)h->max_nodes));
-    IM_CREATE(dev_alloc(h, &m.chunks, (size_t)h->max_chunks));
-    IM_CREATE(dev_alloc(h, &m.avail, (size_t)h->max_chunks));
-    IM_CREATE(dev_alloc(h, &m.pending, (size_t)h->max_chunks));
-    IM_CREATE(dev_alloc(h, &h->d_counters, 16, 0));
+    IM_CUDA(h->dev.alloc(&m.nodes, (size_t)h->max_nodes));
+    IM_CUDA(h->dev.alloc(&m.planes, (size_t)h->max_nodes));
+    IM_CUDA(h->dev.alloc(&m.chunks, (size_t)h->max_chunks));
+    IM_CUDA(h->dev.alloc(&m.avail, (size_t)h->max_chunks));
+    IM_CUDA(h->dev.alloc(&m.pending, (size_t)h->max_chunks));
+    IM_CUDA(h->dev.alloc(&h->d_counters, 16, 0));
     m.node_count = h->d_counters + 0; m.chunk_bump = h->d_counters + 1; m.avail_top = h->d_counters + 2; m.pending_n = h->d_counters + 3;
     m.err = h->d_counters + 4; m.n_roots = h->d_counters + 5; m.stat = h->d_counters + 9;
     m.max_nodes = h->max_nodes; m.max_chunks = h->max_chunks;
-    IM_CREATE(dev_alloc(h, &m.pub, (size_t)h->max_nodes));
-    IM_CREATE(dev_alloc(h, &m.pub_mark, h->cap, 0));
-    IM_CREATE(dev_alloc(h, &m.pub_list, h->cap));
+    IM_CUDA(h->dev.alloc(&m.pub, (size_t)h->max_nodes));
+    IM_CUDA(h->dev.alloc(&m.pub_mark, h->cap, 0));
+    IM_CUDA(h->dev.alloc(&m.pub_list, h->cap));
     m.pub_n = h->d_counters + 12;
     ScanBuf& sb = h->sb;
     const size_t ms = (size_t)h->max_scan;
     float* d_body = nullptr;
-    IM_CREATE(dev_alloc(h, &d_body, IM_SLOTS * ms * 3));
-    IM_CREATE(cudaStreamCreateWithFlags(&h->stream_up, cudaStreamNonBlocking));
-    for (int i = 0; i < IM_SLOTS; ++i) IM_CREATE(cudaEventCreateWithFlags(&h->ev_up[i], cudaEventDisableTiming));
+    IM_CUDA(h->dev.alloc(&d_body, IM_SLOTS * ms * 3));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream_up, cudaStreamNonBlocking));
+    for (int i = 0; i < IM_SLOTS; ++i) IM_CUDA(cudaEventCreateWithFlags(&h->ev_up[i], cudaEventDisableTiming));
     sb.body = d_body;
     h->d_body_own = d_body;
-    IM_CREATE(dev_alloc(h, &sb.body_cov, ms * 6));
-    IM_CREATE(dev_alloc(h, &sb.p_imu, ms * 3));
-    IM_CREATE(dev_alloc(h, &sb.bv_imu, ms * 6));
-    IM_CREATE(dev_alloc(h, &sb.match_node, ms, 0xFF));
-    IM_CREATE(dev_alloc(h, &sb.match_layer, ms, 0));
-    IM_CREATE(dev_alloc(h, &sb.wsqrt, ms));
-    IM_CREATE(dev_alloc(h, &sb.pw, ms * 3));
-    IM_CREATE(dev_alloc(h, &sb.var, ms * 6));
-    IM_CREATE(dev_alloc(h, &sb.sortkey, ms));
-    IM_CREATE(dev_alloc(h, &sb.slot, ms));
-    IM_CREATE(dev_alloc(h, &sb.seg, ms));
-    IM_CREATE(dev_alloc(h, &h->d_sorted, ms));
-    IM_CREATE(dev_alloc(h, &h->d_complex, ms));
-    IM_CREATE(dev_alloc(h, &sb.touched, ms));
-    IM_CREATE(dev_alloc(h, &sb.slot_count, h->cap, 0));
-    IM_CREATE(dev_alloc(h, &sb.slot_offset, h->cap, 0));
-    IM_CREATE(dev_alloc(h, &sb.slot_cursor, h->cap, 0));
+    IM_CUDA(h->dev.alloc(&sb.body_cov, ms * 6));
+    IM_CUDA(h->dev.alloc(&sb.p_imu, ms * 3));
+    IM_CUDA(h->dev.alloc(&sb.bv_imu, ms * 6));
+    IM_CUDA(h->dev.alloc(&sb.match_node, ms, 0xFF));
+    IM_CUDA(h->dev.alloc(&sb.match_layer, ms, 0));
+    IM_CUDA(h->dev.alloc(&sb.wsqrt, ms));
+    IM_CUDA(h->dev.alloc(&sb.pw, ms * 3));
+    IM_CUDA(h->dev.alloc(&sb.var, ms * 6));
+    IM_CUDA(h->dev.alloc(&sb.sortkey, ms));
+    IM_CUDA(h->dev.alloc(&sb.slot, ms));
+    IM_CUDA(h->dev.alloc(&sb.seg, ms));
+    IM_CUDA(h->dev.alloc(&h->d_sorted, ms));
+    IM_CUDA(h->dev.alloc(&h->d_complex, ms));
+    IM_CUDA(h->dev.alloc(&sb.touched, ms));
+    IM_CUDA(h->dev.alloc(&sb.slot_count, h->cap, 0));
+    IM_CUDA(h->dev.alloc(&sb.slot_offset, h->cap, 0));
+    IM_CUDA(h->dev.alloc(&sb.slot_cursor, h->cap, 0));
     sb.n_touched = h->d_counters + 6; sb.seg_top = h->d_counters + 7;
     sb.n = 0;
-    IM_CREATE(dev_alloc(h, &h->d_ctrl, 1, 0));
+    IM_CUDA(h->dev.alloc(&h->d_ctrl, 1, 0));
     sb.dyn = &h->d_ctrl->dyn;
-    IM_CREATE(cudaMallocHost((void**)&h->h_body, IM_SLOTS * ms * 3 * sizeof(float)));
-    IM_CREATE(cudaMallocHost((void**)&h->h_state, (IM_STATE_DOUBLES + 64) * sizeof(double)));
-    IM_CREATE(cudaMallocHost((void**)&h->h_ints, 64 * sizeof(int)));
-    IM_CREATE(cudaMallocHost((void**)&h->h_dyn, IM_SLOTS * sizeof(ScanDyn)));
-    IM_CREATE(cudaMallocHost((void**)&h->h_out, IM_SLOTS * sizeof(LioOut)));
+    IM_CUDA(h->pinned.alloc(&h->h_body, IM_SLOTS * ms * 3));
+    IM_CUDA(h->pinned.alloc(&h->h_state, IM_STATE_DOUBLES + 64));
+    IM_CUDA(h->pinned.alloc(&h->h_ints, 64));
+    IM_CUDA(h->pinned.alloc(&h->h_dyn, IM_SLOTS));
+    IM_CUDA(h->pinned.alloc(&h->h_out, IM_SLOTS));
     std::memset(h->h_out, 0, IM_SLOTS * sizeof(LioOut));
     // StatesGroup(): identity rotation, cov = INIT_COV * I  (include/common_lib.h:201-211)
     std::memset(h->h_state, 0, IM_STATE_DOUBLES * sizeof(double));
     h->h_state[0] = h->h_state[4] = h->h_state[8] = 1.0;
     for (int i = 0; i < 18; ++i) h->h_state[24 + i * 18 + i] = 0.0000001;
-    IM_CREATE(cudaMemcpy(h->d_ctrl->state, h->h_state, IM_STATE_DOUBLES * sizeof(double), cudaMemcpyHostToDevice));
-    IM_CREATE(cudaDeviceSynchronize());
-#undef IM_CREATE
-    *out = h;
+    IM_CUDA(cudaMemcpy(h->d_ctrl->state, h->h_state, IM_STATE_DOUBLES * sizeof(double), cudaMemcpyHostToDevice));
+    IM_CUDA(cudaDeviceSynchronize());
+    *out = owner.release();
     return IMMESH_OK;
 }
 
@@ -747,16 +718,6 @@ int immesh_lio_destroy(immesh_lio_t* h) {
     h->graph.destroy();
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && nccl().CommDestroy) nccl().CommDestroy(h->nccl_comm);
-    for (void* p : h->allocs) cudaFree(p);
-    if (h->d_pub_scratch) cudaFree(h->d_pub_scratch);
-    if (h->d_pub_rows) cudaFree(h->d_pub_rows);
-    for (void* p : {(void*)h->d_spub_rows, (void*)h->d_spub_idx, (void*)h->d_spub_tiles, (void*)h->d_spub_in})
-        if (p) cudaFree(p);
-    if (h->h_body) cudaFreeHost(h->h_body);
-    if (h->h_state) cudaFreeHost(h->h_state);
-    if (h->h_ints) cudaFreeHost(h->h_ints);
-    if (h->h_dyn) cudaFreeHost(h->h_dyn);
-    if (h->h_out) cudaFreeHost(h->h_out);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
     if (h->ev_pose) cudaEventDestroy(h->ev_pose);
     for (int i = 0; i < IM_SLOTS; ++i) if (h->ev_up[i]) cudaEventDestroy(h->ev_up[i]);
@@ -794,7 +755,7 @@ int immesh_lio_shard(immesh_lio_t* h, int rank, int nranks, const char* unique_i
     h->P.shard_n = nranks;
     h->graph.destroy();   // the launch sequence changes
     h->words_cap = h->max_scan / 32 + 2;
-    if (!h->d_bits) IM_CUDA(dev_alloc(h, &h->d_bits, (size_t)2 * h->words_cap, 0));
+    if (!h->d_bits) IM_CUDA(h->dev.alloc(&h->d_bits, (size_t)2 * h->words_cap, 0));
     // peer window over NVLink (CUDA IPC): the exchanges of the residual pass are then fused into its kernels.  IMMESH_SHARD_NCCL=1
     // keeps the NCCL all-reduce sequence (the baseline the fused path is measured against; same setting on every rank).  The
     // open is collective and its outcome is the same on every rank (peer_win.cuh).
@@ -832,13 +793,6 @@ int immesh_lio_get_state(immesh_lio_t* h, double* s) {
     return IMMESH_OK;
 }
 
-// true when `p` is page-locked host memory the device can read directly (cudaMallocHost / cudaHostRegister): such a scan is
-// copied straight from the caller's buffer, without the staging memcpy
-static bool host_ptr_is_pinned(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeHost;
-}
 static int push_dyn(immesh_lio* h, int n, int slot = 0, double dt = 0.0, double cov_gyr = 0.0, double cov_acc = 0.0);
 // per-scan inputs: the scan itself (host: staged through pinned slot `slot` unless the caller's buffer is pinned already) and
 // the ScanDyn block every kernel of the sequence reads; both in stream order, so the previous scan is never disturbed
@@ -852,7 +806,7 @@ static int upload_scan(immesh_lio* h, const float* body, int n, int on_device = 
         h->sb.body = dst;
         if (n > 0) {
             const float* src = body;
-            if (!host_ptr_is_pinned(body)) {
+            if (!immesh::host_ptr_is_pinned(body)) {
                 float* stage = h->h_body + (size_t)slot * h->max_scan * 3;
                 std::memcpy(stage, body, (size_t)n * 3 * sizeof(float));
                 src = stage;
@@ -943,7 +897,7 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     if (chunks > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "chunk pool: more than 2^30 chunks (32-bit chunk ids)");
     const bool g_cap = cap > cap0, g_nodes = nodes > nodes0, g_chunks = chunks > chunks0;
     if (!g_cap && !g_nodes && !g_chunks) return IMMESH_OK;
-    const size_t bytes = h->dev_bytes - pool_bytes(cap0, nodes0, chunks0) + pool_bytes(cap, nodes, chunks);
+    const size_t bytes = h->dev.bytes() - pool_bytes(cap0, nodes0, chunks0) + pool_bytes(cap, nodes, chunks);
     if (h->grow_max_bytes > 0 && bytes > (size_t)h->grow_max_bytes) {
         const std::string pools = std::string(g_cap ? " root hash" : "") + (g_nodes ? " node pool" : "") + (g_chunks ? " chunk pool" : "");
         return im_fail(IMMESH_E_CAPACITY, ("growth of the" + pools + " to " + std::to_string(bytes) + " device bytes is above the ceiling of " +
@@ -958,32 +912,25 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     VoxelMapDev nm = h->map;   // the map after the growth
     ScanBuf nsb = h->sb;
     int* slot_map = nullptr;
-    std::vector<void*> fresh;
+    immesh::MemSet fresh, tmp;   // the new buffers (freed on every failure below); the slot map of the rehash (freed on return)
     const char* pool = "";
-    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
-        void* q = nullptr;
-        const cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
-        if (e == cudaSuccess) { fresh.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
-        return e;
-    };
     cudaError_t e = cudaSuccess;
     if (g_nodes && e == cudaSuccess) {
         pool = "node pool";
-        if ((e = alloc(&nm.nodes, nodes)) == cudaSuccess && (e = alloc(&nm.planes, nodes)) == cudaSuccess) e = alloc(&nm.pub, nodes);
+        if ((e = fresh.alloc(&nm.nodes, nodes)) == cudaSuccess && (e = fresh.alloc(&nm.planes, nodes)) == cudaSuccess) e = fresh.alloc(&nm.pub, nodes);
     }
     if (g_chunks && e == cudaSuccess) {
         pool = "chunk pool";
-        if ((e = alloc(&nm.chunks, chunks)) == cudaSuccess && (e = alloc(&nm.avail, chunks)) == cudaSuccess) e = alloc(&nm.pending, chunks);
+        if ((e = fresh.alloc(&nm.chunks, chunks)) == cudaSuccess && (e = fresh.alloc(&nm.avail, chunks)) == cudaSuccess) e = fresh.alloc(&nm.pending, chunks);
     }
     if (g_cap && e == cudaSuccess) {
         pool = "root hash";
-        if ((e = alloc(&nm.keys, cap)) == cudaSuccess && (e = alloc(&nm.root_node, cap)) == cudaSuccess && (e = alloc(&nm.pub_mark, cap)) == cudaSuccess &&
-            (e = alloc(&nm.pub_list, cap)) == cudaSuccess && (e = alloc(&nsb.slot_count, cap)) == cudaSuccess &&
-            (e = alloc(&nsb.slot_offset, cap)) == cudaSuccess && (e = alloc(&nsb.slot_cursor, cap)) == cudaSuccess)
-            e = alloc(&slot_map, cap0);
+        if ((e = fresh.alloc(&nm.keys, cap)) == cudaSuccess && (e = fresh.alloc(&nm.root_node, cap)) == cudaSuccess && (e = fresh.alloc(&nm.pub_mark, cap)) == cudaSuccess &&
+            (e = fresh.alloc(&nm.pub_list, cap)) == cudaSuccess && (e = fresh.alloc(&nsb.slot_count, cap)) == cudaSuccess &&
+            (e = fresh.alloc(&nsb.slot_offset, cap)) == cudaSuccess && (e = fresh.alloc(&nsb.slot_cursor, cap)) == cudaSuccess)
+            e = tmp.alloc(&slot_map, cap0);
     }
     if (e != cudaSuccess) {
-        for (void* q : fresh) cudaFree(q);
         cudaGetLastError();
         const int code = e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA;
         return im_fail(code, (std::string(pool) + ": device allocation for the growth failed (" + cudaGetErrorString(e) + "); the handle is unchanged").c_str());
@@ -1020,22 +967,18 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
         return r;
     };
     if ((e = migrate()) != cudaSuccess) {   // a sticky CUDA error: nothing new is kept
-        for (void* q : fresh) cudaFree(q);
         cudaGetLastError();
         return immesh::im_fail_cuda(e, __FILE__, __LINE__);
     }
-    // the old buffers go; the new ones take their places in the handle's allocation list
-    auto swap_buf = [&](void* oldp, void* newp) {
-        if (oldp == newp) return;
-        for (void*& p : h->allocs)
-            if (p == oldp) p = newp;
-        cudaFree(oldp);
-    };
-    swap_buf(h->map.nodes, nm.nodes); swap_buf(h->map.planes, nm.planes); swap_buf(h->map.pub, nm.pub);
-    swap_buf(h->map.chunks, nm.chunks); swap_buf(h->map.avail, nm.avail); swap_buf(h->map.pending, nm.pending);
-    swap_buf(h->map.keys, nm.keys); swap_buf(h->map.root_node, nm.root_node); swap_buf(h->map.pub_mark, nm.pub_mark); swap_buf(h->map.pub_list, nm.pub_list);
-    swap_buf(h->sb.slot_count, nsb.slot_count); swap_buf(h->sb.slot_offset, nsb.slot_offset); swap_buf(h->sb.slot_cursor, nsb.slot_cursor);
-    if (slot_map) cudaFree(slot_map);
+    // the replaced buffers go; the new ones join the handle's device memory
+    if (g_nodes) { h->dev.free(h->map.nodes); h->dev.free(h->map.planes); h->dev.free(h->map.pub); }
+    if (g_chunks) { h->dev.free(h->map.chunks); h->dev.free(h->map.avail); h->dev.free(h->map.pending); }
+    if (g_cap) {
+        for (const void* p : {(const void*)h->map.keys, (const void*)h->map.root_node, (const void*)h->map.pub_mark, (const void*)h->map.pub_list,
+                              (const void*)h->sb.slot_count, (const void*)h->sb.slot_offset, (const void*)h->sb.slot_cursor})
+            h->dev.free(p);
+    }
+    h->dev.take(std::move(fresh));
     nm.max_nodes = (int)nodes;
     nm.max_chunks = (int)chunks;
     h->map = nm;
@@ -1043,7 +986,6 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     h->cap = (size_t)cap;
     h->max_nodes = (int)nodes;
     h->max_chunks = (int)chunks;
-    h->dev_bytes = bytes;
     h->growths++;
     h->graph.destroy();   // the next pipelined step captures the launch sequence again, with the new pointers
     IM_CUDA(cudaGetLastError());
@@ -1330,7 +1272,7 @@ int immesh_residual_build(immesh_lio_t* h, const float* body, int n, int* index_
     int rc = upload_scan(h, body, n);
     if (rc) return rc;
     scan_rows_overwritten(h, "immesh_residual_build");
-    if (!h->d_ptpl) IM_CUDA(dev_alloc(h, &h->d_ptpl, (size_t)h->max_scan * 31));
+    if (!h->d_ptpl) IM_CUDA(h->dev.alloc(&h->d_ptpl, (size_t)h->max_scan * 31));
     IM_LAUNCH(k_reset_scan, 2, 256, 0, h->stream, h->sb, h->d_ctrl, 0);
     *n_out = 0;
     if (n == 0) return IMMESH_OK;
@@ -1505,13 +1447,7 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     if (n == 0) return IMMESH_OK;
     const int nb = (n + VG_TILE - 1) / VG_TILE;
     const size_t need = (size_t)6 * n + (size_t)256 * nb + 8;
-    if (need > h->pub_scratch_ints) {
-        if (h->d_pub_scratch) cudaFree(h->d_pub_scratch);
-        h->d_pub_scratch = nullptr;
-        h->pub_scratch_ints = 0;
-        IM_CUDA(cudaMalloc((void**)&h->d_pub_scratch, need * sizeof(int)));
-        h->pub_scratch_ints = need;
-    }
+    IM_CUDA(h->scratch.regrow(&h->d_pub_scratch, &h->pub_scratch_ints, need));
     unsigned int* ku[2] = {(unsigned int*)h->d_pub_scratch, (unsigned int*)h->d_pub_scratch + n};
     unsigned int* vu[2] = {(unsigned int*)h->d_pub_scratch + 2 * (size_t)n, (unsigned int*)h->d_pub_scratch + 3 * (size_t)n};
     int* slots = h->d_pub_scratch + 4 * (size_t)n;
@@ -1541,14 +1477,8 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     *n_out = total;
     if (counts) for (int k = 0; k < 4; ++k) counts[k] = h->h_ints[41 + k];
     if (total > cap) return im_fail(IMMESH_E_CAPACITY, "plane markers: more rows than cap (*n_out holds the number needed; nothing was consumed)");
-    if ((size_t)total > h->pub_rows_cap || !h->d_pub_rows) {
-        if (h->d_pub_rows) cudaFree(h->d_pub_rows);
-        h->d_pub_rows = nullptr;
-        h->pub_rows_cap = 0;
-        const size_t rc = std::max<size_t>((size_t)total, 1024);
-        IM_CUDA(cudaMalloc((void**)&h->d_pub_rows, rc * IM_PUB_COLS * sizeof(double)));
-        h->pub_rows_cap = rc;
-    }
+    // at least one row, so that k_pub_emit never gets a null pointer
+    IM_CUDA(h->scratch.regrow(&h->d_pub_rows, &h->pub_rows_doubles, std::max<size_t>((size_t)total, 1) * IM_PUB_COLS, (size_t)1024 * IM_PUB_COLS));
     IM_CUDA(cudaMemsetAsync(h->map.pub_n, 0, sizeof(int), st));
     IM_LAUNCH(k_pub_emit, g, PUB_THREADS, 0, st, h->map, n, (const int*)slots, (const int*)cnt, h->d_pub_rows);
     IM_CUDA(cudaGetLastError());
@@ -1566,8 +1496,7 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, i
     const int n_max = h->dyn_last.n;              // the scan's count, or its bound when the count is device resident
     if (h->scan_rows == 0 || n_max <= 0) return IMMESH_OK;
     const int nb = (n_max + SPUB_THREADS - 1) / SPUB_THREADS;
-    rc = spub_grow(&h->d_spub_tiles, &h->spub_tiles_cap, (size_t)nb + 1);
-    if (rc) return rc;
+    IM_CUDA(h->scratch.regrow(&h->d_spub_tiles, &h->spub_tiles_cap, (size_t)nb + 1, 1024));
     int* tiles = h->d_spub_tiles;
     cudaStream_t st = h->stream;
     IM_LAUNCH(k_eff_count, nb, SPUB_THREADS, 0, st, h->sb, tiles);
@@ -1579,9 +1508,8 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, i
     *n_out = total;
     if (total > cap) return im_fail(IMMESH_E_CAPACITY, "effect cloud: more rows than cap (*n_out holds the number needed)");
     if (total == 0) return IMMESH_OK;
-    rc = spub_grow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)total);
-    if (!rc && scan_index) rc = spub_grow(&h->d_spub_idx, &h->spub_idx_cap, (size_t)total);
-    if (rc) return rc;
+    IM_CUDA(h->scratch.regrow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)total, 1024));
+    if (scan_index) IM_CUDA(h->scratch.regrow(&h->d_spub_idx, &h->spub_idx_cap, (size_t)total, 1024));
     IM_LAUNCH(k_eff_emit, nb, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)tiles, h->d_spub_rows, scan_index ? h->d_spub_idx : (int*)nullptr);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
@@ -1605,8 +1533,7 @@ static int registered_rows(immesh_lio_t* h, const float* pts, const float* inten
     }
     IM_CUDA(cudaStreamSynchronize(st));
     if (!pts) {
-        const int rc = spub_grow(&h->d_spub_tiles, &h->spub_tiles_cap, 1);
-        if (rc) return rc;
+        IM_CUDA(h->scratch.regrow(&h->d_spub_tiles, &h->spub_tiles_cap, 1, 1024));
         IM_LAUNCH(k_scan_n, 1, 1, 0, st, h->sb, h->d_spub_tiles);
         IM_CUDA(cudaGetLastError());
         IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, h->d_spub_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1620,13 +1547,11 @@ static int registered_rows(immesh_lio_t* h, const float* pts, const float* inten
     const float* src = pts;
     if (pts && !on_device) {
         const size_t floats = ((size_t)(m - 1) * point_skip + 1) * stride;   // up to the last point published
-        int rc = spub_grow(&h->d_spub_in, &h->spub_in_cap, floats);
-        if (rc) return rc;
+        IM_CUDA(h->scratch.regrow(&h->d_spub_in, &h->spub_in_cap, floats, 1024));
         IM_CUDA(cudaMemcpyAsync(h->d_spub_in, pts, floats * sizeof(float), cudaMemcpyHostToDevice, st));
         src = h->d_spub_in;
     }
-    int rc = spub_grow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)m);
-    if (rc) return rc;
+    IM_CUDA(h->scratch.regrow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)m, 1024));
     const int g = std::min((m + SPUB_THREADS - 1) / SPUB_THREADS, h->n_sm * 16);
     IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows, inten);
     IM_CUDA(cudaGetLastError());
@@ -1658,7 +1583,7 @@ int immesh_lio_capacity(immesh_lio_t* h, int64_t* out) {
     out[0] = (int64_t)h->cap; out[1] = c[5];
     out[2] = h->max_nodes; out[3] = c[0];
     out[4] = h->max_chunks; out[5] = (int64_t)c[1] - std::max(c[2], 0);
-    out[6] = (int64_t)h->dev_bytes; out[7] = h->growths;
+    out[6] = (int64_t)h->dev.bytes(); out[7] = h->growths;
     return IMMESH_OK;
 }
 int immesh_lio_reserve(immesh_lio_t* h, int64_t root_slots, int64_t nodes, int64_t chunks) {

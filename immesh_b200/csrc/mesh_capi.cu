@@ -713,17 +713,6 @@ __global__ void __launch_bounds__(MGROW_THREADS) k_rehash_tris(MeshDev from, Mes
 
 // ------------------------------------------------------------------ host side
 
-template <class T>
-static cudaError_t mdev_alloc(immesh_mesh* h, T** p, size_t count, int memset_byte = -1) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, count * sizeof(T));
-    if (e != cudaSuccess) return e;
-    h->allocs.push_back(q);
-    h->dev_bytes += count * sizeof(T);
-    *p = (T*)q;
-    if (memset_byte >= 0) e = cudaMemset(q, memset_byte, count * sizeof(T));
-    return e;
-}
 static size_t pow2_at_least(size_t v) {
     size_t p = 1;
     while (p < v) p <<= 1;
@@ -738,19 +727,13 @@ extern "C" int immesh_debug_stamps_mesh(long long* out64) {   // debug variant o
 
 extern "C" {
 
-int immesh_mesh_destroy(immesh_mesh_t* h);
 int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     if (!cfg || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     if (!(cfg->points_minimum_scale > 0) || !(cfg->voxel_resolution > 0) || cfg->number_of_pts_append_to_map < 1) return im_fail(IMMESH_E_INVALID, "bad mesh configuration");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return im_fail(IMMESH_E_NO_DEVICE, "no CUDA device: immesh_b200 has no CPU path");
-    immesh_mesh* h = new immesh_mesh();
-    // every failure below releases what has been created so far (immesh_mesh_destroy copes with a partially built handle)
-#define IM_CREATE_M(expr)                                                                   \
-    do {                                                                                    \
-        cudaError_t im_e_ = (expr);                                                         \
-        if (im_e_ != cudaSuccess) { immesh_mesh_destroy(h); return immesh::im_fail_cuda(im_e_, __FILE__, __LINE__); } \
-    } while (0)
+    immesh::Building<immesh_mesh> owner(new immesh_mesh(), immesh_mesh_destroy);   // every failure below releases what was created
+    immesh_mesh* h = owner.get();
     h->F.shard_rank = 0; h->F.shard_n = 1; h->F.x_cap = 0;
     h->F.work_rank = nullptr; h->F.tri_mark = nullptr;   // the per-frame path
     // dilated sets up to warp_nmax vertices are triangulated by one warp each (side stream), larger ones by a thread block each
@@ -774,43 +757,43 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, dev);
-    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
-    for (auto& e : h->ev) IM_CREATE_M(cudaEventCreate(&e));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    for (auto& e : h->ev) IM_CUDA(cudaEventCreate(&e));
     MeshDev& M = h->M;
     M.max_v = max_v;
     M.max_t = max_t;
-    IM_CREATE_M(mdev_alloc(h, &M.vpos, (size_t)max_v));
-    IM_CREATE_M(mdev_alloc(h, &M.vsmooth, (size_t)max_v * 3));
-    IM_CREATE_M(mdev_alloc(h, &M.vsmoothed, (size_t)max_v, 0));
-    IM_CREATE_M(mdev_alloc(h, &M.v_tri_head, (size_t)max_v, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.vpos, (size_t)max_v));
+    IM_CUDA(h->dev.alloc(&M.vsmooth, (size_t)max_v * 3));
+    IM_CUDA(h->dev.alloc(&M.vsmoothed, (size_t)max_v, 0));
+    IM_CUDA(h->dev.alloc(&M.v_tri_head, (size_t)max_v, 0xFF));
     const size_t gcap = pow2_at_least((size_t)max_v * 2);
-    IM_CREATE_M(mdev_alloc(h, &M.gkeys, gcap, 0xFF));
-    IM_CREATE_M(mdev_alloc(h, &M.gval, gcap, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.gkeys, gcap, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.gval, gcap, 0xFF));
     M.gmask = (unsigned)(gcap - 1);
     const size_t vcap = pow2_at_least((size_t)max_vox * 2);
-    IM_CREATE_M(mdev_alloc(h, &M.vkeys, vcap, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.vkeys, vcap, 0xFF));
     M.vmask = (unsigned)(vcap - 1);
-    IM_CREATE_M(mdev_alloc(h, &M.vox_chunk, vcap * IM_VCHUNKS, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.vox_chunk, vcap * IM_VCHUNKS, 0xFF));
     M.max_vchunks = max_v / 4 + 1024;
-    IM_CREATE_M(mdev_alloc(h, &M.vchunk_pts, (size_t)M.max_vchunks * 16));
-    IM_CREATE_M(mdev_alloc(h, &M.vox_count, vcap, 0));
-    IM_CREATE_M(mdev_alloc(h, &M.vox_meshing_times, vcap, 0));
-    IM_CREATE_M(mdev_alloc(h, &M.vox_new_added, vcap, 0));
-    IM_CREATE_M(mdev_alloc(h, &M.vox_frame, vcap, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.vchunk_pts, (size_t)M.max_vchunks * 16));
+    IM_CUDA(h->dev.alloc(&M.vox_count, vcap, 0));
+    IM_CUDA(h->dev.alloc(&M.vox_meshing_times, vcap, 0));
+    IM_CUDA(h->dev.alloc(&M.vox_new_added, vcap, 0));
+    IM_CUDA(h->dev.alloc(&M.vox_frame, vcap, 0xFF));
     M.vox_short_axis = nullptr;
-    IM_CREATE_M(mdev_alloc(h, &M.tri, (size_t)max_t));
-    IM_CREATE_M(mdev_alloc(h, &M.tri_next, (size_t)max_t * 3));
-    IM_CREATE_M(mdev_alloc(h, &M.tri_flip, (size_t)max_t));
+    IM_CUDA(h->dev.alloc(&M.tri, (size_t)max_t));
+    IM_CUDA(h->dev.alloc(&M.tri_next, (size_t)max_t * 3));
+    IM_CUDA(h->dev.alloc(&M.tri_flip, (size_t)max_t));
     const size_t tcap = pow2_at_least((size_t)max_t * 2);
-    IM_CREATE_M(mdev_alloc(h, &M.thash, tcap, 0xFF));
+    IM_CUDA(h->dev.alloc(&M.thash, tcap, 0xFF));
     M.tmask = (unsigned)(tcap - 1);
-    IM_CREATE_M(mdev_alloc(h, &M.cnt, 64, 0));
+    IM_CUDA(h->dev.alloc(&M.cnt, 64, 0));
     {
         int init[32];
         std::memset(init, 0, sizeof(init));
         init[11] = init[12] = init[13] = 0x7fffffff;
         init[14] = init[15] = init[16] = -0x7fffffff;
-        IM_CREATE_M(cudaMemcpy(M.cnt, init, sizeof(init), cudaMemcpyHostToDevice));
+        IM_CUDA(cudaMemcpy(M.cnt, init, sizeof(init), cudaMemcpyHostToDevice));
     }
     FrameBuf& F = h->F;
     const size_t mc = (size_t)h->max_frame_points;  // candidates <= points
@@ -818,66 +801,65 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     F.max_work = max_vox < (1 << 16) ? max_vox : std::min(std::max(max_vox / 16, 1 << 16), 1 << 18);   // voxels (re)meshed per frame; 4 KB of id list each
     F.max_act = (int)std::min<size_t>((size_t)max_vox, mc);
     F.max_list = 4 << 20;
-    IM_CREATE_M(mdev_alloc(h, &h->d_pts, IM_SLOTS * mc * 3));
-    IM_CREATE_M(mdev_alloc(h, &h->d_body, IM_SLOTS * mc * 3));   // staging of body-frame scans handed over by the localization handle (not allocated lazily: a cudaMalloc inside a frame stalls the pipeline)
+    IM_CUDA(h->dev.alloc(&h->d_pts, IM_SLOTS * mc * 3));
+    IM_CUDA(h->dev.alloc(&h->d_body, IM_SLOTS * mc * 3));   // staging of body-frame scans handed over by the localization handle (not allocated lazily: an allocation inside a frame stalls the pipeline)
     F.pts = h->d_pts;
-    IM_CREATE_M(mdev_alloc(h, &h->d_fp, IM_SLOTS));
-    for (int i = 0; i < IM_SLOTS; ++i) { IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_in[i], cudaEventDisableTiming)); IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming)); }
-    IM_CREATE_M(mdev_alloc(h, &F.cand_gkey, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_vslot, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_status, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_scan, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_conf, mc * IM_CONF_K));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_nconf, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_next, mc));
-    IM_CREATE_M(mdev_alloc(h, &F.cand_pos, mc));
+    IM_CUDA(h->dev.alloc(&h->d_fp, IM_SLOTS));
+    for (int i = 0; i < IM_SLOTS; ++i) { IM_CUDA(cudaEventCreateWithFlags(&h->ev_in[i], cudaEventDisableTiming)); IM_CUDA(cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming)); }
+    IM_CUDA(h->dev.alloc(&F.cand_gkey, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_vslot, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_status, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_scan, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_conf, mc * IM_CONF_K));
+    IM_CUDA(h->dev.alloc(&F.cand_nconf, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_next, mc));
+    IM_CUDA(h->dev.alloc(&F.cand_pos, mc));
     h->ccap = pow2_at_least(mc * 2);
-    IM_CREATE_M(mdev_alloc(h, &F.ckeys, h->ccap));
-    IM_CREATE_M(mdev_alloc(h, &F.chead, h->ccap));
+    IM_CUDA(h->dev.alloc(&F.ckeys, h->ccap));
+    IM_CUDA(h->dev.alloc(&F.chead, h->ccap));
     F.scan_block = nullptr;
-    IM_CREATE_M(mdev_alloc(h, &F.act, (size_t)F.max_act));
-    IM_CREATE_M(mdev_alloc(h, &F.work, (size_t)F.max_work));
-    IM_CREATE_M(mdev_alloc(h, &F.work_n_ids, (size_t)F.max_work));
-    IM_CREATE_M(mdev_alloc(h, &F.work_ids, (size_t)F.max_work * IM_MAXD));
-    IM_CREATE_M(mdev_alloc(h, &F.work_nfaces, (size_t)F.max_work));
-    IM_CREATE_M(mdev_alloc(h, &F.work_bits, (size_t)F.max_work * (IM_MAXG / 32), 0));
-    IM_CREATE_M(mdev_alloc(h, &F.work_ring, (size_t)F.max_work, 0));
-    IM_CREATE_M(mdev_alloc(h, &F.work_done, (size_t)F.max_work, 0));
+    IM_CUDA(h->dev.alloc(&F.act, (size_t)F.max_act));
+    IM_CUDA(h->dev.alloc(&F.work, (size_t)F.max_work));
+    IM_CUDA(h->dev.alloc(&F.work_n_ids, (size_t)F.max_work));
+    IM_CUDA(h->dev.alloc(&F.work_ids, (size_t)F.max_work * IM_MAXD));
+    IM_CUDA(h->dev.alloc(&F.work_nfaces, (size_t)F.max_work));
+    IM_CUDA(h->dev.alloc(&F.work_bits, (size_t)F.max_work * (IM_MAXG / 32), 0));
+    IM_CUDA(h->dev.alloc(&F.work_ring, (size_t)F.max_work, 0));
+    IM_CUDA(h->dev.alloc(&F.work_done, (size_t)F.max_work, 0));
     F.max_ditem = F.max_work * 4;
-    IM_CREATE_M(mdev_alloc(h, &F.ditem, (size_t)F.max_ditem));
+    IM_CUDA(h->dev.alloc(&F.ditem, (size_t)F.max_ditem));
     F.max_vref = 8 << 20;
-    IM_CREATE_M(mdev_alloc(h, &F.all_faces, (size_t)F.max_list));
-    IM_CREATE_M(mdev_alloc(h, &F.all_vref, (size_t)F.max_vref));
-    IM_CREATE_M(mdev_alloc(h, &F.pulled, (size_t)F.max_list * 2));
+    IM_CUDA(h->dev.alloc(&F.all_faces, (size_t)F.max_list));
+    IM_CUDA(h->dev.alloc(&F.all_vref, (size_t)F.max_vref));
+    IM_CUDA(h->dev.alloc(&F.pulled, (size_t)F.max_list * 2));
     F.fset_mask = (1u << 21) - 1;
-    IM_CREATE_M(mdev_alloc(h, &F.fset, (size_t)F.fset_mask + 1, 0xFF));
-    IM_CREATE_M(mdev_alloc(h, &F.work_axes, (size_t)F.max_work * 9));
-    IM_CREATE_M(mdev_alloc(h, &F.add_tri, (size_t)F.max_list * 3));
-    IM_CREATE_M(mdev_alloc(h, &F.add_flip, (size_t)F.max_list));
-    IM_CREATE_M(mdev_alloc(h, &F.rem_tri, (size_t)F.max_list));
-    IM_CREATE_M(cudaMallocHost((void**)&h->h_pts, IM_SLOTS * mc * 3 * sizeof(float)));
-    IM_CREATE_M(cudaMallocHost((void**)&h->h_cnt, IM_SLOTS * 32 * sizeof(int)));
-    IM_CREATE_M(cudaMallocHost((void**)&h->h_fp, IM_SLOTS * sizeof(FramePose)));
-    IM_CREATE_M(cudaMallocHost((void**)&h->h_dyn, IM_SLOTS * sizeof(FrameDyn)));
-    IM_CREATE_M(mdev_alloc(h, &h->d_dyn, 1, 0));
-    IM_CREATE_M(mdev_alloc(h, &h->cam_ring, IM_RF_RING, 0));
-    IM_CREATE_M(mdev_alloc(h, &h->cam_ring_frame, IM_RF_RING, 0));
+    IM_CUDA(h->dev.alloc(&F.fset, (size_t)F.fset_mask + 1, 0xFF));
+    IM_CUDA(h->dev.alloc(&F.work_axes, (size_t)F.max_work * 9));
+    IM_CUDA(h->dev.alloc(&F.add_tri, (size_t)F.max_list * 3));
+    IM_CUDA(h->dev.alloc(&F.add_flip, (size_t)F.max_list));
+    IM_CUDA(h->dev.alloc(&F.rem_tri, (size_t)F.max_list));
+    IM_CUDA(h->pinned.alloc(&h->h_pts, IM_SLOTS * mc * 3));
+    IM_CUDA(h->pinned.alloc(&h->h_cnt, IM_SLOTS * 32));
+    IM_CUDA(h->pinned.alloc(&h->h_fp, IM_SLOTS));
+    IM_CUDA(h->pinned.alloc(&h->h_dyn, IM_SLOTS));
+    IM_CUDA(h->dev.alloc(&h->d_dyn, 1, 0));
+    IM_CUDA(h->dev.alloc(&h->cam_ring, IM_RF_RING, 0));
+    IM_CUDA(h->dev.alloc(&h->cam_ring_frame, IM_RF_RING, 0));
     F.dyn = h->d_dyn;
     F.epoch = 0;
-    IM_CREATE_M(cudaFuncSetAttribute(k_voxel_mesh<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<1024>)));
-    IM_CREATE_M(cudaFuncSetAttribute(k_voxel_tri_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * sizeof(MeshWarpSmem<128>))));
-    IM_CREATE_M(cudaFuncSetAttribute(k_voxel_mesh<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<256>)));
-    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
-    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream3, cudaStreamNonBlocking));
-    IM_CREATE_M(cudaStreamCreateWithFlags(&h->stream_up, cudaStreamNonBlocking));
-    for (int i = 0; i < IM_SLOTS; ++i) IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_up[i], cudaEventDisableTiming));
-    IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-    IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
-    IM_CREATE_M(cudaEventCreateWithFlags(&h->ev_join3, cudaEventDisableTiming));
+    IM_CUDA(cudaFuncSetAttribute(k_voxel_mesh<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<1024>)));
+    IM_CUDA(cudaFuncSetAttribute(k_voxel_tri_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(4 * sizeof(MeshWarpSmem<128>))));
+    IM_CUDA(cudaFuncSetAttribute(k_voxel_mesh<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(MeshSmem<256>)));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream3, cudaStreamNonBlocking));
+    IM_CUDA(cudaStreamCreateWithFlags(&h->stream_up, cudaStreamNonBlocking));
+    for (int i = 0; i < IM_SLOTS; ++i) IM_CUDA(cudaEventCreateWithFlags(&h->ev_up[i], cudaEventDisableTiming));
+    IM_CUDA(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
+    IM_CUDA(cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
+    IM_CUDA(cudaEventCreateWithFlags(&h->ev_join3, cudaEventDisableTiming));
     std::memset(h->last_cnt, 0, sizeof(h->last_cnt));
-    IM_CREATE_M(cudaDeviceSynchronize());
-#undef IM_CREATE_M
-    *out = h;
+    IM_CUDA(cudaDeviceSynchronize());
+    *out = owner.release();
     return IMMESH_OK;
 }
 
@@ -887,14 +869,6 @@ int immesh_mesh_destroy(immesh_mesh_t* h) {
     h->graph.destroy();
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && immesh::nccl().CommDestroy) immesh::nccl().CommDestroy(h->nccl_comm);
-    for (void* p : h->allocs) cudaFree(p);
-    for (void* p : h->rb_buf) if (p) cudaFree(p);
-    for (void* p : h->rf.bufs) cudaFree(p);
-    if (h->rf.h_rd) cudaFreeHost(h->rf.h_rd);
-    if (h->h_pts) cudaFreeHost(h->h_pts);
-    if (h->h_cnt) cudaFreeHost(h->h_cnt);
-    if (h->h_fp) cudaFreeHost(h->h_fp);
-    if (h->h_dyn) cudaFreeHost(h->h_dyn);
     for (int i = 0; i < IM_SLOTS; ++i) { if (h->ev_in[i]) cudaEventDestroy(h->ev_in[i]); if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]); }
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
     if (h->stream) cudaStreamDestroy(h->stream);
@@ -1101,7 +1075,7 @@ static void mesh_note(immesh_mesh* h, const int* c, int frame) {
 }
 // Enlarge the pools to (vertices, triangles, voxels), each >= the current one: as lio_grow (lio_capi.cu) -- drain, allocate all,
 // migrate on the stream, free the old buffers, drop the captured launch sequence.  The batched frame's scratch (sized by max_voxels
-// and max_triangles) is freed and allocated again at the new sizes by the next batched frame.
+// and max_triangles) is freed, and allocated again at the new sizes by the next batched frame.
 static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long vox) {
     if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "a sharded mesh handle cannot grow (its replicas would have to grow in lockstep)");
     if (verts > IM_MPOOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "vertex pool: more than 2^30 vertices (32-bit vertex ids)");
@@ -1112,8 +1086,8 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
     const bool gv = verts > v0, gt = tris > t0, gx = vox > x0;
     if (!gv && !gt && !gx) return IMMESH_OK;
     verts = std::max(verts, v0); tris = std::max(tris, t0); vox = std::max(vox, x0);
-    const size_t drop = h->b_fp ? h->b_bytes : 0;   // the batched frame's scratch goes
-    const size_t bytes = h->dev_bytes - drop - mesh_pool_bytes(h, v0, t0, x0) + mesh_pool_bytes(h, verts, tris, vox);
+    // the batched frame's scratch (h->batch) goes, so it is not part of the sum
+    const size_t bytes = h->dev.bytes() - mesh_pool_bytes(h, v0, t0, x0) + mesh_pool_bytes(h, verts, tris, vox);
     if (h->grow_max_bytes > 0 && bytes > (size_t)h->grow_max_bytes) {
         const std::string pools = std::string(gv ? " vertex pool" : "") + (gt ? " triangle pool" : "") + (gx ? " voxel hash" : "");
         return im_fail(IMMESH_E_CAPACITY, ("growth of the" + pools + " to " + std::to_string(bytes) + " device bytes is above the ceiling of " +
@@ -1125,40 +1099,33 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
     const int nv = std::min(c[0], M.max_v), nt = std::min(c[1], M.max_t), nch = std::min(c[27], M.max_vchunks);
     MeshDev nm = M;
     FrameBuf nf = h->F;
-    std::vector<void*> fresh;
+    immesh::MemSet fresh;   // the new buffers, freed on every failure below
     const char* pool = "";
-    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
-        void* q = nullptr;
-        const cudaError_t e = cudaMalloc(&q, count * sizeof(**p));
-        if (e == cudaSuccess) { fresh.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
-        return e;
-    };
     const size_t gcap = pow2_at_least((size_t)verts * 2), tcap = pow2_at_least((size_t)tris * 2), vcap = pow2_at_least((size_t)vox * 2);
     const int vch = (int)(verts / 4 + 1024), act = (int)std::min<long long>(vox, h->max_frame_points);
     cudaError_t e = cudaSuccess;
     if (gv) {
         pool = "vertex pool";
-        if ((e = alloc(&nm.vpos, verts)) == cudaSuccess && (e = alloc(&nm.vsmooth, verts * 3)) == cudaSuccess && (e = alloc(&nm.vsmoothed, verts)) == cudaSuccess &&
-            (e = alloc(&nm.v_tri_head, verts)) == cudaSuccess && (e = alloc(&nm.vchunk_pts, (size_t)vch * 16)) == cudaSuccess && gcap > (size_t)M.gmask + 1 &&
-            (e = alloc(&nm.gkeys, gcap)) == cudaSuccess)
-            e = alloc(&nm.gval, gcap);
+        if ((e = fresh.alloc(&nm.vpos, verts)) == cudaSuccess && (e = fresh.alloc(&nm.vsmooth, verts * 3)) == cudaSuccess && (e = fresh.alloc(&nm.vsmoothed, verts)) == cudaSuccess &&
+            (e = fresh.alloc(&nm.v_tri_head, verts)) == cudaSuccess && (e = fresh.alloc(&nm.vchunk_pts, (size_t)vch * 16)) == cudaSuccess && gcap > (size_t)M.gmask + 1 &&
+            (e = fresh.alloc(&nm.gkeys, gcap)) == cudaSuccess)
+            e = fresh.alloc(&nm.gval, gcap);
     }
     if (gt && e == cudaSuccess) {
         pool = "triangle pool";
-        if ((e = alloc(&nm.tri, tris)) == cudaSuccess && (e = alloc(&nm.tri_next, tris * 3)) == cudaSuccess && (e = alloc(&nm.tri_flip, tris)) == cudaSuccess &&
+        if ((e = fresh.alloc(&nm.tri, tris)) == cudaSuccess && (e = fresh.alloc(&nm.tri_next, tris * 3)) == cudaSuccess && (e = fresh.alloc(&nm.tri_flip, tris)) == cudaSuccess &&
             tcap > (size_t)M.tmask + 1)
-            e = alloc(&nm.thash, tcap);
+            e = fresh.alloc(&nm.thash, tcap);
     }
     if (gx && e == cudaSuccess) {
         pool = "voxel hash";
-        if (vcap > (size_t)M.vmask + 1 && (e = alloc(&nm.vkeys, vcap)) == cudaSuccess && (e = alloc(&nm.vox_chunk, vcap * IM_VCHUNKS)) == cudaSuccess &&
-            (e = alloc(&nm.vox_count, vcap)) == cudaSuccess && (e = alloc(&nm.vox_meshing_times, vcap)) == cudaSuccess &&
-            (e = alloc(&nm.vox_new_added, vcap)) == cudaSuccess)
-            e = alloc(&nm.vox_frame, vcap);
-        if (e == cudaSuccess && act > h->F.max_act) e = alloc(&nf.act, act);
+        if (vcap > (size_t)M.vmask + 1 && (e = fresh.alloc(&nm.vkeys, vcap)) == cudaSuccess && (e = fresh.alloc(&nm.vox_chunk, vcap * IM_VCHUNKS)) == cudaSuccess &&
+            (e = fresh.alloc(&nm.vox_count, vcap)) == cudaSuccess && (e = fresh.alloc(&nm.vox_meshing_times, vcap)) == cudaSuccess &&
+            (e = fresh.alloc(&nm.vox_new_added, vcap)) == cudaSuccess)
+            e = fresh.alloc(&nm.vox_frame, vcap);
+        if (e == cudaSuccess && act > h->F.max_act) e = fresh.alloc(&nf.act, act);
     }
     auto fail = [&](cudaError_t err, const char* what) {
-        for (void* q : fresh) cudaFree(q);
         cudaGetLastError();
         return im_fail(err == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA,
                        (std::string(what) + ": " + cudaGetErrorString(err) + " during the growth; the handle is unchanged").c_str());
@@ -1216,34 +1183,25 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
     };
     e = migrate();
     if (e != cudaSuccess) return fail(e, "mesh migration");   // the old buffers were only read: the handle is as it was
-    auto swap_buf = [&](void* oldp, void* newp) {
-        if (oldp == newp) return;
-        for (void*& q : h->allocs)
-            if (q == oldp) q = newp;
-        cudaFree(oldp);
-    };
-    swap_buf(M.vpos, nm.vpos); swap_buf(M.vsmooth, nm.vsmooth); swap_buf(M.vsmoothed, nm.vsmoothed); swap_buf(M.v_tri_head, nm.v_tri_head);
-    swap_buf(M.vchunk_pts, nm.vchunk_pts); swap_buf(M.gkeys, nm.gkeys); swap_buf(M.gval, nm.gval);
-    swap_buf(M.tri, nm.tri); swap_buf(M.tri_next, nm.tri_next); swap_buf(M.tri_flip, nm.tri_flip); swap_buf(M.thash, nm.thash);
-    swap_buf(M.vkeys, nm.vkeys); swap_buf(M.vox_chunk, nm.vox_chunk); swap_buf(M.vox_count, nm.vox_count);
-    swap_buf(M.vox_meshing_times, nm.vox_meshing_times); swap_buf(M.vox_new_added, nm.vox_new_added); swap_buf(M.vox_frame, nm.vox_frame);
-    swap_buf(h->F.act, nf.act);
+    // the replaced buffers go; the new ones join the handle's device memory
+    const std::pair<const void*, const void*> replaced[] = {   // (old, new)
+        {M.vpos, nm.vpos}, {M.vsmooth, nm.vsmooth}, {M.vsmoothed, nm.vsmoothed}, {M.v_tri_head, nm.v_tri_head}, {M.vchunk_pts, nm.vchunk_pts},
+        {M.gkeys, nm.gkeys}, {M.gval, nm.gval}, {M.tri, nm.tri}, {M.tri_next, nm.tri_next}, {M.tri_flip, nm.tri_flip}, {M.thash, nm.thash},
+        {M.vkeys, nm.vkeys}, {M.vox_chunk, nm.vox_chunk}, {M.vox_count, nm.vox_count}, {M.vox_meshing_times, nm.vox_meshing_times},
+        {M.vox_new_added, nm.vox_new_added}, {M.vox_frame, nm.vox_frame}, {h->F.act, nf.act}};
+    for (const auto& r : replaced)
+        if (r.first != r.second) h->dev.free(r.first);
+    h->dev.take(std::move(fresh));
     if (h->b_fp) {   // batched-frame scratch: allocated again at the new sizes by the next batched frame
-        for (void* q : {(void*)h->b_act, (void*)h->b_sel, (void*)h->b_key, (void*)h->b_ku, (void*)h->b_vu, (void*)h->b_hist, (void*)h->b_rank,
-                        (void*)h->b_mark, (void*)h->b_fset, (void*)h->b_fp}) {
-            h->allocs.erase(std::remove(h->allocs.begin(), h->allocs.end(), q), h->allocs.end());
-            cudaFree(q);
-        }
+        h->batch = immesh::MemSet();
         h->b_act = h->b_sel = h->b_rank = h->b_hist = h->b_fset = nullptr;
         h->b_key = nullptr; h->b_ku = h->b_vu = nullptr; h->b_mark = nullptr; h->b_fp = nullptr;
-        h->b_bytes = 0;
     }
     nf.max_act = std::max(h->F.max_act, act);
     M = nm;
     h->F.act = nf.act;
     h->F.max_act = nf.max_act;
     h->max_vox = (int)vox;
-    h->dev_bytes = bytes;
     h->growths++;
     h->graph.destroy();
     IM_CUDA(cudaGetLastError());
@@ -1281,11 +1239,6 @@ static int mesh_growth_check(immesh_mesh* h, long long m) {
     return IMMESH_OK;
 }
 
-static bool mesh_host_ptr_is_pinned(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeHost;
-}
 static int mesh_grid_fixed(const immesh_mesh* h, long long n_cap, int threads, int waves = 8) {
     long long g = (n_cap + threads - 1) / threads;
     if (g > (long long)h->n_sm * waves) g = (long long)h->n_sm * waves;
@@ -1347,7 +1300,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         if (n > 0) {
             if (src_mode == 0) {
                 const float* src = xyz;
-                if (!mesh_host_ptr_is_pinned(xyz)) { std::memcpy(h_pts, xyz, (size_t)n * 3 * sizeof(float)); src = h_pts; }
+                if (!immesh::host_ptr_is_pinned(xyz)) { std::memcpy(h_pts, xyz, (size_t)n * 3 * sizeof(float)); src = h_pts; }
                 IM_CUDA(cudaMemcpyAsync(d_pts, src, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream_up));
                 IM_CUDA(cudaEventRecord(h->ev_up[s], h->stream_up));
                 IM_CUDA(cudaStreamWaitEvent(st, h->ev_up[s], 0));
@@ -1359,9 +1312,8 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         // the body-frame scan does not depend on the localization: it is uploaded on the mesh stream right away
         d_body = xyz;
         if (src_mode == 2 && n > 0) {
-            if (!h->d_body) IM_CUDA(mdev_alloc(h, &h->d_body, IM_SLOTS * slot_pts));
             const float* src = xyz;
-            if (!mesh_host_ptr_is_pinned(xyz)) { std::memcpy(h_pts, xyz, (size_t)n * 3 * sizeof(float)); src = h_pts; }
+            if (!immesh::host_ptr_is_pinned(xyz)) { std::memcpy(h_pts, xyz, (size_t)n * 3 * sizeof(float)); src = h_pts; }
             // upload stream: overlaps the kernels of the frame before (slot s was released by mesh_harvest above)
             IM_CUDA(cudaMemcpyAsync(h->d_body + s * slot_pts, src, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream_up));
             IM_CUDA(cudaEventRecord(h->ev_up[s], h->stream_up));
@@ -1553,8 +1505,8 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     h->seg1_bytes = 16 + (size_t)F.x_cap * sizeof(immesh::XSmooth);
     h->seg2_bytes = 16 + (size_t)F.x_cap * (16 + 8 + 16);
     unsigned char *s1 = nullptr, *s2 = nullptr;
-    IM_CUDA(mdev_alloc(h, &s1, h->seg1_bytes, 0));
-    IM_CUDA(mdev_alloc(h, &s2, h->seg2_bytes, 0));
+    IM_CUDA(h->dev.alloc(&s1, h->seg1_bytes, 0));
+    IM_CUDA(h->dev.alloc(&s2, h->seg2_bytes, 0));
     // receive areas: inside a peer window (other ranks store into it over NVLink) or, with NCCL transport, private buffers
     const char* force_nccl = std::getenv("IMMESH_SHARD_NCCL");
     if (!(force_nccl && force_nccl[0] == '1')) {
@@ -1567,10 +1519,10 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (h->win.ok) {
         h->d_recv1 = h->win.local + 256;
         h->d_recv2 = h->win.local + 256 + h->seg1_bytes * (size_t)nranks;
-        IM_CUDA(mdev_alloc(h, &h->d_xdone, 2, 0));
+        IM_CUDA(h->dev.alloc(&h->d_xdone, 2, 0));
     } else {
-        IM_CUDA(mdev_alloc(h, &h->d_recv1, h->seg1_bytes * nranks, 0));
-        IM_CUDA(mdev_alloc(h, &h->d_recv2, h->seg2_bytes * nranks, 0));
+        IM_CUDA(h->dev.alloc(&h->d_recv1, h->seg1_bytes * nranks, 0));
+        IM_CUDA(h->dev.alloc(&h->d_recv2, h->seg2_bytes * nranks, 0));
     }
     h->d_seg1 = s1; h->d_seg2 = s2;
     F.x_smooth = (immesh::XSmooth*)(s1 + 16);
@@ -1613,7 +1565,7 @@ int immesh_mesh_capacity(immesh_mesh_t* h, int64_t* out) {
     out[0] = h->M.max_v; out[1] = c[0];
     out[2] = h->M.max_t; out[3] = c[1];
     out[4] = h->max_vox; out[5] = c[4];
-    out[6] = (int64_t)h->dev_bytes; out[7] = h->growths;
+    out[6] = (int64_t)(h->dev.bytes() + h->batch.bytes()); out[7] = h->growths;
     return IMMESH_OK;
 }
 int immesh_mesh_reserve(immesh_mesh_t* h, int64_t vertices, int64_t triangles, int64_t voxels) {
@@ -1659,17 +1611,17 @@ int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, 
         for (int i = 0; i < nv; ++i) { vertices[i * 3] = v[i].x; vertices[i * 3 + 1] = v[i].y; vertices[i * 3 + 2] = v[i].z; }
     }
     if ((triangles || flips) && nlive > 0) {
+        immesh::MemSet tmp;
         int *d_tri = nullptr, *d_flip = nullptr, *d_n = nullptr;
-        IM_CUDA(cudaMalloc(&d_tri, (size_t)nlive * 3 * sizeof(int)));
-        IM_CUDA(cudaMalloc(&d_flip, (size_t)nlive * sizeof(int)));
-        IM_CUDA(cudaMalloc(&d_n, sizeof(int)));
+        IM_CUDA(tmp.alloc(&d_tri, (size_t)nlive * 3));
+        IM_CUDA(tmp.alloc(&d_flip, (size_t)nlive));
+        IM_CUDA(tmp.alloc(&d_n, 1));
         IM_CUDA(cudaMemset(d_n, 0, sizeof(int)));
         IM_LAUNCH(k_snapshot, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, d_tri, d_flip, d_n);
         std::vector<int> t((size_t)nlive * 3), f(nlive);
         IM_CUDA(cudaMemcpyAsync(t.data(), d_tri, (size_t)nlive * 3 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         IM_CUDA(cudaMemcpyAsync(f.data(), d_flip, (size_t)nlive * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         IM_CUDA(cudaStreamSynchronize(h->stream));
-        cudaFree(d_tri); cudaFree(d_flip); cudaFree(d_n);
         std::vector<int> order(nlive);
         for (int i = 0; i < nlive; ++i) order[i] = i;
         std::sort(order.begin(), order.end(), [&](int a, int b) {
@@ -1689,19 +1641,19 @@ int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, 
 int immesh_knn(immesh_mesh_t* h, const float* query_xyz, int nq, int k, double max_dist, int32_t* idx, float* d2) {
     if (!h || !query_xyz || !idx || !d2 || nq < 0 || k < 1 || k > KNN_KMAX) return im_fail(IMMESH_E_INVALID, "bad argument (k must be in [1,32])");
     if (nq == 0) return IMMESH_OK;
+    immesh::MemSet tmp;
     float* dq = nullptr;
     int* di = nullptr;
     float* dd = nullptr;
-    IM_CUDA(cudaMalloc(&dq, (size_t)nq * 3 * sizeof(float)));
-    IM_CUDA(cudaMalloc(&di, (size_t)nq * k * sizeof(int)));
-    IM_CUDA(cudaMalloc(&dd, (size_t)nq * k * sizeof(float)));
+    IM_CUDA(tmp.alloc(&dq, (size_t)nq * 3));
+    IM_CUDA(tmp.alloc(&di, (size_t)nq * k));
+    IM_CUDA(tmp.alloc(&dd, (size_t)nq * k));
     IM_CUDA(cudaMemcpyAsync(dq, query_xyz, (size_t)nq * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream));
     IM_LAUNCH(k_knn, mesh_grid(h, nq * 32, 128), 128, 0, h->stream, h->M, h->P, (const float*)dq, 3, nq, k, max_dist, di, dd);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(idx, di, (size_t)nq * k * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaMemcpyAsync(d2, dd, (size_t)nq * k * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    cudaFree(dq); cudaFree(di); cudaFree(dd);
     return IMMESH_OK;
 }
 
@@ -1712,18 +1664,18 @@ int immesh_mesh_smooth_all(immesh_mesh_t* h, double smooth_factor, int knn, doub
     IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
     const int nv = cnt[0];
     if (nv == 0) return IMMESH_OK;
+    immesh::MemSet tmp;
     int* di = nullptr;
     float* dd = nullptr;
     double* dout = nullptr;
-    IM_CUDA(cudaMalloc(&di, (size_t)nv * knn * sizeof(int)));
-    IM_CUDA(cudaMalloc(&dd, (size_t)nv * knn * sizeof(float)));
-    if (smoothed) IM_CUDA(cudaMalloc(&dout, (size_t)nv * 3 * sizeof(double)));
+    IM_CUDA(tmp.alloc(&di, (size_t)nv * knn));
+    IM_CUDA(tmp.alloc(&dd, (size_t)nv * knn));
+    if (smoothed) IM_CUDA(tmp.alloc(&dout, (size_t)nv * 3));
     IM_LAUNCH(k_knn, mesh_grid(h, nv, 4), 128, 0, h->stream, h->M, h->P, (const float*)h->M.vpos, 4, nv, knn, (double)INFINITY, di, dd);
     IM_LAUNCH(k_smooth_all, mesh_grid(h, nv, 128), 128, 0, h->stream, h->M, nv, knn, (const int*)di, (const float*)dd, smooth_factor, h->P.accept, dout);
     IM_CUDA(cudaGetLastError());
     if (smoothed) IM_CUDA(cudaMemcpyAsync(smoothed, dout, (size_t)nv * 3 * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    cudaFree(di); cudaFree(dd); if (dout) cudaFree(dout);
     return IMMESH_OK;
 }
 
@@ -1735,17 +1687,17 @@ int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* reg
     const int nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
     *n_regions = 0;
     if (nlive == 0) { if (region_offsets && cap_regions >= 0) region_offsets[0] = 0; return IMMESH_OK; }
+    immesh::MemSet tmp;
     int *d_tri = nullptr, *d_key = nullptr, *d_n = nullptr;
-    IM_CUDA(cudaMalloc(&d_tri, (size_t)nlive * 3 * sizeof(int)));
-    IM_CUDA(cudaMalloc(&d_key, (size_t)nlive * 3 * sizeof(int)));
-    IM_CUDA(cudaMalloc(&d_n, sizeof(int)));
+    IM_CUDA(tmp.alloc(&d_tri, (size_t)nlive * 3));
+    IM_CUDA(tmp.alloc(&d_key, (size_t)nlive * 3));
+    IM_CUDA(tmp.alloc(&d_n, 1));
     IM_CUDA(cudaMemset(d_n, 0, sizeof(int)));
     IM_LAUNCH(k_region_keys, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, region_size, d_tri, d_key, d_n);
     std::vector<int> t((size_t)nlive * 3), kx((size_t)nlive * 3);
     IM_CUDA(cudaMemcpyAsync(t.data(), d_tri, t.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaMemcpyAsync(kx.data(), d_key, kx.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    cudaFree(d_tri); cudaFree(d_key); cudaFree(d_n);
     std::vector<int> order(nlive);
     for (int i = 0; i < nlive; ++i) order[i] = i;
     std::sort(order.begin(), order.end(), [&](int a, int b) {   // regions by ascending key, triangles by ascending triple inside a region
@@ -1774,19 +1726,6 @@ int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* reg
     return nr <= cap_regions ? IMMESH_OK : im_fail(IMMESH_E_CAPACITY, "more regions than cap_regions");
 }
 
-// scratch buffer i of the region-buffer call, at least `bytes` long (grow-only)
-static cudaError_t rb_scratch(immesh_mesh* h, int i, size_t bytes, void** out) {
-    if (bytes > h->rb_cap[i]) {
-        if (h->rb_buf[i]) cudaFree(h->rb_buf[i]);
-        h->rb_buf[i] = nullptr;
-        h->rb_cap[i] = 0;
-        const cudaError_t e = cudaMalloc(&h->rb_buf[i], std::max<size_t>(bytes, 4096));
-        if (e != cudaSuccess) return e;
-        h->rb_cap[i] = std::max<size_t>(bytes, 4096);
-    }
-    *out = h->rb_buf[i];
-    return cudaSuccess;
-}
 static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
     int b = 0;
     while (b < 64 && (max_value >> b)) ++b;
@@ -1829,14 +1768,20 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
     const int nv = cnt[0], nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
     const size_t nl = (size_t)std::max(nlive, 1);
+    // scratch buffer i of the call, at least `bytes` long (grow-only, kept by the handle)
+    auto grown = [h](int i, size_t bytes, void** out) {
+        const cudaError_t e = h->scratch.regrow(&h->region_scratch[i], &h->region_scratch_cap[i], bytes, 4096);
+        *out = h->region_scratch[i];
+        return e;
+    };
     void *p_slot, *p_rk, *p_k, *p_v, *p_flag, *p_misc, *p_q;
-    IM_CUDA(rb_scratch(h, 0, nl * sizeof(int), &p_slot));
-    IM_CUDA(rb_scratch(h, 1, nl * sizeof(unsigned long long), &p_rk));
-    IM_CUDA(rb_scratch(h, 2, nl * 2 * sizeof(unsigned int), &p_k));
-    IM_CUDA(rb_scratch(h, 3, nl * 2 * sizeof(unsigned int), &p_v));
-    IM_CUDA(rb_scratch(h, 4, (nl + 1) * sizeof(int), &p_flag));
-    IM_CUDA(rb_scratch(h, 5, 8 * sizeof(int), &p_misc));
-    IM_CUDA(rb_scratch(h, 6, std::max<size_t>(qk.size(), 1) * (sizeof(unsigned long long) + sizeof(int)), &p_q));
+    IM_CUDA(grown(0, nl * sizeof(int), &p_slot));
+    IM_CUDA(grown(1, nl * sizeof(unsigned long long), &p_rk));
+    IM_CUDA(grown(2, nl * 2 * sizeof(unsigned int), &p_k));
+    IM_CUDA(grown(3, nl * 2 * sizeof(unsigned int), &p_v));
+    IM_CUDA(grown(4, (nl + 1) * sizeof(int), &p_flag));
+    IM_CUDA(grown(5, 8 * sizeof(int), &p_misc));
+    IM_CUDA(grown(6, std::max<size_t>(qk.size(), 1) * (sizeof(unsigned long long) + sizeof(int)), &p_q));
     int* slot = (int*)p_slot;
     unsigned long long* rk = (unsigned long long*)p_rk;
     unsigned int* ku[2] = {(unsigned int*)p_k, (unsigned int*)p_k + nl};
@@ -1865,7 +1810,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     if (n > 0) {
         const int nb = (n + VG_TILE - 1) / VG_TILE;
         void* p_hist;
-        IM_CUDA(rb_scratch(h, 7, (size_t)256 * nb * sizeof(int), &p_hist));
+        IM_CUDA(grown(7, (size_t)256 * nb * sizeof(int), &p_hist));
         int* hist = (int*)p_hist;
         const int g = mesh_grid(h, n, RB_THREADS);
         const int tri_passes = rb_passes((unsigned long long)std::max(nv - 1, 0));
@@ -1897,7 +1842,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
         return im_fail(IMMESH_E_CAPACITY, "region_buffers: more triangles than cap or more regions than cap_regions (*n_tris / *n_regions hold the numbers needed; nothing was smoothed)");
     const unsigned int* order = vu[cur];
     void *p_reg, *p_rows, *p_part, *p_box;
-    IM_CUDA(rb_scratch(h, 8, ((size_t)nr * 3 + (size_t)nr + 1) * sizeof(int), &p_reg));
+    IM_CUDA(grown(8, ((size_t)nr * 3 + (size_t)nr + 1) * sizeof(int), &p_reg));
     int* d_rkeys = (int*)p_reg;
     int* d_roff = d_rkeys + (size_t)nr * 3;
     int* h_off_src = nullptr;
@@ -1915,10 +1860,10 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     int nq = 0;
     if (n > 0) {
         void *p_bits, *p_list, *p_qpos;
-        IM_CUDA(rb_scratch(h, 9, (((size_t)nv + 31) / 32) * sizeof(unsigned int), &p_bits));
+        IM_CUDA(grown(9, (((size_t)nv + 31) / 32) * sizeof(unsigned int), &p_bits));
         const size_t qmax = (size_t)std::min<long long>((long long)nv, 3LL * n);
-        IM_CUDA(rb_scratch(h, 10, qmax * sizeof(int), &p_list));
-        IM_CUDA(rb_scratch(h, 11, qmax * sizeof(float4), &p_qpos));
+        IM_CUDA(grown(10, qmax * sizeof(int), &p_list));
+        IM_CUDA(grown(11, qmax * sizeof(float4), &p_qpos));
         IM_CUDA(cudaMemsetAsync(p_bits, 0, (((size_t)nv + 31) / 32) * sizeof(unsigned int), st));
         IM_LAUNCH(k_rb_claim, mesh_grid(h, 3 * n, RB_THREADS), RB_THREADS, 0, st, h->M, n, (const int*)slot, (unsigned int*)p_bits, misc, (int*)p_list, (float4*)p_qpos);
         IM_CUDA(cudaGetLastError());
@@ -1927,8 +1872,8 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
         nq = hm[2];
         if (nq > 0) {
             void *p_idx, *p_d2;
-            IM_CUDA(rb_scratch(h, 12, (size_t)nq * knn * sizeof(int), &p_idx));
-            IM_CUDA(rb_scratch(h, 13, (size_t)nq * knn * sizeof(float), &p_d2));
+            IM_CUDA(grown(12, (size_t)nq * knn * sizeof(int), &p_idx));
+            IM_CUDA(grown(13, (size_t)nq * knn * sizeof(float), &p_d2));
             IM_LAUNCH(k_knn, mesh_grid(h, nq * 32, 128), 128, 0, st, h->M, h->P, (const float*)p_qpos, 4, nq, knn, (double)INFINITY, (int*)p_idx, (float*)p_d2);
             IM_LAUNCH(k_rb_smooth, mesh_grid(h, nq, RB_THREADS), RB_THREADS, 0, st, h->M, nq, knn, (const int*)p_list, (const int*)p_idx, (const float*)p_d2, smooth_factor, h->P.accept);
         }
@@ -1936,8 +1881,8 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     if (n_smoothed) *n_smoothed = nq;
     // rows + axis box
     const int ge = mesh_grid(h, std::max(n, 1), RB_THREADS);
-    IM_CUDA(rb_scratch(h, 14, std::max<size_t>((size_t)n, 1) * 12 * sizeof(float), &p_rows));
-    IM_CUDA(rb_scratch(h, 15, (size_t)ge * sizeof(AxisAcc) + 8 * sizeof(float), &p_part));
+    IM_CUDA(grown(14, std::max<size_t>((size_t)n, 1) * 12 * sizeof(float), &p_rows));
+    IM_CUDA(grown(15, (size_t)ge * sizeof(AxisAcc) + 8 * sizeof(float), &p_part));
     float* d_rows = (float*)p_rows;
     int* d_ids = (int*)(d_rows + (size_t)std::max(n, 1) * 9);
     AxisAcc* part = (AxisAcc*)p_part;
@@ -1979,23 +1924,28 @@ int immesh_mesh_reconstruct_from_pointcloud(immesh_mesh_t* h, immesh_voxelgrid_t
 }
 
 // scratch of the batched frame: sized by max_voxels, max_work, max_triangles and max_list, never by the frame
+// (all or nothing: after a failure the handle has none of it)
 static cudaError_t mesh_batched_scratch(immesh_mesh* h) {
     if (h->b_fp) return cudaSuccess;
     const size_t nv = (size_t)std::max(h->max_vox, 1), nb = (nv + VG_TILE - 1) / VG_TILE, fcap = pow2_at_least((size_t)h->F.max_list * 2);
+    immesh::MemSet b;
+    int *act, *sel, *hist, *rank, *fset;
+    unsigned long long* key;
+    unsigned int *ku, *vu;
+    unsigned char* mark;
+    FramePose* fp;
     cudaError_t e;
-    if ((e = mdev_alloc(h, &h->b_act, nv)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_sel, nv)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_key, nv)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_ku, 2 * nv)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_vu, 2 * nv)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_hist, 256 * nb)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_rank, (size_t)h->F.max_work)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_mark, (size_t)h->M.max_t, 0)) != cudaSuccess) return e;
-    if ((e = mdev_alloc(h, &h->b_fset, fcap, 0xFF)) != cudaSuccess) return e;
+    if ((e = b.alloc(&act, nv)) != cudaSuccess || (e = b.alloc(&sel, nv)) != cudaSuccess || (e = b.alloc(&key, nv)) != cudaSuccess ||
+        (e = b.alloc(&ku, 2 * nv)) != cudaSuccess || (e = b.alloc(&vu, 2 * nv)) != cudaSuccess || (e = b.alloc(&hist, 256 * nb)) != cudaSuccess ||
+        (e = b.alloc(&rank, (size_t)h->F.max_work)) != cudaSuccess || (e = b.alloc(&mark, (size_t)h->M.max_t, 0)) != cudaSuccess ||
+        (e = b.alloc(&fset, fcap, 0xFF)) != cudaSuccess || (e = b.alloc(&fp, 1)) != cudaSuccess)
+        return e;
+    // the initialising memsets ran on the legacy stream, which the handle's non-blocking streams do not wait for
+    if ((e = cudaDeviceSynchronize()) != cudaSuccess) return e;
+    h->b_act = act; h->b_sel = sel; h->b_key = key; h->b_ku = ku; h->b_vu = vu; h->b_hist = hist; h->b_rank = rank; h->b_mark = mark; h->b_fset = fset; h->b_fp = fp;
     h->b_fset_mask = (unsigned int)(fcap - 1);
-    h->b_bytes = nv * (4 + 4 + 8 + 16) + 256 * nb * 4 + (size_t)h->F.max_work * 4 + (size_t)h->M.max_t + fcap * 4 + sizeof(FramePose);
-    if ((e = mdev_alloc(h, &h->b_fp, 1)) != cudaSuccess) return e;
-    return cudaDeviceSynchronize();   // the initialising memsets ran on the legacy stream, which the handle's non-blocking streams do not wait for
+    h->batch = std::move(b);
+    return cudaSuccess;
 }
 
 // incremental_mesh_reconstruction (src/ImMesh_mesh_reconstruction.cpp:92-267) as ONE frame of any size: append in chunks of <= B
@@ -2134,7 +2084,7 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     IM_CUDA(cudaStreamSynchronize(st));
     std::memcpy(h->last_cnt, cnt, sizeof(cnt));
     if (h->grow_max_bytes > 0) mesh_note(h, cnt, F.frame);
-    if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->b_bytes; stats[3] = cnt[7]; }
+    if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->batch.bytes(); stats[3] = cnt[7]; }
     return mesh_status(cnt[3]);
 }
 
@@ -2185,13 +2135,14 @@ int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int wid
     for (int i = 0; i < 3; ++i) C.t[i] = cam_t[i];
     C.w = width; C.h = height;
     const int n = width * height;
+    immesh::MemSet tmp;
     unsigned int* d_depth = nullptr;
     float *d_out = nullptr, *d_pts = nullptr;
     int* d_n = nullptr;
-    IM_CUDA(cudaMalloc(&d_depth, (size_t)n * 4));
-    IM_CUDA(cudaMalloc(&d_out, (size_t)n * 4));
-    if (points) IM_CUDA(cudaMalloc(&d_pts, (size_t)n * 16));
-    IM_CUDA(cudaMalloc(&d_n, 4));
+    IM_CUDA(tmp.alloc(&d_depth, (size_t)n));
+    IM_CUDA(tmp.alloc(&d_out, (size_t)n));
+    if (points) IM_CUDA(tmp.alloc(&d_pts, (size_t)n * 4));
+    IM_CUDA(tmp.alloc(&d_n, 1));
     IM_CUDA(cudaMemsetAsync(d_n, 0, 4, h->stream));
     IM_LAUNCH(k_depth_clear, mesh_grid(h, n, 128), 128, 0, h->stream, d_depth, n);
     if (nalloc > 0) IM_LAUNCH(k_depth_raster, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, C, d_depth);
@@ -2219,15 +2170,9 @@ int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int wid
         }
     }
     if (n_points) *n_points = np;
-    cudaFree(d_depth); cudaFree(d_out); if (d_pts) cudaFree(d_pts); cudaFree(d_n);
     return IMMESH_OK;
 }
 
-static void mesh_reinforce_free(immesh_mesh* h) {
-    for (void* p : h->rf.bufs) cudaFree(p);
-    if (h->rf.h_rd) cudaFreeHost(h->rf.h_rd);
-    h->rf = immesh_mesh::Reinforce();
-}
 int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, int win) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "reinforce_enable: a sharded mesh handle is not supported (the reinforcement runs on a single GPU)");
@@ -2239,9 +2184,9 @@ int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics, int
     }
     IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
     h->graph.destroy();                          // the captured sequence changes
-    mesh_reinforce_free(h);
+    h->rf = immesh_mesh::Reinforce();            // the buffers of an earlier enable go
     if (!intrinsics) return IMMESH_OK;
-    auto& r = h->rf;
+    immesh_mesh::Reinforce r;   // built in full before it replaces h->rf: after a failure the reinforcement stays disabled
     DepthCam& C = r.base;
     C.fx = intrinsics[0]; C.fy = intrinsics[1]; C.cx = intrinsics[2]; C.cy = intrinsics[3]; C.z_near = z_near; C.z_far = z_far;
     C.w = width; C.h = height;
@@ -2250,28 +2195,22 @@ int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics, int
     r.nb = (int)((n + RF_FIN - 1) / RF_FIN);
     r.bin_cap = std::max(1 << 22, 16 * r.ntiles);   // beyond it a frame's tiles walk every triangle slot (same image, slower)
     r.win = win;
-    auto alloc = [&](auto** p, size_t count) -> cudaError_t {
-        void* q = nullptr;
-        const cudaError_t e = cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(**p));
-        if (e == cudaSuccess) { r.bufs.push_back(q); *p = (std::remove_reference_t<decltype(**p)>*)q; }
-        return e;
-    };
-    RfDyn* rd = nullptr;
+    RfDyn *rd = nullptr, *h_rd = nullptr;
     cudaError_t e = cudaSuccess;
-    auto step = [&](cudaError_t x) { if (e == cudaSuccess) e = x; };
-    step(alloc(&rd, 1)); step(alloc(&r.cam, 1));
-    step(alloc(&r.tile_cnt, (size_t)r.ntiles)); step(alloc(&r.tile_off, (size_t)r.ntiles + 1)); step(alloc(&r.bin, (size_t)r.bin_cap)); step(alloc(&r.misc, 4));
-    step(alloc(&r.blk, (size_t)r.nb)); step(alloc(&r.blk_off, (size_t)r.nb + 1)); step(alloc(&r.depth_bits, n));
-    for (int b = 0; b < 2; ++b) { step(alloc(&r.depth[b], n)); step(alloc(&r.pts[b], n * 3)); step(alloc(&r.pix[b], n)); step(alloc(&r.n[b], 1)); step(alloc(&r.pose[b], 12)); }
-    step(cudaMallocHost(&r.h_rd, IM_SLOTS * sizeof(RfDyn)));
+    auto add = [&e, &r](auto** p, size_t count) { if (e == cudaSuccess) e = r.dev.alloc(p, std::max<size_t>(count, 1)); };   // stops at the first failure
+    add(&rd, 1); add(&r.cam, 1);
+    add(&r.tile_cnt, (size_t)r.ntiles); add(&r.tile_off, (size_t)r.ntiles + 1); add(&r.bin, (size_t)r.bin_cap); add(&r.misc, 4);
+    add(&r.blk, (size_t)r.nb); add(&r.blk_off, (size_t)r.nb + 1); add(&r.depth_bits, n);
+    for (int b = 0; b < 2; ++b) { add(&r.depth[b], n); add(&r.pts[b], n * 3); add(&r.pix[b], n); add(&r.n[b], 1); add(&r.pose[b], 12); }
+    if (e == cudaSuccess) e = r.pinned.alloc(&h_rd, IM_SLOTS, 0);
     if (e != cudaSuccess) {
-        mesh_reinforce_free(h);
         cudaGetLastError();
         return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "reinforce_enable: allocation of the reinforcement buffers failed");
     }
-    std::memset(r.h_rd, 0, IM_SLOTS * sizeof(RfDyn));
     r.rd = rd;
+    r.h_rd = h_rd;
     r.on = 1;
+    h->rf = std::move(r);
     return IMMESH_OK;
 }
 int immesh_mesh_reinforce_pose(immesh_mesh_t* h, const double* cam_R, const double* cam_t) {
