@@ -335,15 +335,7 @@ static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf
     IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d_pts, n, h->d_grid);
     IM_LAUNCH(k_vg_setup, 1, 32, 0, st, h->d_grid, inv);
     IM_LAUNCH(k_vg_keys, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, inv, h->d_k[0], h->d_v[0]);
-    int cur = 0;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 8 * pass;
-        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, shift, h->d_hist, nb);
-        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_hist, 256 * nb, (int*)nullptr);
-        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], h->d_k[cur ^ 1], h->d_v[cur ^ 1], n, shift,
-                  (const int*)h->d_hist, nb);
-        cur ^= 1;
-    }
+    const int cur = rs_sort_passes(st, h->d_k, h->d_v, 0, n, 4, h->d_hist);
     IM_LAUNCH(k_vg_heads, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, h->d_tile);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_tile, nb, h->d_tile + h->nblocks_max);
     IM_LAUNCH(k_vg_head_pos, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, (const int*)h->d_tile, h->d_head);

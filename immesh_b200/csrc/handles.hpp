@@ -92,6 +92,18 @@ struct immesh_lio {
     int max_step_nodes = 0, max_step_chunks = 0;   // largest node / chunk use between two noted steps (finished blocks are noted in step order)
 };
 
+// the device buffers of one depth image of the tiled rasteriser (mesh_capi.cu: rf_image_alloc, rf_image_launch): the camera, the tile
+// counters and offsets, the bins, misc[0] (the bins overflowed), the valid pixels per block and their offsets, the depth bits, and
+// result buffers 0 and 1 (image, points, pixels, count; the pose is the queued reinforcement's own)
+struct RfOut { float* depth; float* pts; int* pix; int* n; double* pose; };
+struct RfImage {
+    int ntiles = 0, nb = 0, bin_cap = 0;
+    immesh::DepthCam* cam = nullptr;
+    int *tile_cnt = nullptr, *tile_off = nullptr, *bin = nullptr, *misc = nullptr, *blk = nullptr, *blk_off = nullptr;
+    unsigned int* depth_bits = nullptr;
+    RfOut out[2] = {};
+};
+
 struct immesh_mesh {
     MeshParams P;
     MeshDev M;
@@ -163,17 +175,14 @@ struct immesh_mesh {
     double (*cam_ring)[12] = nullptr;   // [IM_RF_RING] rot_end, pos_end of the frames handed over by the localization handle
     int* cam_ring_frame = nullptr;      // [IM_RF_RING] frame number each ring entry belongs to (0: none)
     struct Reinforce {
-        int on = 0, win = 1, ntiles = 0, nb = 0, bin_cap = 0;
+        int on = 0, win = 1;
         int last_frame = 0;               // newest frame queued with the reinforcement (0: none since enable)
         int explicit_pose = 0;            // immesh_mesh_reinforce_pose: the caller's pose from the next frame on
         double R[9] = {}, t[3] = {};
         immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
         void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
         void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
-        immesh::DepthCam* cam = nullptr;
-        int *tile_cnt = nullptr, *tile_off = nullptr, *bin = nullptr, *misc = nullptr, *blk = nullptr, *blk_off = nullptr;
-        unsigned int* depth_bits = nullptr;
-        float* depth[2] = {}; float* pts[2] = {}; int* pix[2] = {}; int* n[2] = {}; double* pose[2] = {};
+        RfImage img;                      // result buffer (frame & 1) holds the frame's image and pose
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
     } rf;
 };

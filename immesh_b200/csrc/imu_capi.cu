@@ -207,15 +207,7 @@ static int imu_enqueue_undistort(immesh_imu* h, immesh_lio* lio, const double* i
     const int nb = (n + VG_TILE - 1) / VG_TILE;
     const int gs = std::min(nb * (VG_TILE / VG_THREADS), h->n_sm * 8);
     IM_LAUNCH(k_imu_keys, gs, VG_THREADS, 0, st, d_pts, n, h->d_k[0], h->d_v[0]);
-    int cur = 0;
-    for (int pass = 0; pass < 4; ++pass) {
-        const int shift = 8 * pass;
-        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, shift, h->d_hist, nb);
-        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_hist, 256 * nb, (int*)nullptr);
-        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], (const unsigned int*)h->d_v[cur], h->d_k[cur ^ 1], h->d_v[cur ^ 1], n, shift,
-                  (const int*)h->d_hist, nb);
-        cur ^= 1;
-    }
+    const int cur = rs_sort_passes(st, h->d_k, h->d_v, 0, n, 4, h->d_hist);
     IM_LAUNCH(k_imu_gather, gs, VG_THREADS, 0, st, (const float4*)d_pts, (const unsigned int*)h->d_v[cur], n, (float4*)h->d_out,
               icol >= 0 ? (const float*)h->d_in_i : (const float*)nullptr, icol >= 0 ? h->d_out_i : (float*)nullptr);
     const size_t smem = (size_t)(n_imu + 1) * IM_POSE_DOUBLES * sizeof(double);   // IMUpose holds at most n_imu + 1 entries

@@ -1460,13 +1460,7 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     int cur = 0;
     for (int half = 0; half < 2; ++half) {
         IM_LAUNCH(k_pub_keys, g, PUB_THREADS, 0, st, h->map, n, half, half ? (const unsigned int*)vu[cur] : (const unsigned int*)nullptr, ku[cur ^ half], vu[cur ^ half]);
-        cur ^= half;
-        for (int pass = 0; pass < 4; ++pass) {
-            IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], n, 8 * pass, hist, nb);
-            IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
-            IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
-            cur ^= 1;
-        }
+        cur = rs_sort_passes(st, ku, vu, cur ^ half, n, 4, hist);
     }
     IM_LAUNCH(k_pub_count, g, PUB_THREADS, 0, st, h->map, n, (const unsigned int*)vu[cur], slots, cnt, misc + 1);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, cnt, n, misc);

@@ -19,6 +19,9 @@
 #include "reinforce.cuh"
 
 using namespace immesh;
+namespace {
+#include "radix_sort.cuh"
+}
 
 // ------------------------------------------------------------------ kernels
 __global__ void k_frame_begin(MeshDev M, FrameBuf F_) {
@@ -66,38 +69,24 @@ __global__ void __launch_bounds__(128) k_cand_resolve(MeshDev M, MeshParams P, F
         }
     }
 }
-// exclusive scan of the accept flags by one block in ONE pass: thread t owns a contiguous chunk of ceil(m/1024) candidates
+// exclusive scan of n items by one block of 1024 threads in ONE pass: thread t owns a contiguous chunk of ceil(n/1024) items.
+// count(c) is item c's value; emit(c, run) stores item c's offset run and returns its value.  Returns the offset after the thread's
+// chunk (thread 1023: the total).
+template <class Count, class Emit>
+__device__ __forceinline__ int chunk_scan_1024(int n, Count count, Emit emit) {
+    const int per = (n + 1023) / 1024;
+    const int lo = threadIdx.x * per, hi = min(lo + per, n);
+    int mine = 0;
+    for (int c = lo; c < hi; ++c) mine += count(c);
+    int run = block_scan_1024(mine);
+    for (int c = lo; c < hi; ++c) run += emit(c, run);
+    return run;
+}
+// the accept flags into the candidates' output ranks
 __global__ void __launch_bounds__(1024) k_cand_scan(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    __shared__ int s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int per = (F.m + 1023) / 1024;
-    const int lo = threadIdx.x * per, hi = min(lo + per, F.m);
-    int mine = 0;
-    for (int c = lo; c < hi; ++c) mine += (F.cand_status[c] == CAND_ACCEPT) ? 1 : 0;
-    int v = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += u;
-    }
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        int wv = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, wv, o);
-            if (lane >= o) wv += u;
-        }
-        s_warp[lane] = wv;
-    }
-    __syncthreads();
-    int run = (warp ? s_warp[warp - 1] : 0) + v - mine;
-    for (int c = lo; c < hi; ++c) {
-        F.cand_scan[c] = run;
-        run += (F.cand_status[c] == CAND_ACCEPT) ? 1 : 0;
-    }
+    chunk_scan_1024(F.m, [&](int c) { return F.cand_status[c] == CAND_ACCEPT ? 1 : 0; },
+                    [&](int c, int run) { F.cand_scan[c] = run; return F.cand_status[c] == CAND_ACCEPT ? 1 : 0; });
 }
 __global__ void __launch_bounds__(128) k_cand_commit(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
@@ -319,45 +308,13 @@ __global__ void __launch_bounds__(128) k_region_keys(MeshDev M, int n_alloc, dou
 // 418).  The reference lets OpenGL rasterise; here a CUDA rasteriser with a defined sampling rule produces the metric depth directly:
 // camera frame x right / y down / z forward (the frame unproject_point inverts: world = R diag(1,-1,-1) p + t), pixel (u, v) =
 // (fx x / z + cx, fy y / z + cy), samples at integer pixel coordinates, a sample is covered when the three edge functions have one
-// sign (zero included), depth interpolated perspective-correctly (1/z is affine in the image), nearest surface wins (atomicMin on the
-// float bits).  Triangles with a vertex outside (z_near, z_far) are skipped (GL would clip them).  DepthCam, the triangle set-up and
-// the sample are in reinforce.cuh; k_depth_raster (one thread per triangle) is the reference the tiled rasteriser below is tested against.
-__global__ void __launch_bounds__(128) k_depth_clear(unsigned int* depth, int n) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) depth[i] = 0x7f800000u;   // +inf
-}
-__global__ void __launch_bounds__(128) k_depth_raster(MeshDev M, int n_alloc, DepthCam C, unsigned int* depth) {
-    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[t];
-        if (!r.w) continue;
-        DepthTri T;
-        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
-        for (int y = T.y_lo; y <= T.y_hi; ++y)
-            for (int x = T.x_lo; x <= T.x_hi; ++x) {
-                float zf;
-                if (depth_sample(T, x, y, &zf)) atomicMin(&depth[(size_t)y * C.w + x], __float_as_uint(zf));
-            }
-    }
-}
-// convert_depth_buffer_to_truth_depth's validity rule (val < 0.99 z_far, else -1) + unproject_point (openGL_camera_view.cpp:407-414)
-__global__ void __launch_bounds__(128) k_depth_finish(DepthCam C, const unsigned int* depth, float* out_depth, float* out_pts, int* n_pts) {
-    const int n = C.w * C.h;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const float val = __uint_as_float(depth[i]);
-        const bool ok = depth_valid(C, val);
-        out_depth[i] = ok ? val : -1.0f;
-        if (ok && out_pts) {
-            const int k = atomicAdd(n_pts, 1);
-            depth_unproject(C, i % C.w, i / C.w, val, out_pts + (size_t)k * 4);
-            out_pts[(size_t)k * 4 + 3] = __int_as_float(i);   // the pixel the point came from (the order of the list is arbitrary)
-        }
-    }
-}
-
-// ---- the queued reinforcement (immesh_mesh_reinforce_enable): behind every frame, on the mesh stream and inside its graph, the
-// camera pose (k_rf_pose), the tiled rasteriser (k_rf_count -> k_rf_scan -> k_rf_fill -> k_rf_tile) and the compaction of the valid
-// pixels in ascending pixel order (k_rf_fcount -> k_rf_scan -> k_rf_emit) into result buffer (frame & 1).
+// sign (zero included), depth interpolated perspective-correctly (1/z is affine in the image), nearest surface wins.  Triangles with a
+// vertex outside (z_near, z_far) are skipped (GL would clip them).  DepthCam, the triangle set-up and the sample are in reinforce.cuh.
+// One image (rf_image_launch): the tiled rasteriser (k_rf_count -> k_rf_scan -> k_rf_fill -> k_rf_tile) and the compaction of the
+// valid pixels in ascending pixel order (k_rf_fcount -> k_rf_scan -> k_rf_emit).  The blocking immesh_mesh_render_depth runs it at the
+// caller's pose; the queued reinforcement (immesh_mesh_reinforce_enable) runs it behind every frame, on the mesh stream and inside its
+// graph, after the camera pose (k_rf_pose), into result buffer (frame & 1).
 struct RfDyn { int mode, pad; double R[9], t[3]; };   // per frame: mode 1 = the caller's pose (immesh_mesh_reinforce_pose)
-struct RfOut { float* depth; float* pts; int* pix; int* n; double* pose; };
 // one block: the frame's camera (sensor-bound or the caller's), the tile counters cleared
 __global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const int* ring_frame, const FrameDyn* dyn, const RfDyn* rd, int win, DepthCam base,
                                                  DepthCam* cam, RfOut o0, RfOut o1, int* tile_cnt, int ntiles) {
@@ -397,43 +354,18 @@ __global__ void __launch_bounds__(128) k_rf_count(MeshDev M, const DepthCam* cam
             for (int tx = tx0; tx <= tx1; ++tx) atomicAdd(&tile_cnt[ty * ntx + tx], 1);
     }
 }
-// one block: exclusive scan of cnt[0, n) into off[0, n] (off[n] = total), in one pass over contiguous chunks (as k_cand_scan);
-// cur (or null) gets a copy of the offsets, the fill cursors; misc[0] (or null) = total > cap, the bins' overflow flag
+// one block: exclusive scan of cnt[0, n) into off[0, n] (off[n] = total); cur (or null, or cnt itself) gets a copy of the offsets,
+// the fill cursors; misc[0] (or null) = total > cap, the bins' overflow flag
 __global__ void __launch_bounds__(1024) k_rf_scan(const int* cnt, int n, int* off, int* cur, int cap, int* misc) {
-    __shared__ int s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int per = (n + 1023) / 1024;
-    const int lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
-    int mine = 0;
-    for (int c = lo; c < hi; ++c) mine += cnt[c];
-    int v = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += u;
-    }
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        int wv = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, wv, o);
-            if (lane >= o) wv += u;
-        }
-        s_warp[lane] = wv;
-    }
-    __syncthreads();
-    int run = (warp ? s_warp[warp - 1] : 0) + v - mine;
-    for (int c = lo; c < hi; ++c) {
+    const int total = chunk_scan_1024(n, [&](int c) { return cnt[c]; }, [&](int c, int run) {
         const int k = cnt[c];
         off[c] = run;
         if (cur) cur[c] = run;
-        run += k;
-    }
+        return k;
+    });
     if (threadIdx.x == 1023) {
-        off[n] = run;
-        if (misc) misc[0] = run > cap ? 1 : 0;
+        off[n] = total;
+        if (misc) misc[0] = total > cap ? 1 : 0;
     }
 }
 // fill pass: triangle slots into the bins (order inside a bin is free: the tile takes the minimum)
@@ -521,9 +453,6 @@ __global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const F
 // unique), so nothing depends on the compaction order.  The vertices of the kept triangles whose m_smoothed is clear are claimed once
 // (bitmap), compacted, searched with k_knn and smoothed from raw positions; k_rb_emit gathers vsmooth into the float rows and reduces
 // the axis box per block.
-namespace {
-#include "radix_sort.cuh"
-}
 #define RB_THREADS 128
 __global__ void __launch_bounds__(RB_THREADS) k_rb_select(MeshDev M, int n_alloc, double region_size, const unsigned long long* qkeys, const int* qval, unsigned int qmask,
                                                           int use_keys, int* slot, unsigned long long* rk, int* misc) {
@@ -1244,21 +1173,39 @@ static int mesh_grid_fixed(const immesh_mesh* h, long long n_cap, int threads, i
     if (g > (long long)h->n_sm * waves) g = (long long)h->n_sm * waves;
     return g < 1 ? 1 : (int)g;
 }
-static RfOut rf_out(const immesh_mesh* h, int b) { return RfOut{h->rf.depth[b], h->rf.pts[b], h->rf.pix[b], h->rf.n[b], h->rf.pose[b]}; }
-// the reinforcement of the frame just queued (fixed grids: every per-frame value is read on the device)
+// the buffers of one w x h depth image and `nout` result buffers (image, points, pixels, count) into dev; stops at the first failure
+static cudaError_t rf_image_alloc(immesh::MemSet& dev, int w, int h, int nout, RfImage* im) {
+    const size_t n = (size_t)w * h;
+    im->ntiles = ((w + IM_RT_TILE - 1) / IM_RT_TILE) * ((h + IM_RT_TILE - 1) / IM_RT_TILE);
+    im->nb = (int)((n + RF_FIN - 1) / RF_FIN);
+    im->bin_cap = std::max(1 << 22, 16 * im->ntiles);   // beyond it an image's tiles walk every triangle slot (same image, slower)
+    cudaError_t e = cudaSuccess;
+    auto add = [&e, &dev](auto** p, size_t count) { if (e == cudaSuccess) e = dev.alloc(p, std::max<size_t>(count, 1)); };
+    add(&im->cam, 1);
+    add(&im->tile_cnt, (size_t)im->ntiles); add(&im->tile_off, (size_t)im->ntiles + 1); add(&im->bin, (size_t)im->bin_cap); add(&im->misc, 4);
+    add(&im->blk, (size_t)im->nb); add(&im->blk_off, (size_t)im->nb + 1); add(&im->depth_bits, n);
+    for (int b = 0; b < nout; ++b) { RfOut& o = im->out[b]; add(&o.depth, n); add(&o.pts, n * 3); add(&o.pix, n); add(&o.n, 1); }
+    return e;
+}
+// the image of the camera in im.cam, with the tile counters zeroed, into result buffer (dyn->frame & 1) (fixed grids: every
+// per-image value is read on the device)
+static void rf_image_launch(const immesh_mesh* h, const RfImage& im, const FrameDyn* dyn, cudaStream_t st) {
+    const int g = h->n_sm * 8;
+    const DepthCam* cam = im.cam;
+    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, cam, im.tile_cnt);
+    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.tile_cnt, im.ntiles, im.tile_off, im.tile_cnt, im.bin_cap, im.misc);
+    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, cam, im.tile_cnt, im.bin, (const int*)im.misc);
+    IM_LAUNCH(k_rf_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, cam, (const int*)im.tile_off, (const int*)im.bin, (const int*)im.misc, im.depth_bits);
+    IM_LAUNCH(k_rf_fcount, im.nb, RF_FIN, 0, st, cam, (const unsigned int*)im.depth_bits, im.blk);
+    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.blk, im.nb, im.blk_off, (int*)nullptr, 0, (int*)nullptr);
+    IM_LAUNCH(k_rf_emit, im.nb, RF_FIN, 0, st, cam, dyn, (const unsigned int*)im.depth_bits, (const int*)im.blk_off, im.nb, im.out[0], im.out[1]);
+}
+// the reinforcement of the frame just queued: its camera, then its image
 static void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st) {
     auto& r = h->rf;
     IM_LAUNCH(k_rf_pose, 1, 256, 0, st, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame, (const FrameDyn*)h->d_dyn, (const RfDyn*)r.rd, r.win, r.base,
-              r.cam, rf_out(h, 0), rf_out(h, 1), r.tile_cnt, r.ntiles);
-    const int g = h->n_sm * 8;
-    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, (const DepthCam*)r.cam, r.tile_cnt);
-    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)r.tile_cnt, r.ntiles, r.tile_off, r.tile_cnt, r.bin_cap, r.misc);
-    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, (const DepthCam*)r.cam, r.tile_cnt, r.bin, (const int*)r.misc);
-    IM_LAUNCH(k_rf_tile, r.ntiles, IM_RT_THREADS, 0, st, h->M, (const DepthCam*)r.cam, (const int*)r.tile_off, (const int*)r.bin, (const int*)r.misc, r.depth_bits);
-    IM_LAUNCH(k_rf_fcount, r.nb, RF_FIN, 0, st, (const DepthCam*)r.cam, (const unsigned int*)r.depth_bits, r.blk);
-    IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)r.blk, r.nb, r.blk_off, (int*)nullptr, 0, (int*)nullptr);
-    IM_LAUNCH(k_rf_emit, r.nb, RF_FIN, 0, st, (const DepthCam*)r.cam, (const FrameDyn*)h->d_dyn, (const unsigned int*)r.depth_bits, (const int*)r.blk_off, r.nb,
-              rf_out(h, 0), rf_out(h, 1));
+              r.img.cam, r.img.out[0], r.img.out[1], r.img.tile_cnt, r.img.ntiles);
+    rf_image_launch(h, r.img, h->d_dyn, st);
 }
 
 // src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state.
@@ -1819,13 +1766,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
             const int passes = w < 3 ? tri_passes : use_keys ? rb_passes((unsigned long long)std::max(nk - 1, 0)) : 4;
             IM_LAUNCH(k_rb_word, g, RB_THREADS, 0, st, h->M, n, w, (const int*)slot, (const unsigned long long*)rk, w == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur],
                       ku[cur ^ 1], vu[cur ^ 1]);
-            cur ^= 1;
-            for (int pass = 0; pass < passes; ++pass) {
-                IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], n, 8 * pass, hist, nb);
-                IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
-                IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
-                cur ^= 1;
-            }
+            cur = rs_sort_passes(st, ku, vu, cur ^ 1, n, passes, hist);
         }
         if (!use_keys) {
             IM_LAUNCH(k_rb_starts, g, RB_THREADS, 0, st, n, (const unsigned int*)vu[cur], (const unsigned long long*)rk, flag);
@@ -2031,18 +1972,11 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     unsigned int* vu[2] = {h->b_vu, h->b_vu + h->max_vox};
     int cur = 0;
     if (nsel > 0) {
-        const int nb = (nsel + VG_TILE - 1) / VG_TILE, g = mesh_grid(h, nsel, 128);
+        const int g = mesh_grid(h, nsel, 128);
         for (int half = 0; half < 2; ++half) {
             IM_LAUNCH(k_bat_word, g, 128, 0, st, nsel, half, (const unsigned long long*)h->b_key, half == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur],
                       ku[cur ^ 1], vu[cur ^ 1]);
-            cur ^= 1;
-            for (int pass = 0; pass < 4; ++pass) {
-                IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], nsel, 8 * pass, h->b_hist, nb);
-                IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->b_hist, 256 * nb, (int*)nullptr);
-                IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)ku[cur], (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1], nsel, 8 * pass,
-                          (const int*)h->b_hist, nb);
-                cur ^= 1;
-            }
+            cur = rs_sort_passes(st, ku, vu, cur ^ 1, nsel, 4, h->b_hist);
         }
     }
     const unsigned int* order = vu[cur];
@@ -2126,48 +2060,28 @@ int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int wid
     if (!h || !intrinsics || !cam_R || !cam_t || !depth || width < 1 || height < 1 || (long long)width * height > (1 << 26) || !(z_near > 0) || !(z_far > z_near))
         return im_fail(IMMESH_E_INVALID, "bad argument");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int cnt[32];
-    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    const int nalloc = std::min(cnt[1], h->M.max_t);
     DepthCam C;
     C.fx = intrinsics[0]; C.fy = intrinsics[1]; C.cx = intrinsics[2]; C.cy = intrinsics[3]; C.z_near = z_near; C.z_far = z_far;
     for (int i = 0; i < 9; ++i) C.R[i] = cam_R[i];
     for (int i = 0; i < 3; ++i) C.t[i] = cam_t[i];
     C.w = width; C.h = height;
     const int n = width * height;
-    immesh::MemSet tmp;
-    unsigned int* d_depth = nullptr;
-    float *d_out = nullptr, *d_pts = nullptr;
-    int* d_n = nullptr;
-    IM_CUDA(tmp.alloc(&d_depth, (size_t)n));
-    IM_CUDA(tmp.alloc(&d_out, (size_t)n));
-    if (points) IM_CUDA(tmp.alloc(&d_pts, (size_t)n * 4));
-    IM_CUDA(tmp.alloc(&d_n, 1));
-    IM_CUDA(cudaMemsetAsync(d_n, 0, 4, h->stream));
-    IM_LAUNCH(k_depth_clear, mesh_grid(h, n, 128), 128, 0, h->stream, d_depth, n);
-    if (nalloc > 0) IM_LAUNCH(k_depth_raster, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, C, d_depth);
-    IM_LAUNCH(k_depth_finish, mesh_grid(h, n, 128), 128, 0, h->stream, C, (const unsigned int*)d_depth, d_out, d_pts, d_n);
+    immesh::MemSet tmp;   // h->rf is not touched: a queued frame's result stays readable
+    RfImage im;
+    IM_CUDA(rf_image_alloc(tmp, width, height, 1, &im));
+    im.out[1] = im.out[0];   // k_rf_emit picks out[frame & 1]
+    IM_CUDA(cudaMemcpyAsync(im.cam, &C, sizeof(C), cudaMemcpyHostToDevice, h->stream));
+    IM_CUDA(cudaMemsetAsync(im.tile_cnt, 0, (size_t)im.ntiles * sizeof(int), h->stream));
+    rf_image_launch(h, im, h->d_dyn, h->stream);
     IM_CUDA(cudaGetLastError());
     int np = 0;
-    IM_CUDA(cudaMemcpyAsync(depth, d_out, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
-    IM_CUDA(cudaMemcpyAsync(&np, d_n, 4, cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaMemcpyAsync(depth, im.out[0].depth, (size_t)n * 4, cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaMemcpyAsync(&np, im.out[0].n, 4, cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    if (points && np > 0) {
-        std::vector<float> tmp((size_t)np * 4);
-        IM_CUDA(cudaMemcpy(tmp.data(), d_pts, (size_t)np * 16, cudaMemcpyDeviceToHost));
-        // deterministic order: ascending pixel index (the image scan order of convert_depth_buffer_to_truth_depth)
-        std::vector<int> order(np);
-        for (int i = 0; i < np; ++i) order[i] = i;
-        std::sort(order.begin(), order.end(), [&](int a, int b) {
-            int pa, pb;
-            std::memcpy(&pa, &tmp[(size_t)a * 4 + 3], 4); std::memcpy(&pb, &tmp[(size_t)b * 4 + 3], 4);
-            return pa < pb;
-        });
-        for (int i = 0; i < np; ++i) {
-            const float* q = &tmp[(size_t)order[i] * 4];
-            points[(size_t)i * 3] = q[0]; points[(size_t)i * 3 + 1] = q[1]; points[(size_t)i * 3 + 2] = q[2];
-            if (point_pixel) std::memcpy(&point_pixel[i], &q[3], 4);
-        }
+    if (!points) np = 0;   // the count is that of the points written
+    if (np > 0) {
+        IM_CUDA(cudaMemcpy(points, im.out[0].pts, (size_t)np * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+        if (point_pixel) IM_CUDA(cudaMemcpy(point_pixel, im.out[0].pix, (size_t)np * sizeof(int), cudaMemcpyDeviceToHost));
     }
     if (n_points) *n_points = np;
     return IMMESH_OK;
@@ -2190,18 +2104,11 @@ int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics, int
     DepthCam& C = r.base;
     C.fx = intrinsics[0]; C.fy = intrinsics[1]; C.cx = intrinsics[2]; C.cy = intrinsics[3]; C.z_near = z_near; C.z_far = z_far;
     C.w = width; C.h = height;
-    const size_t n = (size_t)width * height;
-    r.ntiles = ((width + IM_RT_TILE - 1) / IM_RT_TILE) * ((height + IM_RT_TILE - 1) / IM_RT_TILE);
-    r.nb = (int)((n + RF_FIN - 1) / RF_FIN);
-    r.bin_cap = std::max(1 << 22, 16 * r.ntiles);   // beyond it a frame's tiles walk every triangle slot (same image, slower)
     r.win = win;
     RfDyn *rd = nullptr, *h_rd = nullptr;
-    cudaError_t e = cudaSuccess;
-    auto add = [&e, &r](auto** p, size_t count) { if (e == cudaSuccess) e = r.dev.alloc(p, std::max<size_t>(count, 1)); };   // stops at the first failure
-    add(&rd, 1); add(&r.cam, 1);
-    add(&r.tile_cnt, (size_t)r.ntiles); add(&r.tile_off, (size_t)r.ntiles + 1); add(&r.bin, (size_t)r.bin_cap); add(&r.misc, 4);
-    add(&r.blk, (size_t)r.nb); add(&r.blk_off, (size_t)r.nb + 1); add(&r.depth_bits, n);
-    for (int b = 0; b < 2; ++b) { add(&r.depth[b], n); add(&r.pts[b], n * 3); add(&r.pix[b], n); add(&r.n[b], 1); add(&r.pose[b], 12); }
+    cudaError_t e = rf_image_alloc(r.dev, width, height, 2, &r.img);
+    if (e == cudaSuccess) e = r.dev.alloc(&rd, 1);
+    for (int b = 0; b < 2 && e == cudaSuccess; ++b) e = r.dev.alloc(&r.img.out[b].pose, 12);
     if (e == cudaSuccess) e = r.pinned.alloc(&h_rd, IM_SLOTS, 0);
     if (e != cudaSuccess) {
         cudaGetLastError();
@@ -2232,13 +2139,14 @@ int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth, float* points, 
     IM_CUDA(cudaEventSynchronize(h->ev_done[f & (IM_SLOTS - 1)]));
     int n = 0;
     double pose[12];
-    IM_CUDA(cudaMemcpy(&n, h->rf.n[b], sizeof(int), cudaMemcpyDeviceToHost));
-    IM_CUDA(cudaMemcpy(pose, h->rf.pose[b], sizeof(pose), cudaMemcpyDeviceToHost));
+    const RfOut& o = h->rf.img.out[b];
+    IM_CUDA(cudaMemcpy(&n, o.n, sizeof(int), cudaMemcpyDeviceToHost));
+    IM_CUDA(cudaMemcpy(pose, o.pose, sizeof(pose), cudaMemcpyDeviceToHost));
     *n_out = n;
     if (n > cap) return im_fail(IMMESH_E_CAPACITY, "reinforced_cloud: more points than cap (*n_out holds the number needed; nothing was written)");
-    if (depth) IM_CUDA(cudaMemcpy(depth, h->rf.depth[b], (size_t)h->rf.base.w * h->rf.base.h * sizeof(float), cudaMemcpyDeviceToHost));
-    if (points && n > 0) IM_CUDA(cudaMemcpy(points, h->rf.pts[b], (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
-    if (point_pixel && n > 0) IM_CUDA(cudaMemcpy(point_pixel, h->rf.pix[b], (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
+    if (depth) IM_CUDA(cudaMemcpy(depth, o.depth, (size_t)h->rf.base.w * h->rf.base.h * sizeof(float), cudaMemcpyDeviceToHost));
+    if (points && n > 0) IM_CUDA(cudaMemcpy(points, o.pts, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    if (point_pixel && n > 0) IM_CUDA(cudaMemcpy(point_pixel, o.pix, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
     if (pose_out) std::memcpy(pose_out, pose, sizeof(pose));
     return IMMESH_OK;
 }

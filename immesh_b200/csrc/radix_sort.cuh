@@ -1,6 +1,7 @@
-// immesh_b200 -- stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, 2048-element tiles; ranks inside a tile from
-// __match_any_sync (warp) + per-warp digit counts in shared memory.  Used by the pcl::VoxelGrid front-end (cell index -> point) and by
-// the IMU undistortion (time stamp -> point).  Include inside an anonymous namespace of the translation unit that launches it.
+// immesh_b200 -- the one-block scan and the stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, 2048-element tiles;
+// ranks inside a tile from __match_any_sync (warp) + per-warp digit counts in shared memory.  Used by the pcl::VoxelGrid front-end
+// (cell index -> point), the IMU undistortion (time stamp -> point), the plane-map publisher, the viewer's region buffers and the
+// batched frame.  Include inside an anonymous namespace of a translation unit that includes common_host.hpp (IM_LAUNCH).
 #pragma once
 #define VG_TILE 2048
 #define VG_THREADS 256
@@ -18,32 +19,42 @@ __global__ void __launch_bounds__(VG_THREADS) k_rs_hist(const unsigned int* __re
     __syncthreads();
     hist[threadIdx.x * nblocks + blockIdx.x] = h[threadIdx.x];
 }
+// exclusive scan of v over a block of 1024 threads, which all call it: warp shuffle, then a scan of the 32 warp totals in warp 0
+__device__ __forceinline__ int block_scan_1024(int v) {
+    __shared__ int s_warp[32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += u;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        int wv = s_warp[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int u = __shfl_up_sync(0xffffffffu, wv, o);
+            if (lane >= o) wv += u;
+        }
+        s_warp[lane] = wv;
+    }
+    __syncthreads();
+    return (warp ? s_warp[warp - 1] : 0) + x - v;
+}
 // exclusive scan of `len` ints in place by ONE block (len <= a few 100 k); total -> *total_out if not null
 __global__ void __launch_bounds__(1024) k_rs_scan(int* a, int len, int* total_out) {
-    __shared__ int s_warp[32];
     __shared__ int s_carry;
     if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int base = 0; base < len; base += 1024) {
         const int i = base + threadIdx.x;
         const int v = i < len ? a[i] : 0;
-        int x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-        if (lane == 31) s_warp[warp] = x;
+        const int excl = block_scan_1024(v) + s_carry;
+        if (i < len) a[i] = excl;
         __syncthreads();
-        if (warp == 0) {
-            int w = s_warp[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += y; }
-            s_warp[lane] = w;
-        }
-        __syncthreads();
-        const int incl = x + (warp > 0 ? s_warp[warp - 1] : 0) + s_carry;
-        if (i < len) a[i] = incl - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) s_carry = incl;
+        if (threadIdx.x == 1023) s_carry = excl + v;
         __syncthreads();
     }
     if (threadIdx.x == 0 && total_out) *total_out = s_carry;
@@ -80,4 +91,15 @@ __global__ void __launch_bounds__(VG_THREADS) k_rs_scatter(const unsigned int* _
         __syncthreads();
     }
 }
-
+// the LSD passes over the low `passes` 8-bit digits of the n keys in k[cur] (values in v[cur]), each from one buffer of the pairs into
+// the other; hist holds 256 * ceil(n / VG_TILE) ints.  Returns the index of the buffers that hold the sorted pairs.
+inline int rs_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist) {
+    const int nb = (n + VG_TILE - 1) / VG_TILE;
+    for (int pass = 0; pass < passes; ++pass) {
+        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], n, 8 * pass, hist, nb);
+        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
+        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], (const unsigned int*)v[cur], k[cur ^ 1], v[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
+        cur ^= 1;
+    }
+    return cur;
+}

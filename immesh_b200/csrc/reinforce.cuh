@@ -67,7 +67,7 @@ IM_HD void depth_unproject(const DepthCam& C, int x, int y, float val, float* ou
 #define IM_RT_TILE 16
 #define IM_RT_THREADS (IM_RT_TILE * IM_RT_TILE)
 // the nearest surface over triangles tris[0, n) at pixel (x, y), as the bits of a positive float (+inf: none); unsigned order of
-// the bits is the order of the floats, so the result is the atomicMin of k_depth_raster whatever the order of the triangles
+// the bits is the order of the floats, so the result is the nearest sample whatever the order of the triangles
 IM_HD unsigned int rt_pixel_min(const DepthTri* tris, int n, int x, int y, unsigned int acc) {
     for (int j = 0; j < n; ++j) {
         const DepthTri& T = tris[j];

@@ -389,8 +389,8 @@ int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics /*[4]*/,
  *     so does a window holding no frame with a pose (world-frame frames carry none; the reference divides by zero there).
  *   immesh_mesh_reinforce_pose(h, cam_R, cam_t): the caller's camera pose instead, from the next queued frame on, for every frame
  *     (the form for frames pushed with world points); NULL, NULL returns to the sensor-bound pose.  Enabling starts sensor-bound.
- *   Result: exactly immesh_mesh_render_depth at that pose -- same depth image bit for bit, same points and pixels in ascending pixel
- *     order -- computed by a tiled rasteriser (16 x 16 pixel tiles; the triangles binned by their pixel boxes).
+ *   Result: exactly immesh_mesh_render_depth at that pose -- both run the same tiled rasteriser (16 x 16 pixel tiles; the triangles
+ *     binned by their pixel boxes), so the same depth image bit for bit and the same points and pixels in ascending pixel order.
  *   immesh_mesh_reinforced_cloud: blocking read of the newest queued frame's result (waits for that frame only).  The result is
  *     double-buffered: a frame queued after the read started writes the other buffer.  depth [height][width] (-1 where empty),
  *     points [n][3], point_pixel [n] (y * width + x), pose_out [12] = R row-major, t; each may be NULL.  *n_out > cap:

@@ -1,7 +1,8 @@
 """GPU tier: the LiDAR point-cloud reinforcement queued behind every mesh frame (immesh_mesh_reinforce_enable / _pose /
-immesh_mesh_reinforced_cloud).  Every frame's result against the blocking immesh_mesh_render_depth (k_depth_raster, one thread per
-triangle) at the pose the frame used, bit for bit; that pose against the numpy restatement of get_last_avr_pose; nothing else changes;
-the frames are graph-replayed; the error paths."""
+immesh_mesh_reinforced_cloud).  Every frame's result against the blocking immesh_mesh_render_depth at the pose the frame used, bit
+for bit (both run the same kernels: this checks the pose, the double buffer and the graph); the newest frame of a stream, a facet
+that fills the image and the empty mesh also against the numpy restatement of the sampling rule on the mesh's snapshot, bit for bit;
+the pose against the numpy restatement of get_last_avr_pose; nothing else changes; the frames are graph-replayed; the error paths."""
 import ctypes as C
 
 import numpy as np
@@ -9,7 +10,7 @@ import pytest
 
 from immesh_b200 import api, synth
 from mesh_common import SMALL
-from reinforce_reference import avr_pose
+from reinforce_reference import avr_pose, raster
 
 pytestmark = pytest.mark.gpu
 
@@ -21,12 +22,19 @@ def same(a, b):
     return a.shape == b.shape and np.array_equal(np.ascontiguousarray(a).view(np.uint32), np.ascontiguousarray(b).view(np.uint32))
 
 
-def check_frame(mesh, K=K0, w=640, h=480, zn=ZN, zf=ZF):
-    """the newest frame's queued result against render_depth at the pose it reports; returns (points, pose)"""
+def check_frame(mesh, K=K0, w=640, h=480, zn=ZN, zf=ZF, restated=False):
+    """the newest frame's queued result against render_depth at the pose it reports and, with restated, against the numpy
+    rasteriser on the mesh's snapshot; returns (points, pose)"""
     d, p, x, R, t = mesh.reinforced_cloud()
     dr, pr, xr = mesh.render_depth(K, w, h, zn, zf, R, t)
-    assert same(d, dr), "depth image differs from k_depth_raster"
+    assert same(d, dr), "depth image differs from render_depth"
     assert np.array_equal(x, xr) and same(p, pr), "points / pixels differ from render_depth"
+    if restated:
+        mesh.wait()   # snapshot() sizes its arrays by counts(), which a queued frame updates when it is drained
+        v, tri, _ = mesh.snapshot()
+        dn, pn, xn = raster(K, w, h, zn, zf, R, t, v, tri)
+        assert same(d, dn), "depth image differs from the numpy restatement"
+        assert np.array_equal(x, xn) and same(p, pn), "points / pixels differ from the numpy restatement"
     return p, (R, t)
 
 
@@ -45,7 +53,7 @@ def run_stream(lib, win=1, reinforce=True, n_scans=8, seed=3, read=True):
         lio.step_async(scans[k]["body_ds"], dt=scans[k]["dt"])
         mesh.push_frame_from_lio_async(lio, scans[k]["body_full"])
         if reinforce and read:
-            pts, (R, t) = check_frame(mesh)
+            pts, (R, t) = check_frame(mesh, restated=k == n_scans - 1)
             s = lio.get_state()
             poses[k] = (s[0:9].reshape(3, 3).copy(), s[9:12].copy())   # the pose frame k was transformed with
             Rn, tn = avr_pose(poses, k, win)
@@ -95,7 +103,7 @@ def test_large_triangle_and_explicit_pose(cuda_lib):
     mesh.push_frame(np.zeros((0, 3), np.float32), cam_t)
     d, p, x, Rr, tr = mesh.reinforced_cloud()
     assert np.array_equal(Rr, R) and np.array_equal(tr, cam_t)
-    check_frame(mesh, K, 640, 480, 0.005, 100.0)
+    check_frame(mesh, K, 640, 480, 0.005, 100.0, restated=True)
     assert (d > 0).mean() > 0.9
     # back to the sensor-bound pose: a frame with world points records none, so the window is empty -> identity
     mesh.reinforce_pose(None)
@@ -110,7 +118,7 @@ def test_empty_mesh(cuda_lib):
     mesh.push_frame(np.zeros((0, 3), np.float32), np.zeros(3))
     d, p, x, R, t = mesh.reinforced_cloud()
     assert (d == -1).all() and len(p) == 0 and np.array_equal(R, np.eye(3))
-    check_frame(mesh)
+    check_frame(mesh, restated=True)
 
 
 def test_error_paths(cuda_lib):
