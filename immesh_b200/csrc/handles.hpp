@@ -15,13 +15,17 @@ using immesh::MeshParams; using immesh::MeshDev; using immesh::FrameBuf; using i
 // (2 was enough for the device, but a host hiccup of ~1 ms then drained the pipeline: seen as single ranks of an 8-rank run falling
 // back to the blocking-call rate)
 #define IM_SLOTS 4
+// immesh_lio::h_ints (pinned, 64 ints) past its copy of the counter block: the iteration count of a blocking estimate, the count a
+// publisher reads back (the plane markers' four counters behind it)
+constexpr int IM_HINT_ITERS = 32, IM_HINT_PUB = 40, IM_HINT_SIZE = 64;
+static_assert(immesh::IM_LC_SIZE <= IM_HINT_ITERS && IM_HINT_PUB + 5 <= IM_HINT_SIZE, "immesh_lio::h_ints layout");
 
 struct immesh_lio {
     LioParams P;
     VoxelMapDev map;
     ScanBuf sb;
     LioCtrl* d_ctrl = nullptr;
-    int* d_counters = nullptr;  // node_count, chunk_bump, avail_top, pending_n, err, n_roots, n_touched, seg_top, work_counter, .., pub_n (12)
+    int* d_counters = nullptr;  // [IM_LC_SIZE] the counter block, slots IM_LC_*
     // grow-only scratch of the publishers, in `scratch`
     int* d_pub_scratch = nullptr;    // immesh_voxelmap_plane_markers: key sort, per-root row counts / offsets
     size_t pub_scratch_ints = 0;
@@ -69,7 +73,7 @@ struct immesh_lio {
     unsigned int* d_bits = nullptr;  // [2][words] exists / matched-in-own-voxel bit words of the sharded residual pass
     immesh::PeerWindow win;          // peer window of the sharded residual pass (NVLink peer memory, replaces the NCCL all-reduces)
     int words_cap = 0;
-    int* h_ints = nullptr;     // pinned
+    int* h_ints = nullptr;     // pinned, IM_HINT_SIZE: a copy of the counter block, a count read back at IM_HINT_ITERS or IM_HINT_PUB
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     size_t cap = 0;
@@ -85,7 +89,7 @@ struct immesh_lio {
     // growth of the map pools (immesh_lio_reserve / immesh_lio_set_growth)
     long long growths = 0;        // calls that enlarged at least one pool
     int64_t grow_max_bytes = 0;   // automatic growth before every step: 0 off, > 0 ceiling on dev.bytes()
-    int known[16] = {};           // counters (d_counters layout) of the last step known to have finished
+    int known[immesh::IM_LC_SIZE] = {};   // counters (IM_LC_* slots) of the last step known to have finished
     long long known_step = 0;     // its number among the map-growing steps (0: the empty map at create)
     long long map_steps = 0;      // map-growing steps queued so far
     long long slot_step[IM_SLOTS] = {};   // number of the step that used staging slot s
@@ -113,7 +117,7 @@ struct immesh_mesh {
     float* d_pts = nullptr;   // IM_SLOTS slots of max_frame_points*3
     float* d_body = nullptr;  // IM_SLOTS slots, staging for body-frame scans handed over by the localization handle
     float* h_pts = nullptr;   // pinned, IM_SLOTS slots
-    int* h_cnt = nullptr;     // pinned, IM_SLOTS slots of 32
+    int* h_cnt = nullptr;     // pinned, IM_SLOTS slots of IM_MC_HOST
     FramePose* d_fp = nullptr;  // IM_SLOTS slots
     FramePose* h_fp = nullptr;  // pinned, IM_SLOTS slots
     immesh::FrameDyn* h_dyn = nullptr;  // pinned, IM_SLOTS slots: per-frame inputs of the launch sequence
@@ -146,7 +150,7 @@ struct immesh_mesh {
     int n_sm = 132;
     size_t ccap = 0;
     double last_ms[4] = {0, 0, 0, 0};
-    int last_cnt[32];
+    int last_cnt[immesh::IM_MC_HOST];
     immesh::MemSet dev;       // device memory counted in immesh_mesh_capacity (with `batch`): the create-time buffers, the pools and the shard segments
     immesh::MemSet scratch;   // device memory not counted: the region buffers' scratch
     immesh::MemSet pinned{immesh::MemSet::Pinned};
@@ -168,7 +172,7 @@ struct immesh_mesh {
     // growth of the mesh pools (immesh_mesh_reserve / immesh_mesh_set_growth)
     long long growths = 0;
     int64_t grow_max_bytes = 0;
-    int known[32] = {};           // counters (MeshDev::cnt layout) of the last frame known to have finished
+    int known[immesh::IM_MC_HOST] = {};   // counters (IM_MC_* slots) of the last frame known to have finished
     int known_frame = 0;          // its frame number (0: the empty mesh at create)
     int max_step_tris = 0;        // largest triangle allocation between two noted frames (noted oldest first)
     // LiDAR point-cloud reinforcement (immesh_mesh_reinforce_enable)

@@ -433,23 +433,23 @@ __global__ void __launch_bounds__(128) k_grow_voxel(VoxelMapDev map, LioParams P
 }
 // last kernel of a scan: recycle chunks, reset the per-scan counters, publish the converged pose for the mesher's frame (which
 // runs behind on another stream) and assemble the block the host reads back with one D2H copy
-__global__ void k_grow_finish(VoxelMapDev map, ScanBuf sb, int* work_counter, LioCtrl* ctrl, const int* counters) {
+__global__ void k_grow_finish(VoxelMapDev map, ScanBuf sb, LioCtrl* ctrl, int* counters) {
     recycle_chunks(map, threadIdx.x, blockDim.x);
     if (threadIdx.x == 0) {
         *sb.n_touched = 0;
         *sb.seg_top = 0;
-        *work_counter = 0;
-        work_counter[3] = 0;   // n_complex (d_counters + 11)
+        counters[IM_LC_WORK] = 0;
+        counters[IM_LC_COMPLEX] = 0;
     }
     if (ctrl) {
         const int si = ctrl->dyn.scan_idx;
         for (int i = threadIdx.x; i < IM_STATE_DOUBLES; i += blockDim.x) ctrl->out.state[i] = ctrl->state[i];
         if (threadIdx.x < 12) ctrl->pose_ring[si & (IM_POSE_RING - 1)][threadIdx.x] = ctrl->state[threadIdx.x];
-        if (threadIdx.x < 16) ctrl->out.counters[threadIdx.x] = counters[threadIdx.x];
+        if (threadIdx.x < IM_LC_SIZE) ctrl->out.counters[threadIdx.x] = counters[threadIdx.x];
         if (threadIdx.x == 0) { ctrl->out.iters_run = ctrl->iters_run; ctrl->out.scan_idx = si; }
     }
     __syncthreads();
-    if (threadIdx.x == 0 && map.stat) { map.stat[0] = 0; map.stat[1] = 0; }   // per-scan work counters (reported through LioOut::counters[9..10])
+    if (threadIdx.x == 0 && map.stat) { map.stat[0] = 0; map.stat[1] = 0; }   // per-scan work counters (IM_LC_REFITS, IM_LC_REFIT_POINTS)
 }
 // BuildResidualListOMP on caller-supplied Point_with_var data (world point + covariance per point)
 __global__ void __launch_bounds__(128) k_match_pv(VoxelMapDev map, LioParams P, ScanBuf sb, const double* pw, int n) {   // API call: explicit n
@@ -659,14 +659,15 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     IM_CUDA(h->dev.alloc(&m.chunks, (size_t)h->max_chunks));
     IM_CUDA(h->dev.alloc(&m.avail, (size_t)h->max_chunks));
     IM_CUDA(h->dev.alloc(&m.pending, (size_t)h->max_chunks));
-    IM_CUDA(h->dev.alloc(&h->d_counters, 16, 0));
-    m.node_count = h->d_counters + 0; m.chunk_bump = h->d_counters + 1; m.avail_top = h->d_counters + 2; m.pending_n = h->d_counters + 3;
-    m.err = h->d_counters + 4; m.n_roots = h->d_counters + 5; m.stat = h->d_counters + 9;
+    IM_CUDA(h->dev.alloc(&h->d_counters, IM_LC_SIZE, 0));
+    m.node_count = h->d_counters + IM_LC_NODES; m.chunk_bump = h->d_counters + IM_LC_CHUNK_BUMP; m.avail_top = h->d_counters + IM_LC_AVAIL_TOP;
+    m.pending_n = h->d_counters + IM_LC_PENDING; m.err = h->d_counters + IM_LC_ERR; m.n_roots = h->d_counters + IM_LC_ROOTS;
+    m.stat = h->d_counters + IM_LC_REFITS;   // [0] refits, [1] refit points
     m.max_nodes = h->max_nodes; m.max_chunks = h->max_chunks;
     IM_CUDA(h->dev.alloc(&m.pub, (size_t)h->max_nodes));
     IM_CUDA(h->dev.alloc(&m.pub_mark, h->cap, 0));
     IM_CUDA(h->dev.alloc(&m.pub_list, h->cap));
-    m.pub_n = h->d_counters + 12;
+    m.pub_n = h->d_counters + IM_LC_PUB_N;
     ScanBuf& sb = h->sb;
     const size_t ms = (size_t)h->max_scan;
     float* d_body = nullptr;
@@ -692,13 +693,13 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     IM_CUDA(h->dev.alloc(&sb.slot_count, h->cap, 0));
     IM_CUDA(h->dev.alloc(&sb.slot_offset, h->cap, 0));
     IM_CUDA(h->dev.alloc(&sb.slot_cursor, h->cap, 0));
-    sb.n_touched = h->d_counters + 6; sb.seg_top = h->d_counters + 7;
+    sb.n_touched = h->d_counters + IM_LC_TOUCHED; sb.seg_top = h->d_counters + IM_LC_SEG_TOP;
     sb.n = 0;
     IM_CUDA(h->dev.alloc(&h->d_ctrl, 1, 0));
     sb.dyn = &h->d_ctrl->dyn;
     IM_CUDA(h->pinned.alloc(&h->h_body, IM_SLOTS * ms * 3));
     IM_CUDA(h->pinned.alloc(&h->h_state, IM_STATE_DOUBLES + 64));
-    IM_CUDA(h->pinned.alloc(&h->h_ints, 64));
+    IM_CUDA(h->pinned.alloc(&h->h_ints, IM_HINT_SIZE));
     IM_CUDA(h->pinned.alloc(&h->h_dyn, IM_SLOTS));
     IM_CUDA(h->pinned.alloc(&h->h_out, IM_SLOTS));
     std::memset(h->h_out, 0, IM_SLOTS * sizeof(LioOut));
@@ -853,8 +854,8 @@ static void scan_rows_overwritten(immesh_lio* h, const char* by) {
 static void note_counters(immesh_lio* h, const int* c, long long step) {
     if (step <= h->known_step) return;
     // the difference to the last known step; over several steps (their blocks were not all seen) it bounds one step from above
-    h->max_step_nodes = std::max(h->max_step_nodes, c[0] - h->known[0]);
-    h->max_step_chunks = std::max(h->max_step_chunks, c[1] - h->known[1]);
+    h->max_step_nodes = std::max(h->max_step_nodes, c[IM_LC_NODES] - h->known[IM_LC_NODES]);
+    h->max_step_chunks = std::max(h->max_step_chunks, c[IM_LC_CHUNK_BUMP] - h->known[IM_LC_CHUNK_BUMP]);
     std::memcpy(h->known, c, sizeof(h->known));
     h->known_step = step;
 }
@@ -867,11 +868,15 @@ static void note_slots(immesh_lio* h, bool only_finished) {
     std::sort(order, order + n, [&](int a, int b) { return h->slot_step[a] < h->slot_step[b]; });
     for (int i = 0; i < n; ++i) note_counters(h, h->h_out[order[i]].counters, h->slot_step[order[i]]);
 }
+// the counter block into c (IM_LC_SIZE ints), blocking: the caller has drained what it needs
+static cudaError_t lio_read_counters(const immesh_lio* h, int* c) {
+    return cudaMemcpy(c, h->d_counters, IM_LC_SIZE * sizeof(int), cudaMemcpyDeviceToHost);
+}
 static int check_flags(immesh_lio* h) {
-    IM_CUDA(cudaMemcpyAsync(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaMemcpyAsync(h->h_ints, h->d_counters, IM_LC_SIZE * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
     if (h->grow_max_bytes > 0) note_counters(h, h->h_ints, h->map_steps);
-    return lio_flags_status(h->h_ints[4]);
+    return lio_flags_status(h->h_ints[IM_LC_ERR]);
 }
 
 // ---- growth of the map pools.  Bytes per record: root slot 32 (key 8, root_node 4, pub_mark 4, pub_list 4, the per-scan
@@ -904,10 +909,11 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
                                            std::to_string(h->grow_max_bytes) + " (immesh_lio_set_growth)").c_str());
     }
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
-    const int n_nodes = std::min(h->h_ints[0], h->max_nodes), n_chunks = std::min(h->h_ints[1], h->max_chunks);
-    const int n_avail = std::max(0, std::min(h->h_ints[2], h->max_chunks)), n_pending = std::min(h->h_ints[3], h->max_chunks);
-    const int n_pub = std::min<long long>(h->h_ints[12], cap0);
+    IM_CUDA(lio_read_counters(h, h->h_ints));
+    const int* c = h->h_ints;
+    const int n_nodes = std::min(c[IM_LC_NODES], h->max_nodes), n_chunks = std::min(c[IM_LC_CHUNK_BUMP], h->max_chunks);
+    const int n_avail = std::max(0, std::min(c[IM_LC_AVAIL_TOP], h->max_chunks)), n_pending = std::min(c[IM_LC_PENDING], h->max_chunks);
+    const int n_pub = std::min<long long>(c[IM_LC_PUB_N], cap0);
 
     VoxelMapDev nm = h->map;   // the map after the growth
     ScanBuf nsb = h->sb;
@@ -1012,7 +1018,7 @@ static int lio_growth_check(immesh_lio* h, long long n) {
         if (pass == 1) return lio_grow(h, cap, nodes, chunks);
         IM_CUDA(cudaStreamSynchronize(h->stream));
         note_slots(h, false);
-        IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+        IM_CUDA(lio_read_counters(h, h->h_ints));
         note_counters(h, h->h_ints, h->map_steps);
         steps = 1;
         n_max = n;
@@ -1027,9 +1033,10 @@ static void launch_grow(immesh_lio* h, int mode) {
     IM_LAUNCH(k_grow_point, g, 128, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, mode);
     IM_LAUNCH(k_grow_segment, grid_fixed(h, 128, 2), 128, 0, h->stream, h->sb);
     IM_LAUNCH(k_grow_scatter, g, 128, 0, h->stream, h->sb);
-    IM_LAUNCH(k_grow_simple, h->n_sm * 16, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_complex, h->d_counters + 11);
-    IM_LAUNCH(k_grow_voxel, h->n_sm * GROW_VOXEL_BPS, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + 8, (const int*)h->d_complex, (const int*)(h->d_counters + 11));
-    IM_LAUNCH(k_grow_finish, 1, 256, 0, h->stream, h->map, h->sb, h->d_counters + 8, h->d_ctrl, (const int*)h->d_counters);
+    int* n_complex = h->d_counters + IM_LC_COMPLEX;
+    IM_LAUNCH(k_grow_simple, h->n_sm * 16, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_complex, n_complex);
+    IM_LAUNCH(k_grow_voxel, h->n_sm * GROW_VOXEL_BPS, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + IM_LC_WORK, (const int*)h->d_complex, (const int*)n_complex);
+    IM_LAUNCH(k_grow_finish, 1, 256, 0, h->stream, h->map, h->sb, h->d_ctrl, h->d_counters);
 }
 // IESKF iterations.  One GPU: per iteration k_match then k_terms; the last block of k_terms runs the 6x6 IESKF update.
 // Sharded over peer windows: pass1(+publish bits) -> pass2(wait bits, +publish sums) -> solve(wait sums), exchanges fused in.
@@ -1108,9 +1115,9 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
     if (rc) return rc;
     h->scan_rows = 1;
     IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(h->h_ints + 32, &h->d_ctrl->iters_run, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_ITERS, &h->d_ctrl->iters_run, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     rc = check_flags(h);
-    if (iters_run) *iters_run = h->h_ints[32];
+    if (iters_run) *iters_run = h->h_ints[IM_HINT_ITERS];
     h->pose_pub_idx = -1;
     return rc;
 }
@@ -1197,7 +1204,7 @@ static int lio_wait_impl(immesh_lio_t* h, double* state_out, int* iters_run, boo
         cudaEventElapsedTime(&c, h->ev[2], h->ev[3]);
         h->last_ms[0] = a; h->last_ms[1] = b; h->last_ms[2] = c;
     }
-    return lio_flags_status(o.counters[4]);
+    return lio_flags_status(o.counters[IM_LC_ERR]);
 }
 
 int immesh_lio_step(immesh_lio_t* h, const float* body, int n, double dt, double cov_gyr, double cov_acc, double* state_out, int* iters_run) {
@@ -1258,7 +1265,7 @@ int immesh_lio_enqueue_memset(immesh_lio_t* h, void* d_buf, size_t bytes) {
 int immesh_lio_work_stats(immesh_lio_t* h, int64_t* out /*[4]*/) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const LioOut& o = h->h_out[h->step_counter & (IM_SLOTS - 1)];
-    out[0] = h->last_n; out[1] = o.counters[5]; out[2] = o.counters[9]; out[3] = o.counters[10];
+    out[0] = h->last_n; out[1] = o.counters[IM_LC_ROOTS]; out[2] = o.counters[IM_LC_REFITS]; out[3] = o.counters[IM_LC_REFIT_POINTS];
     return IMMESH_OK;
 }
 int immesh_lio_last_timing(immesh_lio_t* h, double* ms) {
@@ -1419,9 +1426,9 @@ int immesh_lio_match_nodes(immesh_lio_t* h, int* node, int n) {
 
 int64_t immesh_voxelmap_dump(immesh_lio_t* h, double* rows, int64_t cap_rows) {
     if (!h) return -1;
-    int counters[16];
-    if (cudaMemcpy(counters, h->d_counters, sizeof(counters), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    const int nn = counters[0] < h->max_nodes ? counters[0] : h->max_nodes;
+    int c[IM_LC_SIZE];
+    if (lio_read_counters(h, c) != cudaSuccess) return -1;
+    const int nn = c[IM_LC_NODES] < h->max_nodes ? c[IM_LC_NODES] : h->max_nodes;
     std::vector<unsigned long long> keys(h->cap);
     std::vector<int> roots(h->cap);
     std::vector<NodeRec> nodes(nn > 0 ? nn : 1);
@@ -1440,9 +1447,9 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     *n_out = 0;
     if (counts) for (int k = 0; k < 5; ++k) counts[k] = 0;
     IM_CUDA(cudaStreamSynchronize(h->stream));   // everything queued on the handle, the pipelined steps included
-    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, h->map.pub_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_PUB, h->map.pub_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    const int n = h->h_ints[40];
+    const int n = h->h_ints[IM_HINT_PUB];
     if (counts) counts[4] = n;
     if (n == 0) return IMMESH_OK;
     const int nb = (n + VG_TILE - 1) / VG_TILE;
@@ -1465,11 +1472,11 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     IM_LAUNCH(k_pub_count, g, PUB_THREADS, 0, st, h->map, n, (const unsigned int*)vu[cur], slots, cnt, misc + 1);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, cnt, n, misc);
     IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, misc, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_PUB, misc, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
-    const int total = h->h_ints[40];
+    const int total = h->h_ints[IM_HINT_PUB];
     *n_out = total;
-    if (counts) for (int k = 0; k < 4; ++k) counts[k] = h->h_ints[41 + k];
+    if (counts) for (int k = 0; k < 4; ++k) counts[k] = h->h_ints[IM_HINT_PUB + 1 + k];
     if (total > cap) return im_fail(IMMESH_E_CAPACITY, "plane markers: more rows than cap (*n_out holds the number needed; nothing was consumed)");
     // at least one row, so that k_pub_emit never gets a null pointer
     IM_CUDA(h->scratch.regrow(&h->d_pub_rows, &h->pub_rows_doubles, std::max<size_t>((size_t)total, 1) * IM_PUB_COLS, (size_t)1024 * IM_PUB_COLS));
@@ -1496,9 +1503,9 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, i
     IM_LAUNCH(k_eff_count, nb, SPUB_THREADS, 0, st, h->sb, tiles);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, tiles, nb, tiles + nb);
     IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, tiles + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_PUB, tiles + nb, sizeof(int), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
-    const int total = h->h_ints[40];
+    const int total = h->h_ints[IM_HINT_PUB];
     *n_out = total;
     if (total > cap) return im_fail(IMMESH_E_CAPACITY, "effect cloud: more rows than cap (*n_out holds the number needed)");
     if (total == 0) return IMMESH_OK;
@@ -1530,9 +1537,9 @@ static int registered_rows(immesh_lio_t* h, const float* pts, const float* inten
         IM_CUDA(h->scratch.regrow(&h->d_spub_tiles, &h->spub_tiles_cap, 1, 1024));
         IM_LAUNCH(k_scan_n, 1, 1, 0, st, h->sb, h->d_spub_tiles);
         IM_CUDA(cudaGetLastError());
-        IM_CUDA(cudaMemcpyAsync(h->h_ints + 40, h->d_spub_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_PUB, h->d_spub_tiles, sizeof(int), cudaMemcpyDeviceToHost, st));
         IM_CUDA(cudaStreamSynchronize(st));
-        n = h->h_ints[40];
+        n = h->h_ints[IM_HINT_PUB];
     }
     const int m = n > 0 ? (n - 1) / point_skip + 1 : 0;
     *n_out = m;
@@ -1563,20 +1570,20 @@ int immesh_lio_registered_cloud_sep(immesh_lio_t* h, const float* d_xyz, const f
 
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
-    int counters[16];
-    IM_CUDA(cudaMemcpy(counters, h->d_counters, sizeof(counters), cudaMemcpyDeviceToHost));
-    out[0] = counters[5]; out[1] = counters[0]; out[2] = counters[1]; out[3] = counters[4];
+    int c[IM_LC_SIZE];
+    IM_CUDA(lio_read_counters(h, c));
+    out[0] = c[IM_LC_ROOTS]; out[1] = c[IM_LC_NODES]; out[2] = c[IM_LC_CHUNK_BUMP]; out[3] = c[IM_LC_ERR];
     return IMMESH_OK;
 }
 
 int immesh_lio_capacity(immesh_lio_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+    IM_CUDA(lio_read_counters(h, h->h_ints));
     const int* c = h->h_ints;
-    out[0] = (int64_t)h->cap; out[1] = c[5];
-    out[2] = h->max_nodes; out[3] = c[0];
-    out[4] = h->max_chunks; out[5] = (int64_t)c[1] - std::max(c[2], 0);
+    out[0] = (int64_t)h->cap; out[1] = c[IM_LC_ROOTS];
+    out[2] = h->max_nodes; out[3] = c[IM_LC_NODES];
+    out[4] = h->max_chunks; out[5] = (int64_t)c[IM_LC_CHUNK_BUMP] - std::max(c[IM_LC_AVAIL_TOP], 0);
     out[6] = (int64_t)h->dev.bytes(); out[7] = h->growths;
     return IMMESH_OK;
 }
@@ -1595,7 +1602,7 @@ int immesh_lio_set_growth(immesh_lio_t* h, int64_t max_bytes) {
     if (max_bytes > 0 && h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_set_growth: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
     if (max_bytes > 0 && h->grow_max_bytes <= 0) {   // growth starts from the map as it is now
         IM_CUDA(cudaStreamSynchronize(h->stream));
-        IM_CUDA(cudaMemcpy(h->h_ints, h->d_counters, 16 * sizeof(int), cudaMemcpyDeviceToHost));
+        IM_CUDA(lio_read_counters(h, h->h_ints));
         note_counters(h, h->h_ints, ++h->map_steps);   // the map as it is now, under a step number of its own
     }
     h->grow_max_bytes = max_bytes;

@@ -43,12 +43,30 @@ struct ScanDyn {
     const int* n_dev;         // when not null: the number of points is read from here at execution time (a device-resident
                               // front-end produced the scan: no host round trip of the count)
 };
+// Slots of the localization's counter block (immesh_lio::d_counters), wired into VoxelMapDev and ScanBuf at create: name, writer, reset
+enum : int {
+    IM_LC_NODES = 0,         // VoxelMapDev::node_count: node records allocated (alloc_node); never reset
+    IM_LC_CHUNK_BUMP = 1,    // VoxelMapDev::chunk_bump: chunks ever taken from the pool (alloc_chunk); never reset
+    IM_LC_AVAIL_TOP = 2,     // VoxelMapDev::avail_top: recycled chunks on the free stack (alloc_chunk, recycle_chunks)
+    IM_LC_PENDING = 3,       // VoxelMapDev::pending_n: chunks freed this scan (node_free_points); recycle_chunks
+    IM_LC_ERR = 4,           // VoxelMapDev::err: IM_ERR_* flags; never reset
+    IM_LC_ROOTS = 5,         // VoxelMapDev::n_roots: root voxels; never reset
+    IM_LC_TOUCHED = 6,       // ScanBuf::n_touched: root voxels the scan touched (grow_point); k_grow_finish
+    IM_LC_SEG_TOP = 7,       // ScanBuf::seg_top: points placed into the touched voxels' segments; k_grow_finish
+    IM_LC_WORK = 8,          // voxel ticket of k_grow_voxel; k_grow_finish
+    IM_LC_REFITS = 9,        // VoxelMapDev::stat[0]: plane refits of the scan; k_grow_finish
+    IM_LC_REFIT_POINTS = 10, // VoxelMapDev::stat[1]: points read by the refits; k_grow_finish
+    IM_LC_COMPLEX = 11,      // touched root voxels left to k_grow_voxel (k_grow_simple); k_grow_finish
+    IM_LC_PUB_N = 12,        // VoxelMapDev::pub_n: entries of the plane-map publisher's pending list; immesh_voxelmap_plane_markers
+    IM_LC_SIZE = 16,         // ints allocated, read back and copied into LioOut::counters
+};
+
 // what the host reads back after a scan, one D2H copy
 struct LioOut {
     double state[IM_STATE_DOUBLES];
     int iters_run;
     int scan_idx;
-    int counters[16];
+    int counters[IM_LC_SIZE];
     int pad_[2];
 };
 #define IM_POSE_RING 8

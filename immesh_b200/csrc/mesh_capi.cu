@@ -29,13 +29,7 @@ __global__ void k_frame_begin(MeshDev M, FrameBuf F_) {
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
     for (unsigned int i = tid; i <= F.cmask; i += nt) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
     for (unsigned int i = tid; i <= F.fset_mask; i += nt) F.fset[i] = -1;
-    if (tid == 0) {
-        for (int k = 5; k <= 10; ++k) M.cnt[k] = 0;
-        for (int k = 17; k <= 26; ++k) M.cnt[k] = 0;
-        M.cnt[28] = 0;
-        M.cnt[29] = 0;
-        M.cnt[30] = 0; M.cnt[31] = 0; M.cnt[32] = 0;
-    }
+    if (tid == 0) mesh_cnt_frame_begin(M);
 }
 __global__ void __launch_bounds__(128) k_cand_init(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
@@ -53,7 +47,7 @@ __global__ void __launch_bounds__(128) k_cand_resolve(MeshDev M, MeshParams P, F
     __shared__ int s_ticket;
     const int nblocks = (F.m + blockDim.x - 1) / blockDim.x;
     while (true) {
-        if (threadIdx.x == 0) s_ticket = atomicAdd(&M.cnt[18], 1);
+        if (threadIdx.x == 0) s_ticket = atomicAdd(&M.cnt[IM_MC_RESOLVE_TICKET], 1);
         __syncthreads();
         const int b = s_ticket;
         __syncthreads();
@@ -62,7 +56,7 @@ __global__ void __launch_bounds__(128) k_cand_resolve(MeshDev M, MeshParams P, F
         if (c < F.m && F.cand_status[c] == CAND_UNDECIDED) {
             int polls = 0;
             while (!cand_poll(M, P, F, c)) {
-                if (++polls > (1 << 22)) { atomicOr(&M.cnt[3], IM_MERR_LIST_CAP); atomicAdd(&M.cnt[9], 1); break; }
+                if (++polls > (1 << 22)) { atomicOr(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP); atomicAdd(&M.cnt[IM_MC_UNDECIDED], 1); break; }
                 __nanosleep(64);
             }
             __threadfence();
@@ -90,17 +84,17 @@ __global__ void __launch_bounds__(1024) k_cand_scan(MeshDev M, FrameBuf F_) {
 }
 __global__ void __launch_bounds__(128) k_cand_commit(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int base = M.cnt[0];
+    const int base = M.cnt[IM_MC_VERTICES];
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_commit(M, P, F, c, base);
 }
 __global__ void __launch_bounds__(128) k_cand_place(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int base = M.cnt[0];
+    const int base = M.cnt[IM_MC_VERTICES];
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_place(M, F, c, base);
 }
 __global__ void __launch_bounds__(128) k_voxel_select(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int na = min(M.cnt[5], F.max_act);
+    const int na = min(M.cnt[IM_MC_ACT], F.max_act);
     for (int a = blockIdx.x * blockDim.x + threadIdx.x; a < na; a += gridDim.x * blockDim.x) voxel_select(M, F, a);
 }
 // stage A: dilation (exact 20-NN of the in-voxel vertices + smoothing); one block per (voxel, group of <= 8 queries)
@@ -108,9 +102,9 @@ __global__ void __launch_bounds__(128) k_voxel_dilate(MeshDev M, MeshParams P, F
     const FrameBuf F = frame_load_dyn(F_);
     __shared__ DilateSmem S;
     __shared__ int s_item;
-    const int ni = min(M.cnt[29], F.max_ditem);
+    const int ni = min(M.cnt[IM_MC_DITEMS], F.max_ditem);
     while (true) {
-        if (threadIdx.x == 0) s_item = atomicAdd(&M.cnt[24], 1);
+        if (threadIdx.x == 0) s_item = atomicAdd(&M.cnt[IM_MC_DILATE_TICKET], 1);
         __syncthreads();
         const int i = s_item;
         __syncthreads();
@@ -132,7 +126,7 @@ __global__ void __launch_bounds__(128) k_voxel_tri_warp(MeshDev M, MeshParams P,
     int n_done = 0;
     while (true) {
         int i = 0;
-        if (lane == 0) i = atomicAdd(&M.cnt[19], 1);
+        if (lane == 0) i = atomicAdd(&M.cnt[IM_MC_TRI_TICKET], 1);
         i = __shfl_sync(0xffffffffu, i, 0);
         if (i >= nw) break;
         voxel_mesh_warp<128>(M, P, F, work_slot(M, F, i), S, lane, 32, n_max);
@@ -145,17 +139,17 @@ __global__ void __launch_bounds__(128) k_voxel_tri_warp(MeshDev M, MeshParams P,
 // stage C (flat): after every voxel's smoothing is final
 __global__ void __launch_bounds__(128) k_commit_faces(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int nf = min(M.cnt[25], F.max_list);
+    const int nf = min(M.cnt[IM_MC_FACES], F.max_list);
     for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < nf; f += gridDim.x * blockDim.x) commit_face(M, P, F, f);
 }
 __global__ void __launch_bounds__(128) k_pull_vertices(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int nr = min(M.cnt[26], F.max_vref);
+    const int nr = min(M.cnt[IM_MC_VREFS], F.max_vref);
     for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nr; r += gridDim.x * blockDim.x) pull_vertex(M, P, F, r);
 }
 __global__ void __launch_bounds__(128) k_pull_check(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int ne = min(M.cnt[28], F.max_list);
+    const int ne = min(M.cnt[IM_MC_PULLED], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < ne; e += gridDim.x * blockDim.x) pull_check(M, F, e);
 }
 template <int MAXD>
@@ -174,18 +168,16 @@ __global__ void __launch_bounds__(128) k_voxel_mesh(MeshDev M, MeshParams P, Fra
 }
 __global__ void __launch_bounds__(128) k_push_remove(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int n = min(M.cnt[8], F.max_list);
+    const int n = min(M.cnt[IM_MC_REMOVE], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) tri_remove(M, F.rem_tri[e]);
 }
 __global__ void __launch_bounds__(128) k_push_add(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
-    const int n = min(M.cnt[7], F.max_list);
+    const int n = min(M.cnt[IM_MC_ADD], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x)
         tri_add(M, F.add_tri[(size_t)e * 3 + 0], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
 }
-__global__ void k_frame_end(MeshDev M) {
-    M.cnt[0] += M.cnt[10];
-}
+__global__ void k_frame_end(MeshDev M) { mesh_cnt_frame_end(M); }
 // snapshot: compact live triangles
 __global__ void __launch_bounds__(128) k_snapshot(MeshDev M, int n_alloc, int* out_tri, int* out_flip, int* out_n) {
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
@@ -211,10 +203,10 @@ __global__ void __launch_bounds__(128) k_knn(MeshDev M, MeshParams P, const floa
         int lid[KNN_KMAX];
         int ln = 0;
         int far = 0;
-        if (M.cnt[4] > 0) {
-            far = max(far, max(abs(cx - M.cnt[11]), abs(cx - M.cnt[14])));
-            far = max(far, max(abs(cy - M.cnt[12]), abs(cy - M.cnt[15])));
-            far = max(far, max(abs(cz - M.cnt[13]), abs(cz - M.cnt[16])));
+        if (M.cnt[IM_MC_VOXELS] > 0) {
+            far = max(far, max(abs(cx - M.cnt[IM_MC_BBOX_MIN_X]), abs(cx - M.cnt[IM_MC_BBOX_MAX_X])));
+            far = max(far, max(abs(cy - M.cnt[IM_MC_BBOX_MIN_Y]), abs(cy - M.cnt[IM_MC_BBOX_MAX_Y])));
+            far = max(far, max(abs(cz - M.cnt[IM_MC_BBOX_MIN_Z]), abs(cz - M.cnt[IM_MC_BBOX_MAX_Z])));
         } else {
             far = -1;
         }
@@ -342,7 +334,7 @@ __device__ __forceinline__ void rf_tiles(const DepthTri& T, int* tx0, int* tx1, 
 // count pass: bin entries per tile
 __global__ void __launch_bounds__(128) k_rf_count(MeshDev M, const DepthCam* cam, int* tile_cnt) {
     const DepthCam C = *cam;
-    const int n_alloc = min(M.cnt[1], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
@@ -372,7 +364,7 @@ __global__ void __launch_bounds__(1024) k_rf_scan(const int* cnt, int n, int* of
 __global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, const DepthCam* cam, int* cur, int* bin, const int* misc) {
     if (misc[0]) return;
     const DepthCam C = *cam;
-    const int n_alloc = min(M.cnt[1], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
@@ -392,7 +384,7 @@ __global__ void __launch_bounds__(IM_RT_THREADS) k_rf_tile(MeshDev M, const Dept
     const int ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
     const int x = (blockIdx.x % ntx) * IM_RT_TILE + (int)(threadIdx.x % IM_RT_TILE), y = (blockIdx.x / ntx) * IM_RT_TILE + (int)(threadIdx.x / IM_RT_TILE);
     const bool all = misc[0] != 0;
-    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[1], M.max_t) : tile_off[blockIdx.x + 1];
+    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t) : tile_off[blockIdx.x + 1];
     unsigned int acc = 0x7f800000u;   // +inf
     for (int b = lo; b < hi; b += IM_RT_THREADS) {
         const int i = b + (int)threadIdx.x;
@@ -553,25 +545,20 @@ __global__ void k_rb_axis(const AxisAcc* part, int nb, float* box) {
 }
 
 // ---- the batched frame (immesh_mesh_push_frame_batched): one frame, append in chunks, per-voxel stage in batches.  The frame-level
-// counters of the per-frame path are accumulated across chunks / batches in cnt[33] (new vertices), cnt[34] (add entries), cnt[35]
-// (meshed voxels) and written back by k_bat_frame_end; cnt[36] counts the meshed voxels of the selection.
+// counters of the per-frame path are accumulated across chunks / batches in the IM_MC_BAT_* slots and written back by k_bat_frame_end.
 __global__ void k_bat_chunk_begin(MeshDev M, FrameBuf F) {   // the candidate grid of one append chunk after the first
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
     for (unsigned int i = tid; i <= F.cmask; i += nt) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
-    if (tid == 0) { M.cnt[9] = 0; M.cnt[18] = 0; }
+    if (tid == 0) mesh_cnt_bat_chunk_begin(M);
 }
-__global__ void k_bat_chunk_end(MeshDev M) {   // the chunk's vertices are in the map before the next chunk is examined
-    M.cnt[0] += M.cnt[10];
-    M.cnt[33] += M.cnt[10];
-    M.cnt[10] = 0;
-}
+__global__ void k_bat_chunk_end(MeshDev M) { mesh_cnt_bat_chunk_end(M); }
 // activation rule over every activated voxel of the frame (after the last chunk); the meshed ones with their keys
 __global__ void __launch_bounds__(128) k_bat_select(MeshDev M, FrameBuf F, int* sel, unsigned long long* key) {
-    const int na = min(M.cnt[5], F.max_act);
+    const int na = min(M.cnt[IM_MC_ACT], F.max_act);
     for (int a = blockIdx.x * blockDim.x + threadIdx.x; a < na; a += gridDim.x * blockDim.x) {
         const int vs = F.act[a];
         if (!voxel_activate(M, F, vs)) continue;
-        const int k = atomicAdd(&M.cnt[36], 1);
+        const int k = atomicAdd(&M.cnt[IM_MC_BAT_SELECTED], 1);
         sel[k] = vs;
         key[k] = M.vkeys[vs];
     }
@@ -587,10 +574,7 @@ __global__ void __launch_bounds__(128) k_bat_word(int n, int half, const unsigne
 __global__ void k_bat_reset(MeshDev M, FrameBuf F, int clear_fset) {   // the per-batch lists
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
     if (clear_fset) for (unsigned int i = tid; i <= F.fset_mask; i += nt) F.fset[i] = -1;
-    if (tid == 0) {
-        M.cnt[6] = 0; M.cnt[7] = 0; M.cnt[17] = 0; M.cnt[19] = 0;
-        M.cnt[24] = 0; M.cnt[25] = 0; M.cnt[26] = 0; M.cnt[28] = 0; M.cnt[29] = 0;
-    }
+    if (tid == 0) mesh_cnt_bat_reset(M);
 }
 // meshed voxels [lo, hi) in key order -> the batch's work list; the rank is the flip priority
 __global__ void __launch_bounds__(128) k_bat_fill(MeshDev M, FrameBuf F, const int* sel, const unsigned int* order, int lo, int hi, int* rank) {
@@ -601,19 +585,16 @@ __global__ void __launch_bounds__(128) k_bat_fill(MeshDev M, FrameBuf F, const i
 }
 // the batch's additions, pushed at once; marked so that later batches' pulls and commits do not see them as pre-frame triangles
 __global__ void __launch_bounds__(128) k_bat_push_add(MeshDev M, FrameBuf F) {
-    const int n = min(M.cnt[7], F.max_list);
+    const int n = min(M.cnt[IM_MC_ADD], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
         const int t = tri_add(M, F.add_tri[(size_t)e * 3 + 0], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
         if (t >= 0) F.tri_mark[t] = IM_TRI_BORN;
     }
 }
-__global__ void k_bat_batch_end(MeshDev M) {
-    M.cnt[34] += M.cnt[7];
-    M.cnt[35] += M.cnt[6] + M.cnt[17];
-}
+__global__ void k_bat_batch_end(MeshDev M) { mesh_cnt_bat_batch_end(M); }
 // after the last batch: the deferred removals; every mark cleared for the next frame
 __global__ void __launch_bounds__(128) k_bat_sweep(MeshDev M, FrameBuf F) {
-    const int n = min(M.cnt[1], M.max_t);
+    const int n = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t);
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
         const unsigned char m = F.tri_mark[t];
         if (!m) continue;
@@ -621,12 +602,7 @@ __global__ void __launch_bounds__(128) k_bat_sweep(MeshDev M, FrameBuf F) {
         F.tri_mark[t] = 0;
     }
 }
-__global__ void k_bat_frame_end(MeshDev M) {
-    M.cnt[10] = M.cnt[33];
-    M.cnt[7] = M.cnt[34];
-    M.cnt[6] = M.cnt[35];
-    M.cnt[17] = 0;
-}
+__global__ void k_bat_frame_end(MeshDev M) { mesh_cnt_bat_frame_end(M); }
 
 // ---- growth of the mesh pools (immesh_mesh_reserve): the three open-addressed tables rebuilt into tables of the new size
 #define MGROW_THREADS 256
@@ -716,12 +692,10 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     const size_t tcap = pow2_at_least((size_t)max_t * 2);
     IM_CUDA(h->dev.alloc(&M.thash, tcap, 0xFF));
     M.tmask = (unsigned)(tcap - 1);
-    IM_CUDA(h->dev.alloc(&M.cnt, 64, 0));
+    IM_CUDA(h->dev.alloc(&M.cnt, IM_MC_ALLOC, 0));
     {
-        int init[32];
-        std::memset(init, 0, sizeof(init));
-        init[11] = init[12] = init[13] = 0x7fffffff;
-        init[14] = init[15] = init[16] = -0x7fffffff;
+        int init[IM_MC_HOST] = {};
+        mesh_cnt_init(init);
         IM_CUDA(cudaMemcpy(M.cnt, init, sizeof(init), cudaMemcpyHostToDevice));
     }
     FrameBuf& F = h->F;
@@ -768,7 +742,7 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     IM_CUDA(h->dev.alloc(&F.add_flip, (size_t)F.max_list));
     IM_CUDA(h->dev.alloc(&F.rem_tri, (size_t)F.max_list));
     IM_CUDA(h->pinned.alloc(&h->h_pts, IM_SLOTS * mc * 3));
-    IM_CUDA(h->pinned.alloc(&h->h_cnt, IM_SLOTS * 32));
+    IM_CUDA(h->pinned.alloc(&h->h_cnt, IM_SLOTS * IM_MC_HOST));
     IM_CUDA(h->pinned.alloc(&h->h_fp, IM_SLOTS));
     IM_CUDA(h->pinned.alloc(&h->h_dyn, IM_SLOTS));
     IM_CUDA(h->dev.alloc(&h->d_dyn, 1, 0));
@@ -860,9 +834,9 @@ struct XHeader { int n_smooth, n_face, n_rem, pad; };
 __global__ void k_xhdr(MeshDev M, FrameBuf F_, XHeader* hdr) {
     const FrameBuf F = frame_load_dyn(F_);
     if (threadIdx.x == 0) {
-        hdr->n_smooth = min(M.cnt[32], F.x_cap);
-        hdr->n_face = min(M.cnt[30], F.x_cap);
-        hdr->n_rem = min(M.cnt[31], F.x_cap);
+        hdr->n_smooth = min(M.cnt[IM_MC_X_SMOOTHS], F.x_cap);
+        hdr->n_face = min(M.cnt[IM_MC_X_FACES], F.x_cap);
+        hdr->n_rem = min(M.cnt[IM_MC_X_REMS], F.x_cap);
         hdr->pad = 0;
     }
 }
@@ -883,7 +857,7 @@ __global__ void __launch_bounds__(256) k_xpush(MeshDev M, FrameBuf F_, const uns
     const unsigned long long epoch = F.epoch;
     __shared__ int s_last;
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
-    const int n_smooth = min(M.cnt[32], F.x_cap), n_face = min(M.cnt[30], F.x_cap), n_rem = min(M.cnt[31], F.x_cap);
+    const int n_smooth = min(M.cnt[IM_MC_X_SMOOTHS], F.x_cap), n_face = min(M.cnt[IM_MC_X_FACES], F.x_cap), n_rem = min(M.cnt[IM_MC_X_REMS], F.x_cap);
     for (int r = 0; r < pe.n; ++r) {
         unsigned char* dst = pe.w[r] + pe.recv_off[which] + (size_t)pe.rank * pe.seg_bytes[which];
         if (tid == 0) *(int4*)dst = make_int4(n_smooth, n_face, n_rem, 0);
@@ -918,7 +892,7 @@ __device__ __forceinline__ void mesh_wait_peers(const MeshPeers& pe, int which, 
 __global__ void __launch_bounds__(256) k_apply_smooth(MeshDev M, FrameBuf F_, const unsigned char* recv, size_t seg_bytes, MeshPeers pe) {
     const FrameBuf F = frame_load_dyn(F_);
     const unsigned long long epoch = F.epoch;
-    mesh_wait_peers(pe, 0, epoch, &M.cnt[3]);
+    mesh_wait_peers(pe, 0, epoch, &M.cnt[IM_MC_ERR]);
     for (int r = 0; r < F.shard_n; ++r) {
         if (r == F.shard_rank) continue;
         const unsigned char* seg = recv + (size_t)r * seg_bytes;
@@ -935,7 +909,7 @@ __global__ void __launch_bounds__(256) k_apply_smooth(MeshDev M, FrameBuf F_, co
 __global__ void __launch_bounds__(256) k_apply_lists(MeshDev M, FrameBuf F_, const unsigned char* recv, size_t seg_bytes, MeshPeers pe) {
     const FrameBuf F = frame_load_dyn(F_);
     const unsigned long long epoch = F.epoch;
-    mesh_wait_peers(pe, 1, epoch, &M.cnt[3]);
+    mesh_wait_peers(pe, 1, epoch, &M.cnt[IM_MC_ERR]);
     for (int r = 0; r < F.shard_n; ++r) {
         const unsigned char* seg = recv + (size_t)r * seg_bytes;
         const int4 h = __ldcg((const int4*)seg);   // n_smooth, n_face, n_rem, -
@@ -967,6 +941,10 @@ static int mesh_status(int err) {
     return IMMESH_OK;
 }
 static void mesh_note(immesh_mesh* h, const int* c, int frame);
+// the host's copy of the counters (the first IM_MC_HOST slots), blocking: the caller has drained what it needs
+static cudaError_t mesh_read_counters(const immesh_mesh* h, int (&c)[IM_MC_HOST]) {
+    return cudaMemcpy(c, h->M.cnt, sizeof(c), cudaMemcpyDeviceToHost);
+}
 // wait for the frame queued in slot s and take over its counters
 static int mesh_harvest(immesh_mesh* h, int s) {
     if (!h->inflight[s]) return IMMESH_OK;
@@ -977,9 +955,9 @@ static int mesh_harvest(immesh_mesh* h, int s) {
         h->host_wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     }
     h->inflight[s] = 0;
-    std::memcpy(h->last_cnt, h->h_cnt + 32 * s, 32 * sizeof(int));
+    std::memcpy(h->last_cnt, h->h_cnt + IM_MC_HOST * s, sizeof(h->last_cnt));
     if (h->grow_max_bytes > 0) mesh_note(h, h->last_cnt, h->h_dyn[s].frame);
-    const int rc = mesh_status(h->last_cnt[3]);
+    const int rc = mesh_status(h->last_cnt[IM_MC_ERR]);
     if (rc && !h->pending_rc) h->pending_rc = rc;
     return rc;
 }
@@ -998,7 +976,7 @@ static size_t mesh_pool_bytes(const immesh_mesh* h, long long v, long long t, lo
 // counters of frame number `frame`, finished (see note_counters of the localization handle)
 static void mesh_note(immesh_mesh* h, const int* c, int frame) {
     if (frame <= h->known_frame) return;
-    h->max_step_tris = std::max(h->max_step_tris, c[1] - h->known[1]);   // over several frames: an upper bound of one
+    h->max_step_tris = std::max(h->max_step_tris, c[IM_MC_TRIS_ALLOC] - h->known[IM_MC_TRIS_ALLOC]);   // over several frames: an upper bound of one
     std::memcpy(h->known, c, sizeof(h->known));
     h->known_frame = frame;
 }
@@ -1023,9 +1001,9 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
                                            std::to_string(h->grow_max_bytes) + " (immesh_mesh_set_growth)").c_str());
     }
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int c[64];
-    IM_CUDA(cudaMemcpy(c, M.cnt, sizeof(c), cudaMemcpyDeviceToHost));
-    const int nv = std::min(c[0], M.max_v), nt = std::min(c[1], M.max_t), nch = std::min(c[27], M.max_vchunks);
+    int c[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, c));
+    const int nv = std::min(c[IM_MC_VERTICES], M.max_v), nt = std::min(c[IM_MC_TRIS_ALLOC], M.max_t), nch = std::min(c[IM_MC_VERT_CHUNKS], M.max_vchunks);
     MeshDev nm = M;
     FrameBuf nf = h->F;
     immesh::MemSet fresh;   // the new buffers, freed on every failure below
@@ -1145,7 +1123,7 @@ static int mesh_growth_check(immesh_mesh* h, long long m) {
         const int s = (h->frame_counter + i) & (IM_SLOTS - 1);
         if (!h->inflight[s]) continue;
         if (cudaEventQuery(h->ev_done[s]) == cudaSuccess) {
-            mesh_note(h, h->h_cnt + 32 * s, h->h_dyn[s].frame);
+            mesh_note(h, h->h_cnt + IM_MC_HOST * s, h->h_dyn[s].frame);
         } else {
             ++steps;
             m_max = std::max<long long>(m_max, h->h_dyn[s].m);
@@ -1160,7 +1138,7 @@ static int mesh_growth_check(immesh_mesh* h, long long m) {
         IM_CUDA(cudaStreamSynchronize(h->stream));
         for (int i = 1; i <= IM_SLOTS; ++i) {
             const int s = (h->frame_counter + i) & (IM_SLOTS - 1);
-            if (h->inflight[s]) mesh_note(h, h->h_cnt + 32 * s, h->h_dyn[s].frame);
+            if (h->inflight[s]) mesh_note(h, h->h_cnt + IM_MC_HOST * s, h->h_dyn[s].frame);
         }
         steps = 1;
         m_max = m;
@@ -1366,7 +1344,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     if (!queued) launch_frame(true);
     if (nccl_failed) return im_fail(IMMESH_E_CUDA, "ncclAllGather failed");
     IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(h->h_cnt + 32 * s, h->M.cnt, 32 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaMemcpyAsync(h->h_cnt + IM_MC_HOST * s, h->M.cnt, IM_MC_HOST * sizeof(int), cudaMemcpyDeviceToHost, st));
     if (!queued) IM_CUDA(cudaEventRecord(h->ev[4], st));
     IM_CUDA(cudaEventRecord(h->ev_done[s], st));
     h->inflight[s] = 1;
@@ -1507,11 +1485,11 @@ int immesh_mesh_wait(immesh_mesh_t* h) {
 int immesh_mesh_capacity(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int c[32];
-    IM_CUDA(cudaMemcpy(c, h->M.cnt, sizeof(c), cudaMemcpyDeviceToHost));
-    out[0] = h->M.max_v; out[1] = c[0];
-    out[2] = h->M.max_t; out[3] = c[1];
-    out[4] = h->max_vox; out[5] = c[4];
+    int c[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, c));
+    out[0] = h->M.max_v; out[1] = c[IM_MC_VERTICES];
+    out[2] = h->M.max_t; out[3] = c[IM_MC_TRIS_ALLOC];
+    out[4] = h->max_vox; out[5] = c[IM_MC_VOXELS];
     out[6] = (int64_t)(h->dev.bytes() + h->batch.bytes()); out[7] = h->growths;
     return IMMESH_OK;
 }
@@ -1527,7 +1505,7 @@ int immesh_mesh_set_growth(immesh_mesh_t* h, int64_t max_bytes) {
     if (max_bytes > 0 && h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_mesh_set_growth: a sharded handle cannot grow (its replicas would have to grow in lockstep)");
     if (max_bytes > 0 && h->grow_max_bytes <= 0) {   // growth starts from the mesh as it is now
         IM_CUDA(cudaStreamSynchronize(h->stream));
-        IM_CUDA(cudaMemcpy(h->known, h->M.cnt, sizeof(h->known), cudaMemcpyDeviceToHost));
+        IM_CUDA(mesh_read_counters(h, h->known));
         h->known_frame = h->frame_counter;
     }
     h->grow_max_bytes = max_bytes;
@@ -1536,22 +1514,24 @@ int immesh_mesh_set_growth(immesh_mesh_t* h, int64_t max_bytes) {
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const int* c = h->last_cnt;
-    out[0] = c[0]; out[1] = c[2]; out[2] = c[10]; out[3] = c[6] + c[17]; out[4] = c[7]; out[5] = c[8]; out[6] = c[4]; out[7] = c[5];
+    out[0] = c[IM_MC_VERTICES]; out[1] = c[IM_MC_TRIS_LIVE]; out[2] = c[IM_MC_NEW_VERTICES]; out[3] = c[IM_MC_WORK_FRONT] + c[IM_MC_WORK_BACK];
+    out[4] = c[IM_MC_ADD]; out[5] = c[IM_MC_REMOVE]; out[6] = c[IM_MC_VOXELS]; out[7] = c[IM_MC_ACT];
     return IMMESH_OK;
 }
 
 int immesh_mesh_work_stats(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const int* c = h->last_cnt;
-    out[0] = h->F.m; out[1] = c[20]; out[2] = c[21]; out[3] = c[22]; out[4] = c[23]; out[5] = c[6] + c[17]; out[6] = c[7]; out[7] = c[8];
+    out[0] = h->F.m; out[1] = c[IM_MC_STAT_GATHERED]; out[2] = c[IM_MC_STAT_QUERIES]; out[3] = c[IM_MC_STAT_DILATED]; out[4] = c[IM_MC_STAT_FACETS];
+    out[5] = c[IM_MC_WORK_FRONT] + c[IM_MC_WORK_BACK]; out[6] = c[IM_MC_ADD]; out[7] = c[IM_MC_REMOVE];
     return IMMESH_OK;
 }
 
 int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, int32_t* flips) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
-    int cnt[32];
-    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    const int nv = cnt[0], nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
+    int cnt[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, cnt));
+    const int nv = cnt[IM_MC_VERTICES], nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
     if (vertices && nv > 0) {
         std::vector<float4> v(nv);
         IM_CUDA(cudaMemcpy(v.data(), h->M.vpos, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -1607,9 +1587,9 @@ int immesh_knn(immesh_mesh_t* h, const float* query_xyz, int nq, int k, double m
 int immesh_mesh_smooth_all(immesh_mesh_t* h, double smooth_factor, int knn, double* smoothed) {
     if (!h || knn < 1 || knn > KNN_KMAX) return im_fail(IMMESH_E_INVALID, "bad argument (knn must be in [1,32])");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int cnt[32];
-    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    const int nv = cnt[0];
+    int cnt[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, cnt));
+    const int nv = cnt[IM_MC_VERTICES];
     if (nv == 0) return IMMESH_OK;
     immesh::MemSet tmp;
     int* di = nullptr;
@@ -1629,9 +1609,9 @@ int immesh_mesh_smooth_all(immesh_mesh_t* h, double smooth_factor, int knn, doub
 int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* region_keys, int32_t* region_offsets, int cap_regions, int32_t* triangles, int* n_regions) {
     if (!h || !(region_size > 0) || !n_regions) return im_fail(IMMESH_E_INVALID, "bad argument");
     IM_CUDA(cudaStreamSynchronize(h->stream));
-    int cnt[32];
-    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    const int nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
+    int cnt[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, cnt));
+    const int nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
     *n_regions = 0;
     if (nlive == 0) { if (region_offsets && cap_regions >= 0) region_offsets[0] = 0; return IMMESH_OK; }
     immesh::MemSet tmp;
@@ -1711,9 +1691,9 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     }
     IM_CUDA(cudaStreamSynchronize(h->stream));   // everything queued on the handle, the pipelined frames included
     cudaStream_t st = h->stream;
-    int cnt[32];
-    IM_CUDA(cudaMemcpy(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    const int nv = cnt[0], nalloc = std::min(cnt[1], h->M.max_t), nlive = cnt[2];
+    int cnt[IM_MC_HOST];
+    IM_CUDA(mesh_read_counters(h, cnt));
+    const int nv = cnt[IM_MC_VERTICES], nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
     const size_t nl = (size_t)std::max(nlive, 1);
     // scratch buffer i of the call, at least `bytes` long (grow-only, kept by the handle)
     auto grown = [h](int i, size_t bytes, void** out) {
@@ -1921,7 +1901,7 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     FramePose fp;
     for (int j = 0; j < 3; ++j) { fp.pose_t[j] = pose_t[j]; fp.prio_origin[j] = 0; }
     IM_CUDA(cudaMemcpyAsync(h->b_fp, &fp, sizeof(FramePose), cudaMemcpyHostToDevice, st));
-    IM_CUDA(cudaMemsetAsync(h->M.cnt + 33, 0, 4 * sizeof(int), st));
+    IM_CUDA(cudaMemsetAsync(h->M.cnt + IM_MC_BAT_VERTICES, 0, (IM_MC_BAT_SELECTED + 1 - IM_MC_BAT_VERTICES) * sizeof(int), st));
     // ---- append, chunk c = candidates [c B, (c + 1) B), candidate i = point i step.  Host input: gathered into the pinned slot c & 1
     // while the device works on the other one
     const size_t slot_pts = (size_t)h->max_frame_points * 3;
@@ -1966,7 +1946,7 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     IM_LAUNCH(k_bat_select, mesh_grid(h, h->max_vox, 128), 128, 0, st, h->M, F, h->b_sel, h->b_key);
     int nsel = 0;
     IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(&nsel, h->M.cnt + 36, sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaMemcpyAsync(&nsel, h->M.cnt + IM_MC_BAT_SELECTED, sizeof(int), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
     unsigned int* ku[2] = {h->b_ku, h->b_ku + h->max_vox};
     unsigned int* vu[2] = {h->b_vu, h->b_vu + h->max_vox};
@@ -2013,13 +1993,13 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     IM_LAUNCH(k_bat_sweep, h->n_sm * 8, 128, 0, st, h->M, F);
     IM_LAUNCH(k_bat_frame_end, 1, 1, 0, st, h->M);
     IM_CUDA(cudaGetLastError());
-    int cnt[32];
+    int cnt[IM_MC_HOST];
     IM_CUDA(cudaMemcpyAsync(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
     std::memcpy(h->last_cnt, cnt, sizeof(cnt));
     if (h->grow_max_bytes > 0) mesh_note(h, cnt, F.frame);
-    if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->batch.bytes(); stats[3] = cnt[7]; }
-    return mesh_status(cnt[3]);
+    if (stats) { stats[0] = chunks; stats[1] = nbat; stats[2] = (int64_t)h->batch.bytes(); stats[3] = cnt[IM_MC_ADD]; }
+    return mesh_status(cnt[IM_MC_ERR]);
 }
 
 int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* world_xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels,

@@ -95,10 +95,95 @@ struct MeshDev {
     int* thash;           // open addressing on the triple, value = triangle index
     unsigned int tmask;
     int max_t;
-    // counters: 0 n_vertices, 1 n_tris_alloc, 2 n_live, 3 err, 4 n_voxels, 5 n_act, 6 n_work, 7 n_add, 8 n_remove,
-    //           9 n_undecided, 10 frame_new_vertices, 11..13 key bbox min, 14..16 key bbox max, 17 bbox valid
-    int* cnt;
+    int* cnt;             // [IM_MC_ALLOC] the counter block, slots IM_MC_*
 };
+
+// Slots of MeshDev::cnt: name, writer, reset.  "Frame begin" is k_frame_begin (mesh_cnt_frame_begin); "batch" is k_bat_reset
+// (mesh_cnt_bat_reset); "chunk" is k_bat_chunk_begin.  The host copies the first IM_MC_HOST slots after every frame.
+enum : int {
+    IM_MC_VERTICES = 0,        // vertices: the id base of the frame's new ones; += IM_MC_NEW_VERTICES at frame / chunk end; never reset
+    IM_MC_TRIS_ALLOC = 1,      // triangle records allocated (tri_add); never reset
+    IM_MC_TRIS_LIVE = 2,       // live triangles (tri_add / tri_remove); never reset
+    IM_MC_ERR = 3,             // IM_MERR_* flags, or-ed by every stage; never reset
+    IM_MC_VOXELS = 4,          // mesh voxels created (cand_init); never reset
+    IM_MC_ACT = 5,             // activated voxels of the frame (cand_init); frame begin
+    IM_MC_WORK_FRONT = 6,      // front end of the two-ended work list (voxel_enqueue); frame begin, batch; batched frame end: its meshed total
+    IM_MC_ADD = 7,             // add-list entries (apply_face); frame begin, batch; batched frame end: its total
+    IM_MC_REMOVE = 8,          // remove-list entries (emit_remove, apply_remove); frame begin
+    IM_MC_UNDECIDED = 9,       // candidates left undecided by the resolve's poll cap (k_cand_resolve); frame begin, chunk
+    IM_MC_NEW_VERTICES = 10,   // vertices the frame appends (cand_commit); frame begin, chunk end; batched frame end: its total
+    IM_MC_BBOX_MIN_X = 11,     // key bounding box of the mesh voxels (cand_init), minimum x, y, z; set to +0x7fffffff at create
+    IM_MC_BBOX_MIN_Y = 12,
+    IM_MC_BBOX_MIN_Z = 13,
+    IM_MC_BBOX_MAX_X = 14,     // maximum x, y, z; set to -0x7fffffff at create
+    IM_MC_BBOX_MAX_Y = 15,
+    IM_MC_BBOX_MAX_Z = 16,
+    IM_MC_WORK_BACK = 17,      // back end of the two-ended work list (voxel_enqueue); frame begin, batch, batched frame end
+    IM_MC_RESOLVE_TICKET = 18, // block ticket of k_cand_resolve; frame begin, chunk
+    IM_MC_TRI_TICKET = 19,     // voxel ticket of k_voxel_tri_warp; frame begin, batch
+    IM_MC_STAT_GATHERED = 20,  // work statistics (voxel_dilate, triangulation): kNN candidates gathered, kNN queries, dilated
+    IM_MC_STAT_QUERIES = 21,   //   vertices, facets produced; frame begin
+    IM_MC_STAT_DILATED = 22,
+    IM_MC_STAT_FACETS = 23,
+    IM_MC_DILATE_TICKET = 24,  // item ticket of k_voxel_dilate; frame begin, batch
+    IM_MC_FACES = 25,          // entries of FrameBuf::all_faces (triangulation); frame begin, batch
+    IM_MC_VREFS = 26,          // entries of FrameBuf::all_vref (voxel_dilate); frame begin, batch
+    IM_MC_VERT_CHUNKS = 27,    // vertex chunks allocated (cand_commit); never reset
+    IM_MC_PULLED = 28,         // entries of FrameBuf::pulled (pull_vertex); frame begin, batch
+    IM_MC_DITEMS = 29,         // dilation items (voxel_enqueue); frame begin, batch
+    IM_MC_X_FACES = 30,        // sharded frame: entries of FrameBuf::x_face, x_rem, x_smooth (emit_face, emit_remove, emit_smooth); frame begin
+    IM_MC_X_REMS = 31,
+    IM_MC_X_SMOOTHS = 32,
+    IM_MC_BAT_VERTICES = 33,   // batched frame: its new vertices (chunk end), add entries and meshed voxels (batch end), set to
+    IM_MC_BAT_ADD = 34,        //   zero with IM_MC_BAT_SELECTED when the batched frame starts
+    IM_MC_BAT_MESHED = 35,
+    IM_MC_BAT_SELECTED = 36,   // batched frame: voxels its activation rule meshes (k_bat_select)
+    IM_MC_HOST = 32,           // slots the host copies back: [0, IM_MC_HOST)
+    IM_MC_ALLOC = 64,          // ints allocated
+};
+// every slot the host reads from its copy (counts, work_stats, capacity, snapshot, growth, the frame's error flags)
+static_assert(IM_MC_VERTICES < IM_MC_HOST && IM_MC_TRIS_ALLOC < IM_MC_HOST && IM_MC_TRIS_LIVE < IM_MC_HOST && IM_MC_ERR < IM_MC_HOST &&
+              IM_MC_VOXELS < IM_MC_HOST && IM_MC_ACT < IM_MC_HOST && IM_MC_WORK_FRONT < IM_MC_HOST && IM_MC_ADD < IM_MC_HOST &&
+              IM_MC_REMOVE < IM_MC_HOST && IM_MC_NEW_VERTICES < IM_MC_HOST && IM_MC_WORK_BACK < IM_MC_HOST &&
+              IM_MC_STAT_GATHERED < IM_MC_HOST && IM_MC_STAT_QUERIES < IM_MC_HOST && IM_MC_STAT_DILATED < IM_MC_HOST &&
+              IM_MC_STAT_FACETS < IM_MC_HOST && IM_MC_VERT_CHUNKS < IM_MC_HOST, "a slot the host reads lies outside its copy");
+static_assert(IM_MC_BAT_SELECTED < IM_MC_ALLOC, "mesh counter block too small");
+
+// ---- the counter bookkeeping of the frame stages (one thread of the kernels in mesh_capi.cu; the host emulation of the tests)
+IM_HD void mesh_cnt_init(int* c) {   // create: c holds IM_MC_HOST zeros
+    c[IM_MC_BBOX_MIN_X] = c[IM_MC_BBOX_MIN_Y] = c[IM_MC_BBOX_MIN_Z] = 0x7fffffff;
+    c[IM_MC_BBOX_MAX_X] = c[IM_MC_BBOX_MAX_Y] = c[IM_MC_BBOX_MAX_Z] = -0x7fffffff;
+}
+IM_HD void mesh_cnt_frame_begin(const MeshDev& M) {
+    M.cnt[IM_MC_ACT] = 0; M.cnt[IM_MC_WORK_FRONT] = 0; M.cnt[IM_MC_ADD] = 0; M.cnt[IM_MC_REMOVE] = 0; M.cnt[IM_MC_UNDECIDED] = 0;
+    M.cnt[IM_MC_NEW_VERTICES] = 0; M.cnt[IM_MC_WORK_BACK] = 0; M.cnt[IM_MC_RESOLVE_TICKET] = 0; M.cnt[IM_MC_TRI_TICKET] = 0;
+    M.cnt[IM_MC_STAT_GATHERED] = 0; M.cnt[IM_MC_STAT_QUERIES] = 0; M.cnt[IM_MC_STAT_DILATED] = 0; M.cnt[IM_MC_STAT_FACETS] = 0;
+    M.cnt[IM_MC_DILATE_TICKET] = 0; M.cnt[IM_MC_FACES] = 0; M.cnt[IM_MC_VREFS] = 0; M.cnt[IM_MC_PULLED] = 0; M.cnt[IM_MC_DITEMS] = 0;
+    M.cnt[IM_MC_X_FACES] = 0; M.cnt[IM_MC_X_REMS] = 0; M.cnt[IM_MC_X_SMOOTHS] = 0;
+}
+IM_HD void mesh_cnt_frame_end(const MeshDev& M) { M.cnt[IM_MC_VERTICES] += M.cnt[IM_MC_NEW_VERTICES]; }
+// batched frame: the start of an append chunk after the first, its end (the chunk's vertices are in the map before the next chunk
+// is examined), the per-batch lists, the end of a batch, the end of the frame (the per-frame totals written back)
+IM_HD void mesh_cnt_bat_chunk_begin(const MeshDev& M) { M.cnt[IM_MC_UNDECIDED] = 0; M.cnt[IM_MC_RESOLVE_TICKET] = 0; }
+IM_HD void mesh_cnt_bat_chunk_end(const MeshDev& M) {
+    M.cnt[IM_MC_VERTICES] += M.cnt[IM_MC_NEW_VERTICES];
+    M.cnt[IM_MC_BAT_VERTICES] += M.cnt[IM_MC_NEW_VERTICES];
+    M.cnt[IM_MC_NEW_VERTICES] = 0;
+}
+IM_HD void mesh_cnt_bat_reset(const MeshDev& M) {
+    M.cnt[IM_MC_WORK_FRONT] = 0; M.cnt[IM_MC_ADD] = 0; M.cnt[IM_MC_WORK_BACK] = 0; M.cnt[IM_MC_TRI_TICKET] = 0;
+    M.cnt[IM_MC_DILATE_TICKET] = 0; M.cnt[IM_MC_FACES] = 0; M.cnt[IM_MC_VREFS] = 0; M.cnt[IM_MC_PULLED] = 0; M.cnt[IM_MC_DITEMS] = 0;
+}
+IM_HD void mesh_cnt_bat_batch_end(const MeshDev& M) {
+    M.cnt[IM_MC_BAT_ADD] += M.cnt[IM_MC_ADD];
+    M.cnt[IM_MC_BAT_MESHED] += M.cnt[IM_MC_WORK_FRONT] + M.cnt[IM_MC_WORK_BACK];
+}
+IM_HD void mesh_cnt_bat_frame_end(const MeshDev& M) {
+    M.cnt[IM_MC_NEW_VERTICES] = M.cnt[IM_MC_BAT_VERTICES];
+    M.cnt[IM_MC_ADD] = M.cnt[IM_MC_BAT_ADD];
+    M.cnt[IM_MC_WORK_FRONT] = M.cnt[IM_MC_BAT_MESHED];
+    M.cnt[IM_MC_WORK_BACK] = 0;
+}
 
 struct FramePose {        // per-frame sensor position (device resident so that a frame can be queued behind the localization)
     double pose_t[3];
@@ -163,10 +248,10 @@ struct FrameBuf {
     // exchange lists (all-gathered, then applied by every rank to its replica of the store) instead of being applied
     int shard_rank, shard_n;
     int x_cap;            // capacity of each exchange list (entries)
-    XSmooth* x_smooth;    // smoothed positions written by this rank's dilations      (count: cnt[32])
-    int4* x_face;         // new facets (a, b, c, -) of this rank's voxels             (count: cnt[30])
+    XSmooth* x_smooth;    // smoothed positions written by this rank's dilations
+    int4* x_face;         // new facets (a, b, c, -) of this rank's voxels
     unsigned long long* x_word;   // their flip-priority words
-    int4* x_rem;          // triangles (a, b, c, -) this rank's voxels want removed    (count: cnt[31])
+    int4* x_rem;          // triangles (a, b, c, -) this rank's voxels want removed
     // batched frame (immesh_mesh_push_frame_batched: one frame's per-voxel stage in several batches); null on the per-frame path
     const int* work_rank; // [max_work] flip priority of the work voxel: its rank among the frame's meshed voxels in (x, y, z) key order
     unsigned char* tri_mark;   // [max_t] IM_TRI_BORN: made live by an earlier batch of this frame; IM_TRI_REMOVE: removal deferred to the frame's end
@@ -287,23 +372,23 @@ IM_HDN inline void cand_init(const MeshDev& M, const MeshParams& P, const FrameB
     F.cand_vslot[c] = -1;
     F.cand_nconf[c] = 0;
     F.cand_next[c] = -1;
-    if (!ikey_ok(gx, gy, gz) || !ikey_ok(bx, by, bz)) { im_atomic_or(&M.cnt[3], IM_MERR_KEY_RANGE); return; }
+    if (!ikey_ok(gx, gy, gz) || !ikey_ok(bx, by, bz)) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_KEY_RANGE); return; }
     const unsigned long long gkey = pack_ikey(gx, gy, gz);
     F.cand_gkey[c] = gkey;
     // voxel get-or-create (:482-495); every examined point activates its voxel, accepted or not
     int created = 0;
     const int vs = table_insert(M.vkeys, M.vmask, pack_ikey(bx, by, bz), &created);
-    if (vs < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); return; }
+    if (vs < 0) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); return; }
     IM_STAMP(55, vs);
     if (created) {
-        im_atomic_add(&M.cnt[4], 1);
-        im_atomic_min(&M.cnt[11], bx); im_atomic_min(&M.cnt[12], by); im_atomic_min(&M.cnt[13], bz);
-        im_atomic_max(&M.cnt[14], bx); im_atomic_max(&M.cnt[15], by); im_atomic_max(&M.cnt[16], bz);
+        im_atomic_add(&M.cnt[IM_MC_VOXELS], 1);
+        im_atomic_min(&M.cnt[IM_MC_BBOX_MIN_X], bx); im_atomic_min(&M.cnt[IM_MC_BBOX_MIN_Y], by); im_atomic_min(&M.cnt[IM_MC_BBOX_MIN_Z], bz);
+        im_atomic_max(&M.cnt[IM_MC_BBOX_MAX_X], bx); im_atomic_max(&M.cnt[IM_MC_BBOX_MAX_Y], by); im_atomic_max(&M.cnt[IM_MC_BBOX_MAX_Z], bz);
     }
     F.cand_vslot[c] = vs;
     if (im_atomic_exch(&M.vox_frame[vs], F.frame) != F.frame) {
-        const int a = im_atomic_add(&M.cnt[5], 1);
-        if (a < F.max_act) F.act[a] = vs; else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        const int a = im_atomic_add(&M.cnt[IM_MC_ACT], 1);
+        if (a < F.max_act) F.act[a] = vs; else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
     }
     IM_STAMP(56, 0);
     // occupied xi-cell (:473-481)
@@ -345,7 +430,7 @@ IM_HDN inline void cand_init(const MeshDev& M, const MeshParams& P, const FrameB
     F.cand_status[c] = CAND_UNDECIDED;
     int cc = 0;
     const int cs = table_insert(F.ckeys, F.cmask, gkey, &cc);
-    if (cs < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); F.cand_status[c] = CAND_REJECT; return; }
+    if (cs < 0) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); F.cand_status[c] = CAND_REJECT; return; }
     // push onto the cell's candidate list
 #if defined(__CUDA_ARCH__)
     // The lists are only walked by the kernels after this one, so the moment in which the head already names c while c's link is not
@@ -428,7 +513,7 @@ IM_HDN inline bool cand_poll(const MeshDev& M, const MeshParams& P, const FrameB
 IM_HDN inline void cand_commit(const MeshDev& M, const MeshParams& P, const FrameBuf& F, int c, int base) {
     if (F.cand_status[c] != CAND_ACCEPT) return;
     const int id = base + F.cand_scan[c];
-    if (id >= M.max_v) { im_atomic_or(&M.cnt[3], IM_MERR_VERT_POOL); return; }
+    if (id >= M.max_v) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VERT_POOL); return; }
     const float* p = F.pts + (size_t)c * F.step * 3;
     M.vpos[id] = make_float4(p[0], p[1], p[2], 0.f);
     M.vsmooth[(size_t)id * 3 + 0] = (double)p[0];
@@ -438,20 +523,20 @@ IM_HDN inline void cand_commit(const MeshDev& M, const MeshParams& P, const Fram
     M.v_tri_head[id] = -1;
     int created = 0;
     const int gs = table_insert(M.gkeys, M.gmask, F.cand_gkey[c], &created);
-    if (gs < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); return; }
+    if (gs < 0) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); return; }
     M.gval[gs] = id;
     const int vs = F.cand_vslot[c];
     const int pos = im_atomic_add(&M.vox_count[vs], 1);
     F.cand_pos[c] = pos;
-    if (pos >= IM_VCHUNKS * 16) { im_atomic_or(&M.cnt[3], IM_MERR_VOXEL_CAP); F.cand_pos[c] = -1; }
+    if (pos >= IM_VCHUNKS * 16) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VOXEL_CAP); F.cand_pos[c] = -1; }
     else if ((pos & 15) == 0) {   // first vertex of a chunk: allocate it (published for the placement kernel that follows)
-        const int ch = im_atomic_add(&M.cnt[27], 1);
-        if (ch >= M.max_vchunks) { im_atomic_or(&M.cnt[3], IM_MERR_VERT_POOL); F.cand_pos[c] = -1; }
+        const int ch = im_atomic_add(&M.cnt[IM_MC_VERT_CHUNKS], 1);
+        if (ch >= M.max_vchunks) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VERT_POOL); F.cand_pos[c] = -1; }
         else M.vox_chunk[(size_t)vs * IM_VCHUNKS + (pos >> 4)] = ch;
     }
     im_atomic_add(&M.vox_new_added[vs], 1);
     M.vox_meshing_times[vs] = 0;
-    im_atomic_add(&M.cnt[10], 1);
+    im_atomic_add(&M.cnt[IM_MC_NEW_VERTICES], 1);
 }
 
 // chunk id of a voxel's chunk table entry for the readers: an entry left at -1 by a chunk-pool overflow (the frame fails with
@@ -485,18 +570,18 @@ IM_HD bool voxel_activate(const MeshDev& M, const FrameBuf& F, int vs) {
 // voxel vs -> work list + dilation items; returns its work slot (-1: the work list is full)
 IM_HDN inline int voxel_enqueue(const MeshDev& M, const FrameBuf& F, int vs) {
     // two-ended work list: populous voxels (the expensive ones) from the front, the rest from the back, so that the
-    // per-voxel stages start the long jobs first (cnt[6] = front count, cnt[17] = back count)
+    // per-voxel stages start the long jobs first (IM_MC_WORK_FRONT counts from the front, IM_MC_WORK_BACK from the back)
     int w;
-    if (M.vox_count[vs] >= 20) w = im_atomic_add(&M.cnt[6], 1);
-    else w = F.max_work - 1 - im_atomic_add(&M.cnt[17], 1);
-    if (w >= 0 && w < F.max_work && M.cnt[6] + M.cnt[17] <= F.max_work) F.work[w] = vs; else { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return -1; }
+    if (M.vox_count[vs] >= 20) w = im_atomic_add(&M.cnt[IM_MC_WORK_FRONT], 1);
+    else w = F.max_work - 1 - im_atomic_add(&M.cnt[IM_MC_WORK_BACK], 1);
+    if (w >= 0 && w < F.max_work && M.cnt[IM_MC_WORK_FRONT] + M.cnt[IM_MC_WORK_BACK] <= F.max_work) F.work[w] = vs; else { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP); return -1; }
     // dilation items: groups of up to 8 of the voxel's vertices (the kNN queries), so that a populous voxel is spread over
     // several thread blocks instead of serialising on one
     int nq = M.vox_count[vs];
     if (nq > IM_MAXIN) nq = IM_MAXIN;
     const int ng = (nq + 7) >> 3;
-    const int base = im_atomic_add(&M.cnt[29], ng);
-    if (base + ng > F.max_ditem) { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); return w; }
+    const int base = im_atomic_add(&M.cnt[IM_MC_DITEMS], ng);
+    if (base + ng > F.max_ditem) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP); return w; }
     for (int g = 0; g < ng; ++g) F.ditem[base + g] = (w << 5) | g;
     return w;
 }
@@ -514,17 +599,17 @@ IM_HD unsigned long long voxel_prio(const MeshDev& M, const FrameBuf& F, int w, 
     int kx, ky, kz;
     unpack_ikey(M.vkeys[F.work[w]], &kx, &ky, &kz);
     const long long lx = kx - F.fp->prio_origin[0], ly = ky - F.fp->prio_origin[1], lz = kz - F.fp->prio_origin[2];
-    if (report && (lx < 0 || lx >= 2048 || ly < 0 || ly >= 2048 || lz < 0 || lz >= 2048)) im_atomic_or(&M.cnt[3], IM_MERR_PRIO_RANGE);
+    if (report && (lx < 0 || lx >= 2048 || ly < 0 || ly >= 2048 || lz < 0 || lz >= 2048)) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_PRIO_RANGE);
     return ((unsigned long long)(lx & 2047) << 22) | ((unsigned long long)(ly & 2047) << 11) | (unsigned long long)(lz & 2047);
 }
 
-// i-th work item (0 <= i < cnt[6] + cnt[17]) -> slot in the two-ended work arrays
+// i-th work item (0 <= i < IM_MC_WORK_FRONT + IM_MC_WORK_BACK entries) -> slot in the two-ended work arrays
 IM_HD int work_slot(const MeshDev& M, const FrameBuf& F, int i) {
-    const int na = M.cnt[6];
+    const int na = M.cnt[IM_MC_WORK_FRONT];
     return i < na ? i : F.max_work - 1 - (i - na);
 }
 IM_HD int work_total(const MeshDev& M, const FrameBuf& F) {
-    const int t = M.cnt[6] + M.cnt[17];
+    const int t = M.cnt[IM_MC_WORK_FRONT] + M.cnt[IM_MC_WORK_BACK];
     return t < F.max_work ? t : F.max_work;
 }
 
@@ -733,8 +818,8 @@ IM_HDN inline int tri_add(const MeshDev& M, int a, int b, int c, unsigned long l
         int cur = im_vload(&M.thash[s]);
         if (cur < 0) {
             if (mine < 0) {
-                mine = im_atomic_add(&M.cnt[1], 1);
-                if (mine >= M.max_t) { im_atomic_or(&M.cnt[3], IM_MERR_TRI_POOL); return -1; }
+                mine = im_atomic_add(&M.cnt[IM_MC_TRIS_ALLOC], 1);
+                if (mine >= M.max_t) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_TRI_POOL); return -1; }
                 M.tri[mine] = make_int4(a, b, c, 0);
                 M.tri_flip[mine] = 0ull;
                 M.tri_next[(size_t)mine * 3 + 0] = -1; M.tri_next[(size_t)mine * 3 + 1] = -1; M.tri_next[(size_t)mine * 3 + 2] = -1;
@@ -747,7 +832,7 @@ IM_HDN inline int tri_add(const MeshDev& M, int a, int b, int c, unsigned long l
         if (r.x == a && r.y == b && r.z == c) { t = cur; break; }
         s = (s + 1) & M.tmask;
     }
-    if (t < 0) { im_atomic_or(&M.cnt[3], IM_MERR_HASH_FULL); return -1; }
+    if (t < 0) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); return -1; }
     if (t == mine) {
         const int vs[3] = {a, b, c};
 #if defined(__CUDA_ARCH__)
@@ -766,12 +851,12 @@ IM_HDN inline int tri_add(const MeshDev& M, int a, int b, int c, unsigned long l
 #endif
     }
     // (a record allocated by a thread that lost the publication race stays unused: a leaked slot, never linked)
-    if (im_atomic_exch(&M.tri[t].w, 1) == 0) im_atomic_add(&M.cnt[2], 1);
+    if (im_atomic_exch(&M.tri[t].w, 1) == 0) im_atomic_add(&M.cnt[IM_MC_TRIS_LIVE], 1);
     im_atomic_max64(&M.tri_flip[t], flipword);
     return t;
 }
 IM_HD void tri_remove(const MeshDev& M, int t) {  // erase_triangle, triangle.hpp:164-210
-    if (im_atomic_exch(&M.tri[t].w, 0) == 1) im_atomic_add(&M.cnt[2], -1);
+    if (im_atomic_exch(&M.tri[t].w, 0) == 1) im_atomic_add(&M.cnt[IM_MC_TRIS_LIVE], -1);
 }
 
 // ------------------------------------------------------------------ smoothed positions and the viewer's region sets

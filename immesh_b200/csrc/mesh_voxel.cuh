@@ -49,20 +49,20 @@ IM_HD void apply_face(const MeshDev& M, const FrameBuf& F, int a, int b, int c, 
     if (t >= 0 && M.tri[t].w && tri_pre_frame(F, t)) {
         im_atomic_max64(&M.tri_flip[t], word);
     } else {
-        const int e = im_atomic_add(&M.cnt[7], 1);
+        const int e = im_atomic_add(&M.cnt[IM_MC_ADD], 1);
         if (e < F.max_list) {
             F.add_tri[(size_t)e * 3 + 0] = a; F.add_tri[(size_t)e * 3 + 1] = b; F.add_tri[(size_t)e * 3 + 2] = c;
             F.add_flip[e] = word;
         } else {
-            im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+            im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
         }
     }
 }
 IM_HD void emit_face(const MeshDev& M, const FrameBuf& F, int a, int b, int c, unsigned long long word) {
     if (F.shard_n > 1) {
-        const int e = im_atomic_add(&M.cnt[30], 1);
+        const int e = im_atomic_add(&M.cnt[IM_MC_X_FACES], 1);
         if (e < F.x_cap) { F.x_face[e] = make_int4(a, b, c, 0); F.x_word[e] = word; }
-        else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
         return;
     }
     apply_face(M, F, a, b, c, word);
@@ -70,30 +70,30 @@ IM_HD void emit_face(const MeshDev& M, const FrameBuf& F, int a, int b, int c, u
 IM_HD void emit_remove(const MeshDev& M, const FrameBuf& F, int t) {
     if (F.shard_n > 1) {
         const int4 tr = M.tri[t];
-        const int e = im_atomic_add(&M.cnt[31], 1);
-        if (e < F.x_cap) F.x_rem[e] = make_int4(tr.x, tr.y, tr.z, 0); else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        const int e = im_atomic_add(&M.cnt[IM_MC_X_REMS], 1);
+        if (e < F.x_cap) F.x_rem[e] = make_int4(tr.x, tr.y, tr.z, 0); else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
         return;
     }
     if (F.tri_mark) {   // batched frame: counted now, removed after the last batch (only pre-frame triangles are pulled)
-        im_atomic_add(&M.cnt[8], 1);
+        im_atomic_add(&M.cnt[IM_MC_REMOVE], 1);
         F.tri_mark[t] = IM_TRI_REMOVE;
         return;
     }
-    const int e = im_atomic_add(&M.cnt[8], 1);
-    if (e < F.max_list) F.rem_tri[e] = t; else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+    const int e = im_atomic_add(&M.cnt[IM_MC_REMOVE], 1);
+    if (e < F.max_list) F.rem_tri[e] = t; else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
 }
 IM_HD void apply_remove(const MeshDev& M, const FrameBuf& F, int a, int b, int c) {
     const int t = tri_find(M, a, b, c);
     if (t < 0 || !M.tri[t].w) return;
-    const int e = im_atomic_add(&M.cnt[8], 1);
-    if (e < F.max_list) F.rem_tri[e] = t; else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+    const int e = im_atomic_add(&M.cnt[IM_MC_REMOVE], 1);
+    if (e < F.max_list) F.rem_tri[e] = t; else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
 }
 IM_HD void emit_smooth(const MeshDev& M, const FrameBuf& F, int v, double x, double y, double z) {
     store_smooth(M, v, x, y, z);
     if (F.shard_n > 1) {
-        const int e = im_atomic_add(&M.cnt[32], 1);
+        const int e = im_atomic_add(&M.cnt[IM_MC_X_SMOOTHS], 1);
         if (e < F.x_cap) { XSmooth r; r.id = v; r.pad = 0; r.x = x; r.y = y; r.z = z; F.x_smooth[e] = r; }
-        else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
     }
 }
 
@@ -416,7 +416,7 @@ IM_HDN inline void voxel_dilate(const MeshDev& M, const MeshParams& P, const Fra
             }
         if (tid == 0) {
             im_atomic_max(&F.work_ring[w], ring_used);
-            if (S->overflow) im_atomic_or(&M.cnt[3], IM_MERR_VOXEL_CAP);
+            if (S->overflow) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VOXEL_CAP);
         }
     }
     im_fence();
@@ -463,23 +463,23 @@ IM_HDN inline void voxel_dilate(const MeshDev& M, const MeshParams& P, const Fra
         }
     for (int i = tid; i < n; i += nthreads) F.work_ids[(size_t)w * IM_MAXD + i] = S->ids[i];
     // frame-wide list of (voxel, dilated vertex) references for the flat pull stage
-    if (tid == 0) S->need_more = (n >= 3) ? im_atomic_add(&M.cnt[26], n) : -1;
+    if (tid == 0) S->need_more = (n >= 3) ? im_atomic_add(&M.cnt[IM_MC_VREFS], n) : -1;
     IM_SYNCBLOCK_M();
     {
         const int voff = S->need_more;
         if (voff >= 0) {
-            if (voff + n > F.max_vref) { if (tid == 0) im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); }
+            if (voff + n > F.max_vref) { if (tid == 0) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP); }
             else for (int i = tid; i < n; i += nthreads) F.all_vref[voff + i] = (w << 10) | i;
         }
     }
     if (tid == 0) {
         F.work_nfaces[w] = 0;
         F.work_n_ids[w] = n;
-        if (S->overflow) im_atomic_or(&M.cnt[3], IM_MERR_VOXEL_CAP);
+        if (S->overflow) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VOXEL_CAP);
         // work accounting for the roofline (DESIGN.md): gathered candidates, queries, dilated vertices
-        im_atomic_add(&M.cnt[20], S->n_cand);
-        im_atomic_add(&M.cnt[21], nqt);
-        im_atomic_add(&M.cnt[22], n);
+        im_atomic_add(&M.cnt[IM_MC_STAT_GATHERED], S->n_cand);
+        im_atomic_add(&M.cnt[IM_MC_STAT_QUERIES], nqt);
+        im_atomic_add(&M.cnt[IM_MC_STAT_DILATED], n);
     }
 }
 
@@ -611,7 +611,7 @@ IM_HDN inline void voxel_mesh(const MeshDev& M, const MeshParams& P, const Frame
     if (S->scratch[4] == 0) return;  // all points collinear: T.number_of_faces() == 0 (mesh_rec_geometry.cpp:257-260)
     if (S->scratch[6]) {   // cavity capacity exceeded
         if (store_only) { if (tid == 0) { F.work_nfaces[w] = -1; F.work_n_ids[w] = -n; } }
-        else if (tid == 0) im_atomic_or(&M.cnt[3], IM_MERR_VOXEL_CAP);
+        else if (tid == 0) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_VOXEL_CAP);
         return;
     }
     // finite faces passing the 150-degree filter (is_face_is_ok), as sorted global id triples
@@ -636,16 +636,16 @@ IM_HDN inline void voxel_mesh(const MeshDev& M, const MeshParams& P, const Frame
     }
     IM_SYNCBLOCK_M();
     const int nf = S->nface;
-    if (tid == 0) im_atomic_add(&M.cnt[23], nf);
+    if (tid == 0) im_atomic_add(&M.cnt[IM_MC_STAT_FACETS], nf);
     if (store_only) {
         // fused dilate+triangulate kernel: the facets and the voxel's principal axes go to global memory; commit / orientation
         // run in a later kernel, once the smoothed positions of ALL voxels of the frame are final
         // compact frame-wide lists (arbitrary order): facets (a,b,c,w) and vertex references (w,i)
-        if (tid == 0) S->scratch[0] = im_atomic_add(&M.cnt[25], nf);
+        if (tid == 0) S->scratch[0] = im_atomic_add(&M.cnt[IM_MC_FACES], nf);
         IM_SYNCBLOCK_M();
         const int foff = S->scratch[0];
         if (foff + nf > F.max_list) {
-            if (tid == 0) im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+            if (tid == 0) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
         } else {
             for (int k = tid; k < nf; k += nthreads) F.all_faces[foff + k] = make_int4(S->faces[k][0], S->faces[k][1], S->faces[k][2], w);
         }
@@ -931,13 +931,13 @@ IM_HDN inline void voxel_mesh_warp(const MeshDev& M, const MeshParams& P, const 
     IM_STAMP_IF(blockIdx.x == 0 && threadIdx.x == 0, 37, nf);
     // facets + principal axes to the frame-wide lists; commit / orientation / pull run in the flat stage-C kernels
     if (lane == 0) {
-        im_atomic_add(&M.cnt[23], nf);
-        S->scratch[0] = im_atomic_add(&M.cnt[25], nf);
+        im_atomic_add(&M.cnt[IM_MC_STAT_FACETS], nf);
+        S->scratch[0] = im_atomic_add(&M.cnt[IM_MC_FACES], nf);
     }
     IM_SYNCWARP();
     const int foff = S->scratch[0];
     if (foff + nf > F.max_list) {
-        if (lane == 0) im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+        if (lane == 0) im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
     } else {
         for (int k = lane; k < nf; k += nlanes) F.all_faces[foff + k] = make_int4(faces[k][0], faces[k][1], faces[k][2], w);
     }
@@ -963,7 +963,7 @@ IM_HDN inline void commit_face(const MeshDev& M, const MeshParams& P, const Fram
     // bounded probe: a full set is a capacity error, never a spin
     unsigned int hs = (tri_hash(fc.x, fc.y, fc.z) + (unsigned int)w * 0x9E3779B1u) & F.fset_mask;
     for (unsigned int probe = 0;; ++probe) {
-        if (probe > F.fset_mask) { im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP); break; }
+        if (probe > F.fset_mask) { im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP); break; }
         if (im_atomic_cas32(&F.fset[hs], -1, f) == -1) break;
         hs = (hs + 1) & F.fset_mask;
     }
@@ -997,9 +997,9 @@ IM_HDN inline void pull_vertex(const MeshDev& M, const MeshParams& P, const Fram
                 in_set = hit;
             }
             if (in_set) {
-                const int e = im_atomic_add(&M.cnt[28], 1);
+                const int e = im_atomic_add(&M.cnt[IM_MC_PULLED], 1);
                 if (e < F.max_list) { F.pulled[2 * (size_t)e] = w; F.pulled[2 * (size_t)e + 1] = t; }
-                else im_atomic_or(&M.cnt[3], IM_MERR_LIST_CAP);
+                else im_atomic_or(&M.cnt[IM_MC_ERR], IM_MERR_LIST_CAP);
             }
         }
         t = nx;

@@ -10,8 +10,8 @@
 // (grow_point).  No output of the library depends on it: the map dump and the plane markers are ordered by root key, and the
 // match and update walks reach a root through its key.
 #pragma once
+#include "lio_core.cuh"
 #include "mesh_core.cuh"
-#include "voxelmap.cuh"
 
 namespace immesh {
 
@@ -44,7 +44,7 @@ IM_HD void rehash_xi_slot(const MeshDev& from, const MeshDev& to, unsigned int s
     if (key == IM_EMPTY_KEY) return;
     int created = 0;
     const int ns = table_insert(to.gkeys, to.gmask, key, &created);
-    if (ns < 0) { im_atomic_or(&to.cnt[3], IM_MERR_HASH_FULL); return; }
+    if (ns < 0) { im_atomic_or(&to.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); return; }
     to.gval[ns] = from.gval[s];
 }
 // mesh-voxel hash: the slot IS the voxel id, so every per-voxel array row moves with its key
@@ -53,7 +53,7 @@ IM_HD void rehash_voxel_slot(const MeshDev& from, const MeshDev& to, unsigned in
     if (key == IM_EMPTY_KEY) return;
     int created = 0;
     const int ns = table_insert(to.vkeys, to.vmask, key, &created);
-    if (ns < 0) { im_atomic_or(&to.cnt[3], IM_MERR_HASH_FULL); return; }
+    if (ns < 0) { im_atomic_or(&to.cnt[IM_MC_ERR], IM_MERR_HASH_FULL); return; }
     for (int k = 0; k < IM_VCHUNKS; ++k) to.vox_chunk[(size_t)ns * IM_VCHUNKS + k] = from.vox_chunk[(size_t)s * IM_VCHUNKS + k];
     to.vox_count[ns] = from.vox_count[s];
     to.vox_meshing_times[ns] = from.vox_meshing_times[s];
@@ -71,11 +71,11 @@ IM_HD void rehash_tri_slot(const MeshDev& from, const MeshDev& to, unsigned int 
         if (im_atomic_cas32(&to.thash[p], -1, t) < 0) return;
         p = (p + 1) & to.tmask;
     }
-    im_atomic_or(&to.cnt[3], IM_MERR_HASH_FULL);
+    im_atomic_or(&to.cnt[IM_MC_ERR], IM_MERR_HASH_FULL);
 }
 
 // Automatic growth (immesh_lio_set_growth): the capacities the next `steps` steps need (the steps still in flight and the one
-// being queued), each of at most n_max points, from the counters c (d_counters layout) of the last step known to have finished.
+// being queued), each of at most n_max points, from the counters c (IM_LC_* slots) of the last step known to have finished.
 // *cap, *nodes, *chunks hold the current capacities on entry; a pool is doubled until
 //   root hash : load factor <= 1/2 after the steps, each adding at most n_max roots (one per point at most: a sound bound)
 //   nodes     : free >= max(capacity / 4, steps x max(2 x the largest per-step use seen, n_max))
@@ -84,21 +84,21 @@ IM_HD void rehash_tri_slot(const MeshDev& from, const MeshDev& to, unsigned int 
 // returns IMMESH_E_CAPACITY as it does without growth.
 inline void growth_targets(const int* c, long long steps, long long n_max, int max_step_nodes, int max_step_chunks, long long* cap,
                            long long* nodes, long long* chunks) {
-    while ((c[5] + steps * n_max) * 2 > *cap) *cap *= 2;
+    while ((c[IM_LC_ROOTS] + steps * n_max) * 2 > *cap) *cap *= 2;
     const long long per_node = 2LL * max_step_nodes > n_max ? 2LL * max_step_nodes : n_max;
     const long long per_chunk = 2LL * max_step_chunks > n_max ? 2LL * max_step_chunks : n_max;
-    const long long used_chunks = (long long)c[1] - (c[2] > 0 ? c[2] : 0);
+    const long long used_chunks = (long long)c[IM_LC_CHUNK_BUMP] - (c[IM_LC_AVAIL_TOP] > 0 ? c[IM_LC_AVAIL_TOP] : 0);
     auto need = [&](long long capacity, long long used, long long per) {
         const long long q = capacity / 4;
         return capacity - used < (q > steps * per ? q : steps * per);
     };
-    while (need(*nodes, c[0], per_node)) *nodes *= 2;
+    while (need(*nodes, c[IM_LC_NODES], per_node)) *nodes *= 2;
     while (need(*chunks, used_chunks, per_chunk)) *chunks *= 2;
 }
 
 // Automatic growth of the mesh handle (immesh_mesh_set_growth), the same scheme before a frame of at most m candidates: a frame
 // appends at most m vertices, xi-cells, mesh voxels and vertex chunks (one per candidate at most: sound bounds); its facets are
-// bounded by twice the largest per-frame use seen, and by 8 m (neither is sound).  c: the mesh counters (MeshDev::cnt layout) of the last frame known to have
+// bounded by twice the largest per-frame use seen, and by 8 m (neither is sound).  c: the mesh counters (IM_MC_* slots) of the last frame known to have
 // finished; *vertices, *triangles, *voxels hold the current capacities on entry and are doubled until
 //   vertices, voxels : free >= max(capacity / 4, steps x m), for the vertices and for the vertex chunks that come with them   (the xi-grid and the voxel hash keep a load factor <= 1/2: they are
 //                      sized at twice these capacities)
@@ -110,9 +110,9 @@ inline void mesh_growth_targets(const int* c, long long steps, long long m, int 
         return capacity - used < (q > steps * per ? q : steps * per);
     };
     const long long per_tri = 2LL * max_step_tris > 8 * m ? 2LL * max_step_tris : 8 * m;
-    while (need(*vertices, c[0], m) || need(*vertices / 4 + 1024, c[27], m)) *vertices *= 2;   // vertex chunks: max_v / 4 + 1024
-    while (need(*voxels, c[4], m)) *voxels *= 2;
-    while (need(*triangles, c[1], per_tri)) *triangles *= 2;
+    while (need(*vertices, c[IM_MC_VERTICES], m) || need(*vertices / 4 + 1024, c[IM_MC_VERT_CHUNKS], m)) *vertices *= 2;   // vertex chunks: max_v / 4 + 1024
+    while (need(*voxels, c[IM_MC_VOXELS], m)) *voxels *= 2;
+    while (need(*triangles, c[IM_MC_TRIS_ALLOC], per_tri)) *triangles *= 2;
 }
 
 }  // namespace immesh

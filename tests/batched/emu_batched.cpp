@@ -21,9 +21,6 @@ struct BatchState {
 };
 std::unordered_map<immesh_mesh*, BatchState*> g_batch;
 
-void batch_reset(MeshDev& M) {   // per-batch lists: work, dilation items, facets, vertex refs, pulls, add list
-    for (int k : {6, 7, 17, 19, 24, 25, 26, 28, 29}) M.cnt[k] = 0;
-}
 void batch_fill(immesh_mesh* h, const FrameBuf& F, std::vector<int>& rank, const std::vector<int>& sel, size_t lo, size_t hi) {
     for (size_t r = lo; r < hi; ++r) {
         const int w = voxel_enqueue(h->M, F, sel[r]);
@@ -51,7 +48,7 @@ int immesh_mesh_destroy(immesh_mesh_t* h) {
 }
 // the flags and smoothed positions of the vertices (test access)
 int emu_mesh_smooth_state(immesh_mesh_t* h, unsigned char* flags, double* smooth) {
-    const int nv = h->M.cnt[0];
+    const int nv = h->M.cnt[IM_MC_VERTICES];
     if (flags) std::memcpy(flags, h->M.vsmoothed, (size_t)nv);
     if (smooth) std::memcpy(smooth, h->M.vsmooth, (size_t)nv * 3 * sizeof(double));
     return nv;
@@ -83,9 +80,8 @@ int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* xyz, int64_t n
     F.frame = ++h->frame_counter;
     for (int j = 0; j < 3; ++j) { h->fp_storage.pose_t[j] = pose_t[j]; h->fp_storage.prio_origin[j] = 0; }
     F.fp = &h->fp_storage;
-    for (int k = 5; k <= 10; ++k) M.cnt[k] = 0;
-    for (int k = 17; k <= 26; ++k) M.cnt[k] = 0;
-    for (int k = 28; k <= 35; ++k) M.cnt[k] = 0;
+    mesh_cnt_frame_begin(M);
+    std::memset(M.cnt + IM_MC_BAT_VERTICES, 0, (IM_MC_BAT_SELECTED + 1 - IM_MC_BAT_VERTICES) * sizeof(int));
     // append, chunk by chunk: candidates [c B, (c + 1) B) of the frame (candidate i = point i step)
     long long chunks = 0;
     for (long long c0 = 0; c0 < m_total; c0 += B, ++chunks) {
@@ -94,40 +90,40 @@ int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* xyz, int64_t n
         F.pts = h->pts.data(); F.step = 1; F.m = m; F.n = m;
         F.cmask = (unsigned)(p2((size_t)std::max(m, 1) * 2) - 1);
         for (unsigned i = 0; i <= F.cmask; ++i) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
-        M.cnt[9] = 0; M.cnt[18] = 0;
+        mesh_cnt_bat_chunk_begin(M);
         for (int c = 0; c < m; ++c) cand_init(M, P, F, c);
         for (int c = 0; c < m; ++c) cand_conflicts(M, P, F, c);
         for (int c = 0; c < m; ++c)
             if (F.cand_status[c] == CAND_UNDECIDED && !cand_poll(M, P, F, c)) return -100;
         int run = 0;
         for (int c = 0; c < m; ++c) { F.cand_scan[c] = run; run += F.cand_status[c] == CAND_ACCEPT; }
-        const int base = M.cnt[0];
+        const int base = M.cnt[IM_MC_VERTICES];
         for (int c = 0; c < m; ++c) cand_commit(M, P, F, c, base);
         for (int c = 0; c < m; ++c) cand_place(M, F, c, base);
-        M.cnt[0] += M.cnt[10]; M.cnt[33] += M.cnt[10]; M.cnt[10] = 0;
+        mesh_cnt_bat_chunk_end(M);
     }
     // activation rule over the frame's activated voxels; the meshed ones in ascending key order (their rank = flip priority)
     std::vector<int> sel;
-    for (int a = 0; a < std::min(M.cnt[5], F.max_act); ++a)
+    for (int a = 0; a < std::min(M.cnt[IM_MC_ACT], F.max_act); ++a)
         if (voxel_activate(M, F, F.act[a])) sel.push_back(F.act[a]);
     std::sort(sel.begin(), sel.end(), [&](int a, int b) { return M.vkeys[a] < M.vkeys[b]; });
     const size_t nbat = (sel.size() + V - 1) / V;
     DilateSmem* DS = new DilateSmem();
     // pass 1: every dilation's smoothing before any orientation
     for (size_t b = 0; b < nbat; ++b) {
-        batch_reset(M);
+        mesh_cnt_bat_reset(M);
         batch_fill(h, F, S.rank, sel, b * V, std::min(sel.size(), (b + 1) * V));
-        for (int i = 0; i < std::min(M.cnt[29], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
+        for (int i = 0; i < std::min(M.cnt[IM_MC_DITEMS], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
     }
     // pass 2: dilation lists again (the re-stored smoothing writes the same bits), triangulation, pull + commit, this batch's additions
     MeshSmem<256>* S1 = new MeshSmem<256>();
     MeshSmem<1024>* S2 = new MeshSmem<1024>();
     MeshWarpSmem<128>* SW = new MeshWarpSmem<128>();
     for (size_t b = 0; b < nbat; ++b) {
-        batch_reset(M);
+        mesh_cnt_bat_reset(M);
         for (unsigned i = 0; i <= F.fset_mask; ++i) F.fset[i] = -1;
         batch_fill(h, F, S.rank, sel, b * V, std::min(sel.size(), (b + 1) * V));
-        for (int i = 0; i < std::min(M.cnt[29], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
+        for (int i = 0; i < std::min(M.cnt[IM_MC_DITEMS], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
         const int nw = work_total(M, F);
         for (int i = 0; i < nw; ++i) voxel_mesh_warp<128>(M, P, F, work_slot(M, F, i), SW, 0, 1, 96);
         for (int i = 0; i < nw; ++i) {
@@ -135,35 +131,35 @@ int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* xyz, int64_t n
             const int nd = F.work_n_ids[w];
             if (nd > 96 && nd <= 256) voxel_mesh<256>(M, P, F, w, S1, 0, 1, 1);
         }
-        for (int f = 0; f < std::min(M.cnt[25], F.max_list); ++f) commit_face(M, P, F, f);
-        for (int r = 0; r < std::min(M.cnt[26], F.max_vref); ++r) pull_vertex(M, P, F, r);
-        for (int e = 0; e < std::min(M.cnt[28], F.max_list); ++e) pull_check(M, F, e);
+        for (int f = 0; f < std::min(M.cnt[IM_MC_FACES], F.max_list); ++f) commit_face(M, P, F, f);
+        for (int r = 0; r < std::min(M.cnt[IM_MC_VREFS], F.max_vref); ++r) pull_vertex(M, P, F, r);
+        for (int e = 0; e < std::min(M.cnt[IM_MC_PULLED], F.max_list); ++e) pull_check(M, F, e);
         for (int i = 0; i < nw; ++i) {
             const int w = work_slot(M, F, i);
             const int nd = F.work_n_ids[w];
             if (nd < 0 || nd > 256) voxel_mesh<1024>(M, P, F, w, S2, 0, 1);
         }
-        const int nadd = std::min(M.cnt[7], F.max_list);
+        const int nadd = std::min(M.cnt[IM_MC_ADD], F.max_list);
         for (int e = 0; e < nadd; ++e) {
             const int t = tri_add(M, F.add_tri[(size_t)e * 3], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
             if (t >= 0) F.tri_mark[t] = IM_TRI_BORN;
         }
-        M.cnt[34] += M.cnt[7]; M.cnt[35] += M.cnt[6] + M.cnt[17];
+        mesh_cnt_bat_batch_end(M);
     }
     delete DS; delete S1; delete S2; delete SW;
     // deferred removals; marks cleared for the next frame
-    for (int t = 0; t < std::min(M.cnt[1], M.max_t); ++t) {
+    for (int t = 0; t < std::min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t); ++t) {
         if (F.tri_mark[t] == IM_TRI_REMOVE) tri_remove(M, t);
         F.tri_mark[t] = 0;
     }
-    M.cnt[10] = M.cnt[33]; M.cnt[7] = M.cnt[34]; M.cnt[6] = M.cnt[35]; M.cnt[17] = 0;
-    std::memcpy(h->last_cnt, M.cnt, 32 * sizeof(int));
+    mesh_cnt_bat_frame_end(M);
+    std::memcpy(h->last_cnt, M.cnt, sizeof(h->last_cnt));
     if (stats) {
         stats[0] = chunks; stats[1] = (int64_t)nbat;
         stats[2] = (int64_t)(S.act.size() * 4 + S.rank.size() * 4 + S.mark.size() + S.fset.size() * 4);
-        stats[3] = M.cnt[7];
+        stats[3] = M.cnt[IM_MC_ADD];
     }
-    if (M.cnt[3] & ~(IM_MERR_KEY_RANGE | IM_MERR_PRIO_RANGE)) return IMMESH_E_CAPACITY;
-    return M.cnt[3] ? IMMESH_E_RANGE : 0;
+    if (M.cnt[IM_MC_ERR] & ~(IM_MERR_KEY_RANGE | IM_MERR_PRIO_RANGE)) return IMMESH_E_CAPACITY;
+    return M.cnt[IM_MC_ERR] ? IMMESH_E_RANGE : 0;
 }
 }  // extern "C"

@@ -26,7 +26,7 @@ struct immesh_lio {
     std::vector<float> body, pw;
     std::vector<double> body_cov, p_imu, bv_imu, var, sortkey;
     std::vector<int> match_node, match_layer, slot, seg, seg2, slot_count, slot_offset, slot_cursor, touched;
-    int counters[16];
+    int counters[IM_LC_SIZE];
     int max_scan;
     std::vector<unsigned int> bits;   // sharded mode: [exists words | ok words]
 };
@@ -70,10 +70,10 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     std::memset(h->counters, 0, sizeof(h->counters));
     VoxelMapDev& m = h->map;
     m.keys = h->keys.data(); m.root_node = h->root_node.data(); m.cap_mask = (unsigned)(cap - 1);
-    m.nodes = h->nodes.data(); m.planes = h->planes.data(); m.node_count = &h->counters[0]; m.max_nodes = max_nodes;
-    m.chunks = h->chunks.data(); m.chunk_bump = &h->counters[1]; m.max_chunks = max_chunks;
-    m.avail = h->avail.data(); m.avail_top = &h->counters[2]; m.pending = h->pending.data(); m.pending_n = &h->counters[3];
-    m.err = &h->counters[4]; m.n_roots = &h->counters[5]; m.stat = nullptr;
+    m.nodes = h->nodes.data(); m.planes = h->planes.data(); m.node_count = &h->counters[IM_LC_NODES]; m.max_nodes = max_nodes;
+    m.chunks = h->chunks.data(); m.chunk_bump = &h->counters[IM_LC_CHUNK_BUMP]; m.max_chunks = max_chunks;
+    m.avail = h->avail.data(); m.avail_top = &h->counters[IM_LC_AVAIL_TOP]; m.pending = h->pending.data(); m.pending_n = &h->counters[IM_LC_PENDING];
+    m.err = &h->counters[IM_LC_ERR]; m.n_roots = &h->counters[IM_LC_ROOTS]; m.stat = nullptr;
     const int ms = h->max_scan;
     h->body.resize((size_t)ms * 3); h->pw.resize((size_t)ms * 3);
     h->body_cov.resize((size_t)ms * 6); h->p_imu.resize((size_t)ms * 3); h->bv_imu.resize((size_t)ms * 6); h->var.resize((size_t)ms * 6); h->sortkey.resize(ms);
@@ -85,7 +85,7 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     sb.match_node = h->match_node.data(); sb.match_layer = h->match_layer.data(); sb.pw = h->pw.data(); sb.var = h->var.data();
     sb.sortkey = h->sortkey.data(); sb.slot = h->slot.data(); sb.seg = h->seg.data();
     sb.slot_count = h->slot_count.data(); sb.slot_offset = h->slot_offset.data(); sb.slot_cursor = h->slot_cursor.data();
-    sb.touched = h->touched.data(); sb.n_touched = &h->counters[6]; sb.seg_top = &h->counters[7];
+    sb.touched = h->touched.data(); sb.n_touched = &h->counters[IM_LC_TOUCHED]; sb.seg_top = &h->counters[IM_LC_SEG_TOP];
     std::memset(&h->ctrl, 0, sizeof(LioCtrl));
     double* s = h->ctrl.state;
     s[0] = s[4] = s[8] = 1.0;
@@ -316,7 +316,7 @@ int64_t immesh_voxelmap_dump(immesh_lio_t* h, double* rows, int64_t cap_rows) {
     return dump_voxelmap(h->keys.data(), h->root_node.data(), h->keys.size(), h->nodes.data(), h->planes.data(), rows, cap_rows);
 }
 int immesh_voxelmap_counts(immesh_lio_t* h, int64_t* out) {
-    out[0] = h->counters[5]; out[1] = h->counters[0]; out[2] = h->counters[1]; out[3] = h->counters[4];
+    out[0] = h->counters[IM_LC_ROOTS]; out[1] = h->counters[IM_LC_NODES]; out[2] = h->counters[IM_LC_CHUNK_BUMP]; out[3] = h->counters[IM_LC_ERR];
     return 0;
 }
 }

@@ -32,7 +32,7 @@ struct immesh_mesh {
     FramePose fp_storage;
     int nw = 0;
     int frame_counter = 0;
-    int last_cnt[32];
+    int last_cnt[IM_MC_HOST];
 };
 static size_t p2(size_t v) { size_t p = 1; while (p < v) p <<= 1; return p; }
 
@@ -51,8 +51,8 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     h->gkeys.assign(gcap, IM_EMPTY_KEY); h->gval.assign(gcap, -1);
     h->vkeys.assign(vcap, IM_EMPTY_KEY); h->vox_chunk.assign(vcap * IM_VCHUNKS, -1); h->vox_count.assign(vcap, 0); h->vox_mt.assign(vcap, 0); h->vox_na.assign(vcap, 0); h->vox_frame.assign(vcap, -1);
     h->tri.resize(max_t); h->tri_next.resize((size_t)max_t * 3); h->tri_flip.resize(max_t); h->thash.assign(tcap, -1);
-    h->cnt.assign(64, 0);
-    h->cnt[11] = h->cnt[12] = h->cnt[13] = 0x7fffffff; h->cnt[14] = h->cnt[15] = h->cnt[16] = -0x7fffffff;
+    h->cnt.assign(IM_MC_ALLOC, 0);
+    mesh_cnt_init(h->cnt.data());
     M.vpos = h->vpos.data(); M.vsmooth = h->vsmooth.data(); M.v_tri_head = h->v_tri_head.data();
     M.gkeys = h->gkeys.data(); M.gval = h->gval.data(); M.gmask = (unsigned)(gcap - 1);
     M.vkeys = h->vkeys.data(); M.vmask = (unsigned)(vcap - 1); M.vox_chunk = h->vox_chunk.data(); M.vox_count = h->vox_count.data(); M.max_vchunks = max_v / 4 + 1024; h->vchunk_pts.resize((size_t)M.max_vchunks * 16); M.vchunk_pts = h->vchunk_pts.data();
@@ -93,11 +93,7 @@ int emu_mesh_phase_a(immesh_mesh_t* h, const float* world_xyz, int n, const doub
     F.cmask = (unsigned)(p2((size_t)std::max(F.m, 1) * 2) - 1);
     if (n > 0) std::memcpy(h->pts.data(), world_xyz, (size_t)n * 12);
     for (unsigned i = 0; i <= F.cmask; ++i) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
-    for (int k = 5; k <= 10; ++k) M.cnt[k] = 0;
-    for (int k = 17; k <= 26; ++k) M.cnt[k] = 0;
-    M.cnt[28] = 0;
-    M.cnt[29] = 0;
-    M.cnt[30] = 0; M.cnt[31] = 0; M.cnt[32] = 0;
+    mesh_cnt_frame_begin(M);
     for (unsigned i = 0; i <= F.fset_mask; ++i) F.fset[i] = -1;
     for (int c = 0; c < F.m; ++c) cand_init(M, P, F, c);
     for (int c = 0; c < F.m; ++c) cand_conflicts(M, P, F, c);
@@ -105,14 +101,14 @@ int emu_mesh_phase_a(immesh_mesh_t* h, const float* world_xyz, int n, const doub
         if (F.cand_status[c] == CAND_UNDECIDED && !cand_poll(M, P, F, c)) return -100;
     int run = 0;
     for (int c = 0; c < F.m; ++c) { F.cand_scan[c] = run; run += F.cand_status[c] == CAND_ACCEPT; }
-    const int base = M.cnt[0];
+    const int base = M.cnt[IM_MC_VERTICES];
     for (int c = 0; c < F.m; ++c) cand_commit(M, P, F, c, base);
     for (int c = 0; c < F.m; ++c) cand_place(M, F, c, base);
-    const int na = std::min(M.cnt[5], F.max_act);
+    const int na = std::min(M.cnt[IM_MC_ACT], F.max_act);
     for (int a = 0; a < na; ++a) voxel_select(M, F, a);
     h->nw = work_total(M, F);
     DilateSmem* DS = new DilateSmem();
-    for (int i = 0; i < std::min(M.cnt[29], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
+    for (int i = 0; i < std::min(M.cnt[IM_MC_DITEMS], F.max_ditem); ++i) voxel_dilate(M, P, F, F.ditem[i], DS, 0, 1);
     delete DS;
     return 0;
 }
@@ -132,9 +128,9 @@ int emu_mesh_phase_b(immesh_mesh_t* h) {
         const int nd = F.work_n_ids[w];
         if (nd > 96 && nd <= 256) voxel_mesh<256>(M, P, F, w, S1, 0, 1, 1);
     }
-    for (int f = 0; f < std::min(M.cnt[25], F.max_list); ++f) commit_face(M, P, F, f);
-    for (int r = 0; r < std::min(M.cnt[26], F.max_vref); ++r) pull_vertex(M, P, F, r);
-    for (int e = 0; e < std::min(M.cnt[28], F.max_list); ++e) pull_check(M, F, e);
+    for (int f = 0; f < std::min(M.cnt[IM_MC_FACES], F.max_list); ++f) commit_face(M, P, F, f);
+    for (int r = 0; r < std::min(M.cnt[IM_MC_VREFS], F.max_vref); ++r) pull_vertex(M, P, F, r);
+    for (int e = 0; e < std::min(M.cnt[IM_MC_PULLED], F.max_list); ++e) pull_check(M, F, e);
     for (int i = 0; i < nw; ++i) {
         const int w = work_slot(M, F, i);
         const int nd = F.work_n_ids[w];
@@ -147,12 +143,12 @@ int emu_mesh_phase_b(immesh_mesh_t* h) {
 int emu_mesh_phase_c(immesh_mesh_t* h) {
     FrameBuf& F = h->F;
     MeshDev& M = h->M;
-    const int nr = std::min(M.cnt[8], F.max_list), nadd = std::min(M.cnt[7], F.max_list);
+    const int nr = std::min(M.cnt[IM_MC_REMOVE], F.max_list), nadd = std::min(M.cnt[IM_MC_ADD], F.max_list);
     for (int e = 0; e < nr; ++e) tri_remove(M, F.rem_tri[e]);
     for (int e = 0; e < nadd; ++e) tri_add(M, F.add_tri[(size_t)e * 3], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
-    M.cnt[0] += M.cnt[10];
-    std::memcpy(h->last_cnt, M.cnt, 32 * sizeof(int));
-    return M.cnt[3] ? IMMESH_E_CAPACITY : 0;
+    mesh_cnt_frame_end(M);
+    std::memcpy(h->last_cnt, M.cnt, sizeof(h->last_cnt));
+    return M.cnt[IM_MC_ERR] ? IMMESH_E_CAPACITY : 0;
 }
 int immesh_mesh_push_frame(immesh_mesh_t* h, const float* world_xyz, int n, const double* pose_t, int) {
     int rc = emu_mesh_phase_a(h, world_xyz, n, pose_t);
@@ -169,7 +165,7 @@ int emu_mesh_set_shard(immesh_mesh_t* h, int rank, int nranks) {
     return 0;
 }
 int emu_mesh_xcounts(immesh_mesh_t* h, int* out) {   // smooth, face, remove
-    out[0] = std::min(h->M.cnt[32], h->F.x_cap); out[1] = std::min(h->M.cnt[30], h->F.x_cap); out[2] = std::min(h->M.cnt[31], h->F.x_cap);
+    out[0] = std::min(h->M.cnt[IM_MC_X_SMOOTHS], h->F.x_cap); out[1] = std::min(h->M.cnt[IM_MC_X_FACES], h->F.x_cap); out[2] = std::min(h->M.cnt[IM_MC_X_REMS], h->F.x_cap);
     return 0;
 }
 int emu_mesh_xget(immesh_mesh_t* h, void* smooth32, int* face4, unsigned long long* word, int* rem4) {
@@ -191,7 +187,7 @@ int emu_mesh_xapply_lists(immesh_mesh_t* h, const int* face4, const unsigned lon
     for (int i = 0; i < nr; ++i) apply_remove(h->M, h->F, rem4[i * 4], rem4[i * 4 + 1], rem4[i * 4 + 2]);
     return 0;
 }
-int emu_mesh_error_word(immesh_mesh_t* h) { return h->last_cnt[3]; }   // IM_MERR_* flags of the last frame
+int emu_mesh_error_word(immesh_mesh_t* h) { return h->last_cnt[IM_MC_ERR]; }   // IM_MERR_* flags of the last frame
 // keys (x, y, z) of the voxels the last frame meshed (its work list, in work-list order); returns their number
 int emu_mesh_frame_voxels(immesh_mesh_t* h, int32_t* keys) {
     const int nw = work_total(h->M, h->F);
@@ -204,12 +200,13 @@ int emu_mesh_frame_voxels(immesh_mesh_t* h, int32_t* keys) {
 }
 int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
     const int* c = h->last_cnt;
-    out[0] = c[0]; out[1] = c[2]; out[2] = c[10]; out[3] = c[6] + c[17]; out[4] = c[7]; out[5] = c[8]; out[6] = c[4]; out[7] = c[5];
+    out[0] = c[IM_MC_VERTICES]; out[1] = c[IM_MC_TRIS_LIVE]; out[2] = c[IM_MC_NEW_VERTICES]; out[3] = c[IM_MC_WORK_FRONT] + c[IM_MC_WORK_BACK];
+    out[4] = c[IM_MC_ADD]; out[5] = c[IM_MC_REMOVE]; out[6] = c[IM_MC_VOXELS]; out[7] = c[IM_MC_ACT];
     return 0;
 }
 int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, int32_t* flips) {
     const MeshDev& M = h->M;
-    const int nv = M.cnt[0], nalloc = M.cnt[1];
+    const int nv = M.cnt[IM_MC_VERTICES], nalloc = M.cnt[IM_MC_TRIS_ALLOC];
     if (vertices)
         for (int i = 0; i < nv; ++i) { vertices[i * 3] = M.vpos[i].x; vertices[i * 3 + 1] = M.vpos[i].y; vertices[i * 3 + 2] = M.vpos[i].z; }
     std::vector<std::array<int, 4>> rows;

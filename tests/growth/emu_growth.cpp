@@ -32,7 +32,7 @@ void rebuild_roots(const VoxelMapDev& m, VoxelMapDev& nm, size_t cap0, std::vect
 }
 struct GrowState {
     int64_t max_bytes = 0;
-    int known[16] = {};
+    int known[IM_LC_SIZE] = {};
     int max_step_nodes = 0, max_step_chunks = 0;
 };
 std::unordered_map<immesh_lio*, GrowState> g_grow;
@@ -49,8 +49,8 @@ static int growth_check(immesh_lio* h, long long n) {
     if (it == g_grow.end() || it->second.max_bytes <= 0) return 0;
     GrowState& g = it->second;
     const int* c = h->counters;
-    g.max_step_nodes = std::max(g.max_step_nodes, c[0] - g.known[0]);
-    g.max_step_chunks = std::max(g.max_step_chunks, c[1] - g.known[1]);
+    g.max_step_nodes = std::max(g.max_step_nodes, c[IM_LC_NODES] - g.known[IM_LC_NODES]);
+    g.max_step_chunks = std::max(g.max_step_chunks, c[IM_LC_CHUNK_BUMP] - g.known[IM_LC_CHUNK_BUMP]);
     std::memcpy(g.known, c, sizeof(g.known));
     long long cap = (long long)h->keys.size(), nodes = (long long)h->nodes.size(), chunks = (long long)h->chunks.size();
     growth_targets(g.known, 1, n, g.max_step_nodes, g.max_step_chunks, &cap, &nodes, &chunks);
@@ -100,9 +100,9 @@ int immesh_lio_reserve(immesh_lio_t* h, int64_t root_slots, int64_t nodes, int64
 }
 int immesh_lio_capacity(immesh_lio_t* h, int64_t* out) {
     const int* c = h->counters;
-    out[0] = (int64_t)h->keys.size(); out[1] = c[5];
-    out[2] = (int64_t)h->nodes.size(); out[3] = c[0];
-    out[4] = (int64_t)h->chunks.size(); out[5] = (int64_t)c[1] - std::max(c[2], 0);
+    out[0] = (int64_t)h->keys.size(); out[1] = c[IM_LC_ROOTS];
+    out[2] = (int64_t)h->nodes.size(); out[3] = c[IM_LC_NODES];
+    out[4] = (int64_t)h->chunks.size(); out[5] = (int64_t)c[IM_LC_CHUNK_BUMP] - std::max(c[IM_LC_AVAIL_TOP], 0);
     out[6] = 0; out[7] = g_growths;
     return 0;
 }
@@ -128,13 +128,13 @@ int emu_hash_home(unsigned long long key, int log2_cap) { return (int)(hash_key(
 int emu_rehash_check(const unsigned long long* keys, const int* marks, int n, int log2_old, int log2_new, int* out_slot, int* out_root,
                      int* out_mark, int* out_node_slot, int* out_list, int* list_key) {
     const size_t cap0 = (size_t)1 << log2_old, cap = (size_t)1 << log2_new;
-    int counters[16] = {};
+    int counters[IM_LC_SIZE] = {};
     std::vector<unsigned long long> k0(cap0, IM_EMPTY_KEY), k1(cap, IM_EMPTY_KEY);
     std::vector<int> r0(cap0, -1), m0(cap0, 0), l0(cap0, 0), r1(cap, -1), m1(cap, 0), l1(cap, 0), slot_map;
     std::vector<NodeRec> nodes(n > 0 ? n : 1);
     VoxelMapDev m{};
     m.keys = k0.data(); m.root_node = r0.data(); m.cap_mask = (unsigned)(cap0 - 1); m.nodes = nodes.data(); m.max_nodes = n;
-    m.err = &counters[4]; m.pub_mark = m0.data(); m.pub_list = l0.data(); m.pub_n = &counters[12];
+    m.err = &counters[IM_LC_ERR]; m.pub_mark = m0.data(); m.pub_list = l0.data(); m.pub_n = &counters[IM_LC_PUB_N];
     for (int i = 0; i < n; ++i) {
         int created = 0;
         const int s = hash_insert(m, keys[i], &created);
@@ -147,7 +147,7 @@ int emu_rehash_check(const unsigned long long* keys, const int* marks, int n, in
     VoxelMapDev nm = m;
     nm.keys = k1.data(); nm.root_node = r1.data(); nm.pub_mark = m1.data(); nm.pub_list = l1.data(); nm.cap_mask = (unsigned)(cap - 1);
     rebuild_roots(m, nm, cap0, slot_map, n, l0.data(), *m.pub_n);
-    if (counters[4]) return -2;
+    if (counters[IM_LC_ERR]) return -2;
     for (int i = 0; i < n; ++i) {
         const int s = hash_find(nm, keys[i]);
         out_slot[i] = s;
@@ -165,7 +165,7 @@ int emu_rehash_check(const unsigned long long* keys, const int* marks, int n, in
 // not map to their old index (0 when the rebuild is right); -1 when the set-up overflowed.
 int emu_mesh_rehash_check(const unsigned long long* vkeys, int n, const int* tris, int nt, int log2_old, int log2_new) {
     const size_t c0 = (size_t)1 << log2_old, c1 = (size_t)1 << log2_new;
-    std::vector<int> cnt(64, 0);
+    std::vector<int> cnt(IM_MC_ALLOC, 0);
     std::vector<unsigned long long> k0(c0, IM_EMPTY_KEY), k1(c1, IM_EMPTY_KEY);
     std::vector<int> ch0(c0 * IM_VCHUNKS, -1), ch1(c1 * IM_VCHUNKS, -1), r0[4], r1[4];
     for (int a = 0; a < 4; ++a) { r0[a].assign(c0, 0); r1[a].assign(c1, 0); }
@@ -195,7 +195,7 @@ int emu_mesh_rehash_check(const unsigned long long* vkeys, int n, const int* tri
     nm.thash = th1.data(); nm.tmask = (unsigned)(c1 - 1);
     for (unsigned s : visit_order(c0)) rehash_voxel_slot(m, nm, s);
     for (unsigned s : visit_order(c0)) rehash_tri_slot(m, nm, s);
-    if (cnt[3]) return -1;
+    if (cnt[IM_MC_ERR]) return -1;
     int bad = 0;
     for (int i = 0; i < n; ++i) {
         const int s = table_find(nm.vkeys, nm.vmask, vkeys[i]);

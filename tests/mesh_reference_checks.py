@@ -6,10 +6,10 @@ from it with its own voxel counters and its own smoothed positions, so a decisio
 
 Compared after every frame:
 * the vertices (positions and ids): exact;
-* the counts of immesh_mesh_counts (mesh_capi.cu), exact: n_vertices (vertex counter, cnt[0]), frame_new_vertices (this frame's
-  appends, cnt[10]), n_voxels (mesh voxels ever created, cnt[4]: a voxel is created by every examined point, appended or not),
-  n_activated (distinct voxels of this frame's examined points, cnt[5]), frame_voxels_meshed (work-list length cnt[6] + cnt[17]:
-  activated voxels that passed the meshing-times test and hold at least 3 points);
+* the counts of immesh_mesh_counts (mesh_capi.cu), exact: n_vertices (vertex counter, IM_MC_VERTICES), frame_new_vertices (this
+  frame's appends, IM_MC_NEW_VERTICES), n_voxels (mesh voxels ever created, IM_MC_VOXELS: a voxel is created by every examined point,
+  appended or not), n_activated (distinct voxels of this frame's examined points, IM_MC_ACT), frame_voxels_meshed (work-list length
+  IM_MC_WORK_FRONT + IM_MC_WORK_BACK: activated voxels that passed the meshing-times test and hold at least 3 points);
 * the set of meshed voxels (where the implementation exposes it: the emulation's work list): exact;
 * the live facet set and the flips: exact outside the exclusions below.
 

@@ -24,10 +24,10 @@ void emu_knn(const MeshDev& M, const MeshParams& P, const float* q, int k, doubl
     const double max_d2 = max_dist * max_dist;
     std::vector<std::pair<float, int>> best;
     int far = -1;
-    if (M.cnt[4] > 0) {
-        far = std::max(std::abs(cx - M.cnt[11]), std::abs(cx - M.cnt[14]));
-        far = std::max(far, std::max(std::abs(cy - M.cnt[12]), std::abs(cy - M.cnt[15])));
-        far = std::max(far, std::max(std::abs(cz - M.cnt[13]), std::abs(cz - M.cnt[16])));
+    if (M.cnt[IM_MC_VOXELS] > 0) {
+        far = std::max(std::abs(cx - M.cnt[IM_MC_BBOX_MIN_X]), std::abs(cx - M.cnt[IM_MC_BBOX_MAX_X]));
+        far = std::max(far, std::max(std::abs(cy - M.cnt[IM_MC_BBOX_MIN_Y]), std::abs(cy - M.cnt[IM_MC_BBOX_MAX_Y])));
+        far = std::max(far, std::max(std::abs(cz - M.cnt[IM_MC_BBOX_MIN_Z]), std::abs(cz - M.cnt[IM_MC_BBOX_MAX_Z])));
     }
     for (int ring = 0; ring <= far; ++ring) {
         if (ring >= 1) {
@@ -97,14 +97,14 @@ int emu_mesh_xapply_smooth(immesh_mesh_t* h, const void* smooth32, int n) {
 }
 // the flags and smoothed positions of the first n vertices (test access)
 int emu_mesh_smooth_state(immesh_mesh_t* h, unsigned char* flags, double* smooth) {
-    const int nv = h->M.cnt[0];
+    const int nv = h->M.cnt[IM_MC_VERTICES];
     if (flags) std::memcpy(flags, h->M.vsmoothed, (size_t)nv);
     if (smooth) std::memcpy(smooth, h->M.vsmooth, (size_t)nv * 3 * sizeof(double));
     return nv;
 }
 int immesh_mesh_smooth_all(immesh_mesh_t* h, double smooth_factor, int knn, double* smoothed) {
     if (!h || knn < 1 || knn > 32) return IMMESH_E_INVALID;
-    const int nv = h->M.cnt[0];
+    const int nv = h->M.cnt[IM_MC_VERTICES];
     std::vector<int> all((size_t)nv);
     for (int v = 0; v < nv; ++v) all[v] = v;
     emu_smooth_list(h, all, knn, smooth_factor);
@@ -130,7 +130,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     // k_rb_select + the radix sort's result: (region word, i, j, k) ascending
     struct Kept { unsigned long long word; int a, b, c, slot; };
     std::vector<Kept> kept;
-    const int nalloc = std::min(M.cnt[1], M.max_t);
+    const int nalloc = std::min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t);
     for (int t = 0; t < nalloc; ++t) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
@@ -176,7 +176,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     *n_regions = nr;
     if (n > cap || nr > cap_regions) return IMMESH_E_CAPACITY;
     // k_rb_claim + k_knn + k_rb_smooth
-    std::vector<unsigned char> claimed((size_t)M.cnt[0], 0);
+    std::vector<unsigned char> claimed((size_t)M.cnt[IM_MC_VERTICES], 0);
     std::vector<int> list;
     for (const Kept& e : kept)
         for (int v : {e.a, e.b, e.c})

@@ -135,8 +135,8 @@ def _targets(lib, fn, c, steps, n, *rest, caps):
 
 
 def test_growth_policy_with_steps_in_flight(lib):
-    # localization: c[5] roots, c[0] nodes, c[1] chunk bump, c[2] free-list top; every result is the least doubling that satisfies
-    # the documented rule, for one step and for the five a full pipeline can hold
+    # localization, counters by slot (lio_core.cuh): 5 IM_LC_ROOTS, 0 IM_LC_NODES, 1 IM_LC_CHUNK_BUMP, 2 IM_LC_AVAIL_TOP (free-list
+    # top); every result is the least doubling that satisfies the documented rule, for one step and for the five a full pipeline can hold
     c = {5: 3000, 0: 3100, 1: 4000, 2: 200}
     for steps in (1, 2, 5):
         cap, nodes, chunks = _targets(lib, "emu_growth_targets", c, steps, 1000, 700, 900, caps=[1024, 4096, 4096])
@@ -145,7 +145,7 @@ def test_growth_policy_with_steps_in_flight(lib):
             assert capac - used >= max(capac // 4, steps * per)
             half = capac // 2
             assert capac == 4096 or half - used < max(half // 4, steps * per)
-    # the mesh: c[0] vertices, c[27] vertex chunks, c[4] voxels, c[1] triangles
+    # the mesh, counters by slot (mesh_core.cuh): 0 IM_MC_VERTICES, 27 IM_MC_VERT_CHUNKS, 4 IM_MC_VOXELS, 1 IM_MC_TRIS_ALLOC
     c = {0: 5000, 27: 2000, 4: 1500, 1: 20000}
     for steps in (1, 3):
         v, t, x = _targets(lib, "emu_mesh_growth_targets", c, steps, 800, 9000, caps=[6000, 21000, 2000])
