@@ -151,6 +151,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_reinforce_enable", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int]),
         ("immesh_mesh_reinforce_pose", [vp, dp, dp]),
         ("immesh_mesh_reinforced_cloud", [vp, fp, fp, C.POINTER(C.c_int32), C.c_int, ip, dp]),
+        ("immesh_mesh_changes_enable", [vp, C.c_int64, C.c_int]),
+        ("immesh_mesh_changes", [vp, C.c_int64, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int32), C.c_int64, fp, C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
         ("immesh_mesh_push_frame_batched", [vp, vp, C.c_int64, C.c_int, dp, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud_batched", [vp, vp, vp, C.c_int64, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
@@ -659,6 +661,39 @@ class Mesh:
         _check(self.lib, self.lib.immesh_mesh_reinforced_cloud(self._h, depth.ctypes.data_as(C.POINTER(C.c_float)), pts.ctypes.data_as(C.POINTER(C.c_float)),
                                                                pix.ctypes.data_as(C.POINTER(C.c_int32)), n.value, C.byref(n), pose.ctypes.data_as(dp)), "mesh_reinforced_cloud")
         return depth, pts[:n.value].copy(), pix[:n.value].copy(), pose[:9].reshape(3, 3).copy(), pose[9:].copy()
+
+    def changes_enable(self, max_rows=1 << 20, max_frames=256):
+        """Record every later frame's triangle changes on the device: a ring of max_rows rows, the headers of the last max_frames frames.
+        The published state starts as the mesh is now (snapshot())."""
+        _check(self.lib, self.lib.immesh_mesh_changes_enable(self._h, max_rows, max_frames), "mesh_changes_enable")
+
+    def changes_disable(self):
+        _check(self.lib, self.lib.immesh_mesh_changes_enable(self._h, 0, 0), "mesh_changes_enable")
+
+    def changes_newest(self) -> int:
+        """the newest frame queued with the change feed on (where a mirror resynchronised by snapshot() reads on from)"""
+        counts = np.zeros(4, dtype=np.int64)
+        rc = self.lib.immesh_mesh_changes(self._h, -1, None, 0, None, 0, None, 0, counts.ctypes.data_as(C.POINTER(C.c_int64)))
+        if rc != -5:   # before the enable: IMMESH_E_RANGE with counts[3] = newest
+            _check(self.lib, rc, "mesh_changes")
+        return int(counts[3])
+
+    def changes(self, since: int):
+        """The frames (since, newest] of the change feed: dict(frames int64[n][4] = frame, v_begin, v_end, rows_end; rows int32[m][4] =
+        a, b, c, code (0 removed, 2 | flip added, 4 | flip re-oriented), ascending triples inside a frame; vertices float32[k][3] of the
+        ids [frames[0, 1], frames[-1, 2]); newest).  RuntimeError with code -5 (IMMESH_E_RANGE) when a frame is no longer held."""
+        counts = np.zeros(4, dtype=np.int64)
+        cp = counts.ctypes.data_as(C.POINTER(C.c_int64))
+        rc = self.lib.immesh_mesh_changes(self._h, since, None, 0, None, 0, None, 0, cp)
+        if rc not in (0, -3):
+            _check(self.lib, rc, "mesh_changes")
+        fr = np.zeros((int(counts[0]), 4), dtype=np.int64)
+        rows = np.zeros((int(counts[1]), 4), dtype=np.int32)
+        v = np.zeros((int(counts[2]), 3), dtype=np.float32)
+        if rc:
+            _check(self.lib, self.lib.immesh_mesh_changes(self._h, since, fr.ctypes.data_as(C.POINTER(C.c_int64)), len(fr), rows.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                          len(rows), v.ctypes.data_as(C.POINTER(C.c_float)), len(v), cp), "mesh_changes")
+        return dict(frames=fr, rows=rows, vertices=v, newest=int(counts[3]))
 
     def smooth_all(self, smooth_factor=0.1, knn=20):
         """smooth_all_pts: returns the smoothed positions float64[nv,3] (and stores them as the vertices' smoothed positions)."""

@@ -155,6 +155,16 @@ def build_reinforce(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "reinforce", "emu_reinforce.cpp"), EMU_REINFORCE, force)
 
 
+EMU_CHANGES = os.path.join(_ROOT, "tests", "changes", "libimmesh_emu_changes.so")
+
+
+def build_changes(force=False):
+    """tests/changes: the host emulation of the mesher and the batched frame with the change feed's bodies (mesh_changes.cuh) run in
+    the device's order (the localization emulation linked in unchanged)"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "changes", "emu_changes.cpp"), EMU_CHANGES, force,
+                    extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")])
+
+
 DEV_MEM_DIR = os.path.join(_ROOT, "tests", "dev_mem")
 EMU_DEV_MEM = os.path.join(DEV_MEM_DIR, "libdev_mem_emu.so")
 
@@ -187,6 +197,7 @@ def build_all(force=False):
     build_growth(force)
     build_imu_chain(force)
     build_reinforce(force)
+    build_changes(force)
     build_dev_mem(force)
     build_ref()
 

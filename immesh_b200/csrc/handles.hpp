@@ -4,6 +4,7 @@
 
 #include "common_host.hpp"
 #include "lio_core.cuh"
+#include "mesh_changes.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
 #include "reinforce.cuh"
@@ -189,4 +190,14 @@ struct immesh_mesh {
         RfImage img;                      // result buffer (frame & 1) holds the frame's image and pose
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
     } rf;
+    // change feed (immesh_mesh_changes_enable); its per-frame pointers are in F (chg_stamp, chg_list, chg_cnt, chg_cap)
+    struct Changes {
+        int on = 0;
+        int enable_frame = 0;             // frame_counter at enable: the frames after it are recorded
+        int last_frame = 0;               // newest frame queued with the feed
+        immesh::ChgDev C = {};
+        unsigned int *ku = nullptr, *vu = nullptr;   // [2][chg_cap] radix-sort ping-pong of the frame's rows
+        int* hist = nullptr;
+        immesh::MemSet dev;               // every buffer of the feed, freed by disable / destroy (not counted)
+    } chg;
 };

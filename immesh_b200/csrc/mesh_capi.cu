@@ -178,6 +178,48 @@ __global__ void __launch_bounds__(128) k_push_add(MeshDev M, FrameBuf F_) {
         tri_add(M, F.add_tri[(size_t)e * 3 + 0], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
 }
 __global__ void k_frame_end(MeshDev M) { mesh_cnt_frame_end(M); }
+// ---- the change feed (mesh_changes.cuh), queued after the push when enabled.  full: the frame lists its slots by the sweep (batched)
+__global__ void __launch_bounds__(128) k_chg_gather(MeshDev M, FrameBuf F_) {
+    const FrameBuf F = frame_load_dyn(F_);
+    const int n = chg_gather_count(M, F);
+    for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) chg_gather(M, F, e);
+}
+__global__ void __launch_bounds__(128) k_chg_sweep(MeshDev M, FrameBuf F_, ChgDev C, int full) {
+    const FrameBuf F = frame_load_dyn(F_);
+    if (!chg_sweeping(F, full)) return;
+    const int n = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t);
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) chg_sweep_slot(M, F, C, t);
+}
+__global__ void __launch_bounds__(128) k_chg_mark(MeshDev M, FrameBuf F_, ChgDev C, int full) {
+    const FrameBuf F = frame_load_dyn(F_);
+    const int n = min(chg_listed(F, full), F.chg_cap);
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) chg_row_mark(M, F, C, i);
+}
+__global__ void __launch_bounds__(1024) k_chg_rows(FrameBuf F_, ChgDev C, int full) {
+    const FrameBuf F = frame_load_dyn(F_);
+    const int n = min(chg_listed(F, full), F.chg_cap);
+    const int total = chunk_scan_1024(n, [&](int i) { return chg_row_count(C, i); }, [&](int i, int run) { return chg_row_emit(C, i, run); });
+    if (threadIdx.x == 1023) F.chg_cnt[IM_CH_ROWS] = total;
+}
+__global__ void __launch_bounds__(128) k_chg_word(const int* cnt, ChgDev C, int w, const unsigned int* vin, unsigned int* kout, unsigned int* vout) {
+    const int n = cnt[IM_CH_ROWS];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = vin ? vin[i] : (unsigned int)i;
+        kout[i] = chg_word(C, w, (int)v);
+        vout[i] = v;
+    }
+}
+__global__ void __launch_bounds__(128) k_chg_emit(FrameBuf F_, ChgDev C, const unsigned int* order, int full) {
+    const FrameBuf F = frame_load_dyn(F_);
+    if (chg_lost(F, C, full)) return;
+    const int n = F.chg_cnt[IM_CH_ROWS];
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) chg_append(C, order, i);
+}
+__global__ void k_chg_end(MeshDev M, FrameBuf F_, ChgDev C, int full, int v_after) { chg_frame_end(M, frame_load_dyn(F_), C, full, v_after); }
+// enable: the published bytes of the allocated slots from the store as it is
+__global__ void __launch_bounds__(128) k_chg_init(MeshDev M, unsigned char* pub, int n_alloc) {
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) pub[t] = chg_state(M, t);
+}
 // snapshot: compact live triangles
 __global__ void __launch_bounds__(128) k_snapshot(MeshDev M, int n_alloc, int* out_tri, int* out_flip, int* out_n) {
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
@@ -1032,6 +1074,14 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
             e = fresh.alloc(&nm.vox_frame, vcap);
         if (e == cudaSuccess && act > h->F.max_act) e = fresh.alloc(&nf.act, act);
     }
+    // the change feed's per-triangle stamp and published byte follow the triangle pool
+    immesh::MemSet cfresh;
+    int* c_stamp = h->F.chg_stamp;
+    unsigned char* c_pub = h->chg.C.pub;
+    if (gt && h->chg.on && e == cudaSuccess) {
+        pool = "triangle pool (change feed)";
+        if ((e = cfresh.alloc(&c_stamp, tris)) == cudaSuccess) e = cfresh.alloc(&c_pub, tris);
+    }
     auto fail = [&](cudaError_t err, const char* what) {
         cudaGetLastError();
         return im_fail(err == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA,
@@ -1068,6 +1118,14 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
                 MG(cudaMemcpyAsync(nm.tri_next, M.tri_next, (size_t)nt * 3 * sizeof(int), cudaMemcpyDeviceToDevice, st));
                 MG(cudaMemcpyAsync(nm.tri_flip, M.tri_flip, (size_t)nt * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
             }
+            if (c_pub != h->chg.C.pub) {
+                MG(cudaMemsetAsync(c_stamp, 0xFF, (size_t)tris * 4, st));
+                MG(cudaMemsetAsync(c_pub, 0, (size_t)tris, st));
+                if (nt > 0) {
+                    MG(cudaMemcpyAsync(c_stamp, h->F.chg_stamp, (size_t)nt * 4, cudaMemcpyDeviceToDevice, st));
+                    MG(cudaMemcpyAsync(c_pub, h->chg.C.pub, (size_t)nt, cudaMemcpyDeviceToDevice, st));
+                }
+            }
             nm.max_t = (int)tris;
             if (nm.thash != M.thash) {
                 MG(cudaMemsetAsync(nm.thash, 0xFF, tcap * 4, st));
@@ -1099,6 +1157,13 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
     for (const auto& r : replaced)
         if (r.first != r.second) h->dev.free(r.first);
     h->dev.take(std::move(fresh));
+    if (c_pub != h->chg.C.pub) {
+        h->chg.dev.free(h->F.chg_stamp);
+        h->chg.dev.free(h->chg.C.pub);
+        h->chg.dev.take(std::move(cfresh));
+        h->F.chg_stamp = c_stamp;
+        h->chg.C.pub = c_pub;
+    }
     if (h->b_fp) {   // batched-frame scratch: allocated again at the new sizes by the next batched frame
         h->batch = immesh::MemSet();
         h->b_act = h->b_sel = h->b_rank = h->b_hist = h->b_fset = nullptr;
@@ -1186,6 +1251,34 @@ static void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st) {
     rf_image_launch(h, r.img, h->d_dyn, st);
 }
 
+static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
+    int b = 0;
+    while (b < 64 && (max_value >> b)) ++b;
+    return std::max(1, (b + 7) / 8);
+}
+
+// the change feed of the frame whose push was just queued (F: its FrameBuf; batched: a batched frame, after k_bat_frame_end): the
+// touched set (the sweep when batched or overflowed), the rows against the published bytes (marked per slot, then compacted), their LSD sort by (a, b, c) over words
+// of the bits of max_v - 1, the ring append and the header.  Fixed grids: every count is read on the device.
+static void mesh_changes_launch(immesh_mesh* h, const FrameBuf& F, cudaStream_t st, bool batched) {
+    auto& c = h->chg;
+    const int full = batched ? 1 : 0, cap = F.chg_cap;
+    if (!batched) IM_LAUNCH(k_chg_gather, h->n_sm * 2, 128, 0, st, h->M, F);
+    IM_LAUNCH(k_chg_sweep, h->n_sm * 8, 128, 0, st, h->M, F, c.C, full);
+    unsigned int* ku[2] = {c.ku, c.ku + cap};
+    unsigned int* vu[2] = {c.vu, c.vu + cap};
+    const int g = mesh_grid_fixed(h, cap, 128), passes = rb_passes((unsigned long long)std::max(h->M.max_v - 1, 0));
+    IM_LAUNCH(k_chg_mark, g, 128, 0, st, h->M, F, c.C, full);
+    IM_LAUNCH(k_chg_rows, 1, 1024, 0, st, F, c.C, full);
+    int cur = 0;
+    for (int w = 0; w < 3; ++w) {
+        IM_LAUNCH(k_chg_word, g, 128, 0, st, (const int*)F.chg_cnt, c.C, w, w == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur], ku[cur ^ 1], vu[cur ^ 1]);
+        cur = rs_sort_passes(st, ku, vu, cur ^ 1, cap, passes, c.hist, F.chg_cnt + IM_CH_ROWS);
+    }
+    IM_LAUNCH(k_chg_emit, g, 128, 0, st, F, c.C, (const unsigned int*)vu[cur], full);
+    IM_LAUNCH(k_chg_end, 1, 1, 0, st, h->M, F, c.C, full, full);
+}
+
 // src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state.
 // Queues one frame (no host synchronisation except when both staging slots are still busy).  Host work per frame in the
 // pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D FrameDyn + one stream
@@ -1271,7 +1364,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         d.n = F.n; d.step = F.step; d.m = F.m; d.frame = F.frame; d.cmask = F.cmask; d.pose_idx = pose_idx; d.epoch = epoch;
         IM_CUDA(cudaMemcpyAsync(h->d_dyn, &d, sizeof(FrameDyn), cudaMemcpyHostToDevice, st));
     }
-    const bool rf_on = h->rf.on != 0;
+    const bool rf_on = h->rf.on != 0, chg_on = h->chg.on != 0;
     if (rf_on) {   // the camera source of this frame
         RfDyn* r = (RfDyn*)h->rf.h_rd + s;
         r->mode = h->rf.explicit_pose;
@@ -1330,6 +1423,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         if (timing) cudaEventRecord(h->ev[3], st);
         IM_LAUNCH(k_push_remove, h->n_sm * 2, 128, 0, st, h->M, F);
         IM_LAUNCH(k_push_add, h->n_sm * 2, 128, 0, st, h->M, F);
+        if (chg_on) mesh_changes_launch(h, F, st, false);
         IM_LAUNCH(k_frame_end, 1, 1, 0, st, h->M);
         if (rf_on) mesh_reinforce_launch(h, st);
     };
@@ -1350,6 +1444,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     h->inflight[s] = 1;
     h->timed_last = queued ? 0 : 1;
     if (rf_on) h->rf.last_frame = F.frame;
+    if (chg_on) h->chg.last_frame = F.frame;
     return IMMESH_OK;
 }
 // drain the queue; returns the status of the frames harvested since the last call
@@ -1415,6 +1510,7 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (nranks == 1) { h->F.shard_rank = 0; h->F.shard_n = 1; return IMMESH_OK; }
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a mesh handle with automatic growth cannot be sharded (immesh_mesh_set_growth(h, 0) first)");
     if (h->rf.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the reinforcement enabled cannot be sharded (immesh_mesh_reinforce_enable(h, NULL, ...) first)");
+    if (h->chg.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the change feed enabled cannot be sharded (immesh_mesh_changes_enable(h, 0, 0) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -1651,12 +1747,6 @@ int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* reg
     if (region_offsets && nr <= cap_regions) region_offsets[nr] = nlive;
     *n_regions = nr;
     return nr <= cap_regions ? IMMESH_OK : im_fail(IMMESH_E_CAPACITY, "more regions than cap_regions");
-}
-
-static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
-    int b = 0;
-    while (b < 64 && (max_value >> b)) ++b;
-    return std::max(1, (b + 7) / 8);
 }
 
 int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32_t* keys, int n_keys, double smooth_factor, int knn,
@@ -1992,6 +2082,10 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     }
     IM_LAUNCH(k_bat_sweep, h->n_sm * 8, 128, 0, st, h->M, F);
     IM_LAUNCH(k_bat_frame_end, 1, 1, 0, st, h->M);
+    if (h->chg.on) {
+        mesh_changes_launch(h, F, st, true);
+        h->chg.last_frame = F.frame;
+    }
     IM_CUDA(cudaGetLastError());
     int cnt[IM_MC_HOST];
     IM_CUDA(cudaMemcpyAsync(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
@@ -2128,6 +2222,93 @@ int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth, float* points, 
     if (points && n > 0) IM_CUDA(cudaMemcpy(points, o.pts, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
     if (point_pixel && n > 0) IM_CUDA(cudaMemcpy(point_pixel, o.pix, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
     if (pose_out) std::memcpy(pose_out, pose, sizeof(pose));
+    return IMMESH_OK;
+}
+
+int immesh_mesh_changes_enable(immesh_mesh_t* h, int64_t max_rows, int max_frames) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (max_rows < 0 || max_rows > IM_MPOOL_LIMIT || (max_rows > 0 && (max_frames < 1 || max_frames > (1 << 20))))
+        return im_fail(IMMESH_E_INVALID, "changes_enable: bad argument (0 <= max_rows <= 2^30; 1 <= max_frames <= 2^20 when max_rows > 0)");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "changes_enable: a sharded mesh handle is not supported");
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
+    h->graph.destroy();                          // the captured sequence changes
+    h->chg = immesh_mesh::Changes();             // the buffers of an earlier enable go
+    h->F.chg_stamp = nullptr; h->F.chg_list = nullptr; h->F.chg_cnt = nullptr; h->F.chg_cap = 0;
+    if (max_rows == 0) return IMMESH_OK;
+    immesh_mesh::Changes c;   // built in full before it replaces h->chg: after a failure the feed stays disabled
+    ChgDev& C = c.C;
+    C.max_rows = max_rows;
+    C.max_frames = max_frames;
+    const int cap = (int)std::min<int64_t>(max_rows, 1 << 21), max_t = h->M.max_t;   // a frame's touched slots: a bounded list
+    int *stamp = nullptr, *list = nullptr, *cnt = nullptr;
+    cudaError_t e = c.dev.alloc(&stamp, (size_t)max_t, 0xFF);
+    auto add = [&e, &c](auto** p, size_t count, int fill = -1) { if (e == cudaSuccess) e = c.dev.alloc(p, std::max<size_t>(count, 1), fill); };
+    add(&C.pub, (size_t)max_t, 0); add(&list, (size_t)cap); add(&cnt, IM_CH_SIZE, 0); add(&C.marked, (size_t)cap); add(&C.rowbuf, (size_t)cap);
+    add(&c.ku, 2 * (size_t)cap); add(&c.vu, 2 * (size_t)cap); add(&c.hist, 256 * (((size_t)cap + VG_TILE - 1) / VG_TILE));
+    add(&C.hdr, (size_t)max_frames, 0xFF); add(&C.ring, (size_t)max_rows); add(&C.written, 1, 0);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // the initialising memsets ran on the legacy stream
+    int cnt_host[IM_MC_HOST];
+    if (e == cudaSuccess) e = mesh_read_counters(h, cnt_host);
+    if (e == cudaSuccess) {
+        const int nalloc = std::min(cnt_host[IM_MC_TRIS_ALLOC], max_t);
+        if (nalloc > 0) IM_LAUNCH(k_chg_init, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, C.pub, nalloc);
+        if ((e = cudaGetLastError()) == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    }
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "changes_enable: allocation of the change feed's buffers failed");
+    }
+    c.on = 1;
+    c.enable_frame = c.last_frame = h->frame_counter;
+    h->chg = std::move(c);
+    h->F.chg_stamp = stamp; h->F.chg_list = list; h->F.chg_cnt = cnt; h->F.chg_cap = cap;
+    return IMMESH_OK;
+}
+int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames, int cap_frames, int32_t* rows, int64_t cap_rows, float* vertices,
+                        int64_t cap_vertices, int64_t* counts) {
+    if (!h || !counts || cap_frames < 0 || cap_rows < 0 || cap_vertices < 0 || (cap_frames > 0 && !frames) || (cap_rows > 0 && !rows) || (cap_vertices > 0 && !vertices))
+        return im_fail(IMMESH_E_INVALID, "changes: bad argument");
+    for (int i = 0; i < 4; ++i) counts[i] = 0;
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "changes: a sharded mesh handle is not supported");
+    const auto& c = h->chg;
+    if (!c.on) return im_fail(IMMESH_E_INVALID, "changes: the change feed is not enabled (immesh_mesh_changes_enable)");
+    const int64_t newest = c.last_frame, nf = newest - since_frame;
+    counts[3] = newest;
+    if (since_frame > newest) return im_fail(IMMESH_E_INVALID, "changes: since_frame is newer than the newest queued frame");
+    if (since_frame < c.enable_frame) return im_fail(IMMESH_E_RANGE, "changes: since_frame is older than the enable (resync: snapshot, then read from the newest frame)");
+    if (nf > c.C.max_frames) return im_fail(IMMESH_E_RANGE, "changes: the frames after since_frame are no longer held (max_frames; resync: snapshot, then read from the newest frame)");
+    if (nf == 0) return IMMESH_OK;
+    IM_CUDA(cudaEventSynchronize(h->ev_done[newest & (IM_SLOTS - 1)]));   // the newest frame only (a batched frame has finished already)
+    std::vector<ChgHdr> hdr((size_t)c.C.max_frames);
+    long long written = 0;
+    IM_CUDA(cudaMemcpy(hdr.data(), c.C.hdr, hdr.size() * sizeof(ChgHdr), cudaMemcpyDeviceToHost));
+    IM_CUDA(cudaMemcpy(&written, c.C.written, sizeof(written), cudaMemcpyDeviceToHost));
+    for (int64_t f = since_frame + 1; f <= newest; ++f) {
+        const ChgHdr& r = hdr[(size_t)(f % c.C.max_frames)];
+        if (r.frame != f || r.lost || r.r_begin < written - c.C.max_rows)
+            return im_fail(IMMESH_E_RANGE, ("changes: the rows of frame " + std::to_string(f) + " are not held (" + (r.frame != f ? "not recorded" : r.lost ? "lost to the feed's per-frame list or ring" : "ring wrapped") +
+                                            "; resync: snapshot, then read from the newest frame)").c_str());
+    }
+    const ChgHdr& first = hdr[(size_t)((since_frame + 1) % c.C.max_frames)];
+    const ChgHdr& last = hdr[(size_t)(newest % c.C.max_frames)];
+    const int64_t nrows = last.r_end - first.r_begin, nverts = last.v_end - first.v_begin;
+    counts[0] = nf; counts[1] = nrows; counts[2] = nverts;
+    if (nf > cap_frames || nrows > cap_rows || nverts > cap_vertices)
+        return im_fail(IMMESH_E_CAPACITY, "changes: a buffer is smaller than the counts (counts holds them; nothing was written)");
+    for (int64_t f = since_frame + 1, k = 0; f <= newest; ++f, ++k) {
+        const ChgHdr& r = hdr[(size_t)(f % c.C.max_frames)];
+        frames[k * 4 + 0] = f; frames[k * 4 + 1] = r.v_begin; frames[k * 4 + 2] = r.v_end; frames[k * 4 + 3] = r.r_end - first.r_begin;
+    }
+    for (int64_t g = first.r_begin; g < last.r_end;) {   // the ring range, in at most two pieces
+        const int64_t pos = g % c.C.max_rows, len = std::min(last.r_end - g, c.C.max_rows - pos);
+        IM_CUDA(cudaMemcpy(rows + (g - first.r_begin) * 4, c.C.ring + pos, (size_t)len * sizeof(int4), cudaMemcpyDeviceToHost));
+        g += len;
+    }
+    if (nverts > 0) {   // a vertex never moves after its append: the positions are read now
+        std::vector<float4> v((size_t)nverts);
+        IM_CUDA(cudaMemcpy(v.data(), h->M.vpos + first.v_begin, (size_t)nverts * sizeof(float4), cudaMemcpyDeviceToHost));
+        for (int64_t i = 0; i < nverts; ++i) { vertices[i * 3] = v[i].x; vertices[i * 3 + 1] = v[i].y; vertices[i * 3 + 2] = v[i].z; }
+    }
     return IMMESH_OK;
 }
 

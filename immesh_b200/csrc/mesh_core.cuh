@@ -255,8 +255,21 @@ struct FrameBuf {
     // batched frame (immesh_mesh_push_frame_batched: one frame's per-voxel stage in several batches); null on the per-frame path
     const int* work_rank; // [max_work] flip priority of the work voxel: its rank among the frame's meshed voxels in (x, y, z) key order
     unsigned char* tri_mark;   // [max_t] IM_TRI_BORN: made live by an earlier batch of this frame; IM_TRI_REMOVE: removal deferred to the frame's end
+    // change feed (immesh_mesh_changes_enable; chg_stamp null: off): the frame number of each triangle slot's first touch, the
+    // frame's touched slots and the feed's counter block (slots IM_CH_*)
+    int* chg_stamp;       // [max_t]
+    int* chg_list;        // [chg_cap]
+    int* chg_cnt;
+    int chg_cap;
 };
 enum : unsigned char { IM_TRI_BORN = 1, IM_TRI_REMOVE = 2 };
+// Slots of FrameBuf::chg_cnt: name, writer.  All three are reset by chg_frame_end (mesh_changes.cuh) and at enable.
+enum : int {
+    IM_CH_TOUCHED = 0,   // touched slots listed (chg_touch); may exceed chg_cap: the frame then falls back to a sweep
+    IM_CH_SWEPT = 1,     // slots listed by the sweep (chg_sweep_slot)
+    IM_CH_ROWS = 2,      // rows of the frame (k_chg_rows)
+    IM_CH_SIZE = 4,
+};
 // a live triangle that was live before the frame began (the only ones the frame's pull and commit see)
 IM_HD bool tri_pre_frame(const FrameBuf& F, int t) { return !F.tri_mark || F.tri_mark[t] != IM_TRI_BORN; }
 
@@ -351,6 +364,12 @@ IM_HD void im_fence() {
 #if defined(__CUDA_ARCH__)
     __threadfence();
 #endif
+}
+// change feed: the first touch of triangle slot t in this frame puts it on the frame's list (once, whichever writer comes first)
+IM_HD void chg_touch(const FrameBuf& F, int t) {
+    if (!F.chg_stamp || im_atomic_exch(&F.chg_stamp[t], F.frame) == F.frame) return;
+    const int e = im_atomic_add(&F.chg_cnt[IM_CH_TOUCHED], 1);
+    if (e < F.chg_cap) F.chg_list[e] = t;
 }
 // float squared distance exactly as KD_TREE::calc_dist (ikd_Tree.cpp:1722-1727): ((dx*dx + dy*dy) + dz*dz), no FMA
 IM_HD float dist2f(float ax, float ay, float az, float bx, float by, float bz) {

@@ -48,6 +48,7 @@ IM_HD void apply_face(const MeshDev& M, const FrameBuf& F, int a, int b, int c, 
     const int t = tri_find(M, a, b, c);
     if (t >= 0 && M.tri[t].w && tri_pre_frame(F, t)) {
         im_atomic_max64(&M.tri_flip[t], word);
+        chg_touch(F, t);   // its orientation may change
     } else {
         const int e = im_atomic_add(&M.cnt[IM_MC_ADD], 1);
         if (e < F.max_list) {

@@ -1,13 +1,14 @@
 // immesh_b200 -- the one-block scan and the stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, 2048-element tiles;
 // ranks inside a tile from __match_any_sync (warp) + per-warp digit counts in shared memory.  Used by the pcl::VoxelGrid front-end
-// (cell index -> point), the IMU undistortion (time stamp -> point), the plane-map publisher, the viewer's region buffers and the
-// batched frame.  Include inside an anonymous namespace of a translation unit that includes common_host.hpp (IM_LAUNCH).
+// (cell index -> point), the IMU undistortion (time stamp -> point), the plane-map publisher, the viewer's region buffers, the
+// batched frame and the mesh's change feed.  Include inside an anonymous namespace of a translation unit that includes common_host.hpp (IM_LAUNCH).
 #pragma once
 #define VG_TILE 2048
 #define VG_THREADS 256
 
-// ---- stable LSD radix sort, 8-bit digits.  hist is digit-major: hist[d * nblocks + b]
-__global__ void __launch_bounds__(VG_THREADS) k_rs_hist(const unsigned int* __restrict__ keys, int n, int shift, int* hist, int nblocks) {
+// ---- stable LSD radix sort, 8-bit digits.  hist is digit-major: hist[d * nblocks + b].  Each kernel has a variant (_dev) that reads
+// the count from the device: its grid covers a capacity, and the blocks past the count's tiles return at once.
+__device__ __forceinline__ void rs_hist_tile(const unsigned int* __restrict__ keys, int n, int shift, int* hist, int nblocks) {
     __shared__ int h[256];
     h[threadIdx.x] = 0;
     __syncthreads();
@@ -18,6 +19,13 @@ __global__ void __launch_bounds__(VG_THREADS) k_rs_hist(const unsigned int* __re
     }
     __syncthreads();
     hist[threadIdx.x * nblocks + blockIdx.x] = h[threadIdx.x];
+}
+__global__ void __launch_bounds__(VG_THREADS) k_rs_hist(const unsigned int* __restrict__ keys, int n, int shift, int* hist, int nblocks) {
+    rs_hist_tile(keys, n, shift, hist, nblocks);
+}
+__global__ void __launch_bounds__(VG_THREADS) k_rs_hist_dev(const unsigned int* __restrict__ keys, const int* n_dev, int shift, int* hist) {
+    const int n = *n_dev, nb = (n + VG_TILE - 1) / VG_TILE;
+    if ((int)blockIdx.x < nb) rs_hist_tile(keys, n, shift, hist, nb);
 }
 // exclusive scan of v over a block of 1024 threads, which all call it: warp shuffle, then a scan of the 32 warp totals in warp 0
 __device__ __forceinline__ int block_scan_1024(int v) {
@@ -44,7 +52,7 @@ __device__ __forceinline__ int block_scan_1024(int v) {
     return (warp ? s_warp[warp - 1] : 0) + x - v;
 }
 // exclusive scan of `len` ints in place by ONE block (len <= a few 100 k); total -> *total_out if not null
-__global__ void __launch_bounds__(1024) k_rs_scan(int* a, int len, int* total_out) {
+__device__ __forceinline__ void rs_scan_block(int* a, int len, int* total_out) {
     __shared__ int s_carry;
     if (threadIdx.x == 0) s_carry = 0;
     __syncthreads();
@@ -59,8 +67,10 @@ __global__ void __launch_bounds__(1024) k_rs_scan(int* a, int len, int* total_ou
     }
     if (threadIdx.x == 0 && total_out) *total_out = s_carry;
 }
-__global__ void __launch_bounds__(VG_THREADS) k_rs_scatter(const unsigned int* __restrict__ kin, const unsigned int* __restrict__ vin, unsigned int* kout, unsigned int* vout,
-                                                            int n, int shift, const int* __restrict__ hist, int nblocks) {
+__global__ void __launch_bounds__(1024) k_rs_scan(int* a, int len, int* total_out) { rs_scan_block(a, len, total_out); }
+__global__ void __launch_bounds__(1024) k_rs_scan_dev(int* a, const int* n_dev) { rs_scan_block(a, 256 * ((*n_dev + VG_TILE - 1) / VG_TILE), nullptr); }
+__device__ __forceinline__ void rs_scatter_tile(const unsigned int* __restrict__ kin, const unsigned int* __restrict__ vin, unsigned int* kout, unsigned int* vout,
+                                                int n, int shift, const int* __restrict__ hist, int nblocks) {
     __shared__ int run[256];                      // next free slot of every digit for this tile (global position)
     __shared__ int wcnt[VG_THREADS / 32][256];    // per-warp digit counts of the current round
     run[threadIdx.x] = hist[threadIdx.x * nblocks + blockIdx.x];
@@ -91,14 +101,30 @@ __global__ void __launch_bounds__(VG_THREADS) k_rs_scatter(const unsigned int* _
         __syncthreads();
     }
 }
+__global__ void __launch_bounds__(VG_THREADS) k_rs_scatter(const unsigned int* __restrict__ kin, const unsigned int* __restrict__ vin, unsigned int* kout, unsigned int* vout,
+                                                            int n, int shift, const int* __restrict__ hist, int nblocks) {
+    rs_scatter_tile(kin, vin, kout, vout, n, shift, hist, nblocks);
+}
+__global__ void __launch_bounds__(VG_THREADS) k_rs_scatter_dev(const unsigned int* __restrict__ kin, const unsigned int* __restrict__ vin, unsigned int* kout,
+                                                                unsigned int* vout, const int* n_dev, int shift, const int* __restrict__ hist) {
+    const int n = *n_dev, nb = (n + VG_TILE - 1) / VG_TILE;
+    if ((int)blockIdx.x < nb) rs_scatter_tile(kin, vin, kout, vout, n, shift, hist, nb);
+}
 // the LSD passes over the low `passes` 8-bit digits of the n keys in k[cur] (values in v[cur]), each from one buffer of the pairs into
-// the other; hist holds 256 * ceil(n / VG_TILE) ints.  Returns the index of the buffers that hold the sorted pairs.
-inline int rs_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist) {
+// the other; hist holds 256 * ceil(n / VG_TILE) ints.  Returns the index of the buffers that hold the sorted pairs.  n_dev: the count
+// is read on the device (*n_dev <= n), and n is the capacity the grids cover.
+inline int rs_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist, const int* n_dev = nullptr) {
     const int nb = (n + VG_TILE - 1) / VG_TILE;
     for (int pass = 0; pass < passes; ++pass) {
-        IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], n, 8 * pass, hist, nb);
-        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
-        IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], (const unsigned int*)v[cur], k[cur ^ 1], v[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
+        if (n_dev) {
+            IM_LAUNCH(k_rs_hist_dev, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], n_dev, 8 * pass, hist);
+            IM_LAUNCH(k_rs_scan_dev, 1, 1024, 0, st, hist, n_dev);
+            IM_LAUNCH(k_rs_scatter_dev, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], (const unsigned int*)v[cur], k[cur ^ 1], v[cur ^ 1], n_dev, 8 * pass, (const int*)hist);
+        } else {
+            IM_LAUNCH(k_rs_hist, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], n, 8 * pass, hist, nb);
+            IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, hist, 256 * nb, (int*)nullptr);
+            IM_LAUNCH(k_rs_scatter, nb, VG_THREADS, 0, st, (const unsigned int*)k[cur], (const unsigned int*)v[cur], k[cur ^ 1], v[cur ^ 1], n, 8 * pass, (const int*)hist, nb);
+        }
         cur ^= 1;
     }
     return cur;

@@ -400,6 +400,35 @@ int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics /*[4
 int immesh_mesh_reinforce_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/);
 int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth /*[h][w] or NULL*/, float* points /*[cap][3] or NULL*/, int32_t* point_pixel /*[cap] or NULL*/,
                                  int cap, int* n_out, double* pose_out /*[12] or NULL*/);
+/* The change feed: each frame's added and removed triangles (the reference's per-frame added_triangle_list / removed_triangle_list,
+ * src/ImMesh_mesh_reconstruction.cpp:122-123, 209-244), recorded on the device, so that a caller that keeps its own copy of the mesh
+ * (publisher, remote viewer, recorder) applies the difference instead of calling immesh_mesh_snapshot after every frame.
+ *   The state described is what immesh_mesh_snapshot returns: the vertices (raw x y z, ids in append order) and the live triangles
+ *     as ascending (i<j<k) triples with their m_index_flip.  Frame f (the handle's frames counted from 1; a batched frame is one frame)
+ *     appended the vertex ids [v_begin, v_end) and has one row (a, b, c, code) per triangle whose (live, flip) state differs between
+ *     the end of frame f - 1 and the end of frame f: code 0 removed; 2 | flip made live; 4 | flip stayed live with its flip changed
+ *     (an "existing" facet re-oriented by correct_triangle_index, src/meshing/mesh_rec_geometry.cpp:399-433).  The rows are the net
+ *     difference (a triangle touched without a change of state gives none), in ascending (a, b, c) order inside a frame: the same with
+ *     and without CUDA graphs and for any batch sizes.  Applying them to immesh_mesh_snapshot's result at frame f - 1 gives its
+ *     result at frame f bit for bit.
+ *   immesh_mesh_changes_enable(h, max_rows, max_frames): drains the frames in flight, allocates the feed (a ring of max_rows rows, the
+ *     headers of the last max_frames frames, a per-frame list of min(max_rows, 2^21) touched triangles, a byte and a stamp per
+ *     triangle slot) and takes the mesh as it is as the published state (it may be non-empty); the frames queued after it are
+ *     recorded, on the mesh stream inside each frame's captured graph, with no host synchronisation and no allocation.  max_rows = 0
+ *     turns it off and frees the buffers; enabling again starts afresh.  max_rows outside [0, 2^30], max_frames outside [1, 2^20],
+ *     or a sharded handle: IMMESH_E_INVALID (immesh_mesh_shard refuses a handle with the feed on).
+ *   immesh_mesh_changes(h, since_frame, ...): the frames (since_frame, newest] in order, newest = the newest frame queued; blocks
+ *     until that frame has finished.  frames [n][4] = frame, v_begin, v_end, rows_end (the end of its rows in `rows`); rows [n][4];
+ *     vertices [n][3] = the positions of the ids [v_begin of the first frame, v_end of the last).  counts [4] = n_frames, n_rows,
+ *     n_vertices, newest_frame.  A count above its cap: IMMESH_E_CAPACITY with the counts, nothing written (caps 0: a count query).
+ *     IMMESH_E_RANGE, with counts[3] = newest: since_frame is before the enable, a frame after it is no longer held (max_frames
+ *     wrapped, or its rows were overwritten in the ring), or it was lost to the feed (more rows than max_rows, or more touched
+ *     triangles than the per-frame list holds).  A loss never fails a push and never changes the mesh.  Resync: immesh_mesh_snapshot,
+ *     then read on from counts[3] (a query with caps 0 returns it).  Not enabled, since_frame > newest, bad arguments or a sharded
+ *     handle: IMMESH_E_INVALID. */
+int immesh_mesh_changes_enable(immesh_mesh_t* h, int64_t max_rows, int max_frames);
+int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames /*[cap_frames][4]*/, int cap_frames, int32_t* rows /*[cap_rows][4]*/,
+                        int64_t cap_rows, float* vertices /*[cap_vertices][3]*/, int64_t cap_vertices, int64_t* counts /*[4]*/);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
