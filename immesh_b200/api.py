@@ -131,6 +131,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_profile_timeline", [C.c_char_p, C.c_int]),
         ("immesh_launch_count", []),
         ("immesh_graph_stats", [vp, vp, C.POINTER(C.c_int64)]),
+        ("immesh_graph_pdl_edges", [vp, vp, C.POINTER(C.c_int64)]),
         ("immesh_lio_last_timing", [vp, dp]),
         ("immesh_lio_capacity", [vp, C.POINTER(C.c_int64)]),
         ("immesh_lio_reserve", [vp, C.c_int64, C.c_int64, C.c_int64]),
@@ -1004,12 +1005,17 @@ def launch_count(lib: Optional[C.CDLL] = None) -> int:
 
 
 def graph_stats(lio: Optional["Lio"], mesh: Optional["Mesh"]) -> dict:
-    """CUDA-graph replay accounting of the pipelined entry points."""
+    """CUDA-graph replay accounting of the pipelined entry points, and the programmatic dependent-launch edges of each captured graph."""
     lib = (lio or mesh).lib
+    h_lio, h_mesh = lio._h if lio else None, mesh._h if mesh else None
     out = (C.c_int64 * 6)()
-    _check(lib, lib.immesh_graph_stats(lio._h if lio else None, mesh._h if mesh else None, out), "graph_stats")
+    _check(lib, lib.immesh_graph_stats(h_lio, h_mesh, out), "graph_stats")
     keys = ("lio_captures", "lio_replays", "lio_failures", "mesh_captures", "mesh_replays", "mesh_failures")
-    return dict(zip(keys, [int(v) for v in out]))
+    res = dict(zip(keys, [int(v) for v in out]))
+    pdl = (C.c_int64 * 2)()
+    _check(lib, lib.immesh_graph_pdl_edges(h_lio, h_mesh, pdl), "graph_pdl_edges")
+    res["lio_pdl_edges"], res["mesh_pdl_edges"] = int(pdl[0]), int(pdl[1])
+    return res
 
 
 def host_wait_ms(lio: Optional["Lio"], mesh: Optional["Mesh"]):

@@ -116,21 +116,25 @@ struct GraphCtx {
     cudaGraphExec_t exec = nullptr;
     cudaGraph_t graph = nullptr;
     long long kernels = 0;             // kernel launches recorded into the graph
+    long long pdl_edges = 0;           // programmatic (IM_LAUNCH_PDL) edges of the captured graph
     unsigned sig = 0;                  // control-flow signature the graph was captured with
     cudaError_t err = cudaSuccess;
     long long captures = 0, replays = 0, failures = 0;
     void destroy() {
         if (exec) cudaGraphExecDestroy(exec);
         if (graph) cudaGraphDestroy(graph);
-        exec = nullptr; graph = nullptr; kernels = 0;
+        exec = nullptr; graph = nullptr; kernels = 0; pdl_edges = 0;
     }
 };
 inline GraphCtx*& graph_ctx() {
     static thread_local GraphCtx* g = nullptr;
     return g;
 }
+// pdl: launch with programmatic stream serialization (Hopper programmatic dependent launch): the kernel may be scheduled while the
+// previous kernel on `st` still runs, and must call pdl_wait() (pdl.cuh) before it touches global memory.  Only for a kernel that
+// directly follows another kernel on the same stream; under stream capture the attribute becomes a programmatic graph edge.
 template <typename... KArgs, typename... Args>
-inline void im_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline void im_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args&&... args) {
     Profiler& pr = profiler();
     pr.launches++;
     std::tuple<KArgs...> vals(std::forward<Args>(args)...);   // exactly the kernel's parameter types
@@ -141,7 +145,18 @@ inline void im_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 
     }
     GraphCtx* g = graph_ctx();
     if (pr.enabled) pr.begin(name, st);
-    cudaError_t e = cudaLaunchKernel((const void*)kern, grid, block, ptrs, smem, st);
+    cudaError_t e;
+    if (pdl) {
+        cudaLaunchAttribute attr;
+        attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr.val.programmaticStreamSerializationAllowed = 1;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+        cfg.attrs = &attr; cfg.numAttrs = 1;
+        e = cudaLaunchKernelExC(&cfg, (const void*)kern, ptrs);
+    } else {
+        e = cudaLaunchKernel((const void*)kern, grid, block, ptrs, smem, st);
+    }
     if (pr.enabled) pr.end(st);
     if (g) {   // capturing: the launch must have been recorded on a stream of the capture
         cudaStreamCaptureStatus status;
@@ -149,6 +164,18 @@ inline void im_launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 
         if (e == cudaSuccess && e2 == cudaSuccess && status == cudaStreamCaptureStatusActive) g->kernels++;
         else if (g->err == cudaSuccess) g->err = (e != cudaSuccess) ? e : (e2 != cudaSuccess ? e2 : cudaErrorUnknown);
     }
+}
+inline cudaError_t count_pdl_edges(GraphCtx& g) {
+    size_t n = 0;
+    cudaError_t e = cudaGraphGetEdges_v2(g.graph, nullptr, nullptr, nullptr, &n);
+    if (e != cudaSuccess || n == 0) return e;
+    std::vector<cudaGraphNode_t> from(n), to(n);
+    std::vector<cudaGraphEdgeData> data(n);
+    e = cudaGraphGetEdges_v2(g.graph, from.data(), to.data(), data.data(), &n);
+    if (e != cudaSuccess) return e;
+    g.pdl_edges = 0;
+    for (size_t i = 0; i < n; ++i) g.pdl_edges += data[i].type == cudaGraphDependencyTypeProgrammatic;
+    return cudaSuccess;
 }
 // The body's launches take every per-call value from device memory, so once captured the graph is replayed by a bare
 // cudaGraphLaunch -- the body is not run again.  `sig` must cover everything that changes the sequence or its arguments
@@ -167,6 +194,7 @@ inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st
         e = cudaStreamEndCapture(st, &g.graph);
         if (e == cudaSuccess && g.err != cudaSuccess) e = g.err;
         if (e == cudaSuccess) e = cudaGraphInstantiate(&g.exec, g.graph, 0);
+        if (e == cudaSuccess) e = count_pdl_edges(g);
         if (e != cudaSuccess) { g.destroy(); cudaGetLastError(); g.failures++; return e; }
         g.sig = sig;
         g.captures++;
@@ -179,4 +207,6 @@ inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st
 }  // namespace immesh
 
 // kernel launch with accounting; wrap template kernels in parentheses: IM_LAUNCH((k<256>), grid, block, smem, stream, args...)
-#define IM_LAUNCH(KERN, GRID, BLOCK, SMEM, STREAM, ...) immesh::im_launch(#KERN, KERN, dim3(GRID), dim3(BLOCK), (SMEM), (STREAM), ##__VA_ARGS__)
+#define IM_LAUNCH(KERN, GRID, BLOCK, SMEM, STREAM, ...) immesh::im_launch(#KERN, KERN, dim3(GRID), dim3(BLOCK), (SMEM), (STREAM), false, ##__VA_ARGS__)
+// the same, with programmatic dependent launch when PDL is true (see im_launch; KERN must call pdl_wait() first on every path)
+#define IM_LAUNCH_PDL(PDL, KERN, GRID, BLOCK, SMEM, STREAM, ...) immesh::im_launch(#KERN, KERN, dim3(GRID), dim3(BLOCK), (SMEM), (STREAM), (bool)(PDL), ##__VA_ARGS__)

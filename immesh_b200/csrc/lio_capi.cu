@@ -19,17 +19,21 @@
 #include "handles.hpp"
 #include "map_dump.hpp"
 #include "pool_growth.cuh"
+#include "pdl.cuh"
 
 using namespace immesh;
 
 // ------------------------------------------------------------------ kernels
 __global__ void __launch_bounds__(128) k_prepare(LioParams P, ScanBuf sb_) {
+    pdl_wait();
     const ScanBuf sb = scan_load_dyn(sb_);
     const int n = sb.n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) prepare_point(P, sb, i);
+    pdl_trigger();
 }
 
 __global__ void k_reset_scan(ScanBuf sb, LioCtrl* ctrl, int copy_prop) {
+    pdl_wait();
     const int tid = blockIdx.x * blockDim.x + threadIdx.x;
     const int nt = gridDim.x * blockDim.x;
     unsigned long long* acc = &ctrl->acc[0][0];
@@ -42,6 +46,7 @@ __global__ void k_reset_scan(ScanBuf sb, LioCtrl* ctrl, int copy_prop) {
         ctrl->rematch_num = 0;
         for (int i = 0; i < IM_MAX_ITER; ++i) ctrl->blocks_done[i] = 0;
     }
+    pdl_trigger();
 }
 
 // K2+K3.  Default (one GPU): two kernels per IESKF iteration.
@@ -76,6 +81,7 @@ struct MatchCombine8 {
 };
 __global__ void __launch_bounds__(MATCH_THREADS, 8) k_match(VoxelMapDev map, LioParams P, ScanBuf sb_, LioCtrl* ctrl) {
     __shared__ double s_state[24 + 6 * 18];
+    pdl_wait();
     IM_STAMP(0, 0);
     // the stop flag, the scan's device-resident description and the state are loaded together (one trip to L2 instead of three)
     const int stop = ctrl->stop;
@@ -97,6 +103,7 @@ __global__ void __launch_bounds__(MATCH_THREADS, 8) k_match(VoxelMapDev map, Lio
     comb.mask = (lanes == 1) ? 0u : 0xFFu << ((threadIdx.x & 31) & ~(MATCH_LANES - 1));
     for (int i = blockIdx.x * per_block + (threadIdx.x / lanes); i < n; i += gridDim.x * per_block)
         residual_match_lanes(map, P, sb, s_state, i, sub, lanes, comb);
+    pdl_trigger();
     IM_STAMP(7, 0);
 }
 
@@ -135,6 +142,7 @@ __device__ __forceinline__ void publish_terms(const long long (&acc)[IM_NTERMS],
 template <bool MATCHED>
 __device__ __forceinline__ void residual_block(const VoxelMapDev& map, const LioParams& P, const ScanBuf& sb_, LioCtrl* ctrl, int iter, int fused_solve) {
     __shared__ double s_state[24 + 6 * 18];
+    pdl_wait();
     IM_STAMP(10, 0);
     // the stop flag, the scan's device-resident description and the state -- rot/pos and the 6x6 pose block of the covariance, the only
     // parts this pass reads -- are loaded together (one trip to L2 instead of three)
@@ -175,6 +183,7 @@ __device__ __forceinline__ void residual_block(const VoxelMapDev& map, const Lio
         __threadfence();
         ieskf_solve(P, ctrl, iter, &S, threadIdx.x, blockDim.x);
     }
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(RES_THREADS) k_residual(VoxelMapDev map, LioParams P, ScanBuf sb_, LioCtrl* ctrl, int iter, int fused_solve) {
     residual_block<false>(map, P, sb_, ctrl, iter, fused_solve);
@@ -345,18 +354,24 @@ __global__ void __launch_bounds__(PREDICT_THREADS) k_predict(LioCtrl* ctrl) {
 }
 
 __global__ void __launch_bounds__(128) k_grow_point(VoxelMapDev map, LioParams P, ScanBuf sb_, LioCtrl* ctrl, int mode) {
+    pdl_wait();
     const ScanBuf sb = scan_load_dyn(sb_);
     const int n = sb.n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) grow_point(map, P, sb, ctrl->state, i, mode);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_grow_segment(ScanBuf sb) {
+    pdl_wait();
     const int nt = *sb.n_touched;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < nt; t += gridDim.x * blockDim.x) grow_segment(sb, t);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_grow_scatter(ScanBuf sb_) {
+    pdl_wait();
     const ScanBuf sb = scan_load_dyn(sb_);
     const int n = sb.n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) grow_scatter(sb, i);
+    pdl_trigger();
 }
 // Most touched root voxels receive one or two points of a scan and stay in an append-only regime (a node still collecting its
 // first points, or a planar node between two refits): no plane fit, no split, no descent.  k_grow_simple finishes those -- same
@@ -367,6 +382,7 @@ __global__ void __launch_bounds__(128) k_grow_scatter(ScanBuf sb_) {
 // 60 dependent moment read-modify-writes take longer than the warp's two per lane.)
 #define GROW_SIMPLE_MAX 4
 __global__ void __launch_bounds__(128) k_grow_simple(VoxelMapDev map, LioParams P, ScanBuf sb, int mode, int* complex_list, int* n_complex) {
+    pdl_wait();
     const int lane = threadIdx.x & 31;
     const int nt = *sb.n_touched;
     const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -418,9 +434,11 @@ __global__ void __launch_bounds__(128) k_grow_simple(VoxelMapDev map, LioParams 
             sb.slot_cursor[slot] = 0;
         }
     }
+    pdl_trigger();
 }
 // one warp per remaining touched root voxel, voxels claimed dynamically (their cost varies by orders of magnitude)
 __global__ void __launch_bounds__(128) k_grow_voxel(VoxelMapDev map, LioParams P, ScanBuf sb, int mode, int* sorted_scratch, int* work_counter, const int* complex_list, const int* n_complex) {
+    pdl_wait();
     const int lane = threadIdx.x & 31;
     const int nt = *n_complex;
     while (true) {
@@ -430,10 +448,12 @@ __global__ void __launch_bounds__(128) k_grow_voxel(VoxelMapDev map, LioParams P
         if (t >= nt) break;
         grow_voxel(map, P, sb, complex_list[t], mode, lane, 32, sorted_scratch);
     }
+    pdl_trigger();
 }
 // last kernel of a scan: recycle chunks, reset the per-scan counters, publish the converged pose for the mesher's frame (which
 // runs behind on another stream) and assemble the block the host reads back with one D2H copy
 __global__ void k_grow_finish(VoxelMapDev map, ScanBuf sb, LioCtrl* ctrl, int* counters) {
+    pdl_wait();
     recycle_chunks(map, threadIdx.x, blockDim.x);
     if (threadIdx.x == 0) {
         *sb.n_touched = 0;
@@ -1027,23 +1047,25 @@ static int lio_growth_check(immesh_lio* h, long long n) {
 }
 // resident blocks per SM of the persistent per-voxel map update k_grow_voxel (headroom for the kernels on the other streams)
 #define GROW_VOXEL_BPS 4
-// map growth of the scan described by the device-resident ScanDyn
-static void launch_grow(immesh_lio* h, int mode) {
+// map growth of the scan described by the device-resident ScanDyn.  pdl: every launch is a programmatic dependent launch (the
+// sequence directly follows a kernel on h->stream, with no event or copy in between)
+static void launch_grow(immesh_lio* h, int mode, bool pdl = false) {
     const int g = grid_fixed(h, 128);
-    IM_LAUNCH(k_grow_point, g, 128, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, mode);
-    IM_LAUNCH(k_grow_segment, grid_fixed(h, 128, 2), 128, 0, h->stream, h->sb);
-    IM_LAUNCH(k_grow_scatter, g, 128, 0, h->stream, h->sb);
+    IM_LAUNCH_PDL(pdl, k_grow_point, g, 128, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, mode);
+    IM_LAUNCH_PDL(pdl, k_grow_segment, grid_fixed(h, 128, 2), 128, 0, h->stream, h->sb);
+    IM_LAUNCH_PDL(pdl, k_grow_scatter, g, 128, 0, h->stream, h->sb);
     int* n_complex = h->d_counters + IM_LC_COMPLEX;
-    IM_LAUNCH(k_grow_simple, h->n_sm * 16, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_complex, n_complex);
-    IM_LAUNCH(k_grow_voxel, h->n_sm * GROW_VOXEL_BPS, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + IM_LC_WORK, (const int*)h->d_complex, (const int*)n_complex);
-    IM_LAUNCH(k_grow_finish, 1, 256, 0, h->stream, h->map, h->sb, h->d_ctrl, h->d_counters);
+    IM_LAUNCH_PDL(pdl, k_grow_simple, h->n_sm * 16, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_complex, n_complex);
+    IM_LAUNCH_PDL(pdl, k_grow_voxel, h->n_sm * GROW_VOXEL_BPS, 128, 0, h->stream, h->map, h->P, h->sb, mode, h->d_sorted, h->d_counters + IM_LC_WORK, (const int*)h->d_complex, (const int*)n_complex);
+    IM_LAUNCH_PDL(pdl, k_grow_finish, 1, 256, 0, h->stream, h->map, h->sb, h->d_ctrl, h->d_counters);
 }
 // IESKF iterations.  One GPU: per iteration k_match then k_terms; the last block of k_terms runs the 6x6 IESKF update.
 // Sharded over peer windows: pass1(+publish bits) -> pass2(wait bits, +publish sums) -> solve(wait sums), exchanges fused in.
 // Sharded over NCCL (baseline): pass1 -> all-reduce(bit words) -> pass2 -> all-reduce(58 int64 sums) -> solve.
-static int launch_estimate(immesh_lio* h) {
-    IM_LAUNCH(k_reset_scan, 2, 256, 0, h->stream, h->sb, h->d_ctrl, 1);
-    IM_LAUNCH(k_prepare, grid_fixed(h, 128), 128, 0, h->stream, h->P, h->sb);
+// pdl (one GPU only): every launch is a programmatic dependent launch, as in launch_grow.
+static int launch_estimate(immesh_lio* h, bool pdl = false) {
+    IM_LAUNCH_PDL(pdl, k_reset_scan, 2, 256, 0, h->stream, h->sb, h->d_ctrl, 1);
+    IM_LAUNCH_PDL(pdl, k_prepare, grid_fixed(h, 128), 128, 0, h->stream, h->P, h->sb);
     const int g = grid_fixed(h, RES_THREADS, 4);
     if (h->P.shard_n > 1 && h->win.ok) {
         LioPeers pe;
@@ -1071,8 +1093,8 @@ static int launch_estimate(immesh_lio* h) {
     }
     const int gm = h->n_sm * 8;   // one resident wave of k_match blocks (__launch_bounds__(128, 8)); k_match picks the lanes per point from n
     for (int it = 0; it < h->P.max_iter; ++it) {
-        IM_LAUNCH(k_match, gm, MATCH_THREADS, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl);
-        IM_LAUNCH(k_terms, g, RES_THREADS, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, it, 1);
+        IM_LAUNCH_PDL(pdl, k_match, gm, MATCH_THREADS, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl);
+        IM_LAUNCH_PDL(pdl, k_terms, g, RES_THREADS, 0, h->stream, h->map, h->P, h->sb, h->d_ctrl, it, 1);
     }
     return IMMESH_OK;
 }
@@ -1160,10 +1182,12 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     int lrc = IMMESH_OK;
     if (!timing) {
         const unsigned sig = 1u | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
+        // one GPU: every kernel after k_predict is a programmatic dependent launch (the sharded paths wait on peers and NCCL)
+        const bool pdl = h->P.shard_n <= 1;
         queued = immesh::run_graphed_static(h->graph, sig, h->stream, [&] {
             IM_LAUNCH(k_predict, 1, PREDICT_THREADS, 0, h->stream, h->d_ctrl);
-            lrc = launch_estimate(h);
-            launch_grow(h, 0);
+            lrc = launch_estimate(h, pdl);
+            launch_grow(h, 0, pdl);
         }) == cudaSuccess;
         if (!queued) h->use_graph = 0;   // not expected; keep working through direct launches
     }

@@ -17,6 +17,7 @@
 #include "pool_growth.cuh"
 #include "nccl_api.hpp"
 #include "reinforce.cuh"
+#include "pdl.cuh"
 
 using namespace immesh;
 namespace {
@@ -25,24 +26,31 @@ namespace {
 
 // ------------------------------------------------------------------ kernels
 __global__ void k_frame_begin(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nt = gridDim.x * blockDim.x;
     for (unsigned int i = tid; i <= F.cmask; i += nt) { F.ckeys[i] = IM_EMPTY_KEY; F.chead[i] = -1; }
     for (unsigned int i = tid; i <= F.fset_mask; i += nt) F.fset[i] = -1;
     if (tid == 0) mesh_cnt_frame_begin(M);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_cand_init(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_init(M, P, F, c);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_cand_conflicts(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_conflicts(M, P, F, c);
+    pdl_trigger();
 }
 // Priority polling: candidate c waits only on candidates with a smaller index.  Blocks take tickets so that the
 // block holding the smallest undecided candidate is always resident; a poll cap turns a (never observed) livelock
 // into an error flag instead of a hang.
 __global__ void __launch_bounds__(128) k_cand_resolve(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     __shared__ int s_ticket;
     const int nblocks = (F.m + blockDim.x - 1) / blockDim.x;
@@ -62,6 +70,7 @@ __global__ void __launch_bounds__(128) k_cand_resolve(MeshDev M, MeshParams P, F
             __threadfence();
         }
     }
+    pdl_trigger();
 }
 // exclusive scan of n items by one block of 1024 threads in ONE pass: thread t owns a contiguous chunk of ceil(n/1024) items.
 // count(c) is item c's value; emit(c, run) stores item c's offset run and returns its value.  Returns the offset after the thread's
@@ -78,27 +87,36 @@ __device__ __forceinline__ int chunk_scan_1024(int n, Count count, Emit emit) {
 }
 // the accept flags into the candidates' output ranks
 __global__ void __launch_bounds__(1024) k_cand_scan(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     chunk_scan_1024(F.m, [&](int c) { return F.cand_status[c] == CAND_ACCEPT ? 1 : 0; },
                     [&](int c, int run) { F.cand_scan[c] = run; return F.cand_status[c] == CAND_ACCEPT ? 1 : 0; });
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_cand_commit(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int base = M.cnt[IM_MC_VERTICES];
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_commit(M, P, F, c, base);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_cand_place(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int base = M.cnt[IM_MC_VERTICES];
     for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < F.m; c += gridDim.x * blockDim.x) cand_place(M, F, c, base);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_voxel_select(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int na = min(M.cnt[IM_MC_ACT], F.max_act);
     for (int a = blockIdx.x * blockDim.x + threadIdx.x; a < na; a += gridDim.x * blockDim.x) voxel_select(M, F, a);
+    pdl_trigger();
 }
 // stage A: dilation (exact 20-NN of the in-voxel vertices + smoothing); one block per (voxel, group of <= 8 queries)
 __global__ void __launch_bounds__(128) k_voxel_dilate(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     __shared__ DilateSmem S;
     __shared__ int s_item;
@@ -112,6 +130,7 @@ __global__ void __launch_bounds__(128) k_voxel_dilate(MeshDev M, MeshParams P, F
         voxel_dilate(M, P, F, F.ditem[i], &S, threadIdx.x, blockDim.x);
         __syncthreads();
     }
+    pdl_trigger();
 }
 // stage B, small dilated sets: one warp per voxel (four independent voxels per block), voxels claimed dynamically
 #define IM_WARP_NMAX 96
@@ -138,9 +157,11 @@ __global__ void __launch_bounds__(128) k_voxel_tri_warp(MeshDev M, MeshParams P,
 }
 // stage C (flat): after every voxel's smoothing is final
 __global__ void __launch_bounds__(128) k_commit_faces(MeshDev M, MeshParams P, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int nf = min(M.cnt[IM_MC_FACES], F.max_list);
     for (int f = blockIdx.x * blockDim.x + threadIdx.x; f < nf; f += gridDim.x * blockDim.x) commit_face(M, P, F, f);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_pull_vertices(MeshDev M, MeshParams P, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
@@ -148,9 +169,11 @@ __global__ void __launch_bounds__(128) k_pull_vertices(MeshDev M, MeshParams P, 
     for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nr; r += gridDim.x * blockDim.x) pull_vertex(M, P, F, r);
 }
 __global__ void __launch_bounds__(128) k_pull_check(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int ne = min(M.cnt[IM_MC_PULLED], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < ne; e += gridDim.x * blockDim.x) pull_check(M, F, e);
+    pdl_trigger();
 }
 template <int MAXD>
 __global__ void __launch_bounds__(128) k_voxel_mesh(MeshDev M, MeshParams P, FrameBuf F_, int lo, int store_only) {
@@ -167,17 +190,24 @@ __global__ void __launch_bounds__(128) k_voxel_mesh(MeshDev M, MeshParams P, Fra
     }
 }
 __global__ void __launch_bounds__(128) k_push_remove(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int n = min(M.cnt[IM_MC_REMOVE], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) tri_remove(M, F.rem_tri[e]);
+    pdl_trigger();
 }
 __global__ void __launch_bounds__(128) k_push_add(MeshDev M, FrameBuf F_) {
+    pdl_wait();
     const FrameBuf F = frame_load_dyn(F_);
     const int n = min(M.cnt[IM_MC_ADD], F.max_list);
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x)
         tri_add(M, F.add_tri[(size_t)e * 3 + 0], F.add_tri[(size_t)e * 3 + 1], F.add_tri[(size_t)e * 3 + 2], F.add_flip[e]);
+    pdl_trigger();
 }
-__global__ void k_frame_end(MeshDev M) { mesh_cnt_frame_end(M); }
+__global__ void k_frame_end(MeshDev M) {
+    pdl_wait();
+    mesh_cnt_frame_end(M);
+}
 // ---- the change feed (mesh_changes.cuh), queued after the push when enabled.  full: the frame lists its slots by the sweep (batched)
 __global__ void __launch_bounds__(128) k_chg_gather(MeshDev M, FrameBuf F_) {
     const FrameBuf F = frame_load_dyn(F_);
@@ -1376,19 +1406,23 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     bool nccl_failed = false;
     const int g_pts = mesh_grid_fixed(h, h->max_frame_points, 128);
     const int g_cand = mesh_grid_fixed(h, std::min<long long>(h->max_frame_points, 2LL * P.append_target), 128);
+    // Graph-replayed and not sharded: a kernel that directly follows another kernel on `st` is a programmatic dependent launch.  The
+    // first kernel after a copy, an event wait or the triangulation's join keeps an ordinary edge, as do the change feed's kernels.
+    const bool pdl_frame = F.shard_n <= 1;
     auto launch_frame = [&](bool timing) {
+        const bool pdl = pdl_frame && !timing;
         if (src_mode >= 2) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
-        IM_LAUNCH(k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl && src_mode >= 2, k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[1], st);
-        IM_LAUNCH(k_cand_init, g_cand, 128, 0, st, h->M, P, F);
-        IM_LAUNCH(k_cand_conflicts, g_cand, 128, 0, st, h->M, P, F);
-        IM_LAUNCH(k_cand_resolve, h->n_sm * 4, 128, 0, st, h->M, P, F);
-        IM_LAUNCH(k_cand_scan, 1, 1024, 0, st, h->M, F);
-        IM_LAUNCH(k_cand_commit, g_cand, 128, 0, st, h->M, P, F);
-        IM_LAUNCH(k_cand_place, g_cand, 128, 0, st, h->M, F);
-        IM_LAUNCH(k_voxel_select, g_cand, 128, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_cand_init, g_cand, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_cand_conflicts, g_cand, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_cand_resolve, h->n_sm * 4, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_cand_scan, 1, 1024, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_cand_commit, g_cand, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_cand_place, g_cand, 128, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_voxel_select, g_cand, 128, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[2], st);
-        IM_LAUNCH(k_voxel_dilate, h->n_sm * MESH_DILATE_BPS, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_voxel_dilate, h->n_sm * MESH_DILATE_BPS, 128, 0, st, h->M, P, F);
         if (F.shard_n > 1 && h->win.ok) {   // smoothed positions of the other ranks' voxels, pushed into their windows
             IM_LAUNCH(k_xpush, h->n_sm, 256, 0, st, h->M, F, (const unsigned char*)h->d_seg1, 0, pe, h->d_xdone);
             IM_LAUNCH(k_apply_smooth, h->n_sm * 2, 256, 0, st, h->M, F, (const unsigned char*)h->d_recv1, h->seg1_bytes, pe);
@@ -1410,8 +1444,8 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         cudaStreamWaitEvent(st, h->ev_join, 0);
         cudaStreamWaitEvent(st, h->ev_join3, 0);
         IM_LAUNCH((k_voxel_mesh<1024>), h->n_sm * 2, 128, sizeof(MeshSmem<1024>), st, h->M, P, F, 256, 0);
-        IM_LAUNCH(k_commit_faces, h->n_sm * 8, 128, 0, st, h->M, P, F);
-        IM_LAUNCH(k_pull_check, h->n_sm * 8, 128, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_commit_faces, h->n_sm * 8, 128, 0, st, h->M, P, F);
+        IM_LAUNCH_PDL(pdl, k_pull_check, h->n_sm * 8, 128, 0, st, h->M, F);
         if (F.shard_n > 1 && h->win.ok) {   // every rank applies the facets / removals of all ranks to its replica of the store
             IM_LAUNCH(k_xpush, h->n_sm, 256, 0, st, h->M, F, (const unsigned char*)h->d_seg2, 1, pe, h->d_xdone + 1);
             IM_LAUNCH(k_apply_lists, h->n_sm * 2, 256, 0, st, h->M, F, (const unsigned char*)h->d_recv2, h->seg2_bytes, pe);
@@ -1421,10 +1455,10 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
             IM_LAUNCH(k_apply_lists, h->n_sm * 2, 256, 0, st, h->M, F, (const unsigned char*)h->d_recv2, h->seg2_bytes, pe);
         }
         if (timing) cudaEventRecord(h->ev[3], st);
-        IM_LAUNCH(k_push_remove, h->n_sm * 2, 128, 0, st, h->M, F);
-        IM_LAUNCH(k_push_add, h->n_sm * 2, 128, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_push_remove, h->n_sm * 2, 128, 0, st, h->M, F);
+        IM_LAUNCH_PDL(pdl, k_push_add, h->n_sm * 2, 128, 0, st, h->M, F);
         if (chg_on) mesh_changes_launch(h, F, st, false);
-        IM_LAUNCH(k_frame_end, 1, 1, 0, st, h->M);
+        IM_LAUNCH_PDL(pdl && !chg_on, k_frame_end, 1, 1, 0, st, h->M);
         if (rf_on) mesh_reinforce_launch(h, st);
     };
     bool queued = false;
@@ -1561,6 +1595,12 @@ int immesh_graph_stats(immesh_lio_t* lio, immesh_mesh_t* mesh, int64_t* out) {
     for (int i = 0; i < 6; ++i) out[i] = 0;
     if (lio) { out[0] = lio->graph.captures; out[1] = lio->graph.replays; out[2] = lio->graph.failures; }
     if (mesh) { out[3] = mesh->graph.captures; out[4] = mesh->graph.replays; out[5] = mesh->graph.failures; }
+    return IMMESH_OK;
+}
+int immesh_graph_pdl_edges(immesh_lio_t* lio, immesh_mesh_t* mesh, int64_t* out) {
+    if (!out) return im_fail(IMMESH_E_INVALID, "null argument");
+    out[0] = lio ? lio->graph.pdl_edges : 0;
+    out[1] = mesh ? mesh->graph.pdl_edges : 0;
     return IMMESH_OK;
 }
 // host time (ms) the enqueue calls spent blocked on busy staging slots since the last call of this function: [lio, mesh].

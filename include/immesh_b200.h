@@ -582,6 +582,9 @@ long long immesh_launch_count(void);
 /* CUDA-graph replay accounting of the pipelined entry points: [lio captures, lio replays, lio failures, mesh captures,
  * mesh replays, mesh failures]; either handle may be NULL */
 int immesh_graph_stats(immesh_lio_t* lio, immesh_mesh_t* mesh, int64_t* out /*[6]*/);
+/* programmatic dependent-launch edges of the captured graphs: [lio, mesh] (0 while a handle has no captured graph); either
+ * handle may be NULL */
+int immesh_graph_pdl_edges(immesh_lio_t* lio, immesh_mesh_t* mesh, int64_t* out /*[2]*/);
 
 const char* immesh_last_error(void);
 const char* immesh_version(void);
