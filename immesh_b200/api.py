@@ -33,6 +33,16 @@ class _MeshCfg(C.Structure):
     ]
 
 
+class _EvalCfg(C.Structure):
+    _fields_ = [("sample_spacing", C.c_double), ("gt_leaf", C.c_double), ("threshold", C.c_double), ("max_dist", C.c_double),
+                ("incorrect_ratio", C.c_double), ("positions", C.c_int), ("pad", C.c_int), ("max_batch_bytes", C.c_int64)]
+
+
+EVAL_COUNT_KEYS = ("live_triangles", "degenerate", "samples", "gt_points", "samples_within", "gt_within", "samples_far", "gt_far",
+                   "incorrect_facets", "sum_q_samples", "sum_q_gt", "max_subdivisions")
+EVAL_METRIC_KEYS = ("maxmin_deg", "c2se", "accuracy", "completeness", "precision", "recall", "fscore")
+
+
 class _ImuCfg(C.Structure):
     _fields_ = [("cov_gyr", C.c_double * 3), ("cov_acc", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3),
                 ("mean_acc_norm", C.c_double), ("lid_R", C.c_double * 9), ("lid_T", C.c_double * 3), ("max_points", C.c_int), ("max_imu", C.c_int)]
@@ -158,6 +168,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_push_frame_batched", [vp, vp, C.c_int64, C.c_int, dp, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud_batched", [vp, vp, vp, C.c_int64, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_smooth_all", [vp, C.c_double, C.c_int, dp]),
+        ("immesh_mesh_evaluate", [vp, vp, C.c_int64, C.c_int, C.POINTER(_EvalCfg), C.POINTER(C.c_int64), dp, C.POINTER(C.c_int32), C.c_int64,
+                                  C.POINTER(C.c_int64)]),
+        ("immesh_mesh_evaluate_stats", [C.POINTER(C.c_int64)]),
         ("immesh_mesh_region_stream", [vp, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32), ip]),
         ("immesh_mesh_region_buffers", [vp, C.c_double, C.POINTER(C.c_int32), C.c_int, C.c_double, C.c_int, fp, C.POINTER(C.c_int32), C.c_int,
                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, fp, ip, ip, ip]),
@@ -701,6 +714,41 @@ class Mesh:
         nv = self.counts()["n_vertices"]
         out = np.zeros((nv, 3))
         _check(self.lib, self.lib.immesh_mesh_smooth_all(self._h, smooth_factor, knn, out.ctypes.data_as(C.POINTER(C.c_double))), "mesh_smooth_all")
+        return out
+
+    def evaluate(self, gt, *, spacing=0.01, gt_leaf=0.01, threshold=0.05, max_dist=1.0, incorrect_ratio=0.8, smoothed=False, facets=False,
+                 max_batch_bytes=0, on_device=False):
+        """The paper's Experiment-3 metrics of the mesh against the ground-truth cloud gt (float32[n,3] host array, or (CUDA address, n)
+        when on_device).  Returns dict(counts={EVAL_COUNT_KEYS: int}, metrics={EVAL_METRIC_KEYS: float}) and, with facets, rows
+        int32[live][5] = a b c n_samples n_far in ascending triple order.  smoothed: evaluate the smoothed positions (smooth_all first)."""
+        if on_device:
+            ptr, n = C.c_void_p(gt[0]), int(gt[1])
+        else:
+            a, p = _f32(np.asarray(gt).reshape(-1, 3))
+            ptr, n = C.cast(p, C.c_void_p), a.shape[0]
+        cfg = _EvalCfg(spacing, gt_leaf, threshold, max_dist, incorrect_ratio, 1 if smoothed else 0, 0, max_batch_bytes)
+        counts = np.zeros(12, dtype=np.int64)
+        metrics = np.zeros(8)
+        nr = C.c_int64(0)
+        i64 = C.POINTER(C.c_int64)
+        rows = None
+        if facets:   # a count query (cap_rows = 0) sizes the rows
+            dummy = np.zeros(5, dtype=np.int32)
+            rc = self.lib.immesh_mesh_evaluate(self._h, ptr, n, 1 if on_device else 0, C.byref(cfg), counts.ctypes.data_as(i64), metrics.ctypes.data_as(C.POINTER(C.c_double)),
+                                               dummy.ctypes.data_as(C.POINTER(C.c_int32)), 0, C.byref(nr))
+            if rc not in (0, -3):
+                _check(self.lib, rc, "mesh_evaluate")
+            rows = np.zeros((max(nr.value, 1), 5), dtype=np.int32)
+        _check(self.lib, self.lib.immesh_mesh_evaluate(self._h, ptr, n, 1 if on_device else 0, C.byref(cfg), counts.ctypes.data_as(i64),
+                                                       metrics.ctypes.data_as(C.POINTER(C.c_double)),
+                                                       rows.ctypes.data_as(C.POINTER(C.c_int32)) if facets else None, len(rows) if facets else 0,
+                                                       C.byref(nr)), "mesh_evaluate")
+        out = dict(counts=dict(zip(EVAL_COUNT_KEYS, (int(v) for v in counts))), metrics=dict(zip(EVAL_METRIC_KEYS, (float(v) for v in metrics[:7]))))
+        if facets:
+            out["rows"] = rows[:nr.value].copy()
+        st = np.zeros(4, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_mesh_evaluate_stats(st.ctypes.data_as(i64)), "mesh_evaluate_stats")
+        out["stats"] = dict(zip(("tiles", "plan_boxes", "scratch_bytes", "table_bytes"), (int(v) for v in st)))
         return out
 
     def region_stream(self, region_size=10.0, cap=1 << 16):

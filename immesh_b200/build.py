@@ -165,6 +165,17 @@ def build_changes(force=False):
                     extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")])
 
 
+EMU_EVAL = os.path.join(_ROOT, "tests", "eval", "libimmesh_emu_eval.so")
+
+
+def build_eval(force=False):
+    """tests/eval: the evaluation's per-element bodies (immesh_b200/csrc/mesh_eval.cuh) in a sequential host evaluator"""
+    src = os.path.join(_ROOT, "tests", "eval", "emu_eval.cpp")
+    if force or _newer(EMU_EVAL, [src, os.path.join(CSRC, "mesh_eval.cuh"), os.path.join(CSRC, "hd_math.cuh")]):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared", "-o", EMU_EVAL, src])
+    return EMU_EVAL
+
+
 DEV_MEM_DIR = os.path.join(_ROOT, "tests", "dev_mem")
 EMU_DEV_MEM = os.path.join(DEV_MEM_DIR, "libdev_mem_emu.so")
 
@@ -198,6 +209,7 @@ def build_all(force=False):
     build_imu_chain(force)
     build_reinforce(force)
     build_changes(force)
+    build_eval(force)
     build_dev_mem(force)
     build_ref()
 

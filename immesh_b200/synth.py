@@ -224,6 +224,24 @@ def make_scan(sensor: SensorModel, k: int, seed: int, ext_R: np.ndarray | None =
     return body, R, t
 
 
+def make_gt_cloud(kind: str, n_scans: int, seed: int = 0, n_points: int | None = None, ext_R=None, ext_T=None) -> np.ndarray:
+    """The noise-free world-frame hits of exactly the rays make_scan draws for scans 0 .. n_scans - 1 (the ground truth of
+    make_stream with the same arguments), float32[N,3] in scan order.  make_scan's random stream is replayed, not changed."""
+    sensor = make_sensor(kind, n_points)
+    eR = np.eye(3) if ext_R is None else np.asarray(ext_R, dtype=np.float64).reshape(3, 3)
+    eT = np.zeros(3) if ext_T is None else np.asarray(ext_T, dtype=np.float64)
+    out = []
+    for k in range(n_scans):
+        rng = np.random.default_rng([seed, k])
+        R, t = trajectory_pose(sensor, k)
+        d_w = sensor.directions(rng) @ (R @ eR).T
+        oL = R @ eT + t
+        rng_true = _raycast(oL, d_w, sensor.max_range)
+        ok = np.isfinite(rng_true) & (rng_true > sensor.blind)
+        out.append((oL + d_w[ok] * rng_true[ok, None]).astype(np.float32))
+    return np.concatenate(out) if out else np.zeros((0, 3), dtype=np.float32)
+
+
 def make_stream(kind: str, n_scans: int, seed: int = 0, leaf: float = 0.4, n_points: int | None = None,
                 ext_R=None, ext_T=None):
     """List of dicts with body_full, body_ds (voxel-grid down-sampled), R_true, t_true, dt."""

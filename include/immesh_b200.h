@@ -429,6 +429,67 @@ int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth /*[h][w] or NULL
 int immesh_mesh_changes_enable(immesh_mesh_t* h, int64_t max_rows, int max_frames);
 int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames /*[cap_frames][4]*/, int cap_frames, int32_t* rows /*[cap_rows][4]*/,
                         int64_t cap_rows, float* vertices /*[cap_vertices][3]*/, int64_t cap_vertices, int64_t* counts /*[4]*/);
+/* Evaluation of the mesh against a ground-truth cloud with the metrics of the ImMesh paper's Experiment-3 (section VIII-C, Tables V
+ * and VI, Fig. 8 and 9): fairness (mean Max-Min interior angle, mean circumradius-to-shortest-edge ratio) and correctness (accuracy,
+ * completeness, precision, recall, F-score between points sampled on the mesh and the down-sampled ground truth).
+ *   Positions: float32, the raw vertex positions (positions = 0, as immesh_mesh_snapshot) or (float) of the stored smoothed positions
+ *     (positions = 1, what save_to_ply_file writes with smooth_factor != 0).  positions = 1 with a vertex of a live triangle whose
+ *     m_smoothed flag is clear: IMMESH_E_INVALID ("smooth first"; immesh_mesh_smooth_all sets every flag).  The call smooths nothing.
+ *   Fairness, per live triangle in float64: the interior angles atan2(|u x v|, u . v) in degrees; C2SE = |a||b||c| / (2 |AB x AC|) /
+ *     shortest edge.  A triangle with |AB x AC| == 0 is degenerate: counted, left out of both means, and given no samples.
+ *   Mesh samples: with A < B < C the vertex ids and n = max(1, ceil(longest edge / sample_spacing)), the centroids of the n^2
+ *     sub-triangles of the n-subdivision: "up" at barycentrics ((3i+1)/(3n), (3j+1)/(3n)), i in [0, n), j in [0, n-i), and "down" at
+ *     ((3i+2)/(3n), (3j+2)/(3n)), j in [0, n-i-1); sample = (float)(A + (u (B-A) + v (C-A))) in float64 without FMA.  Every sample
+ *     lies inside exactly one facet: none is repeated along a shared edge.  A triangle that needs n > 2^15: IMMESH_E_RANGE.
+ *   Ground truth: gt_leaf > 0: leaf key floor((double)p / gt_leaf) (int64, per axis); every occupied leaf gives one point,
+ *     (float)(sum of (double)p / count) with the sum taken in input order.  There is no index-overflow pass-through (unlike
+ *     pcl::VoxelGrid): a 1 cm leaf over a city down-samples.  gt_leaf = 0: every point as given.  A non-finite point: IMMESH_E_INVALID.
+ *     At most 2^31 - 1 points per call (IMMESH_E_RANGE).
+ *   Distances: d = sqrt((dx dx + dy dy) + dz dz) in float64 from the float32 coordinates, the exact minimum over the other set's points
+ *     within max_dist (d <= max_dist).  A query with none takes d = max_dist and is "far".  d is quantised to q = rint(d 2^20) and
+ *     summed in int64 (q <= 2^30, at most 2^33 samples, else IMMESH_E_RANGE): the sums do not depend on order, batching or tiling and
+ *     compare exactly.  "Within" is d < threshold (strict).
+ *   counts [12]: live triangles, degenerate triangles, samples, ground-truth points after down-sampling, samples within, ground-truth
+ *     points within, far samples, far ground-truth points, incorrect facets, sum q over the samples, sum q over the ground truth,
+ *     subdivisions n of the largest triangle.
+ *   metrics [8] (float64): mean Max-Min angle (degrees), mean C2SE, accuracy (m) = sum q / 2^20 / samples, completeness (m) = sum q /
+ *     2^20 / ground-truth points, precision = samples within / samples, recall = ground-truth points within / ground-truth points,
+ *     F-score = 2 P R / (P + R) (0 when P + R = 0), 0 (spare).  A mean over an empty set is NaN (and so is an F-score with one).
+ *     Accuracy and completeness are lower bounds when the far counts are non-zero: a far query counts max_dist, not its distance.
+ *   facet_rows [cap_rows][5] (or NULL: none): one row a b c n_samples n_far per live triangle in ascending (a, b, c) order (the change
+ *     feed's order), n_far = its samples not within threshold.  A facet is incorrect (paper Fig. 8) when n_samples > 0 and
+ *     n_far >= incorrect_ratio * n_samples.  *n_rows (or NULL) = live triangles.  facet_rows given and cap_rows below the live count:
+ *     IMMESH_E_CAPACITY before any work, nothing else written (cap_rows = 0: the count query).
+ *   Contract: blocks; drains the frames queued on h first, those of immesh_mesh_push_frame_from_lio_async included.  Changes nothing
+ *     on the handle (vertices, flags, smoothed positions, counters, captured graphs).  The ground truth is read in place (on_device = 1,
+ *     a device pointer) or copied to the device once.  Every other device buffer is allocated by the call and freed before it returns,
+ *     at most max_batch_bytes in all (0: 2 GiB): one block for the table (about 110 bytes per live triangle, 130 with the rows), then one
+ *     block the size of the largest tile's scratch, reused by every tile.  A tile is a box of the bisected bounding box; its scratch holds
+ *     the samples and ground-truth points of the box grown by max_dist, with their hashed grids.  Tiles are halved until each fits
+ *     what the table leaves of the budget.  A budget too small for the table, or for a tile that cannot be halved further (side
+ *     max(max_dist / 4, 2 grid cells)): IMMESH_E_CAPACITY, naming it.  A configuration whose smallest tile would span more than
+ *     2^21 - 4 grid cells or ground-truth leaves per axis (gt_leaf far below max_dist, or coordinates beyond about 10^6 m):
+ *     IMMESH_E_RANGE before any tile is processed.
+ *   immesh_mesh_evaluate_stats(out[4]): what the calling thread's last immesh_mesh_evaluate that got past its argument checks did:
+ *     tiles processed, boxes counted by the tile planner, device scratch bytes (table + tile block, the ground-truth copy excluded),
+ *     table bytes.
+ *   IMMESH_E_INVALID: NULL h, cfg, counts or metrics; sample_spacing <= 0; gt_leaf < 0; not 0 < threshold <= max_dist <= 1024;
+ *     incorrect_ratio outside (0, 1]; positions not 0 or 1; max_batch_bytes < 0; n_gt < 0 or gt_xyz NULL with n_gt > 0; a non-finite
+ *     configuration value; a sharded handle. */
+typedef struct {
+    double sample_spacing;    /* mesh sampling step (paper: 0.01 m), > 0 */
+    double gt_leaf;           /* ground-truth down-sampling leaf (paper: 0.01 m); 0 = every point as given */
+    double threshold;         /* precision / recall / correct-sample distance (paper: 0.05 m), > 0 */
+    double max_dist;          /* nearest-neighbour search radius, threshold <= max_dist <= 1024 */
+    double incorrect_ratio;   /* facet incorrect when n_far >= ratio * n_samples (paper Fig. 8: 0.8), in (0, 1] */
+    int positions;            /* 0: raw vertex positions (immesh_mesh_snapshot); 1: smoothed (what save_to_ply_file writes, smooth_factor != 0) */
+    int pad;
+    int64_t max_batch_bytes;  /* scratch budget of the call beyond the ground-truth copy; 0 = a default (2 GiB) */
+} immesh_eval_config;
+int immesh_mesh_evaluate(immesh_mesh_t* h, const float* gt_xyz /*[n_gt][3]*/, int64_t n_gt, int on_device, const immesh_eval_config* cfg,
+                         int64_t* counts /*[12]*/, double* metrics /*[8]*/, int32_t* facet_rows /*[cap_rows][5] or NULL*/, int64_t cap_rows,
+                         int64_t* n_rows /*or NULL*/);
+int immesh_mesh_evaluate_stats(int64_t* out /*[4]*/);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
