@@ -146,6 +146,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_lio_capacity", [vp, C.POINTER(C.c_int64)]),
         ("immesh_lio_reserve", [vp, C.c_int64, C.c_int64, C.c_int64]),
         ("immesh_lio_set_growth", [vp, C.c_int64]),
+        ("immesh_lio_local_map", [vp, C.c_double, C.c_float, C.c_float]),
+        ("immesh_voxelmap_evict_boxes", [vp, fp, C.c_int]),
+        ("immesh_lio_local_map_state", [vp, fp, C.POINTER(C.c_int64)]),
         ("immesh_mesh_capacity", [vp, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reserve", [vp, C.c_int64, C.c_int64, C.c_int64]),
         ("immesh_mesh_set_growth", [vp, C.c_int64]),
@@ -501,6 +504,28 @@ class Lio:
     def set_growth(self, max_bytes):
         """Automatic growth before every step, up to max_bytes of device memory for the handle (0: off)."""
         _check(self.lib, self.lib.immesh_lio_set_growth(self._h, max_bytes), "lio_set_growth")
+
+    # --- long runs: the local map (a cube that follows the sensor; root voxels it leaves behind are evicted)
+    def local_map(self, cube_len, det_range=300.0, mov_threshold=1.5):
+        """Turn the automatic local map on (cube_len: the reference's cube_side_length) or off (cube_len = 0).  Drains the handle;
+        the box is placed at the next evaluation (once per scan, before its IESKF)."""
+        _check(self.lib, self.lib.immesh_lio_local_map(self._h, float(cube_len), float(det_range), float(mov_threshold)), "lio_local_map")
+
+    def evict_boxes(self, boxes):
+        """Evict the root voxels whose centre lies in one of the boxes, float32[n, 6] rows min xyz, max xyz (half-open
+        min <= c < max); queued behind the steps already queued."""
+        a = np.ascontiguousarray(np.asarray(boxes, dtype=np.float32).reshape(-1, 6))
+        _check(self.lib, self.lib.immesh_voxelmap_evict_boxes(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0]), "voxelmap_evict_boxes")
+
+    def local_map_state(self):
+        """(box float32[6] min xyz, max xyz, dict(placed, moves, roots_evicted, nodes_freed, chunks_freed, tombstones, rebuilds,
+        free_nodes)); blocking."""
+        box = np.zeros(6, dtype=np.float32)
+        o = np.zeros(8, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_lio_local_map_state(self._h, box.ctypes.data_as(C.POINTER(C.c_float)), o.ctypes.data_as(C.POINTER(C.c_int64))),
+               "lio_local_map_state")
+        keys = ("placed", "moves", "roots_evicted", "nodes_freed", "chunks_freed", "tombstones", "rebuilds", "free_nodes")
+        return box, dict(zip(keys, (int(v) for v in o)))
 
 
 class Mesh:

@@ -176,6 +176,18 @@ def build_eval(force=False):
     return EMU_EVAL
 
 
+LOCAL_MAP_DIR = os.path.join(_ROOT, "tests", "local_map")
+EMU_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "libimmesh_emu_local_map.so")
+ORACLE_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "liborc_local_map.so")
+
+
+def build_local_map(force=False):
+    """tests/local_map: the host emulation with the local map's box rule, eviction sweep and purge (immesh_b200/csrc/local_map.cuh),
+    and the oracle extended by laser_map_fov_segment and the deletion of the boxes it leaves behind"""
+    return (_emu_ext(os.path.join(LOCAL_MAP_DIR, "emu_local_map.cpp"), EMU_LOCAL_MAP, force),
+            _oracle_ext(os.path.join(LOCAL_MAP_DIR, "orc_local_map.cpp"), ORACLE_LOCAL_MAP, force))
+
+
 DEV_MEM_DIR = os.path.join(_ROOT, "tests", "dev_mem")
 EMU_DEV_MEM = os.path.join(DEV_MEM_DIR, "libdev_mem_emu.so")
 
@@ -210,6 +222,7 @@ def build_all(force=False):
     build_reinforce(force)
     build_changes(force)
     build_eval(force)
+    build_local_map(force)
     build_dev_mem(force)
     build_ref()
 

@@ -95,6 +95,12 @@ struct immesh_lio {
     long long map_steps = 0;      // map-growing steps queued so far
     long long slot_step[IM_SLOTS] = {};   // number of the step that used staging slot s
     int max_step_nodes = 0, max_step_chunks = 0;   // largest node / chunk use between two noted steps (finished blocks are noted in step order)
+    // local map (immesh_lio_local_map / immesh_voxelmap_evict_boxes); map.node_free is allocated by the first of them, in `dev`
+    int lm_on = 0;                // the box rule and the eviction sweep are queued with every step
+    long long lm_purges = 0;      // rebuilds of the root hash that dropped tombstones (lio_purge_check)
+    int tombs_known = 0;          // tombstones after the last step known to have finished
+    float* d_lm_boxes = nullptr;  // the caller's boxes of immesh_voxelmap_evict_boxes, in `scratch`
+    size_t lm_boxes_cap = 0;
 };
 
 // the device buffers of one depth image of the tiled rasteriser (mesh_capi.cu: rf_image_alloc, rf_image_launch): the camera, the tile

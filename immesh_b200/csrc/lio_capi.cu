@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -592,6 +593,41 @@ __global__ void __launch_bounds__(GROW_THREADS) k_remap_roots(VoxelMapDev to, in
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_pub; i += gridDim.x * blockDim.x) remap_pub_entry(from_pub_list, to, i, slot_map);
 }
 
+// ---- local map (local_map.cuh).  k_local_map_box: one thread evaluates laser_map_fov_segment at the state the scan's IESKF starts
+// from (automatic = 1, gated by LocalMapCtrl::on), after clamping the node free stack's top that the previous scan's pops may have
+// left negative (before any push).  k_evict_roots: a grid-stride sweep over the hash slots against this scan's removal boxes (or
+// the caller's, immesh_voxelmap_evict_boxes); it leaves at once when there are none.
+__global__ void k_local_map_box(LioCtrl* ctrl, int* node_free_top, int automatic) {
+    pdl_wait();
+    if (threadIdx.x == 0) {
+        if (*node_free_top < 0) *node_free_top = 0;
+        LocalMapCtrl& L = ctrl->lm;
+        L.n_rm = 0;
+        if (automatic && L.on) local_map_rule(L, ctrl->state + 9);   // pos_end
+    }
+    pdl_trigger();
+}
+#define EVICT_THREADS 256
+__global__ void __launch_bounds__(EVICT_THREADS) k_evict_roots(VoxelMapDev map, LioCtrl* ctrl, const float* boxes, int n_boxes) {
+    pdl_wait();
+    if (!boxes) { boxes = &ctrl->lm.rm[0][0]; n_boxes = ctrl->lm.n_rm; }
+    if (n_boxes <= 0) return;
+    const unsigned int cap = map.cap_mask + 1u;
+    unsigned long long roots = 0, nodes = 0, chunks = 0;
+    for (unsigned int s = blockIdx.x * blockDim.x + threadIdx.x; s < cap; s += gridDim.x * blockDim.x) {
+        int nn, nc;
+        roots += evict_root_slot(map, s, boxes, n_boxes, &nn, &nc);
+        nodes += nn;
+        chunks += nc;
+    }
+    if (roots) {
+        atomicAdd(&ctrl->lm.roots, roots);
+        atomicAdd(&ctrl->lm.nodes, nodes);
+        atomicAdd(&ctrl->lm.chunks, chunks);
+    }
+    pdl_trigger();
+}
+
 // ------------------------------------------------------------------ host side
 
 #include "nccl_api.hpp"
@@ -688,6 +724,8 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     IM_CUDA(h->dev.alloc(&m.pub_mark, h->cap, 0));
     IM_CUDA(h->dev.alloc(&m.pub_list, h->cap));
     m.pub_n = h->d_counters + IM_LC_PUB_N;
+    m.node_free = nullptr;   // allocated by the first immesh_lio_local_map / immesh_voxelmap_evict_boxes
+    m.node_free_top = h->d_counters + IM_LC_NODE_FREE; m.n_tombs = h->d_counters + IM_LC_TOMBS;
     ScanBuf& sb = h->sb;
     const size_t ms = (size_t)h->max_scan;
     float* d_body = nullptr;
@@ -765,6 +803,8 @@ int immesh_lio_shard(immesh_lio_t* h, int rank, int nranks, const char* unique_i
     if (nranks > IM_MAX_RANKS) return im_fail(IMMESH_E_INVALID, "at most 8 ranks (one node)");
     if (nranks == 1) { h->P.shard_rank = 0; h->P.shard_n = 1; return IMMESH_OK; }
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a handle with automatic growth cannot be sharded (immesh_lio_set_growth(h, 0) first)");
+    if (h->lm_on || h->map.node_free)   // its tombstones would need a rebuild of the table, which a sharded handle cannot do
+        return im_fail(IMMESH_E_INVALID, "a handle that used the local map (immesh_lio_local_map / immesh_voxelmap_evict_boxes) cannot be sharded");
     if (!nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -895,6 +935,7 @@ static cudaError_t lio_read_counters(const immesh_lio* h, int* c) {
 static int check_flags(immesh_lio* h) {
     IM_CUDA(cudaMemcpyAsync(h->h_ints, h->d_counters, IM_LC_SIZE * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaStreamSynchronize(h->stream));
+    h->tombs_known = h->h_ints[IM_LC_TOMBS];
     if (h->grow_max_bytes > 0) note_counters(h, h->h_ints, h->map_steps);
     return lio_flags_status(h->h_ints[IM_LC_ERR]);
 }
@@ -914,15 +955,16 @@ static size_t pool_bytes(long long cap, long long nodes, long long chunks) {
 // Enlarge the pools to (cap slots, nodes, chunks), each >= the current one.  Drains the handle's stream; allocates every new
 // buffer before anything is touched, so that a failure (allocation, ceiling, id limits) leaves the handle as it was; migrates on
 // the stream; frees the old buffers after the migration and drops the captured launch sequence (it holds the old pointers).
-static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chunks) {
+static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chunks, bool rehash = false) {
     if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "a sharded handle cannot grow (its replicas would have to grow in lockstep)");
     const long long cap0 = (long long)h->cap, nodes0 = h->max_nodes, chunks0 = h->max_chunks;
     if (cap > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "root hash: more than 2^30 slots (32-bit slot ids)");
     if (nodes > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "node pool: more than 2^30 node records (32-bit node ids)");
     if (chunks > IM_POOL_LIMIT) return im_fail(IMMESH_E_CAPACITY, "chunk pool: more than 2^30 chunks (32-bit chunk ids)");
-    const bool g_cap = cap > cap0, g_nodes = nodes > nodes0, g_chunks = chunks > chunks0;
+    const bool g_cap = cap > cap0 || rehash, g_nodes = nodes > nodes0, g_chunks = chunks > chunks0;   // rehash: the table at its size
     if (!g_cap && !g_nodes && !g_chunks) return IMMESH_OK;
-    const size_t bytes = h->dev.bytes() - pool_bytes(cap0, nodes0, chunks0) + pool_bytes(cap, nodes, chunks);
+    size_t bytes = h->dev.bytes() - pool_bytes(cap0, nodes0, chunks0) + pool_bytes(cap, nodes, chunks);
+    if (h->map.node_free) bytes += (size_t)(nodes - nodes0) * sizeof(int);   // the local map's node free stack follows the node pool
     if (h->grow_max_bytes > 0 && bytes > (size_t)h->grow_max_bytes) {
         const std::string pools = std::string(g_cap ? " root hash" : "") + (g_nodes ? " node pool" : "") + (g_chunks ? " chunk pool" : "");
         return im_fail(IMMESH_E_CAPACITY, ("growth of the" + pools + " to " + std::to_string(bytes) + " device bytes is above the ceiling of " +
@@ -934,6 +976,8 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     const int n_nodes = std::min(c[IM_LC_NODES], h->max_nodes), n_chunks = std::min(c[IM_LC_CHUNK_BUMP], h->max_chunks);
     const int n_avail = std::max(0, std::min(c[IM_LC_AVAIL_TOP], h->max_chunks)), n_pending = std::min(c[IM_LC_PENDING], h->max_chunks);
     const int n_pub = std::min<long long>(c[IM_LC_PUB_N], cap0);
+    const int n_free = std::max(0, std::min(c[IM_LC_NODE_FREE], h->max_nodes));
+    const bool had_tombs = c[IM_LC_TOMBS] > 0;
 
     VoxelMapDev nm = h->map;   // the map after the growth
     ScanBuf nsb = h->sb;
@@ -944,6 +988,7 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     if (g_nodes && e == cudaSuccess) {
         pool = "node pool";
         if ((e = fresh.alloc(&nm.nodes, nodes)) == cudaSuccess && (e = fresh.alloc(&nm.planes, nodes)) == cudaSuccess) e = fresh.alloc(&nm.pub, nodes);
+        if (e == cudaSuccess && h->map.node_free) e = fresh.alloc(&nm.node_free, nodes);
     }
     if (g_chunks && e == cudaSuccess) {
         pool = "chunk pool";
@@ -970,6 +1015,7 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
             MG(cudaMemcpyAsync(nm.planes, h->map.planes, (size_t)n_nodes * sizeof(PlaneRec), cudaMemcpyDeviceToDevice, st));
             MG(cudaMemcpyAsync(nm.pub, h->map.pub, (size_t)n_nodes * sizeof(PubRec), cudaMemcpyDeviceToDevice, st));
         }
+        if (g_nodes && nm.node_free && n_free > 0) MG(cudaMemcpyAsync(nm.node_free, h->map.node_free, (size_t)n_free * sizeof(int), cudaMemcpyDeviceToDevice, st));
         if (g_chunks) {
             if (n_chunks > 0) MG(cudaMemcpyAsync(nm.chunks, h->map.chunks, (size_t)n_chunks * sizeof(Chunk), cudaMemcpyDeviceToDevice, st));
             if (n_avail > 0) MG(cudaMemcpyAsync(nm.avail, h->map.avail, (size_t)n_avail * sizeof(int), cudaMemcpyDeviceToDevice, st));
@@ -986,9 +1032,18 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
             // with the node pool kept, root_slot is rewritten in place: the last step of the migration, after every allocation succeeded
             const int gn = (int)std::min<long long>((std::max(n_nodes, n_pub) + GROW_THREADS - 1) / GROW_THREADS + 1, (long long)h->n_sm * 16);
             IM_LAUNCH(k_remap_roots, gn, GROW_THREADS, 0, st, nm, n_nodes, (const int*)h->map.pub_list, n_pub, (const int*)slot_map);
+            MG(cudaMemsetAsync(nm.n_tombs, 0, sizeof(int), st));   // the rebuilt table holds no tombstone
         }
         MG(cudaGetLastError());
         MG(cudaStreamSynchronize(st));
+        if (g_cap && had_tombs && n_pub > 0) {
+            // pending plane-marker entries of evicted roots were remapped to -1: the list keeps the others, in order
+            std::vector<int> lst(n_pub);
+            MG(cudaMemcpy(lst.data(), nm.pub_list, (size_t)n_pub * sizeof(int), cudaMemcpyDeviceToHost));
+            const int kept = (int)(std::remove(lst.begin(), lst.end(), -1) - lst.begin());
+            if (kept > 0) MG(cudaMemcpy(nm.pub_list, lst.data(), (size_t)kept * sizeof(int), cudaMemcpyHostToDevice));
+            MG(cudaMemcpy(nm.pub_n, &kept, sizeof(int), cudaMemcpyHostToDevice));
+        }
 #undef MG
         return r;
     };
@@ -997,7 +1052,7 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
         return immesh::im_fail_cuda(e, __FILE__, __LINE__);
     }
     // the replaced buffers go; the new ones join the handle's device memory
-    if (g_nodes) { h->dev.free(h->map.nodes); h->dev.free(h->map.planes); h->dev.free(h->map.pub); }
+    if (g_nodes) { h->dev.free(h->map.nodes); h->dev.free(h->map.planes); h->dev.free(h->map.pub); if (h->map.node_free) h->dev.free(h->map.node_free); }
     if (g_chunks) { h->dev.free(h->map.chunks); h->dev.free(h->map.avail); h->dev.free(h->map.pending); }
     if (g_cap) {
         for (const void* p : {(const void*)h->map.keys, (const void*)h->map.root_node, (const void*)h->map.pub_mark, (const void*)h->map.pub_list,
@@ -1012,7 +1067,8 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
     h->cap = (size_t)cap;
     h->max_nodes = (int)nodes;
     h->max_chunks = (int)chunks;
-    h->growths++;
+    if (cap > cap0 || g_nodes || g_chunks) h->growths++;
+    if (g_cap) h->tombs_known = 0;
     h->graph.destroy();   // the next pipelined step captures the launch sequence again, with the new pointers
     IM_CUDA(cudaGetLastError());
     return IMMESH_OK;
@@ -1020,7 +1076,30 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
 // Automatic growth (immesh_lio_set_growth) before a step of n points is queued: growth_targets (pool_growth.cuh) on the use of the
 // last step known to have finished, without waiting for the others.  Only when a pool is short is the handle drained; the decision
 // is then taken again on its exact counters.
+// Purge of the local map's tombstones before a step: when the last finished step left more than an eighth of the root hash's slots
+// as tombstones, the handle is drained and the table rebuilt at its size through the growth's rehash, which drops them (hash_find
+// walks a probe chain that tombstones only lengthen).  Independent of immesh_lio_set_growth.
+static int lio_purge_check(immesh_lio* h) {
+    if (!h->map.node_free) return IMMESH_OK;   // nothing was ever evicted
+    long long newest = -1;
+    for (int s = 0; s < IM_SLOTS; ++s)
+        if (h->slot_busy[s] && h->slot_step[s] > newest && cudaEventQuery(h->ev_slot[s]) == cudaSuccess) {
+            newest = h->slot_step[s];
+            h->tombs_known = h->h_out[s].counters[IM_LC_TOMBS];
+        }
+    cudaGetLastError();   // cudaErrorNotReady of the queries
+    if ((long long)h->tombs_known * 8 <= (long long)h->cap) return IMMESH_OK;
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    IM_CUDA(lio_read_counters(h, h->h_ints));
+    h->tombs_known = h->h_ints[IM_LC_TOMBS];
+    if ((long long)h->tombs_known * 8 <= (long long)h->cap) return IMMESH_OK;
+    const int rc = lio_grow(h, (long long)h->cap, h->max_nodes, h->max_chunks, true);
+    if (rc == IMMESH_OK) h->lm_purges++;
+    return rc;
+}
 static int lio_growth_check(immesh_lio* h, long long n) {
+    const int prc = lio_purge_check(h);
+    if (prc) return prc;
     if (h->grow_max_bytes <= 0) return IMMESH_OK;
     long long steps = 1, n_max = n;
     note_slots(h, true);
@@ -1044,6 +1123,12 @@ static int lio_growth_check(immesh_lio* h, long long n) {
         n_max = n;
     }
     return IMMESH_OK;
+}
+// the local map's two launches: the box rule (boxes == null; gated on the device by LocalMapCtrl::on) or the caller's boxes, then the
+// eviction sweep.  pdl as in launch_grow.
+static void launch_local_map(immesh_lio* h, const float* boxes = nullptr, int n_boxes = 0, bool pdl = false) {
+    IM_LAUNCH_PDL(pdl, k_local_map_box, 1, 32, 0, h->stream, h->d_ctrl, h->map.node_free_top, boxes ? 0 : 1);
+    IM_LAUNCH_PDL(pdl, k_evict_roots, grid_fixed(h, EVICT_THREADS), EVICT_THREADS, 0, h->stream, h->map, h->d_ctrl, boxes, n_boxes);
 }
 // resident blocks per SM of the persistent per-voxel map update k_grow_voxel (headroom for the kernels on the other streams)
 #define GROW_VOXEL_BPS 4
@@ -1122,6 +1207,7 @@ int immesh_voxelmap_build(immesh_lio_t* h, const float* body, int n) {
     if (rc) return rc;
     h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
     ++h->map_steps;
+    if (h->lm_on) launch_local_map(h);   // places the box at the building scan's pose
     launch_grow(h, 1);
     IM_CUDA(cudaGetLastError());
     return check_flags(h);
@@ -1133,6 +1219,7 @@ int immesh_lio_estimate(immesh_lio_t* h, const float* body, int n, int* iters_ru
     h->win.epoch += IM_MAX_ITER + 1;   // epoch base of this scan (same sequence of calls on every rank)
     int rc = upload_scan(h, body, n);
     if (rc) return rc;
+    if (h->lm_on) launch_local_map(h);
     rc = launch_estimate(h);
     if (rc) return rc;
     h->scan_rows = 1;
@@ -1181,11 +1268,12 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     bool queued = false;
     int lrc = IMMESH_OK;
     if (!timing) {
-        const unsigned sig = 1u | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
+        const unsigned sig = 1u | (h->lm_on ? 4u : 0u) | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
         // one GPU: every kernel after k_predict is a programmatic dependent launch (the sharded paths wait on peers and NCCL)
         const bool pdl = h->P.shard_n <= 1;
         queued = immesh::run_graphed_static(h->graph, sig, h->stream, [&] {
             IM_LAUNCH(k_predict, 1, PREDICT_THREADS, 0, h->stream, h->d_ctrl);
+            if (h->lm_on) launch_local_map(h, nullptr, 0, pdl);
             lrc = launch_estimate(h, pdl);
             launch_grow(h, 0, pdl);
         }) == cudaSuccess;
@@ -1194,6 +1282,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     if (!queued) {
         if (!timing) IM_CUDA(cudaEventRecord(h->ev[0], h->stream));
         IM_LAUNCH(k_predict, 1, PREDICT_THREADS, 0, h->stream, h->d_ctrl);
+        if (h->lm_on) launch_local_map(h);
         IM_CUDA(cudaEventRecord(h->ev[1], h->stream));
         lrc = launch_estimate(h);
         IM_CUDA(cudaEventRecord(h->ev[2], h->stream));
@@ -1219,6 +1308,7 @@ static int lio_wait_impl(immesh_lio_t* h, double* state_out, int* iters_run, boo
     for (int i = 0; i < IM_SLOTS; ++i) h->slot_busy[i] = 0;
     if (profiler().enabled) profiler().collect();
     const LioOut& o = h->h_out[s];
+    h->tombs_known = o.counters[IM_LC_TOMBS];
     if (state_out) std::memcpy(state_out, o.state, IM_STATE_DOUBLES * sizeof(double));
     if (iters_run) *iters_run = o.iters_run;
     if (timings && h->timed_last) {
@@ -1266,6 +1356,7 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     ++h->map_steps;
     int rc = upload_scan(h, d_body_xyz, n, 1, s);
     if (rc) return rc;
+    if (h->lm_on) launch_local_map(h);   // places the box at the building scan's pose
     launch_grow(h, 1);
     h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
     IM_CUDA(cudaGetLastError());
@@ -1630,6 +1721,75 @@ int immesh_lio_set_growth(immesh_lio_t* h, int64_t max_bytes) {
         note_counters(h, h->h_ints, ++h->map_steps);   // the map as it is now, under a step number of its own
     }
     h->grow_max_bytes = max_bytes;
+    return IMMESH_OK;
+}
+
+// ---- local map (local_map.cuh)
+// the node free stack, allocated once: from then on alloc_node pops it first (the captured launch sequence holds the map: dropped)
+static int lio_node_free_alloc(immesh_lio* h) {
+    if (h->map.node_free) return IMMESH_OK;
+    IM_CUDA(h->dev.alloc(&h->map.node_free, (size_t)h->max_nodes));
+    h->graph.destroy();
+    return IMMESH_OK;
+}
+int immesh_lio_local_map(immesh_lio_t* h, double cube_len, float det_range, float mov_threshold) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_local_map: the local map runs on a single GPU: the handle is sharded");
+    const bool on = cube_len != 0.0;
+    if (on && !(std::isfinite(cube_len) && cube_len > 0 && std::isfinite(det_range) && det_range > 0 && std::isfinite(mov_threshold) && mov_threshold > 0))
+        return im_fail(IMMESH_E_INVALID, "immesh_lio_local_map: cube_len, det_range and mov_threshold must be finite and positive (cube_len = 0 turns the local map off)");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    if (on) {
+        const int rc = lio_node_free_alloc(h);
+        if (rc) return rc;
+    }
+    LocalMapCtrl L;
+    IM_CUDA(cudaMemcpy(&L, &h->d_ctrl->lm, sizeof(L), cudaMemcpyDeviceToHost));
+    L.cube_len = on ? cube_len : 0.0;
+    L.det_range = on ? det_range : 0.f;
+    L.mov_threshold = on ? mov_threshold : 0.f;
+    L.on = on ? 1 : 0;
+    L.placed = 0;   // the box is placed at the next evaluation
+    L.n_rm = 0;
+    IM_CUDA(cudaMemcpy(&h->d_ctrl->lm, &L, sizeof(L), cudaMemcpyHostToDevice));
+    if (h->lm_on != (on ? 1 : 0)) h->graph.destroy();   // the launch sequence changes
+    h->lm_on = on ? 1 : 0;
+    return IMMESH_OK;
+}
+int immesh_voxelmap_evict_boxes(immesh_lio_t* h, const float* boxes, int n) {
+    if (!h || n < 0 || (n > 0 && !boxes)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_voxelmap_evict_boxes: the handle is sharded");
+    for (int i = 0; i < 6 * n; ++i)
+        if (std::isnan(boxes[i])) return im_fail(IMMESH_E_INVALID, "immesh_voxelmap_evict_boxes: a box edge is NaN");
+    if (n == 0) return IMMESH_OK;
+    if (!h->map.node_free) {
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        const int rc = lio_node_free_alloc(h);
+        if (rc) return rc;
+    }
+    // the device copy of the boxes is reused by every call: a queued sweep must not see it freed by a regrow (drain first)
+    if ((size_t)n * 6 > h->lm_boxes_cap) IM_CUDA(cudaStreamSynchronize(h->stream));
+    IM_CUDA(h->scratch.regrow(&h->d_lm_boxes, &h->lm_boxes_cap, (size_t)n * 6, 64));
+    // staged through a host copy of the library's own (pageable) memory: the copy from pageable memory has read its source when it
+    // returns, so the caller may reuse `boxes` at once whatever memory they are in (a pinned source would still be read later)
+    const std::vector<float> staged(boxes, boxes + (size_t)n * 6);
+    IM_CUDA(cudaMemcpyAsync(h->d_lm_boxes, staged.data(), staged.size() * sizeof(float), cudaMemcpyHostToDevice, h->stream));
+    launch_local_map(h, h->d_lm_boxes, n);   // queued behind the handle's steps
+    IM_CUDA(cudaGetLastError());
+    return IMMESH_OK;
+}
+int immesh_lio_local_map_state(immesh_lio_t* h, float* box, int64_t* stats) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    LocalMapCtrl L;
+    IM_CUDA(cudaMemcpy(&L, &h->d_ctrl->lm, sizeof(L), cudaMemcpyDeviceToHost));
+    int c[IM_LC_SIZE];
+    IM_CUDA(lio_read_counters(h, c));
+    if (box) for (int k = 0; k < 6; ++k) box[k] = L.box[k];
+    if (stats) {
+        stats[0] = L.placed; stats[1] = (int64_t)L.moves; stats[2] = (int64_t)L.roots; stats[3] = (int64_t)L.nodes; stats[4] = (int64_t)L.chunks;
+        stats[5] = c[IM_LC_TOMBS]; stats[6] = h->lm_purges; stats[7] = std::max(c[IM_LC_NODE_FREE], 0);
+    }
     return IMMESH_OK;
 }
 

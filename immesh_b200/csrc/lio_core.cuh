@@ -7,7 +7,7 @@
 // The bodies are __host__ __device__ so that tests/emu can execute the very same source on the
 // CPU (single lane / single thread) for logic tests; the product only ever runs them on the GPU.
 #pragma once
-#include "voxelmap.cuh"
+#include "local_map.cuh"
 
 #if defined(__CUDA_ARCH__)
 #define IM_SYNCBLOCK() __syncthreads()
@@ -58,6 +58,9 @@ enum : int {
     IM_LC_REFIT_POINTS = 10, // VoxelMapDev::stat[1]: points read by the refits; k_grow_finish
     IM_LC_COMPLEX = 11,      // touched root voxels left to k_grow_voxel (k_grow_simple); k_grow_finish
     IM_LC_PUB_N = 12,        // VoxelMapDev::pub_n: entries of the plane-map publisher's pending list; immesh_voxelmap_plane_markers
+    IM_LC_NODE_FREE = 13,    // VoxelMapDev::node_free_top: node records on the free stack (evict_root_slot, alloc_node; may be negative
+                             // after a scan's pops, clamped by k_local_map_box); never reset
+    IM_LC_TOMBS = 14,        // VoxelMapDev::n_tombs: tombstones in the root hash (evict_root_slot); zeroed by a rebuild of the table
     IM_LC_SIZE = 16,         // ints allocated, read back and copied into LioOut::counters
 };
 
@@ -86,6 +89,7 @@ struct LioCtrl {
     int blocks_done[IM_MAX_ITER];  // residual blocks that have published their sums (the last one runs the solve)
     int shard_cnt[2];              // peer-window exchange: blocks of pass 1 / pass 2 that have finished (reset by the last one)
     int pad2_[2];
+    LocalMapCtrl lm;               // local map (local_map.cuh)
 };
 
 struct ScanBuf {

@@ -18,7 +18,7 @@ namespace immesh {
 // old slot s of `from` into `to`; slot_map[s] = its new slot (-1: empty, or `to` full, with IM_ERR_HASH_FULL raised)
 IM_HD void rehash_root_slot(const VoxelMapDev& from, const VoxelMapDev& to, unsigned int s, int* slot_map) {
     const unsigned long long key = from.keys[s];
-    if (key == IM_EMPTY_KEY) { slot_map[s] = -1; return; }
+    if (key >> 63) { slot_map[s] = -1; return; }   // empty, or a tombstone of the local map (dropped)
     int created = 0;
     const int ns = hash_insert(to, key, &created);
     slot_map[s] = ns;
@@ -29,7 +29,7 @@ IM_HD void rehash_root_slot(const VoxelMapDev& from, const VoxelMapDev& to, unsi
 // node nd of the (copied) pool in `to`: its root's slot in the rebuilt table
 IM_HD void remap_node_root_slot(const VoxelMapDev& to, int nd, const int* slot_map) {
     NodeRec& n = to.nodes[nd];
-    n.root_slot = slot_map[n.root_slot];
+    if (n.root_slot >= 0) n.root_slot = slot_map[n.root_slot];   // < 0: a record freed with an evicted root
 }
 // entry i of the plane-map publisher's pending list
 IM_HD void remap_pub_entry(const int* from_list, const VoxelMapDev& to, int i, const int* slot_map) {
@@ -77,14 +77,16 @@ IM_HD void rehash_tri_slot(const MeshDev& from, const MeshDev& to, unsigned int 
 // Automatic growth (immesh_lio_set_growth): the capacities the next `steps` steps need (the steps still in flight and the one
 // being queued), each of at most n_max points, from the counters c (IM_LC_* slots) of the last step known to have finished.
 // *cap, *nodes, *chunks hold the current capacities on entry; a pool is doubled until
-//   root hash : load factor <= 1/2 after the steps, each adding at most n_max roots (one per point at most: a sound bound)
-//   nodes     : free >= max(capacity / 4, steps x max(2 x the largest per-step use seen, n_max))
+//   root hash : load factor <= 1/2 after the steps, each adding at most n_max roots (one per point at most: a sound bound); the
+//               local map's tombstones count as occupied slots
+//   nodes     : free >= max(capacity / 4, steps x max(2 x the largest per-step use seen, n_max)), with nodes in use =
+//               node_count - the records on the local map's node free stack
 //   chunks    : the same, with chunks in use = chunk_bump - avail_top
 // The node and chunk bounds are not sound (a plane fit that splits a node redistributes its points): a step that overflows anyway
 // returns IMMESH_E_CAPACITY as it does without growth.
 inline void growth_targets(const int* c, long long steps, long long n_max, int max_step_nodes, int max_step_chunks, long long* cap,
                            long long* nodes, long long* chunks) {
-    while ((c[IM_LC_ROOTS] + steps * n_max) * 2 > *cap) *cap *= 2;
+    while (((long long)c[IM_LC_ROOTS] + c[IM_LC_TOMBS] + steps * n_max) * 2 > *cap) *cap *= 2;
     const long long per_node = 2LL * max_step_nodes > n_max ? 2LL * max_step_nodes : n_max;
     const long long per_chunk = 2LL * max_step_chunks > n_max ? 2LL * max_step_chunks : n_max;
     const long long used_chunks = (long long)c[IM_LC_CHUNK_BUMP] - (c[IM_LC_AVAIL_TOP] > 0 ? c[IM_LC_AVAIL_TOP] : 0);
@@ -92,7 +94,8 @@ inline void growth_targets(const int* c, long long steps, long long n_max, int m
         const long long q = capacity / 4;
         return capacity - used < (q > steps * per ? q : steps * per);
     };
-    while (need(*nodes, c[IM_LC_NODES], per_node)) *nodes *= 2;
+    const long long used_nodes = (long long)c[IM_LC_NODES] - (c[IM_LC_NODE_FREE] > 0 ? c[IM_LC_NODE_FREE] : 0);
+    while (need(*nodes, used_nodes, per_node)) *nodes *= 2;
     while (need(*chunks, used_chunks, per_chunk)) *chunks *= 2;
 }
 

@@ -142,9 +142,16 @@ struct VoxelMapDev {
     int* pub_mark;
     int* pub_list;
     int* pub_n;
+    // local map (local_map.cuh): node ids freed by the eviction of root voxels, popped by alloc_node before it bumps node_count.
+    // node_free == null: nothing was ever evicted from this map (alloc_node only bumps); n_tombs counts the tombstones in the table.
+    int* node_free;
+    int* node_free_top;
+    int* n_tombs;
 };
 
 #define IM_EMPTY_KEY 0xFFFFFFFFFFFFFFFFull
+// a root voxel evicted by the local map: bit 63 set (pack_key never sets it), not IM_EMPTY_KEY; never matches a key, never claimed
+#define IM_TOMB_KEY 0x8000000000000000ull
 
 // ------------------------------------------------------------------ atomics (plain ops in the host emulation)
 IM_HD int im_atomic_add(int* p, int v) {
@@ -239,6 +246,10 @@ IM_HD int hash_insert(const VoxelMapDev& m, unsigned long long key, int* created
 
 // ------------------------------------------------------------------ pools
 IM_HD int alloc_node(const VoxelMapDev& m) {
+    if (m.node_free) {   // node records freed by an eviction first, as alloc_chunk takes recycled chunks first
+        const int i = im_atomic_add(m.node_free_top, -1) - 1;
+        if (i >= 0) return m.node_free[i];
+    }
     const int id = im_atomic_add(m.node_count, 1);
     if (id >= m.max_nodes) { im_atomic_or(m.err, IM_ERR_NODE_POOL); return -1; }
     return id;
@@ -338,15 +349,17 @@ IM_HDN inline void node_moments_add(const VoxelMapDev& m, int nd, float x, float
         n.mq[e] = n.mq[e] + w * var6[sidx];
     }
 }
-// std::vector<Point_with_var>().swap(m_temp_points_): chunks go to the pending-free list (recycled between scans)
-IM_HD void node_free_points(const VoxelMapDev& m, int nd) {
+// std::vector<Point_with_var>().swap(m_temp_points_): chunks go to the pending-free list (recycled between scans); returns their number
+IM_HD int node_free_points(const VoxelMapDev& m, int nd) {
     NodeRec& n = m.nodes[nd];
     int ch = n.first_chunk;
+    int freed = 0;
     while (ch >= 0) {
         const int nx = m.chunks[ch].next;
         const int i = im_atomic_add(m.pending_n, 1);
         if (i < m.max_chunks) m.pending[i] = ch;
         ch = nx;
+        ++freed;
     }
     n.first_chunk = -1;
     n.last_chunk = -1;
@@ -354,6 +367,7 @@ IM_HD void node_free_points(const VoxelMapDev& m, int nd) {
     for (int i = 0; i < 3; ++i) n.sum_p[i] = 0.0;
     for (int i = 0; i < 6; ++i) n.sum_pp[i] = 0.0;
     for (int i = 0; i < 60; ++i) n.mq[i] = 0.0;
+    return freed;
 }
 
 // ------------------------------------------------------------------ init_plane (voxel_loc.cpp:47-139)

@@ -78,6 +78,44 @@ def _raycast(origin: np.ndarray, dirs: np.ndarray, max_range: float) -> np.ndarr
     return best
 
 
+# open-ended scene: the boxes and spheres above repeated along x every _OPEN_PERIOD metres, the ground and the two long side walls of
+# the room, no end walls -- a straight drive through it keeps reaching new ground for as long as it lasts
+_OPEN_PERIOD = 80.0
+
+
+def _raycast_open(origin: np.ndarray, dirs: np.ndarray, max_range: float) -> np.ndarray:
+    """Nearest hit distance along unit rays in the open-ended scene (inf when nothing within max_range)."""
+    n = dirs.shape[0]
+    best = np.full(n, np.inf)
+    lo, hi = origin[0] - max_range - _BOXES[:, 3].max(), origin[0] + max_range - _BOXES[:, 0].min()
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv = 1.0 / dirs
+        for k in range(int(np.floor(lo / _OPEN_PERIOD)), int(np.ceil(hi / _OPEN_PERIOD)) + 1):
+            shift = np.array([k * _OPEN_PERIOD, 0.0, 0.0])
+            for b in _BOXES:
+                t1 = (b[:3] + shift - origin) * inv
+                t2 = (b[3:] + shift - origin) * inv
+                tmin = np.nanmax(np.minimum(t1, t2), axis=1)
+                tmax = np.nanmin(np.maximum(t1, t2), axis=1)
+                hit = (tmax >= np.maximum(tmin, 0.0)) & (tmin > 1e-6)
+                best = np.where(hit & (tmin < best), tmin, best)
+            for sp in _SPHERES:
+                oc = origin - (sp[:3] + shift)
+                bq = dirs @ oc
+                cq = oc @ oc - sp[3] * sp[3]
+                disc = bq * bq - cq
+                t = -bq - np.sqrt(np.where(disc > 0, disc, np.nan))
+                hit = (disc > 0) & (t > 1e-6)
+                best = np.where(hit & (t < best), t, best)
+        tg = np.where(dirs[:, 2] < 0, (_ROOM[2] - origin[2]) * inv[:, 2], np.inf)            # ground
+        tw = np.where(dirs[:, 1] > 0, (_ROOM[4] - origin[1]) * inv[:, 1],
+                      np.where(dirs[:, 1] < 0, (_ROOM[1] - origin[1]) * inv[:, 1], np.inf))  # side walls
+        for t in (tg, tw):
+            best = np.where((t > 1e-6) & (t < best), t, best)
+    best[best > max_range] = np.inf
+    return best
+
+
 def _rot_z(a: float) -> np.ndarray:
     c, s = np.cos(a), np.sin(a)
     return np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
@@ -142,6 +180,11 @@ def make_sensor(kind: str, n_points: int | None = None) -> SensorModel:
         return s
     if kind == "hdl64loop":
         s = Spinning("hdl64loop", n_points or 131072, 2.0, 120.0, 0.04, 0.1, 10.0, 10.0)
+        s.rings, s.el_hi, s.el_lo = 64, 2.0, -24.8
+        return s
+    if kind == "hdl64open":
+        # the HDL-64 shape on a straight drive through the open-ended scene (trajectory_pose's weave along +x, 1 m per scan)
+        s = Spinning("hdl64open", n_points or 131072, 2.0, 120.0, 0.04, 0.1, 10.0, 10.0)
         s.rings, s.el_hi, s.el_lo = 64, 2.0, -24.8
         return s
     if kind == "ouster1m":
@@ -211,7 +254,7 @@ def make_scan(sensor: SensorModel, k: int, seed: int, ext_R: np.ndarray | None =
     RL = R @ eR                                   # LiDAR -> world rotation
     oL = R @ eT + t                               # LiDAR origin in world
     d_w = d_l @ RL.T
-    rng_true = _raycast(oL, d_w, sensor.max_range)
+    rng_true = (_raycast_open if sensor.name.endswith("open") else _raycast)(oL, d_w, sensor.max_range)
     ok = np.isfinite(rng_true) & (rng_true > sensor.blind)
     d_l = d_l[ok]
     r = rng_true[ok] + rng.normal(0.0, sensor.dept_err, ok.sum())

@@ -168,6 +168,37 @@ int immesh_lio_capacity(immesh_lio_t* h, int64_t* out /*[8]*/);
 int immesh_lio_reserve(immesh_lio_t* h, int64_t root_slots, int64_t nodes, int64_t chunks);
 int immesh_lio_set_growth(immesh_lio_t* h, int64_t max_bytes);
 
+/* Local map: a cube that follows the sensor, and the eviction of the root voxels it leaves behind, so that the VoxelMap of a drive
+ * that keeps reaching new ground stays bounded.  Opt-in and off by default; while it is off (and nothing was evicted) no output,
+ * launch sequence or captured graph changes.
+ * Box rule: Voxel_mapping::laser_map_fov_segment (src/voxel_mapping_common.cpp:214-288) in the reference's own types -- pos_end
+ *   double, the box vertex_min / vertex_max float, dist_to_map_edge float, thresholds mov_threshold * det_range in float, and
+ *   mov_dist = max((cube_len - 2 mov det) * 0.5 * 0.9, det (mov - 1)) (:256).  The first evaluation places the box around the pose
+ *   (:227-239); each later evaluation that moves it removes, for each axis that moved, the old box with that axis narrowed to the
+ *   slab it gave up (:257-278).
+ * When: once per scan at the state the scan's IESKF starts from -- after the prediction (for the IMU chain: after UndistortPcl),
+ *   before the first match -- by immesh_lio_estimate and the immesh_lio_step* entry points; immesh_voxelmap_build and the IMU chain's
+ *   first scan evaluate it at the building scan's pose, which places the box.  The *_pv calls never evaluate it.
+ * What is evicted: a root voxel whose centre (the root node's voxel centre, double) lies in a removed box, the float edges widened
+ *   to double, half-open min <= c < max as ikd-Tree's Delete_Point_Boxes (include/ikd-Tree/ikd_Tree.cpp:826-827).  Its whole octree
+ *   goes: the chunks back to the chunk pool, the node records onto a free stack that new nodes are taken from first, its hash slot
+ *   becomes a tombstone.  A root created there later is a fresh root, exactly as on a first visit.  A run with the local map equals
+ *   the oracle run with the same eviction (state, match sets, canonical dump); node ids may differ, as between any two runs.
+ * Tombstones: when those left by the last finished step exceed 1/8 of the root slots, the next step first drains the handle and
+ *   rebuilds the root hash at its size (whatever immesh_lio_set_growth says).  Growth counts tombstones as occupied slots and the
+ *   free node records as unused.
+ * local_map: cube_len > 0 turns the automatic rule on (the reference's values: cube_side_length, det_range 300, mov_threshold 1.5);
+ *   cube_len = 0 turns it off.  Drains the handle; the box is placed at the next evaluation.  A non-finite or non-positive value, or
+ *   a sharded handle: IMMESH_E_INVALID; immesh_lio_shard refuses a handle that ever used the local map or evict_boxes.  cube_len <= 2 mov det is allowed
+ *   (the reference only warns): the box then moves on every scan.
+ * evict_boxes: evicts the root voxels whose centre lies in one of n boxes [n][6] (min xyz, max xyz), by the same rule; queued in
+ *   stream order behind the steps already queued (the Delete_Point_Boxes analogue); `boxes` is copied before the call returns.  A NaN edge or a sharded handle: IMMESH_E_INVALID.
+ * local_map_state: blocking.  box = the current box (min xyz, max xyz); stats = [box placed, moves, roots evicted, node records
+ *   freed, chunks freed, live tombstones, hash rebuilds that dropped tombstones, free node records]. */
+int immesh_lio_local_map(immesh_lio_t* h, double cube_len, float det_range, float mov_threshold);
+int immesh_voxelmap_evict_boxes(immesh_lio_t* h, const float* boxes /*[n][6]*/, int n);
+int immesh_lio_local_map_state(immesh_lio_t* h, float* box /*[6]*/, int64_t* stats /*[8]*/);
+
 /* pubPlaneMap(m_feat_map, voxel_pub, state.pos_end) (src/voxel_mapping.cpp:947-1159), called after voxel_map_init and after every
  * map_incremental_grow (:1899-1900, :1975-1976): the markers of the planes refitted since the last call, one row per pubPlane call
  * (:919-945), with the reference's walk -- a root whose m_is_update flag is set is published and its children wait for a later
