@@ -3,7 +3,7 @@
 // mesh_eval.cuh; the rules are stated in include/immesh_b200.h.
 //
 // Shape of the call (every step on the device, the host only plans tiles and reads a few counts):
-//   1. live triangles compacted and sorted by (a, b, c) (stable LSD passes on c, b, a); per triangle the float32 corner positions,
+//   1. live triangles compacted and sorted by (a, b, c) (mesh_tri_order, as immesh_mesh_snapshot orders them); per triangle the float32 corner positions,
 //      the fairness terms and the subdivision count n.
 //   2. space is split into tiles (bisection of the bounding box of the mesh and the ground truth) until the scratch one tile needs
 //      fits the budget.  A query (sample or down-sampled ground-truth point) is answered in the tile that holds it, against the
@@ -104,21 +104,6 @@ __device__ __forceinline__ void acc_add(unsigned long long* acc, int slot, unsig
 }
 
 // ---- 1. live triangles
-__global__ void __launch_bounds__(128) k_eval_live(MeshDev M, int n_alloc, int4* out, int* out_n) {
-    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[t];
-        if (r.w) out[atomicAdd(out_n, 1)] = r;
-    }
-}
-// sort key of pass `comp` (0 a, 1 b, 2 c) of the triangles in the order perm (null: as compacted); the value is the compacted index
-__global__ void __launch_bounds__(128) k_eval_tri_key(const int4* tri, const unsigned* perm, int n, int comp, unsigned* key, unsigned* val) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const unsigned s = perm ? perm[i] : (unsigned)i;
-        const int4 t = tri[s];
-        key[i] = (unsigned)(comp == 0 ? t.x : comp == 1 ? t.y : t.z);
-        val[i] = s;
-    }
-}
 // per sorted triangle: its triple, the float32 corners (raw or (float) of the smoothed position), fairness and subdivisions
 __global__ void __launch_bounds__(128) k_eval_tri(MeshDev M, int smoothed, const int4* tri, const unsigned* perm, int n, double spacing, int4* st,
                                                    float* tp, int* nsub, double* fair, unsigned long long* acc) {
@@ -413,18 +398,18 @@ struct Carve {
         off += n * sizeof(T);
     }
 };
-// the per-call table: accumulators, counters, and per live triangle its triple (compacted and sorted), corners, subdivisions, fairness,
-// per-facet counts, the triple sort and the rows
+// the per-call table: accumulators, counters, and per live triangle its record (mesh_tri_order's buffers), its triple in order,
+// corners, subdivisions, fairness, per-facet counts and the rows
 struct Table {
     unsigned long long* acc; int* d_n; double* fsum;
-    int4 *tri, *stri; float* tp; int* nsub; double* fair; int *f_s, *f_f; unsigned *tk[2], *tv[2]; int* hist; int* rows;
+    TriOrder ord; int4* stri; float* tp; int* nsub; double* fair; int *f_s, *f_f; int* rows;
 };
 size_t table_carve(Carve& c, long long nt, bool rows, Table& T) {
     const size_t n1 = (size_t)std::max<long long>(nt, 1);
     c.take(T.acc, EA_SIZE); c.take(T.d_n, 8); c.take(T.fsum, 2);
-    c.take(T.tri, n1); c.take(T.stri, n1); c.take(T.tp, n1 * 9); c.take(T.nsub, n1); c.take(T.fair, n1 * 2); c.take(T.f_s, n1); c.take(T.f_f, n1);
-    for (int b = 0; b < 2; ++b) { c.take(T.tk[b], n1); c.take(T.tv[b], n1); }
-    c.take(T.hist, hist_ints(nt));
+    c.take(T.ord.rec, n1); c.take(T.stri, n1); c.take(T.tp, n1 * 9); c.take(T.nsub, n1); c.take(T.fair, n1 * 2); c.take(T.f_s, n1); c.take(T.f_f, n1);
+    for (int b = 0; b < 2; ++b) { c.take(T.ord.k[b], n1); c.take(T.ord.v[b], n1); }
+    c.take(T.ord.hist, hist_ints(nt));
     T.rows = nullptr;
     if (rows) c.take(T.rows, n1 * 5);
     return c.off;
@@ -482,12 +467,12 @@ int immesh_mesh_evaluate(immesh_mesh_t* h, const float* gt_xyz, int64_t n_gt, in
     cudaStream_t st = h->stream;
     int mc[IM_MC_HOST];
     IM_CUDA(cudaMemcpy(mc, h->M.cnt, sizeof(mc), cudaMemcpyDeviceToHost));
-    const int nalloc = std::min(mc[IM_MC_TRIS_ALLOC], h->M.max_t), nt = mc[IM_MC_TRIS_LIVE];
+    const int nt = mc[IM_MC_TRIS_LIVE];
     if (n_rows) *n_rows = nt;
     if (facet_rows && cap_rows < nt) return im_fail(IMMESH_E_CAPACITY, "evaluate: cap_rows is below the live triangle count (*n_rows)");
 
     const size_t budget = cfg->max_batch_bytes ? (size_t)cfg->max_batch_bytes : ((size_t)2 << 30);
-    Table T;
+    Table T = {};
     Carve tc;
     const size_t tb = table_carve(tc, nt, facet_rows != nullptr, T);
     if (tb > budget)
@@ -511,19 +496,12 @@ int immesh_mesh_evaluate(immesh_mesh_t* h, const float* gt_xyz, int64_t n_gt, in
         IM_CUDA(cudaMemsetAsync(T.f_f, 0, (size_t)std::max(nt, 1) * sizeof(int), st));
     }
 
-    // 1. live triangles, sorted by (a, b, c): stable LSD passes on c, then b, then a
+    // 1. live triangles in triple order (mesh_tri_order, with the table's buffers)
     if (nt > 0) {
-        IM_LAUNCH(k_eval_live, eval_grid_dim(nsm, nalloc, 128), 128, 0, st, h->M, nalloc, T.tri, d_n);
-        int passes = 1;
-        while (passes < 4 && ((unsigned long long)mc[IM_MC_VERTICES] >> (8 * passes)) != 0) ++passes;
-        int cur = 0;
-        for (int comp = 2; comp >= 0; --comp) {
-            IM_LAUNCH(k_eval_tri_key, eval_grid_dim(nsm, nt, 128), 128, 0, st, (const int4*)T.tri, (const unsigned*)(comp == 2 ? nullptr : T.tv[cur]), nt, comp,
-                      T.tk[cur ^ (comp == 2 ? 0 : 1)], T.tv[cur ^ (comp == 2 ? 0 : 1)]);
-            if (comp != 2) cur ^= 1;
-            cur = rs_sort_passes(st, T.tk, T.tv, cur, nt, passes, T.hist);
-        }
-        IM_LAUNCH(k_eval_tri, eval_grid_dim(nsm, nt, 128), 128, 0, st, h->M, cfg->positions, (const int4*)T.tri, (const unsigned*)T.tv[cur], nt, spacing, T.stri,
+        T.ord.cap = nt;
+        T.ord.misc = d_n;
+        if (const int rc = mesh_tri_order(h, mc, 0.0, T.ord)) return rc;
+        IM_LAUNCH(k_eval_tri, eval_grid_dim(nsm, nt, 128), 128, 0, st, h->M, cfg->positions, (const int4*)T.ord.rec, T.ord.order, nt, spacing, T.stri,
                   T.tp, T.nsub, T.fair, acc);
         IM_LAUNCH(k_eval_fair_sum, 1, 1024, 0, st, (const double*)T.fair, nt, T.fsum);
     }

@@ -146,9 +146,6 @@ struct immesh_mesh {
     immesh::PeerWindow win;           // peer window: [flags][recv1 x n][recv2 x n] when the segments are pushed over NVLink
     int* d_xdone = nullptr;           // block-done counters of the two push kernels
     size_t seg1_bytes = 0, seg2_bytes = 0;
-    int* d_snap_tri = nullptr;
-    int* d_snap_flip = nullptr;
-    int* d_snap_n = nullptr;
     int max_frame_points = 0;
     immesh::GraphCtx graph;   // replay of the per-frame launch sequence (pipelined API)
     int use_graph = 1;
@@ -161,8 +158,8 @@ struct immesh_mesh {
     immesh::MemSet dev;       // device memory counted in immesh_mesh_capacity (with `batch`): the create-time buffers, the pools and the shard segments
     immesh::MemSet scratch;   // device memory not counted: the region buffers' scratch
     immesh::MemSet pinned{immesh::MemSet::Pinned};
-    unsigned char* region_scratch[16] = {};   // immesh_mesh_region_buffers, grow-only, in `scratch`
-    size_t region_scratch_cap[16] = {};
+    unsigned char* region_scratch[12] = {};   // immesh_mesh_region_buffers, grow-only, in `scratch`
+    size_t region_scratch_cap[12] = {};
     // batched frame (immesh_mesh_push_frame_batched), allocated by its first call into `batch`, sized by the handle's capacities only
     immesh::MemSet batch;
     int max_vox = 0;
@@ -207,3 +204,22 @@ struct immesh_mesh {
         immesh::MemSet dev;               // every buffer of the feed, freed by disable / destroy (not counted)
     } chg;
 };
+
+// The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate
+// (mesh_tri_order, mesh_capi.cu): the live records compacted (w = the slot) and sorted by the triple (a, b, c); with a region size
+// first by the region of tri_region_key, either every region by its key (ascending x, y, z) or, with qkeys, only the regions of the
+// table qkeys / qval by the caller's index.  The caller provides the buffers for `cap` records.  A key outside +-1048000 sets `range`.
+struct TriOrder {
+    int cap;
+    int4* rec;                         // [cap] the kept records
+    int* reg;                          // [3 cap] the keys (all regions) or [cap] the caller's index (requested regions)
+    unsigned int *k[2], *v[2];         // [cap] each: the sort's ping-pong
+    int* hist;                         // 256 * ceil(cap / VG_TILE) ints
+    int* misc;                         // [8] on the device: count, range flag, minimum and maximum of each region word
+    const unsigned long long* qkeys;   // requested regions: packed keys (qmask + 1 slots) and each slot's index
+    const int* qval;
+    unsigned int qmask;
+    int n, range;                      // out: the records kept, the range flag
+    const unsigned int* order;         // out: the kept records' indices into rec, in order
+};
+int mesh_tri_order(immesh_mesh* h, const int* cnt, double region_size, TriOrder& o);

@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <array>
 #include <chrono>
+#include <climits>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -250,14 +251,57 @@ __global__ void k_chg_end(MeshDev M, FrameBuf F_, ChgDev C, int full, int v_afte
 __global__ void __launch_bounds__(128) k_chg_init(MeshDev M, unsigned char* pub, int n_alloc) {
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) pub[t] = chg_state(M, t);
 }
-// snapshot: compact live triangles
-__global__ void __launch_bounds__(128) k_snapshot(MeshDev M, int n_alloc, int* out_tri, int* out_flip, int* out_n) {
+// ---- the live triangles in order (mesh_tri_order).  k_tri_gather compacts the live records of the slots [0, n_alloc) into rec[0, cap),
+// w = the slot, and counts every kept one in misc[0].  With a region size it keys them (tri_region_key): all regions (qkeys null) keep
+// the key in reg[3 e ..]; requested regions keep only the triangles of a region in the table, with the caller's index in reg[e].  The
+// minimum and maximum of each region word go to misc[2..7], reduced once per warp.  A key outside ikey_ok sets misc[1].
+__global__ void __launch_bounds__(128) k_tri_gather(MeshDev M, int n_alloc, int cap, double region_size, const unsigned long long* qkeys, const int* qval,
+                                                    unsigned int qmask, int4* rec, int* reg, int* misc) {
+    const int nreg = region_size > 0 ? (qkeys ? 1 : 3) : 0;
+    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[t];
+        int4 r = M.tri[t];
         if (!r.w) continue;
-        const int k = atomicAdd(out_n, 1);
-        out_tri[(size_t)k * 3 + 0] = r.x; out_tri[(size_t)k * 3 + 1] = r.y; out_tri[(size_t)k * 3 + 2] = r.z;
-        out_flip[k] = (int)(M.tri_flip[t] & 1ull);
+        int k[3] = {0, 0, 0};
+        if (region_size > 0) {
+            tri_region_key(M, r, region_size, k);
+            if (!ikey_ok(k[0], k[1], k[2])) atomicOr(&misc[1], 1);
+            if (qkeys) {
+                const int s = table_find(qkeys, qmask, pack_ikey(k[0], k[1], k[2]));
+                if (s < 0) continue;
+                k[0] = qval[s];
+            }
+            for (int c = 0; c < 3; ++c) { lo[c] = min(lo[c], k[c]); hi[c] = max(hi[c], k[c]); }
+        }
+        const int e = atomicAdd(&misc[0], 1);
+        if (e >= cap) continue;
+        r.w = t;
+        rec[e] = r;
+        for (int c = 0; c < nreg; ++c) reg[(size_t)e * nreg + c] = k[c];
+    }
+    for (int c = 0; c < nreg; ++c) {
+        const int a = __reduce_min_sync(0xffffffffu, lo[c]), b = __reduce_max_sync(0xffffffffu, hi[c]);
+        if ((threadIdx.x & 31) == 0 && a <= b) { atomicMin(&misc[2 + c], a); atomicMax(&misc[5 + c], b); }
+    }
+}
+// sort word w of the records in the order vin (null: as gathered): 0..2 = c, b, a of the triple; 3 + j = region word j less its minimum
+__global__ void __launch_bounds__(128) k_tri_word(const int4* rec, const int* reg, int nreg, int n, int w, unsigned int base, const unsigned int* vin,
+                                                  unsigned int* kout, unsigned int* vout) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const unsigned int v = vin ? vin[i] : (unsigned int)i;
+        unsigned int x;
+        if (w < 3) { const int4 r = rec[v]; x = (unsigned int)(w == 0 ? r.z : w == 1 ? r.y : r.x); }
+        else x = (unsigned int)reg[(size_t)v * nreg + (w - 3)] - base;
+        kout[i] = x;
+        vout[i] = v;
+    }
+}
+// snapshot and region stream: the records in order, their triples and (flip not null) the orientation flags of their slots
+__global__ void __launch_bounds__(128) k_tri_emit(MeshDev M, const int4* rec, const unsigned int* order, int n, int* tri, int* flip) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const int4 r = rec[order[i]];
+        tri[(size_t)i * 3 + 0] = r.x; tri[(size_t)i * 3 + 1] = r.y; tri[(size_t)i * 3 + 2] = r.z;
+        if (flip) flip[i] = (int)(M.tri_flip[r.w] & 1ull);
     }
 }
 
@@ -354,16 +398,6 @@ __global__ void __launch_bounds__(128) k_smooth_all(MeshDev M, int nv, int k, co
         smooth_vertex(M, v, k, idx + (size_t)v * k, d2 + (size_t)v * k, sf, max_dis, r);
         store_smooth(M, v, r[0], r[1], r[2]);
         if (out) { out[(size_t)v * 3 + 0] = r[0]; out[(size_t)v * 3 + 1] = r[1]; out[(size_t)v * 3 + 2] = r[2]; }
-    }
-}
-// Triangle_manager::insert_triangle_to_list (triangle.cpp:35-53): region = round(centre / region_size) of every live triangle
-__global__ void __launch_bounds__(128) k_region_keys(MeshDev M, int n_alloc, double region_size, int* out_tri, int* out_key, int* out_n) {
-    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[t];
-        if (!r.w) continue;
-        const int e = atomicAdd(out_n, 1);
-        out_tri[(size_t)e * 3 + 0] = r.x; out_tri[(size_t)e * 3 + 1] = r.y; out_tri[(size_t)e * 3 + 2] = r.z;
-        tri_region_key(M, r, region_size, out_key + (size_t)e * 3);
     }
 }
 
@@ -511,72 +545,43 @@ __global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const F
     if (blockIdx.x == 0 && threadIdx.x == 0) *o.n = blk_off[nb];
 }
 
-// ---- the viewer's region buffers (immesh_mesh_region_buffers, mesh_rec_display.cpp:78-137 + :220-258).  k_rb_select keys the live
-// triangles and keeps those of the requested regions, compacted in any order.  A stable LSD radix sort of the kept positions over
-// 32-bit words -- the triple's ids k, j, i, then the region -- orders them by (region, triple); that order is total (a live triple is
-// unique), so nothing depends on the compaction order.  The vertices of the kept triangles whose m_smoothed is clear are claimed once
-// (bitmap), compacted, searched with k_knn and smoothed from raw positions; k_rb_emit gathers vsmooth into the float rows and reduces
-// the axis box per block.
+// ---- the region segments of records in region order (mesh_tri_order with a region size): the region stream and the viewer's region
+// buffers (immesh_mesh_region_buffers, mesh_rec_display.cpp:78-137 + :220-258).  For the buffers, the vertices of the kept triangles
+// whose m_smoothed is clear are claimed once (bitmap), compacted, searched with k_knn and smoothed from raw positions; k_rb_emit
+// gathers vsmooth into the float rows and reduces the axis box per block.
 #define RB_THREADS 128
-__global__ void __launch_bounds__(RB_THREADS) k_rb_select(MeshDev M, int n_alloc, double region_size, const unsigned long long* qkeys, const int* qval, unsigned int qmask,
-                                                          int use_keys, int* slot, unsigned long long* rk, int* misc) {
-    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[t];
-        if (!r.w) continue;
-        int k[3];
-        tri_region_key(M, r, region_size, k);
-        if (!ikey_ok(k[0], k[1], k[2])) { atomicOr(&misc[1], 1); continue; }
-        unsigned long long word = pack_ikey(k[0], k[1], k[2]);
-        if (use_keys) {
-            const int s = table_find(qkeys, qmask, word);
-            if (s < 0) continue;
-            word = (unsigned long long)qval[s];   // the region's index in the caller's list
-        }
-        const int e = atomicAdd(&misc[0], 1);
-        slot[e] = t;
-        rk[e] = word;
-    }
+__device__ __forceinline__ bool rb_same_region(const int* reg, unsigned int a, unsigned int b) {   // all regions: three key words per record
+    return reg[(size_t)a * 3] == reg[(size_t)b * 3] && reg[(size_t)a * 3 + 1] == reg[(size_t)b * 3 + 1] && reg[(size_t)a * 3 + 2] == reg[(size_t)b * 3 + 2];
 }
-// sort word w of kept position v: 0..2 = the triple's k, j, i; 3 / 4 = low / high half of the region word
-__global__ void __launch_bounds__(RB_THREADS) k_rb_word(MeshDev M, int n, int w, const int* slot, const unsigned long long* rk, const unsigned int* vin, unsigned int* kout, unsigned int* vout) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const unsigned int v = vin ? vin[i] : (unsigned int)i;
-        unsigned int x;
-        if (w < 3) { const int4 r = M.tri[slot[v]]; x = (unsigned int)(w == 0 ? r.z : w == 1 ? r.y : r.x); }
-        else x = w == 3 ? (unsigned int)rk[v] : (unsigned int)(rk[v] >> 32);
-        kout[i] = x;
-        vout[i] = v;
-    }
-}
-__global__ void __launch_bounds__(RB_THREADS) k_rb_starts(int n, const unsigned int* order, const unsigned long long* rk, int* flag) {
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) flag[i] = (i == 0 || rk[order[i]] != rk[order[i - 1]]) ? 1 : 0;
+__global__ void __launch_bounds__(RB_THREADS) k_rb_starts(int n, const unsigned int* order, const int* reg, int* flag) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) flag[i] = (i == 0 || !rb_same_region(reg, order[i], order[i - 1])) ? 1 : 0;
 }
 // all regions: the first row of every region writes its key and offset (scan: exclusive region number of each row)
-__global__ void __launch_bounds__(RB_THREADS) k_rb_regions(int n, const unsigned int* order, const unsigned long long* rk, const int* scan, int* keys, int* off) {
+__global__ void __launch_bounds__(RB_THREADS) k_rb_regions(int n, const unsigned int* order, const int* reg, const int* scan, int* keys, int* off) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        if (i > 0 && rk[order[i]] == rk[order[i - 1]]) continue;
+        if (i > 0 && rb_same_region(reg, order[i], order[i - 1])) continue;
         const int r = scan[i];
-        unpack_ikey(rk[order[i]], keys + (size_t)r * 3, keys + (size_t)r * 3 + 1, keys + (size_t)r * 3 + 2);
+        for (int c = 0; c < 3; ++c) keys[(size_t)r * 3 + c] = reg[(size_t)order[i] * 3 + c];
         off[r] = i;
     }
 }
 // requested regions (n >= 1 rows): offsets of nk segments, empty ones included
-__global__ void __launch_bounds__(RB_THREADS) k_rb_offsets(int n, int nk, const unsigned int* order, const unsigned long long* rk, int* off) {
+__global__ void __launch_bounds__(RB_THREADS) k_rb_offsets(int n, int nk, const unsigned int* order, const int* reg, int* off) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const int cur = (int)rk[order[i]], prev = i > 0 ? (int)rk[order[i - 1]] : -1;
+        const int cur = reg[order[i]], prev = i > 0 ? reg[order[i - 1]] : -1;
         for (int r = prev + 1; r <= cur; ++r) off[r] = i;
         if (i == n - 1) for (int r = cur + 1; r <= nk; ++r) off[r] = n;
     }
 }
 // vertices of the kept triangles with m_smoothed clear, each claimed once, compacted with its position as a k_knn query
-__global__ void __launch_bounds__(RB_THREADS) k_rb_claim(MeshDev M, int n, const int* slot, unsigned int* bits, int* misc, int* list, float4* q) {
+__global__ void __launch_bounds__(RB_THREADS) k_rb_claim(MeshDev M, int n, const int4* rec, unsigned int* bits, int* claimed, int* list, float4* q) {
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < 3 * n; e += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[slot[e / 3]];
+        const int4 r = rec[e / 3];
         const int v = e % 3 == 0 ? r.x : e % 3 == 1 ? r.y : r.z;
         if (M.vsmoothed[v]) continue;
         const unsigned int bit = 1u << (v & 31);
         if (atomicOr(&bits[v >> 5], bit) & bit) continue;
-        const int k = atomicAdd(&misc[2], 1);
+        const int k = atomicAdd(claimed, 1);
         list[k] = v;
         q[k] = M.vpos[v];
     }
@@ -588,12 +593,12 @@ __global__ void __launch_bounds__(RB_THREADS) k_rb_smooth(MeshDev M, int nq, int
         store_smooth(M, list[i], r[0], r[1], r[2]);
     }
 }
-__global__ void __launch_bounds__(RB_THREADS) k_rb_emit(MeshDev M, int n, const unsigned int* order, const int* slot, float* xyz, int* ids, AxisAcc* part) {
+__global__ void __launch_bounds__(RB_THREADS) k_rb_emit(MeshDev M, int n, const unsigned int* order, const int4* rec, float* xyz, int* ids, AxisAcc* part) {
     __shared__ AxisAcc s[RB_THREADS];
     AxisAcc a;
     axis_init(a);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const int4 r = M.tri[slot[order[i]]];
+        const int4 r = rec[order[i]];
         float row[9];
         region_row(M, r, row);
         for (int c = 0; c < 9; ++c) xyz[(size_t)i * 9 + c] = row[c];
@@ -1287,6 +1292,49 @@ static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes tha
     return std::max(1, (b + 7) / 8);
 }
 
+// TriOrder (handles.hpp): the gather, one read-back of its counters, then the LSD passes over c, b, a and the region words from the last,
+// each over the bits it can hold: the vertex ids below cnt[IM_MC_VERTICES], or the word's range (less its minimum)
+extern "C++" int mesh_tri_order(immesh_mesh* h, const int* cnt, double region_size, TriOrder& o) {
+    cudaStream_t st = h->stream;
+    const int nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nv = cnt[IM_MC_VERTICES];
+    const int nreg = region_size > 0 ? (o.qkeys ? 1 : 3) : 0;
+    int m[8] = {0, 0, INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
+    IM_CUDA(cudaMemcpyAsync(o.misc, m, sizeof(m), cudaMemcpyHostToDevice, st));
+    IM_LAUNCH(k_tri_gather, mesh_grid(h, nalloc, 128), 128, 0, st, h->M, nalloc, o.cap, region_size, o.qkeys, o.qval, o.qmask, o.rec, o.reg, o.misc);
+    IM_CUDA(cudaMemcpyAsync(m, o.misc, sizeof(m), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    if (m[0] > o.cap) return im_fail(IMMESH_E_CUDA, "more live triangles than the mesh's counters hold (internal error)");
+    o.n = m[0];
+    o.range = m[1];
+    int cur = 0;
+    for (int w = 0; o.n > 0 && w < 3 + nreg; ++w) {
+        const int c = w < 3 ? 0 : nreg - 1 - (w - 3);   // the region word of this pass
+        const unsigned int base = w < 3 ? 0u : (unsigned int)m[2 + c];
+        const unsigned long long top = w < 3 ? (unsigned long long)std::max(nv - 1, 0) : (unsigned long long)((unsigned int)m[5 + c] - base);
+        IM_LAUNCH(k_tri_word, mesh_grid(h, o.n, 128), 128, 0, st, (const int4*)o.rec, (const int*)o.reg, nreg, o.n, w < 3 ? w : 3 + c, base,
+                  w == 0 ? (const unsigned int*)nullptr : (const unsigned int*)o.v[cur], o.k[cur ^ 1], o.v[cur ^ 1]);
+        cur = rs_sort_passes(st, o.k, o.v, cur ^ 1, o.n, rb_passes(top), o.hist);
+    }
+    IM_CUDA(cudaGetLastError());
+    o.order = o.v[cur];
+    return IMMESH_OK;
+}
+// mesh_tri_order's buffers for cap records with nreg region words each, placed in one block of 4-byte words: the records, the sort's
+// keys and values, misc, hist, the region words.  Returns the block's words; a null base only counts them.
+static size_t tri_order_carve(unsigned int* base, int cap, int nreg, TriOrder& o) {
+    const size_t c = (size_t)std::max(cap, 1), nh = 256 * ((c + VG_TILE - 1) / VG_TILE);
+    if (base) {
+        o.cap = cap;
+        o.rec = (int4*)base;
+        o.k[0] = base + 4 * c; o.k[1] = o.k[0] + c;
+        o.v[0] = o.k[1] + c; o.v[1] = o.v[0] + c;
+        o.misc = (int*)(o.v[1] + c);
+        o.hist = o.misc + 8;
+        o.reg = o.hist + nh;
+    }
+    return 8 * c + 8 + nh + (size_t)nreg * c;
+}
+
 // the change feed of the frame whose push was just queued (F: its FrameBuf; batched: a batched frame, after k_bat_frame_end): the
 // touched set (the sweep when batched or overflowed), the rows against the published bytes (marked per slot, then compacted), their LSD sort by (a, b, c) over words
 // of the bits of max_v - 1, the ring append and the header.  Fixed grids: every count is read on the device.
@@ -1667,7 +1715,7 @@ int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, 
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     int cnt[IM_MC_HOST];
     IM_CUDA(mesh_read_counters(h, cnt));
-    const int nv = cnt[IM_MC_VERTICES], nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
+    const int nv = cnt[IM_MC_VERTICES], nlive = cnt[IM_MC_TRIS_LIVE];
     if (vertices && nv > 0) {
         std::vector<float4> v(nv);
         IM_CUDA(cudaMemcpy(v.data(), h->M.vpos, (size_t)nv * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -1675,28 +1723,19 @@ int immesh_mesh_snapshot(immesh_mesh_t* h, float* vertices, int32_t* triangles, 
     }
     if ((triangles || flips) && nlive > 0) {
         immesh::MemSet tmp;
-        int *d_tri = nullptr, *d_flip = nullptr, *d_n = nullptr;
-        IM_CUDA(tmp.alloc(&d_tri, (size_t)nlive * 3));
-        IM_CUDA(tmp.alloc(&d_flip, (size_t)nlive));
-        IM_CUDA(tmp.alloc(&d_n, 1));
-        IM_CUDA(cudaMemset(d_n, 0, sizeof(int)));
-        IM_LAUNCH(k_snapshot, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, d_tri, d_flip, d_n);
-        std::vector<int> t((size_t)nlive * 3), f(nlive);
-        IM_CUDA(cudaMemcpyAsync(t.data(), d_tri, (size_t)nlive * 3 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-        IM_CUDA(cudaMemcpyAsync(f.data(), d_flip, (size_t)nlive * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        TriOrder o = {};
+        unsigned int* block = nullptr;
+        int* d_tri = nullptr;   // [3 nlive] triples, then [nlive] flips
+        IM_CUDA(tmp.alloc(&block, tri_order_carve(nullptr, nlive, 0, o)));
+        tri_order_carve(block, nlive, 0, o);
+        IM_CUDA(tmp.alloc(&d_tri, (size_t)nlive * 4));
+        int* d_flip = d_tri + (size_t)nlive * 3;
+        if (const int rc = mesh_tri_order(h, cnt, 0.0, o)) return rc;
+        if (o.n > 0) IM_LAUNCH(k_tri_emit, mesh_grid(h, o.n, 128), 128, 0, h->stream, h->M, (const int4*)o.rec, o.order, o.n, d_tri, d_flip);
+        IM_CUDA(cudaGetLastError());
+        if (triangles) IM_CUDA(cudaMemcpyAsync(triangles, d_tri, (size_t)o.n * 3 * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        if (flips) IM_CUDA(cudaMemcpyAsync(flips, d_flip, (size_t)o.n * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         IM_CUDA(cudaStreamSynchronize(h->stream));
-        std::vector<int> order(nlive);
-        for (int i = 0; i < nlive; ++i) order[i] = i;
-        std::sort(order.begin(), order.end(), [&](int a, int b) {
-            for (int j = 0; j < 3; ++j)
-                if (t[(size_t)a * 3 + j] != t[(size_t)b * 3 + j]) return t[(size_t)a * 3 + j] < t[(size_t)b * 3 + j];
-            return false;
-        });
-        for (int i = 0; i < nlive; ++i) {
-            if (triangles)
-                for (int j = 0; j < 3; ++j) triangles[(size_t)i * 3 + j] = t[(size_t)order[i] * 3 + j];
-            if (flips) flips[i] = f[order[i]];
-        }
     }
     return IMMESH_OK;
 }
@@ -1747,44 +1786,34 @@ int immesh_mesh_region_stream(immesh_mesh_t* h, double region_size, int32_t* reg
     IM_CUDA(cudaStreamSynchronize(h->stream));
     int cnt[IM_MC_HOST];
     IM_CUDA(mesh_read_counters(h, cnt));
-    const int nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
+    const int nlive = cnt[IM_MC_TRIS_LIVE];
     *n_regions = 0;
     if (nlive == 0) { if (region_offsets && cap_regions >= 0) region_offsets[0] = 0; return IMMESH_OK; }
+    cudaStream_t st = h->stream;
     immesh::MemSet tmp;
-    int *d_tri = nullptr, *d_key = nullptr, *d_n = nullptr;
-    IM_CUDA(tmp.alloc(&d_tri, (size_t)nlive * 3));
-    IM_CUDA(tmp.alloc(&d_key, (size_t)nlive * 3));
-    IM_CUDA(tmp.alloc(&d_n, 1));
-    IM_CUDA(cudaMemset(d_n, 0, sizeof(int)));
-    IM_LAUNCH(k_region_keys, mesh_grid(h, nalloc, 128), 128, 0, h->stream, h->M, nalloc, region_size, d_tri, d_key, d_n);
-    std::vector<int> t((size_t)nlive * 3), kx((size_t)nlive * 3);
-    IM_CUDA(cudaMemcpyAsync(t.data(), d_tri, t.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    IM_CUDA(cudaMemcpyAsync(kx.data(), d_key, kx.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    IM_CUDA(cudaStreamSynchronize(h->stream));
-    std::vector<int> order(nlive);
-    for (int i = 0; i < nlive; ++i) order[i] = i;
-    std::sort(order.begin(), order.end(), [&](int a, int b) {   // regions by ascending key, triangles by ascending triple inside a region
-        for (int j = 0; j < 3; ++j)
-            if (kx[(size_t)a * 3 + j] != kx[(size_t)b * 3 + j]) return kx[(size_t)a * 3 + j] < kx[(size_t)b * 3 + j];
-        for (int j = 0; j < 3; ++j)
-            if (t[(size_t)a * 3 + j] != t[(size_t)b * 3 + j]) return t[(size_t)a * 3 + j] < t[(size_t)b * 3 + j];
-        return false;
-    });
+    TriOrder o = {};
+    unsigned int* block = nullptr;
+    int* d_flag = nullptr;   // [nlive + 1] region starts, scanned; then the keys [3 nlive], offsets [nlive] and triples [3 nlive]
+    IM_CUDA(tmp.alloc(&block, tri_order_carve(nullptr, nlive, 3, o)));
+    tri_order_carve(block, nlive, 3, o);
+    IM_CUDA(tmp.alloc(&d_flag, (size_t)nlive * 8 + 1));
+    int *d_keys = d_flag + nlive + 1, *d_off = d_keys + (size_t)nlive * 3, *d_tri = d_off + nlive;
+    if (const int rc = mesh_tri_order(h, cnt, region_size, o)) return rc;   // a key past +-1048000 is ordered as any other: o.range is not an error here
+    const int n = o.n, g = mesh_grid(h, n, RB_THREADS);
+    IM_LAUNCH(k_rb_starts, g, RB_THREADS, 0, st, n, o.order, (const int*)o.reg, d_flag);
+    IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, d_flag, n, d_flag + nlive);
+    IM_LAUNCH(k_rb_regions, g, RB_THREADS, 0, st, n, o.order, (const int*)o.reg, (const int*)d_flag, d_keys, d_off);
+    IM_LAUNCH(k_tri_emit, g, RB_THREADS, 0, st, h->M, (const int4*)o.rec, o.order, n, d_tri, (int*)nullptr);
+    IM_CUDA(cudaGetLastError());
     int nr = 0;
-    for (int i = 0; i < nlive; ++i) {
-        const int o = order[i];
-        const bool first = (i == 0) || kx[(size_t)o * 3] != kx[(size_t)order[i - 1] * 3] || kx[(size_t)o * 3 + 1] != kx[(size_t)order[i - 1] * 3 + 1] ||
-                           kx[(size_t)o * 3 + 2] != kx[(size_t)order[i - 1] * 3 + 2];
-        if (first) {
-            if (nr < cap_regions) {
-                if (region_keys) for (int j = 0; j < 3; ++j) region_keys[(size_t)nr * 3 + j] = kx[(size_t)o * 3 + j];
-                if (region_offsets) region_offsets[nr] = i;
-            }
-            ++nr;
-        }
-        if (triangles) for (int j = 0; j < 3; ++j) triangles[(size_t)i * 3 + j] = t[(size_t)o * 3 + j];
-    }
-    if (region_offsets && nr <= cap_regions) region_offsets[nr] = nlive;
+    IM_CUDA(cudaMemcpyAsync(&nr, d_flag + nlive, sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    const int nc = std::min(nr, std::max(cap_regions, 0));   // the regions whose keys and offsets fit
+    if (region_keys && nc > 0) IM_CUDA(cudaMemcpyAsync(region_keys, d_keys, (size_t)nc * 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (region_offsets && nc > 0) IM_CUDA(cudaMemcpyAsync(region_offsets, d_off, (size_t)nc * sizeof(int), cudaMemcpyDeviceToHost, st));
+    if (triangles && n > 0) IM_CUDA(cudaMemcpyAsync(triangles, d_tri, (size_t)n * 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    IM_CUDA(cudaStreamSynchronize(st));
+    if (region_offsets && nr <= cap_regions) region_offsets[nr] = n;
     *n_regions = nr;
     return nr <= cap_regions ? IMMESH_OK : im_fail(IMMESH_E_CAPACITY, "more regions than cap_regions");
 }
@@ -1823,7 +1852,7 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     cudaStream_t st = h->stream;
     int cnt[IM_MC_HOST];
     IM_CUDA(mesh_read_counters(h, cnt));
-    const int nv = cnt[IM_MC_VERTICES], nalloc = std::min(cnt[IM_MC_TRIS_ALLOC], h->M.max_t), nlive = cnt[IM_MC_TRIS_LIVE];
+    const int nv = cnt[IM_MC_VERTICES], nlive = cnt[IM_MC_TRIS_LIVE];
     const size_t nl = (size_t)std::max(nlive, 1);
     // scratch buffer i of the call, at least `bytes` long (grow-only, kept by the handle)
     auto grown = [h](int i, size_t bytes, void** out) {
@@ -1831,69 +1860,42 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
         *out = h->region_scratch[i];
         return e;
     };
-    void *p_slot, *p_rk, *p_k, *p_v, *p_flag, *p_misc, *p_q;
-    IM_CUDA(grown(0, nl * sizeof(int), &p_slot));
-    IM_CUDA(grown(1, nl * sizeof(unsigned long long), &p_rk));
-    IM_CUDA(grown(2, nl * 2 * sizeof(unsigned int), &p_k));
-    IM_CUDA(grown(3, nl * 2 * sizeof(unsigned int), &p_v));
-    IM_CUDA(grown(4, (nl + 1) * sizeof(int), &p_flag));
-    IM_CUDA(grown(5, 8 * sizeof(int), &p_misc));
-    IM_CUDA(grown(6, std::max<size_t>(qk.size(), 1) * (sizeof(unsigned long long) + sizeof(int)), &p_q));
-    int* slot = (int*)p_slot;
-    unsigned long long* rk = (unsigned long long*)p_rk;
-    unsigned int* ku[2] = {(unsigned int*)p_k, (unsigned int*)p_k + nl};
-    unsigned int* vu[2] = {(unsigned int*)p_v, (unsigned int*)p_v + nl};
+    void *p_order, *p_flag, *p_misc, *p_q;
+    TriOrder o = {};
+    IM_CUDA(grown(0, tri_order_carve(nullptr, (int)nl, 3, o) * sizeof(unsigned int), &p_order));
+    tri_order_carve((unsigned int*)p_order, (int)nl, 3, o);
+    IM_CUDA(grown(1, (nl + 1) * sizeof(int), &p_flag));
+    IM_CUDA(grown(2, 8 * sizeof(int), &p_misc));
+    IM_CUDA(grown(3, std::max<size_t>(qk.size(), 1) * (sizeof(unsigned long long) + sizeof(int)), &p_q));
     int* flag = (int*)p_flag;
-    int* misc = (int*)p_misc;   // [0] kept triangles, [1] key out of range, [2] vertices claimed, [3] regions
+    int* misc = (int*)p_misc;   // [0] vertices claimed, [1] regions
     unsigned long long* d_qk = (unsigned long long*)p_q;
     int* d_qv = (int*)(d_qk + std::max<size_t>(qk.size(), 1));
-    int hm[4] = {0, 0, 0, 0};
-    IM_CUDA(cudaMemsetAsync(misc, 0, 8 * sizeof(int), st));
     if (use_keys) {
         IM_CUDA(cudaMemcpyAsync(d_qk, qk.data(), qk.size() * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
         IM_CUDA(cudaMemcpyAsync(d_qv, qv.data(), qv.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     }
-    if (nalloc > 0)
-        IM_LAUNCH(k_rb_select, mesh_grid(h, nalloc, RB_THREADS), RB_THREADS, 0, st, h->M, nalloc, region_size, (const unsigned long long*)d_qk, (const int*)d_qv, qmask,
-                  use_keys ? 1 : 0, slot, rk, misc);
-    IM_CUDA(cudaGetLastError());
-    IM_CUDA(cudaMemcpyAsync(hm, misc, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    IM_CUDA(cudaStreamSynchronize(st));
-    if (hm[1]) return im_fail(IMMESH_E_RANGE, "region_buffers: a region key is out of range (region_size too small for the mesh's extent)");
-    const int n = hm[0];
+    o.qkeys = use_keys ? d_qk : nullptr;
+    o.qval = d_qv;
+    o.qmask = qmask;
+    IM_CUDA(cudaMemsetAsync(misc, 0, 8 * sizeof(int), st));
+    if (const int rc = mesh_tri_order(h, cnt, region_size, o)) return rc;
+    if (o.range) return im_fail(IMMESH_E_RANGE, "region_buffers: a region key is out of range (region_size too small for the mesh's extent)");
+    const int n = o.n;
     int nr = use_keys ? nk : 0;
-    // (region, triple) order
-    int cur = 0;
-    if (n > 0) {
-        const int nb = (n + VG_TILE - 1) / VG_TILE;
-        void* p_hist;
-        IM_CUDA(grown(7, (size_t)256 * nb * sizeof(int), &p_hist));
-        int* hist = (int*)p_hist;
-        const int g = mesh_grid(h, n, RB_THREADS);
-        const int tri_passes = rb_passes((unsigned long long)std::max(nv - 1, 0));
-        const int n_words = use_keys ? 4 : 5;   // k, j, i, region (index, or the two halves of the packed key)
-        for (int w = 0; w < n_words; ++w) {
-            const int passes = w < 3 ? tri_passes : use_keys ? rb_passes((unsigned long long)std::max(nk - 1, 0)) : 4;
-            IM_LAUNCH(k_rb_word, g, RB_THREADS, 0, st, h->M, n, w, (const int*)slot, (const unsigned long long*)rk, w == 0 ? (const unsigned int*)nullptr : (const unsigned int*)vu[cur],
-                      ku[cur ^ 1], vu[cur ^ 1]);
-            cur = rs_sort_passes(st, ku, vu, cur ^ 1, n, passes, hist);
-        }
-        if (!use_keys) {
-            IM_LAUNCH(k_rb_starts, g, RB_THREADS, 0, st, n, (const unsigned int*)vu[cur], (const unsigned long long*)rk, flag);
-            IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, flag, n, misc + 3);
-            IM_CUDA(cudaGetLastError());
-            IM_CUDA(cudaMemcpyAsync(hm + 3, misc + 3, sizeof(int), cudaMemcpyDeviceToHost, st));
-            IM_CUDA(cudaStreamSynchronize(st));
-            nr = hm[3];
-        }
+    if (n > 0 && !use_keys) {
+        IM_LAUNCH(k_rb_starts, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, o.order, (const int*)o.reg, flag);
+        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, flag, n, misc + 1);
+        IM_CUDA(cudaGetLastError());
+        IM_CUDA(cudaMemcpyAsync(&nr, misc + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaStreamSynchronize(st));
     }
     *n_tris = n;
     *n_regions = nr;
     if (n > cap || nr > cap_regions)
         return im_fail(IMMESH_E_CAPACITY, "region_buffers: more triangles than cap or more regions than cap_regions (*n_tris / *n_regions hold the numbers needed; nothing was smoothed)");
-    const unsigned int* order = vu[cur];
     void *p_reg, *p_rows, *p_part, *p_box;
-    IM_CUDA(grown(8, ((size_t)nr * 3 + (size_t)nr + 1) * sizeof(int), &p_reg));
+    IM_CUDA(grown(4, ((size_t)nr * 3 + (size_t)nr + 1) * sizeof(int), &p_reg));
     int* d_rkeys = (int*)p_reg;
     int* d_roff = d_rkeys + (size_t)nr * 3;
     int* h_off_src = nullptr;
@@ -1902,29 +1904,28 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
         zeros.assign((size_t)nr + 1, 0);
         h_off_src = zeros.data();
     } else if (use_keys) {
-        IM_LAUNCH(k_rb_offsets, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, nk, order, (const unsigned long long*)rk, d_roff);
+        IM_LAUNCH(k_rb_offsets, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, nk, o.order, (const int*)o.reg, d_roff);
     } else {
-        IM_LAUNCH(k_rb_regions, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, order, (const unsigned long long*)rk, (const int*)flag, d_rkeys, d_roff);
+        IM_LAUNCH(k_rb_regions, mesh_grid(h, n, RB_THREADS), RB_THREADS, 0, st, n, o.order, (const int*)o.reg, (const int*)flag, d_rkeys, d_roff);
         IM_CUDA(cudaMemcpyAsync(d_roff + nr, &n, sizeof(int), cudaMemcpyHostToDevice, st));
     }
     // lazy smoothing of the kept triangles' vertices (unparse_triangle_set_to_vector, :88-94)
     int nq = 0;
     if (n > 0) {
         void *p_bits, *p_list, *p_qpos;
-        IM_CUDA(grown(9, (((size_t)nv + 31) / 32) * sizeof(unsigned int), &p_bits));
+        IM_CUDA(grown(5, (((size_t)nv + 31) / 32) * sizeof(unsigned int), &p_bits));
         const size_t qmax = (size_t)std::min<long long>((long long)nv, 3LL * n);
-        IM_CUDA(grown(10, qmax * sizeof(int), &p_list));
-        IM_CUDA(grown(11, qmax * sizeof(float4), &p_qpos));
+        IM_CUDA(grown(6, qmax * sizeof(int), &p_list));
+        IM_CUDA(grown(7, qmax * sizeof(float4), &p_qpos));
         IM_CUDA(cudaMemsetAsync(p_bits, 0, (((size_t)nv + 31) / 32) * sizeof(unsigned int), st));
-        IM_LAUNCH(k_rb_claim, mesh_grid(h, 3 * n, RB_THREADS), RB_THREADS, 0, st, h->M, n, (const int*)slot, (unsigned int*)p_bits, misc, (int*)p_list, (float4*)p_qpos);
+        IM_LAUNCH(k_rb_claim, mesh_grid(h, 3 * n, RB_THREADS), RB_THREADS, 0, st, h->M, n, (const int4*)o.rec, (unsigned int*)p_bits, misc, (int*)p_list, (float4*)p_qpos);
         IM_CUDA(cudaGetLastError());
-        IM_CUDA(cudaMemcpyAsync(hm + 2, misc + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
+        IM_CUDA(cudaMemcpyAsync(&nq, misc, sizeof(int), cudaMemcpyDeviceToHost, st));
         IM_CUDA(cudaStreamSynchronize(st));
-        nq = hm[2];
         if (nq > 0) {
             void *p_idx, *p_d2;
-            IM_CUDA(grown(12, (size_t)nq * knn * sizeof(int), &p_idx));
-            IM_CUDA(grown(13, (size_t)nq * knn * sizeof(float), &p_d2));
+            IM_CUDA(grown(8, (size_t)nq * knn * sizeof(int), &p_idx));
+            IM_CUDA(grown(9, (size_t)nq * knn * sizeof(float), &p_d2));
             IM_LAUNCH(k_knn, mesh_grid(h, nq * 32, 128), 128, 0, st, h->M, h->P, (const float*)p_qpos, 4, nq, knn, (double)INFINITY, (int*)p_idx, (float*)p_d2);
             IM_LAUNCH(k_rb_smooth, mesh_grid(h, nq, RB_THREADS), RB_THREADS, 0, st, h->M, nq, knn, (const int*)p_list, (const int*)p_idx, (const float*)p_d2, smooth_factor, h->P.accept);
         }
@@ -1932,14 +1933,14 @@ int immesh_mesh_region_buffers(immesh_mesh_t* h, double region_size, const int32
     if (n_smoothed) *n_smoothed = nq;
     // rows + axis box
     const int ge = mesh_grid(h, std::max(n, 1), RB_THREADS);
-    IM_CUDA(grown(14, std::max<size_t>((size_t)n, 1) * 12 * sizeof(float), &p_rows));
-    IM_CUDA(grown(15, (size_t)ge * sizeof(AxisAcc) + 8 * sizeof(float), &p_part));
+    IM_CUDA(grown(10, std::max<size_t>((size_t)n, 1) * 12 * sizeof(float), &p_rows));
+    IM_CUDA(grown(11, (size_t)ge * sizeof(AxisAcc) + 8 * sizeof(float), &p_part));
     float* d_rows = (float*)p_rows;
     int* d_ids = (int*)(d_rows + (size_t)std::max(n, 1) * 9);
     AxisAcc* part = (AxisAcc*)p_part;
     p_box = (void*)(part + ge);
     if (n > 0) {
-        IM_LAUNCH(k_rb_emit, ge, RB_THREADS, 0, st, h->M, n, order, (const int*)slot, d_rows, d_ids, part);
+        IM_LAUNCH(k_rb_emit, ge, RB_THREADS, 0, st, h->M, n, o.order, (const int4*)o.rec, d_rows, d_ids, part);
         if (axis_min_max) {
             IM_CUDA(cudaMemcpyAsync(p_box, axis_min_max, 6 * sizeof(float), cudaMemcpyHostToDevice, st));
             IM_LAUNCH(k_rb_axis, 1, 1, 0, st, (const AxisAcc*)part, ge, (float*)p_box);
