@@ -43,6 +43,15 @@ EVAL_COUNT_KEYS = ("live_triangles", "degenerate", "samples", "gt_points", "samp
 EVAL_METRIC_KEYS = ("maxmin_deg", "c2se", "accuracy", "completeness", "precision", "recall", "fscore")
 
 
+class _ViewStyle(C.Structure):
+    _fields_ = [("positions", C.c_int), ("color_by_height", C.c_int), ("z_range", C.c_double * 2)]
+
+
+def _view_style(positions, color_by_height, z_range):
+    lo, hi = (float("nan"), float("nan")) if z_range is None else (float(z_range[0]), float(z_range[1]))
+    return _ViewStyle(int(positions), 1 if color_by_height else 0, (C.c_double * 2)(lo, hi))
+
+
 class _ImuCfg(C.Structure):
     _fields_ = [("cov_gyr", C.c_double * 3), ("cov_acc", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3),
                 ("mean_acc_norm", C.c_double), ("lid_R", C.c_double * 9), ("lid_T", C.c_double * 3), ("max_points", C.c_int), ("max_imu", C.c_int)]
@@ -165,6 +174,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_reinforce_enable", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int]),
         ("immesh_mesh_reinforce_pose", [vp, dp, dp]),
         ("immesh_mesh_reinforced_cloud", [vp, fp, fp, C.POINTER(C.c_int32), C.c_int, ip, dp]),
+        ("immesh_mesh_render_view", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, dp, dp, C.POINTER(_ViewStyle), C.POINTER(C.c_uint8), fp]),
+        ("immesh_mesh_view_enable", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.POINTER(_ViewStyle)]),
+        ("immesh_mesh_view_pose", [vp, dp, dp, C.c_int]),
+        ("immesh_mesh_view_image", [vp, C.POINTER(C.c_uint8), fp, dp, C.POINTER(C.c_int64)]),
         ("immesh_mesh_changes_enable", [vp, C.c_int64, C.c_int]),
         ("immesh_mesh_changes", [vp, C.c_int64, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int32), C.c_int64, fp, C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
@@ -700,6 +713,55 @@ class Mesh:
         _check(self.lib, self.lib.immesh_mesh_reinforced_cloud(self._h, depth.ctypes.data_as(C.POINTER(C.c_float)), pts.ctypes.data_as(C.POINTER(C.c_float)),
                                                                pix.ctypes.data_as(C.POINTER(C.c_int32)), n.value, C.byref(n), pose.ctypes.data_as(dp)), "mesh_reinforced_cloud")
         return depth, pts[:n.value].copy(), pix[:n.value].copy(), pose[:9].reshape(3, 3).copy(), pose[9:].copy()
+
+    def render_view(self, intrinsics, width, height, z_near, z_far, cam_R, cam_t, positions=0, color_by_height=False, z_range=None):
+        """(rgba uint8[h,w,4], depth float32[h,w]) -- the viewer's shaded image of the live mesh at the caller's camera (positions 0: raw,
+        1: smoothed where the vertex is smoothed; z_range None: the height colour's range from the mesh)."""
+        K = np.ascontiguousarray(intrinsics, dtype=np.float64)
+        R = np.ascontiguousarray(cam_R, dtype=np.float64).reshape(9)
+        t = np.ascontiguousarray(cam_t, dtype=np.float64).reshape(3)
+        rgba = np.zeros((height, width, 4), dtype=np.uint8)
+        depth = np.zeros((height, width), dtype=np.float32)
+        st = _view_style(positions, color_by_height, z_range)
+        dp = C.POINTER(C.c_double)
+        _check(self.lib, self.lib.immesh_mesh_render_view(self._h, K.ctypes.data_as(dp), width, height, z_near, z_far, R.ctypes.data_as(dp), t.ctypes.data_as(dp),
+                                                          C.byref(st), rgba.ctypes.data_as(C.POINTER(C.c_uint8)), depth.ctypes.data_as(C.POINTER(C.c_float))),
+               "mesh_render_view")
+        return rgba, depth
+
+    def view_enable(self, intrinsics=None, width=640, height=480, z_near=0.1, z_far=1500.0, win=1, positions=0, color_by_height=False, z_range=None):
+        """Queue the shaded view behind every frame (intrinsics None: the reference's camera, reinforce_intrinsics), sensor-bound."""
+        if intrinsics is None:
+            intrinsics = reinforce_intrinsics(width, height)
+        K = np.ascontiguousarray(intrinsics, dtype=np.float64)
+        st = _view_style(positions, color_by_height, z_range)
+        _check(self.lib, self.lib.immesh_mesh_view_enable(self._h, K.ctypes.data_as(C.POINTER(C.c_double)), width, height, z_near, z_far, win, C.byref(st)),
+               "mesh_view_enable")
+        self._vw_shape = (height, width)
+
+    def view_disable(self):
+        _check(self.lib, self.lib.immesh_mesh_view_enable(self._h, None, 0, 0, 0.0, 0.0, 0, None), "mesh_view_enable")
+
+    def view_pose(self, cam_R=None, cam_t=None, follow=False):
+        """The queued view's camera from the next frame on: None the sensor-bound pose; (cam_R, cam_t) a fixed camera; with follow, the
+        rotation cam_R at the sensor window's mean position plus the offset cam_t."""
+        dp = C.POINTER(C.c_double)
+        if cam_R is None:
+            _check(self.lib, self.lib.immesh_mesh_view_pose(self._h, None, None, 0), "mesh_view_pose")
+            return
+        R = np.ascontiguousarray(cam_R, dtype=np.float64).reshape(9)
+        t = np.ascontiguousarray(cam_t, dtype=np.float64).reshape(3)
+        _check(self.lib, self.lib.immesh_mesh_view_pose(self._h, R.ctypes.data_as(dp), t.ctypes.data_as(dp), 1 if follow else 0), "mesh_view_pose")
+
+    def view_image(self):
+        """(rgba uint8[h,w,4], depth float32[h,w], cam_R float64[3,3], cam_t float64[3], frame) of the newest queued frame."""
+        rgba = np.zeros(self._vw_shape + (4,), dtype=np.uint8)
+        depth = np.zeros(self._vw_shape, dtype=np.float32)
+        pose = np.zeros(12)
+        frame = C.c_int64(0)
+        _check(self.lib, self.lib.immesh_mesh_view_image(self._h, rgba.ctypes.data_as(C.POINTER(C.c_uint8)), depth.ctypes.data_as(C.POINTER(C.c_float)),
+                                                         pose.ctypes.data_as(C.POINTER(C.c_double)), C.byref(frame)), "mesh_view_image")
+        return rgba, depth, pose[:9].reshape(3, 3).copy(), pose[9:].copy(), frame.value
 
     def changes_enable(self, max_rows=1 << 20, max_frames=256):
         """Record every later frame's triangle changes on the device: a ring of max_rows rows, the headers of the last max_frames frames.

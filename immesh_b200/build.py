@@ -155,6 +155,15 @@ def build_reinforce(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "reinforce", "emu_reinforce.cpp"), EMU_REINFORCE, force)
 
 
+EMU_VIEW = os.path.join(_ROOT, "tests", "view", "libimmesh_emu_view.so")
+
+
+def build_view(force=False):
+    """tests/view: the shaded view's visibility, shading and height-colour bodies and its camera sources (immesh_b200/csrc/reinforce.cuh)
+    in the tiled rasteriser's orchestration, built for the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "view", "emu_view.cpp"), EMU_VIEW, force)
+
+
 EMU_CHANGES = os.path.join(_ROOT, "tests", "changes", "libimmesh_emu_changes.so")
 
 
@@ -220,6 +229,7 @@ def build_all(force=False):
     build_growth(force)
     build_imu_chain(force)
     build_reinforce(force)
+    build_view(force)
     build_changes(force)
     build_eval(force)
     build_local_map(force)

@@ -193,6 +193,24 @@ struct immesh_mesh {
         RfImage img;                      // result buffer (frame & 1) holds the frame's image and pose
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
     } rf;
+    // the viewer's shaded image (immesh_mesh_view_enable queues it behind every frame; immesh_mesh_render_view builds one for a call)
+    struct View {
+        int on = 0, win = 1;
+        int last_frame = 0;               // newest frame queued with the view (0: none since enable)
+        int mode = 0;                     // the camera source (RfDyn::mode): 0 sensor-bound, 1 the caller's fixed pose, 2 the follow camera
+        double R[9] = {}, t[3] = {};
+        int pos = 0, color = 0, auto_range = 0;   // immesh_view_style: positions, color_by_height, z range from the mesh
+        immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
+        void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
+        void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
+        RfImage img;                      // binning buffers; out[b].depth and out[b].pose of result buffer b
+        uchar4* rgba[2] = {};             // the colour image of result buffer b
+        float* zr = nullptr;              // [2] the height colour's z range (the caller's, or k_view_zrange's)
+        unsigned int* zr_part = nullptr;  // [2 zr_blocks] k_view_zrange's per-block partials
+        int* zr_done = nullptr;           // k_view_zrange's finished-block counter (0 between launches)
+        int zr_blocks = 1;
+        immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
+    } vw;
     // change feed (immesh_mesh_changes_enable); its per-frame pointers are in F (chg_stamp, chg_list, chg_cnt, chg_cap)
     struct Changes {
         int on = 0;

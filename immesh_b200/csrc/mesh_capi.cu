@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(128) k_smooth_all(MeshDev M, int nv, int k, co
 // valid pixels in ascending pixel order (k_rf_fcount -> k_rf_scan -> k_rf_emit).  The blocking immesh_mesh_render_depth runs it at the
 // caller's pose; the queued reinforcement (immesh_mesh_reinforce_enable) runs it behind every frame, on the mesh stream and inside its
 // graph, after the camera pose (k_rf_pose), into result buffer (frame & 1).
-struct RfDyn { int mode, pad; double R[9], t[3]; };   // per frame: mode 1 = the caller's pose (immesh_mesh_reinforce_pose)
+struct RfDyn { int mode, pad; double R[9], t[3]; };   // per frame: rf_frame_pose's source (1 = the caller's pose, 2 = the view's follow camera)
 // one block: the frame's camera (sensor-bound or the caller's), the tile counters cleared
 __global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const int* ring_frame, const FrameDyn* dyn, const RfDyn* rd, int win, DepthCam base,
                                                  DepthCam* cam, RfOut o0, RfOut o1, int* tile_cnt, int ntiles) {
@@ -420,12 +420,7 @@ __global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const
     if (threadIdx.x != 0) return;
     const int frame = dyn->frame;
     double R[9], t[3];
-    if (rd->mode == 1) {
-        for (int i = 0; i < 9; ++i) R[i] = rd->R[i];
-        for (int i = 0; i < 3; ++i) t[i] = rd->t[i];
-    } else {
-        rf_avr_pose(ring, ring_frame, frame, win, R, t);
-    }
+    rf_frame_pose(ring, ring_frame, frame, win, rd->mode, rd->R, rd->t, R, t);
     for (int i = 0; i < 9; ++i) base.R[i] = R[i];
     for (int i = 0; i < 3; ++i) base.t[i] = t[i];
     *cam = base;
@@ -433,19 +428,21 @@ __global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const
     for (int i = 0; i < 9; ++i) pose[i] = R[i];
     for (int i = 0; i < 3; ++i) pose[9 + i] = t[i];
 }
+// the position a binning pass reads (view_vertex; pos_mode 0, the depth image's, is M.vpos)
+__device__ __forceinline__ float4 rf_vertex(const MeshDev& M, int pos_mode, int v) { return view_vertex(M.vpos, M.vsmooth, M.vsmoothed, pos_mode, v); }
 // the screen tiles a triangle's pixel box touches
 __device__ __forceinline__ void rf_tiles(const DepthTri& T, int* tx0, int* tx1, int* ty0, int* ty1) {
     *tx0 = T.x_lo / IM_RT_TILE; *tx1 = T.x_hi / IM_RT_TILE; *ty0 = T.y_lo / IM_RT_TILE; *ty1 = T.y_hi / IM_RT_TILE;
 }
-// count pass: bin entries per tile
-__global__ void __launch_bounds__(128) k_rf_count(MeshDev M, const DepthCam* cam, int* tile_cnt) {
+// count pass: bin entries per tile (positions by pos_mode)
+__global__ void __launch_bounds__(128) k_rf_count(MeshDev M, int pos_mode, const DepthCam* cam, int* tile_cnt) {
     const DepthCam C = *cam;
     const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
         DepthTri T;
-        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
+        if (!depth_tri_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &T)) continue;
         int tx0, tx1, ty0, ty1;
         rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
         for (int ty = ty0; ty <= ty1; ++ty)
@@ -467,7 +464,7 @@ __global__ void __launch_bounds__(1024) k_rf_scan(const int* cnt, int n, int* of
     }
 }
 // fill pass: triangle slots into the bins (order inside a bin is free: the tile takes the minimum)
-__global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, const DepthCam* cam, int* cur, int* bin, const int* misc) {
+__global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, int pos_mode, const DepthCam* cam, int* cur, int* bin, const int* misc) {
     if (misc[0]) return;
     const DepthCam C = *cam;
     const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
@@ -475,7 +472,7 @@ __global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, const DepthCam* cam,
         const int4 r = M.tri[t];
         if (!r.w) continue;
         DepthTri T;
-        if (!depth_tri_setup(C, M.vpos[r.x], M.vpos[r.y], M.vpos[r.z], &T)) continue;
+        if (!depth_tri_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &T)) continue;
         int tx0, tx1, ty0, ty1;
         rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
         for (int ty = ty0; ty <= ty1; ++ty)
@@ -543,6 +540,110 @@ __global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const F
         o.pix[k] = i;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) *o.n = blk_off[nb];
+}
+
+// ---- the viewer's shaded image of the live mesh (draw_triangle with the facet shader, mesh_rec_display.cpp:273-282; the rule is
+// immesh_mesh_render_view's, include/immesh_b200.h).  The binning passes of the depth image (k_rf_count -> k_rf_scan -> k_rf_fill,
+// with the view's positions), the z range of the height colour when it is automatic (k_view_zrange), then one block per tile
+// (k_view_tile): the nearest sample with the triple tie-break per pixel, shaded from the winning triangle.  The blocking
+// immesh_mesh_render_view runs it at the caller's camera; the queued view (immesh_mesh_view_enable) behind every frame after the
+// reinforcement, its camera from k_rf_pose, into result buffer (frame & 1).
+struct ViewOut { uchar4* rgba; float* depth; };
+#define VIEW_ZR_THREADS 128
+// min / max z (view_ordered) over the vertices of the live triangles: per-block partials, reduced by the last block to finish into
+// zr[0], zr[1]; the last block resets the done counter for the next launch
+__global__ void __launch_bounds__(VIEW_ZR_THREADS) k_view_zrange(MeshDev M, int pos_mode, unsigned int* part, int* done, float* zr) {
+    __shared__ unsigned int s_lo[VIEW_ZR_THREADS / 32], s_hi[VIEW_ZR_THREADS / 32];
+    __shared__ bool s_last;
+    const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned int lo = 0xffffffffu, hi = 0u;
+    for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
+        const int4 r = M.tri[t];
+        if (!r.w) continue;
+        const int v[3] = {r.x, r.y, r.z};
+        for (int k = 0; k < 3; ++k) {
+            const unsigned int u = view_ordered(rf_vertex(M, pos_mode, v[k]).z);
+            lo = min(lo, u); hi = max(hi, u);
+        }
+    }
+    auto block_reduce = [&](unsigned int& a, unsigned int& b) {
+        a = __reduce_min_sync(0xffffffffu, a); b = __reduce_max_sync(0xffffffffu, b);
+        if (lane == 0) { s_lo[warp] = a; s_hi[warp] = b; }
+        __syncthreads();
+        if (threadIdx.x == 0)
+            for (int w = 1; w < VIEW_ZR_THREADS / 32; ++w) { a = min(a, s_lo[w]); b = max(b, s_hi[w]); }
+    };
+    block_reduce(lo, hi);
+    if (threadIdx.x == 0) {
+        part[2 * blockIdx.x] = lo; part[2 * blockIdx.x + 1] = hi;
+        __threadfence();
+        s_last = atomicAdd(done, 1) == (int)gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    lo = 0xffffffffu; hi = 0u;
+    for (int b = threadIdx.x; b < (int)gridDim.x; b += blockDim.x) {
+        lo = min(lo, __ldcg(part + 2 * b)); hi = max(hi, __ldcg(part + 2 * b + 1));
+    }
+    __syncthreads();   // s_lo / s_hi are reused
+    block_reduce(lo, hi);
+    if (threadIdx.x == 0) { zr[0] = view_unordered(lo); zr[1] = view_unordered(hi); *done = 0; }
+}
+// one block per tile, one thread per pixel (k_rf_tile's shape): the bin's set-ups and (a, b, c, slot) records staged IM_RT_THREADS at
+// a time in shared memory; each thread keeps its pixel's best (depth bits, triple, slot) in registers, then shades the winner and
+// writes the pixel's colour and depth.  Bins over capacity (misc[0]): every triangle slot instead, the same image.
+__global__ void __launch_bounds__(IM_RT_THREADS) k_view_tile(MeshDev M, int pos_mode, int color, const float* zr, const DepthCam* cam, const int* tile_off,
+                                                             const int* bin, const int* misc, const FrameDyn* dyn, ViewOut o0, ViewOut o1) {
+    __shared__ DepthTri S[IM_RT_THREADS];
+    __shared__ int4 Q[IM_RT_THREADS];
+    const DepthCam C = *cam;
+    const int ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    const int x = (blockIdx.x % ntx) * IM_RT_TILE + (int)(threadIdx.x % IM_RT_TILE), y = (blockIdx.x / ntx) * IM_RT_TILE + (int)(threadIdx.x / IM_RT_TILE);
+    const bool all = misc[0] != 0;
+    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t) : tile_off[blockIdx.x + 1];
+    unsigned int best = 0x7f800000u;   // +inf: nothing drawn
+    int ba = INT_MAX, bb = INT_MAX, bc = INT_MAX, bs = -1;
+    for (int b = lo; b < hi; b += IM_RT_THREADS) {
+        const int i = b + (int)threadIdx.x;
+        bool ok = false;
+        if (i < hi) {
+            const int slot = all ? i : bin[i];
+            const int4 r = M.tri[slot];
+            ok = r.w && depth_tri_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &S[threadIdx.x]);
+            Q[threadIdx.x] = make_int4(r.x, r.y, r.z, slot);
+        }
+        if (!ok) { S[threadIdx.x].x_lo = 1; S[threadIdx.x].x_hi = 0; }   // an empty box
+        __syncthreads();
+        const int n = min(IM_RT_THREADS, hi - b);
+        for (int j = 0; j < n; ++j) {
+            const DepthTri& T = S[j];
+            if (x < T.x_lo || x > T.x_hi || y < T.y_lo || y > T.y_hi) continue;
+            float zf;
+            if (!depth_sample(T, x, y, &zf)) continue;
+            const unsigned int bits = __float_as_uint(zf);
+            const int4 q = Q[j];
+            if (bits < 0x7f800000u && view_better(bits, q.x, q.y, q.z, best, ba, bb, bc)) { best = bits; ba = q.x; bb = q.y; bc = q.z; bs = q.w; }
+        }
+        __syncthreads();
+    }
+    if (x >= C.w || y >= C.h) return;
+    const ViewOut o = (dyn->frame & 1) ? o1 : o0;
+    const size_t px = (size_t)y * C.w + x;
+    const float val = __uint_as_float(best);
+    o.depth[px] = depth_valid(C, val) ? val : -1.0f;
+    uchar4 c = make_uchar4(0, 0, 0, 255);
+    if (bs >= 0) {
+        const int4 r = M.tri[bs];
+        const float4 p[3] = {rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z)};
+        DepthTri T;
+        depth_tri_setup(C, p[0], p[1], p[2], &T);
+        const float zlo = color ? zr[0] : 0.f, zhi = color ? zr[1] : 0.f;
+        double col[3][3];
+        for (int k = 0; k < 3; ++k) view_color(color, p[k].z, zlo, zhi, col[k]);
+        c = view_shade(T, x, y, p, col, C.t);
+    }
+    o.rgba[px] = c;
 }
 
 // ---- the region segments of records in region order (mesh_tri_order with a region size): the region stream and the viewer's region
@@ -1267,12 +1368,16 @@ static cudaError_t rf_image_alloc(immesh::MemSet& dev, int w, int h, int nout, R
 }
 // the image of the camera in im.cam, with the tile counters zeroed, into result buffer (dyn->frame & 1) (fixed grids: every
 // per-image value is read on the device)
-static void rf_image_launch(const immesh_mesh* h, const RfImage& im, const FrameDyn* dyn, cudaStream_t st) {
+// the binning passes of an image: the triangles at positions pos_mode (view_vertex) into the tiles' bins
+static void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st) {
     const int g = h->n_sm * 8;
-    const DepthCam* cam = im.cam;
-    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, cam, im.tile_cnt);
+    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, pos_mode, (const DepthCam*)im.cam, im.tile_cnt);
     IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.tile_cnt, im.ntiles, im.tile_off, im.tile_cnt, im.bin_cap, im.misc);
-    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, cam, im.tile_cnt, im.bin, (const int*)im.misc);
+    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, pos_mode, (const DepthCam*)im.cam, im.tile_cnt, im.bin, (const int*)im.misc);
+}
+static void rf_image_launch(const immesh_mesh* h, const RfImage& im, const FrameDyn* dyn, cudaStream_t st) {
+    const DepthCam* cam = im.cam;
+    rf_bin_launch(h, im, 0, st);
     IM_LAUNCH(k_rf_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, cam, (const int*)im.tile_off, (const int*)im.bin, (const int*)im.misc, im.depth_bits);
     IM_LAUNCH(k_rf_fcount, im.nb, RF_FIN, 0, st, cam, (const unsigned int*)im.depth_bits, im.blk);
     IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.blk, im.nb, im.blk_off, (int*)nullptr, 0, (int*)nullptr);
@@ -1284,6 +1389,22 @@ static void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st) {
     IM_LAUNCH(k_rf_pose, 1, 256, 0, st, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame, (const FrameDyn*)h->d_dyn, (const RfDyn*)r.rd, r.win, r.base,
               r.img.cam, r.img.out[0], r.img.out[1], r.img.tile_cnt, r.img.ntiles);
     rf_image_launch(h, r.img, h->d_dyn, st);
+}
+// the shaded image of the camera in im.cam (tile counters zeroed) with style v into out[dyn->frame & 1]: binning, the automatic z
+// range when the height colour needs it, the tiles
+static void view_image_launch(const immesh_mesh* h, const immesh_mesh::View& v, const RfImage& im, const ViewOut* out, const FrameDyn* dyn, cudaStream_t st) {
+    rf_bin_launch(h, im, v.pos, st);
+    if (v.color && v.auto_range) IM_LAUNCH(k_view_zrange, v.zr_blocks, VIEW_ZR_THREADS, 0, st, h->M, v.pos, v.zr_part, v.zr_done, v.zr);
+    IM_LAUNCH(k_view_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, v.pos, v.color, (const float*)v.zr, (const DepthCam*)im.cam, (const int*)im.tile_off,
+              (const int*)im.bin, (const int*)im.misc, dyn, out[0], out[1]);
+}
+// the queued view of the frame just queued: its camera (k_rf_pose, pose into the result buffer), then its image
+static void mesh_view_launch(immesh_mesh* h, cudaStream_t st) {
+    auto& v = h->vw;
+    IM_LAUNCH(k_rf_pose, 1, 256, 0, st, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame, (const FrameDyn*)h->d_dyn, (const RfDyn*)v.rd, v.win, v.base,
+              v.img.cam, v.img.out[0], v.img.out[1], v.img.tile_cnt, v.img.ntiles);
+    const ViewOut out[2] = {{v.rgba[0], v.img.out[0].depth}, {v.rgba[1], v.img.out[1].depth}};
+    view_image_launch(h, v, v.img, out, h->d_dyn, st);
 }
 
 static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
@@ -1450,6 +1571,14 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         for (int i = 0; i < 3; ++i) r->t[i] = h->rf.t[i];
         IM_CUDA(cudaMemcpyAsync(h->rf.rd, r, sizeof(RfDyn), cudaMemcpyHostToDevice, st));
     }
+    const bool vw_on = h->vw.on != 0;
+    if (vw_on) {   // the view's camera source of this frame
+        RfDyn* r = (RfDyn*)h->vw.h_rd + s;
+        r->mode = h->vw.mode;
+        for (int i = 0; i < 9; ++i) r->R[i] = h->vw.R[i];
+        for (int i = 0; i < 3; ++i) r->t[i] = h->vw.t[i];
+        IM_CUDA(cudaMemcpyAsync(h->vw.rd, r, sizeof(RfDyn), cudaMemcpyHostToDevice, st));
+    }
     // the frame's launch sequence (fixed grids: grid-stride loops over the counts the kernels read on the device)
     bool nccl_failed = false;
     const int g_pts = mesh_grid_fixed(h, h->max_frame_points, 128);
@@ -1508,6 +1637,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         if (chg_on) mesh_changes_launch(h, F, st, false);
         IM_LAUNCH_PDL(pdl && !chg_on, k_frame_end, 1, 1, 0, st, h->M);
         if (rf_on) mesh_reinforce_launch(h, st);
+        if (vw_on) mesh_view_launch(h, st);
     };
     bool queued = false;
     if (graphed) {
@@ -1526,6 +1656,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     h->inflight[s] = 1;
     h->timed_last = queued ? 0 : 1;
     if (rf_on) h->rf.last_frame = F.frame;
+    if (vw_on) h->vw.last_frame = F.frame;
     if (chg_on) h->chg.last_frame = F.frame;
     return IMMESH_OK;
 }
@@ -1593,6 +1724,7 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a mesh handle with automatic growth cannot be sharded (immesh_mesh_set_growth(h, 0) first)");
     if (h->rf.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the reinforcement enabled cannot be sharded (immesh_mesh_reinforce_enable(h, NULL, ...) first)");
     if (h->chg.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the change feed enabled cannot be sharded (immesh_mesh_changes_enable(h, 0, 0) first)");
+    if (h->vw.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the queued view enabled cannot be sharded (immesh_mesh_view_enable(h, NULL, ...) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);
@@ -2263,6 +2395,127 @@ int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth, float* points, 
     if (points && n > 0) IM_CUDA(cudaMemcpy(points, o.pts, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost));
     if (point_pixel && n > 0) IM_CUDA(cudaMemcpy(point_pixel, o.pix, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
     if (pose_out) std::memcpy(pose_out, pose, sizeof(pose));
+    return IMMESH_OK;
+}
+
+// the style of a view (NULL: raw positions, white); the caller's z range is checked only when the height colour is on
+static int view_style_set(const immesh_view_style* style, const char* what, immesh_mesh::View& v, float* zr) {
+    const immesh_view_style d = {0, 0, {NAN, NAN}}, &s = style ? *style : d;
+    if ((s.positions != 0 && s.positions != 1) || (s.color_by_height != 0 && s.color_by_height != 1))
+        return im_fail(IMMESH_E_INVALID, (std::string(what) + ": bad style (positions and color_by_height are 0 or 1)").c_str());
+    v.pos = s.positions;
+    v.color = s.color_by_height;
+    v.auto_range = v.color && std::isnan(s.z_range[0]) && std::isnan(s.z_range[1]);
+    if (v.color && !v.auto_range) {
+        if (!std::isfinite(s.z_range[0]) || !std::isfinite(s.z_range[1]) || !(s.z_range[0] < s.z_range[1]))
+            return im_fail(IMMESH_E_INVALID, (std::string(what) + ": bad z_range (finite with z_range[0] < z_range[1], or both NaN)").c_str());
+        zr[0] = (float)s.z_range[0];
+        zr[1] = (float)s.z_range[1];
+    }
+    return IMMESH_OK;
+}
+// the buffers of a w x h view with `nbuf` result buffers into v.dev; stops at the first failure
+static cudaError_t view_alloc(immesh_mesh::View& v, int w, int h, int nbuf, int zr_blocks) {
+    const size_t n = (size_t)w * h;
+    cudaError_t e = rf_image_alloc(v.dev, w, h, 0, &v.img);
+    auto add = [&e, &v](auto** p, size_t count) { if (e == cudaSuccess) e = v.dev.alloc(p, std::max<size_t>(count, 1)); };
+    for (int b = 0; b < nbuf; ++b) { add(&v.img.out[b].depth, n); add(&v.img.out[b].pose, 12); add(&v.rgba[b], n); }
+    v.zr_blocks = zr_blocks;
+    add(&v.zr, 2); add(&v.zr_part, 2 * (size_t)zr_blocks); add(&v.zr_done, 1);
+    return e;
+}
+static bool view_camera(const double* K, int width, int height, double z_near, double z_far, DepthCam* C) {
+    if (!K || width < 1 || height < 1 || (long long)width * height > (1 << 26) || !(z_near > 0) || !(z_far > z_near)) return false;
+    C->fx = K[0]; C->fy = K[1]; C->cx = K[2]; C->cy = K[3]; C->z_near = z_near; C->z_far = z_far;
+    C->w = width; C->h = height;
+    return true;
+}
+int immesh_mesh_render_view(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, const double* cam_R, const double* cam_t,
+                            const immesh_view_style* style, uint8_t* rgba, float* depth) {
+    DepthCam C;
+    if (!h || !cam_R || !cam_t || !rgba || !view_camera(intrinsics, width, height, z_near, z_far, &C)) return im_fail(IMMESH_E_INVALID, "render_view: bad argument");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "render_view: a sharded mesh handle is not supported");
+    immesh_mesh::View v;   // this call's buffers; h->vw is not touched, so a queued frame's result stays readable
+    float zr[2] = {0.f, 0.f};
+    if (const int rc = view_style_set(style, "render_view", v, zr)) return rc;
+    for (int i = 0; i < 9; ++i) C.R[i] = cam_R[i];
+    for (int i = 0; i < 3; ++i) C.t[i] = cam_t[i];
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    const cudaError_t e = view_alloc(v, width, height, 1, h->n_sm * 4);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "render_view: allocation of the image buffers failed");
+    }
+    const size_t n = (size_t)width * height;
+    IM_CUDA(cudaMemcpyAsync(v.img.cam, &C, sizeof(C), cudaMemcpyHostToDevice, h->stream));
+    IM_CUDA(cudaMemsetAsync(v.img.tile_cnt, 0, (size_t)v.img.ntiles * sizeof(int), h->stream));
+    IM_CUDA(cudaMemsetAsync(v.zr_done, 0, sizeof(int), h->stream));
+    IM_CUDA(cudaMemcpyAsync(v.zr, zr, sizeof(zr), cudaMemcpyHostToDevice, h->stream));
+    const ViewOut out[2] = {{v.rgba[0], v.img.out[0].depth}, {v.rgba[0], v.img.out[0].depth}};   // k_view_tile picks out[frame & 1]
+    view_image_launch(h, v, v.img, out, h->d_dyn, h->stream);
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(rgba, v.rgba[0], n * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (depth) IM_CUDA(cudaMemcpyAsync(depth, v.img.out[0].depth, n * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    return IMMESH_OK;
+}
+int immesh_mesh_view_enable(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, int win, const immesh_view_style* style) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "view_enable: a sharded mesh handle is not supported (the view runs on a single GPU)");
+    immesh_mesh::View v;   // built in full before it replaces h->vw: after a failure the view stays disabled
+    float zr[2] = {0.f, 0.f};
+    if (intrinsics) {
+        const double* K = intrinsics;
+        if (!view_camera(K, width, height, z_near, z_far, &v.base) || !std::isfinite(z_far) || win < 1 || win > IM_RF_RING - 1 || !std::isfinite(K[0]) ||
+            !std::isfinite(K[1]) || !std::isfinite(K[2]) || !std::isfinite(K[3]) || K[0] == 0.0 || K[1] == 0.0)
+            return im_fail(IMMESH_E_INVALID, "view_enable: bad argument (finite intrinsics with fx, fy != 0; 1 <= width * height <= 2^26; 0 < z_near < z_far < inf; 1 <= win <= 63)");
+        if (const int rc = view_style_set(style, "view_enable", v, zr)) return rc;
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
+    h->graph.destroy();                          // the captured sequence changes
+    h->vw = immesh_mesh::View();                 // the buffers of an earlier enable go
+    if (!intrinsics) return IMMESH_OK;
+    v.win = win;
+    RfDyn *rd = nullptr, *h_rd = nullptr;
+    cudaError_t e = view_alloc(v, width, height, 2, h->n_sm * 4);
+    if (e == cudaSuccess) e = v.dev.alloc(&rd, 1);
+    if (e == cudaSuccess) e = v.pinned.alloc(&h_rd, IM_SLOTS, 0);
+    if (e == cudaSuccess) e = cudaMemsetAsync(v.zr_done, 0, sizeof(int), h->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(v.zr, zr, sizeof(zr), cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "view_enable: allocation of the view's buffers failed");
+    }
+    v.rd = rd;
+    v.h_rd = h_rd;
+    v.on = 1;
+    h->vw = std::move(v);
+    return IMMESH_OK;
+}
+int immesh_mesh_view_pose(immesh_mesh_t* h, const double* cam_R, const double* cam_t, int follow) {
+    if (!h || (!cam_R) != (!cam_t) || (follow != 0 && follow != 1) || (!cam_R && follow))
+        return im_fail(IMMESH_E_INVALID, "view_pose: bad argument (cam_R and cam_t both given or both NULL; follow 0 or 1, and 0 with NULL)");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "view_pose: a sharded mesh handle is not supported");
+    if (!h->vw.on) return im_fail(IMMESH_E_INVALID, "view_pose: the view is not enabled (immesh_mesh_view_enable)");
+    h->vw.mode = cam_R ? (follow ? 2 : 1) : 0;
+    for (int i = 0; i < 9; ++i) h->vw.R[i] = cam_R ? cam_R[i] : 0.0;
+    for (int i = 0; i < 3; ++i) h->vw.t[i] = cam_t ? cam_t[i] : 0.0;
+    return IMMESH_OK;
+}
+int immesh_mesh_view_image(immesh_mesh_t* h, uint8_t* rgba, float* depth, double* pose_out, int64_t* frame_out) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "view_image: a sharded mesh handle is not supported");
+    if (!h->vw.on) return im_fail(IMMESH_E_INVALID, "view_image: the view is not enabled (immesh_mesh_view_enable)");
+    if (!h->vw.last_frame) return im_fail(IMMESH_E_INVALID, "view_image: no frame has been queued since immesh_mesh_view_enable");
+    // the newest frame's result; the next queued frame writes the other buffer, so these copies (legacy stream) do not wait for it
+    const int f = h->vw.last_frame, b = f & 1;
+    const size_t n = (size_t)h->vw.base.w * h->vw.base.h;
+    IM_CUDA(cudaEventSynchronize(h->ev_done[f & (IM_SLOTS - 1)]));
+    if (rgba) IM_CUDA(cudaMemcpy(rgba, h->vw.rgba[b], n * 4, cudaMemcpyDeviceToHost));
+    if (depth) IM_CUDA(cudaMemcpy(depth, h->vw.img.out[b].depth, n * sizeof(float), cudaMemcpyDeviceToHost));
+    if (pose_out) IM_CUDA(cudaMemcpy(pose_out, h->vw.img.out[b].pose, 12 * sizeof(double), cudaMemcpyDeviceToHost));
+    if (frame_out) *frame_out = f;
     return IMMESH_OK;
 }
 

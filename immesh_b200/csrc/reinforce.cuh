@@ -43,11 +43,16 @@ IM_HD bool depth_tri_setup(const DepthCam& C, const float4& p0, const float4& p1
 }
 // the sample at pixel (x, y) inside the triangle's box: covered when the three edge functions share a sign (zero included); the
 // depth is 1 / (1/z interpolated affinely).  Returns whether the sample writes *zf (> 0).
-IM_HD bool depth_sample(const DepthTri& T, int x, int y, float* zf) {
+IM_HD void depth_edges(const DepthTri& T, int x, int y, double* e) {
     const double px = (double)x, py = (double)y;
-    const double e0 = (T.u2 - T.u1) * (py - T.v1) - (T.v2 - T.v1) * (px - T.u1);   // weight of vertex 0
-    const double e1 = (T.u0 - T.u2) * (py - T.v2) - (T.v0 - T.v2) * (px - T.u2);
-    const double e2 = (T.u1 - T.u0) * (py - T.v0) - (T.v1 - T.v0) * (px - T.u0);
+    e[0] = (T.u2 - T.u1) * (py - T.v1) - (T.v2 - T.v1) * (px - T.u1);   // weight of vertex 0
+    e[1] = (T.u0 - T.u2) * (py - T.v2) - (T.v0 - T.v2) * (px - T.u2);
+    e[2] = (T.u1 - T.u0) * (py - T.v0) - (T.v1 - T.v0) * (px - T.u0);
+}
+IM_HD bool depth_sample(const DepthTri& T, int x, int y, float* zf) {
+    double e[3];
+    depth_edges(T, x, y, e);
+    const double e0 = e[0], e1 = e[1], e2 = e[2];
     if (!((e0 >= 0 && e1 >= 0 && e2 >= 0) || (e0 <= 0 && e1 <= 0 && e2 <= 0))) return false;
     const double iz = ((e0 * T.iz0 + e1 * T.iz1) + e2 * T.iz2) / T.area;
     *zf = (float)(1.0 / iz);
@@ -80,6 +85,78 @@ IM_HD unsigned int rt_pixel_min(const DepthTri* tris, int n, int x, int y, unsig
         }
     }
     return acc;
+}
+
+// ---- the shaded view (immesh_mesh_render_view's image rule, include/immesh_b200.h): the viewer's facet shader (if_light, face mode)
+// at the winning sample of the same rasteriser.
+// the vertex position drawn: pos_mode 0 the raw position; 1 the stored smoothed position (as float) where m_smoothed is set
+IM_HD float4 view_vertex(const float4* vpos, const double* vsmooth, const unsigned char* vsmoothed, int pos_mode, int v) {
+    if (pos_mode == 1 && vsmoothed && vsmoothed[v])
+        return make_float4((float)vsmooth[(size_t)v * 3 + 0], (float)vsmooth[(size_t)v * 3 + 1], (float)vsmooth[(size_t)v * 3 + 2], 0.f);
+    return vpos[v];
+}
+// the visibility order: the nearer sample (smaller depth bits) wins; on equal bits the lower (a, b, c) triple
+IM_HD bool view_better(unsigned int bits, int a, int b, int c, unsigned int best_bits, int ba, int bb, int bc) {
+    if (bits != best_bits) return bits < best_bits;
+    if (a != ba) return a < ba;
+    if (b != bb) return b < bb;
+    return c < bc;
+}
+// the height colour of one vertex: t = (z - lo) / (hi - lo) in float (0 when hi == lo), s = clamp(1 - t, 0, 1) at 4 s on the ramp
+// blue, cyan, green, yellow, red (linear between neighbouring stops), each channel truncated to a byte
+IM_HD void view_heat(float z, float lo, float hi, unsigned char* rgb) {
+    const float val = hi == lo ? 0.0f : (z - lo) / (hi - lo);
+    double s = 1.0 - (double)val;
+    s = s < 0.0 ? 0.0 : (s > 1.0 ? 1.0 : s);
+    const double a = s * 4.0, i = floor(a), f = a - i;
+    // the five stops, channel by channel (r, g, b)
+    const double stop[5][3] = {{0, 0, 1}, {0, 1, 1}, {0, 1, 0}, {1, 1, 0}, {1, 0, 0}};
+    const int i0 = (int)i, i1 = (int)ceil(a);
+    for (int k = 0; k < 3; ++k) rgb[k] = (unsigned char)(((1.0 - f) * stop[i0][k] + f * stop[i1][k]) * 255.0);
+}
+// a colour channel in [0, 1] to a byte (NaN and below 0 give 0)
+IM_HD unsigned char view_byte(double c) {
+    const double k = c > 0.0 ? (c < 1.0 ? c : 1.0) : 0.0;
+    return (unsigned char)floor(k * 255.0 + 0.5);
+}
+// the shaded colour of the winning triangle (p[3] in stored order, colours col[3][3] in [0, 1]) at pixel (x, y) of its set-up T,
+// lit from the camera position cam_t: face normal, perspective-correct weights e_i / z_i, two-sided diffuse 0.2 + 0.5 |n . l|
+IM_HD uchar4 view_shade(const DepthTri& T, int x, int y, const float4* p, const double (*col)[3], const double* cam_t) {
+    const double P[3][3] = {{p[0].x, p[0].y, p[0].z}, {p[1].x, p[1].y, p[1].z}, {p[2].x, p[2].y, p[2].z}};
+    const double a[3] = {P[1][0] - P[0][0], P[1][1] - P[0][1], P[1][2] - P[0][2]};
+    const double b[3] = {P[2][0] - P[0][0], P[2][1] - P[0][1], P[2][2] - P[0][2]};
+    const double n[3] = {a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]};
+    double e[3];
+    depth_edges(T, x, y, e);
+    const double w0 = e[0] * T.iz0, w1 = e[1] * T.iz1, w2 = e[2] * T.iz2, ws = (w0 + w1) + w2;
+    double l[3], c[3];
+    for (int k = 0; k < 3; ++k) {
+        l[k] = cam_t[k] - ((w0 * P[0][k] + w1 * P[1][k]) + w2 * P[2][k]) / ws;
+        c[k] = ((w0 * col[0][k] + w1 * col[1][k]) + w2 * col[2][k]) / ws;
+    }
+    const double nn = sqrt((n[0] * n[0] + n[1] * n[1]) + n[2] * n[2]), ln = sqrt((l[0] * l[0] + l[1] * l[1]) + l[2] * l[2]);
+    const double d = ((n[0] / nn) * (l[0] / ln) + (n[1] / nn) * (l[1] / ln)) + (n[2] / nn) * (l[2] / ln);
+    const double s = 0.2 + 0.5 * fabs(d);
+    return make_uchar4(view_byte(s * c[0]), view_byte(s * c[1]), view_byte(s * c[2]), 255);
+}
+// a vertex's colour: white, or the height colour of its z
+IM_HD void view_color(int color, float z, float lo, float hi, double* out) {
+    if (!color) { out[0] = out[1] = out[2] = 1.0; return; }
+    unsigned char rgb[3];
+    view_heat(z, lo, hi, rgb);
+    for (int k = 0; k < 3; ++k) out[k] = (double)rgb[k] / 255.0;
+}
+// float min / max through integer atomics: an order-preserving map of the float bits to unsigned int
+IM_HD unsigned int view_ordered(float f) {
+    unsigned int u;
+    memcpy(&u, &f, 4);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+IM_HD float view_unordered(unsigned int u) {
+    u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
 }
 
 // ---- get_last_avr_pose (src/ImMesh_node.cpp:169-206) on the poses the mesher's frames used.  Quaternions are (w, x, y, z).
@@ -199,6 +276,22 @@ IM_HD void rf_avr_pose(const double (*ring)[12], const int* ring_frame, int fram
     rf_quat_from_rot(l2c, c);
     rf_quat_mul(q, c, qc);
     rf_quat_to_rot(qc, R);
+}
+// A queued image's camera for frame `frame` by its per-frame source: mode 0 the sensor-bound pose (rf_avr_pose); 1 the caller's
+// (R_in, t_in); 2 the follow camera (g_follow_cam with tracking_camera(Identity, t_last_avr), ImMesh_node.cpp:434-440): the fixed
+// rotation R_in at the window's mean translation plus the offset t_in (a window without a pose: a zero mean translation).
+IM_HD void rf_frame_pose(const double (*ring)[12], const int* ring_frame, int frame, int win, int mode, const double* R_in, const double* t_in,
+                         double* R, double* t) {
+    if (mode == 1) {
+        for (int i = 0; i < 9; ++i) R[i] = R_in[i];
+        for (int i = 0; i < 3; ++i) t[i] = t_in[i];
+        return;
+    }
+    rf_avr_pose(ring, ring_frame, frame, win, R, t);
+    if (mode == 2) {
+        for (int i = 0; i < 9; ++i) R[i] = R_in[i];
+        for (int i = 0; i < 3; ++i) t[i] = t[i] + t_in[i];
+    }
 }
 
 }  // namespace immesh

@@ -431,6 +431,68 @@ int immesh_mesh_reinforce_enable(immesh_mesh_t* h, const double* intrinsics /*[4
 int immesh_mesh_reinforce_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/);
 int immesh_mesh_reinforced_cloud(immesh_mesh_t* h, float* depth /*[h][w] or NULL*/, float* points /*[cap][3] or NULL*/, int32_t* point_pixel /*[cap] or NULL*/,
                                  int cap, int* n_out, double* pose_out /*[12] or NULL*/);
+/* The mesh viewer's shaded image, rendered on the device: the reference's draw_triangle (src/meshing/mesh_rec_display.cpp:273-282)
+ * with the facet shader in face mode (g_display_face, if_light = true; src/shader/triangle_facets.vs / .fs), for a node without a
+ * display.  A blocking call at the caller's camera, or an image queued behind every frame.  The view reads the mesh and writes nothing
+ * on the handle (no vertex, m_smoothed flag, smoothed position, counter or change-feed row); it never smooths.
+ *   style (NULL: positions 0, white):
+ *     positions 0: the raw vertex positions (immesh_mesh_snapshot's); 1: the stored smoothed position (as float) where the vertex's
+ *       m_smoothed flag is set, the raw position where it is not.  This draws what the viewer shows once its lazy smoothing has run:
+ *       to match the viewer exactly, call immesh_mesh_region_buffers or immesh_mesh_smooth_all first.
+ *     color_by_height 0: white (g_mesh_if_color = false, the viewer's default); 1: the height colour (set_color_by_axis on z).
+ *     z_range: the height colour's range; both NaN: min / max z over the vertices of the live triangles, in the chosen positions, at
+ *       render time.  Read only with color_by_height = 1; then ends that are not finite (other than both NaN) or z_range[0] >=
+ *       z_range[1]: IMMESH_E_INVALID.
+ *   Image rule (defined here, where GL leaves it to the implementation):
+ *     Visibility: immesh_mesh_render_depth's sampling rule unchanged, with the positions of style.positions: samples at integer pixel
+ *       coordinates, covered when the three edge functions share a sign (zero included), 1/z interpolated affinely, a triangle with a
+ *       vertex outside (z_near, z_far) skipped.  At each pixel the nearest sample wins (the smaller bits of its float depth); on equal
+ *       bits the lower (a, b, c) triple of vertex ids, so shared edges are drawn the same whatever the slot or bin order.
+ *     depth [height][width] (may be NULL): what immesh_mesh_render_depth writes -- the metric depth, -1 at or beyond 0.99 z_far or
+ *       where nothing was drawn; with positions 0 equal to immesh_mesh_render_depth's image bit for bit.
+ *     rgba [height][width][4]: the winning triangle's vertices p0 p1 p2 in stored (ascending id) order, in float64 from the float
+ *       positions, evaluated in the order written here without fused multiply-adds:
+ *         normal n = (p1 - p0) x (p2 - p0); weights w_i = e_i (1 / z_i) from the sample's edge functions e_i;
+ *         frag = ((w0 p0 + w1 p1) + w2 p2) / ((w0 + w1) + w2), the vertex colours interpolated with the same weights;
+ *         light at the camera position: l = cam_t - frag;  d = n / |n| . l / |l| (components summed (x + y) + z, |v| likewise);
+ *         per channel c = (0.2 + 0.5 |d|) colour;  byte = floor(clamp(c, 0, 1) 255 + 0.5) (NaN: 0);  alpha 255.
+ *       Every pixel with a sample is shaded (also one whose depth is -1 beyond 0.99 z_far); a pixel without one is opaque black
+ *       (0, 0, 0, 255), the reference's clear colour.
+ *     Height colour of a vertex at z: t = (z - lo) / (hi - lo) in float32 with lo, hi the range as floats (t = 0 when hi == lo, as for
+ *       a flat mesh); s = 1 - t clamped to [0, 1]; on the five stops blue (0,0,1), cyan (0,1,1), green (0,1,0), yellow (1,1,0), red
+ *       (1,0,0) at a = 4 s: the stops floor(a) and ceil(a) mixed (1 - f) c0 + f c1 with f = a - floor(a), in float64; each channel
+ *       truncated to the byte (unsigned char)(c 255); the vertex colour is byte / 255.  White is (1, 1, 1).
+ *   immesh_mesh_render_view: blocking, at the caller's camera (the convention and argument checks of immesh_mesh_render_depth); bad
+ *     style or a sharded handle: IMMESH_E_INVALID.
+ *   immesh_mesh_view_enable: allocates the buffers once and from then on queues the image behind every frame of
+ *     immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async (and reconstruct_from_pointcloud), on the mesh stream after the
+ *     reinforcement and inside the captured graph: no host synchronisation, no allocation.  The batched frames are not followed.
+ *     intrinsics = NULL turns it off and frees the buffers; either call drains the frames in flight and drops the captured graph.
+ *     Arguments as immesh_mesh_reinforce_enable's (bad ones: IMMESH_E_INVALID); enabling starts with the sensor-bound pose.  While the
+ *     view is off, no launch, graph or output changes.  immesh_mesh_shard refuses a handle with the view on.
+ *   immesh_mesh_view_pose(h, cam_R, cam_t, follow), from the next queued frame on:
+ *     NULL, NULL (follow 0): the sensor-bound pose, the reinforcement's camera over `win` frames (the depth-view window with
+ *       g_if_depth_bind_cam, ImMesh_node.cpp:312-319);
+ *     follow 0: the fixed camera (cam_R, cam_t);
+ *     follow 1: the follow camera (g_follow_cam, ImMesh_node.cpp:434-440): rotation cam_R, position the window's mean translation of
+ *       the sensor-bound pose plus cam_t (a window without a pose contributes a zero translation).
+ *     Not enabled, mismatched NULLs, follow not 0 / 1, follow 1 without a pose: IMMESH_E_INVALID.
+ *   immesh_mesh_view_image: blocking read of the newest queued frame's image (waits for that frame only), double-buffered by
+ *     frame & 1: rgba [h][w][4], depth [h][w], pose_out [12] = the frame's camera R row-major and t, frame_out = its frame number;
+ *     each may be NULL.  Not enabled, no frame queued since enable, or a sharded handle: IMMESH_E_INVALID. */
+typedef struct {
+    int positions;        /* 0: raw vertex positions; 1: the smoothed position where m_smoothed is set, else the raw one */
+    int color_by_height;  /* 0: white; 1: the height colour on z */
+    double z_range[2];    /* height colour range; both NaN: min / max z over the live triangles' vertices at render time */
+} immesh_view_style;
+int immesh_mesh_render_view(immesh_mesh_t* h, const double* intrinsics /*[4]*/, int width, int height, double z_near, double z_far,
+                            const double* cam_R /*[9]*/, const double* cam_t /*[3]*/, const immesh_view_style* style /*or NULL*/,
+                            uint8_t* rgba /*[h][w][4]*/, float* depth /*[h][w] or NULL*/);
+int immesh_mesh_view_enable(immesh_mesh_t* h, const double* intrinsics /*[4] or NULL*/, int width, int height, double z_near, double z_far, int win,
+                            const immesh_view_style* style /*or NULL*/);
+int immesh_mesh_view_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/, int follow);
+int immesh_mesh_view_image(immesh_mesh_t* h, uint8_t* rgba /*[h][w][4] or NULL*/, float* depth /*[h][w] or NULL*/, double* pose_out /*[12] or NULL*/,
+                           int64_t* frame_out /*or NULL*/);
 /* The change feed: each frame's added and removed triangles (the reference's per-frame added_triangle_list / removed_triangle_list,
  * src/ImMesh_mesh_reconstruction.cpp:122-123, 209-244), recorded on the device, so that a caller that keeps its own copy of the mesh
  * (publisher, remote viewer, recorder) applies the difference instead of calling immesh_mesh_snapshot after every frame.
