@@ -52,6 +52,11 @@ def _view_style(positions, color_by_height, z_range):
     return _ViewStyle(int(positions), 1 if color_by_height else 0, (C.c_double * 2)(lo, hi))
 
 
+class _ViewOverlay(C.Structure):
+    _fields_ = [("wireframe", C.c_int), ("scan_point_size", C.c_int), ("reinforced_point_size", C.c_int), ("axis_and_grid", C.c_int),
+                ("camera_size", C.c_double), ("path_width", C.c_int), ("path_capacity", C.c_int)]
+
+
 class _ImuCfg(C.Structure):
     _fields_ = [("cov_gyr", C.c_double * 3), ("cov_acc", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3),
                 ("mean_acc_norm", C.c_double), ("lid_R", C.c_double * 9), ("lid_T", C.c_double * 3), ("max_points", C.c_int), ("max_imu", C.c_int)]
@@ -178,6 +183,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_view_enable", [vp, dp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.POINTER(_ViewStyle)]),
         ("immesh_mesh_view_pose", [vp, dp, dp, C.c_int]),
         ("immesh_mesh_view_image", [vp, C.POINTER(C.c_uint8), fp, dp, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_view_overlay", [vp, C.POINTER(_ViewOverlay)]),
         ("immesh_mesh_changes_enable", [vp, C.c_int64, C.c_int]),
         ("immesh_mesh_changes", [vp, C.c_int64, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int32), C.c_int64, fp, C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
@@ -752,6 +758,19 @@ class Mesh:
         R = np.ascontiguousarray(cam_R, dtype=np.float64).reshape(9)
         t = np.ascontiguousarray(cam_t, dtype=np.float64).reshape(3)
         _check(self.lib, self.lib.immesh_mesh_view_pose(self._h, R.ctypes.data_as(dp), t.ctypes.data_as(dp), 1 if follow else 0), "mesh_view_pose")
+
+    def view_overlay(self, wireframe=False, scan_point_size=2, reinforced_point_size=2, axis_and_grid=True, camera_size=1.0, path_width=4,
+                     path_capacity=1 << 16):
+        """Draw the rest of the viewer's window into the queued view from the next frame on (defaults: the reference's): the current
+        scan, the reinforced points, the axis and ground grid, the sensor's camera frustum and the trajectory of the frames queued
+        from now on (the newest path_capacity positions); wireframe draws the live triangles' edges instead of the faces.  Sizes and
+        widths in pixels, 0: off."""
+        o = _ViewOverlay(1 if wireframe else 0, int(scan_point_size), int(reinforced_point_size), 1 if axis_and_grid else 0, float(camera_size),
+                         int(path_width), int(path_capacity))
+        _check(self.lib, self.lib.immesh_mesh_view_overlay(self._h, C.byref(o)), "mesh_view_overlay")
+
+    def view_overlay_off(self):
+        _check(self.lib, self.lib.immesh_mesh_view_overlay(self._h, None), "mesh_view_overlay")
 
     def view_image(self):
         """(rgba uint8[h,w,4], depth float32[h,w], cam_R float64[3,3], cam_t float64[3], frame) of the newest queued frame."""

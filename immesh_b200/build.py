@@ -164,6 +164,15 @@ def build_view(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "view", "emu_view.cpp"), EMU_VIEW, force)
 
 
+EMU_VIEW_OVERLAY = os.path.join(_ROOT, "tests", "view_overlay", "libimmesh_emu_view_overlay.so")
+
+
+def build_view_overlay(force=False):
+    """tests/view_overlay: the queued view's overlay bodies (immesh_b200/csrc/view_overlay.cuh) -- points, clipped wide lines, the
+    wireframe, the frustum, the trajectory ring and the layered key -- in the device chain's orchestration, built for the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "view_overlay", "emu_view_overlay.cpp"), EMU_VIEW_OVERLAY, force)
+
+
 EMU_CHANGES = os.path.join(_ROOT, "tests", "changes", "libimmesh_emu_changes.so")
 
 
@@ -230,6 +239,7 @@ def build_all(force=False):
     build_imu_chain(force)
     build_reinforce(force)
     build_view(force)
+    build_view_overlay(force)
     build_changes(force)
     build_eval(force)
     build_local_map(force)

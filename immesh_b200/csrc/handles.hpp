@@ -7,7 +7,7 @@
 #include "mesh_changes.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
-#include "reinforce.cuh"
+#include "view_overlay.cuh"
 
 using immesh::LioParams; using immesh::VoxelMapDev; using immesh::ScanBuf; using immesh::LioCtrl;
 using immesh::MeshParams; using immesh::MeshDev; using immesh::FrameBuf; using immesh::FramePose;
@@ -210,6 +210,8 @@ struct immesh_mesh {
         int* zr_done = nullptr;           // k_view_zrange's finished-block counter (0 between launches)
         int zr_blocks = 1;
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
+        immesh::ViewOverlay ov = {};      // immesh_mesh_view_overlay (ov.on = 0: none)
+        immesh::MemSet ov_dev;            // its keys, trajectory and frustum, freed by the next overlay call, disable or destroy (not counted)
     } vw;
     // change feed (immesh_mesh_changes_enable); its per-frame pointers are in F (chg_stamp, chg_list, chg_cnt, chg_cap)
     struct Changes {

@@ -18,6 +18,7 @@
 #include "pool_growth.cuh"
 #include "nccl_api.hpp"
 #include "reinforce.cuh"
+#include "view_overlay.cuh"
 #include "pdl.cuh"
 
 using namespace immesh;
@@ -434,15 +435,22 @@ __device__ __forceinline__ float4 rf_vertex(const MeshDev& M, int pos_mode, int 
 __device__ __forceinline__ void rf_tiles(const DepthTri& T, int* tx0, int* tx1, int* ty0, int* ty1) {
     *tx0 = T.x_lo / IM_RT_TILE; *tx1 = T.x_hi / IM_RT_TILE; *ty0 = T.y_lo / IM_RT_TILE; *ty1 = T.y_hi / IM_RT_TILE;
 }
-// count pass: bin entries per tile (positions by pos_mode)
-__global__ void __launch_bounds__(128) k_rf_count(MeshDev M, int pos_mode, const DepthCam* cam, int* tile_cnt) {
+// a triangle's set-up for the bins: the face rule's (depth_tri_setup), or with `wire` the wireframe's widened box (view_wire_setup)
+__device__ __forceinline__ bool rf_bin_setup(const DepthCam& C, const MeshDev& M, int pos_mode, int wire, const int4& r, DepthTri* T) {
+    const float4 p0 = rf_vertex(M, pos_mode, r.x), p1 = rf_vertex(M, pos_mode, r.y), p2 = rf_vertex(M, pos_mode, r.z);
+    if (!wire) return depth_tri_setup(C, p0, p1, p2, T);
+    int4 fb;
+    return view_wire_setup(C, p0, p1, p2, T, &fb);
+}
+// count pass: bin entries per tile (positions by pos_mode; boxes of the wireframe with `wire`)
+__global__ void __launch_bounds__(128) k_rf_count(MeshDev M, int pos_mode, int wire, const DepthCam* cam, int* tile_cnt) {
     const DepthCam C = *cam;
     const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
     for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n_alloc; t += gridDim.x * blockDim.x) {
         const int4 r = M.tri[t];
         if (!r.w) continue;
         DepthTri T;
-        if (!depth_tri_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &T)) continue;
+        if (!rf_bin_setup(C, M, pos_mode, wire, r, &T)) continue;
         int tx0, tx1, ty0, ty1;
         rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
         for (int ty = ty0; ty <= ty1; ++ty)
@@ -464,7 +472,7 @@ __global__ void __launch_bounds__(1024) k_rf_scan(const int* cnt, int n, int* of
     }
 }
 // fill pass: triangle slots into the bins (order inside a bin is free: the tile takes the minimum)
-__global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, int pos_mode, const DepthCam* cam, int* cur, int* bin, const int* misc) {
+__global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, int pos_mode, int wire, const DepthCam* cam, int* cur, int* bin, const int* misc) {
     if (misc[0]) return;
     const DepthCam C = *cam;
     const int n_alloc = min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t), ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
@@ -472,7 +480,7 @@ __global__ void __launch_bounds__(128) k_rf_fill(MeshDev M, int pos_mode, const 
         const int4 r = M.tri[t];
         if (!r.w) continue;
         DepthTri T;
-        if (!depth_tri_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &T)) continue;
+        if (!rf_bin_setup(C, M, pos_mode, wire, r, &T)) continue;
         int tx0, tx1, ty0, ty1;
         rf_tiles(T, &tx0, &tx1, &ty0, &ty1);
         for (int ty = ty0; ty <= ty1; ++ty)
@@ -592,9 +600,11 @@ __global__ void __launch_bounds__(VIEW_ZR_THREADS) k_view_zrange(MeshDev M, int 
 }
 // one block per tile, one thread per pixel (k_rf_tile's shape): the bin's set-ups and (a, b, c, slot) records staged IM_RT_THREADS at
 // a time in shared memory; each thread keeps its pixel's best (depth bits, triple, slot) in registers, then shades the winner and
-// writes the pixel's colour and depth.  Bins over capacity (misc[0]): every triangle slot instead, the same image.
+// writes the pixel's colour and depth.  Bins over capacity (misc[0]): every triangle slot instead, the same image.  With the
+// overlays' keys (ov, or null), an overlay fragment drawn over the winner (ov_over_mesh) gives the pixel its colour instead.
 __global__ void __launch_bounds__(IM_RT_THREADS) k_view_tile(MeshDev M, int pos_mode, int color, const float* zr, const DepthCam* cam, const int* tile_off,
-                                                             const int* bin, const int* misc, const FrameDyn* dyn, ViewOut o0, ViewOut o1) {
+                                                             const int* bin, const int* misc, const FrameDyn* dyn, ViewOut o0, ViewOut o1,
+                                                             const unsigned long long* ov) {
     __shared__ DepthTri S[IM_RT_THREADS];
     __shared__ int4 Q[IM_RT_THREADS];
     const DepthCam C = *cam;
@@ -633,7 +643,10 @@ __global__ void __launch_bounds__(IM_RT_THREADS) k_view_tile(MeshDev M, int pos_
     const float val = __uint_as_float(best);
     o.depth[px] = depth_valid(C, val) ? val : -1.0f;
     uchar4 c = make_uchar4(0, 0, 0, 255);
-    if (bs >= 0) {
+    const unsigned long long k = ov ? ov[px] : OV_NONE;
+    if (ov_over_mesh(k, best)) {
+        c = ov_color(k);
+    } else if (bs >= 0) {
         const int4 r = M.tri[bs];
         const float4 p[3] = {rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z)};
         DepthTri T;
@@ -644,6 +657,101 @@ __global__ void __launch_bounds__(IM_RT_THREADS) k_view_tile(MeshDev M, int pos_
         c = view_shade(T, x, y, p, col, C.t);
     }
     o.rgba[px] = c;
+}
+
+// The wireframe (immesh_mesh_view_overlay with wireframe): k_view_tile's shape over the bins of the wireframe's widened boxes.  Per
+// pixel, the nearest face sample (the depth image, as in face mode) and the best edge fragment by (depth bits, triple, edge); the
+// winning edge coloured from its ends (view_wire_color), unless an overlay fragment is drawn over it.
+__global__ void __launch_bounds__(IM_RT_THREADS) k_view_wire_tile(MeshDev M, int pos_mode, int color, const float* zr, const DepthCam* cam, const int* tile_off,
+                                                                  const int* bin, const int* misc, const FrameDyn* dyn, ViewOut o0, ViewOut o1,
+                                                                  const unsigned long long* ov) {
+    __shared__ DepthTri S[IM_RT_THREADS];
+    __shared__ int4 Q[IM_RT_THREADS];
+    __shared__ int4 FB[IM_RT_THREADS];
+    const DepthCam C = *cam;
+    const int ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE;
+    const int x = (blockIdx.x % ntx) * IM_RT_TILE + (int)(threadIdx.x % IM_RT_TILE), y = (blockIdx.x / ntx) * IM_RT_TILE + (int)(threadIdx.x / IM_RT_TILE);
+    const bool all = misc[0] != 0;
+    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t) : tile_off[blockIdx.x + 1];
+    unsigned int face = 0x7f800000u, best = 0x7f800000u;
+    int ba = INT_MAX, bb = INT_MAX, bc = INT_MAX, be = 3, bs = -1;
+    for (int b = lo; b < hi; b += IM_RT_THREADS) {
+        const int i = b + (int)threadIdx.x;
+        bool ok = false;
+        if (i < hi) {
+            const int slot = all ? i : bin[i];
+            const int4 r = M.tri[slot];
+            ok = r.w && view_wire_setup(C, rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z), &S[threadIdx.x], &FB[threadIdx.x]);
+            Q[threadIdx.x] = make_int4(r.x, r.y, r.z, slot);
+        }
+        if (!ok) { S[threadIdx.x].x_lo = 1; S[threadIdx.x].x_hi = 0; }
+        __syncthreads();
+        const int n = min(IM_RT_THREADS, hi - b);
+        for (int j = 0; j < n; ++j) {
+            const DepthTri& T = S[j];
+            if (x < T.x_lo || x > T.x_hi || y < T.y_lo || y > T.y_hi) continue;
+            const int4 q = Q[j];
+            view_wire_pixel(T, FB[j], q.x, q.y, q.z, q.w, x, y, &face, &best, &ba, &bb, &bc, &be, &bs);
+        }
+        __syncthreads();
+    }
+    if (x >= C.w || y >= C.h) return;
+    const ViewOut o = (dyn->frame & 1) ? o1 : o0;
+    const size_t px = (size_t)y * C.w + x;
+    const float val = __uint_as_float(face);
+    o.depth[px] = depth_valid(C, val) ? val : -1.0f;
+    uchar4 c = make_uchar4(0, 0, 0, 255);
+    const unsigned long long k = ov ? ov[px] : OV_NONE;
+    if (ov_over_mesh(k, best)) {
+        c = ov_color(k);
+    } else if (bs >= 0) {
+        const int4 r = M.tri[bs];
+        const float4 p[3] = {rf_vertex(M, pos_mode, r.x), rf_vertex(M, pos_mode, r.y), rf_vertex(M, pos_mode, r.z)};
+        const float zlo = color ? zr[0] : 0.f, zhi = color ? zr[1] : 0.f;
+        double col[3][3];
+        for (int v = 0; v < 3; ++v) view_color(color, p[v].z, zlo, zhi, col[v]);
+        c = view_wire_color(C, p, col, be, x, y);
+    }
+    o.rgba[px] = c;
+}
+
+// ---- the overlays of the queued view (immesh_mesh_view_overlay; the rule is in include/immesh_b200.h): k_ov_begin clears the
+// per-pixel keys, appends the frame's sensor position to the trajectory and places the frame's camera frustum; k_ov_points rasterises
+// the scan and reinforced points, k_ov_lines the axis, grid, frustum and trajectory segments (a warp per segment), each fragment an
+// atomicMin of its 64-bit key (ov_key); the tile kernels then resolve the keys against the mesh.
+__global__ void __launch_bounds__(256) k_ov_begin(ViewOverlay O, const FrameDyn* dyn, const double (*ring)[12], const int* ring_frame) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < O.npx; i += gridDim.x * blockDim.x) O.key[i] = OV_NONE;
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    const FrameDyn d = *dyn;
+    ov_begin_frame(O, d.frame, d.fp->pose_t, ring, ring_frame);
+}
+__global__ void __launch_bounds__(128) k_ov_points(ViewOverlay O, const DepthCam* cam, const FrameDyn* dyn, RfOut r0, RfOut r1, int rf_on) {
+    const DepthCam C = *cam;
+    const FrameDyn d = *dyn;
+    const int n_scan = O.scan_size > 0 && d.frame >= 2 ? d.n : 0;
+    const RfOut r = (d.frame & 1) ? r1 : r0;
+    const int n_rf = O.reinforced_size > 0 && rf_on ? *r.n : 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_scan + n_rf; i += gridDim.x * blockDim.x) {
+        const bool scan = i < n_scan;
+        const int j = scan ? i : i - n_scan, layer = scan ? OV_SCAN : OV_REINFORCED;
+        const float* q = (scan ? d.pts : r.pts) + (size_t)j * 3;
+        const double p[3] = {(double)q[0], (double)q[1], (double)q[2]};
+        ov_point_raster(C, p, scan ? O.scan_size : O.reinforced_size,
+                        [&](int x, int y, float zf) { atomicMin(&O.key[(size_t)y * C.w + x], ov_key(zf, layer, (unsigned)j)); });
+    }
+}
+__global__ void __launch_bounds__(128) k_ov_lines(ViewOverlay O, const DepthCam* cam) {
+    const DepthCam C = *cam;
+    const int frustum_on = *O.frustum_on, path_n = O.path_width > 0 ? *O.path_n : 0, lane = threadIdx.x & 31;
+    const int nseg = (O.axis_and_grid ? OV_N_AXIS + OV_N_GRID : 0) + (frustum_on ? OV_N_CAMERA : 0) + max(ov_path_kept(O, path_n) - 1, 0);
+    for (int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < nseg; i += (gridDim.x * blockDim.x) >> 5) {
+        int layer, idx, width;
+        double p0[3], p1[3];
+        OvSeg S;
+        if (!ov_line(O, frustum_on, path_n, i, &layer, &idx, &width, p0, p1) || !ov_seg_setup(C, p0, p1, &S)) continue;
+        ov_seg_raster(C, S, width, lane, 32,
+                      [&](int x, int y, float zf, double) { atomicMin(&O.key[(size_t)y * C.w + x], ov_key(zf, layer, (unsigned)idx)); });
+    }
 }
 
 // ---- the region segments of records in region order (mesh_tri_order with a region size): the region stream and the viewer's region
@@ -1369,11 +1477,11 @@ static cudaError_t rf_image_alloc(immesh::MemSet& dev, int w, int h, int nout, R
 // the image of the camera in im.cam, with the tile counters zeroed, into result buffer (dyn->frame & 1) (fixed grids: every
 // per-image value is read on the device)
 // the binning passes of an image: the triangles at positions pos_mode (view_vertex) into the tiles' bins
-static void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st) {
+static void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st, int wire = 0) {
     const int g = h->n_sm * 8;
-    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, pos_mode, (const DepthCam*)im.cam, im.tile_cnt);
+    IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, pos_mode, wire, (const DepthCam*)im.cam, im.tile_cnt);
     IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.tile_cnt, im.ntiles, im.tile_off, im.tile_cnt, im.bin_cap, im.misc);
-    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, pos_mode, (const DepthCam*)im.cam, im.tile_cnt, im.bin, (const int*)im.misc);
+    IM_LAUNCH(k_rf_fill, g, 128, 0, st, h->M, pos_mode, wire, (const DepthCam*)im.cam, im.tile_cnt, im.bin, (const int*)im.misc);
 }
 static void rf_image_launch(const immesh_mesh* h, const RfImage& im, const FrameDyn* dyn, cudaStream_t st) {
     const DepthCam* cam = im.cam;
@@ -1392,17 +1500,30 @@ static void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st) {
 }
 // the shaded image of the camera in im.cam (tile counters zeroed) with style v into out[dyn->frame & 1]: binning, the automatic z
 // range when the height colour needs it, the tiles
+// (the overlays' keys resolved in the tiles when v.ov is on; the wireframe in place of the faces with v.ov.wire)
 static void view_image_launch(const immesh_mesh* h, const immesh_mesh::View& v, const RfImage& im, const ViewOut* out, const FrameDyn* dyn, cudaStream_t st) {
-    rf_bin_launch(h, im, v.pos, st);
+    const int wire = v.ov.on && v.ov.wire;
+    const unsigned long long* ov = v.ov.on ? v.ov.key : nullptr;
+    rf_bin_launch(h, im, v.pos, st, wire);
     if (v.color && v.auto_range) IM_LAUNCH(k_view_zrange, v.zr_blocks, VIEW_ZR_THREADS, 0, st, h->M, v.pos, v.zr_part, v.zr_done, v.zr);
-    IM_LAUNCH(k_view_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, v.pos, v.color, (const float*)v.zr, (const DepthCam*)im.cam, (const int*)im.tile_off,
-              (const int*)im.bin, (const int*)im.misc, dyn, out[0], out[1]);
+    if (wire)
+        IM_LAUNCH(k_view_wire_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, v.pos, v.color, (const float*)v.zr, (const DepthCam*)im.cam, (const int*)im.tile_off,
+                  (const int*)im.bin, (const int*)im.misc, dyn, out[0], out[1], ov);
+    else
+        IM_LAUNCH(k_view_tile, im.ntiles, IM_RT_THREADS, 0, st, h->M, v.pos, v.color, (const float*)v.zr, (const DepthCam*)im.cam, (const int*)im.tile_off,
+                  (const int*)im.bin, (const int*)im.misc, dyn, out[0], out[1], ov);
 }
 // the queued view of the frame just queued: its camera (k_rf_pose, pose into the result buffer), then its image
 static void mesh_view_launch(immesh_mesh* h, cudaStream_t st) {
     auto& v = h->vw;
     IM_LAUNCH(k_rf_pose, 1, 256, 0, st, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame, (const FrameDyn*)h->d_dyn, (const RfDyn*)v.rd, v.win, v.base,
               v.img.cam, v.img.out[0], v.img.out[1], v.img.tile_cnt, v.img.ntiles);
+    if (v.ov.on) {   // the overlays' keys; the reinforced points are those of the reinforcement queued just before, while it is on
+        const int g = h->n_sm * 8;
+        IM_LAUNCH(k_ov_begin, g, 256, 0, st, v.ov, (const FrameDyn*)h->d_dyn, (const double (*)[12])h->cam_ring, (const int*)h->cam_ring_frame);
+        IM_LAUNCH(k_ov_points, g, 128, 0, st, v.ov, (const DepthCam*)v.img.cam, (const FrameDyn*)h->d_dyn, h->rf.img.out[0], h->rf.img.out[1], h->rf.on);
+        IM_LAUNCH(k_ov_lines, g, 128, 0, st, v.ov, (const DepthCam*)v.img.cam);
+    }
     const ViewOut out[2] = {{v.rgba[0], v.img.out[0].depth}, {v.rgba[1], v.img.out[1].depth}};
     view_image_launch(h, v, v.img, out, h->d_dyn, st);
 }
@@ -2516,6 +2637,52 @@ int immesh_mesh_view_image(immesh_mesh_t* h, uint8_t* rgba, float* depth, double
     if (depth) IM_CUDA(cudaMemcpy(depth, h->vw.img.out[b].depth, n * sizeof(float), cudaMemcpyDeviceToHost));
     if (pose_out) IM_CUDA(cudaMemcpy(pose_out, h->vw.img.out[b].pose, 12 * sizeof(double), cudaMemcpyDeviceToHost));
     if (frame_out) *frame_out = f;
+    return IMMESH_OK;
+}
+
+int immesh_mesh_view_overlay(immesh_mesh_t* h, const immesh_view_overlay* o) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "view_overlay: a sharded mesh handle is not supported");
+    if (!h->vw.on) return im_fail(IMMESH_E_INVALID, "view_overlay: the view is not enabled (immesh_mesh_view_enable)");
+    if (o) {
+        auto size_ok = [](int s) { return s >= 0 && s <= 64; };
+        if ((o->wireframe != 0 && o->wireframe != 1) || (o->axis_and_grid != 0 && o->axis_and_grid != 1) || !size_ok(o->scan_point_size) ||
+            !size_ok(o->reinforced_point_size) || !size_ok(o->path_width) || !std::isfinite(o->camera_size) || o->camera_size < 0.0 ||
+            (o->path_width > 0 && (o->path_capacity < 1 || o->path_capacity > (1 << 24))))
+            return im_fail(IMMESH_E_INVALID, "view_overlay: bad argument (wireframe and axis_and_grid 0 or 1; sizes and widths in [0, 64]; finite camera_size >= 0; "
+                                             "1 <= path_capacity <= 2^24 with a path)");
+        if (o->scan_point_size > 0 && h->max_frame_points >= (1 << OV_IDX_BITS))
+            return im_fail(IMMESH_E_INVALID, "view_overlay: scan points need max_frame_points < 2^29");
+    }
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
+    h->graph.destroy();                          // the captured sequence changes
+    auto& v = h->vw;
+    v.ov = ViewOverlay{};
+    v.ov_dev = immesh::MemSet();
+    if (!o || !(o->wireframe || o->scan_point_size || o->reinforced_point_size || o->axis_and_grid || o->camera_size > 0.0 || o->path_width))
+        return IMMESH_OK;   // every layer off: as NULL
+    ViewOverlay ov = {};
+    ov.wire = o->wireframe;
+    ov.scan_size = o->scan_point_size;
+    ov.reinforced_size = o->reinforced_point_size;
+    ov.axis_and_grid = o->axis_and_grid;
+    ov.camera_size = o->camera_size;
+    ov.path_width = o->path_width;
+    ov.path_cap = o->path_width > 0 ? o->path_capacity : 1;
+    ov.npx = v.base.w * v.base.h;
+    immesh::MemSet dev;
+    cudaError_t e = dev.alloc(&ov.key, (size_t)ov.npx);
+    if (e == cudaSuccess) e = dev.alloc(&ov.path, (size_t)ov.path_cap);
+    if (e == cudaSuccess) e = dev.alloc(&ov.path_n, 1, 0);
+    if (e == cudaSuccess) e = dev.alloc(&ov.frustum, 11);
+    if (e == cudaSuccess) e = dev.alloc(&ov.frustum_on, 1, 0);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "view_overlay: allocation of the overlay's buffers failed");
+    }
+    ov.on = 1;
+    v.ov = ov;
+    v.ov_dev = std::move(dev);
     return IMMESH_OK;
 }
 

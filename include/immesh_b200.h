@@ -493,6 +493,54 @@ int immesh_mesh_view_enable(immesh_mesh_t* h, const double* intrinsics /*[4] or 
 int immesh_mesh_view_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/, int follow);
 int immesh_mesh_view_image(immesh_mesh_t* h, uint8_t* rgba /*[h][w][4] or NULL*/, float* depth /*[h][w] or NULL*/, double* pose_out /*[12] or NULL*/,
                            int64_t* frame_out /*or NULL*/);
+/* The rest of the viewer's window in the queued view (src/ImMesh_node.cpp:422-470): the current scan (display_current_LiDAR_pts),
+ * the reinforced points (display_reinforced_LiDAR_pts), the axis (g_axis_shader), the ground grid (g_ground_plane_shader), the
+ * wireframe in place of the faces (draw_triangle with g_display_face = 0), the sensor's camera frustum (draw_camera_pose) and the
+ * trajectory (draw_camera_trajectory).
+ *   immesh_mesh_view_overlay(h, o): from the next queued frame on; needs the view enabled (immesh_mesh_view_enable, which, like
+ *     disabling, clears the overlay).  Drains the frames in flight, drops the captured graph and allocates the overlay's buffers
+ *     (per-pixel keys, trajectory ring, frustum) here and nowhere else.  o = NULL, or every layer off: no overlay; then no launch, graph
+ *     or output differs from a handle that never called it.  Sizes or widths outside [0, 64], wireframe or axis_and_grid not 0 / 1,
+ *     a non-finite or negative camera_size, path_capacity outside [1, 2^24] with path_width > 0, scan points with max_frame_points >=
+ *     2^29, the view not enabled, or a sharded handle: IMMESH_E_INVALID.  The blocking immesh_mesh_render_view draws no overlay.
+ *   Image rule (adds to immesh_mesh_render_view's, which stays as it is for the faces):
+ *     Camera: the queued view's, in every mode.  Mesh vertices at style.positions.  Overlays unlit and opaque; their bytes by
+ *       floor(clamp(c) 255 + 0.5): scan points, frustum and trajectory white; reinforced points magenta (255, 0, 255); the x, y, z axes
+ *       red, green, blue; the grid grey 0.45 (115).
+ *     Points: camera z in (z_near, z_far), depth the camera z as float; a point of size s at (u, v) covers the integer pixels with
+ *       u - s/2 <= x < u + s/2 and v - s/2 <= y < v + s/2, cut to the image.
+ *     Segments: the ends in camera space (float64), clipped to [z_near, z_far] (an end beyond a plane moves along the segment to it:
+ *       s = (zp - za) / (zb - za), a + s (b - a), near first, then far; a segment wholly outside is dropped), then projected.  A line of
+ *       width w, non-antialiased: x-major when |du| >= |dv|; it covers every integer column min(u0, u1) <= x < max(u0, u1), with
+ *       t = (x - u0) / (u1 - u0) and v = v0 + t (v1 - v0) the rows v - w/2 <= y < v + w/2; 1/z = 1/z0 + t (1/z1 - 1/z0), the
+ *       depth its float inverse.  A y-major line swaps the axes.  Float64 without fused multiply-adds.
+ *     Wireframe: the edges (a, b), (b, c), (a, c) of each live triangle whose three vertices lie in (z_near, z_far), each from its
+ *       lower vertex id to its higher, width 1, in the vertex colours of style (white or the height colour): w0 = (1 - t) / z0,
+ *       w1 = t / z1, c = (w0 c0 + w1 c1) / (w0 + w1).  A shared edge rasterises to the same pixels from either triangle.
+ *     Layers: the axis (from the origin, 1 m, width 10) and the grid (21 + 21 lines at z = 0, 10 m apart from -100 m to 100 m, line
+ *       2i at x = 10 (i - 10) from y = -100 to 100 and line 2i + 1 at y = 10 (i - 10) from x = -100 to 100, width 1) with
+ *       axis_and_grid; the scan: frame n's own world points for n >= 2 (frames counted from 1); the reinforced points: the queued
+ *       reinforcement's cloud of the same frame, while the reinforcement is on; the frustum: frame n's rot_end R and pos_end t in
+ *       float64 (a world-frame push carries no rotation: none), the 11-vertex strip of the hard-coded K (704.504153913163,
+ *       703.6790228113778, 708.8501128392297, 562.7041625276061) and 1440 x 1080 at scale 1.5: fu = 1 / fx, u0 = -cx / fx (v
+ *       likewise), xl = 1.5 u0, xh = 1.5 (1440 fu + u0), yl = 1.5 v0, yh = 1.5 (1080 fv + v0), the local vertices (xl,yl,1.5)
+ *       (xh,yl,1.5) (xh,yh,1.5) (xl,yh,1.5) (xl,yl,1.5) 0 (xh,yl,1.5) 0 (xl,yh,1.5) 0 (xh,yh,1.5), in the world t_k + camera_size
+ *       ((-R_k1 x + -R_k2 y) + R_k0 z), width 5; the trajectory: a line strip through the positions of the frames queued since this
+ *       call (a localization frame's pos_end, a world-frame push's pose_t), the newest path_capacity kept, oldest first.
+ *     Visibility: per pixel the smallest float depth bits win; on equal bits the earlier layer in the reference's draw order (scan,
+ *       reinforced, axis, grid, mesh, frustum, trajectory), inside a layer the lower index (point order; segment order as listed; for
+ *       faces the lower triple; for edges the lower (triple, edge)).
+ *     depth of immesh_mesh_view_image: unchanged, the faces' depth image, also with the wireframe.  Batched frames are not followed. */
+typedef struct {
+    int    wireframe;              /* 1: the live triangles' edges instead of the faces (g_display_face = 0) */
+    int    scan_point_size;        /* pixels; 0: off.  Reference 2 */
+    int    reinforced_point_size;  /* pixels; 0: off.  Reference 2.  Drawn only while the reinforcement is enabled */
+    int    axis_and_grid;          /* g_if_draw_z_plane (reference: on) */
+    double camera_size;            /* g_display_camera_size; 0: no frustum.  Reference 1.0 */
+    int    path_width;             /* g_draw_path_size + 2; 0: no trajectory.  Reference 4 */
+    int    path_capacity;          /* positions kept for the trajectory; the oldest drop out */
+} immesh_view_overlay;
+int immesh_mesh_view_overlay(immesh_mesh_t* h, const immesh_view_overlay* o /* NULL: none */);
 /* The change feed: each frame's added and removed triangles (the reference's per-frame added_triangle_list / removed_triangle_list,
  * src/ImMesh_mesh_reconstruction.cpp:122-123, 209-244), recorded on the device, so that a caller that keeps its own copy of the mesh
  * (publisher, remote viewer, recorder) applies the difference instead of calling immesh_mesh_snapshot after every frame.
