@@ -57,6 +57,23 @@ class _ViewOverlay(C.Structure):
                 ("camera_size", C.c_double), ("path_width", C.c_int), ("path_capacity", C.c_int)]
 
 
+class _FeedCfg(C.Structure):
+    _fields_ = [("max_scans", C.c_int64), ("max_rows", C.c_int64), ("effect", C.c_int), ("registered", C.c_int), ("point_skip", C.c_int), ("pad", C.c_int)]
+
+
+FEED_HDR = 12   # IMMESH_LIO_FEED_HDR: the header columns of a recorded scan, in this order
+FEED_HDR_KEYS = ("scan", "kind", "branch", "iters", "matches", "converged", "err", "row_begin", "row_effect_end", "row_end", "source", "rows_lost")
+FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i")   # IMMESH_FEED_KIND_*
+
+
+class FeedLost(RuntimeError):
+    """immesh_lio_feed returned IMMESH_E_RANGE: scans of the range left the rings.  Read on from newest_finished."""
+
+    def __init__(self, msg, newest_finished):
+        super().__init__(msg)
+        self.newest_finished = newest_finished
+
+
 class _ImuCfg(C.Structure):
     _fields_ = [("cov_gyr", C.c_double * 3), ("cov_acc", C.c_double * 3), ("cov_bias_gyr", C.c_double * 3), ("cov_bias_acc", C.c_double * 3),
                 ("mean_acc_norm", C.c_double), ("lid_R", C.c_double * 9), ("lid_T", C.c_double * 3), ("max_points", C.c_int), ("max_imu", C.c_int)]
@@ -217,6 +234,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_lio_step_async_raw_i", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_double, C.c_double, C.c_double]),
         ("immesh_lio_step_async_imu_i", [vp, vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, ip]),
         ("immesh_lio_frontend_cloud", [vp, vp, C.c_int, C.c_int, fp, C.c_int, ip]),
+        ("immesh_lio_feed_enable", [vp, C.POINTER(_FeedCfg)]),
+        ("immesh_lio_feed", [vp, C.c_int64, C.c_int, C.POINTER(C.c_int64), dp, C.c_int, fp, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64)]),
+        ("immesh_odometry_pose", [dp, dp]),
+        ("immesh_lio_state_line", [dp, C.c_double, C.c_char_p, C.c_int]),
     ):
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
@@ -483,6 +504,46 @@ class Lio:
         rows = np.zeros((max(n_out.value, 1), SCAN_PUB_COLS), dtype=np.float32)
         _check(self.lib, call(rows.ctypes.data_as(C.POINTER(C.c_float)), n_out.value), "lio_registered_cloud")
         return rows[: n_out.value]
+
+    def feed_enable(self, max_scans=1024, max_rows=1 << 22, effect=True, registered=1, point_skip=1):
+        """Record every queued scan's header, state and published clouds on the device (immesh_lio_feed_enable).  registered: 0 none,
+        1 the down-sampled scan, 2 the full scan where the chain has one."""
+        c = _FeedCfg(max_scans, max_rows, 1 if effect else 0, registered, point_skip, 0)
+        _check(self.lib, self.lib.immesh_lio_feed_enable(self._h, C.byref(c)), "lio_feed_enable")
+
+    def feed_disable(self):
+        _check(self.lib, self.lib.immesh_lio_feed_enable(self._h, None), "lio_feed_enable")
+
+    def feed(self, since: int, wait: bool = False):
+        """The scans (since, newest finished] of the scan feed: dict(scans=int64[m, FEED_HDR], states=float64[m, 348],
+        rows=float32[r, 4], row_index=int32[r] (-1 on registered rows), newest_finished, newest_queued).  wait=False never blocks on
+        unfinished work.  Raises FeedLost when scans of the range left the rings."""
+        counts = np.zeros(4, dtype=np.int64)
+        cp = counts.ctypes.data_as(C.POINTER(C.c_int64))
+        for _ in range(8):   # scans may finish between the count query and the read
+            rc = self.lib.immesh_lio_feed(self._h, since, 1 if wait else 0, None, None, 0, None, None, 0, cp)
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, "lio_feed")
+            ns, nr = int(counts[0]), int(counts[1])
+            scans = np.zeros((max(ns, 1), FEED_HDR), dtype=np.int64)
+            states = np.zeros((max(ns, 1), STATE_DOUBLES))
+            rows = np.zeros((max(nr, 1), SCAN_PUB_COLS), dtype=np.float32)
+            idx = np.zeros(max(nr, 1), dtype=np.int32)
+            if ns == 0:
+                break
+            rc = self.lib.immesh_lio_feed(self._h, since, 0, scans.ctypes.data_as(C.POINTER(C.c_int64)), states.ctypes.data_as(C.POINTER(C.c_double)), ns,
+                                          rows.ctypes.data_as(C.POINTER(C.c_float)), idx.ctypes.data_as(C.POINTER(C.c_int32)), nr, cp)
+            if rc == -3:
+                continue
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, "lio_feed")
+            ns, nr = int(counts[0]), int(counts[1])
+            break
+        else:
+            raise RuntimeError("lio_feed: the scans kept finishing faster than they were read")
+        return dict(scans=scans[:ns], states=states[:ns], rows=rows[:nr], row_index=idx[:nr], newest_finished=int(counts[2]), newest_queued=int(counts[3]))
 
     def frontend_cloud(self, vg: "VoxelGrid", dense: bool, point_skip=1):
         """publish_frame_world from the front-end clouds of the last _i step through vg (immesh_lio_frontend_cloud): float32[m, 4] rows
@@ -1116,6 +1177,24 @@ def kitti_pose_line(state, stamp: float, lib: Optional[C.CDLL] = None) -> str:
     s = np.ascontiguousarray(state, dtype=np.float64)
     buf = C.create_string_buffer(512)
     _check(lib, lib.immesh_kitti_pose_line(s.ctypes.data_as(C.POINTER(C.c_double)), stamp, buf, 512), "kitti_pose_line")
+    return buf.value.decode()
+
+
+def odometry_pose(state, lib: Optional[C.CDLL] = None) -> np.ndarray:
+    """publish_odometry's pose of a state: float64[7] pos_end, then the quaternion x y z w of tf's setRPY(RotMtoEuler(rot_end))."""
+    lib = lib or load_library()
+    s = np.ascontiguousarray(state, dtype=np.float64)
+    out = np.zeros(7)
+    _check(lib, lib.immesh_odometry_pose(s.ctypes.data_as(C.POINTER(C.c_double)), out.ctypes.data_as(C.POINTER(C.c_double))), "odometry_pose")
+    return out
+
+
+def lio_state_line(state, t: float, lib: Optional[C.CDLL] = None) -> str:
+    """dump_lio_state_to_log's line of a state at time t (ending in \\r\\n)."""
+    lib = lib or load_library()
+    s = np.ascontiguousarray(state, dtype=np.float64)
+    buf = C.create_string_buffer(4096)
+    _check(lib, lib.immesh_lio_state_line(s.ctypes.data_as(C.POINTER(C.c_double)), t, buf, 4096), "lio_state_line")
     return buf.value.decode()
 
 

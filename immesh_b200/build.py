@@ -183,6 +183,15 @@ def build_changes(force=False):
                     extra=[os.path.join(_ROOT, "tests", "emu", "emu_lio.cpp")])
 
 
+EMU_LIO_FEED = os.path.join(_ROOT, "tests", "lio_feed", "libimmesh_emu_lio_feed.so")
+
+
+def build_lio_feed(force=False):
+    """tests/lio_feed: the scan feed's ring bookkeeping and read (immesh_b200/csrc/lio_feed.cuh) with the device kernels' order restated
+    on the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "lio_feed", "emu_lio_feed.cpp"), EMU_LIO_FEED, force)
+
+
 EMU_EVAL = os.path.join(_ROOT, "tests", "eval", "libimmesh_emu_eval.so")
 
 
@@ -241,6 +250,7 @@ def build_all(force=False):
     build_view(force)
     build_view_overlay(force)
     build_changes(force)
+    build_lio_feed(force)
     build_eval(force)
     build_local_map(force)
     build_dev_mem(force)

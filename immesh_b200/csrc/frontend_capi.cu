@@ -499,7 +499,15 @@ int immesh_frontend_step_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const f
     if (rc) return rc;
     rc = vg_enqueue(h, h->d_in, n, leaf, st, with_i ? h->d_in_i_ring[h->in_idx] : nullptr);
     if (rc) return rc;
+    // the scan feed's full scan (registered source 2): the calibrated input cloud immesh_voxelgrid_input_points returns, with its
+    // intensity on the _i chains; the IMU chain has set its own kind and branch
+    immesh_lio::FeedNext& nx = lio->feed_next;
+    if (nx.kind < 0) { nx.kind = with_i ? IMMESH_FEED_KIND_RAW_I : IMMESH_FEED_KIND_RAW; nx.branch = 0; }
+    nx.pts = h->d_in;
+    nx.inten = with_i ? h->d_in_i_ring[h->in_idx] : nullptr;
+    nx.n = n;
     rc = immesh_lio_step_async_dev_n(lio, h->d_out, n < lio->max_scan ? n : lio->max_scan, &h->d_grid->m_out, dt, cov_gyr, cov_acc);
+    lio->feed_next = immesh_lio::FeedNext();
     if (rc || !with_i) return rc;
     lio->fe_vg = h;
     lio->fe_uploads = lio->uploads;
@@ -545,7 +553,9 @@ int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const 
     if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
     const int rc = frontend_pack(h, d_pts, n, stride, 1, calib_laser, lio->stream, -1, d_inten);
     if (rc) return rc;
-    return immesh_voxelmap_build_async_dev(lio, h->d_in, n);
+    const int brc = immesh_voxelmap_build_async_dev(lio, h->d_in, n);   // takes the IMU chain's feed_next (branch 2)
+    lio->feed_next = immesh_lio::FeedNext();
+    return brc;
 }
 
 }  // extern "C"

@@ -4,6 +4,7 @@
 
 #include "common_host.hpp"
 #include "lio_core.cuh"
+#include "lio_feed.cuh"
 #include "mesh_changes.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
@@ -101,7 +102,34 @@ struct immesh_lio {
     int tombs_known = 0;          // tombstones after the last step known to have finished
     float* d_lm_boxes = nullptr;  // the caller's boxes of immesh_voxelmap_evict_boxes, in `scratch`
     size_t lm_boxes_cap = 0;
+    // the scan the next lio_enqueue / immesh_voxelmap_build_async_dev records in the scan feed, when the front-end or the IMU chain
+    // queues it (set around their inner step call; kind < 0: the entry point's own kind, no full scan)
+    struct FeedNext {
+        int kind = -1, branch = 0, n = 0;
+        const float* pts = nullptr;     // the full scan (registered source 2)
+        const float* inten = nullptr;   // its intensity, or null
+    } feed_next;
+    // scan feed (immesh_lio_feed_enable)
+    struct Feed {
+        int on = 0, effect = 0, registered = 0, skip = 1;
+        long long max_scans = 0, max_rows = 0;
+        long long queued = 0;             // scans recorded since enable: the newest one's number
+        int nb = 0;                       // tiles of the effect count (max_scan points)
+        immesh::LioFeedDev* dev = nullptr;
+        long long* hdr = nullptr;         // [max_scans][IMMESH_LIO_FEED_HDR]
+        double* states = nullptr;         // [max_scans][IM_STATE_DOUBLES]
+        float4* rows = nullptr;           // [max_rows]
+        int* idx = nullptr;               // [max_rows] scan index of the effect rows (effect = 1)
+        int* tiles = nullptr;             // [nb + 1] the effect count's tiles and total
+        immesh::FeedDyn* h_dyn = nullptr; // pinned ring of IM_FEED_DYN_RING: the per-scan inputs
+        long long* h_done = nullptr;      // pinned, written by k_feed_done: the newest scan whose record is complete
+        long long* d_done = nullptr;      // its device address
+        cudaStream_t stream = nullptr;    // the reader's copies (never the handle's stream)
+        cudaEvent_t ev = nullptr;         // recorded behind the newest scan's record
+        immesh::MemSet dev_mem, pinned{immesh::MemSet::Pinned};
+    } feed;
 };
+#define IM_FEED_DYN_RING 64
 
 // the device buffers of one depth image of the tiled rasteriser (mesh_capi.cu: rf_image_alloc, rf_image_launch): the camera, the tile
 // counters and offsets, the bins, misc[0] (the bins overflowed), the valid pixels per block and their offsets, the depth bits, and

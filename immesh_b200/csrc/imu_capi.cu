@@ -130,6 +130,7 @@ extern "C" int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h);
 extern "C" int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser, const float* d_inten);
 extern "C" int immesh_frontend_step_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
                                           double dt, double cov_gyr, double cov_acc, int icol, const float* isep);
+extern "C" int immesh_lio_feed_record_state(immesh_lio_t* lio, int kind, int branch);
 
 // the next staging slot; blocks (back-pressure, counted in the localization handle's host wait) while its last copies are in flight
 static int imu_stage_slot(immesh_imu* h, immesh_lio* lio) {
@@ -339,6 +340,7 @@ static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg,
     if (n > lio->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than the localization handle's max_scan_points (the map is built from the whole scan, and a scan the VoxelGrid passes through reaches the step whole)");
     cudaStream_t st = lio->stream;
     lio->fe_vg = nullptr;   // branches 1 and 2 publish nothing (voxel_mapping.cpp:1879, :1903)
+    const int feed_kind = icol >= 0 ? IMMESH_FEED_KIND_IMU_I : IMMESH_FEED_KIND_IMU;   // how the scan feed records this scan
     if (icol >= 0) {
         const int rc = imu_records_alloc(h, on_device ? 0 : stride);
         if (rc) return rc;
@@ -384,7 +386,9 @@ static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg,
                 h->P.mean_acc_norm = norm;
             }
         }
-        const int rc = imu_stage_release(h, s, st);
+        int rc = imu_stage_release(h, s, st);
+        if (rc) return rc;
+        rc = immesh_lio_feed_record_state(lio, feed_kind, 1);
         if (rc) return rc;
         if (branch_out) *branch_out = 1;
         return IMMESH_OK;
@@ -397,14 +401,20 @@ static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg,
     const float* d_out_i = icol >= 0 ? h->d_out_i : nullptr;
     if (!h->map_built) {
         // branch 2: voxel_map_init from the full-resolution, undistorted, calibrated scan (voxel_mapping.cpp:1844-1859, :1894-1904)
+        lio->feed_next.kind = feed_kind;
+        lio->feed_next.branch = 2;
         rc = immesh_frontend_build_async(lio, vg, h->d_out, n, 4, calib_laser, d_out_i);
+        lio->feed_next = immesh_lio::FeedNext();
         if (rc) return rc;
         h->map_built = 1;
         if (branch_out) *branch_out = 2;
         return IMMESH_OK;
     }
     // branch 3: calibration -> VoxelGrid -> IESKF on the propagated state (no Forward_without_imu) -> map_incremental_grow
+    lio->feed_next.kind = feed_kind;
+    lio->feed_next.branch = 3;
     rc = immesh_frontend_step_async(lio, vg, h->d_out, n, 4, 1, calib_laser, leaf, 0.0, 0.0, 0.0, -1, d_out_i);
+    lio->feed_next = immesh_lio::FeedNext();
     if (rc) return rc;
     if (branch_out) *branch_out = 3;
     return IMMESH_OK;

@@ -534,17 +534,28 @@ __global__ void __launch_bounds__(PUB_THREADS) k_pub_emit(VoxelMapDev map, int n
 // exclusive scan over the tiles (k_rs_scan), then each tile emits its rows in order.  immesh_lio_registered_cloud: a strided gather.
 // Both transform with the state in LioCtrl when they run (the handle's current state) and read the scan through scan_load_dyn, so a
 // scan whose count is device resident is published as it was localised.
+// The scan feed (immesh_lio_feed_enable) runs the same three kernels and the gather inside the scan's launch sequence with `fd` set:
+// the rows then go to the feed's row ring at the cursor k_feed_head placed (row r in slot r % ring), and nothing is written when the
+// scan's rows were lost.  fd == null: the blocking publishers, rows from 0.
 #define SPUB_THREADS 256   // one tile of the scan per block
 static_assert(IMMESH_SCAN_PUB_COLS == 4, "scan publisher row width");
 __global__ void __launch_bounds__(SPUB_THREADS) k_eff_count(ScanBuf sb_, int* tile_cnt) {
+    pdl_wait();
     const ScanBuf sb = scan_load_dyn(sb_);
     const int i = blockIdx.x * SPUB_THREADS + threadIdx.x;
     const int c = __syncthreads_count(i < sb.n && sb.match_node[i] >= 0);
     if (threadIdx.x == 0) tile_cnt[blockIdx.x] = c;
 }
-__global__ void __launch_bounds__(SPUB_THREADS) k_eff_emit(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const int* tile_off, float4* rows, int* scan_index) {
+__global__ void __launch_bounds__(SPUB_THREADS) k_eff_emit(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const int* tile_off, float4* rows, int* scan_index,
+                                                           const LioFeedDev* fd, long long ring) {
     __shared__ int s_warp[SPUB_THREADS / 32];
     __shared__ double s_state[12];
+    pdl_wait();
+    long long base = 0;
+    if (fd) {
+        if (fd->lost) return;   // block-uniform
+        base = fd->eff_base;
+    }
     const ScanBuf sb = scan_load_dyn(sb_);
     if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
     const int i = blockIdx.x * SPUB_THREADS + threadIdx.x;
@@ -558,14 +569,24 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_eff_emit(LioParams P, ScanBuf 
     for (int w = 0; w < warp; ++w) off += s_warp[w];
     float r[4];
     scan_pub_row(P, s_state, sb.body + (size_t)i * 3, sb.wsqrt[i], r);
-    rows[off] = make_float4(r[0], r[1], r[2], r[3]);
-    if (scan_index) scan_index[off] = i;
+    const long long pos = fd ? (base + off) % ring : off;
+    rows[pos] = make_float4(r[0], r[1], r[2], r[3]);
+    if (scan_index) scan_index[pos] = i;
 }
 // rows j = 0 .. ceil(n / skip) - 1 from point j * skip; pts == null: the localised scan.  inten != null: the intensity of point i is
-// inten[i] (the front-end's clouds keep it beside the packed points) instead of column col
+// inten[i] (the front-end's clouds keep it beside the packed points) instead of column col.  fd != null: the source is the scan's
+// FeedDyn (source 2: its full scan, stride 3, intensity inten or 0; source 1: the localised scan)
 __global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBuf sb_, const LioCtrl* ctrl, const float* pts, int n, int stride, int col, int skip, float4* rows,
-                                                             const float* __restrict__ inten) {
+                                                             const float* __restrict__ inten, const LioFeedDev* fd, long long ring) {
     __shared__ double s_state[12];
+    pdl_wait();
+    long long base = 0;
+    if (fd) {
+        if (fd->lost || fd->dyn.src == 0) return;   // block-uniform
+        base = fd->reg_base;
+        pts = nullptr;
+        if (fd->dyn.src == 2) { pts = fd->dyn.pts; n = fd->dyn.n; inten = fd->dyn.inten; stride = 3; col = -1; }
+    }
     if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
     if (!pts) {
         const ScanBuf sb = scan_load_dyn(sb_);
@@ -577,10 +598,55 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBu
         const float* p = pts + (size_t)j * skip * stride;
         float r[4];
         scan_pub_row(P, s_state, p, inten ? inten[(size_t)j * skip] : col >= 0 ? p[col] : 0.0f, r);
-        rows[j] = make_float4(r[0], r[1], r[2], r[3]);
+        rows[fd ? (base + j) % ring : j] = make_float4(r[0], r[1], r[2], r[3]);
     }
 }
 __global__ void k_scan_n(ScanBuf sb_, int* out) { *out = scan_load_dyn(sb_).n; }
+
+// ---- scan feed (immesh_lio_feed_enable): k_feed_head runs right behind the scan's last kernel (k_grow_finish, or the IMU chain's
+// initialisation copies): the state, the header, and the row cursor (feed_append); k_feed_done, behind the row emitters, publishes the
+// scan's number to the host word the reader polls.
+#define FEED_THREADS 128
+__global__ void __launch_bounds__(FEED_THREADS) k_feed_head(ScanBuf sb_, const LioCtrl* ctrl, const int* counters, LioFeedDev* fd, long long* hdr, double* states,
+                                                            long long max_scans, long long max_rows, const int* eff_total, int skip) {
+    pdl_wait();
+    const FeedDyn d = fd->dyn;
+    const long long slot = (d.scan - 1) % max_scans;
+    if (threadIdx.x == 0) {
+        fd->started = d.scan;   // before any byte of the slot changes (a reader checks it after its copy)
+        __threadfence();
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < IM_STATE_DOUBLES; i += blockDim.x) states[slot * IM_STATE_DOUBLES + i] = ctrl->state[i];
+    if (threadIdx.x == 0) {
+        const int iters = d.lio ? ctrl->iters_run : 0;
+        long long ne = 0, nr = 0;
+        if (d.lio) {
+            if (eff_total) ne = *eff_total;
+            const int n = d.src == 2 ? d.n : d.src == 1 ? scan_load_dyn(sb_).n : 0;
+            nr = n > 0 ? (n - 1) / skip + 1 : 0;
+        }
+        long long* h = hdr + slot * IMMESH_LIO_FEED_HDR;
+        feed_append(*fd, ne, nr, max_rows, h);
+        h[IMMESH_FEED_KIND] = d.kind;
+        h[IMMESH_FEED_BRANCH] = d.branch;
+        h[IMMESH_FEED_ITERS] = iters;
+        h[IMMESH_FEED_MATCHES] = iters > 0 ? (long long)ctrl->stats[iters - 1].n_match : 0;
+        h[IMMESH_FEED_CONVERGED] = iters > 0 ? (long long)ctrl->stats[iters - 1].converged : 0;
+        h[IMMESH_FEED_ERR] = counters[IM_LC_ERR];
+        h[IMMESH_FEED_SOURCE] = d.src;
+        h[IMMESH_FEED_SCAN] = d.scan;
+    }
+    __syncthreads();
+    pdl_trigger();
+}
+__global__ void k_feed_done(const LioFeedDev* fd, long long* done) {
+    pdl_wait();
+    if (threadIdx.x == 0) {
+        __threadfence_system();
+        *(volatile long long*)done = fd->dyn.scan;
+    }
+}
 
 // ---- growth of the map pools (immesh_lio_reserve): rebuild of the root hash into a larger table, then the back-pointers to slots
 #define GROW_THREADS 256
@@ -771,10 +837,13 @@ int immesh_lio_create(const immesh_lio_config* cfg, immesh_lio_t** out) {
     return IMMESH_OK;
 }
 
+static void feed_free(immesh_lio* h);
+
 int immesh_lio_destroy(immesh_lio_t* h) {
     if (!h) return IMMESH_OK;
     if (h->stream) cudaStreamSynchronize(h->stream);
     h->graph.destroy();
+    feed_free(h);
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && nccl().CommDestroy) nccl().CommDestroy(h->nccl_comm);
     for (auto& e : h->ev) if (e) cudaEventDestroy(e);
@@ -803,6 +872,7 @@ int immesh_lio_shard(immesh_lio_t* h, int rank, int nranks, const char* unique_i
     if (nranks > IM_MAX_RANKS) return im_fail(IMMESH_E_INVALID, "at most 8 ranks (one node)");
     if (nranks == 1) { h->P.shard_rank = 0; h->P.shard_n = 1; return IMMESH_OK; }
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a handle with automatic growth cannot be sharded (immesh_lio_set_growth(h, 0) first)");
+    if (h->feed.on) return im_fail(IMMESH_E_INVALID, "a handle with the scan feed on cannot be sharded (immesh_lio_feed_enable(h, NULL) first)");
     if (h->lm_on || h->map.node_free)   // its tombstones would need a rebuild of the table, which a sharded handle cannot do
         return im_fail(IMMESH_E_INVALID, "a handle that used the local map (immesh_lio_local_map / immesh_voxelmap_evict_boxes) cannot be sharded");
     if (!nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
@@ -1184,6 +1254,61 @@ static int launch_estimate(immesh_lio* h, bool pdl = false) {
     return IMMESH_OK;
 }
 
+// ---- scan feed.  feed_stage copies the scan's FeedDyn from the pinned ring (in stream order ahead of its kernels); launch_feed queues
+// the record (lio: the scan ran the IESKF, so the effect count, the head and the two row emitters; otherwise the head alone), then
+// k_feed_done; feed_commit numbers the scan as queued and marks it with the feed's event.  pdl as in launch_grow.
+static int feed_stage(immesh_lio* h, const immesh_lio::FeedNext& nx, int kind, int branch, bool lio) {
+    immesh_lio::Feed& f = h->feed;
+    const long long k = f.queued + 1;
+    // the ring entry was last used IM_FEED_DYN_RING scans ago; the staging slots keep far fewer scans in flight, so this never drains
+    if (*(volatile long long*)f.h_done < k - IM_FEED_DYN_RING) IM_CUDA(cudaStreamSynchronize(h->stream));
+    FeedDyn& d = f.h_dyn[k % IM_FEED_DYN_RING];
+    d.scan = k;
+    d.kind = nx.kind >= 0 ? nx.kind : kind;
+    d.branch = nx.kind >= 0 ? nx.branch : branch;
+    d.lio = lio ? 1 : 0;
+    d.src = (!lio || f.registered == 0) ? 0 : (f.registered == 2 && nx.pts) ? 2 : 1;
+    d.pts = d.src == 2 ? nx.pts : nullptr;
+    d.inten = d.src == 2 ? nx.inten : nullptr;
+    d.n = d.src == 2 ? nx.n : 0;
+    d.pad_ = 0;
+    IM_CUDA(cudaMemcpyAsync(&f.dev->dyn, &d, sizeof(FeedDyn), cudaMemcpyHostToDevice, h->stream));
+    return IMMESH_OK;
+}
+static void launch_feed(immesh_lio* h, bool lio, bool pdl = false) {
+    immesh_lio::Feed& f = h->feed;
+    cudaStream_t st = h->stream;
+    const bool eff = lio && f.effect;
+    if (eff) {
+        IM_LAUNCH_PDL(pdl, k_eff_count, f.nb, SPUB_THREADS, 0, st, h->sb, f.tiles);
+        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, f.tiles, f.nb, f.tiles + f.nb);
+    }
+    IM_LAUNCH_PDL(pdl, k_feed_head, 1, FEED_THREADS, 0, st, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)h->d_counters, f.dev, f.hdr, f.states, f.max_scans, f.max_rows,
+                  eff ? (const int*)(f.tiles + f.nb) : (const int*)nullptr, f.skip);
+    if (eff)
+        IM_LAUNCH_PDL(pdl, k_eff_emit, f.nb, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)f.tiles, f.rows, f.idx, (const LioFeedDev*)f.dev, f.max_rows);
+    if (lio && f.registered)
+        IM_LAUNCH_PDL(pdl, k_reg_gather, h->n_sm * 8, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const float*)nullptr, 0, 3, -1, f.skip, f.rows,
+                      (const float*)nullptr, (const LioFeedDev*)f.dev, f.max_rows);
+    IM_LAUNCH_PDL(pdl, k_feed_done, 1, 32, 0, st, (const LioFeedDev*)f.dev, f.d_done);
+}
+static int feed_commit(immesh_lio* h) {
+    ++h->feed.queued;
+    IM_CUDA(cudaEventRecord(h->feed.ev, h->stream));
+    return IMMESH_OK;
+}
+static void feed_free(immesh_lio* h) {
+    immesh_lio::Feed& f = h->feed;
+    if (f.ev) cudaEventDestroy(f.ev);
+    if (f.stream) cudaStreamDestroy(f.stream);
+    f.ev = nullptr; f.stream = nullptr;
+    f.dev_mem = immesh::MemSet();
+    f.pinned = immesh::MemSet(immesh::MemSet::Pinned);
+    f.dev = nullptr; f.hdr = nullptr; f.states = nullptr; f.rows = nullptr; f.idx = nullptr; f.tiles = nullptr;
+    f.h_dyn = nullptr; f.h_done = nullptr; f.d_done = nullptr;
+    f.on = 0; f.queued = 0;
+}
+
 int immesh_lio_predict(immesh_lio_t* h, double dt, double cov_gyr, double cov_acc) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     IM_CUDA(cudaStreamSynchronize(h->stream));
@@ -1244,8 +1369,10 @@ int immesh_voxelmap_update(immesh_lio_t* h) {
 // queue predict + estimate + update for one scan; no host synchronisation unless both staging slots are busy.  Host work per
 // scan in the pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D ScanDyn +
 // ONE cudaGraphLaunch (no node is touched) + ONE D2H of the LioOut block + one event.
-static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device, double dt, double cov_gyr, double cov_acc, bool allow_graph) {
+static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device, double dt, double cov_gyr, double cov_acc, bool allow_graph, int kind) {
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    const immesh_lio::FeedNext nx = h->feed_next;   // the front-end's or the IMU chain's scan, for this call only
+    h->feed_next = immesh_lio::FeedNext();
     const int grc = lio_growth_check(h, n);
     if (grc) return grc;
     const int s = (++h->step_counter) & (IM_SLOTS - 1);
@@ -1262,13 +1389,17 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     if (timing) IM_CUDA(cudaEventRecord(h->ev[0], h->stream));
     int rc = upload_scan(h, body, n, on_device, s, dt, cov_gyr, cov_acc);
     if (rc) return rc;
+    if (h->feed.on) {
+        rc = feed_stage(h, nx, kind, 0, true);
+        if (rc) return rc;
+    }
     // The pipelined entry points replay the scan's launch sequence as one CUDA graph, captured once: every per-scan value is
     // read from the device-resident ScanDyn, so a replay is a bare cudaGraphLaunch.  The blocking entry points launch
     // directly, with stage timing events in between.
     bool queued = false;
     int lrc = IMMESH_OK;
     if (!timing) {
-        const unsigned sig = 1u | (h->lm_on ? 4u : 0u) | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
+        const unsigned sig = 1u | (h->feed.on ? 2u : 0u) | (h->lm_on ? 4u : 0u) | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
         // one GPU: every kernel after k_predict is a programmatic dependent launch (the sharded paths wait on peers and NCCL)
         const bool pdl = h->P.shard_n <= 1;
         queued = immesh::run_graphed_static(h->graph, sig, h->stream, [&] {
@@ -1276,6 +1407,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
             if (h->lm_on) launch_local_map(h, nullptr, 0, pdl);
             lrc = launch_estimate(h, pdl);
             launch_grow(h, 0, pdl);
+            if (h->feed.on) launch_feed(h, true, pdl);
         }) == cudaSuccess;
         if (!queued) h->use_graph = 0;   // not expected; keep working through direct launches
     }
@@ -1293,6 +1425,12 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(h->h_out + s, &h->d_ctrl->out, sizeof(LioOut), cudaMemcpyDeviceToHost, h->stream));
     if (!queued) IM_CUDA(cudaEventRecord(h->ev[3], h->stream));
+    if (h->feed.on) {
+        if (!queued) launch_feed(h, true);   // behind ev[3]: immesh_lio_last_timing stays the step's own
+        IM_CUDA(cudaGetLastError());
+        rc = feed_commit(h);
+        if (rc) return rc;
+    }
     IM_CUDA(cudaEventRecord(h->ev_slot[s], h->stream));
     h->slot_busy[s] = 1;
     h->slot_step[s] = h->map_steps;
@@ -1322,26 +1460,28 @@ static int lio_wait_impl(immesh_lio_t* h, double* state_out, int* iters_run, boo
 }
 
 int immesh_lio_step(immesh_lio_t* h, const float* body, int n, double dt, double cov_gyr, double cov_acc, double* state_out, int* iters_run) {
-    int rc = lio_enqueue(h, body, n, 0, dt, cov_gyr, cov_acc, false);
+    int rc = lio_enqueue(h, body, n, 0, dt, cov_gyr, cov_acc, false, IMMESH_FEED_KIND_STEP);
     return rc ? rc : lio_wait_impl(h, state_out, iters_run, true);
 }
 int immesh_lio_step_dev(immesh_lio_t* h, const float* d_body, int n, double dt, double cov_gyr, double cov_acc, double* state_out, int* iters_run) {
-    int rc = lio_enqueue(h, d_body, n, 1, dt, cov_gyr, cov_acc, false);
+    int rc = lio_enqueue(h, d_body, n, 1, dt, cov_gyr, cov_acc, false, IMMESH_FEED_KIND_STEP_DEV);
     return rc ? rc : lio_wait_impl(h, state_out, iters_run, true);
 }
 int immesh_lio_step_async(immesh_lio_t* h, const float* body, int n, int on_device, double dt, double cov_gyr, double cov_acc) {
-    return lio_enqueue(h, body, n, on_device, dt, cov_gyr, cov_acc, true);
+    return lio_enqueue(h, body, n, on_device, dt, cov_gyr, cov_acc, true, IMMESH_FEED_KIND_STEP_ASYNC);
 }
 // the scan AND its point count are device resident (e.g. produced by the device front-end): n is read at execution time
 int immesh_lio_step_async_dev_n(immesh_lio_t* h, const float* d_body_xyz, int n_max, const int* d_n, double dt, double cov_gyr, double cov_acc) {
     if (!h || !d_n || n_max < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
     h->next_n_dev = d_n;
-    return lio_enqueue(h, d_body_xyz, n_max, 1, dt, cov_gyr, cov_acc, true);
+    return lio_enqueue(h, d_body_xyz, n_max, 1, dt, cov_gyr, cov_acc, true, IMMESH_FEED_KIND_STEP_ASYNC_DEV_N);
 }
 // voxel_map_init queued like a pipelined step (internal: the first scan after the IMU initialisation, immesh_lio_step_async_imu): the
 // build kernels of immesh_voxelmap_build on a device-resident full scan, behind the staging-slot protocol, without a host wait
 int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, int n) {
     if (!h || !d_body_xyz || n < 1) return im_fail(IMMESH_E_INVALID, "bad argument");
+    const immesh_lio::FeedNext nx = h->feed_next;   // the IMU chain's branch 2 (recorded with its header and state)
+    h->feed_next = immesh_lio::FeedNext();
     if (n > h->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than max_scan_points");
     const int grc = lio_growth_check(h, n);
     if (grc) return grc;
@@ -1359,7 +1499,16 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     if (h->lm_on) launch_local_map(h);   // places the box at the building scan's pose
     launch_grow(h, 1);
     h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
+    if (h->feed.on) {
+        rc = feed_stage(h, nx, IMMESH_FEED_KIND_IMU, 2, false);
+        if (rc) return rc;
+        launch_feed(h, false);
+    }
     IM_CUDA(cudaGetLastError());
+    if (h->feed.on) {
+        rc = feed_commit(h);
+        if (rc) return rc;
+    }
     IM_CUDA(cudaMemcpyAsync(h->h_out + s, &h->d_ctrl->out, sizeof(LioOut), cudaMemcpyDeviceToHost, h->stream));
     IM_CUDA(cudaEventRecord(h->ev_slot[s], h->stream));
     h->slot_busy[s] = 1;
@@ -1369,6 +1518,83 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     return IMMESH_OK;
 }
 int immesh_lio_wait(immesh_lio_t* h, double* state_out, int* iters_run) { return lio_wait_impl(h, state_out, iters_run, false); }
+// internal (immesh_lio_step_async_imu, branch 1): record the scan in the feed, header and state only, behind the work queued for it
+int immesh_lio_feed_record_state(immesh_lio_t* h, int kind, int branch) {
+    if (!h || !h->feed.on) return IMMESH_OK;
+    const int rc = feed_stage(h, immesh_lio::FeedNext(), kind, branch, false);
+    if (rc) return rc;
+    launch_feed(h, false);
+    IM_CUDA(cudaGetLastError());
+    return feed_commit(h);
+}
+
+int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* c) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_enable: the scan feed runs on a single GPU: the handle is sharded");
+    if (c && (c->max_scans < 1 || c->max_scans > (1LL << 24) || c->max_rows < 0 || c->max_rows > (1LL << 32) || (c->effect != 0 && c->effect != 1) ||
+              c->registered < 0 || c->registered > 2 || c->point_skip < 1 || ((c->effect || c->registered) && c->max_rows < 1)))
+        return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_enable: needs max_scans in [1, 2^24], max_rows in [0, 2^32] (>= 1 with rows), effect 0 or 1, "
+                                         "registered 0, 1 or 2 and point_skip >= 1");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    h->graph.destroy();   // the launch sequence changes
+    feed_free(h);
+    if (!c) return IMMESH_OK;
+    immesh_lio::Feed& f = h->feed;
+    f.max_scans = c->max_scans;
+    f.max_rows = c->max_rows;
+    f.effect = c->effect;
+    f.registered = c->registered;
+    f.skip = c->point_skip;
+    f.nb = (h->max_scan + SPUB_THREADS - 1) / SPUB_THREADS;
+    if (f.nb < 1) f.nb = 1;
+    auto fail = [&](cudaError_t e) { feed_free(h); cudaGetLastError(); return immesh::im_fail_cuda(e, __FILE__, __LINE__); };
+    cudaError_t e;
+    if ((e = f.dev_mem.alloc(&f.dev, 1, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.hdr, (size_t)f.max_scans * IMMESH_LIO_FEED_HDR, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.states, (size_t)f.max_scans * IM_STATE_DOUBLES, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.rows, (size_t)std::max<long long>(f.max_rows, 1))) != cudaSuccess) return fail(e);
+    if (f.effect && (e = f.dev_mem.alloc(&f.idx, (size_t)f.max_rows)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.tiles, (size_t)f.nb + 1, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.pinned.alloc(&f.h_dyn, IM_FEED_DYN_RING)) != cudaSuccess) return fail(e);
+    if ((e = f.pinned.alloc(&f.h_done, 1)) != cudaSuccess) return fail(e);
+    *f.h_done = 0;
+    std::memset(f.h_dyn, 0, IM_FEED_DYN_RING * sizeof(FeedDyn));
+    if ((e = cudaHostGetDevicePointer((void**)&f.d_done, f.h_done, 0)) != cudaSuccess) return fail(e);
+    if ((e = cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
+    if ((e = cudaEventCreateWithFlags(&f.ev, cudaEventDisableTiming)) != cudaSuccess) return fail(e);
+    if ((e = cudaEventRecord(f.ev, h->stream)) != cudaSuccess) return fail(e);
+    if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return fail(e);
+    f.on = 1;
+    return IMMESH_OK;
+}
+
+int immesh_lio_feed(immesh_lio_t* h, int64_t since, int wait, int64_t* scans, double* states, int cap_scans, float* rows, int32_t* row_index, int64_t cap_rows,
+                    int64_t* counts) {
+    if (!h || !counts || cap_scans < 0 || cap_rows < 0 || (cap_scans > 0 && !scans)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    for (int k = 0; k < 4; ++k) counts[k] = 0;
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed: the handle is sharded");
+    immesh_lio::Feed& f = h->feed;
+    if (!f.on) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed: the scan feed is not enabled (immesh_lio_feed_enable)");
+    if (since < 0 || since > f.queued) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed: since_scan must be in [0, newest queued scan]");
+    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued scan's record, nothing else
+    const long long fin = *(volatile long long*)f.h_done;
+    counts[2] = fin;
+    counts[3] = f.queued;
+    const FeedRings rings{f.max_scans, f.max_rows, f.hdr, f.states, f.rows, f.idx};
+    auto copy = [&](void* dst, const void* src, size_t bytes) {   // on the feed's stream, never the handle's
+        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
+        return IMMESH_OK;
+    };
+    auto marks = [&](long long* m) {
+        IM_CUDA(cudaMemcpyAsync(m, &f.dev->started, 2 * sizeof(long long), cudaMemcpyDeviceToHost, f.stream));
+        IM_CUDA(cudaStreamSynchronize(f.stream));
+        return IMMESH_OK;
+    };
+    const int rc = feed_read(rings, since, fin, scans, states, cap_scans, rows, row_index, cap_rows, counts, copy, marks);
+    if (rc == IMMESH_E_RANGE) return im_fail(rc, "immesh_lio_feed: scans of the range left the rings or were overwritten while they were read; read on from counts[2]");
+    if (rc == IMMESH_E_CAPACITY) return im_fail(rc, "immesh_lio_feed: more scans or rows than the caps (counts holds them)");
+    return rc;
+}
 // queue a write of `bytes` bytes over a caller-provided device buffer on the localization stream (benchmark L2 flush)
 int immesh_lio_enqueue_memset(immesh_lio_t* h, void* d_buf, size_t bytes) {
     if (!h || !d_buf) return im_fail(IMMESH_E_INVALID, "null argument");
@@ -1626,7 +1852,8 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows, int32_t* scan_index, i
     if (total == 0) return IMMESH_OK;
     IM_CUDA(h->scratch.regrow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)total, 1024));
     if (scan_index) IM_CUDA(h->scratch.regrow(&h->d_spub_idx, &h->spub_idx_cap, (size_t)total, 1024));
-    IM_LAUNCH(k_eff_emit, nb, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)tiles, h->d_spub_rows, scan_index ? h->d_spub_idx : (int*)nullptr);
+    IM_LAUNCH(k_eff_emit, nb, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const int*)tiles, h->d_spub_rows, scan_index ? h->d_spub_idx : (int*)nullptr,
+              (const LioFeedDev*)nullptr, 0LL);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost, st));
     if (scan_index) IM_CUDA(cudaMemcpyAsync(scan_index, h->d_spub_idx, (size_t)total * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1669,7 +1896,8 @@ static int registered_rows(immesh_lio_t* h, const float* pts, const float* inten
     }
     IM_CUDA(h->scratch.regrow(&h->d_spub_rows, &h->spub_rows_cap, (size_t)m, 1024));
     const int g = std::min((m + SPUB_THREADS - 1) / SPUB_THREADS, h->n_sm * 16);
-    IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows, inten);
+    IM_LAUNCH(k_reg_gather, g, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, src, n, stride, intensity_col, point_skip, h->d_spub_rows, inten,
+              (const LioFeedDev*)nullptr, 0LL);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(rows, h->d_spub_rows, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));

@@ -116,6 +116,46 @@ int immesh_kitti_pose_line(const double* state /*[>= 12]: rot_end[9] row-major, 
     return (n > 0 && n < cap) ? IMMESH_OK : immesh::im_fail(IMMESH_E_CAPACITY, "buffer too small");
 }
 
+// publish_odometry's pose: pos_end, then RotMtoEuler(rot_end) turned into a quaternion by tf's setRPY (the rule is in the header)
+int immesh_odometry_pose(const double* s, double* out) {
+    if (!s || !out) return immesh::im_fail(IMMESH_E_INVALID, "null argument");
+    const double r00 = s[0], r10 = s[3], r11 = s[4], r12 = s[5], r20 = s[6], r21 = s[7], r22 = s[8];
+    const double sy = std::sqrt(r00 * r00 + r10 * r10);
+    double roll, pitch, yaw;
+    if (!(sy < 1e-6)) {
+        roll = std::atan2(r21, r22);
+        pitch = std::atan2(-r20, sy);
+        yaw = std::atan2(r10, r00);
+    } else {
+        roll = std::atan2(-r12, r11);
+        pitch = std::atan2(-r20, sy);
+        yaw = 0;
+    }
+    const double hy = yaw * 0.5, hp = pitch * 0.5, hr = roll * 0.5;
+    const double cy = std::cos(hy), sy2 = std::sin(hy), cp = std::cos(hp), sp = std::sin(hp), cr = std::cos(hr), sr = std::sin(hr);
+    out[0] = s[9]; out[1] = s[10]; out[2] = s[11];
+    out[3] = sr * cp * cy - cr * sp * sy2;
+    out[4] = cr * sp * cy + sr * cp * sy2;
+    out[5] = cr * cp * sy2 - sr * sp * cy;
+    out[6] = cr * cp * cy + sr * sp * sy2;
+    return IMMESH_OK;
+}
+
+// dump_lio_state_to_log's line (the rule is in the header)
+int immesh_lio_state_line(const double* s, double t, char* buf, int cap) {
+    if (!s || !buf || cap < 1) return immesh::im_fail(IMMESH_E_INVALID, "bad argument");
+    const double tr = (s[0] + s[4]) + s[8];
+    const double theta = (tr > 3.0 - 1e-6) ? 0.0 : std::acos(0.5 * (tr - 1));
+    const double K[3] = {s[7] - s[5], s[2] - s[6], s[3] - s[1]};
+    const double f = std::abs(theta) < 0.001 ? 0.5 : 0.5 * theta / std::sin(theta);
+    const double v[24] = {K[0] * f, K[1] * f, K[2] * f, s[9], s[10], s[11], 0.0, 0.0, 0.0, s[12], s[13], s[14], 0.0, 0.0, 0.0,
+                          s[15], s[16], s[17], s[18], s[19], s[20], s[21], s[22], s[23]};
+    int len = std::snprintf(buf, (size_t)cap, "%lf ", t);
+    for (int i = 0; i < 24 && len >= 0 && len < cap; ++i) len += std::snprintf(buf + len, (size_t)(cap - len), "%lf ", v[i]);
+    if (len >= 0 && len < cap) len += std::snprintf(buf + len, (size_t)(cap - len), "\r\n");
+    return (len > 0 && len < cap) ? IMMESH_OK : immesh::im_fail(IMMESH_E_CAPACITY, "buffer too small");
+}
+
 const char* immesh_last_error(void) { return immesh::last_error_storage().c_str(); }
 const char* immesh_version(void) { return "immesh_b200 0.1.0 (sm_90a)"; }
 

@@ -250,6 +250,83 @@ int immesh_lio_effect_cloud(immesh_lio_t* h, float* rows /*[cap][4]*/, int32_t* 
 int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int stride, int intensity_col, int on_device,
                                 int point_skip, float* rows /*[cap][4]*/, int cap, int* n_out);
 
+/* Scan feed: what the reference publishes after every scan (publish_odometry, kitti_log, dump_lio_state_to_log, publish_path,
+ * publish_mavros, /cloud_registered, /cloud_effected; src/voxel_mapping.cpp:1963-2002), recorded on the device in stream order as
+ * part of each scan's launch sequence, so that a node on the queued chain can publish scan k after scan k + 1 is queued, without
+ * draining.
+ * immesh_lio_feed_enable(h, cfg) drains h, drops its captured launch sequence and allocates the rings once; numbering restarts at
+ *   scan 1.  cfg == NULL turns the feed off and frees the rings; while it is off, nothing is launched or recorded for it.
+ *   max_scans >= 1: header and state ring; max_rows: row ring (>= 1 when effect or registered is set); effect 0/1; registered 0 (none),
+ *   1 (the down-sampled scan, dense_map_en 0) or 2 (the full scan, dense_map_en 1); point_skip >= 1 (publish/pub_point_skip).
+ *   Other values, or a sharded handle: IMMESH_E_INVALID.  immesh_lio_shard refuses a handle with the feed on.
+ * Every call of immesh_lio_step, _step_dev, _step_async, _step_async_dev_n, _step_async_raw, _raw_i, _imu and _imu_i records one scan
+ * (the IMU chain's branches 1 and 2 too: a header and the state, no rows).  The staged calls record nothing.
+ *   header (IMMESH_LIO_FEED_HDR int64): IMMESH_FEED_SCAN number; KIND (IMMESH_FEED_KIND_*); BRANCH (0 LiDAR-only, else the IMU
+ *     chain's 1/2/3); ITERS run; MATCHES of the last IESKF iteration (m_effct_feat_num); CONVERGED flag of that iteration; ERR (the
+ *     IM_LC_ERR flags); ROW_BEGIN, ROW_EFFECT_END, ROW_END: the scan's effect rows [BEGIN, EFFECT_END) and registered rows
+ *     [EFFECT_END, END), numbered over the feed; SOURCE of the registered rows (0 none, 1 down-sampled, 2 full scan); ROWS_LOST.
+ *   state: the 348 doubles the scan ended with, bit-identical to immesh_lio_wait right after it (branches 1 and 2: the state as the
+ *     branch left it).
+ *   rows: effect = 1: immesh_lio_effect_cloud right after the scan (row_index = its scan_index).  registered = 1:
+ *     immesh_lio_registered_cloud(h, NULL, ..., point_skip); registered = 2: on _raw and _imu, immesh_lio_registered_cloud of
+ *     immesh_voxelgrid_input_points (stride 3, intensity column -1), on _raw_i and _imu_i immesh_lio_frontend_cloud(h, vg, 1,
+ *     point_skip), elsewhere (no full scan) source 1.  row_index of a registered row: -1.
+ *   A scan whose rows exceed max_rows keeps its header and state and sets ROWS_LOST.  A loss never fails a step or changes the state,
+ *   the map or the mesh.
+ * immesh_lio_feed(h, since_scan, wait, ...) returns the scans (since_scan, newest finished] oldest first, their states (or NULL) and
+ *   their rows concatenated in scan order (or NULL).  wait = 0 never blocks on unfinished work; wait = 1 first waits for the newest
+ *   queued scan.  counts = [scans, rows, newest finished, newest queued].  cap_scans = 0: a count query (IMMESH_OK, nothing written).
+ *   More scans than cap_scans, or rows != NULL and more rows than cap_rows: IMMESH_E_CAPACITY with the counts, nothing written.  A
+ *   scan of the range whose header or rows were overwritten in the rings: IMMESH_E_RANGE with counts[2] set (read on from there).
+ *   since_scan < 0 or beyond the newest queued scan, the feed off, or a sharded handle: IMMESH_E_INVALID. */
+typedef struct {
+    int64_t max_scans;   /* header + state ring, in scans */
+    int64_t max_rows;    /* row ring, rows of IMMESH_SCAN_PUB_COLS floats */
+    int effect;          /* 1: record publish_effect_world's rows */
+    int registered;      /* 0 none; 1 the down-sampled scan; 2 the full scan where the chain has one */
+    int point_skip;      /* >= 1 */
+    int pad;
+} immesh_lio_feed_config;
+#define IMMESH_LIO_FEED_HDR 12
+#define IMMESH_FEED_SCAN 0
+#define IMMESH_FEED_KIND 1
+#define IMMESH_FEED_BRANCH 2
+#define IMMESH_FEED_ITERS 3
+#define IMMESH_FEED_MATCHES 4
+#define IMMESH_FEED_CONVERGED 5
+#define IMMESH_FEED_ERR 6
+#define IMMESH_FEED_ROW_BEGIN 7
+#define IMMESH_FEED_ROW_EFFECT_END 8
+#define IMMESH_FEED_ROW_END 9
+#define IMMESH_FEED_SOURCE 10
+#define IMMESH_FEED_ROWS_LOST 11
+/* IMMESH_FEED_KIND: the entry point that queued the scan */
+#define IMMESH_FEED_KIND_STEP 0
+#define IMMESH_FEED_KIND_STEP_DEV 1
+#define IMMESH_FEED_KIND_STEP_ASYNC 2
+#define IMMESH_FEED_KIND_STEP_ASYNC_DEV_N 3
+#define IMMESH_FEED_KIND_RAW 4
+#define IMMESH_FEED_KIND_RAW_I 5
+#define IMMESH_FEED_KIND_IMU 6
+#define IMMESH_FEED_KIND_IMU_I 7
+int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* cfg /* NULL: off */);
+int immesh_lio_feed(immesh_lio_t* h, int64_t since_scan, int wait, int64_t* scans /*[cap_scans][12]*/, double* states /*[cap_scans][348] or NULL*/,
+                    int cap_scans, float* rows /*[cap_rows][4] or NULL*/, int32_t* row_index /*[cap_rows] or NULL*/, int64_t cap_rows,
+                    int64_t* counts /*[4]*/);
+/* Host-side formatters of a recorded state (no device work).
+ * immesh_odometry_pose: out = pos_end, then the quaternion x y z w that publish_odometry, publish_path and publish_mavros send:
+ *   (roll, pitch, yaw) = RotMtoEuler(rot_end) (include/so3_math.h: sy = sqrt(r00^2 + r10^2); sy >= 1e-6: roll = atan2(r21, r22),
+ *   pitch = atan2(-r20, sy), yaw = atan2(r10, r00); else roll = atan2(-r12, r11), pitch = atan2(-r20, sy), yaw = 0), then
+ *   tf::createQuaternionMsgFromRollPitchYaw: with c_a = cos(a / 2), s_a = sin(a / 2) of a = roll r, pitch p, yaw y,
+ *   x = s_r c_p c_y - c_r s_p s_y, y = c_r s_p c_y + s_r c_p s_y, z = c_r c_p s_y - s_r s_p c_y, w = c_r c_p c_y + s_r s_p s_y.
+ *   This is not the quaternion of rot_end that Eigen would give (immesh_kitti_pose_line's).
+ * immesh_lio_state_line: dump_lio_state_to_log's line (src/voxel_mapping_common.cpp:100-117): t, Log(rot_end) (include/so3_math.h:
+ *   theta = 0 when the trace exceeds 3 - 1e-6, else acos((trace - 1) / 2); K = (r21 - r12, r02 - r20, r10 - r01); K / 2 when
+ *   |theta| < 0.001, else theta / 2 / sin(theta) K), pos_end, three zeros, vel_end, three zeros, bias_g, bias_a, gravity, each
+ *   printed "%lf ", then "\r\n".  t is the caller's (lidar_beg_time - first_lidar_time).  A line longer than cap - 1: IMMESH_E_CAPACITY. */
+int immesh_odometry_pose(const double* state /*[>= 12]*/, double* out /*[7]*/);
+int immesh_lio_state_line(const double* state /*[>= 24]*/, double t, char* buf, int cap);
+
 /* device time (ms, CUDA events on the handle's stream) of the stages of the last immesh_lio_step call:
  * [0] whole step incl. H2D, [1] residual+solve iterations, [2] map update */
 int immesh_lio_last_timing(immesh_lio_t* h, double* ms /*[3]*/);
