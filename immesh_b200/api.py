@@ -66,6 +66,10 @@ FEED_HDR_KEYS = ("scan", "kind", "branch", "iters", "matches", "converged", "err
 FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i")   # IMMESH_FEED_KIND_*
 
 
+MARKER_HDR = 10   # IMMESH_LIO_FEED_MARKER_HDR: the header columns of a scan's plane-marker record, in this order
+MARKER_HDR_KEYS = ("scan", "row_begin", "row_end", "rows_needed", "lost", "roots_walked", "plane", "sub_plane", "sub_sub_plane", "update")
+
+
 class FeedLost(RuntimeError):
     """immesh_lio_feed returned IMMESH_E_RANGE: scans of the range left the rings.  Read on from newest_finished."""
 
@@ -236,6 +240,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_lio_frontend_cloud", [vp, vp, C.c_int, C.c_int, fp, C.c_int, ip]),
         ("immesh_lio_feed_enable", [vp, C.POINTER(_FeedCfg)]),
         ("immesh_lio_feed", [vp, C.c_int64, C.c_int, C.POINTER(C.c_int64), dp, C.c_int, fp, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64)]),
+        ("immesh_lio_feed_markers_enable", [vp, C.c_int64]),
+        ("immesh_lio_feed_markers", [vp, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.c_int, dp, C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_odometry_pose", [dp, dp]),
         ("immesh_lio_state_line", [dp, C.c_double, C.c_char_p, C.c_int]),
     ):
@@ -544,6 +550,40 @@ class Lio:
         else:
             raise RuntimeError("lio_feed: the scans kept finishing faster than they were read")
         return dict(scans=scans[:ns], states=states[:ns], rows=rows[:nr], row_index=idx[:nr], newest_finished=int(counts[2]), newest_queued=int(counts[3]))
+
+    def feed_markers_enable(self, max_rows: int):
+        """Record each fed scan's plane-map markers (pubPlaneMap) in a ring of max_rows rows (immesh_lio_feed_markers_enable); 0 turns
+        the recording off.  Needs the feed on; feed_enable and feed_disable turn it off."""
+        _check(self.lib, self.lib.immesh_lio_feed_markers_enable(self._h, int(max_rows)), "lio_feed_markers_enable")
+
+    def feed_markers(self, since: int, wait: bool = False):
+        """The plane-marker records of the scans (since, newest finished]: dict(scans=int64[m, MARKER_HDR] (MARKER_HDR_KEYS),
+        rows=float64[r, PLANE_MARKER_COLS] as plane_markers() gives them, newest_finished, newest_queued).  wait=False never blocks on
+        unfinished work.  Raises FeedLost when records of the range left the rings."""
+        counts = np.zeros(4, dtype=np.int64)
+        cp = counts.ctypes.data_as(C.POINTER(C.c_int64))
+        for _ in range(8):   # scans may finish between the count query and the read
+            rc = self.lib.immesh_lio_feed_markers(self._h, since, 1 if wait else 0, None, 0, None, 0, cp)
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, "lio_feed_markers")
+            ns, nr = int(counts[0]), int(counts[1])
+            scans = np.zeros((max(ns, 1), MARKER_HDR), dtype=np.int64)
+            rows = np.zeros((max(nr, 1), PLANE_MARKER_COLS))
+            if ns == 0:
+                break
+            rc = self.lib.immesh_lio_feed_markers(self._h, since, 0, scans.ctypes.data_as(C.POINTER(C.c_int64)), ns, rows.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  nr, cp)
+            if rc == -3:
+                continue
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, "lio_feed_markers")
+            ns, nr = int(counts[0]), int(counts[1])
+            break
+        else:
+            raise RuntimeError("lio_feed_markers: the scans kept finishing faster than they were read")
+        return dict(scans=scans[:ns], rows=rows[:nr], newest_finished=int(counts[2]), newest_queued=int(counts[3]))
 
     def frontend_cloud(self, vg: "VoxelGrid", dense: bool, point_skip=1):
         """publish_frame_world from the front-end clouds of the last _i step through vg (immesh_lio_frontend_cloud): float32[m, 4] rows

@@ -192,6 +192,26 @@ def build_lio_feed(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "lio_feed", "emu_lio_feed.cpp"), EMU_LIO_FEED, force)
 
 
+EMU_LIO_FEED_MARKERS = os.path.join(_ROOT, "tests", "lio_feed", "libimmesh_emu_lio_feed_markers.so")
+
+
+def build_lio_feed_markers(force=False):
+    """tests/lio_feed: the scan feed's plane-marker rings (marker_append, plane_pub_at, feed_read on marker_rings) with the device
+    kernels' order restated on the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "lio_feed", "emu_lio_feed_markers.cpp"), EMU_LIO_FEED_MARKERS, force)
+
+
+RS_CHECK = os.path.join(_ROOT, "tests", "radix_sort", "librs_check.so")
+
+
+def build_rs_check(force=False):
+    """tests/radix_sort: the radix sort (immesh_b200/csrc/radix_sort.cuh) with a host count and with a device count on a chosen grid"""
+    src = os.path.join(_ROOT, "tests", "radix_sort", "rs_check.cu")
+    if force or _newer(RS_CHECK, [src, os.path.join(CSRC, "radix_sort.cuh"), os.path.abspath(__file__)]):
+        subprocess.check_call(["nvcc", *NVCC_FLAGS, "-ccbin", GXX, "-o", RS_CHECK, src], cwd=_ROOT)
+    return RS_CHECK
+
+
 EMU_EVAL = os.path.join(_ROOT, "tests", "eval", "libimmesh_emu_eval.so")
 
 
@@ -251,6 +271,8 @@ def build_all(force=False):
     build_view_overlay(force)
     build_changes(force)
     build_lio_feed(force)
+    build_lio_feed_markers(force)
+    build_rs_check(force)
     build_eval(force)
     build_local_map(force)
     build_dev_mem(force)

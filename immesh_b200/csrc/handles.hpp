@@ -127,6 +127,15 @@ struct immesh_lio {
         cudaStream_t stream = nullptr;    // the reader's copies (never the handle's stream)
         cudaEvent_t ev = nullptr;         // recorded behind the newest scan's record
         immesh::MemSet dev_mem, pinned{immesh::MemSet::Pinned};
+        // plane-map markers (immesh_lio_feed_markers_enable): on while mk_rows > 0
+        long long mk_rows = 0;            // marker ring, rows of IMMESH_PLANE_MARKER_COLS doubles
+        immesh::LioMarkDev* mk_dev = nullptr;
+        long long* mk_hdr = nullptr;      // [max_scans][IMMESH_LIO_FEED_MARKER_HDR]
+        double* mk_ring = nullptr;        // [mk_rows][IMMESH_PLANE_MARKER_COLS]
+        unsigned int* mk_sort = nullptr;  // [4][mk_cap]: the key sort's two buffer pairs; then the roots' slots and row offsets
+        int* mk_hist = nullptr;           // [256 * tiles of mk_cap]
+        size_t mk_cap = 0;                // root slots the sort scratch covers (the hash capacity when it was sized)
+        immesh::MemSet mk_mem, mk_scratch;
     } feed;
 };
 #define IM_FEED_DYN_RING 64

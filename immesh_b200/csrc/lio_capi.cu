@@ -502,7 +502,12 @@ namespace {
 }
 #define PUB_THREADS 256
 static_assert(IM_PUB_COLS == IMMESH_PLANE_MARKER_COLS, "plane-marker row width");
-__global__ void __launch_bounds__(PUB_THREADS) k_pub_keys(VoxelMapDev map, int n, int hi, const unsigned int* order, unsigned int* kout, unsigned int* vout) {
+// n_dev (or null): the count is read on the device.  Every path waits for the predecessor first (launched with IM_LAUNCH_PDL in the
+// scan feed's markers).
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_keys(VoxelMapDev map, int n, const int* n_dev, int hi, const unsigned int* order, unsigned int* kout,
+                                                          unsigned int* vout) {
+    pdl_wait();
+    if (n_dev) n = *n_dev;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const unsigned int v = order ? order[i] : (unsigned int)i;
         const unsigned long long key = map.keys[map.pub_list[v]];
@@ -511,7 +516,9 @@ __global__ void __launch_bounds__(PUB_THREADS) k_pub_keys(VoxelMapDev map, int n
     }
 }
 // per root (in key order): slot, row count; the four reference counters summed with integer atomics (order-free)
-__global__ void __launch_bounds__(PUB_THREADS) k_pub_count(VoxelMapDev map, int n, const unsigned int* order, int* slots, int* cnt, int* counts) {
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_count(VoxelMapDev map, int n, const int* n_dev, const unsigned int* order, int* slots, int* cnt, int* counts) {
+    pdl_wait();
+    if (n_dev) n = *n_dev;
     int c[4] = {0, 0, 0, 0};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int slot = map.pub_list[order[i]];
@@ -522,12 +529,45 @@ __global__ void __launch_bounds__(PUB_THREADS) k_pub_count(VoxelMapDev map, int 
     for (int k = 0; k < 4; ++k)
         if (c[k]) atomicAdd(counts + k, c[k]);
 }
-// per root: its rows at its offset, flags cleared; roots that stay pending go back on the (reset) list
-__global__ void __launch_bounds__(PUB_THREADS) k_pub_emit(VoxelMapDev map, int n, const int* slots, const int* off, double* rows) {
+// per root: its rows at its offset, flags cleared; roots that stay pending go back on the (reset) list.  md (or null): the scan
+// feed's markers -- nothing when the scan's rows were lost, else the rows at the ring cursor k_mark_head placed (row r in slot r % ring)
+__global__ void __launch_bounds__(PUB_THREADS) k_pub_emit(VoxelMapDev map, int n, const int* slots, const int* off, double* rows, const LioMarkDev* md, long long ring) {
+    pdl_wait();
+    long long base = 0;
+    if (md) {
+        if (md->lost) return;
+        n = md->n;
+        base = md->base;
+    }
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int slot = slots[i];
-        if (plane_pub_commit(map, slot, rows + (size_t)off[i] * IM_PUB_COLS)) map.pub_list[atomicAdd(map.pub_n, 1)] = slot;
+        if (plane_pub_commit(map, slot, rows, base + off[i], ring)) map.pub_list[atomicAdd(map.pub_n, 1)] = slot;
     }
+}
+// ---- the scan feed's plane-map markers (immesh_lio_feed_markers_enable): the publication above, queued in the scan's launch sequence
+// with every count read on the device.  k_mark_begin takes the pending count; the key sort, k_pub_count and k_pub_scan run over it;
+// k_mark_head places the rows at the ring cursor (or loses them all), writes the header and -- only when the rows fit -- resets the
+// list (marker_header), so that k_pub_emit publishes and settles the marks; it returns at once for a lost scan (md->lost), the
+// case where marker_header left the list as it was.  A lost scan consumes nothing.
+__global__ void k_mark_begin(const int* pub_n, LioMarkDev* md) {
+    pdl_wait();
+    if (threadIdx.x == 0) md->n = *pub_n;
+    if (threadIdx.x < 5) md->misc[threadIdx.x] = 0;
+}
+__global__ void __launch_bounds__(1024) k_pub_scan(int* cnt, const LioMarkDev* md, int* total) {
+    pdl_wait();
+    rs_scan_block(cnt, md->n, total);
+}
+// walk = 0: a record without a walk (the IMU chain's branch 1)
+__global__ void k_mark_head(const LioFeedDev* fd, LioMarkDev* md, int* pub_n, long long* hdr, long long max_scans, long long max_rows, int walk) {
+    pdl_wait();
+    if (threadIdx.x != 0) return;
+    const long long scan = fd->dyn.scan;
+    md->started = scan;   // before any byte of the slot changes (a reader checks it after its copy)
+    __threadfence();
+    marker_header(*md, scan, walk, pub_n, max_rows, hdr + (scan - 1) % max_scans * IMMESH_LIO_FEED_MARKER_HDR);
+    __threadfence();
+    pdl_trigger();
 }
 
 // ---- scan publishers.  immesh_lio_effect_cloud: a scan-order compaction of match_node >= 0 -- per-tile counts, the one-block
@@ -1275,7 +1315,52 @@ static int feed_stage(immesh_lio* h, const immesh_lio::FeedNext& nx, int kind, i
     IM_CUDA(cudaMemcpyAsync(&f.dev->dyn, &d, sizeof(FeedDyn), cudaMemcpyHostToDevice, h->stream));
     return IMMESH_OK;
 }
-static void launch_feed(immesh_lio* h, bool lio, bool pdl = false) {
+// The plane-map markers (f.mk_rows > 0), behind the scan's rows: walk = the scan ran a map update (not the IMU chain's branch 1).
+// The grids are fixed, so that the cost follows the pending count rather than the hash capacity the scratch covers.
+static void launch_markers(immesh_lio* h, bool walk, bool pdl) {
+    immesh_lio::Feed& f = h->feed;
+    cudaStream_t st = h->stream;
+    LioMarkDev* md = f.mk_dev;
+    if (walk) {
+        const size_t cap = f.mk_cap;
+        unsigned int* ku[2] = {f.mk_sort, f.mk_sort + cap};
+        unsigned int* vu[2] = {f.mk_sort + 2 * cap, f.mk_sort + 3 * cap};
+        const int* n_dev = &md->n;
+        const int tiles = (int)((cap + VG_TILE - 1) / VG_TILE);
+        const int g = h->n_sm * 4, gs = std::min(tiles, h->n_sm);
+        IM_LAUNCH_PDL(pdl, k_mark_begin, 1, 32, 0, st, (const int*)h->map.pub_n, md);
+        int cur = 0;
+        for (int half = 0; half < 2; ++half) {
+            IM_LAUNCH_PDL(pdl, k_pub_keys, g, PUB_THREADS, 0, st, h->map, 0, n_dev, half, half ? (const unsigned int*)vu[cur] : (const unsigned int*)nullptr,
+                          ku[cur ^ half], vu[cur ^ half]);
+            cur = rs_sort_passes(st, ku, vu, cur ^ half, (int)cap, 4, f.mk_hist, n_dev, gs);
+        }
+        int* slots = (int*)ku[0];   // the keys are spent: the sorted order is in vu[cur]
+        int* cnt = (int*)ku[1];
+        IM_LAUNCH_PDL(pdl, k_pub_count, g, PUB_THREADS, 0, st, h->map, 0, n_dev, (const unsigned int*)vu[cur], slots, cnt, md->misc + 1);
+        IM_LAUNCH_PDL(pdl, k_pub_scan, 1, 1024, 0, st, cnt, (const LioMarkDev*)md, md->misc);
+        IM_LAUNCH_PDL(pdl, k_mark_head, 1, 32, 0, st, (const LioFeedDev*)f.dev, md, h->map.pub_n, f.mk_hdr, f.max_scans, f.mk_rows, 1);
+        IM_LAUNCH_PDL(pdl, k_pub_emit, g, PUB_THREADS, 0, st, h->map, 0, (const int*)slots, (const int*)cnt, f.mk_ring, (const LioMarkDev*)md, f.mk_rows);
+    } else {
+        IM_LAUNCH_PDL(pdl, k_mark_head, 1, 32, 0, st, (const LioFeedDev*)f.dev, md, h->map.pub_n, f.mk_hdr, f.max_scans, f.mk_rows, 0);
+    }
+}
+// the markers' sort scratch covers the hash capacity; a growth of the hash (drained, its launch sequence dropped) enlarges it here,
+// before the next scan's launch sequence is queued or captured
+static int markers_fit(immesh_lio* h) {
+    immesh_lio::Feed& f = h->feed;
+    if (f.mk_rows == 0 || f.mk_cap >= h->cap) return IMMESH_OK;
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    h->graph.destroy();
+    f.mk_scratch = immesh::MemSet();
+    f.mk_sort = nullptr; f.mk_hist = nullptr; f.mk_cap = 0;
+    const size_t tiles = (h->cap + VG_TILE - 1) / VG_TILE;
+    IM_CUDA(f.mk_scratch.alloc(&f.mk_sort, 4 * h->cap));
+    IM_CUDA(f.mk_scratch.alloc(&f.mk_hist, 256 * tiles));
+    f.mk_cap = h->cap;
+    return IMMESH_OK;
+}
+static void launch_feed(immesh_lio* h, bool lio, bool walk, bool pdl = false) {
     immesh_lio::Feed& f = h->feed;
     cudaStream_t st = h->stream;
     const bool eff = lio && f.effect;
@@ -1290,12 +1375,20 @@ static void launch_feed(immesh_lio* h, bool lio, bool pdl = false) {
     if (lio && f.registered)
         IM_LAUNCH_PDL(pdl, k_reg_gather, h->n_sm * 8, SPUB_THREADS, 0, st, h->P, h->sb, (const LioCtrl*)h->d_ctrl, (const float*)nullptr, 0, 3, -1, f.skip, f.rows,
                       (const float*)nullptr, (const LioFeedDev*)f.dev, f.max_rows);
+    if (f.mk_rows) launch_markers(h, walk, pdl);
     IM_LAUNCH_PDL(pdl, k_feed_done, 1, 32, 0, st, (const LioFeedDev*)f.dev, f.d_done);
 }
 static int feed_commit(immesh_lio* h) {
     ++h->feed.queued;
     IM_CUDA(cudaEventRecord(h->feed.ev, h->stream));
     return IMMESH_OK;
+}
+static void markers_free(immesh_lio* h) {
+    immesh_lio::Feed& f = h->feed;
+    f.mk_mem = immesh::MemSet();
+    f.mk_scratch = immesh::MemSet();
+    f.mk_dev = nullptr; f.mk_hdr = nullptr; f.mk_ring = nullptr; f.mk_sort = nullptr; f.mk_hist = nullptr;
+    f.mk_rows = 0; f.mk_cap = 0;
 }
 static void feed_free(immesh_lio* h) {
     immesh_lio::Feed& f = h->feed;
@@ -1307,6 +1400,7 @@ static void feed_free(immesh_lio* h) {
     f.dev = nullptr; f.hdr = nullptr; f.states = nullptr; f.rows = nullptr; f.idx = nullptr; f.tiles = nullptr;
     f.h_dyn = nullptr; f.h_done = nullptr; f.d_done = nullptr;
     f.on = 0; f.queued = 0;
+    markers_free(h);
 }
 
 int immesh_lio_predict(immesh_lio_t* h, double dt, double cov_gyr, double cov_acc) {
@@ -1373,7 +1467,8 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
     const immesh_lio::FeedNext nx = h->feed_next;   // the front-end's or the IMU chain's scan, for this call only
     h->feed_next = immesh_lio::FeedNext();
-    const int grc = lio_growth_check(h, n);
+    int grc = lio_growth_check(h, n);
+    if (grc == IMMESH_OK) grc = markers_fit(h);
     if (grc) return grc;
     const int s = (++h->step_counter) & (IM_SLOTS - 1);
     if (h->slot_busy[s]) {
@@ -1399,7 +1494,8 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     bool queued = false;
     int lrc = IMMESH_OK;
     if (!timing) {
-        const unsigned sig = 1u | (h->feed.on ? 2u : 0u) | (h->lm_on ? 4u : 0u) | (h->win.ok ? 8u : 0u) | ((unsigned)h->P.max_iter << 8) | ((unsigned)h->P.shard_n << 16);
+        const unsigned sig = 1u | (h->feed.on ? 2u : 0u) | (h->lm_on ? 4u : 0u) | (h->win.ok ? 8u : 0u) | (h->feed.mk_rows ? 16u : 0u) | ((unsigned)h->P.max_iter << 8) |
+                             ((unsigned)h->P.shard_n << 16);
         // one GPU: every kernel after k_predict is a programmatic dependent launch (the sharded paths wait on peers and NCCL)
         const bool pdl = h->P.shard_n <= 1;
         queued = immesh::run_graphed_static(h->graph, sig, h->stream, [&] {
@@ -1407,7 +1503,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
             if (h->lm_on) launch_local_map(h, nullptr, 0, pdl);
             lrc = launch_estimate(h, pdl);
             launch_grow(h, 0, pdl);
-            if (h->feed.on) launch_feed(h, true, pdl);
+            if (h->feed.on) launch_feed(h, true, true, pdl);
         }) == cudaSuccess;
         if (!queued) h->use_graph = 0;   // not expected; keep working through direct launches
     }
@@ -1426,7 +1522,7 @@ static int lio_enqueue(immesh_lio_t* h, const float* body, int n, int on_device,
     IM_CUDA(cudaMemcpyAsync(h->h_out + s, &h->d_ctrl->out, sizeof(LioOut), cudaMemcpyDeviceToHost, h->stream));
     if (!queued) IM_CUDA(cudaEventRecord(h->ev[3], h->stream));
     if (h->feed.on) {
-        if (!queued) launch_feed(h, true);   // behind ev[3]: immesh_lio_last_timing stays the step's own
+        if (!queued) launch_feed(h, true, true);   // behind ev[3]: immesh_lio_last_timing stays the step's own
         IM_CUDA(cudaGetLastError());
         rc = feed_commit(h);
         if (rc) return rc;
@@ -1483,7 +1579,8 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     const immesh_lio::FeedNext nx = h->feed_next;   // the IMU chain's branch 2 (recorded with its header and state)
     h->feed_next = immesh_lio::FeedNext();
     if (n > h->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than max_scan_points");
-    const int grc = lio_growth_check(h, n);
+    int grc = lio_growth_check(h, n);
+    if (grc == IMMESH_OK) grc = markers_fit(h);
     if (grc) return grc;
     const int s = (++h->step_counter) & (IM_SLOTS - 1);
     if (h->slot_busy[s]) {
@@ -1502,7 +1599,7 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     if (h->feed.on) {
         rc = feed_stage(h, nx, IMMESH_FEED_KIND_IMU, 2, false);
         if (rc) return rc;
-        launch_feed(h, false);
+        launch_feed(h, false, true);   // voxel_map_init is followed by pubPlaneMap (:1899-1900)
     }
     IM_CUDA(cudaGetLastError());
     if (h->feed.on) {
@@ -1523,7 +1620,7 @@ int immesh_lio_feed_record_state(immesh_lio_t* h, int kind, int branch) {
     if (!h || !h->feed.on) return IMMESH_OK;
     const int rc = feed_stage(h, immesh_lio::FeedNext(), kind, branch, false);
     if (rc) return rc;
-    launch_feed(h, false);
+    launch_feed(h, false, false);   // the reference continues before pubPlaneMap
     IM_CUDA(cudaGetLastError());
     return feed_commit(h);
 }
@@ -1593,6 +1690,54 @@ int immesh_lio_feed(immesh_lio_t* h, int64_t since, int wait, int64_t* scans, do
     const int rc = feed_read(rings, since, fin, scans, states, cap_scans, rows, row_index, cap_rows, counts, copy, marks);
     if (rc == IMMESH_E_RANGE) return im_fail(rc, "immesh_lio_feed: scans of the range left the rings or were overwritten while they were read; read on from counts[2]");
     if (rc == IMMESH_E_CAPACITY) return im_fail(rc, "immesh_lio_feed: more scans or rows than the caps (counts holds them)");
+    return rc;
+}
+int immesh_lio_feed_markers_enable(immesh_lio_t* h, int64_t max_rows) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers_enable: the handle is sharded");
+    immesh_lio::Feed& f = h->feed;
+    if (!f.on) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers_enable: the scan feed is not enabled (immesh_lio_feed_enable)");
+    if (max_rows < 0 || max_rows > (1LL << 32)) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers_enable: max_rows must be in [0, 2^32] (0: off)");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    h->graph.destroy();   // the launch sequence changes
+    markers_free(h);
+    if (max_rows == 0) return IMMESH_OK;
+    auto fail = [&](cudaError_t e) { markers_free(h); cudaGetLastError(); return immesh::im_fail_cuda(e, __FILE__, __LINE__); };
+    cudaError_t e;
+    if ((e = f.mk_mem.alloc(&f.mk_dev, 1, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.mk_mem.alloc(&f.mk_hdr, (size_t)f.max_scans * IMMESH_LIO_FEED_MARKER_HDR, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.mk_mem.alloc(&f.mk_ring, (size_t)max_rows * IMMESH_PLANE_MARKER_COLS)) != cudaSuccess) return fail(e);
+    f.mk_rows = max_rows;
+    const int rc = markers_fit(h);
+    if (rc) { markers_free(h); return rc; }
+    return IMMESH_OK;
+}
+
+int immesh_lio_feed_markers(immesh_lio_t* h, int64_t since, int wait, int64_t* scans, int cap_scans, double* rows, int64_t cap_rows, int64_t* counts) {
+    if (!h || !counts || cap_scans < 0 || cap_rows < 0 || (cap_scans > 0 && !scans)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    for (int k = 0; k < 4; ++k) counts[k] = 0;
+    if (h->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers: the handle is sharded");
+    immesh_lio::Feed& f = h->feed;
+    if (!f.on || f.mk_rows == 0) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers: the plane-map markers are not enabled (immesh_lio_feed_markers_enable)");
+    if (since < 0 || since > f.queued) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers: since_scan must be in [0, newest queued scan]");
+    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued scan's record, nothing else
+    const long long fin = *(volatile long long*)f.h_done;
+    counts[2] = fin;
+    counts[3] = f.queued;
+    const FeedRings rings = marker_rings(f.max_scans, f.mk_rows, f.mk_hdr, f.mk_ring);
+    auto copy = [&](void* dst, const void* src, size_t bytes) {   // on the feed's stream, never the handle's
+        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
+        return IMMESH_OK;
+    };
+    auto marks = [&](long long* m) {
+        IM_CUDA(cudaMemcpyAsync(m, &f.mk_dev->started, 2 * sizeof(long long), cudaMemcpyDeviceToHost, f.stream));
+        IM_CUDA(cudaStreamSynchronize(f.stream));
+        return IMMESH_OK;
+    };
+    const int rc = feed_read(rings, since, fin, scans, nullptr, cap_scans, rows, nullptr, cap_rows, counts, copy, marks);
+    if (rc == IMMESH_E_RANGE)
+        return im_fail(rc, "immesh_lio_feed_markers: records of the range left the rings, were overwritten while they were read, or predate the enable; read on from counts[2]");
+    if (rc == IMMESH_E_CAPACITY) return im_fail(rc, "immesh_lio_feed_markers: more scans or rows than the caps (counts holds them)");
     return rc;
 }
 // queue a write of `bytes` bytes over a caller-provided device buffer on the localization stream (benchmark L2 flush)
@@ -1807,10 +1952,11 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     IM_CUDA(cudaMemsetAsync(misc, 0, 8 * sizeof(int), st));
     int cur = 0;
     for (int half = 0; half < 2; ++half) {
-        IM_LAUNCH(k_pub_keys, g, PUB_THREADS, 0, st, h->map, n, half, half ? (const unsigned int*)vu[cur] : (const unsigned int*)nullptr, ku[cur ^ half], vu[cur ^ half]);
+        IM_LAUNCH(k_pub_keys, g, PUB_THREADS, 0, st, h->map, n, (const int*)nullptr, half, half ? (const unsigned int*)vu[cur] : (const unsigned int*)nullptr,
+                  ku[cur ^ half], vu[cur ^ half]);
         cur = rs_sort_passes(st, ku, vu, cur ^ half, n, 4, hist);
     }
-    IM_LAUNCH(k_pub_count, g, PUB_THREADS, 0, st, h->map, n, (const unsigned int*)vu[cur], slots, cnt, misc + 1);
+    IM_LAUNCH(k_pub_count, g, PUB_THREADS, 0, st, h->map, n, (const int*)nullptr, (const unsigned int*)vu[cur], slots, cnt, misc + 1);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, cnt, n, misc);
     IM_CUDA(cudaGetLastError());
     IM_CUDA(cudaMemcpyAsync(h->h_ints + IM_HINT_PUB, misc, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1822,7 +1968,7 @@ int immesh_voxelmap_plane_markers(immesh_lio_t* h, double* rows, int cap, int* n
     // at least one row, so that k_pub_emit never gets a null pointer
     IM_CUDA(h->scratch.regrow(&h->d_pub_rows, &h->pub_rows_doubles, std::max<size_t>((size_t)total, 1) * IM_PUB_COLS, (size_t)1024 * IM_PUB_COLS));
     IM_CUDA(cudaMemsetAsync(h->map.pub_n, 0, sizeof(int), st));
-    IM_LAUNCH(k_pub_emit, g, PUB_THREADS, 0, st, h->map, n, (const int*)slots, (const int*)cnt, h->d_pub_rows);
+    IM_LAUNCH(k_pub_emit, g, PUB_THREADS, 0, st, h->map, n, (const int*)slots, (const int*)cnt, h->d_pub_rows, (const LioMarkDev*)nullptr, 0LL);
     IM_CUDA(cudaGetLastError());
     if (total > 0) IM_CUDA(cudaMemcpyAsync(rows, h->d_pub_rows, (size_t)total * IM_PUB_COLS * sizeof(double), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));

@@ -1,5 +1,6 @@
 // immesh_b200 -- the scan feed (immesh_lio_feed_enable / immesh_lio_feed): the device block its kernels share and the bookkeeping
-// of its two rings.  Header and state ring: scan k (numbered 1, 2, ... from the enable) in slot (k - 1) % max_scans.  Row ring: the
+// of its two rings, and those of its plane-map markers (immesh_lio_feed_markers_enable: a header ring beside the feed's, numbered
+// like it, and a ring of marker rows).  Header and state ring: scan k (numbered 1, 2, ... from the enable) in slot (k - 1) % max_scans.  Row ring: the
 // feed's rows are numbered in the order the scans append them, row r in slot r % max_rows; a scan's rows are its effect rows, then
 // its registered rows.  The bookkeeping is __host__ __device__ and the read is host code, so that the host emulation
 // (tests/lio_feed/emu_lio_feed.cpp) runs both as the product does.
@@ -32,6 +33,18 @@ struct LioFeedDev {
     int lost, pad_;        // the current scan's rows are not written
 };
 
+// the plane-map markers' block (immesh_lio_feed_markers_enable).  started and rows_total lead, in the order of LioFeedDev's, so that
+// the read takes both marks with one copy.
+struct LioMarkDev {
+    long long started;     // newest scan whose header slot is being written
+    long long rows_total;  // rows placed since the enable: the cursor of the marker ring
+    long long base;        // the current scan's first row
+    int lost;              // the current scan's rows are not written (and nothing is consumed)
+    int n;                 // roots the current scan walks: the pending count when its walk began
+    int misc[5];           // the current walk's rows in all, then the reference's four counters
+    int pad_[3];
+};
+
 // place a scan's ne effect and nr registered rows at the cursor, or lose them all when they exceed the ring; the header's row fields
 IM_HD void feed_append(LioFeedDev& f, long long ne, long long nr, long long max_rows, long long* hdr) {
     const long long start = f.rows_total;
@@ -46,18 +59,46 @@ IM_HD void feed_append(LioFeedDev& f, long long ne, long long nr, long long max_
     hdr[IMMESH_FEED_ROWS_LOST] = lost;
 }
 
+// place a scan's `need` marker rows at the cursor, or lose them when they exceed the ring; the header's row fields
+IM_HD void marker_append(LioMarkDev& m, long long need, long long max_rows, long long* hdr) {
+    const int lost = need > max_rows ? 1 : 0;
+    m.lost = lost;
+    m.base = m.rows_total;
+    hdr[IMMESH_MARKER_ROW_BEGIN] = m.rows_total;
+    if (!lost) m.rows_total += need;
+    hdr[IMMESH_MARKER_ROW_END] = m.rows_total;
+    hdr[IMMESH_MARKER_ROWS_NEEDED] = need;
+    hdr[IMMESH_MARKER_LOST] = lost;
+}
+
+// k_mark_head's work after it has marked the slot: the walk's rows placed (marker_append) or lost, the header written from the walk's
+// totals in m (n, misc), and -- only when the rows fit -- the pending count *pub_n reset, so that k_pub_emit publishes and lists
+// again just the roots that stay pending.  A lost scan leaves *pub_n and every flag as they are: nothing is consumed.  walk = 0: a
+// record without a walk (no rows, nothing walked).  Returns 1 when k_pub_emit is to publish.
+IM_HD int marker_header(LioMarkDev& m, long long scan, int walk, int* pub_n, long long max_rows, long long* h) {
+    marker_append(m, walk ? m.misc[0] : 0, max_rows, h);
+    h[IMMESH_MARKER_ROOTS_WALKED] = walk ? m.n : 0;
+    for (int k = 0; k < 4; ++k) h[IMMESH_MARKER_PLANES + k] = walk ? m.misc[1 + k] : 0;
+    h[IMMESH_MARKER_SCAN] = scan;
+    const int commit = walk && !m.lost ? 1 : 0;
+    if (commit) *pub_n = 0;
+    return commit;
+}
+
 // What a read of the scans (since, fin] can return, from their copied headers `hdr` (oldest first) and the device marks read after
 // the copy (`started`, `rows_total`): IMMESH_OK, or IMMESH_E_RANGE when a header slot or a row slot of the range may have been
-// overwritten.  *rows: the rows the range holds.
+// overwritten.  *rows: the rows the range holds.  hdr_len, row_begin, row_end: the header layout (the scan number is field 0).
 IM_HD int feed_check_range(long long since, long long fin, long long max_scans, long long max_rows, const long long* hdr, long long started,
-                              long long rows_total, long long* rows) {
+                              long long rows_total, long long* rows, int hdr_len = IMMESH_LIO_FEED_HDR, int row_begin = IMMESH_FEED_ROW_BEGIN,
+                              int row_end = IMMESH_FEED_ROW_END) {
+    static_assert(IMMESH_FEED_SCAN == 0 && IMMESH_MARKER_SCAN == 0, "the scan number leads every header");
     *rows = 0;
     const long long ns = fin - since;
     if (ns <= 0) return IMMESH_OK;
     if (ns > max_scans || started >= since + 1 + max_scans) return IMMESH_E_RANGE;
     for (long long i = 0; i < ns; ++i)
-        if (hdr[i * IMMESH_LIO_FEED_HDR + IMMESH_FEED_SCAN] != since + 1 + i) return IMMESH_E_RANGE;
-    const long long r0 = hdr[IMMESH_FEED_ROW_BEGIN], r1 = hdr[(ns - 1) * IMMESH_LIO_FEED_HDR + IMMESH_FEED_ROW_END];
+        if (hdr[i * hdr_len] != since + 1 + i) return IMMESH_E_RANGE;
+    const long long r0 = hdr[row_begin], r1 = hdr[(ns - 1) * hdr_len + row_end];
     *rows = r1 - r0;
     if (r1 > r0 && rows_total - max_rows > r0) return IMMESH_E_RANGE;
     return IMMESH_OK;
@@ -67,11 +108,23 @@ IM_HD int feed_check_range(long long since, long long fin, long long max_scans, 
 // returns 0 or an IMMESH_E_* code; `marks(m)` finishes the copies queued before and reads the device marks m = (started, rows_total).
 struct FeedRings {
     long long max_scans, max_rows;
-    const long long* hdr;   // [max_scans][IMMESH_LIO_FEED_HDR]
-    const double* states;   // [max_scans][IM_STATE_DOUBLES]
-    const void* rows;       // [max_rows] float4
-    const int* idx;         // [max_rows] or null (effect off)
+    const long long* hdr;   // [max_scans][hdr_len]
+    const double* states;   // [max_scans][IM_STATE_DOUBLES], or null (the marker records)
+    const void* rows;       // [max_rows] rows of row_bytes
+    const int* idx;         // [max_rows] or null (effect off, the marker records)
+    // the scan feed's header and rows unless set: the marker records' are IMMESH_LIO_FEED_MARKER_HDR and IMMESH_PLANE_MARKER_COLS doubles
+    int hdr_len = IMMESH_LIO_FEED_HDR, row_begin = IMMESH_FEED_ROW_BEGIN, row_end = IMMESH_FEED_ROW_END;
+    size_t row_bytes = 4 * sizeof(float);
 };
+// the marker records' rings in the read's terms (immesh_lio_feed_markers)
+inline FeedRings marker_rings(long long max_scans, long long max_rows, const long long* hdr, const double* ring) {
+    FeedRings r{max_scans, max_rows, hdr, nullptr, ring, nullptr};
+    r.hdr_len = IMMESH_LIO_FEED_MARKER_HDR;
+    r.row_begin = IMMESH_MARKER_ROW_BEGIN;
+    r.row_end = IMMESH_MARKER_ROW_END;
+    r.row_bytes = IMMESH_PLANE_MARKER_COLS * sizeof(double);
+    return r;
+}
 // entries [first, first + count) of a ring of `len` entries of `elem` bytes: the one or two contiguous copies
 template <class Copy>
 inline int feed_copy_ring(Copy& copy, void* dst, const void* ring, size_t elem, long long first, long long count, long long len) {
@@ -83,33 +136,35 @@ inline int feed_copy_ring(Copy& copy, void* dst, const void* ring, size_t elem, 
 // The scans (since, fin] -- fin the newest finished scan -- into the caller's buffers, as immesh_lio_feed documents: counts[0..1] are
 // set once the range is known; IMMESH_E_RANGE when a slot of the range may have been overwritten, before or during the copies;
 // IMMESH_E_CAPACITY with the counts and nothing written; cap_scans = 0 a count query.
+// The marker records (immesh_lio_feed_markers) are read by the same code with their layout in `r`, states and row_index null.
 template <class Copy, class Marks>
-inline int feed_read(const FeedRings& r, long long since, long long fin, int64_t* scans, double* states, int cap_scans, float* rows, int32_t* row_index,
+inline int feed_read(const FeedRings& r, long long since, long long fin, int64_t* scans, double* states, int cap_scans, void* rows, int32_t* row_index,
                      int64_t cap_rows, int64_t* counts, Copy&& copy, Marks&& marks) {
     counts[0] = counts[1] = 0;
     if (since >= fin) return IMMESH_OK;
     const long long k0 = since + 1, ns = fin - since;
     if (ns > r.max_scans) return IMMESH_E_RANGE;
-    std::vector<long long> hb((size_t)ns * IMMESH_LIO_FEED_HDR);
+    std::vector<long long> hb((size_t)ns * r.hdr_len);
     long long m[2];
-    int rc = feed_copy_ring(copy, hb.data(), r.hdr, IMMESH_LIO_FEED_HDR * sizeof(long long), (k0 - 1) % r.max_scans, ns, r.max_scans);
+    int rc = feed_copy_ring(copy, hb.data(), r.hdr, r.hdr_len * sizeof(long long), (k0 - 1) % r.max_scans, ns, r.max_scans);
     if (rc == 0) rc = marks(m);
     if (rc) return rc;
     long long nrows = 0;
-    if (feed_check_range(since, fin, r.max_scans, r.max_rows, hb.data(), m[0], m[1], &nrows) != IMMESH_OK) return IMMESH_E_RANGE;
+    auto check = [&] { return feed_check_range(since, fin, r.max_scans, r.max_rows, hb.data(), m[0], m[1], &nrows, r.hdr_len, r.row_begin, r.row_end); };
+    if (check() != IMMESH_OK) return IMMESH_E_RANGE;
     counts[0] = ns;
     counts[1] = nrows;
     if (cap_scans == 0) return IMMESH_OK;   // a count query
     if (ns > cap_scans || (rows && nrows > cap_rows)) return IMMESH_E_CAPACITY;
-    const long long r0 = hb[IMMESH_FEED_ROW_BEGIN];
-    if (states) rc = feed_copy_ring(copy, states, r.states, IM_STATE_DOUBLES * sizeof(double), (k0 - 1) % r.max_scans, ns, r.max_scans);
+    const long long r0 = hb[r.row_begin];
+    if (states && r.states) rc = feed_copy_ring(copy, states, r.states, IM_STATE_DOUBLES * sizeof(double), (k0 - 1) % r.max_scans, ns, r.max_scans);
     if (rc == 0 && rows && nrows > 0) {
-        rc = feed_copy_ring(copy, rows, r.rows, 4 * sizeof(float), r0 % r.max_rows, nrows, r.max_rows);
+        rc = feed_copy_ring(copy, rows, r.rows, r.row_bytes, r0 % r.max_rows, nrows, r.max_rows);
         if (rc == 0 && row_index && r.idx) rc = feed_copy_ring(copy, row_index, r.idx, sizeof(int), r0 % r.max_rows, nrows, r.max_rows);
     }
     if (rc == 0) rc = marks(m);   // the copies are done: nothing they read may have been overwritten meanwhile
     if (rc) return rc;
-    if (feed_check_range(since, fin, r.max_scans, r.max_rows, hb.data(), m[0], m[1], &nrows) != IMMESH_OK) return IMMESH_E_RANGE;
+    if (check() != IMMESH_OK) return IMMESH_E_RANGE;
     std::memcpy(scans, hb.data(), hb.size() * sizeof(long long));
     if (rows && row_index) {   // registered rows carry no scan index
         for (long long i = 0; i < ns; ++i) {

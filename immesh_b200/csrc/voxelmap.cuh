@@ -694,7 +694,12 @@ IM_HDN inline void update_octo_tree(const VoxelMapDev& m, const LioParams& P, in
 // given) | min_eig | trace | alpha.  path: the dump's encoding (child l -> path * 9 + l + 1); id: the node record index;
 // trace: (pv00 + pv11) + pv22, the order of Eigen's 3-vector sum.  rows == nullptr: nothing written, no flag cleared (a count).
 // counts (may be null) += plane, sub-plane, sub-sub-plane and update counts of the reference's two log lines.
+// The walk's k-th row goes to row first + k of rows[], or of a ring of `ring` rows (slot (first + k) % ring) when ring > 0.
 #define IM_PUB_COLS 16
+IM_HD double* plane_pub_at(double* rows, long long first, int k, long long ring) {
+    const long long r = first + k;
+    return rows + (size_t)(ring > 0 ? r % ring : r) * IM_PUB_COLS;
+}
 IM_HD void plane_pub_row(const VoxelMapDev& m, int nd, long long kx, long long ky, long long kz, long long path, int layer, bool scaled, double* row) {
     const PlaneRec& pl = m.planes[nd];
     const PubRec& q = m.pub[nd];
@@ -706,20 +711,20 @@ IM_HD void plane_pub_row(const VoxelMapDev& m, int nd, long long kx, long long k
     row[14] = (pl.pv[0] + pl.pv[6]) + pl.pv[11];
     row[15] = scaled ? (pl.is_plane ? 1.0 : 0.0) : 1.0;
 }
-IM_HD int plane_pub_root(const VoxelMapDev& m, int root, unsigned long long key, double* rows, int* counts) {
+IM_HD int plane_pub_root(const VoxelMapDev& m, int root, unsigned long long key, double* rows, int* counts, long long first = 0, long long ring = 0) {
     long long kx, ky, kz;
     unpack_key(key, &kx, &ky, &kz);
     int c[4] = {0, 0, 0, 0};
     int nrow = 0;
     if (m.pub[root].updated) {
-        if (rows) { plane_pub_row(m, root, kx, ky, kz, 0, 0, true, rows); m.pub[root].updated = 0; }
+        if (rows) { plane_pub_row(m, root, kx, ky, kz, 0, 0, true, plane_pub_at(rows, first, 0, ring)); m.pub[root].updated = 0; }
         nrow = 1; c[0] = 1; c[3] = 1;
     } else {
         for (int i = 0; i < 8; ++i) {
             const int ch = m.nodes[root].children[i];
             if (ch < 0) continue;
             if (m.pub[ch].updated) {
-                if (rows) { plane_pub_row(m, ch, kx, ky, kz, i + 1, 1, true, rows + (size_t)nrow * IM_PUB_COLS); m.pub[ch].updated = 0; }
+                if (rows) { plane_pub_row(m, ch, kx, ky, kz, i + 1, 1, true, plane_pub_at(rows, first, nrow, ring)); m.pub[ch].updated = 0; }
                 ++nrow; ++c[1]; ++c[3];
                 continue;
             }
@@ -727,7 +732,10 @@ IM_HD int plane_pub_root(const VoxelMapDev& m, int root, unsigned long long key,
                 const int g = m.nodes[ch].children[j];
                 if (g < 0 || m.nodes[g].octo_state != 0 || !m.pub[g].updated) continue;
                 if (m.planes[g].is_plane) {
-                    if (rows) { plane_pub_row(m, g, kx, ky, kz, (long long)(i + 1) * 9 + (j + 1), 2, false, rows + (size_t)nrow * IM_PUB_COLS); m.pub[g].updated = 0; }
+                    if (rows) {
+                        plane_pub_row(m, g, kx, ky, kz, (long long)(i + 1) * 9 + (j + 1), 2, false, plane_pub_at(rows, first, nrow, ring));
+                        m.pub[g].updated = 0;
+                    }
                     ++nrow; ++c[3];
                 }
                 ++c[2];
@@ -741,11 +749,12 @@ IM_HD int plane_pub_root(const VoxelMapDev& m, int root, unsigned long long key,
 // Publish the root listed at `slot` into rows[] (room for what plane_pub_root counted) and settle its mark: the root stays pending
 // while the same walk over what is left would publish something (a child held back by the root's own flag, a grandchild behind a
 // child that was published), and leaves the list otherwise -- flags that can never be published (non-planar or split layer-2 nodes,
-// layers >= 3) do not keep it there; the next fit under it marks it again.  Returns 1 when the root stays pending.
-IM_HD int plane_pub_commit(const VoxelMapDev& m, int slot, double* rows) {
+// layers >= 3) do not keep it there; the next fit under it marks it again.  Returns 1 when the root stays pending.  first, ring: as
+// in plane_pub_root.
+IM_HD int plane_pub_commit(const VoxelMapDev& m, int slot, double* rows, long long first = 0, long long ring = 0) {
     const int root = m.root_node[slot];
     if (root < 0) { m.pub_mark[slot] = 0; return 0; }
-    plane_pub_root(m, root, m.keys[slot], rows, nullptr);
+    plane_pub_root(m, root, m.keys[slot], rows, nullptr, first, ring);
     const int again = plane_pub_root(m, root, m.keys[slot], nullptr, nullptr) > 0 ? 1 : 0;
     if (!again) m.pub_mark[slot] = 0;
     return again;

@@ -313,6 +313,42 @@ int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* cfg /*
 int immesh_lio_feed(immesh_lio_t* h, int64_t since_scan, int wait, int64_t* scans /*[cap_scans][12]*/, double* states /*[cap_scans][348] or NULL*/,
                     int cap_scans, float* rows /*[cap_rows][4] or NULL*/, int32_t* row_index /*[cap_rows] or NULL*/, int64_t cap_rows,
                     int64_t* counts /*[4]*/);
+/* Plane-map markers in the scan feed: pubPlaneMap(m_feat_map, voxel_pub, state.pos_end), which the reference calls after
+ * map_incremental_grow and after voxel_map_init when voxel/pub_plane_en is set (src/voxel_mapping.cpp:1975-1976, :1899-1900),
+ * recorded on the device for each scan the feed records, behind the scan's map update and before the scan counts as finished.
+ * immesh_lio_feed_markers_enable(h, max_rows): max_rows > 0 turns the recording on with a ring of max_rows rows of
+ *   IMMESH_PLANE_MARKER_COLS doubles; 0 turns it off and frees the ring.  Drains h and drops its captured launch sequence.  Needs the
+ *   feed on; every immesh_lio_feed_enable call (NULL included) turns the markers off.  max_rows outside [0, 2^32], the feed off,
+ *   or a sharded handle: IMMESH_E_INVALID.  The recording keeps 16 bytes per root slot of device scratch for the key sort.
+ * A scan's record equals what immesh_voxelmap_plane_markers would return if it were called right after that scan: the same rows in
+ *   the same order, the same counters and roots walked, the same flags consumed and children held back.  The IMU chain's branch 2
+ *   (voxel_map_init) walks as well; branch 1 records no rows and walks nothing.  The blocking call stays allowed: the rows it returns
+ *   are consumed and never appear in the feed.  Staged calls record nothing, so the first message after immesh_voxelmap_build comes
+ *   from one blocking call before the steps are queued.
+ *   header (IMMESH_LIO_FEED_MARKER_HDR int64): IMMESH_MARKER_SCAN (the feed's scan number); ROW_BEGIN, ROW_END: the scan's rows,
+ *     numbered over the marker ring; ROWS_NEEDED: the rows the walk counted; LOST; ROOTS_WALKED; PLANES, SUB_PLANES, SUB_SUB_PLANES,
+ *     UPDATES: the reference's counters (immesh_voxelmap_plane_markers' counts[0..3]).
+ *   A scan whose rows exceed max_rows sets LOST, writes no rows and consumes nothing: its roots stay pending and are published with a
+ *   later scan, as if the node had skipped pubPlaneMap on that scan.  Size the ring from ROWS_NEEDED.  A loss never changes the
+ *   state, the map or the mesh.
+ * immesh_lio_feed_markers(h, since_scan, wait, ...): the marker records of the scans (since_scan, newest finished], oldest first, and
+ *   their rows concatenated (rows may be NULL); since_scan, wait, counts, the count query, IMMESH_E_CAPACITY and IMMESH_E_RANGE as in
+ *   immesh_lio_feed.  Scans queued before the markers were enabled have no record: a range that holds one gives IMMESH_E_RANGE.
+ *   Never synchronises h's stream.  The markers off, the feed off, or a sharded handle: IMMESH_E_INVALID. */
+#define IMMESH_LIO_FEED_MARKER_HDR 10
+#define IMMESH_MARKER_SCAN 0
+#define IMMESH_MARKER_ROW_BEGIN 1
+#define IMMESH_MARKER_ROW_END 2
+#define IMMESH_MARKER_ROWS_NEEDED 3
+#define IMMESH_MARKER_LOST 4
+#define IMMESH_MARKER_ROOTS_WALKED 5
+#define IMMESH_MARKER_PLANES 6
+#define IMMESH_MARKER_SUB_PLANES 7
+#define IMMESH_MARKER_SUB_SUB_PLANES 8
+#define IMMESH_MARKER_UPDATES 9
+int immesh_lio_feed_markers_enable(immesh_lio_t* h, int64_t max_rows /* 0: off */);
+int immesh_lio_feed_markers(immesh_lio_t* h, int64_t since_scan, int wait, int64_t* scans /*[cap_scans][10]*/, int cap_scans,
+                            double* rows /*[cap_rows][16] or NULL*/, int64_t cap_rows, int64_t* counts /*[4]*/);
 /* Host-side formatters of a recorded state (no device work).
  * immesh_odometry_pose: out = pos_end, then the quaternion x y z w that publish_odometry, publish_path and publish_mavros send:
  *   (roll, pitch, yaw) = RotMtoEuler(rot_end) (include/so3_math.h: sy = sqrt(r00^2 + r10^2); sy >= 1e-6: roll = atan2(r21, r22),
