@@ -70,6 +70,17 @@ MARKER_HDR = 10   # IMMESH_LIO_FEED_MARKER_HDR: the header columns of a scan's p
 MARKER_HDR_KEYS = ("scan", "row_begin", "row_end", "rows_needed", "lost", "roots_walked", "plane", "sub_plane", "sub_sub_plane", "update")
 
 
+class _MeshFeedCfg(C.Structure):
+    _fields_ = [("max_frames", C.c_int64), ("max_rows", C.c_int64), ("max_images", C.c_int64), ("depth", C.c_int), ("pad", C.c_int)]
+
+
+MESH_FEED_HDR = 22    # IMMESH_MESH_FEED_HDR: the header columns of a recorded mesh frame, in this order
+MESH_FEED_HDR_KEYS = ("frame", "kind", "n_points", "step", "n_vertices", "n_triangles", "new_vertices", "voxels_meshed", "n_add", "n_remove", "n_voxels",
+                      "n_activated", "err", "has_rotation", "t_begin_ns", "t_end_ns", "row_begin", "row_end", "rows_lost", "rf", "img_begin", "img_end")
+MESH_FEED_POSE = 36   # IMMESH_MESH_FEED_POSE: frame pose, reinforcement camera, view camera; each a row-major R then t
+MESH_FEED_KINDS = ("push", "push_dev", "from_lio", "from_lio_async", "reconstruct", "batched", "reconstruct_batched")   # IMMESH_MFEED_KIND_*
+
+
 class FeedLost(RuntimeError):
     """immesh_lio_feed returned IMMESH_E_RANGE: scans of the range left the rings.  Read on from newest_finished."""
 
@@ -208,6 +219,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_changes_enable", [vp, C.c_int64, C.c_int]),
         ("immesh_mesh_changes", [vp, C.c_int64, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_int32), C.c_int64, fp, C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud", [vp, vp, vp, C.c_int, C.c_int, C.c_double, ip]),
+        ("immesh_mesh_feed_enable", [vp, C.POINTER(_MeshFeedCfg)]),
+        ("immesh_mesh_feed", [vp, C.c_int64, C.c_int, C.POINTER(C.c_int64), dp, C.c_int, fp, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_feed_images", [vp, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.c_int, C.POINTER(C.c_uint8), fp, C.POINTER(C.c_int64)]),
         ("immesh_mesh_push_frame_batched", [vp, vp, C.c_int64, C.c_int, dp, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_reconstruct_from_pointcloud_batched", [vp, vp, vp, C.c_int64, C.c_int, C.c_double, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
         ("immesh_mesh_smooth_all", [vp, C.c_double, C.c_int, dp]),
@@ -845,9 +859,11 @@ class Mesh:
         _check(self.lib, self.lib.immesh_mesh_view_enable(self._h, K.ctypes.data_as(C.POINTER(C.c_double)), width, height, z_near, z_far, win, C.byref(st)),
                "mesh_view_enable")
         self._vw_shape = (height, width)
+        self._feed_img = None   # every view_enable turns the frame feed's images off
 
     def view_disable(self):
         _check(self.lib, self.lib.immesh_mesh_view_enable(self._h, None, 0, 0, 0.0, 0.0, 0, None), "mesh_view_enable")
+        self._feed_img = None
 
     def view_pose(self, cam_R=None, cam_t=None, follow=False):
         """The queued view's camera from the next frame on: None the sensor-bound pose; (cam_R, cam_t) a fixed camera; with follow, the
@@ -915,6 +931,80 @@ class Mesh:
             _check(self.lib, self.lib.immesh_mesh_changes(self._h, since, fr.ctypes.data_as(C.POINTER(C.c_int64)), len(fr), rows.ctypes.data_as(C.POINTER(C.c_int32)),
                                                           len(rows), v.ctypes.data_as(C.POINTER(C.c_float)), len(v), cp), "mesh_changes")
         return dict(frames=fr, rows=rows, vertices=v, newest=int(counts[3]))
+
+    def feed_enable(self, max_frames=1024, max_rows=1 << 22, max_images=0, depth=False):
+        """Record every later frame's header, poses, reinforced points and (max_images > 0, the queued view on) viewer image on the
+        device (immesh_mesh_feed_enable).  The image ring is sized for the view as it is now; view_enable turns the images off."""
+        c = _MeshFeedCfg(int(max_frames), int(max_rows), int(max_images), 1 if depth else 0, 0)
+        _check(self.lib, self.lib.immesh_mesh_feed_enable(self._h, C.byref(c)), "mesh_feed_enable")
+        self._feed_img = (getattr(self, "_vw_shape", None), bool(depth)) if max_images > 0 else None
+
+    def feed_disable(self):
+        _check(self.lib, self.lib.immesh_mesh_feed_enable(self._h, None), "mesh_feed_enable")
+        self._feed_img = None
+
+    def _feed_read(self, call, alloc, what):
+        """count query, then the read; frames may finish between the two"""
+        counts = np.zeros(4, dtype=np.int64)
+        cp = counts.ctypes.data_as(C.POINTER(C.c_int64))
+        for first in (True,) + (False,) * 8:
+            rc = call(None, counts, cp, first)
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, what)
+            bufs = alloc(int(counts[0]), int(counts[1]))
+            if counts[0] == 0:
+                return bufs, counts
+            rc = call(bufs, counts, cp, False)
+            if rc == -3:
+                continue
+            if rc == -5:
+                raise FeedLost(self.lib.immesh_last_error().decode(), int(counts[2]))
+            _check(self.lib, rc, what)
+            return bufs, counts
+        raise RuntimeError(f"{what}: the frames kept finishing faster than they were read")
+
+    def feed(self, since: int, wait: bool = False):
+        """The frames (since, newest finished] of the frame feed: dict(frames=int64[m, MESH_FEED_HDR] (MESH_FEED_HDR_KEYS),
+        poses=float64[m, 3, 12] (frame pose, reinforcement camera, view camera; R row-major then t), points=float32[r, 3],
+        pixels=int32[r], newest_finished, newest_queued).  wait=False never blocks on unfinished work.  Raises FeedLost when frames of
+        the range predate the enable or left the rings."""
+        i64, f32, i32, dp = C.POINTER(C.c_int64), C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_double)
+
+        def alloc(nf, nr):
+            return (np.zeros((max(nf, 1), MESH_FEED_HDR), np.int64), np.zeros((max(nf, 1), MESH_FEED_POSE)), np.zeros((max(nr, 1), 3), np.float32),
+                    np.zeros(max(nr, 1), np.int32), nf, nr)
+
+        def call(b, counts, cp, first):
+            if b is None:
+                return self.lib.immesh_mesh_feed(self._h, since, 1 if (wait and first) else 0, None, None, 0, None, None, 0, cp)
+            return self.lib.immesh_mesh_feed(self._h, since, 0, b[0].ctypes.data_as(i64), b[1].ctypes.data_as(dp), b[4], b[2].ctypes.data_as(f32),
+                                             b[3].ctypes.data_as(i32), b[5], cp)
+        b, counts = self._feed_read(call, alloc, "mesh_feed")
+        nf, nr = int(counts[0]), int(counts[1])
+        return dict(frames=b[0][:nf], poses=b[1][:nf].reshape(nf, 3, 12), points=b[2][:nr], pixels=b[3][:nr], newest_finished=int(counts[2]),
+                    newest_queued=int(counts[3]))
+
+    def feed_images(self, since: int, wait: bool = False):
+        """The frames (since, newest finished] and the view images they hold: dict(frames=int64[m, MESH_FEED_HDR], rgba=uint8[k, h, w, 4],
+        depth=float32[k, h, w] (feed enabled with depth) or None, newest_finished, newest_queued).  Raises FeedLost when an image of the
+        range left the ring, even while its header is held."""
+        (hh, ww), with_depth = getattr(self, "_feed_img", None) or ((1, 1), False)
+        i64 = C.POINTER(C.c_int64)
+
+        def alloc(nf, ni):
+            return (np.zeros((max(nf, 1), MESH_FEED_HDR), np.int64), np.zeros((max(ni, 1), hh, ww, 4), np.uint8),
+                    np.zeros((max(ni, 1), hh, ww), np.float32) if with_depth else None, nf, ni)
+
+        def call(b, counts, cp, first):
+            if b is None:
+                return self.lib.immesh_mesh_feed_images(self._h, since, 1 if (wait and first) else 0, None, 0, None, None, cp)
+            return self.lib.immesh_mesh_feed_images(self._h, since, 0, b[0].ctypes.data_as(i64), b[3], b[1].ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                    b[2].ctypes.data_as(C.POINTER(C.c_float)) if b[2] is not None else None, cp)
+        b, counts = self._feed_read(call, alloc, "mesh_feed_images")
+        nf, ni = int(counts[0]), int(counts[1])
+        return dict(frames=b[0][:nf], rgba=b[1][:ni], depth=b[2][:ni] if b[2] is not None else None, newest_finished=int(counts[2]),
+                    newest_queued=int(counts[3]))
 
     def smooth_all(self, smooth_factor=0.1, knn=20):
         """smooth_all_pts: returns the smoothed positions float64[nv,3] (and stores them as the vertices' smoothed positions)."""

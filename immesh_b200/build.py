@@ -201,6 +201,15 @@ def build_lio_feed_markers(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "lio_feed", "emu_lio_feed_markers.cpp"), EMU_LIO_FEED_MARKERS, force)
 
 
+EMU_MESH_FEED = os.path.join(_ROOT, "tests", "mesh_feed", "libimmesh_emu_mesh_feed.so")
+
+
+def build_mesh_feed(force=False):
+    """tests/mesh_feed: the frame feed's ring bookkeeping (immesh_b200/csrc/mesh_feed.cuh) and the shared read (feed_read) with the
+    device kernels' order restated on the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "mesh_feed", "emu_mesh_feed.cpp"), EMU_MESH_FEED, force)
+
+
 RS_CHECK = os.path.join(_ROOT, "tests", "radix_sort", "librs_check.so")
 
 
@@ -272,6 +281,7 @@ def build_all(force=False):
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)
+    build_mesh_feed(force)
     build_rs_check(force)
     build_eval(force)
     build_local_map(force)

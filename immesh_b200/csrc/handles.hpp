@@ -6,6 +6,7 @@
 #include "lio_core.cuh"
 #include "lio_feed.cuh"
 #include "mesh_changes.cuh"
+#include "mesh_feed.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
 #include "view_overlay.cuh"
@@ -260,6 +261,28 @@ struct immesh_mesh {
         int* hist = nullptr;
         immesh::MemSet dev;               // every buffer of the feed, freed by disable / destroy (not counted)
     } chg;
+    // frame feed (immesh_mesh_feed_enable, mesh_feed.cuh).  Every buffer here is freed only by immesh_mesh_feed_enable and
+    // immesh_mesh_destroy, after the stream is drained and the graph dropped; the image ring also by immesh_mesh_view_enable.
+    struct Feed {
+        int on = 0, depth = 0;
+        long long max_frames = 0, max_rows = 0, max_images = 0;   // max_images = 0: no image recording
+        long long npx = 0;                // pixels of one image (the view's w * h at the enable)
+        long long enable_frame = 0;       // frame_counter at the enable: the frames after it are recorded
+        long long queued = 0;             // newest frame recorded
+        immesh::MeshFeedDev* dev = nullptr;
+        long long* hdr = nullptr;         // [max_frames][IMMESH_MESH_FEED_HDR]
+        double* poses = nullptr;          // [max_frames][IMMESH_MESH_FEED_POSE]
+        float* pts = nullptr;             // [max_rows][3]
+        int* pix = nullptr;               // [max_rows]
+        uchar4* rgba = nullptr;           // [max_images][npx]
+        float* depth_ring = nullptr;      // [max_images][npx] (depth = 1)
+        immesh::MeshFeedDyn* h_dyn = nullptr;   // pinned, IM_SLOTS slots: the per-frame inputs
+        long long* h_done = nullptr;      // pinned, written by k_mfeed_done: the newest frame whose record is complete
+        long long* d_done = nullptr;      // its device address
+        cudaStream_t stream = nullptr;    // the reader's copies (never the handle's stream)
+        cudaEvent_t ev = nullptr;         // recorded behind the newest frame's record
+        immesh::MemSet dev_mem, img_mem, pinned{immesh::MemSet::Pinned};
+    } feed;
 };
 
 // The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate

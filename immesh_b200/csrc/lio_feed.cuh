@@ -4,6 +4,9 @@
 // feed's rows are numbered in the order the scans append them, row r in slot r % max_rows; a scan's rows are its effect rows, then
 // its registered rows.  The bookkeeping is __host__ __device__ and the read is host code, so that the host emulation
 // (tests/lio_feed/emu_lio_feed.cpp) runs both as the product does.
+// The read (feed_check_range, FeedRings, feed_read) is not specific to scans: it serves any ring of numbered headers with a fixed
+// record of doubles beside each and a row ring of one or two per-row arrays -- the mesh frame feed (mesh_feed.cuh) reads its
+// points and its images through it too.
 #pragma once
 #include <cstdint>
 #include <cstring>
@@ -109,12 +112,17 @@ IM_HD int feed_check_range(long long since, long long fin, long long max_scans, 
 struct FeedRings {
     long long max_scans, max_rows;
     const long long* hdr;   // [max_scans][hdr_len]
-    const double* states;   // [max_scans][IM_STATE_DOUBLES], or null (the marker records)
+    const double* states;   // [max_scans][state_doubles], or null (the marker records)
     const void* rows;       // [max_rows] rows of row_bytes
-    const int* idx;         // [max_rows] or null (effect off, the marker records)
+    const void* idx;        // [max_rows] second per-row array of idx_bytes per row, or null (effect off, the marker records)
     // the scan feed's header and rows unless set: the marker records' are IMMESH_LIO_FEED_MARKER_HDR and IMMESH_PLANE_MARKER_COLS doubles
     int hdr_len = IMMESH_LIO_FEED_HDR, row_begin = IMMESH_FEED_ROW_BEGIN, row_end = IMMESH_FEED_ROW_END;
     size_t row_bytes = 4 * sizeof(float);
+    int state_doubles = IM_STATE_DOUBLES;
+    size_t idx_bytes = sizeof(int);
+    // the scan feed's row_index fix-up: the rows of each record from header field fill_col (idx set) or row_begin (idx null) to
+    // row_end carry no index and read -1 (int32).  -1: no fix-up (the second array is copied as it is)
+    int fill_col = IMMESH_FEED_ROW_EFFECT_END;
 };
 // the marker records' rings in the read's terms (immesh_lio_feed_markers)
 inline FeedRings marker_rings(long long max_scans, long long max_rows, const long long* hdr, const double* ring) {
@@ -123,6 +131,7 @@ inline FeedRings marker_rings(long long max_scans, long long max_rows, const lon
     r.row_begin = IMMESH_MARKER_ROW_BEGIN;
     r.row_end = IMMESH_MARKER_ROW_END;
     r.row_bytes = IMMESH_PLANE_MARKER_COLS * sizeof(double);
+    r.fill_col = -1;
     return r;
 }
 // entries [first, first + count) of a ring of `len` entries of `elem` bytes: the one or two contiguous copies
@@ -137,8 +146,9 @@ inline int feed_copy_ring(Copy& copy, void* dst, const void* ring, size_t elem, 
 // set once the range is known; IMMESH_E_RANGE when a slot of the range may have been overwritten, before or during the copies;
 // IMMESH_E_CAPACITY with the counts and nothing written; cap_scans = 0 a count query.
 // The marker records (immesh_lio_feed_markers) are read by the same code with their layout in `r`, states and row_index null.
+// The rings of any other layout are described by `r`: states the records of r.state_doubles, row_index the second per-row array.
 template <class Copy, class Marks>
-inline int feed_read(const FeedRings& r, long long since, long long fin, int64_t* scans, double* states, int cap_scans, void* rows, int32_t* row_index,
+inline int feed_read(const FeedRings& r, long long since, long long fin, int64_t* scans, double* states, int cap_scans, void* rows, void* row_index,
                      int64_t cap_rows, int64_t* counts, Copy&& copy, Marks&& marks) {
     counts[0] = counts[1] = 0;
     if (since >= fin) return IMMESH_OK;
@@ -157,20 +167,21 @@ inline int feed_read(const FeedRings& r, long long since, long long fin, int64_t
     if (cap_scans == 0) return IMMESH_OK;   // a count query
     if (ns > cap_scans || (rows && nrows > cap_rows)) return IMMESH_E_CAPACITY;
     const long long r0 = hb[r.row_begin];
-    if (states && r.states) rc = feed_copy_ring(copy, states, r.states, IM_STATE_DOUBLES * sizeof(double), (k0 - 1) % r.max_scans, ns, r.max_scans);
+    if (states && r.states) rc = feed_copy_ring(copy, states, r.states, (size_t)r.state_doubles * sizeof(double), (k0 - 1) % r.max_scans, ns, r.max_scans);
     if (rc == 0 && rows && nrows > 0) {
         rc = feed_copy_ring(copy, rows, r.rows, r.row_bytes, r0 % r.max_rows, nrows, r.max_rows);
-        if (rc == 0 && row_index && r.idx) rc = feed_copy_ring(copy, row_index, r.idx, sizeof(int), r0 % r.max_rows, nrows, r.max_rows);
+        if (rc == 0 && row_index && r.idx) rc = feed_copy_ring(copy, row_index, r.idx, r.idx_bytes, r0 % r.max_rows, nrows, r.max_rows);
     }
     if (rc == 0) rc = marks(m);   // the copies are done: nothing they read may have been overwritten meanwhile
     if (rc) return rc;
     if (check() != IMMESH_OK) return IMMESH_E_RANGE;
     std::memcpy(scans, hb.data(), hb.size() * sizeof(long long));
-    if (rows && row_index) {   // registered rows carry no scan index
+    if (rows && row_index && r.fill_col >= 0) {   // registered rows carry no scan index
+        int32_t* ri = (int32_t*)row_index;
         for (long long i = 0; i < ns; ++i) {
-            const long long* hd = hb.data() + (size_t)i * IMMESH_LIO_FEED_HDR;
-            const long long a = r.idx ? hd[IMMESH_FEED_ROW_EFFECT_END] : hd[IMMESH_FEED_ROW_BEGIN];
-            for (long long j = a; j < hd[IMMESH_FEED_ROW_END]; ++j) row_index[j - r0] = -1;
+            const long long* hd = hb.data() + (size_t)i * r.hdr_len;
+            const long long a = r.idx ? hd[r.fill_col] : hd[r.row_begin];
+            for (long long j = a; j < hd[r.row_end]; ++j) ri[j - r0] = -1;
         }
     }
     return IMMESH_OK;

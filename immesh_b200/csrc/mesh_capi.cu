@@ -7,6 +7,7 @@
 #include <chrono>
 #include <climits>
 #include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1052,10 +1053,12 @@ int immesh_mesh_create(const immesh_mesh_config* cfg, immesh_mesh_t** out) {
     return IMMESH_OK;
 }
 
+static void mesh_feed_free(immesh_mesh* h);
 int immesh_mesh_destroy(immesh_mesh_t* h) {
     if (!h) return IMMESH_OK;
     if (h->stream) cudaStreamSynchronize(h->stream);
     h->graph.destroy();
+    mesh_feed_free(h);   // after the drain: no queued kernel still writes the done word
     if (h->win.local) immesh::peer_window_close(h->win);
     if (h->nccl_comm && immesh::nccl().CommDestroy) immesh::nccl().CommDestroy(h->nccl_comm);
     for (int i = 0; i < IM_SLOTS; ++i) { if (h->ev_in[i]) cudaEventDestroy(h->ev_in[i]); if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]); }
@@ -1224,6 +1227,7 @@ static int mesh_status(int err) {
     }
     if (err & (IM_MERR_KEY_RANGE | IM_MERR_PRIO_RANGE)) return im_fail(IMMESH_E_RANGE, "mesh key out of range");
     if (err & IM_MERR_PEER_TIMEOUT) return im_fail(IMMESH_E_CUDA, "sharded mesher: a peer rank did not publish its segment in time (peer window epoch flag)");
+    if (err & IM_MERR_FEED_INDEX) return im_fail(IMMESH_E_CUDA, "frame feed: internal error (a record slot outside its ring; nothing was written)");
     return IMMESH_OK;
 }
 static void mesh_note(immesh_mesh* h, const int* c, int frame);
@@ -1528,6 +1532,142 @@ static void mesh_view_launch(immesh_mesh* h, cudaStream_t st) {
     view_image_launch(h, v, v.img, out, h->d_dyn, st);
 }
 
+// ---- the frame feed (immesh_mesh_feed_enable, mesh_feed.cuh).  k_mfeed_begin stamps the start of the frame's launch sequence; behind
+// the frame's last kernel (k_frame_end / k_chg_end, the reinforcement, the view) k_mfeed_head writes the header, the poses and the
+// cursors (mfeed_head), k_mfeed_points and k_mfeed_image copy the reinforced points and the view image into their rings at the cursors,
+// and k_mfeed_done stamps the end and publishes the frame's number to the host word the reader polls.  Fixed grids: every count is
+// read on the device.  A slot outside its ring sets IM_MERR_FEED_INDEX and nothing is written.
+__device__ __forceinline__ long long mfeed_clock() {
+    long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__global__ void k_mfeed_begin(MeshFeedDev* fd) {
+    pdl_wait();
+    if (threadIdx.x == 0) fd->t_begin = mfeed_clock();
+}
+#define MFEED_THREADS 64
+#define MFEED_COPY_THREADS 256
+static_assert(IMMESH_MESH_FEED_POSE <= MFEED_THREADS, "one thread per pose value");
+__global__ void __launch_bounds__(MFEED_THREADS) k_mfeed_head(MeshFeedDev* fd, int* cnt, long long* hdr, double* poses, long long max_frames, long long max_rows,
+                                                              long long max_images, const double (*cam_ring)[12], RfOut rf0, RfOut rf1, const double* vw_pose0,
+                                                              const double* vw_pose1) {
+    pdl_wait();
+    __shared__ long long s_slot, s_img;
+    const long long frame = fd->dyn.frame;
+    const int b = (int)(frame & 1);
+    if (threadIdx.x == 0) {
+        const long long c[8] = {cnt[IM_MC_VERTICES], cnt[IM_MC_TRIS_LIVE], cnt[IM_MC_NEW_VERTICES], (long long)cnt[IM_MC_WORK_FRONT] + cnt[IM_MC_WORK_BACK],
+                                cnt[IM_MC_ADD], cnt[IM_MC_REMOVE], cnt[IM_MC_VOXELS], cnt[IM_MC_ACT]};
+        const int* nrf = b ? rf1.n : rf0.n;
+        const long long slot = mfeed_head(*fd, c, cnt[IM_MC_ERR], (fd->dyn.rf && nrf) ? *nrf : 0, max_frames, max_rows, max_images, hdr);
+        if (slot < 0) im_atomic_or(&cnt[IM_MC_ERR], IM_MERR_FEED_INDEX);
+        s_slot = slot;
+        s_img = fd->img_slot;
+    }
+    __syncthreads();
+    const long long slot = s_slot;
+    if (slot < 0 || threadIdx.x >= IMMESH_MESH_FEED_POSE) return;
+    // the frame pose, the reinforcement camera, the view camera: 12 doubles each (row-major R, then t)
+    const int i = threadIdx.x, part = i / 12, k = i % 12;
+    double v = 0.0;
+    if (part == 0) {
+        if (fd->dyn.has_rot) v = cam_ring[frame % IM_RF_RING][k];
+        else if (k >= 9) v = fd->dyn.pose_t[k - 9];
+    } else if (part == 1) {
+        const double* p = b ? rf1.pose : rf0.pose;
+        if (fd->dyn.rf && p) v = p[k];
+    } else {
+        const double* p = b ? vw_pose1 : vw_pose0;
+        if (s_img >= 0 && p) v = p[k];
+    }
+    poses[slot * IMMESH_MESH_FEED_POSE + i] = v;
+}
+__global__ void __launch_bounds__(MFEED_COPY_THREADS) k_mfeed_points(const MeshFeedDev* fd, int* cnt, RfOut rf0, RfOut rf1, float* pts, int* pix, long long max_rows) {
+    pdl_wait();
+    const long long n = fd->nrows, base = fd->row_base;
+    if (fd->hdr_slot < 0 || n <= 0) return;
+    const RfOut o = (fd->dyn.frame & 1) ? rf1 : rf0;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long s = mfeed_row_slot(base, i, max_rows);
+        if (s < 0) { im_atomic_or(&cnt[IM_MC_ERR], IM_MERR_FEED_INDEX); continue; }
+        pts[s * 3 + 0] = o.pts[i * 3 + 0];
+        pts[s * 3 + 1] = o.pts[i * 3 + 1];
+        pts[s * 3 + 2] = o.pts[i * 3 + 2];
+        pix[s] = o.pix[i];
+    }
+}
+__global__ void __launch_bounds__(MFEED_COPY_THREADS) k_mfeed_image(const MeshFeedDev* fd, int* cnt, const uchar4* rgba0, const uchar4* rgba1, const float* depth0,
+                                                                    const float* depth1, uchar4* ring, float* depth_ring, long long npx, long long max_images) {
+    pdl_wait();
+    const long long s = fd->img_slot;
+    if (s < 0) return;   // no image for this frame
+    if (!mfeed_slot_ok(s, max_images)) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) im_atomic_or(&cnt[IM_MC_ERR], IM_MERR_FEED_INDEX);
+        return;
+    }
+    const int b = (int)(fd->dyn.frame & 1);
+    const uchar4* src = b ? rgba1 : rgba0;
+    const float* dsrc = b ? depth1 : depth0;
+    uchar4* dst = ring + s * npx;
+    float* ddst = depth_ring ? depth_ring + s * npx : nullptr;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < npx; i += (long long)gridDim.x * blockDim.x) {
+        dst[i] = src[i];
+        if (ddst) ddst[i] = dsrc[i];
+    }
+}
+__global__ void k_mfeed_done(const MeshFeedDev* fd, long long* hdr, long long* done) {
+    pdl_wait();
+    if (threadIdx.x == 0) {
+        const long long slot = fd->hdr_slot;   // checked by k_mfeed_head (-1: refused)
+        if (slot >= 0) hdr[slot * IMMESH_MESH_FEED_HDR + IMMESH_MFEED_T_END_NS] = mfeed_clock();
+        __threadfence_system();
+        *(volatile long long*)done = fd->dyn.frame;
+    }
+}
+// the frame's feed inputs, from pinned slot s (released with the frame that last used it), ahead of its kernels in stream order
+static int mesh_feed_stage(immesh_mesh* h, int s, long long frame, long long n, int step, int kind, const double* pose_t, bool rf, bool img) {
+    auto& f = h->feed;
+    MeshFeedDyn& d = f.h_dyn[s];
+    d.frame = frame;
+    d.n = n;
+    d.step = step;
+    d.kind = kind;
+    d.has_rot = pose_t ? 0 : 1;
+    d.rf = rf ? 1 : 0;
+    d.img = img ? 1 : 0;
+    d.pad_ = 0;
+    for (int j = 0; j < 3; ++j) d.pose_t[j] = pose_t ? pose_t[j] : 0.0;
+    IM_CUDA(cudaMemcpyAsync(&f.dev->dyn, &d, sizeof(MeshFeedDyn), cudaMemcpyHostToDevice, h->stream));
+    return IMMESH_OK;
+}
+// the record behind the frame's last kernel; rf / img: the frame ran the reinforcement / its image is recorded (grids fixed)
+static void mesh_feed_launch(immesh_mesh* h, cudaStream_t st, bool rf, bool img) {
+    auto& f = h->feed;
+    const RfOut none = {};
+    const RfOut r0 = rf ? h->rf.img.out[0] : none, r1 = rf ? h->rf.img.out[1] : none;
+    IM_LAUNCH(k_mfeed_head, 1, MFEED_THREADS, 0, st, f.dev, h->M.cnt, f.hdr, f.poses, f.max_frames, f.max_rows, f.max_images, (const double (*)[12])h->cam_ring, r0, r1,
+              img ? (const double*)h->vw.img.out[0].pose : (const double*)nullptr, img ? (const double*)h->vw.img.out[1].pose : (const double*)nullptr);
+    if (rf && f.max_rows > 0)
+        IM_LAUNCH(k_mfeed_points, h->n_sm * 2, MFEED_COPY_THREADS, 0, st, (const MeshFeedDev*)f.dev, h->M.cnt, r0, r1, f.pts, f.pix, f.max_rows);
+    if (img)
+        IM_LAUNCH(k_mfeed_image, h->n_sm * 4, MFEED_COPY_THREADS, 0, st, (const MeshFeedDev*)f.dev, h->M.cnt, (const uchar4*)h->vw.rgba[0], (const uchar4*)h->vw.rgba[1],
+                  (const float*)h->vw.img.out[0].depth, (const float*)h->vw.img.out[1].depth, f.rgba, f.depth_ring, f.npx, f.max_images);
+    IM_LAUNCH(k_mfeed_done, 1, 32, 0, st, (const MeshFeedDev*)f.dev, f.hdr, f.d_done);
+}
+static int mesh_feed_commit(immesh_mesh* h, long long frame) {
+    h->feed.queued = frame;
+    IM_CUDA(cudaEventRecord(h->feed.ev, h->stream));
+    return IMMESH_OK;
+}
+// drops the feed's buffers, stream and event; the caller has drained the stream and dropped the graph
+static void mesh_feed_free(immesh_mesh* h) {
+    auto& f = h->feed;
+    if (f.ev) cudaEventDestroy(f.ev);
+    if (f.stream) cudaStreamDestroy(f.stream);
+    h->feed = immesh_mesh::Feed();
+}
+
 static int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
     int b = 0;
     while (b < 64 && (max_value >> b)) ++b;
@@ -1603,7 +1743,7 @@ static void mesh_changes_launch(immesh_mesh* h, const FrameBuf& F, cudaStream_t 
 // Queues one frame (no host synchronisation except when both staging slots are still busy).  Host work per frame in the
 // pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D FrameDyn + one stream
 // wait + ONE cudaGraphLaunch (no node is touched: every per-frame value is read from the FrameDyn) + one D2H of the counters.
-static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double* pose_t, int src_mode, immesh_lio* lio, bool allow_graph = false) {
+static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double* pose_t, int src_mode, immesh_lio* lio, int kind, bool allow_graph = false) {
     if (!h || (!xyz && n > 0) || n < 0 || (src_mode < 2 && !pose_t)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_frame_points) return im_fail(IMMESH_E_CAPACITY, "frame larger than max_frame_points");
     FrameBuf& F = h->F;
@@ -1693,6 +1833,11 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         IM_CUDA(cudaMemcpyAsync(h->rf.rd, r, sizeof(RfDyn), cudaMemcpyHostToDevice, st));
     }
     const bool vw_on = h->vw.on != 0;
+    const bool fd_on = h->feed.on != 0, fd_img = fd_on && vw_on && h->feed.max_images > 0;
+    if (fd_on) {
+        rc = mesh_feed_stage(h, s, F.frame, F.n, F.step, kind, src_mode < 2 ? pose_t : nullptr, rf_on, fd_img);
+        if (rc) return rc;
+    }
     if (vw_on) {   // the view's camera source of this frame
         RfDyn* r = (RfDyn*)h->vw.h_rd + s;
         r->mode = h->vw.mode;
@@ -1709,6 +1854,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     const bool pdl_frame = F.shard_n <= 1;
     auto launch_frame = [&](bool timing) {
         const bool pdl = pdl_frame && !timing;
+        if (fd_on) IM_LAUNCH(k_mfeed_begin, 1, 32, 0, st, h->feed.dev);
         if (src_mode >= 2) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
         IM_LAUNCH_PDL(pdl && src_mode >= 2, k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[1], st);
@@ -1759,6 +1905,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
         IM_LAUNCH_PDL(pdl && !chg_on, k_frame_end, 1, 1, 0, st, h->M);
         if (rf_on) mesh_reinforce_launch(h, st);
         if (vw_on) mesh_view_launch(h, st);
+        if (fd_on) mesh_feed_launch(h, st, rf_on, fd_img);
     };
     bool queued = false;
     if (graphed) {
@@ -1779,6 +1926,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     if (rf_on) h->rf.last_frame = F.frame;
     if (vw_on) h->vw.last_frame = F.frame;
     if (chg_on) h->chg.last_frame = F.frame;
+    if (fd_on) return mesh_feed_commit(h, F.frame);
     return IMMESH_OK;
 }
 // drain the queue; returns the status of the frames harvested since the last call
@@ -1803,22 +1951,25 @@ static int mesh_wait_impl(immesh_mesh_t* h, bool timings) {
 
 int immesh_mesh_push_frame(immesh_mesh_t* h, const float* world_xyz, int n, const double* pose_t, int frame_idx) {
     (void)frame_idx;
-    int rc = mesh_enqueue(h, world_xyz, n, pose_t, 0, nullptr);
+    int rc = mesh_enqueue(h, world_xyz, n, pose_t, 0, nullptr, IMMESH_MFEED_KIND_PUSH);
+    return rc ? rc : mesh_wait_impl(h, true);
+}
+static int mesh_push_dev(immesh_mesh_t* h, const float* d_world_xyz, int n, const double* pose_t, int kind) {
+    int rc = mesh_enqueue(h, d_world_xyz, n, pose_t, 1, nullptr, kind);
     return rc ? rc : mesh_wait_impl(h, true);
 }
 int immesh_mesh_push_frame_dev(immesh_mesh_t* h, const float* d_world_xyz, int n, const double* pose_t, int frame_idx) {
     (void)frame_idx;
-    int rc = mesh_enqueue(h, d_world_xyz, n, pose_t, 1, nullptr);
-    return rc ? rc : mesh_wait_impl(h, true);
+    return mesh_push_dev(h, d_world_xyz, n, pose_t, IMMESH_MFEED_KIND_PUSH_DEV);
 }
 int immesh_mesh_push_frame_from_lio(immesh_mesh_t* h, immesh_lio_t* lio, const float* body_xyz, int n, int on_device) {
     if (!lio) return im_fail(IMMESH_E_INVALID, "null lio handle");
-    int rc = mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio);
+    int rc = mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio, IMMESH_MFEED_KIND_FROM_LIO);
     return rc ? rc : mesh_wait_impl(h, true);
 }
 int immesh_mesh_push_frame_from_lio_async(immesh_mesh_t* h, immesh_lio_t* lio, const float* body_xyz, int n, int on_device) {
     if (!lio) return im_fail(IMMESH_E_INVALID, "null lio handle");
-    return mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio, true);
+    return mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio, IMMESH_MFEED_KIND_FROM_LIO_ASYNC, true);
 }
 // device-side timing of a pipelined batch: begin mark on the localization stream, end mark behind BOTH streams
 int immesh_pipeline_mark_begin(immesh_lio_t* lio) {
@@ -1845,6 +1996,7 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (h->grow_max_bytes > 0) return im_fail(IMMESH_E_INVALID, "a mesh handle with automatic growth cannot be sharded (immesh_mesh_set_growth(h, 0) first)");
     if (h->rf.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the reinforcement enabled cannot be sharded (immesh_mesh_reinforce_enable(h, NULL, ...) first)");
     if (h->chg.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the change feed enabled cannot be sharded (immesh_mesh_changes_enable(h, 0, 0) first)");
+    if (h->feed.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the frame feed enabled cannot be sharded (immesh_mesh_feed_enable(h, NULL) first)");
     if (h->vw.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the queued view enabled cannot be sharded (immesh_mesh_view_enable(h, NULL, ...) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
@@ -2225,7 +2377,7 @@ int immesh_mesh_reconstruct_from_pointcloud(immesh_mesh_t* h, immesh_voxelgrid_t
     if (rc) return rc;
     if (n_downsampled) *n_downsampled = m;
     const double zero[3] = {0.0, 0.0, 0.0};
-    return immesh_mesh_push_frame_dev(h, immesh_voxelgrid_device_points(vg), m, zero, 0);
+    return mesh_push_dev(h, immesh_voxelgrid_device_points(vg), m, zero, IMMESH_MFEED_KIND_RECONSTRUCT);
 }
 
 // scratch of the batched frame: sized by max_voxels, max_work, max_triangles and max_list, never by the frame
@@ -2255,7 +2407,8 @@ static cudaError_t mesh_batched_scratch(immesh_mesh* h) {
 
 // incremental_mesh_reconstruction (src/ImMesh_mesh_reconstruction.cpp:92-267) as ONE frame of any size: append in chunks of <= B
 // candidates, then the per-voxel stage in batches of <= V meshed voxels (DESIGN.md, batched frame).  Blocking.
-static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels, int64_t* stats) {
+static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels, int64_t* stats,
+                             int kind) {
     if (!h || (!xyz && n > 0) || n < 0 || !pose_t || batch_points < 0 || batch_points > h->max_frame_points || batch_voxels < 0 || batch_voxels > h->F.max_work)
         return im_fail(IMMESH_E_INVALID, "bad argument (batch_points in [0, max_frame_points], batch_voxels in [0, the frame's work capacity])");
     if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "push_frame_batched: a sharded handle is not supported");
@@ -2286,6 +2439,12 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
     for (int j = 0; j < 3; ++j) { fp.pose_t[j] = pose_t[j]; fp.prio_origin[j] = 0; }
     IM_CUDA(cudaMemcpyAsync(h->b_fp, &fp, sizeof(FramePose), cudaMemcpyHostToDevice, st));
     IM_CUDA(cudaMemsetAsync(h->M.cnt + IM_MC_BAT_VERTICES, 0, (IM_MC_BAT_SELECTED + 1 - IM_MC_BAT_VERTICES) * sizeof(int), st));
+    const bool fd_on = h->feed.on != 0;   // a header and the pose: the reinforcement and the view do not follow batched frames
+    if (fd_on) {
+        const int rc = mesh_feed_stage(h, F.frame & (IM_SLOTS - 1), F.frame, n, (int)step, kind, pose_t, false, false);
+        if (rc) return rc;
+        IM_LAUNCH(k_mfeed_begin, 1, 32, 0, st, h->feed.dev);
+    }
     // ---- append, chunk c = candidates [c B, (c + 1) B), candidate i = point i step.  Host input: gathered into the pinned slot c & 1
     // while the device works on the other one
     const size_t slot_pts = (size_t)h->max_frame_points * 3;
@@ -2380,7 +2539,12 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
         mesh_changes_launch(h, F, st, true);
         h->chg.last_frame = F.frame;
     }
+    if (fd_on) mesh_feed_launch(h, st, false, false);
     IM_CUDA(cudaGetLastError());
+    if (fd_on) {
+        const int rc = mesh_feed_commit(h, F.frame);
+        if (rc) return rc;
+    }
     int cnt[IM_MC_HOST];
     IM_CUDA(cudaMemcpyAsync(cnt, h->M.cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
     IM_CUDA(cudaStreamSynchronize(st));
@@ -2392,7 +2556,7 @@ static int mesh_push_batched(immesh_mesh* h, const float* xyz, int64_t n, int on
 
 int immesh_mesh_push_frame_batched(immesh_mesh_t* h, const float* world_xyz, int64_t n, int on_device, const double* pose_t, int batch_points, int batch_voxels,
                                    int64_t* stats) {
-    return mesh_push_batched(h, world_xyz, n, on_device, pose_t, batch_points, batch_voxels, stats);
+    return mesh_push_batched(h, world_xyz, n, on_device, pose_t, batch_points, batch_voxels, stats, IMMESH_MFEED_KIND_BATCHED);
 }
 
 int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int64_t n, int on_device, float leaf, int* too_small);   // frontend_capi.cu
@@ -2412,7 +2576,7 @@ int immesh_mesh_reconstruct_from_pointcloud_batched(immesh_mesh_t* h, immesh_vox
     }
     if (small || n == 0) {   // PCL passes the cloud through: every raw point goes into the frame, whatever the VoxelGrid handle holds
         if (n_meshed_points) *n_meshed_points = n;
-        return mesh_push_batched(h, xyz, n, on_device, zero, batch_points, batch_voxels, nullptr);
+        return mesh_push_batched(h, xyz, n, on_device, zero, batch_points, batch_voxels, nullptr, IMMESH_MFEED_KIND_RECONSTRUCT_BATCHED);
     }
     int m = 0, small2 = 0;
     const int rc = n > 0x7fffffff ? IMMESH_E_CAPACITY : immesh_voxelgrid_filter(vg, xyz, (int)n, on_device, (float)minimum_pts_distance, nullptr, &m, &small2);
@@ -2420,7 +2584,7 @@ int immesh_mesh_reconstruct_from_pointcloud_batched(immesh_mesh_t* h, immesh_vox
         return im_fail(IMMESH_E_CAPACITY, "reconstruct_from_pointcloud_batched: PCL down-samples this cloud and it holds more points than the VoxelGrid handle's max_points");
     if (rc) return rc;
     if (n_meshed_points) *n_meshed_points = m;
-    return mesh_push_batched(h, immesh_voxelgrid_device_points(vg), m, 1, zero, batch_points, batch_voxels, nullptr);
+    return mesh_push_batched(h, immesh_voxelgrid_device_points(vg), m, 1, zero, batch_points, batch_voxels, nullptr, IMMESH_MFEED_KIND_RECONSTRUCT_BATCHED);
 }
 
 int immesh_mesh_render_depth(immesh_mesh_t* h, const double* intrinsics, int width, int height, double z_near, double z_far, const double* cam_R, const double* cam_t,
@@ -2595,6 +2759,12 @@ int immesh_mesh_view_enable(immesh_mesh_t* h, const double* intrinsics, int widt
     IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight use the buffers
     h->graph.destroy();                          // the captured sequence changes
     h->vw = immesh_mesh::View();                 // the buffers of an earlier enable go
+    {   // the frame feed's image ring was sized for the view that goes: image recording stops until the feed is enabled again
+        auto& f = h->feed;
+        f.img_mem = immesh::MemSet();
+        f.rgba = nullptr; f.depth_ring = nullptr;
+        f.max_images = 0; f.npx = 0; f.depth = 0;
+    }
     if (!intrinsics) return IMMESH_OK;
     v.win = win;
     RfDyn *rd = nullptr, *h_rd = nullptr;
@@ -2771,6 +2941,127 @@ int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames, 
         for (int64_t i = 0; i < nverts; ++i) { vertices[i * 3] = v[i].x; vertices[i * 3 + 1] = v[i].y; vertices[i * 3 + 2] = v[i].z; }
     }
     return IMMESH_OK;
+}
+
+int immesh_mesh_feed_enable(immesh_mesh_t* h, const immesh_mesh_feed_config* c) {
+    if (!h) return im_fail(IMMESH_E_INVALID, "null handle");
+    if (c && (c->max_frames < 1 || c->max_frames > (1LL << 20) || c->max_rows < 0 || c->max_rows > (1LL << 32) || c->max_images < 0 || c->max_images > (1LL << 16) ||
+              (c->depth != 0 && c->depth != 1) || (c->depth && c->max_images == 0)))
+        return im_fail(IMMESH_E_INVALID, "feed_enable: bad argument (max_frames in [1, 2^20], max_rows in [0, 2^32], max_images in [0, 2^16], depth 0 or 1 and 1 only with images)");
+    if (c && c->max_images > 0 && !h->vw.on) return im_fail(IMMESH_E_INVALID, "feed_enable: images need the queued view (immesh_mesh_view_enable first)");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "feed_enable: a sharded mesh handle is not supported (the frame feed runs on a single GPU)");
+    IM_CUDA(cudaStreamSynchronize(h->stream));   // frames in flight write the rings and the done word
+    h->graph.destroy();                          // the captured sequence changes
+    mesh_feed_free(h);                           // the rings of an earlier enable go
+    if (!c) return IMMESH_OK;
+    auto& f = h->feed;
+    f.max_frames = c->max_frames;
+    f.max_rows = c->max_rows;
+    f.max_images = c->max_images;
+    f.depth = c->depth;
+    f.npx = c->max_images > 0 ? (long long)h->vw.base.w * h->vw.base.h : 0;   // the view as it is configured now
+    auto fail = [&](cudaError_t e) {
+        mesh_feed_free(h);
+        cudaGetLastError();
+        return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, "feed_enable: allocation of the frame feed's buffers failed");
+    };
+    cudaError_t e;
+    if ((e = f.dev_mem.alloc(&f.dev, 1, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.hdr, (size_t)f.max_frames * IMMESH_MESH_FEED_HDR, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.dev_mem.alloc(&f.poses, (size_t)f.max_frames * IMMESH_MESH_FEED_POSE, 0)) != cudaSuccess) return fail(e);
+    if (f.max_rows > 0) {
+        if ((e = f.dev_mem.alloc(&f.pts, (size_t)f.max_rows * 3)) != cudaSuccess) return fail(e);
+        if ((e = f.dev_mem.alloc(&f.pix, (size_t)f.max_rows)) != cudaSuccess) return fail(e);
+    }
+    if (f.max_images > 0) {
+        if ((e = f.img_mem.alloc(&f.rgba, (size_t)f.max_images * (size_t)f.npx)) != cudaSuccess) return fail(e);
+        if (f.depth && (e = f.img_mem.alloc(&f.depth_ring, (size_t)f.max_images * (size_t)f.npx)) != cudaSuccess) return fail(e);
+    }
+    if ((e = f.pinned.alloc(&f.h_dyn, IM_SLOTS, 0)) != cudaSuccess) return fail(e);
+    if ((e = f.pinned.alloc(&f.h_done, 1)) != cudaSuccess) return fail(e);
+    *f.h_done = h->frame_counter;
+    if ((e = cudaHostGetDevicePointer((void**)&f.d_done, f.h_done, 0)) != cudaSuccess) return fail(e);
+    if ((e = cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(e);
+    if ((e = cudaEventCreateWithFlags(&f.ev, cudaEventDisableTiming)) != cudaSuccess) return fail(e);
+    if ((e = cudaEventRecord(f.ev, h->stream)) != cudaSuccess) return fail(e);
+    if ((e = cudaDeviceSynchronize()) != cudaSuccess) return fail(e);   // the initialising memsets ran on the legacy stream
+    f.enable_frame = f.queued = h->frame_counter;
+    f.on = 1;
+    return IMMESH_OK;
+}
+// the marks a read checks after its copies: the newest frame whose slot is being written and the cursor of the ring read (points or images)
+static int mesh_feed_marks(immesh_mesh* h, bool images, long long* m) {
+    auto& f = h->feed;
+    long long b[3];
+    IM_CUDA(cudaMemcpyAsync(b, &f.dev->started, sizeof(b), cudaMemcpyDeviceToHost, f.stream));
+    IM_CUDA(cudaStreamSynchronize(f.stream));
+    static_assert(offsetof(MeshFeedDev, rows_total) == offsetof(MeshFeedDev, started) + 8 && offsetof(MeshFeedDev, imgs_total) == offsetof(MeshFeedDev, started) + 16,
+                  "the marks are read with one copy");
+    m[0] = b[0];
+    m[1] = images ? b[2] : b[1];
+    return IMMESH_OK;
+}
+// the common part of the two reads: arguments, the wait, counts[2..3]; returns the newest finished frame in *fin
+static int mesh_feed_begin_read(immesh_mesh* h, const char* what, int64_t since, int wait, int64_t* counts, long long* fin) {
+    auto& f = h->feed;
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, (std::string(what) + ": a sharded mesh handle is not supported").c_str());
+    if (!f.on) return im_fail(IMMESH_E_INVALID, (std::string(what) + ": the frame feed is not enabled (immesh_mesh_feed_enable)").c_str());
+    if (since > f.queued) return im_fail(IMMESH_E_INVALID, (std::string(what) + ": since_frame is newer than the newest queued frame").c_str());
+    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued frame's record, nothing else
+    *fin = *(volatile long long*)f.h_done;
+    counts[2] = *fin;
+    counts[3] = f.queued;
+    return IMMESH_OK;
+}
+static int mesh_feed_end_read(int rc, const char* what) {
+    if (rc == IMMESH_E_RANGE)
+        return im_fail(rc, (std::string(what) + ": frames of the range predate the enable, left the rings or were overwritten while they were read; read on from counts[2]").c_str());
+    if (rc == IMMESH_E_CAPACITY) return im_fail(rc, (std::string(what) + ": more frames or rows than the caps (counts holds them; nothing was written)").c_str());
+    return rc;
+}
+int immesh_mesh_feed(immesh_mesh_t* h, int64_t since, int wait, int64_t* frames, double* poses, int cap_frames, float* points, int32_t* pixels, int64_t cap_rows,
+                     int64_t* counts) {
+    if (counts) for (int k = 0; k < 4; ++k) counts[k] = 0;
+    if (!h || !counts || since < 0 || cap_frames < 0 || cap_rows < 0 || (cap_frames > 0 && !frames)) return im_fail(IMMESH_E_INVALID, "feed: bad argument");
+    long long fin = 0;
+    int rc = mesh_feed_begin_read(h, "feed", since, wait, counts, &fin);
+    if (rc) return rc;
+    auto& f = h->feed;
+    const FeedRings rings = mfeed_point_rings(f.max_frames, f.max_rows, f.hdr, f.poses, f.pts, f.pix);
+    auto copy = [&](void* dst, const void* src, size_t bytes) {   // on the feed's stream, never the handle's
+        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
+        return IMMESH_OK;
+    };
+    auto marks = [&](long long* m) { return mesh_feed_marks(h, false, m); };
+    rc = feed_read(rings, since, fin, frames, poses, cap_frames, points, pixels, cap_rows, counts, copy, marks);
+    return mesh_feed_end_read(rc, "feed");
+}
+int immesh_mesh_feed_images(immesh_mesh_t* h, int64_t since, int wait, int64_t* frames, int cap_images, uint8_t* rgba, float* depth, int64_t* counts) {
+    if (counts) for (int k = 0; k < 4; ++k) counts[k] = 0;
+    if (!h || !counts || since < 0 || cap_images < 0 || (cap_images > 0 && !frames)) return im_fail(IMMESH_E_INVALID, "feed_images: bad argument");
+    auto& f = h->feed;
+    if (f.on && f.max_images == 0)
+        return im_fail(IMMESH_E_INVALID, "feed_images: image recording is off (max_images = 0, or immesh_mesh_view_enable was called after the enable)");
+    if (f.on && depth && !f.depth) return im_fail(IMMESH_E_INVALID, "feed_images: depth requested but the feed was enabled without depth");
+    long long fin = 0;
+    int rc = mesh_feed_begin_read(h, "feed_images", since, wait, counts, &fin);
+    if (rc) return rc;
+    FeedRings rings = mfeed_image_rings(f.max_frames, f.max_images, f.npx, f.hdr, f.rgba, f.depth_ring);
+    void* rows = rgba;
+    void* second = depth;
+    if (!rgba && depth) {   // the depth images alone: they are the rows
+        rings.rows = f.depth_ring;
+        rings.idx = nullptr;
+        rows = depth;
+        second = nullptr;
+    }
+    auto copy = [&](void* dst, const void* src, size_t bytes) {
+        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
+        return IMMESH_OK;
+    };
+    auto marks = [&](long long* m) { return mesh_feed_marks(h, true, m); };
+    rc = feed_read(rings, since, fin, frames, nullptr, cap_images, rows, second, cap_images, counts, copy, marks);
+    return mesh_feed_end_read(rc, "feed_images");
 }
 
 int immesh_mesh_last_timing(immesh_mesh_t* h, double* ms) {

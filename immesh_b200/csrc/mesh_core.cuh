@@ -63,6 +63,7 @@ enum : int {
     IM_MERR_KEY_RANGE = 32,
     IM_MERR_PRIO_RANGE = 64, // activated voxel farther than 1024 voxels from the sensor (flip priority)
     IM_MERR_PEER_TIMEOUT = 128,   // sharded mode: a peer rank's epoch flag did not arrive (peer_win.cuh)
+    IM_MERR_FEED_INDEX = 256,     // the frame feed computed a slot outside its ring (mesh_feed.cuh): an internal error, nothing written
 };
 
 struct MeshDev {

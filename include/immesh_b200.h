@@ -683,6 +683,83 @@ int immesh_mesh_view_overlay(immesh_mesh_t* h, const immesh_view_overlay* o /* N
 int immesh_mesh_changes_enable(immesh_mesh_t* h, int64_t max_rows, int max_frames);
 int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames /*[cap_frames][4]*/, int cap_frames, int32_t* rows /*[cap_rows][4]*/,
                         int64_t cap_rows, float* vertices /*[cap_vertices][3]*/, int64_t cap_vertices, int64_t* counts /*[4]*/);
+/* The frame feed: every queued mesh frame's counters, pose, reinforced points and viewer image, recorded on the device inside the
+ * frame's launch sequence (its captured graph), so that a node on the queued chain (immesh_mesh_push_frame_from_lio_async) publishes
+ * per frame what the reference publishes -- the mesh_cost_time.log fields, the trajectory, the reinforced LiDAR points, a video of
+ * the viewer -- without draining.  Records are numbered by the handle's frame numbers (those of immesh_mesh_changes and of
+ * immesh_mesh_view_image's frame_out): frame f in header slot (f - 1) % max_frames; the frames queued after the enable are recorded.
+ *   Every frame of immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async and immesh_mesh_reconstruct_from_pointcloud records one
+ *     frame.  A batched frame (immesh_mesh_push_frame_batched, _reconstruct_from_pointcloud_batched) records its header and pose, with
+ *     no points and no image (the reinforcement and the view do not follow batched frames).
+ *   header (IMMESH_MESH_FEED_HDR int64, IMMESH_MFEED_*): FRAME; KIND (IMMESH_MFEED_KIND_*); N_POINTS and STEP (append_point_step);
+ *     the eight values of immesh_mesh_counts right after the frame (COUNTS + 0..7); ERR (the frame's IM_MERR flags); HAS_ROTATION (1:
+ *     handed over by a localization handle); T_BEGIN_NS, T_END_NS (%globaltimer at the start of the frame's launch sequence and at its
+ *     record: the device analogue of the reference's per-frame mesh time); ROW_BEGIN, ROW_END (the frame's reinforced points, numbered
+ *     over the point ring) and ROWS_LOST; RF (1: the reinforcement ran for the frame); IMG_BEGIN, IMG_END (its image, numbered over the
+ *     image ring: one image or none).
+ *   poses (36 doubles per frame, each a row-major R then t): the frame pose (rot_end, pos_end of the handed-over state; for a
+ *     world-frame push R is all zeros -- HAS_ROTATION = 0 -- and t is pose_t); the reinforcement camera as immesh_mesh_reinforced_cloud's
+ *     pose_out (zeros when RF = 0); the view camera as immesh_mesh_view_image's pose_out (zeros without an image).
+ *   points / pixels: the frame's reinforced points and their pixels, equal to immesh_mesh_reinforced_cloud right after the frame bit
+ *     for bit and in its order.  A frame whose points exceed max_rows keeps its header and poses, sets ROWS_LOST and writes no point;
+ *     a loss never fails a push and never changes the mesh.  max_rows = 0: no point is recorded (ROW_BEGIN == ROW_END, RF still set).
+ *   images: the queued view's rgba (and depth with cfg.depth), equal to immesh_mesh_view_image right after the frame bit for bit; the
+ *     image ring keeps the newest max_images images.  The ring is sized for the view as it is configured at the enable: every
+ *     immesh_mesh_view_enable call (NULL and a new size included) turns the image recording off and frees the ring -- later frames
+ *     record IMG_BEGIN == IMG_END and immesh_mesh_feed_images returns IMMESH_E_INVALID until the feed is enabled again.
+ * immesh_mesh_feed_enable(h, cfg) checks its arguments, drains h, drops its captured launch sequence, frees the rings of an earlier
+ *   enable and allocates everything once (an allocation failure: IMMESH_E_CAPACITY, the feed off).  NULL turns the feed off.
+ *   max_frames in [1, 2^20], max_rows in [0, 2^32], max_images in [0, 2^16] (> 0 needs the queued view, immesh_mesh_view_enable),
+ *   depth 0 or 1 (1 needs max_images > 0); other values or a sharded handle: IMMESH_E_INVALID.  immesh_mesh_shard refuses a handle
+ *   with the feed on.  While the feed is off nothing is launched, captured or allocated for it.
+ * immesh_mesh_feed(h, since_frame, wait, ...) returns the frames (since_frame, newest finished] oldest first, their poses (or NULL)
+ *   and their points and pixels concatenated (or NULL; pixels are written with points); immesh_mesh_feed_images the same frames'
+ *   headers and the images they hold, concatenated oldest first (rgba or depth may be NULL).  wait = 0 never blocks on queued work
+ *   ("finished": a pinned host word the last kernel of each record writes; the copies run on a stream of the feed's own); wait = 1
+ *   first waits for the newest queued frame's record only.  counts [4] = frames, rows (images), newest finished, newest queued.
+ *   cap_frames (cap_images) = 0: a count query.  More frames than the cap, or more points than cap_rows: IMMESH_E_CAPACITY with the
+ *   counts, nothing written.  IMMESH_E_RANGE with counts[2] set (read on from there): the range reaches back before the enable, or a
+ *   slot of it (header, points or image) was overwritten before or during the copy.  Bad arguments, the feed off, since_frame newer
+ *   than the newest queued frame, images requested while image recording is off, depth requested without cfg.depth, or a sharded
+ *   handle: IMMESH_E_INVALID.  A record kernel that computes a slot outside its ring (an internal error) writes nothing and the push
+ *   that harvests the frame returns IMMESH_E_CUDA ("internal error"). */
+typedef struct {
+    int64_t max_frames;   /* header + pose ring, in frames: [1, 2^20] */
+    int64_t max_rows;     /* reinforced-point ring, rows: [0, 2^32]; 0 = no points recorded */
+    int64_t max_images;   /* view image ring, in images: [0, 2^16]; > 0 needs the queued view enabled */
+    int depth;            /* 1: the image ring also keeps the view's depth image */
+    int pad;
+} immesh_mesh_feed_config;
+#define IMMESH_MESH_FEED_HDR 22
+#define IMMESH_MESH_FEED_POSE 36
+#define IMMESH_MFEED_FRAME 0
+#define IMMESH_MFEED_KIND 1
+#define IMMESH_MFEED_N_POINTS 2
+#define IMMESH_MFEED_STEP 3
+#define IMMESH_MFEED_COUNTS 4   /* 8 fields: immesh_mesh_counts' out[0..7] */
+#define IMMESH_MFEED_ERR 12
+#define IMMESH_MFEED_HAS_ROTATION 13
+#define IMMESH_MFEED_T_BEGIN_NS 14
+#define IMMESH_MFEED_T_END_NS 15
+#define IMMESH_MFEED_ROW_BEGIN 16
+#define IMMESH_MFEED_ROW_END 17
+#define IMMESH_MFEED_ROWS_LOST 18
+#define IMMESH_MFEED_RF 19
+#define IMMESH_MFEED_IMG_BEGIN 20
+#define IMMESH_MFEED_IMG_END 21
+/* IMMESH_MFEED_KIND: the entry point that queued the frame */
+#define IMMESH_MFEED_KIND_PUSH 0
+#define IMMESH_MFEED_KIND_PUSH_DEV 1
+#define IMMESH_MFEED_KIND_FROM_LIO 2
+#define IMMESH_MFEED_KIND_FROM_LIO_ASYNC 3
+#define IMMESH_MFEED_KIND_RECONSTRUCT 4
+#define IMMESH_MFEED_KIND_BATCHED 5
+#define IMMESH_MFEED_KIND_RECONSTRUCT_BATCHED 6
+int immesh_mesh_feed_enable(immesh_mesh_t* h, const immesh_mesh_feed_config* cfg /* NULL: off */);
+int immesh_mesh_feed(immesh_mesh_t* h, int64_t since_frame, int wait, int64_t* frames /*[cap_frames][22]*/, double* poses /*[cap_frames][36] or NULL*/,
+                     int cap_frames, float* points /*[cap_rows][3] or NULL*/, int32_t* pixels /*[cap_rows] or NULL*/, int64_t cap_rows, int64_t* counts /*[4]*/);
+int immesh_mesh_feed_images(immesh_mesh_t* h, int64_t since_frame, int wait, int64_t* frames /*[cap_images][22]*/, int cap_images,
+                            uint8_t* rgba /*[cap_images][h][w][4] or NULL*/, float* depth /*[cap_images][h][w] or NULL*/, int64_t* counts /*[4]*/);
 /* Evaluation of the mesh against a ground-truth cloud with the metrics of the ImMesh paper's Experiment-3 (section VIII-C, Tables V
  * and VI, Fig. 8 and 9): fairness (mean Max-Min interior angle, mean circumradius-to-shortest-edge ratio) and correctness (accuracy,
  * completeness, precision, recall, F-score between points sampled on the mesh and the down-sampled ground truth).
