@@ -78,7 +78,33 @@ MESH_FEED_HDR = 22    # IMMESH_MESH_FEED_HDR: the header columns of a recorded m
 MESH_FEED_HDR_KEYS = ("frame", "kind", "n_points", "step", "n_vertices", "n_triangles", "new_vertices", "voxels_meshed", "n_add", "n_remove", "n_voxels",
                       "n_activated", "err", "has_rotation", "t_begin_ns", "t_end_ns", "row_begin", "row_end", "rows_lost", "rf", "img_begin", "img_end")
 MESH_FEED_POSE = 36   # IMMESH_MESH_FEED_POSE: frame pose, reinforcement camera, view camera; each a row-major R then t
-MESH_FEED_KINDS = ("push", "push_dev", "from_lio", "from_lio_async", "reconstruct", "batched", "reconstruct_batched")   # IMMESH_MFEED_KIND_*
+MESH_FEED_KINDS = ("push", "push_dev", "from_lio", "from_lio_async", "reconstruct", "batched", "reconstruct_batched", "depth")   # IMMESH_MFEED_KIND_*
+
+
+class _DepthFrame(C.Structure):
+    _fields_ = [("width", C.c_int), ("height", C.c_int), ("pitch_bytes", C.c_int64), ("format", C.c_int), ("kind", C.c_int), ("depth_scale", C.c_double),
+                ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double), ("z_min", C.c_double), ("z_max", C.c_double),
+                ("stride", C.c_int), ("pad", C.c_int), ("cam_R", C.c_double * 9), ("cam_t", C.c_double * 3)]
+
+
+DEPTH_FORMATS = {"f32": 0, "u16": 1}        # IMMESH_DEPTH_F32, IMMESH_DEPTH_U16
+DEPTH_KINDS = {"planar": 0, "range": 1}     # IMMESH_DEPTH_PLANAR, IMMESH_DEPTH_RANGE
+
+
+@dataclasses.dataclass
+class DepthCamera:
+    """The pinhole camera of a depth stream (immesh_depth_frame): intrinsics in pixels, the depth kind ("planar": z along the optical
+    axis, AirSim DepthPlanar; "range": distance along the ray, AirSim DepthPerspective), the valid z range in metres, the pixel stride
+    and the metres per count of a uint16 image.  Poses are camera to world with OpenCV axes (x right, y down, z forward)."""
+    fx: float
+    fy: float
+    cx: float
+    cy: float
+    kind: str = "planar"
+    z_min: float = 0.1
+    z_max: float = 100.0
+    stride: int = 1
+    depth_scale: float = 0.001
 
 
 class FeedLost(RuntimeError):
@@ -176,6 +202,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_lio_enqueue_memset", [vp, vp, C.c_size_t]),
         ("immesh_mesh_push_frame_from_lio_async", [vp, vp, vp, C.c_int, C.c_int]),
         ("immesh_mesh_wait", [vp]),
+        ("immesh_mesh_push_depth", [vp, C.POINTER(_DepthFrame), vp, C.c_int]),
+        ("immesh_mesh_push_depth_async", [vp, C.POINTER(_DepthFrame), vp, C.c_int]),
+        ("immesh_mesh_depth_points", [vp, fp, C.c_int, ip]),
         ("immesh_pipeline_mark_begin", [vp]),
         ("immesh_pipeline_mark_end", [vp, vp, dp]),
         ("immesh_mesh_work_stats", [vp, C.POINTER(C.c_int64)]),
@@ -715,6 +744,48 @@ class Mesh:
 
     def wait(self):
         _check(self.lib, self.lib.immesh_mesh_wait(self._h), "mesh_wait")
+
+    @staticmethod
+    def _depth_args(cam: DepthCamera, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device):
+        """the immesh_depth_frame of one image: a 2-D float32 / uint16 numpy array (rows may be padded), or a CUDA address with
+        shape = (height, width), fmt ("f32" / "u16") and pitch_bytes (0: tight)"""
+        if on_device:
+            height, width = shape
+            ptr, keep = C.c_void_p(int(depth)), None
+        else:
+            keep = np.asarray(depth)
+            if keep.ndim != 2 or keep.dtype not in (np.float32, np.uint16):
+                raise ValueError("depth: a 2-D float32 or uint16 array")
+            if keep.strides[1] != keep.itemsize or keep.strides[0] < keep.shape[1] * keep.itemsize:
+                keep = np.ascontiguousarray(keep)
+            height, width = keep.shape
+            fmt, pitch_bytes = ("f32" if keep.dtype == np.float32 else "u16"), keep.strides[0]
+            ptr = C.c_void_p(keep.ctypes.data)
+        f = _DepthFrame(int(width), int(height), int(pitch_bytes), DEPTH_FORMATS[fmt], DEPTH_KINDS[cam.kind], float(cam.depth_scale), float(cam.fx),
+                        float(cam.fy), float(cam.cx), float(cam.cy), float(cam.z_min), float(cam.z_max), int(cam.stride), 0,
+                        (C.c_double * 9)(*np.asarray(cam_R, dtype=np.float64).reshape(9)), (C.c_double * 3)(*np.asarray(cam_t, dtype=np.float64).reshape(3)))
+        return f, ptr, keep
+
+    def push_depth(self, depth, cam: DepthCamera, cam_R, cam_t, on_device=False, shape=None, fmt="f32", pitch_bytes=0):
+        """One mesh frame from a depth image, unprojected on the device (immesh_mesh_push_depth): the valid samples' world points,
+        meshed at pose_t = cam_t.  cam_R, cam_t: camera to world, OpenCV axes."""
+        f, ptr, _keep = self._depth_args(cam, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device)
+        _check(self.lib, self.lib.immesh_mesh_push_depth(self._h, C.byref(f), ptr, 1 if on_device else 0), "mesh_push_depth")
+
+    def push_depth_async(self, depth, cam: DepthCamera, cam_R, cam_t, on_device=False, shape=None, fmt="f32", pitch_bytes=0):
+        """queued push_depth; wait() drains.  A host image is staged before the call returns; a device image must stay unchanged
+        until the frame has run."""
+        f, ptr, _keep = self._depth_args(cam, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device)
+        _check(self.lib, self.lib.immesh_mesh_push_depth_async(self._h, C.byref(f), ptr, 1 if on_device else 0), "mesh_push_depth_async")
+
+    def depth_points(self):
+        """the newest depth frame's world points, float32[n][3] in ascending pixel order (immesh_mesh_depth_points; blocking)"""
+        n = C.c_int(0)
+        _check(self.lib, self.lib.immesh_mesh_depth_points(self._h, None, 0, C.byref(n)), "mesh_depth_points")
+        out = np.zeros((n.value, 3), dtype=np.float32)
+        if n.value:
+            _check(self.lib, self.lib.immesh_mesh_depth_points(self._h, out.ctypes.data_as(C.POINTER(C.c_float)), n.value, C.byref(n)), "mesh_depth_points")
+        return out
 
     def counts(self):
         o = np.zeros(8, dtype=np.int64)

@@ -232,6 +232,20 @@ def build_eval(force=False):
     return EMU_EVAL
 
 
+EMU_DEPTH_FRAME = os.path.join(_ROOT, "tests", "depth_frame", "libimmesh_emu_depth_frame.so")
+
+
+def build_depth_frame(force=False):
+    """tests/depth_frame: the depth frame's unprojection and append-step bodies (immesh_b200/csrc/depth_frame.cuh) with the device
+    kernels' compaction restated on the host"""
+    src = os.path.join(_ROOT, "tests", "depth_frame", "emu_depth_frame.cpp")
+    deps = [src, os.path.join(CSRC, "depth_frame.cuh"), os.path.join(CSRC, "hd_math.cuh"), os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_DEPTH_FRAME, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_DEPTH_FRAME, src])
+    return EMU_DEPTH_FRAME
+
+
 LOCAL_MAP_DIR = os.path.join(_ROOT, "tests", "local_map")
 EMU_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "libimmesh_emu_local_map.so")
 ORACLE_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "liborc_local_map.so")
@@ -284,6 +298,7 @@ def build_all(force=False):
     build_mesh_feed(force)
     build_rs_check(force)
     build_eval(force)
+    build_depth_frame(force)
     build_local_map(force)
     build_dev_mem(force)
     build_ref()

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include "common_host.hpp"
+#include "depth_frame.cuh"
 #include "lio_core.cuh"
 #include "lio_feed.cuh"
 #include "mesh_changes.cuh"
@@ -283,6 +284,18 @@ struct immesh_mesh {
         cudaEvent_t ev = nullptr;         // recorded behind the newest frame's record
         immesh::MemSet dev_mem, img_mem, pinned{immesh::MemSet::Pinned};
     } feed;
+    // depth-camera frames (immesh_mesh_push_depth, depth_frame.cuh), allocated by the first of them and kept until destroy.  The points
+    // buffer holds the newest depth frame's world points (one buffer: every frame's kernels run in stream order on `stream`).
+    struct Depth {
+        immesh::DepthFrame* d_df = nullptr;   // the frame's image and camera, written per frame from the pinned slot
+        immesh::DepthFrame* h_df = nullptr;   // pinned, IM_SLOTS slots
+        float* pts = nullptr;                 // [max_frame_points][3] the valid samples' world points (FrameDyn::pts of a depth frame)
+        int* n = nullptr;                     // their count
+        int *blk = nullptr, *blk_off = nullptr;   // valid samples per block of DF_BLOCK sampled pixels, their offsets [nb + 1]
+        int nb = 0;                           // blocks covering max_frame_points sampled pixels
+        int last_frame = 0;                   // newest depth frame queued (0: none)
+        immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // not counted in immesh_mesh_capacity
+    } dep;
 };
 
 // The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate

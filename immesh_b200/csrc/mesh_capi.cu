@@ -551,6 +551,33 @@ __global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const F
     if (blockIdx.x == 0 && threadIdx.x == 0) *o.n = blk_off[nb];
 }
 
+// ---- depth-camera frames (immesh_mesh_push_depth, depth_frame.cuh): the valid samples per block of DF_BLOCK consecutive sampled pixels
+// (k_depth_count), their offsets (k_rf_scan), then each valid sample's world point at its block's offset plus its rank in the block
+// (k_depth_emit), so that the points keep the pixel order the vertex append depends on.  Block 0 of the emit sets the frame's n, step,
+// m and cmask in its FrameDyn (frame_append_dims): the kernels after it read the device count.  Grids cover max_frame_points samples.
+#define DF_BLOCK 1024
+__global__ void __launch_bounds__(DF_BLOCK) k_depth_count(const DepthFrame* df, int* blk) {
+    const DepthFrame& D = *df;
+    const int k = blockIdx.x * DF_BLOCK + threadIdx.x;
+    float p[3];
+    const int c = __syncthreads_count(k < D.sw * D.sh && depth_point(D, k, p));
+    if (threadIdx.x == 0) blk[blockIdx.x] = c;
+}
+__global__ void __launch_bounds__(DF_BLOCK) k_depth_emit(const DepthFrame* df, const int* blk_off, int nb, int append_target, FrameDyn* dyn, float* pts, int* n_out) {
+    const DepthFrame& D = *df;
+    const int k = blockIdx.x * DF_BLOCK + threadIdx.x;
+    float p[3];
+    const bool ok = k < D.sw * D.sh && depth_point(D, k, p);
+    const int i = blk_off[blockIdx.x] + block_scan_1024(ok ? 1 : 0);
+    if (ok) { pts[(size_t)i * 3 + 0] = p[0]; pts[(size_t)i * 3 + 1] = p[1]; pts[(size_t)i * 3 + 2] = p[2]; }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        const int n = blk_off[nb];
+        *n_out = n;
+        dyn->n = n;
+        frame_append_dims(n, append_target, &dyn->step, &dyn->m, &dyn->cmask);
+    }
+}
+
 // ---- the viewer's shaded image of the live mesh (draw_triangle with the facet shader, mesh_rec_display.cpp:273-282; the rule is
 // immesh_mesh_render_view's, include/immesh_b200.h).  The binning passes of the depth image (k_rf_count -> k_rf_scan -> k_rf_fill,
 // with the view's positions), the z range of the height colour when it is automatic (k_view_zrange), then one block per tile
@@ -1551,12 +1578,13 @@ __global__ void k_mfeed_begin(MeshFeedDev* fd) {
 static_assert(IMMESH_MESH_FEED_POSE <= MFEED_THREADS, "one thread per pose value");
 __global__ void __launch_bounds__(MFEED_THREADS) k_mfeed_head(MeshFeedDev* fd, int* cnt, long long* hdr, double* poses, long long max_frames, long long max_rows,
                                                               long long max_images, const double (*cam_ring)[12], RfOut rf0, RfOut rf1, const double* vw_pose0,
-                                                              const double* vw_pose1) {
+                                                              const double* vw_pose1, const FrameDyn* dyn) {
     pdl_wait();
     __shared__ long long s_slot, s_img;
     const long long frame = fd->dyn.frame;
     const int b = (int)(frame & 1);
     if (threadIdx.x == 0) {
+        if (fd->dyn.n < 0) { fd->dyn.n = dyn->n; fd->dyn.step = dyn->step; }   // a depth frame: counted on the device
         const long long c[8] = {cnt[IM_MC_VERTICES], cnt[IM_MC_TRIS_LIVE], cnt[IM_MC_NEW_VERTICES], (long long)cnt[IM_MC_WORK_FRONT] + cnt[IM_MC_WORK_BACK],
                                 cnt[IM_MC_ADD], cnt[IM_MC_REMOVE], cnt[IM_MC_VOXELS], cnt[IM_MC_ACT]};
         const int* nrf = b ? rf1.n : rf0.n;
@@ -1647,7 +1675,8 @@ static void mesh_feed_launch(immesh_mesh* h, cudaStream_t st, bool rf, bool img)
     const RfOut none = {};
     const RfOut r0 = rf ? h->rf.img.out[0] : none, r1 = rf ? h->rf.img.out[1] : none;
     IM_LAUNCH(k_mfeed_head, 1, MFEED_THREADS, 0, st, f.dev, h->M.cnt, f.hdr, f.poses, f.max_frames, f.max_rows, f.max_images, (const double (*)[12])h->cam_ring, r0, r1,
-              img ? (const double*)h->vw.img.out[0].pose : (const double*)nullptr, img ? (const double*)h->vw.img.out[1].pose : (const double*)nullptr);
+              img ? (const double*)h->vw.img.out[0].pose : (const double*)nullptr, img ? (const double*)h->vw.img.out[1].pose : (const double*)nullptr,
+              (const FrameDyn*)h->d_dyn);
     if (rf && f.max_rows > 0)
         IM_LAUNCH(k_mfeed_points, h->n_sm * 2, MFEED_COPY_THREADS, 0, st, (const MeshFeedDev*)f.dev, h->M.cnt, r0, r1, f.pts, f.pix, f.max_rows);
     if (img)
@@ -1739,22 +1768,37 @@ static void mesh_changes_launch(immesh_mesh* h, const FrameBuf& F, cudaStream_t 
     IM_LAUNCH(k_chg_end, 1, 1, 0, st, h->M, F, c.C, full, full);
 }
 
-// src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state.
+// A depth frame's source (src_mode 4): the kernels' DepthFrame, and the host image to stage (null: df.img is the caller's device image)
+struct DepthSrc {
+    DepthFrame df;
+    const unsigned char* host_img;
+    long long pitch;
+    int bpp;
+};
+
+// src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state, 4 a depth
+// image (dsrc; n is the sampled pixels, the upper bound of the count its kernels set on the device).
 // Queues one frame (no host synchronisation except when both staging slots are still busy).  Host work per frame in the
 // pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D FrameDyn + one stream
 // wait + ONE cudaGraphLaunch (no node is touched: every per-frame value is read from the FrameDyn) + one D2H of the counters.
-static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double* pose_t, int src_mode, immesh_lio* lio, int kind, bool allow_graph = false) {
-    if (!h || (!xyz && n > 0) || n < 0 || (src_mode < 2 && !pose_t)) return im_fail(IMMESH_E_INVALID, "bad argument");
+static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double* pose_t, int src_mode, immesh_lio* lio, int kind, bool allow_graph = false,
+                        const DepthSrc* dsrc = nullptr) {
+    const bool from_lio = src_mode == 2 || src_mode == 3, depth = src_mode == 4;
+    if (!h || (!xyz && n > 0 && !depth) || n < 0 || (!from_lio && !pose_t) || (depth && !dsrc)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_frame_points) return im_fail(IMMESH_E_CAPACITY, "frame larger than max_frame_points");
     FrameBuf& F = h->F;
     const MeshParams& P = h->P;
-    // append_point_step = max(1, round(N / appending_pts_frame)), integer division first (ImMesh_mesh_reconstruction.cpp:111)
-    const int step = std::max(1, (int)std::lround((double)(n / P.append_target)));
-    const int grc = mesh_growth_check(h, n > 0 ? (n + step - 1) / step : 0);
+    // a depth frame's n, step, m and cmask are set by its kernels from the valid count: the host holds n = the sampled pixels and the
+    // most candidates they can give, for the growth check and for the grids, which cover max_frame_points anyway
+    int step, m;
+    unsigned int cmask;
+    frame_append_dims(n, P.append_target, &step, &m, &cmask);
+    if (depth) m = frame_append_max_m(n, P.append_target);
+    const int grc = mesh_growth_check(h, m);
     if (grc) return grc;
     F.n = n;
     F.step = step;
-    F.m = n > 0 ? (n + step - 1) / step : 0;
+    F.m = m;
     F.frame = ++h->frame_counter;
     const int s = F.frame & (IM_SLOTS - 1);
     int rc = mesh_harvest(h, s);  // the frame IM_SLOTS calls ago used this slot
@@ -1764,18 +1808,39 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     float* h_pts = h->h_pts + s * slot_pts;
     FramePose* d_fp = h->d_fp + s;
     F.fp = d_fp;
-    F.cmask = (unsigned)(pow2_at_least((size_t)std::max(F.m, 1) * 2) - 1);
+    F.cmask = cmask;
     cudaStream_t st = h->stream;
     const bool graphed = allow_graph && h->use_graph && !profiler().enabled && (F.shard_n <= 1 || h->win.ok);
     if (!graphed) IM_CUDA(cudaEventRecord(h->ev[0], st));
     F.pts = d_pts;
     const float* d_body = nullptr;
     int pose_idx = 0;
-    if (src_mode < 2) {
+    if (!from_lio) {
         FramePose* hp = h->h_fp + s;
         for (int j = 0; j < 3; ++j) { hp->pose_t[j] = pose_t[j]; hp->prio_origin[j] = (long long)std::floor(pose_t[j] / P.res) - 1024; }
         IM_CUDA(cudaMemcpyAsync(d_fp, hp, sizeof(FramePose), cudaMemcpyHostToDevice, st));
-        if (n > 0) {
+        if (depth) {
+            F.pts = h->dep.pts;
+            DepthFrame* hd = h->dep.h_df + s;
+            *hd = dsrc->df;
+            if (dsrc->host_img) {   // the sampled grid, tight, through the pinned slot (sw * sh * bpp <= 4 max_frame_points bytes)
+                unsigned char* hb = reinterpret_cast<unsigned char*>(h_pts);
+                const size_t rowb = (size_t)hd->sw * dsrc->bpp;
+                for (int sv = 0; sv < hd->sh; ++sv) {
+                    const unsigned char* row = dsrc->host_img + (size_t)sv * hd->stride * dsrc->pitch;
+                    if (hd->stride == 1) { std::memcpy(hb + sv * rowb, row, rowb); continue; }
+                    for (int su = 0; su < hd->sw; ++su) std::memcpy(hb + sv * rowb + (size_t)su * dsrc->bpp, row + (size_t)su * hd->stride * dsrc->bpp, dsrc->bpp);
+                }
+                unsigned char* db = reinterpret_cast<unsigned char*>(h->d_body + s * slot_pts);
+                IM_CUDA(cudaMemcpyAsync(db, hb, rowb * hd->sh, cudaMemcpyHostToDevice, h->stream_up));
+                IM_CUDA(cudaEventRecord(h->ev_up[s], h->stream_up));
+                IM_CUDA(cudaStreamWaitEvent(st, h->ev_up[s], 0));
+                hd->img = db;
+                hd->row_bytes = (long long)rowb;
+                hd->col_bytes = dsrc->bpp;
+            }
+            IM_CUDA(cudaMemcpyAsync(h->dep.d_df, hd, sizeof(DepthFrame), cudaMemcpyHostToDevice, st));
+        } else if (n > 0) {
             if (src_mode == 0) {
                 const float* src = xyz;
                 if (!immesh::host_ptr_is_pinned(xyz)) { std::memcpy(h_pts, xyz, (size_t)n * 3 * sizeof(float)); src = h_pts; }
@@ -1835,7 +1900,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     const bool vw_on = h->vw.on != 0;
     const bool fd_on = h->feed.on != 0, fd_img = fd_on && vw_on && h->feed.max_images > 0;
     if (fd_on) {
-        rc = mesh_feed_stage(h, s, F.frame, F.n, F.step, kind, src_mode < 2 ? pose_t : nullptr, rf_on, fd_img);
+        rc = mesh_feed_stage(h, s, F.frame, depth ? -1 : F.n, F.step, kind, from_lio ? nullptr : pose_t, rf_on, fd_img);
         if (rc) return rc;
     }
     if (vw_on) {   // the view's camera source of this frame
@@ -1855,7 +1920,13 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     auto launch_frame = [&](bool timing) {
         const bool pdl = pdl_frame && !timing;
         if (fd_on) IM_LAUNCH(k_mfeed_begin, 1, 32, 0, st, h->feed.dev);
-        if (src_mode >= 2) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
+        if (from_lio) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
+        if (depth) {
+            auto& D = h->dep;
+            IM_LAUNCH(k_depth_count, D.nb, DF_BLOCK, 0, st, (const DepthFrame*)D.d_df, D.blk);
+            IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)D.blk, D.nb, D.blk_off, (int*)nullptr, 0, (int*)nullptr);
+            IM_LAUNCH(k_depth_emit, D.nb, DF_BLOCK, 0, st, (const DepthFrame*)D.d_df, (const int*)D.blk_off, D.nb, P.append_target, h->d_dyn, D.pts, D.n);
+        }
         IM_LAUNCH_PDL(pdl && src_mode >= 2, k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[1], st);
         IM_LAUNCH_PDL(pdl, k_cand_init, g_cand, 128, 0, st, h->M, P, F);
@@ -1926,6 +1997,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     if (rf_on) h->rf.last_frame = F.frame;
     if (vw_on) h->vw.last_frame = F.frame;
     if (chg_on) h->chg.last_frame = F.frame;
+    if (depth) h->dep.last_frame = F.frame;
     if (fd_on) return mesh_feed_commit(h, F.frame);
     return IMMESH_OK;
 }
@@ -1970,6 +2042,89 @@ int immesh_mesh_push_frame_from_lio(immesh_mesh_t* h, immesh_lio_t* lio, const f
 int immesh_mesh_push_frame_from_lio_async(immesh_mesh_t* h, immesh_lio_t* lio, const float* body_xyz, int n, int on_device) {
     if (!lio) return im_fail(IMMESH_E_INVALID, "null lio handle");
     return mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio, IMMESH_MFEED_KIND_FROM_LIO_ASYNC, true);
+}
+
+// ---- depth-camera frames (include/immesh_b200.h, immesh_depth_frame)
+static bool all_finite(const double* v, int n) {
+    for (int i = 0; i < n; ++i) if (!std::isfinite(v[i])) return false;
+    return true;
+}
+// the image and camera of f checked and turned into the kernels' DepthFrame; the handle's depth buffers allocated by the first frame
+static int depth_source(immesh_mesh* h, const immesh_depth_frame* f, const void* img, int on_device, DepthSrc* src, int* n_sampled) {
+    if (!h || !f || !img) return im_fail(IMMESH_E_INVALID, "depth frame: null argument");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "depth frame: a sharded mesh handle takes world-frame points only");
+    if (f->format != IMMESH_DEPTH_F32 && f->format != IMMESH_DEPTH_U16) return im_fail(IMMESH_E_INVALID, "depth frame: unknown format");
+    if (f->kind != IMMESH_DEPTH_PLANAR && f->kind != IMMESH_DEPTH_RANGE) return im_fail(IMMESH_E_INVALID, "depth frame: unknown kind");
+    const int bpp = depth_bytes_per_pixel(f->format);
+    if (f->width < 1 || f->height < 1 || f->stride < 1) return im_fail(IMMESH_E_INVALID, "depth frame: width, height and stride must be >= 1");
+    const long long pitch = f->pitch_bytes ? f->pitch_bytes : (long long)f->width * bpp;
+    if (pitch < (long long)f->width * bpp || pitch % bpp || (uintptr_t)img % bpp)
+        return im_fail(IMMESH_E_INVALID, "depth frame: the pitch is below the row's bytes, or the pitch or the image is not aligned to the pixel size");
+    if (!std::isfinite(f->fx) || !std::isfinite(f->fy) || f->fx == 0.0 || f->fy == 0.0 || !std::isfinite(f->cx) || !std::isfinite(f->cy) ||
+        !all_finite(f->cam_R, 9) || !all_finite(f->cam_t, 3))
+        return im_fail(IMMESH_E_INVALID, "depth frame: fx and fy must be finite and non-zero, cx, cy, cam_R and cam_t finite");
+    if (!(0.0 <= f->z_min && f->z_min < f->z_max && f->z_max < INFINITY)) return im_fail(IMMESH_E_INVALID, "depth frame: needs 0 <= z_min < z_max < inf");
+    if (f->format == IMMESH_DEPTH_U16 && !(f->depth_scale > 0.0 && std::isfinite(f->depth_scale)))
+        return im_fail(IMMESH_E_INVALID, "depth frame: a u16 image needs a positive, finite depth_scale");
+    const int sw = depth_sampled(f->width, f->stride), sh = depth_sampled(f->height, f->stride);
+    if ((long long)sw * sh > h->max_frame_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than max_frame_points");
+    auto& D = h->dep;
+    if (!D.pts) {
+        immesh::MemSet dev, pinned{immesh::MemSet::Pinned};
+        const int nb = (h->max_frame_points + DF_BLOCK - 1) / DF_BLOCK;
+        cudaError_t e = dev.alloc(&D.d_df, 1);
+        if (e == cudaSuccess) e = pinned.alloc(&D.h_df, IM_SLOTS);
+        if (e == cudaSuccess) e = dev.alloc(&D.pts, (size_t)h->max_frame_points * 3);
+        if (e == cudaSuccess) e = dev.alloc(&D.n, 1, 0);
+        if (e == cudaSuccess) e = dev.alloc(&D.blk, (size_t)nb);
+        if (e == cudaSuccess) e = dev.alloc(&D.blk_off, (size_t)nb + 1);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            D = immesh_mesh::Depth();
+            return im_fail(IMMESH_E_CAPACITY, "depth frame: out of device or pinned memory for its buffers");
+        }
+        D.nb = nb;
+        D.dev = std::move(dev);
+        D.pinned = std::move(pinned);
+    }
+    DepthFrame& d = src->df;
+    std::memset(&d, 0, sizeof(d));
+    d.img = static_cast<const unsigned char*>(img);
+    d.row_bytes = (long long)f->stride * pitch;
+    d.col_bytes = (long long)f->stride * bpp;
+    d.sw = sw; d.sh = sh; d.stride = f->stride; d.format = f->format; d.kind = f->kind;
+    d.depth_scale = f->depth_scale; d.fx = f->fx; d.fy = f->fy; d.cx = f->cx; d.cy = f->cy; d.z_min = f->z_min; d.z_max = f->z_max;
+    std::memcpy(d.R, f->cam_R, sizeof(d.R));
+    std::memcpy(d.t, f->cam_t, sizeof(d.t));
+    src->host_img = on_device ? nullptr : static_cast<const unsigned char*>(img);
+    src->pitch = pitch;
+    src->bpp = bpp;
+    *n_sampled = sw * sh;
+    return IMMESH_OK;
+}
+int immesh_mesh_push_depth(immesh_mesh_t* h, const immesh_depth_frame* f, const void* depth, int on_device) {
+    DepthSrc src;
+    int n = 0, rc = depth_source(h, f, depth, on_device, &src, &n);
+    if (!rc) rc = mesh_enqueue(h, nullptr, n, f->cam_t, 4, nullptr, IMMESH_MFEED_KIND_DEPTH, false, &src);
+    return rc ? rc : mesh_wait_impl(h, true);
+}
+int immesh_mesh_push_depth_async(immesh_mesh_t* h, const immesh_depth_frame* f, const void* depth, int on_device) {
+    DepthSrc src;
+    int n = 0;
+    const int rc = depth_source(h, f, depth, on_device, &src, &n);
+    return rc ? rc : mesh_enqueue(h, nullptr, n, f->cam_t, 4, nullptr, IMMESH_MFEED_KIND_DEPTH, true, &src);
+}
+int immesh_mesh_depth_points(immesh_mesh_t* h, float* xyz, int cap, int* n) {
+    if (!h || !n || cap < 0 || (cap > 0 && !xyz)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (!h->dep.last_frame) return im_fail(IMMESH_E_INVALID, "no depth frame was pushed");
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    int c = 0;
+    IM_CUDA(cudaMemcpy(&c, h->dep.n, sizeof(int), cudaMemcpyDeviceToHost));
+    *n = c;
+    if (cap == 0) return IMMESH_OK;
+    if (c > cap) return im_fail(IMMESH_E_CAPACITY, "more depth points than cap");
+    if (c > 0) IM_CUDA(cudaMemcpy(xyz, h->dep.pts, (size_t)c * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+    return IMMESH_OK;
 }
 // device-side timing of a pipelined batch: begin mark on the localization stream, end mark behind BOTH streams
 int immesh_pipeline_mark_begin(immesh_lio_t* lio) {
@@ -2111,7 +2266,14 @@ int immesh_mesh_counts(immesh_mesh_t* h, int64_t* out) {
 int immesh_mesh_work_stats(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const int* c = h->last_cnt;
-    out[0] = h->F.m; out[1] = c[IM_MC_STAT_GATHERED]; out[2] = c[IM_MC_STAT_QUERIES]; out[3] = c[IM_MC_STAT_DILATED]; out[4] = c[IM_MC_STAT_FACETS];
+    int m = h->F.m;
+    if (h->dep.last_frame && h->dep.last_frame == h->frame_counter) {   // the newest frame is a depth frame: its m is set on the device
+        FrameDyn d;
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        IM_CUDA(cudaMemcpy(&d, h->d_dyn, sizeof(d), cudaMemcpyDeviceToHost));
+        m = d.m;
+    }
+    out[0] = m; out[1] = c[IM_MC_STAT_GATHERED]; out[2] = c[IM_MC_STAT_QUERIES]; out[3] = c[IM_MC_STAT_DILATED]; out[4] = c[IM_MC_STAT_FACETS];
     out[5] = c[IM_MC_WORK_FRONT] + c[IM_MC_WORK_BACK]; out[6] = c[IM_MC_ADD]; out[7] = c[IM_MC_REMOVE];
     return IMMESH_OK;
 }

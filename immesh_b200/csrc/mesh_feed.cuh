@@ -26,7 +26,7 @@ namespace immesh {
 // per-frame inputs of the feed's kernels (one H2D copy per frame from a pinned slot): the launch sequence stays the same for every frame
 struct MeshFeedDyn {
     long long frame;      // the handle's frame number
-    long long n;          // N_POINTS
+    long long n;          // N_POINTS (-1: the FrameDyn's, a depth frame's count set on the device; k_mfeed_head fills it in)
     int step;             // STEP
     int kind;             // IMMESH_MFEED_KIND_*
     int has_rot;          // 1: handed over by a localization handle (the pose is in the camera ring)

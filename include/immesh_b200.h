@@ -398,6 +398,55 @@ int immesh_mesh_push_frame_from_lio(immesh_mesh_t* h, immesh_lio_t* lio, const f
  * localization stream) and meshed on the mesh stream while the next scan is being localised; immesh_mesh_wait drains. */
 int immesh_mesh_push_frame_from_lio_async(immesh_mesh_t* h, immesh_lio_t* lio, const float* body_xyz, int n, int on_device);
 int immesh_mesh_wait(immesh_mesh_t* h);
+/* Depth-camera frames: one depth image unprojected on the device, inside the frame's own launch sequence, into the world-frame points
+ * of an ordinary mesh frame -- the ImMesh paper's depth-image workload (AirSim 640 x 480 depth streams turned into point clouds, Table VI),
+ * without a host pass over the pixels or a copy of the cloud.
+ *   Sampling: pixel (u, v) is sampled iff u % stride == 0 and v % stride == 0; the valid samples become the frame's points in ascending
+ *     pixel order (v major, u minor).  The image is width x height pixels with rows pitch_bytes apart (0: tight), float32 metres
+ *     (IMMESH_DEPTH_F32) or uint16 counts of depth_scale metres (IMMESH_DEPTH_U16).
+ *   Arithmetic, float64 in this order without FMA:
+ *     d = raw (f32) or raw * depth_scale (u16); a u16 raw == 0 and a non-finite f32 raw are invalid;
+ *     a = (u - cx) / fx, b = (v - cy) / fy;
+ *     z = d (IMMESH_DEPTH_PLANAR: depth along the optical axis, AirSim DepthPlanar) or
+ *     z = d / sqrt((a*a + b*b) + 1) (IMMESH_DEPTH_RANGE: distance along the ray, AirSim DepthPerspective);
+ *     x = a * z, y = b * z; the pixel is valid iff z_min <= z <= z_max;
+ *     w_i = (float)(((R[i][0]*x + R[i][1]*y) + R[i][2]*z) + t[i]) with R = cam_R (row-major), t = cam_t.
+ *   Axes: cam_R / cam_t map the camera frame to the world, with OpenCV axes (x right, y down, z forward).  A caller whose pose uses
+ *     the OpenGL convention (y up, z backward) multiplies its rotation on the right by diag(1, -1, -1) first.
+ *   The frame is then immesh_mesh_push_frame of those points at pose_t = cam_t (the camera centre is the sensor position of
+ *     correct_triangle_index): its point count, append_point_step and candidate count are set on the device from the valid count, with
+ *     the rule of immesh_mesh_push_frame.  The change feed, the frame feed (KIND = IMMESH_MFEED_KIND_DEPTH; N_POINTS and STEP are the
+ *     device values), the reinforcement and the queued view follow it as any frame.
+ * immesh_mesh_push_depth(h, f, depth, on_device): blocking, as immesh_mesh_push_frame.  on_device != 0: depth is a device pointer, read
+ *   in place.  A host image is staged, sampled pixels only, through the handle's pinned slots.
+ * immesh_mesh_push_depth_async: queued (graph-replayed, no host synchronisation); immesh_mesh_wait drains it and returns its status.
+ *   A device image must stay unchanged until the frame has run.
+ * immesh_mesh_depth_points(h, xyz, cap, n): blocking; the newest depth frame's world points, *n of them.  cap = 0: a count query;
+ *   *n > cap: IMMESH_E_CAPACITY (nothing written).  No depth frame pushed yet: IMMESH_E_INVALID.
+ * Errors: IMMESH_E_INVALID for a null or misaligned image, fx or fy zero or non-finite, cx, cy, cam_R or cam_t non-finite, width or
+ *   height < 1, a pitch below the row's bytes or not a multiple of the pixel size, stride < 1, an unknown format or kind,
+ *   !(0 <= z_min < z_max < inf), a u16 depth_scale that is not positive and finite, or a sharded handle; IMMESH_E_CAPACITY when the
+ *   sampled pixels exceed max_frame_points; otherwise the codes of immesh_mesh_push_frame (e.g. IMMESH_E_RANGE far from cam_t). */
+#define IMMESH_DEPTH_F32 0
+#define IMMESH_DEPTH_U16 1
+#define IMMESH_DEPTH_PLANAR 0
+#define IMMESH_DEPTH_RANGE 1
+typedef struct immesh_depth_frame {
+    int width, height;
+    int64_t pitch_bytes;  /* bytes between rows; 0 = width * bytes per pixel */
+    int format;           /* IMMESH_DEPTH_F32 or IMMESH_DEPTH_U16 */
+    int kind;             /* IMMESH_DEPTH_PLANAR or IMMESH_DEPTH_RANGE */
+    double depth_scale;   /* metres per u16 count (ignored for f32) */
+    double fx, fy, cx, cy;
+    double z_min, z_max;  /* valid z range, metres: 0 <= z_min < z_max < inf */
+    int stride;           /* >= 1: every stride-th pixel of every stride-th row */
+    int pad;
+    double cam_R[9];      /* camera to world, row-major, OpenCV camera axes */
+    double cam_t[3];      /* camera centre in the world */
+} immesh_depth_frame;
+int immesh_mesh_push_depth(immesh_mesh_t* h, const immesh_depth_frame* f, const void* depth, int on_device);
+int immesh_mesh_push_depth_async(immesh_mesh_t* h, const immesh_depth_frame* f, const void* depth, int on_device);
+int immesh_mesh_depth_points(immesh_mesh_t* h, float* xyz /*[cap][3]*/, int cap, int* n);
 /* host time (ms) the queueing calls spent blocked on a busy staging slot (back-pressure from the device, not work) since the
  * last call: out[0] localization handle, out[1] meshing handle; either handle may be NULL */
 int immesh_host_wait_ms(immesh_lio_t* lio, immesh_mesh_t* h, double* out /*[2]*/);
@@ -688,8 +737,8 @@ int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames /
  * per frame what the reference publishes -- the mesh_cost_time.log fields, the trajectory, the reinforced LiDAR points, a video of
  * the viewer -- without draining.  Records are numbered by the handle's frame numbers (those of immesh_mesh_changes and of
  * immesh_mesh_view_image's frame_out): frame f in header slot (f - 1) % max_frames; the frames queued after the enable are recorded.
- *   Every frame of immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async and immesh_mesh_reconstruct_from_pointcloud records one
- *     frame.  A batched frame (immesh_mesh_push_frame_batched, _reconstruct_from_pointcloud_batched) records its header and pose, with
+ *   Every frame of immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async, immesh_mesh_push_depth, _depth_async and
+ *     immesh_mesh_reconstruct_from_pointcloud records one frame.  A batched frame (immesh_mesh_push_frame_batched, _reconstruct_from_pointcloud_batched) records its header and pose, with
  *     no points and no image (the reinforcement and the view do not follow batched frames).
  *   header (IMMESH_MESH_FEED_HDR int64, IMMESH_MFEED_*): FRAME; KIND (IMMESH_MFEED_KIND_*); N_POINTS and STEP (append_point_step);
  *     the eight values of immesh_mesh_counts right after the frame (COUNTS + 0..7); ERR (the frame's IM_MERR flags); HAS_ROTATION (1:
@@ -755,6 +804,7 @@ typedef struct {
 #define IMMESH_MFEED_KIND_RECONSTRUCT 4
 #define IMMESH_MFEED_KIND_BATCHED 5
 #define IMMESH_MFEED_KIND_RECONSTRUCT_BATCHED 6
+#define IMMESH_MFEED_KIND_DEPTH 7   /* immesh_mesh_push_depth and _async */
 int immesh_mesh_feed_enable(immesh_mesh_t* h, const immesh_mesh_feed_config* cfg /* NULL: off */);
 int immesh_mesh_feed(immesh_mesh_t* h, int64_t since_frame, int wait, int64_t* frames /*[cap_frames][22]*/, double* poses /*[cap_frames][36] or NULL*/,
                      int cap_frames, float* points /*[cap_rows][3] or NULL*/, int32_t* pixels /*[cap_rows] or NULL*/, int64_t cap_rows, int64_t* counts /*[4]*/);
