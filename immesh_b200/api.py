@@ -63,7 +63,7 @@ class _FeedCfg(C.Structure):
 
 FEED_HDR = 12   # IMMESH_LIO_FEED_HDR: the header columns of a recorded scan, in this order
 FEED_HDR_KEYS = ("scan", "kind", "branch", "iters", "matches", "converged", "err", "row_begin", "row_effect_end", "row_end", "source", "rows_lost")
-FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i")   # IMMESH_FEED_KIND_*
+FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i", "depth")   # IMMESH_FEED_KIND_*
 
 
 MARKER_HDR = 10   # IMMESH_LIO_FEED_MARKER_HDR: the header columns of a scan's plane-marker record, in this order
@@ -78,13 +78,20 @@ MESH_FEED_HDR = 22    # IMMESH_MESH_FEED_HDR: the header columns of a recorded m
 MESH_FEED_HDR_KEYS = ("frame", "kind", "n_points", "step", "n_vertices", "n_triangles", "new_vertices", "voxels_meshed", "n_add", "n_remove", "n_voxels",
                       "n_activated", "err", "has_rotation", "t_begin_ns", "t_end_ns", "row_begin", "row_end", "rows_lost", "rf", "img_begin", "img_end")
 MESH_FEED_POSE = 36   # IMMESH_MESH_FEED_POSE: frame pose, reinforcement camera, view camera; each a row-major R then t
-MESH_FEED_KINDS = ("push", "push_dev", "from_lio", "from_lio_async", "reconstruct", "batched", "reconstruct_batched", "depth")   # IMMESH_MFEED_KIND_*
+MESH_FEED_KINDS = ("push", "push_dev", "from_lio", "from_lio_async", "reconstruct", "batched", "reconstruct_batched", "depth",
+                   "from_lio_async_dev_n")   # IMMESH_MFEED_KIND_*
 
 
 class _DepthFrame(C.Structure):
     _fields_ = [("width", C.c_int), ("height", C.c_int), ("pitch_bytes", C.c_int64), ("format", C.c_int), ("kind", C.c_int), ("depth_scale", C.c_double),
                 ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double), ("z_min", C.c_double), ("z_max", C.c_double),
                 ("stride", C.c_int), ("pad", C.c_int), ("cam_R", C.c_double * 9), ("cam_t", C.c_double * 3)]
+
+
+def _sampled(f: "_DepthFrame") -> int:
+    """the sampled pixels of a depth frame: ceil(width / stride) * ceil(height / stride)"""
+    s = max(f.stride, 1)   # (stride < 1 is refused by the call)
+    return -(-f.width // s) * -(-f.height // s)
 
 
 DEPTH_FORMATS = {"f32": 0, "u16": 1}        # IMMESH_DEPTH_F32, IMMESH_DEPTH_U16
@@ -205,6 +212,7 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_push_depth", [vp, C.POINTER(_DepthFrame), vp, C.c_int]),
         ("immesh_mesh_push_depth_async", [vp, C.POINTER(_DepthFrame), vp, C.c_int]),
         ("immesh_mesh_depth_points", [vp, fp, C.c_int, ip]),
+        ("immesh_mesh_push_frame_from_lio_async_dev_n", [vp, vp, vp, C.c_int, vp]),
         ("immesh_pipeline_mark_begin", [vp]),
         ("immesh_pipeline_mark_end", [vp, vp, dp]),
         ("immesh_mesh_work_stats", [vp, C.POINTER(C.c_int64)]),
@@ -269,6 +277,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_voxelgrid_input_points", [vp]),
         ("immesh_lio_step_async_raw", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_double, C.c_double, C.c_double]),
         ("immesh_lio_step_async_dev_n", [vp, vp, C.c_int, vp, C.c_double, C.c_double, C.c_double]),
+        ("immesh_frontend_prepare_depth", [vp, C.POINTER(_DepthFrame), vp, C.c_int, C.c_int, C.c_double, fp, C.c_int, ip]),
+        ("immesh_lio_step_async_depth", [vp, vp, C.POINTER(_DepthFrame), vp, C.c_int, C.c_int, C.c_double, C.c_float, C.c_double, C.c_double, C.c_double]),
+        ("immesh_voxelgrid_input_count", [vp]),
         ("immesh_imu_create", [C.POINTER(_ImuCfg), C.POINTER(vp)]),
         ("immesh_imu_destroy", [vp]),
         ("immesh_imu_reset", [vp, dp, C.c_double, C.c_double, dp, dp]),
@@ -296,6 +307,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         lib.immesh_voxelgrid_device_points.restype = C.c_void_p
     if hasattr(lib, "immesh_voxelgrid_input_points"):
         lib.immesh_voxelgrid_input_points.restype = C.c_void_p
+    if hasattr(lib, "immesh_voxelgrid_input_count"):
+        lib.immesh_voxelgrid_input_count.restype = C.c_void_p
     if hasattr(lib, "immesh_launch_count"):
         lib.immesh_launch_count.restype = C.c_longlong
     if hasattr(lib, "immesh_last_error"):
@@ -741,6 +754,12 @@ class Mesh:
             n = a.shape[0]
             ptr = C.cast(p, C.c_void_p)
         _check(self.lib, self.lib.immesh_mesh_push_frame_from_lio_async(self._h, lio._h, ptr, n, 1 if on_device else 0), "mesh_push_frame_from_lio_async")
+
+    def push_frame_from_lio_async_dev_n(self, lio: "Lio", d_body, n_max: int, d_n: int):
+        """push_frame_from_lio_async of a device cloud whose count is device resident (int CUDA address d_n, *d_n <= n_max): e.g.
+        input_points() / input_count() of a VoxelGrid after step_async_depth, with n_max its sampled pixels"""
+        _check(self.lib, self.lib.immesh_mesh_push_frame_from_lio_async_dev_n(self._h, lio._h, C.c_void_p(int(d_body)), int(n_max), C.c_void_p(int(d_n))),
+               "mesh_push_frame_from_lio_async_dev_n")
 
     def wait(self):
         _check(self.lib, self.lib.immesh_mesh_wait(self._h), "mesh_wait")
@@ -1250,6 +1269,33 @@ class VoxelGrid:
 
     def input_points(self) -> int:
         return int(self.lib.immesh_voxelgrid_input_points(self._h) or 0)
+
+    def input_count(self) -> int:
+        """CUDA address of the device count of input_points() after a depth entry point (0 otherwise)"""
+        return int(self.lib.immesh_voxelgrid_input_count(self._h) or 0)
+
+    def prepare_depth(self, depth, cam: DepthCamera, cam_R=np.eye(3), cam_t=np.zeros(3), point_filter_num=1, blind=0.0, on_device=False, shape=None,
+                      fmt="f32", pitch_bytes=0):
+        """The localization's sensor-frame cloud of one depth image (immesh_frontend_prepare_depth; blocking): unprojected with the
+        camera-to-sensor mount cam_R / cam_t, every point_filter_num-th valid sample kept, points closer than blind dropped.  It stays on
+        the device (input_points(), input_count()); returned as float32[n][3] in ascending pixel order."""
+        f, ptr, _keep = Mesh._depth_args(cam, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device)
+        out = np.zeros((_sampled(f), 3), dtype=np.float32)   # the sampled pixels bound the count
+        n = C.c_int(0)
+        _check(self.lib, self.lib.immesh_frontend_prepare_depth(self._h, C.byref(f), ptr, 1 if on_device else 0, int(point_filter_num), float(blind),
+                                                                out.ctypes.data_as(C.POINTER(C.c_float)), out.shape[0], C.byref(n)), "frontend_prepare_depth")
+        return out[:n.value].copy()
+
+    def step_async_depth(self, lio: "Lio", depth, cam: DepthCamera, leaf: float, cam_R=np.eye(3), cam_t=np.zeros(3), point_filter_num=1, blind=0.0,
+                         dt=0.0, cov_gyr=0.1, cov_acc=0.1, on_device=False, shape=None, fmt="f32", pitch_bytes=0) -> int:
+        """The queued depth chain (immesh_lio_step_async_depth): the image's filtered cloud -> VoxelGrid(leaf) -> lio.step_async, every
+        count on the device.  Returns the sampled pixels, the n_max of Mesh.push_frame_from_lio_async_dev_n(lio, input_points(),
+        n_max, input_count())."""
+        f, ptr, _keep = Mesh._depth_args(cam, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device)
+        _check(self.lib, self.lib.immesh_lio_step_async_depth(lio._h, self._h, C.byref(f), ptr, 1 if on_device else 0, int(point_filter_num), float(blind),
+                                                              C.c_float(leaf), dt, cov_gyr, cov_acc), "lio_step_async_depth")
+        lio._last_n = _sampled(f)
+        return lio._last_n
 
     def step_async_raw(self, lio: "Lio", pts, leaf: float, dt=0.0, calib_laser=False, cov_gyr=0.1, cov_acc=0.1, n=None, stride=3, on_device=False):
         """The device-resident front-end chain: [calibration] -> VoxelGrid -> lio.step_async, no host round trip in between."""

@@ -246,6 +246,20 @@ def build_depth_frame(force=False):
     return EMU_DEPTH_FRAME
 
 
+EMU_DEPTH_LIO = os.path.join(_ROOT, "tests", "depth_lio", "libimmesh_emu_depth_lio.so")
+
+
+def build_depth_lio(force=False):
+    """tests/depth_lio: the localization's depth filter (immesh_b200/csrc/depth_frame.cuh: depth_point, depth_keep) with the front-end
+    kernels' multi-pass block compaction restated on the host"""
+    src = os.path.join(_ROOT, "tests", "depth_lio", "emu_depth_lio.cpp")
+    deps = [src, os.path.join(CSRC, "depth_frame.cuh"), os.path.join(CSRC, "hd_math.cuh"), os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_DEPTH_LIO, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_DEPTH_LIO, src])
+    return EMU_DEPTH_LIO
+
+
 LOCAL_MAP_DIR = os.path.join(_ROOT, "tests", "local_map")
 EMU_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "libimmesh_emu_local_map.so")
 ORACLE_LOCAL_MAP = os.path.join(LOCAL_MAP_DIR, "liborc_local_map.so")
@@ -299,6 +313,7 @@ def build_all(force=False):
     build_rs_check(force)
     build_eval(force)
     build_depth_frame(force)
+    build_depth_lio(force)
     build_local_map(force)
     build_dev_mem(force)
     build_ref()

@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <vector>
@@ -31,7 +32,7 @@ using immesh::im_fail;
 namespace {
 
 #include "radix_sort.cuh"
-
+#include "depth_kernels.cuh"
 
 struct VgGrid {
     int mn[3], mx[3];        // ordered-int encodings of the float box (atomicMin / atomicMax targets)
@@ -50,7 +51,9 @@ __global__ void k_vg_reset(VgGrid* g) {
     if (threadIdx.x < 3) { g->mn[threadIdx.x] = 0x7fffffff; g->mx[threadIdx.x] = (int)0x80000000; }
     if (threadIdx.x == 0) { g->too_small = 0; g->n_finite = 0; g->m_out = 0; }
 }
-__global__ void __launch_bounds__(VG_THREADS) k_vg_minmax(const float* __restrict__ pts, int n, VgGrid* g) {
+// n_dev (or null): the kernels from k_vg_minmax to k_vg_copy_if_small read the count there; n is then its upper bound, which sizes the grids
+__global__ void __launch_bounds__(VG_THREADS) k_vg_minmax(const float* __restrict__ pts, int n, const int* n_dev, VgGrid* g) {
+    if (n_dev) n = *n_dev;
     float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
     int cnt = 0;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -90,7 +93,9 @@ __global__ void k_vg_setup(VgGrid* g, float inv) {
     }
     g->mul[0] = 1; g->mul[1] = g->div_b[0]; g->mul[2] = g->div_b[0] * g->div_b[1];
 }
-__global__ void __launch_bounds__(VG_THREADS) k_vg_keys(const float* __restrict__ pts, int n, const VgGrid* g, float inv, unsigned int* keys, unsigned int* vals) {
+__global__ void __launch_bounds__(VG_THREADS) k_vg_keys(const float* __restrict__ pts, int n, const int* n_dev, const VgGrid* g, float inv, unsigned int* keys,
+                                                         unsigned int* vals) {
+    if (n_dev) n = *n_dev;
     const int mb0 = g->min_b[0], mb1 = g->min_b[1], mb2 = g->min_b[2], m1 = g->mul[1], m2 = g->mul[2];
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float x = pts[3 * (size_t)i], y = pts[3 * (size_t)i + 1], z = pts[3 * (size_t)i + 2];
@@ -105,7 +110,8 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_keys(const float* __restrict_
 }
 
 // ---- runs of equal idx -> centroids
-__global__ void __launch_bounds__(VG_THREADS) k_vg_heads(const unsigned int* __restrict__ keys, int n, int* tile_heads) {
+__global__ void __launch_bounds__(VG_THREADS) k_vg_heads(const unsigned int* __restrict__ keys, int n, const int* n_dev, int* tile_heads) {
+    if (n_dev) n = *n_dev;
     __shared__ int s_cnt;
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
@@ -125,7 +131,9 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_heads(const unsigned int* __r
     if (threadIdx.x == 0) tile_heads[blockIdx.x] = s_cnt;
 }
 // record where every run starts: head_pos[slot] (the sums are then taken by k_vg_centroid_warp)
-__global__ void __launch_bounds__(VG_THREADS) k_vg_head_pos(const unsigned int* __restrict__ keys, int n, const int* __restrict__ tile_base, int* head_pos) {
+__global__ void __launch_bounds__(VG_THREADS) k_vg_head_pos(const unsigned int* __restrict__ keys, int n, const int* n_dev, const int* __restrict__ tile_base,
+                                                             int* head_pos) {
+    if (n_dev) n = *n_dev;
     __shared__ int s_warp[VG_THREADS / 32];
     __shared__ int s_run;
     if (threadIdx.x == 0) s_run = tile_base[blockIdx.x];
@@ -187,11 +195,13 @@ __global__ void __launch_bounds__(VG_THREADS) k_vg_centroid_warp(const float* __
         }
     }
 }
-__global__ void k_vg_finish(VgGrid* g, const int* total_heads, int n) {
-    if (threadIdx.x == 0) g->m_out = g->too_small ? n : *total_heads;
+__global__ void k_vg_finish(VgGrid* g, const int* total_heads, int n, const int* n_dev) {
+    if (threadIdx.x == 0) g->m_out = g->too_small ? (n_dev ? *n_dev : n) : *total_heads;
 }
-__global__ void __launch_bounds__(VG_THREADS) k_vg_copy_if_small(const float* __restrict__ pts, int n, const VgGrid* g, float* out, const float* __restrict__ inten, float* out_i) {
+__global__ void __launch_bounds__(VG_THREADS) k_vg_copy_if_small(const float* __restrict__ pts, int n, const int* n_dev, const VgGrid* g, float* out,
+                                                                  const float* __restrict__ inten, float* out_i) {
     if (!g->too_small) return;
+    if (n_dev) n = *n_dev;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < 3 * (size_t)n; i += (size_t)gridDim.x * blockDim.x) {
         out[i] = pts[i];
         if (inten && i < (size_t)n) out_i[i] = inten[i];
@@ -238,6 +248,16 @@ struct immesh_voxelgrid {
     float* d_out_i = nullptr;    // [max_points] intensity of the down-sampled cloud d_out
     float* h_out_i = nullptr;    // pinned [max_points]
     long long calls = 0;         // calls that queued work on the handle (immesh_lio_frontend_cloud: has vg run another call since)
+    // depth images (immesh_frontend_prepare_depth, immesh_lio_step_async_depth), allocated by the first of them: per ring slot, the
+    // image's DepthFrame and the count of the filtered cloud the kernels write into d_in_ring[k]
+    struct Depth {
+        immesh::DepthFrame* d_df = nullptr;   // [8]
+        immesh::DepthFrame* h_df = nullptr;   // pinned [8]
+        int* d_n = nullptr;                   // [8] (immesh_voxelgrid_input_count)
+        int* h_n = nullptr;                   // pinned: a count read back by immesh_frontend_prepare_depth
+        int *blk = nullptr, *kblk = nullptr;  // [nb + 1] valid and kept samples per block of DF_BLOCK sampled pixels, scanned in place
+        int has_n[8] = {};                    // 1: d_in_ring[k] holds a depth cloud, counted in d_n[k]
+    } dep;
     immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // every buffer above
 };
 
@@ -324,25 +344,26 @@ static bool records_ok(int stride, int icol, int tcol) {
 }
 
 // queue the filter's launch sequence for the packed device cloud d_pts on stream st (no host synchronisation); inten != nullptr:
-// the points' intensity ([n]), averaged into d_out_i
-static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf, cudaStream_t st, const float* inten = nullptr) {
+// the points' intensity ([n]), averaged into d_out_i.  n_dev != nullptr: the count is read on the device (*n_dev <= n; the grids and
+// the sort's scratch cover n)
+static int vg_enqueue(immesh_voxelgrid* h, const float* d_pts, int n, float leaf, cudaStream_t st, const float* inten = nullptr, const int* n_dev = nullptr) {
     ++h->calls;
     float* out_i = inten ? h->d_out_i : nullptr;
     const float inv = 1.0f / leaf;
     const int nb = (n + VG_TILE - 1) / VG_TILE;
     const int gs = std::min(nb * (VG_TILE / VG_THREADS), h->n_sm * 8);
     IM_LAUNCH(k_vg_reset, 1, 32, 0, st, h->d_grid);
-    IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d_pts, n, h->d_grid);
+    IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d_pts, n, n_dev, h->d_grid);
     IM_LAUNCH(k_vg_setup, 1, 32, 0, st, h->d_grid, inv);
-    IM_LAUNCH(k_vg_keys, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, inv, h->d_k[0], h->d_v[0]);
-    const int cur = rs_sort_passes(st, h->d_k, h->d_v, 0, n, 4, h->d_hist);
-    IM_LAUNCH(k_vg_heads, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, h->d_tile);
+    IM_LAUNCH(k_vg_keys, gs, VG_THREADS, 0, st, d_pts, n, n_dev, (const VgGrid*)h->d_grid, inv, h->d_k[0], h->d_v[0]);
+    const int cur = rs_sort_passes(st, h->d_k, h->d_v, 0, n, 4, h->d_hist, n_dev);
+    IM_LAUNCH(k_vg_heads, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, n_dev, h->d_tile);
     IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, h->d_tile, nb, h->d_tile + h->nblocks_max);
-    IM_LAUNCH(k_vg_head_pos, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, (const int*)h->d_tile, h->d_head);
+    IM_LAUNCH(k_vg_head_pos, nb, VG_THREADS, 0, st, (const unsigned int*)h->d_k[cur], n, n_dev, (const int*)h->d_tile, h->d_head);
     IM_LAUNCH(k_vg_centroid_warp, h->n_sm * 4, VG_THREADS, 0, st, d_pts, (const unsigned int*)h->d_v[cur], (const int*)h->d_head,
               (const int*)(h->d_tile + h->nblocks_max), (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
-    IM_LAUNCH(k_vg_finish, 1, 32, 0, st, h->d_grid, (const int*)(h->d_tile + h->nblocks_max), n);
-    IM_LAUNCH(k_vg_copy_if_small, gs, VG_THREADS, 0, st, d_pts, n, (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
+    IM_LAUNCH(k_vg_finish, 1, 32, 0, st, h->d_grid, (const int*)(h->d_tile + h->nblocks_max), n, n_dev);
+    IM_LAUNCH(k_vg_copy_if_small, gs, VG_THREADS, 0, st, d_pts, n, n_dev, (const VgGrid*)h->d_grid, h->d_out, inten, out_i);
     IM_CUDA(cudaGetLastError());
     return IMMESH_OK;
 }
@@ -395,7 +416,7 @@ int immesh_voxelgrid_leaf_too_small(immesh_voxelgrid_t* h, const float* xyz, int
             d = h->d_in;
         }
         const int gs = std::min(((m + VG_TILE - 1) / VG_TILE) * (VG_TILE / VG_THREADS), h->n_sm * 8);
-        IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d, m, h->d_grid);
+        IM_LAUNCH(k_vg_minmax, gs, VG_THREADS, 0, st, d, m, (const int*)nullptr, h->d_grid);
     }
     IM_LAUNCH(k_vg_setup, 1, 32, 0, st, h->d_grid, 1.0f / leaf);
     IM_CUDA(cudaGetLastError());
@@ -417,6 +438,7 @@ static int frontend_pack(immesh_voxelgrid* h, const float* pts, int n, int strid
     ++h->calls;
     h->in_idx = (h->in_idx + 1) & 7;
     h->d_in = h->d_in_ring[h->in_idx];
+    h->dep.has_n[h->in_idx] = 0;
     const float* d_src = pts;
     if (!on_device) {
         const float* src = pts;
@@ -452,6 +474,91 @@ int immesh_frontend_prepare(immesh_voxelgrid_t* h, const float* pts, int n, int 
     return IMMESH_OK;
 }
 const float* immesh_voxelgrid_input_points(immesh_voxelgrid_t* h) { return h ? h->d_in : nullptr; }
+const int* immesh_voxelgrid_input_count(immesh_voxelgrid_t* h) { return h && h->dep.has_n[h->in_idx] ? h->dep.d_n + h->in_idx : nullptr; }
+
+// ---- depth images into the localization (immesh_frontend_prepare_depth, immesh_lio_step_async_depth): the image checked, then the
+// kernels of depth_kernels.cuh queued on st into the next input ring slot -- the filtered sensor-frame cloud and its count, both on the
+// device.  *n_sampled: the sampled pixels, the upper bound of the count.
+static int depth_pack(immesh_voxelgrid* h, const immesh_depth_frame* f, const void* img, int on_device, int point_filter_num, double blind, cudaStream_t st,
+                      int* n_sampled) {
+    if (point_filter_num < 1) return im_fail(IMMESH_E_INVALID, "depth frame: point_filter_num must be >= 1");
+    if (!(blind >= 0.0 && std::isfinite(blind))) return im_fail(IMMESH_E_INVALID, "depth frame: blind must be finite and >= 0");
+    immesh::DepthFrame d;
+    long long pitch = 0;
+    int bpp = 0;
+    if (const char* bad = immesh::depth_frame_setup(f, img, &d, &pitch, &bpp)) return im_fail(IMMESH_E_INVALID, bad);
+    const int ns = d.sw * d.sh;
+    if ((long long)d.sw * d.sh > h->max_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than the VoxelGrid's max_points");
+    auto& D = h->dep;
+    if (!D.d_n) {   // all or nothing: after a failure the handle is as it was
+        const size_t nb = (size_t)(h->max_points + DF_BLOCK - 1) / DF_BLOCK;
+        immesh::MemSet dev, pinned(immesh::MemSet::Pinned);
+        immesh_voxelgrid::Depth b;
+        IM_CUDA(dev.alloc(&b.d_df, 8));
+        IM_CUDA(pinned.alloc(&b.h_df, 8));
+        IM_CUDA(dev.alloc(&b.d_n, 8, 0));
+        IM_CUDA(pinned.alloc(&b.h_n, 1));
+        IM_CUDA(dev.alloc(&b.blk, nb + 1));
+        IM_CUDA(dev.alloc(&b.kblk, nb + 1));
+        D.d_df = b.d_df; D.h_df = b.h_df; D.d_n = b.d_n; D.h_n = b.h_n; D.blk = b.blk; D.kblk = b.kblk;
+        h->dev.take(std::move(dev));
+        h->pinned.take(std::move(pinned));
+    }
+    ++h->calls;
+    h->in_idx = (h->in_idx + 1) & 7;
+    const int k = h->in_idx;
+    h->d_in = h->d_in_ring[k];
+    if (!on_device) {   // the sampled grid, tight, through the pinned staging (sw * sh * bpp <= 4 max_points bytes, within h_raw)
+        if (h->raw_pending) { IM_CUDA(cudaEventSynchronize(h->ev_raw)); h->raw_pending = 0; }   // the previous copy out of the staging buffer
+        unsigned char* hb = reinterpret_cast<unsigned char*>(h->h_raw);
+        immesh::depth_stage_grid(d, static_cast<const unsigned char*>(img), pitch, bpp, hb);
+        IM_CUDA(cudaMemcpyAsync(h->d_raw, hb, (size_t)ns * bpp, cudaMemcpyHostToDevice, st));
+        IM_CUDA(cudaEventRecord(h->ev_raw, st));
+        h->raw_pending = 1;
+        d.img = reinterpret_cast<const unsigned char*>(h->d_raw);
+        d.row_bytes = (long long)d.sw * bpp;
+        d.col_bytes = bpp;
+    }
+    // the pinned slot k was last copied from 8 calls ago, behind which the localization's staging slots have since been waited on
+    D.h_df[k] = d;
+    IM_CUDA(cudaMemcpyAsync(D.d_df + k, D.h_df + k, sizeof(immesh::DepthFrame), cudaMemcpyHostToDevice, st));
+    const int nb = (ns + DF_BLOCK - 1) / DF_BLOCK;
+    const bool filter = point_filter_num > 1 || blind > 0.0;
+    const immesh::DepthFrame* df = D.d_df + k;
+    IM_LAUNCH(k_depth_count, nb, DF_BLOCK, 0, st, df, D.blk);
+    IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, D.blk, nb, D.blk + nb);
+    if (filter) {
+        IM_LAUNCH(k_depth_keep, nb, DF_BLOCK, 0, st, df, (const int*)D.blk, point_filter_num, blind, D.kblk);
+        IM_LAUNCH(k_rs_scan, 1, 1024, 0, st, D.kblk, nb, D.kblk + nb);
+    }
+    IM_LAUNCH(k_depth_emit, nb, DF_BLOCK, 0, st, df, (const int*)D.blk, (const int*)(filter ? D.kblk : D.blk), nb, point_filter_num, blind, 0,
+              (immesh::FrameDyn*)nullptr, h->d_in, D.d_n + k);
+    D.has_n[k] = 1;
+    *n_sampled = ns;
+    return IMMESH_OK;
+}
+
+int immesh_frontend_prepare_depth(immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num, double blind,
+                                  float* out_xyz, int cap, int* n_out) {
+    if (!h || !n_out || cap < 0 || (cap > 0 && !out_xyz)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    *n_out = 0;
+    int ns = 0;
+    int rc = depth_pack(h, f, depth, on_device, point_filter_num, blind, h->stream, &ns);
+    if (rc) return rc;
+    IM_CUDA(cudaGetLastError());
+    IM_CUDA(cudaMemcpyAsync(h->dep.h_n, h->dep.d_n + h->in_idx, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    IM_CUDA(cudaStreamSynchronize(h->stream));
+    const int n = *h->dep.h_n;
+    *n_out = n;
+    if (cap == 0) return IMMESH_OK;
+    if (n > cap) return im_fail(IMMESH_E_CAPACITY, "more filtered points than cap");
+    if (n > 0) {
+        IM_CUDA(cudaMemcpyAsync(h->h_pts, h->d_in, (size_t)n * 3 * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+        IM_CUDA(cudaStreamSynchronize(h->stream));
+        std::memcpy(out_xyz, h->h_pts, (size_t)n * 3 * sizeof(float));
+    }
+    return IMMESH_OK;
+}
 
 int immesh_voxelgrid_filter_i(immesh_voxelgrid_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, float leaf, float* out_xyzi, int* m_out,
                               int* leaf_too_small) {
@@ -520,6 +627,31 @@ int immesh_lio_step_async_raw(immesh_lio_t* lio, immesh_voxelgrid_t* h, const fl
     if (!lio || !h || (!pts && n > 0) || n < 1 || (stride != 3 && stride != 4) || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");
     return immesh_frontend_step_async(lio, h, pts, n, stride, on_device, calib_laser, leaf, dt, cov_gyr, cov_acc, -1, nullptr);
+}
+// The chain of one depth image (the reference's lidar_type 4, imu_en false): unproject + filter -> pcl::VoxelGrid -> predict + IESKF +
+// map update, every count on the device.  A frame with no point left is predicted only (the step's *d_n == 0 path).
+int immesh_lio_step_async_depth(immesh_lio_t* lio, immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num,
+                                double blind, float leaf, double dt, double cov_gyr, double cov_acc) {
+    if (!lio || !h || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_depth runs on a single GPU: the localization handle is sharded");
+    lio->fe_vg = nullptr;
+    cudaStream_t st = lio->stream;
+    int ns = 0;
+    int rc = depth_pack(h, f, depth, on_device, point_filter_num, blind, st, &ns);
+    if (rc) return rc;
+    const int* d_n = h->dep.d_n + h->in_idx;
+    rc = vg_enqueue(h, h->d_in, ns, leaf, st, nullptr, d_n);
+    if (rc) return rc;
+    immesh_lio::FeedNext& nx = lio->feed_next;   // the scan feed's full scan (registered source 2): the filtered cloud, counted on the device
+    nx.kind = IMMESH_FEED_KIND_DEPTH;
+    nx.branch = 0;
+    nx.pts = h->d_in;
+    nx.inten = nullptr;
+    nx.n = ns;
+    nx.n_dev = d_n;
+    rc = immesh_lio_step_async_dev_n(lio, h->d_out, ns < lio->max_scan ? ns : lio->max_scan, &h->d_grid->m_out, dt, cov_gyr, cov_acc);
+    lio->feed_next = immesh_lio::FeedNext();
+    return rc;
 }
 int immesh_lio_step_async_raw_i(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int intensity_col, int on_device, int calib_laser,
                                 float leaf, double dt, double cov_gyr, double cov_acc) {

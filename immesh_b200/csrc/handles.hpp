@@ -110,6 +110,7 @@ struct immesh_lio {
         int kind = -1, branch = 0, n = 0;
         const float* pts = nullptr;     // the full scan (registered source 2)
         const float* inten = nullptr;   // its intensity, or null
+        const int* n_dev = nullptr;     // its count when that is device resident (n: the upper bound)
     } feed_next;
     // scan feed (immesh_lio_feed_enable)
     struct Feed {
@@ -296,6 +297,7 @@ struct immesh_mesh {
         int last_frame = 0;                   // newest depth frame queued (0: none)
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // not counted in immesh_mesh_capacity
     } dep;
+    int dev_dims_frame = 0;   // newest frame whose n, step and m were set on the device (a depth frame, a device-count hand-off)
 };
 
 // The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate

@@ -625,7 +625,7 @@ __global__ void __launch_bounds__(SPUB_THREADS) k_reg_gather(LioParams P, ScanBu
         if (fd->lost || fd->dyn.src == 0) return;   // block-uniform
         base = fd->reg_base;
         pts = nullptr;
-        if (fd->dyn.src == 2) { pts = fd->dyn.pts; n = fd->dyn.n; inten = fd->dyn.inten; stride = 3; col = -1; }
+        if (fd->dyn.src == 2) { pts = fd->dyn.pts; n = feed_full_n(fd->dyn); inten = fd->dyn.inten; stride = 3; col = -1; }
     }
     if (threadIdx.x < 12) s_state[threadIdx.x] = ctrl->state[threadIdx.x];
     if (!pts) {
@@ -663,7 +663,7 @@ __global__ void __launch_bounds__(FEED_THREADS) k_feed_head(ScanBuf sb_, const L
         long long ne = 0, nr = 0;
         if (d.lio) {
             if (eff_total) ne = *eff_total;
-            const int n = d.src == 2 ? d.n : d.src == 1 ? scan_load_dyn(sb_).n : 0;
+            const int n = d.src == 2 ? feed_full_n(d) : d.src == 1 ? scan_load_dyn(sb_).n : 0;
             nr = n > 0 ? (n - 1) / skip + 1 : 0;
         }
         long long* h = hdr + slot * IMMESH_LIO_FEED_HDR;
@@ -1311,6 +1311,7 @@ static int feed_stage(immesh_lio* h, const immesh_lio::FeedNext& nx, int kind, i
     d.pts = d.src == 2 ? nx.pts : nullptr;
     d.inten = d.src == 2 ? nx.inten : nullptr;
     d.n = d.src == 2 ? nx.n : 0;
+    d.n_dev = d.src == 2 ? nx.n_dev : nullptr;
     d.pad_ = 0;
     IM_CUDA(cudaMemcpyAsync(&f.dev->dyn, &d, sizeof(FeedDyn), cudaMemcpyHostToDevice, h->stream));
     return IMMESH_OK;

@@ -22,12 +22,15 @@ struct FeedDyn {
     long long scan;        // the scan's number
     const float* pts;      // registered source 2: the full scan, [n][3] (device)
     const float* inten;    // its intensity, [n] (device), or null (intensity 0)
-    int n;                 // points of pts
+    const int* n_dev;      // the count of pts when it is device resident (a depth image's filtered cloud), else null
+    int n;                 // points of pts (the upper bound of *n_dev)
     int kind, branch;      // IMMESH_FEED_KIND_*, IMU branch (0: LiDAR-only)
     int src;               // registered source used: 0 none, 1 the down-sampled scan, 2 the full scan
     int lio;               // 1: the scan ran the IESKF (iterations, matches, rows); 0: an IMU branch 1 / 2 scan (header and state only)
     int pad_;
 };
+// the points of the full scan (registered source 2)
+IM_HD int feed_full_n(const FeedDyn& d) { return d.n_dev ? *d.n_dev : d.n; }
 struct LioFeedDev {
     FeedDyn dyn;
     long long started;     // newest scan whose slot is being written (set before the slot's first byte changes)

@@ -551,31 +551,10 @@ __global__ void __launch_bounds__(RF_FIN) k_rf_emit(const DepthCam* cam, const F
     if (blockIdx.x == 0 && threadIdx.x == 0) *o.n = blk_off[nb];
 }
 
-// ---- depth-camera frames (immesh_mesh_push_depth, depth_frame.cuh): the valid samples per block of DF_BLOCK consecutive sampled pixels
-// (k_depth_count), their offsets (k_rf_scan), then each valid sample's world point at its block's offset plus its rank in the block
-// (k_depth_emit), so that the points keep the pixel order the vertex append depends on.  Block 0 of the emit sets the frame's n, step,
-// m and cmask in its FrameDyn (frame_append_dims): the kernels after it read the device count.  Grids cover max_frame_points samples.
-#define DF_BLOCK 1024
-__global__ void __launch_bounds__(DF_BLOCK) k_depth_count(const DepthFrame* df, int* blk) {
-    const DepthFrame& D = *df;
-    const int k = blockIdx.x * DF_BLOCK + threadIdx.x;
-    float p[3];
-    const int c = __syncthreads_count(k < D.sw * D.sh && depth_point(D, k, p));
-    if (threadIdx.x == 0) blk[blockIdx.x] = c;
-}
-__global__ void __launch_bounds__(DF_BLOCK) k_depth_emit(const DepthFrame* df, const int* blk_off, int nb, int append_target, FrameDyn* dyn, float* pts, int* n_out) {
-    const DepthFrame& D = *df;
-    const int k = blockIdx.x * DF_BLOCK + threadIdx.x;
-    float p[3];
-    const bool ok = k < D.sw * D.sh && depth_point(D, k, p);
-    const int i = blk_off[blockIdx.x] + block_scan_1024(ok ? 1 : 0);
-    if (ok) { pts[(size_t)i * 3 + 0] = p[0]; pts[(size_t)i * 3 + 1] = p[1]; pts[(size_t)i * 3 + 2] = p[2]; }
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
-        const int n = blk_off[nb];
-        *n_out = n;
-        dyn->n = n;
-        frame_append_dims(n, append_target, &dyn->step, &dyn->m, &dyn->cmask);
-    }
+// ---- depth-camera frames (immesh_mesh_push_depth): the kernels of depth_kernels.cuh without a filter; block 0 of k_depth_emit sets the
+// frame's n, step, m and cmask in its FrameDyn, and the kernels after it read the device count.  Grids cover max_frame_points samples.
+namespace {
+#include "depth_kernels.cuh"
 }
 
 // ---- the viewer's shaded image of the live mesh (draw_triangle with the facet shader, mesh_rec_display.cpp:273-282; the rule is
@@ -1116,9 +1095,18 @@ static int mesh_grid(const immesh_mesh* h, int n, int threads, int waves = 8) {
 // localization handle: the pose is the one that scan converged to (LioCtrl::pose_ring, written by the last kernel of the
 // scan's sequence; the localization stream may already be working on later scans).  Block 0 also derives the frame's sensor
 // position + the origin of the flip-priority rank, and records the pose in the handle's camera ring (reinforce.cuh, rf_avr_pose).
-__global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCtrl* ctrl, FrameBuf F_, double res, double (*cam_ring)[12], int* cam_ring_frame) {
+// A count read on the device (FrameDyn::n_dev, immesh_mesh_push_frame_from_lio_async_dev_n): every block reads it there, and block 0 sets
+// the frame's n, step, m and cmask from it (frame_append_dims) for the kernels after this one.
+__global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCtrl* ctrl, FrameBuf F_, double res, double (*cam_ring)[12], int* cam_ring_frame,
+                                                        int append_target) {
     __shared__ double s[12];
     const FrameDyn d = *F_.dyn;
+    const int n = d.n_dev ? *d.n_dev : d.n;
+    if (d.n_dev && blockIdx.x == 0 && threadIdx.x == 0) {
+        FrameDyn* w = const_cast<FrameDyn*>(F_.dyn);
+        w->n = n;
+        frame_append_dims(n, append_target, &w->step, &w->m, &w->cmask);
+    }
     if (threadIdx.x < 12) s[threadIdx.x] = ctrl->pose_ring[d.pose_idx][threadIdx.x];
     __syncthreads();
     if (blockIdx.x == 0 && threadIdx.x < 3) {
@@ -1132,7 +1120,6 @@ __global__ void __launch_bounds__(128) k_transform_full(LioParams P, const LioCt
     }
     const float* body = d.body;
     float* world = const_cast<float*>(d.pts);
-    const int n = d.n;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const double pb[3] = {(double)body[(size_t)i * 3 + 0], (double)body[(size_t)i * 3 + 1], (double)body[(size_t)i * 3 + 2]};
         double pw[3];
@@ -1776,24 +1763,27 @@ struct DepthSrc {
     int bpp;
 };
 
-// src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state, 4 a depth
-// image (dsrc; n is the sampled pixels, the upper bound of the count its kernels set on the device).
+// src_mode: 0 host world points, 1 device world points, 2 host body points + lio state, 3 device body points + lio state (n_dev: their
+// count is read on the device, n its upper bound), 4 a depth image (dsrc; n is the sampled pixels, the upper bound of the count its
+// kernels set on the device).
 // Queues one frame (no host synchronisation except when both staging slots are still busy).  Host work per frame in the
 // pipelined form: (memcpy into the pinned slot unless the caller's buffer is pinned) + H2D scan + H2D FrameDyn + one stream
 // wait + ONE cudaGraphLaunch (no node is touched: every per-frame value is read from the FrameDyn) + one D2H of the counters.
 static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double* pose_t, int src_mode, immesh_lio* lio, int kind, bool allow_graph = false,
-                        const DepthSrc* dsrc = nullptr) {
+                        const DepthSrc* dsrc = nullptr, const int* n_dev = nullptr) {
     const bool from_lio = src_mode == 2 || src_mode == 3, depth = src_mode == 4;
+    const bool dev_dims = depth || n_dev;   // n, step, m and cmask are set on the device
     if (!h || (!xyz && n > 0 && !depth) || n < 0 || (!from_lio && !pose_t) || (depth && !dsrc)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_frame_points) return im_fail(IMMESH_E_CAPACITY, "frame larger than max_frame_points");
     FrameBuf& F = h->F;
     const MeshParams& P = h->P;
-    // a depth frame's n, step, m and cmask are set by its kernels from the valid count: the host holds n = the sampled pixels and the
-    // most candidates they can give, for the growth check and for the grids, which cover max_frame_points anyway
+    // a depth frame's n, step, m and cmask are set by its kernels from the valid count, a device-count hand-off's by k_transform_full:
+    // the host holds n = the upper bound and the most candidates it can give, for the growth check and for the grids, which cover
+    // max_frame_points anyway
     int step, m;
     unsigned int cmask;
     frame_append_dims(n, P.append_target, &step, &m, &cmask);
-    if (depth) m = frame_append_max_m(n, P.append_target);
+    if (dev_dims) m = frame_append_max_m(n, P.append_target);
     const int grc = mesh_growth_check(h, m);
     if (grc) return grc;
     F.n = n;
@@ -1826,11 +1816,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
             if (dsrc->host_img) {   // the sampled grid, tight, through the pinned slot (sw * sh * bpp <= 4 max_frame_points bytes)
                 unsigned char* hb = reinterpret_cast<unsigned char*>(h_pts);
                 const size_t rowb = (size_t)hd->sw * dsrc->bpp;
-                for (int sv = 0; sv < hd->sh; ++sv) {
-                    const unsigned char* row = dsrc->host_img + (size_t)sv * hd->stride * dsrc->pitch;
-                    if (hd->stride == 1) { std::memcpy(hb + sv * rowb, row, rowb); continue; }
-                    for (int su = 0; su < hd->sw; ++su) std::memcpy(hb + sv * rowb + (size_t)su * dsrc->bpp, row + (size_t)su * hd->stride * dsrc->bpp, dsrc->bpp);
-                }
+                depth_stage_grid(*hd, dsrc->host_img, dsrc->pitch, dsrc->bpp, hb);
                 unsigned char* db = reinterpret_cast<unsigned char*>(h->d_body + s * slot_pts);
                 IM_CUDA(cudaMemcpyAsync(db, hb, rowb * hd->sh, cudaMemcpyHostToDevice, h->stream_up));
                 IM_CUDA(cudaEventRecord(h->ev_up[s], h->stream_up));
@@ -1886,7 +1872,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     {   // the frame's device-resident inputs
         FrameDyn& d = h->h_dyn[s];
         d.pts = F.pts; d.body = d_body; d.fp = d_fp;
-        d.n = F.n; d.step = F.step; d.m = F.m; d.frame = F.frame; d.cmask = F.cmask; d.pose_idx = pose_idx; d.epoch = epoch;
+        d.n = F.n; d.step = F.step; d.m = F.m; d.frame = F.frame; d.cmask = F.cmask; d.pose_idx = pose_idx; d.epoch = epoch; d.n_dev = n_dev;
         IM_CUDA(cudaMemcpyAsync(h->d_dyn, &d, sizeof(FrameDyn), cudaMemcpyHostToDevice, st));
     }
     const bool rf_on = h->rf.on != 0, chg_on = h->chg.on != 0;
@@ -1900,7 +1886,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     const bool vw_on = h->vw.on != 0;
     const bool fd_on = h->feed.on != 0, fd_img = fd_on && vw_on && h->feed.max_images > 0;
     if (fd_on) {
-        rc = mesh_feed_stage(h, s, F.frame, depth ? -1 : F.n, F.step, kind, from_lio ? nullptr : pose_t, rf_on, fd_img);
+        rc = mesh_feed_stage(h, s, F.frame, dev_dims ? -1 : F.n, F.step, kind, from_lio ? nullptr : pose_t, rf_on, fd_img);
         if (rc) return rc;
     }
     if (vw_on) {   // the view's camera source of this frame
@@ -1920,12 +1906,13 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     auto launch_frame = [&](bool timing) {
         const bool pdl = pdl_frame && !timing;
         if (fd_on) IM_LAUNCH(k_mfeed_begin, 1, 32, 0, st, h->feed.dev);
-        if (from_lio) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame);
+        if (from_lio) IM_LAUNCH(k_transform_full, g_pts, 128, 0, st, lio->P, (const LioCtrl*)lio->d_ctrl, F, P.res, h->cam_ring, h->cam_ring_frame, P.append_target);
         if (depth) {
             auto& D = h->dep;
             IM_LAUNCH(k_depth_count, D.nb, DF_BLOCK, 0, st, (const DepthFrame*)D.d_df, D.blk);
             IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)D.blk, D.nb, D.blk_off, (int*)nullptr, 0, (int*)nullptr);
-            IM_LAUNCH(k_depth_emit, D.nb, DF_BLOCK, 0, st, (const DepthFrame*)D.d_df, (const int*)D.blk_off, D.nb, P.append_target, h->d_dyn, D.pts, D.n);
+            IM_LAUNCH(k_depth_emit, D.nb, DF_BLOCK, 0, st, (const DepthFrame*)D.d_df, (const int*)D.blk_off, (const int*)D.blk_off, D.nb, 1, 0.0, P.append_target,
+                      h->d_dyn, D.pts, D.n);
         }
         IM_LAUNCH_PDL(pdl && src_mode >= 2, k_frame_begin, h->n_sm * 8, 256, 0, st, h->M, F);
         if (timing) cudaEventRecord(h->ev[1], st);
@@ -1998,6 +1985,7 @@ static int mesh_enqueue(immesh_mesh_t* h, const float* xyz, int n, const double*
     if (vw_on) h->vw.last_frame = F.frame;
     if (chg_on) h->chg.last_frame = F.frame;
     if (depth) h->dep.last_frame = F.frame;
+    if (dev_dims) h->dev_dims_frame = F.frame;
     if (fd_on) return mesh_feed_commit(h, F.frame);
     return IMMESH_OK;
 }
@@ -2043,30 +2031,19 @@ int immesh_mesh_push_frame_from_lio_async(immesh_mesh_t* h, immesh_lio_t* lio, c
     if (!lio) return im_fail(IMMESH_E_INVALID, "null lio handle");
     return mesh_enqueue(h, body_xyz, n, nullptr, on_device ? 3 : 2, lio, IMMESH_MFEED_KIND_FROM_LIO_ASYNC, true);
 }
+int immesh_mesh_push_frame_from_lio_async_dev_n(immesh_mesh_t* h, immesh_lio_t* lio, const float* d_body_xyz, int n_max, const int* d_n) {
+    if (!h || !lio || !d_body_xyz || !d_n || n_max < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_mesh_push_frame_from_lio_async_dev_n: the mesh handle is sharded");
+    return mesh_enqueue(h, d_body_xyz, n_max, nullptr, 3, lio, IMMESH_MFEED_KIND_FROM_LIO_ASYNC_DEV_N, true, nullptr, d_n);
+}
 
 // ---- depth-camera frames (include/immesh_b200.h, immesh_depth_frame)
-static bool all_finite(const double* v, int n) {
-    for (int i = 0; i < n; ++i) if (!std::isfinite(v[i])) return false;
-    return true;
-}
 // the image and camera of f checked and turned into the kernels' DepthFrame; the handle's depth buffers allocated by the first frame
 static int depth_source(immesh_mesh* h, const immesh_depth_frame* f, const void* img, int on_device, DepthSrc* src, int* n_sampled) {
-    if (!h || !f || !img) return im_fail(IMMESH_E_INVALID, "depth frame: null argument");
+    if (!h) return im_fail(IMMESH_E_INVALID, "depth frame: null argument");
     if (h->F.shard_n > 1) return im_fail(IMMESH_E_INVALID, "depth frame: a sharded mesh handle takes world-frame points only");
-    if (f->format != IMMESH_DEPTH_F32 && f->format != IMMESH_DEPTH_U16) return im_fail(IMMESH_E_INVALID, "depth frame: unknown format");
-    if (f->kind != IMMESH_DEPTH_PLANAR && f->kind != IMMESH_DEPTH_RANGE) return im_fail(IMMESH_E_INVALID, "depth frame: unknown kind");
-    const int bpp = depth_bytes_per_pixel(f->format);
-    if (f->width < 1 || f->height < 1 || f->stride < 1) return im_fail(IMMESH_E_INVALID, "depth frame: width, height and stride must be >= 1");
-    const long long pitch = f->pitch_bytes ? f->pitch_bytes : (long long)f->width * bpp;
-    if (pitch < (long long)f->width * bpp || pitch % bpp || (uintptr_t)img % bpp)
-        return im_fail(IMMESH_E_INVALID, "depth frame: the pitch is below the row's bytes, or the pitch or the image is not aligned to the pixel size");
-    if (!std::isfinite(f->fx) || !std::isfinite(f->fy) || f->fx == 0.0 || f->fy == 0.0 || !std::isfinite(f->cx) || !std::isfinite(f->cy) ||
-        !all_finite(f->cam_R, 9) || !all_finite(f->cam_t, 3))
-        return im_fail(IMMESH_E_INVALID, "depth frame: fx and fy must be finite and non-zero, cx, cy, cam_R and cam_t finite");
-    if (!(0.0 <= f->z_min && f->z_min < f->z_max && f->z_max < INFINITY)) return im_fail(IMMESH_E_INVALID, "depth frame: needs 0 <= z_min < z_max < inf");
-    if (f->format == IMMESH_DEPTH_U16 && !(f->depth_scale > 0.0 && std::isfinite(f->depth_scale)))
-        return im_fail(IMMESH_E_INVALID, "depth frame: a u16 image needs a positive, finite depth_scale");
-    const int sw = depth_sampled(f->width, f->stride), sh = depth_sampled(f->height, f->stride);
+    if (const char* bad = depth_frame_setup(f, img, &src->df, &src->pitch, &src->bpp)) return im_fail(IMMESH_E_INVALID, bad);
+    const int sw = src->df.sw, sh = src->df.sh;
     if ((long long)sw * sh > h->max_frame_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than max_frame_points");
     auto& D = h->dep;
     if (!D.pts) {
@@ -2087,18 +2064,7 @@ static int depth_source(immesh_mesh* h, const immesh_depth_frame* f, const void*
         D.dev = std::move(dev);
         D.pinned = std::move(pinned);
     }
-    DepthFrame& d = src->df;
-    std::memset(&d, 0, sizeof(d));
-    d.img = static_cast<const unsigned char*>(img);
-    d.row_bytes = (long long)f->stride * pitch;
-    d.col_bytes = (long long)f->stride * bpp;
-    d.sw = sw; d.sh = sh; d.stride = f->stride; d.format = f->format; d.kind = f->kind;
-    d.depth_scale = f->depth_scale; d.fx = f->fx; d.fy = f->fy; d.cx = f->cx; d.cy = f->cy; d.z_min = f->z_min; d.z_max = f->z_max;
-    std::memcpy(d.R, f->cam_R, sizeof(d.R));
-    std::memcpy(d.t, f->cam_t, sizeof(d.t));
     src->host_img = on_device ? nullptr : static_cast<const unsigned char*>(img);
-    src->pitch = pitch;
-    src->bpp = bpp;
     *n_sampled = sw * sh;
     return IMMESH_OK;
 }
@@ -2267,7 +2233,7 @@ int immesh_mesh_work_stats(immesh_mesh_t* h, int64_t* out) {
     if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
     const int* c = h->last_cnt;
     int m = h->F.m;
-    if (h->dep.last_frame && h->dep.last_frame == h->frame_counter) {   // the newest frame is a depth frame: its m is set on the device
+    if (h->dev_dims_frame && h->dev_dims_frame == h->frame_counter) {   // the newest frame's m is set on the device
         FrameDyn d;
         IM_CUDA(cudaStreamSynchronize(h->stream));
         IM_CUDA(cudaMemcpy(&d, h->d_dyn, sizeof(d), cudaMemcpyDeviceToHost));

@@ -201,6 +201,7 @@ struct FrameDyn {
     unsigned int cmask;
     int pose_idx;         // slot of LioCtrl::pose_ring holding the pose the scan converged to
     unsigned long long epoch;   // peer-window epoch of this frame (sharded mode)
+    const int* n_dev;     // a handed-over frame whose count is device resident: n is read here, and n, step, m, cmask set (k_transform_full)
 };
 struct FrameBuf {
     const float* pts;     // [n][3] world-frame scan

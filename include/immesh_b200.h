@@ -259,7 +259,7 @@ int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int st
  *   max_scans >= 1: header and state ring; max_rows: row ring (>= 1 when effect or registered is set); effect 0/1; registered 0 (none),
  *   1 (the down-sampled scan, dense_map_en 0) or 2 (the full scan, dense_map_en 1); point_skip >= 1 (publish/pub_point_skip).
  *   Other values, or a sharded handle: IMMESH_E_INVALID.  immesh_lio_shard refuses a handle with the feed on.
- * Every call of immesh_lio_step, _step_dev, _step_async, _step_async_dev_n, _step_async_raw, _raw_i, _imu and _imu_i records one scan
+ * Every call of immesh_lio_step, _step_dev, _step_async, _step_async_dev_n, _step_async_raw, _raw_i, _imu, _imu_i and _depth records one scan
  * (the IMU chain's branches 1 and 2 too: a header and the state, no rows).  The staged calls record nothing.
  *   header (IMMESH_LIO_FEED_HDR int64): IMMESH_FEED_SCAN number; KIND (IMMESH_FEED_KIND_*); BRANCH (0 LiDAR-only, else the IMU
  *     chain's 1/2/3); ITERS run; MATCHES of the last IESKF iteration (m_effct_feat_num); CONVERGED flag of that iteration; ERR (the
@@ -268,8 +268,8 @@ int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int st
  *   state: the 348 doubles the scan ended with, bit-identical to immesh_lio_wait right after it (branches 1 and 2: the state as the
  *     branch left it).
  *   rows: effect = 1: immesh_lio_effect_cloud right after the scan (row_index = its scan_index).  registered = 1:
- *     immesh_lio_registered_cloud(h, NULL, ..., point_skip); registered = 2: on _raw and _imu, immesh_lio_registered_cloud of
- *     immesh_voxelgrid_input_points (stride 3, intensity column -1), on _raw_i and _imu_i immesh_lio_frontend_cloud(h, vg, 1,
+ *     immesh_lio_registered_cloud(h, NULL, ..., point_skip); registered = 2: on _raw, _imu and _depth, immesh_lio_registered_cloud of
+ *     immesh_voxelgrid_input_points (stride 3, intensity column -1; _depth: its device count), on _raw_i and _imu_i immesh_lio_frontend_cloud(h, vg, 1,
  *     point_skip), elsewhere (no full scan) source 1.  row_index of a registered row: -1.
  *   A scan whose rows exceed max_rows keeps its header and state and sets ROWS_LOST.  A loss never fails a step or changes the state,
  *   the map or the mesh.
@@ -309,6 +309,7 @@ typedef struct {
 #define IMMESH_FEED_KIND_RAW_I 5
 #define IMMESH_FEED_KIND_IMU 6
 #define IMMESH_FEED_KIND_IMU_I 7
+#define IMMESH_FEED_KIND_DEPTH 8   /* immesh_lio_step_async_depth */
 int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* cfg /* NULL: off */);
 int immesh_lio_feed(immesh_lio_t* h, int64_t since_scan, int wait, int64_t* scans /*[cap_scans][12]*/, double* states /*[cap_scans][348] or NULL*/,
                     int cap_scans, float* rows /*[cap_rows][4] or NULL*/, int32_t* row_index /*[cap_rows] or NULL*/, int64_t cap_rows,
@@ -737,7 +738,7 @@ int immesh_mesh_changes(immesh_mesh_t* h, int64_t since_frame, int64_t* frames /
  * per frame what the reference publishes -- the mesh_cost_time.log fields, the trajectory, the reinforced LiDAR points, a video of
  * the viewer -- without draining.  Records are numbered by the handle's frame numbers (those of immesh_mesh_changes and of
  * immesh_mesh_view_image's frame_out): frame f in header slot (f - 1) % max_frames; the frames queued after the enable are recorded.
- *   Every frame of immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async, immesh_mesh_push_depth, _depth_async and
+ *   Every frame of immesh_mesh_push_frame, _dev, _from_lio, _from_lio_async, _from_lio_async_dev_n, immesh_mesh_push_depth, _depth_async and
  *     immesh_mesh_reconstruct_from_pointcloud records one frame.  A batched frame (immesh_mesh_push_frame_batched, _reconstruct_from_pointcloud_batched) records its header and pose, with
  *     no points and no image (the reinforcement and the view do not follow batched frames).
  *   header (IMMESH_MESH_FEED_HDR int64, IMMESH_MFEED_*): FRAME; KIND (IMMESH_MFEED_KIND_*); N_POINTS and STEP (append_point_step);
@@ -805,6 +806,7 @@ typedef struct {
 #define IMMESH_MFEED_KIND_BATCHED 5
 #define IMMESH_MFEED_KIND_RECONSTRUCT_BATCHED 6
 #define IMMESH_MFEED_KIND_DEPTH 7   /* immesh_mesh_push_depth and _async */
+#define IMMESH_MFEED_KIND_FROM_LIO_ASYNC_DEV_N 8   /* immesh_mesh_push_frame_from_lio_async_dev_n */
 int immesh_mesh_feed_enable(immesh_mesh_t* h, const immesh_mesh_feed_config* cfg /* NULL: off */);
 int immesh_mesh_feed(immesh_mesh_t* h, int64_t since_frame, int wait, int64_t* frames /*[cap_frames][22]*/, double* poses /*[cap_frames][36] or NULL*/,
                      int cap_frames, float* points /*[cap_rows][3] or NULL*/, int32_t* pixels /*[cap_rows] or NULL*/, int64_t cap_rows, int64_t* counts /*[4]*/);
@@ -907,6 +909,50 @@ const float* immesh_voxelgrid_input_points(immesh_voxelgrid_t* h);
  * Replaces src/voxel_mapping.cpp:1844-1859 + :1888-1889 + lio_state_estimation + map_incremental_grow for the scan. */
 int immesh_lio_step_async_raw(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* pts, int n, int stride, int on_device, int calib_laser, float leaf,
                               double dt, double cov_gyr, double cov_acc);
+
+/* ---- depth cameras through the localization: the reference's preprocess/lidar_type 4 (L515; include/common_lib.h:66), whose
+ * Preprocess::l515_handler (src/preprocess.cpp:234-275) turns the camera's cloud into the LiDAR scan of the imu_en: false loop
+ * (Forward_without_imu, pcl::VoxelGrid, voxel_map_init / lio_state_estimation + map_incremental_grow, the mesher hand-off).
+ * One depth image becomes one sensor-frame cloud, on the device:
+ *   Sampling and validity: exactly those of immesh_depth_frame (stride, format, kind, z_min / z_max, the float64 arithmetic), with
+ *     cam_R / cam_t mapping the camera to the sensor frame -- the frame the localization calls its LiDAR frame, which
+ *     immesh_lio_config's ext_R / ext_T then map to the body as for any LiDAR.  Identity gives the camera-optical-frame cloud the
+ *     L515 / RealSense driver publishes.
+ *   point_filter_num (>= 1): the valid samples are numbered i = 0, 1, 2, ... in ascending pixel order (the order of the driver's
+ *     unorganised cloud); sample i is kept iff i % point_filter_num == 0 (preprocess.cpp:250).
+ *   blind (finite, >= 0), after the decimation: a kept point (x, y, z) (the float32 values) is dropped iff (double)r < blind * blind,
+ *     r = (x*x + y*y) + z*z in float32 without FMA (preprocess.cpp:253-256).
+ *   The survivors, in that order, are the cloud: float32 [n][3] in the VoxelGrid handle's input ring (immesh_voxelgrid_input_points),
+ *     its count on the device (immesh_voxelgrid_input_count).  A host image is staged, sampled pixels only, through the handle's
+ *     pinned staging; a device image is read in place at its pitch and must stay unchanged until the chain has run.
+ * immesh_frontend_prepare_depth(vg, f, depth, on_device, point_filter_num, blind, out_xyz, cap, n_out): blocking; the cloud of one
+ *   image, *n_out points, copied to out_xyz when cap >= *n_out (cap = 0: a count query; 0 < cap < *n_out: IMMESH_E_CAPACITY, nothing
+ *   written).  The first frame's voxel_map_init is immesh_lio_predict + immesh_voxelmap_build on this cloud, as the reference's
+ *   imu_en: false loop does (it meshes nothing for that frame).
+ * immesh_lio_step_async_depth(lio, vg, f, depth, on_device, point_filter_num, blind, leaf, dt, cov_gyr, cov_acc): queued on the
+ *   localization stream, no host synchronisation: the cloud -> pcl::VoxelGrid(leaf) (immesh_voxelgrid_filter with the count read on
+ *   the device) -> predict + IESKF + map update (immesh_lio_step_async_dev_n).  The result equals immesh_lio_step_async_raw fed the
+ *   same cloud.  A frame with no point left keeps what a zero device count does: the prediction is applied, the IESKF and the map
+ *   update are skipped (the reference runs Forward_without_imu before its "No point" continue).  The scan feed records it with
+ *   KIND = IMMESH_FEED_KIND_DEPTH; its full scan (registered = 2) is the filtered cloud.
+ *   Hand the frame to the mesher after it with immesh_mesh_push_frame_from_lio_async_dev_n(mesh, lio,
+ *   immesh_voxelgrid_input_points(vg), sampled pixels, immesh_voxelgrid_input_count(vg)).
+ * immesh_voxelgrid_input_count(vg): device pointer to the count of the cloud immesh_voxelgrid_input_points returns when a depth entry
+ *   point wrote it, else NULL; valid until that ring slot is reused (8 calls later).
+ * immesh_mesh_push_frame_from_lio_async_dev_n(h, lio, d_body_xyz, n_max, d_n): immesh_mesh_push_frame_from_lio_async(h, lio,
+ *   d_body_xyz, *d_n, 1) with the count read on the device (*d_n <= n_max): the frame's append_point_step and candidates are set
+ *   there, with the rule of immesh_mesh_push_frame; the frame's grids cover n_max.  The frame feed records it with
+ *   KIND = IMMESH_MFEED_KIND_FROM_LIO_ASYNC_DEV_N (N_POINTS, STEP: the device values).  *d_n == 0 adds nothing to the mesh.
+ * Errors: the checks of immesh_depth_frame (IMMESH_E_INVALID), and IMMESH_E_INVALID for point_filter_num < 1, a negative or
+ *   non-finite blind, leaf <= 0 or a sharded localization or mesh handle; IMMESH_E_CAPACITY when the sampled pixels exceed the
+ *   VoxelGrid's max_points, or n_max > max_frame_points.  The down-sampled cloud must fit max_scan_points, as for
+ *   immesh_lio_step_async_raw. */
+int immesh_frontend_prepare_depth(immesh_voxelgrid_t* vg, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num, double blind,
+                                  float* out_xyz /*[cap][3] or NULL*/, int cap, int* n_out);
+int immesh_lio_step_async_depth(immesh_lio_t* lio, immesh_voxelgrid_t* vg, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num,
+                                double blind, float leaf, double dt, double cov_gyr, double cov_acc);
+const int* immesh_voxelgrid_input_count(immesh_voxelgrid_t* vg);
+int immesh_mesh_push_frame_from_lio_async_dev_n(immesh_mesh_t* h, immesh_lio_t* lio, const float* d_body_xyz, int n_max, const int* d_n);
 
 /* ---- point intensity through the front-end.  The reference keeps every PointType field through the front-end: the KITTI
  * calibration copies the whole point (src/voxel_mapping.cpp:1844-1859), and pcl::VoxelGrid (:1888-1889) runs with PCL's default
