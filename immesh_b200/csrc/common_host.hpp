@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdio>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <string>
@@ -28,6 +29,14 @@ inline bool host_ptr_is_pinned(const void* p) {
     return a.type == cudaMemoryTypeHost;
 }
 
+// H2D on the upload stream, overlapping earlier kernels, joined by `st` through `ev`; an unpinned source goes through `stage` if given
+inline cudaError_t upload_async(void* dst, const void* src, size_t bytes, void* stage, cudaStream_t up, cudaEvent_t ev, cudaStream_t st) {
+    if (stage && !host_ptr_is_pinned(src)) src = std::memcpy(stage, src, bytes);
+    cudaError_t e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, up);
+    if (e == cudaSuccess) e = cudaEventRecord(ev, up);
+    return e == cudaSuccess ? cudaStreamWaitEvent(st, ev, 0) : e;
+}
+
 inline std::string& last_error_storage() {
     static thread_local std::string s;
     return s;
@@ -35,6 +44,11 @@ inline std::string& last_error_storage() {
 inline int im_fail(int code, const char* msg) {
     last_error_storage() = msg ? msg : "";
     return code;
+}
+// a failed allocation of a call's buffers (the sticky error cleared): IMMESH_E_CAPACITY when memory ran out, IMMESH_E_CUDA otherwise
+inline int im_fail_alloc(cudaError_t e, const char* msg) {
+    cudaGetLastError();
+    return im_fail(e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA, msg);
 }
 inline int im_fail_cuda(cudaError_t e, const char* file, int line) {
     char buf[512];
@@ -205,6 +219,16 @@ inline cudaError_t run_graphed_static(GraphCtx& g, unsigned sig, cudaStream_t st
     return cudaGraphLaunch(g.exec, st);
 }
 }  // namespace immesh
+
+// an enable's start: work in flight uses the stage's buffers and the captured sequence changes, so drain and drop the graph first
+template <class H, class Reset>
+inline cudaError_t im_stage_reset(H* h, Reset&& reset) {
+    const cudaError_t e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) return e;
+    h->graph.destroy();
+    reset();
+    return cudaSuccess;
+}
 
 // kernel launch with accounting; wrap template kernels in parentheses: IM_LAUNCH((k<256>), grid, block, smem, stream, args...)
 #define IM_LAUNCH(KERN, GRID, BLOCK, SMEM, STREAM, ...) immesh::im_launch(#KERN, KERN, dim3(GRID), dim3(BLOCK), (SMEM), (STREAM), false, ##__VA_ARGS__)

@@ -2,12 +2,12 @@
 // the mesh's depth frames (mesh_capi.cu: world points, the frame's FrameDyn set from the count) and the localization's front-end
 // (frontend_capi.cu: sensor-frame points, filtered as Preprocess::l515_handler does, into the VoxelGrid handle's input ring).
 //   k_depth_count  the valid samples per block of DF_BLOCK consecutive sampled pixels
-//   (scan)         their offsets, total behind them: the one-block exclusive scan (k_rf_scan in mesh_capi.cu, k_rs_scan elsewhere)
+//   (scan)         their offsets, total behind them: the one-block exclusive scan (k_rf_scan of mesh_render.cu for the mesh, k_rs_scan elsewhere)
 //   k_depth_keep   with a filter only: each valid sample's global index (block offset + rank), so that the decimation and blind can be
 //                  evaluated; the kept samples per block, then the scan again for their offsets
 //   k_depth_emit   each kept sample's point at its block's offset plus its rank in the block; block 0 writes the count
 // point_filter_num = 1 and blind = 0 keep every valid sample: then the keep pass is not launched and valid_off serves as keep_off.
-// Include inside the anonymous namespace of a translation unit, after handles.hpp (depth_frame.cuh, mesh_core.cuh) and radix_sort.cuh
+// Include inside the anonymous namespace of a translation unit, after handles.hpp (depth_frame.cuh, mesh_core.cuh) and block_scan.cuh
 // (block_scan_1024).
 #pragma once
 

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
 #include "common_host.hpp"
 #include "depth_frame.cuh"
 #include "lio_core.cuh"
@@ -143,7 +145,7 @@ struct immesh_lio {
 };
 #define IM_FEED_DYN_RING 64
 
-// the device buffers of one depth image of the tiled rasteriser (mesh_capi.cu: rf_image_alloc, rf_image_launch): the camera, the tile
+// the device buffers of one depth image of the tiled rasteriser (mesh_render.cu: rf_image_alloc, rf_image_launch): the camera, the tile
 // counters and offsets, the bins, misc[0] (the bins overflowed), the valid pixels per block and their offsets, the depth bits, and
 // result buffers 0 and 1 (image, points, pixels, count; the pose is the queued reinforcement's own)
 struct RfOut { float* depth; float* pts; int* pix; int* n; double* pose; };
@@ -222,34 +224,26 @@ struct immesh_mesh {
     // LiDAR point-cloud reinforcement (immesh_mesh_reinforce_enable)
     double (*cam_ring)[12] = nullptr;   // [IM_RF_RING] rot_end, pos_end of the frames handed over by the localization handle
     int* cam_ring_frame = nullptr;      // [IM_RF_RING] frame number each ring entry belongs to (0: none)
-    struct Reinforce {
+    // a camera queued behind every frame: the reinforcement (immesh_mesh_reinforce_enable) and the view (immesh_mesh_view_enable)
+    struct QueuedCam {
         int on = 0, win = 1;
-        int last_frame = 0;               // newest frame queued with the reinforcement (0: none since enable)
-        int explicit_pose = 0;            // immesh_mesh_reinforce_pose: the caller's pose from the next frame on
+        int last_frame = 0;               // newest frame queued with it (0: none since enable)
+        int mode = 0;                     // the camera source (RfDyn::mode): 0 sensor-bound, 1 the caller's fixed pose, 2 the follow camera
         double R[9] = {}, t[3] = {};
         immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
         void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
         void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
         RfImage img;                      // result buffer (frame & 1) holds the frame's image and pose
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
-    } rf;
+    } rf;                                 // LiDAR point-cloud reinforcement: the caller's pose (mode 1) from immesh_mesh_reinforce_pose
     // the viewer's shaded image (immesh_mesh_view_enable queues it behind every frame; immesh_mesh_render_view builds one for a call)
-    struct View {
-        int on = 0, win = 1;
-        int last_frame = 0;               // newest frame queued with the view (0: none since enable)
-        int mode = 0;                     // the camera source (RfDyn::mode): 0 sensor-bound, 1 the caller's fixed pose, 2 the follow camera
-        double R[9] = {}, t[3] = {};
+    struct View : QueuedCam {
         int pos = 0, color = 0, auto_range = 0;   // immesh_view_style: positions, color_by_height, z range from the mesh
-        immesh::DepthCam base = {};       // intrinsics, z range and image size; the pose is filled in on the device per frame
-        void* rd = nullptr;               // RfDyn, written per frame from the pinned slot
-        void* h_rd = nullptr;             // pinned, IM_SLOTS RfDyn
-        RfImage img;                      // binning buffers; out[b].depth and out[b].pose of result buffer b
         uchar4* rgba[2] = {};             // the colour image of result buffer b
         float* zr = nullptr;              // [2] the height colour's z range (the caller's, or k_view_zrange's)
         unsigned int* zr_part = nullptr;  // [2 zr_blocks] k_view_zrange's per-block partials
         int* zr_done = nullptr;           // k_view_zrange's finished-block counter (0 between launches)
         int zr_blocks = 1;
-        immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // the buffers above, freed by disable / destroy (not counted)
         immesh::ViewOverlay ov = {};      // immesh_mesh_view_overlay (ov.on = 0: none)
         immesh::MemSet ov_dev;            // its keys, trajectory and frustum, freed by the next overlay call, disable or destroy (not counted)
     } vw;
@@ -301,7 +295,7 @@ struct immesh_mesh {
 };
 
 // The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate
-// (mesh_tri_order, mesh_capi.cu): the live records compacted (w = the slot) and sorted by the triple (a, b, c); with a region size
+// (mesh_tri_order, mesh_query.cu): the live records compacted (w = the slot) and sorted by the triple (a, b, c); with a region size
 // first by the region of tri_region_key, either every region by its key (ascending x, y, z) or, with qkeys, only the regions of the
 // table qkeys / qval by the caller's index.  The caller provides the buffers for `cap` records.  A key outside +-1048000 sets `range`.
 struct TriOrder {
@@ -318,3 +312,53 @@ struct TriOrder {
     const unsigned int* order;         // out: the kept records' indices into rec, in order
 };
 int mesh_tri_order(immesh_mesh* h, const int* cnt, double region_size, TriOrder& o);
+
+// ---- what the mesher's translation units call in one another, by the file that defines it: mesh_capi.cu (the handle's bookkeeping and
+// the frame chain's stages the batched frame shares), mesh_render.cu, mesh_feeds.cu, mesh_query.cu (rs_sort_passes of radix_sort.cuh,
+// whose kernels the mesher compiles once, and the ints of its hist for n keys)
+#define IM_MPOOL_LIMIT (1LL << 30)   // ids are 32-bit: every mesh pool (and the change feed's ring) stops at 2^30 records
+
+inline size_t pow2_at_least(size_t v) {
+    size_t p = 1;
+    while (p < v) p <<= 1;
+    return p;
+}
+inline int mesh_grid(const immesh_mesh* h, int n, int threads, int waves = 8) {
+    int g = (n + threads - 1) / threads;
+    if (g > h->n_sm * waves) g = h->n_sm * waves;
+    return g < 1 ? 1 : g;
+}
+inline int mesh_grid_fixed(const immesh_mesh* h, long long n_cap, int threads, int waves = 8) {
+    long long g = (n_cap + threads - 1) / threads;
+    if (g > (long long)h->n_sm * waves) g = (long long)h->n_sm * waves;
+    return g < 1 ? 1 : (int)g;
+}
+inline int rb_passes(unsigned long long max_value) {   // 8-bit radix passes that cover max_value
+    int b = 0;
+    while (b < 64 && (max_value >> b)) ++b;
+    return std::max(1, (b + 7) / 8);
+}
+
+int mesh_status(int err);
+void mesh_note(immesh_mesh* h, const int* c, int frame);
+// the host's copy of the counters (the first IM_MC_HOST slots), blocking: the caller has drained what it needs
+inline cudaError_t mesh_read_counters(const immesh_mesh* h, int (&c)[immesh::IM_MC_HOST]) { return cudaMemcpy(c, h->M.cnt, sizeof(c), cudaMemcpyDeviceToHost); }
+int mesh_growth_check(immesh_mesh* h, long long m);
+int mesh_wait_impl(immesh_mesh* h, bool timings);
+int mesh_push_dev(immesh_mesh* h, const float* d_world_xyz, int n, const double* pose_t, int kind);
+void mesh_frame_begin_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool pdl);
+void mesh_append_launch(const immesh_mesh* h, const immesh::FrameBuf& F, int g, cudaStream_t st, bool pdl);
+void mesh_dilate_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool pdl);
+int mesh_tri_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool pdl);
+int queued_cam_stage(immesh_mesh* h, immesh_mesh::QueuedCam& c, int s);
+void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st);
+void mesh_view_launch(immesh_mesh* h, cudaStream_t st);
+void rf_scan_launch(cudaStream_t st, const int* cnt, int n, int* off);
+void mesh_changes_launch(immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool batched);
+void mesh_feed_begin_launch(immesh_mesh* h, cudaStream_t st);
+int mesh_feed_stage(immesh_mesh* h, int s, long long frame, long long n, int step, int kind, const double* pose_t, bool rf, bool img);
+void mesh_feed_launch(immesh_mesh* h, cudaStream_t st, bool rf, bool img);
+cudaError_t mesh_feed_commit(immesh_mesh* h, long long frame);
+void mesh_feed_free(immesh_mesh* h);
+int mesh_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist, const int* n_dev = nullptr);
+size_t mesh_sort_hist_ints(size_t n);

@@ -975,18 +975,8 @@ static int upload_scan(immesh_lio* h, const float* body, int n, int on_device = 
     } else {
         float* dst = h->d_body_own + (size_t)slot * h->max_scan * 3;   // the slot's previous user has finished (ev_slot waited on by the caller)
         h->sb.body = dst;
-        if (n > 0) {
-            const float* src = body;
-            if (!immesh::host_ptr_is_pinned(body)) {
-                float* stage = h->h_body + (size_t)slot * h->max_scan * 3;
-                std::memcpy(stage, body, (size_t)n * 3 * sizeof(float));
-                src = stage;
-            }
-            // on the upload stream, so that the copy overlaps the kernels of the scan before; the compute stream joins it
-            IM_CUDA(cudaMemcpyAsync((void*)dst, src, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, h->stream_up));
-            IM_CUDA(cudaEventRecord(h->ev_up[slot], h->stream_up));
-            IM_CUDA(cudaStreamWaitEvent(h->stream, h->ev_up[slot], 0));
-        }
+        if (n > 0)
+            IM_CUDA(immesh::upload_async(dst, body, (size_t)n * 3 * sizeof(float), h->h_body + (size_t)slot * h->max_scan * 3, h->stream_up, h->ev_up[slot], h->stream));
     }
     return push_dyn(h, n, slot, dt, cov_gyr, cov_acc);
 }
@@ -1111,11 +1101,8 @@ static int lio_grow(immesh_lio* h, long long cap, long long nodes, long long chu
             (e = fresh.alloc(&nsb.slot_offset, cap)) == cudaSuccess && (e = fresh.alloc(&nsb.slot_cursor, cap)) == cudaSuccess)
             e = tmp.alloc(&slot_map, cap0);
     }
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        const int code = e == cudaErrorMemoryAllocation ? IMMESH_E_CAPACITY : IMMESH_E_CUDA;
-        return im_fail(code, (std::string(pool) + ": device allocation for the growth failed (" + cudaGetErrorString(e) + "); the handle is unchanged").c_str());
-    }
+    if (e != cudaSuccess)
+        return im_fail_alloc(e, (std::string(pool) + ": device allocation for the growth failed (" + cudaGetErrorString(e) + "); the handle is unchanged").c_str());
     cudaStream_t st = h->stream;
     auto migrate = [&]() -> cudaError_t {
         cudaError_t r = cudaSuccess;
@@ -1351,10 +1338,7 @@ static void launch_markers(immesh_lio* h, bool walk, bool pdl) {
 static int markers_fit(immesh_lio* h) {
     immesh_lio::Feed& f = h->feed;
     if (f.mk_rows == 0 || f.mk_cap >= h->cap) return IMMESH_OK;
-    IM_CUDA(cudaStreamSynchronize(h->stream));
-    h->graph.destroy();
-    f.mk_scratch = immesh::MemSet();
-    f.mk_sort = nullptr; f.mk_hist = nullptr; f.mk_cap = 0;
+    IM_CUDA(im_stage_reset(h, [&f] { f.mk_scratch = immesh::MemSet(); f.mk_sort = nullptr; f.mk_hist = nullptr; f.mk_cap = 0; }));
     const size_t tiles = (h->cap + VG_TILE - 1) / VG_TILE;
     IM_CUDA(f.mk_scratch.alloc(&f.mk_sort, 4 * h->cap));
     IM_CUDA(f.mk_scratch.alloc(&f.mk_hist, 256 * tiles));
@@ -1633,9 +1617,7 @@ int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* c) {
               c->registered < 0 || c->registered > 2 || c->point_skip < 1 || ((c->effect || c->registered) && c->max_rows < 1)))
         return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_enable: needs max_scans in [1, 2^24], max_rows in [0, 2^32] (>= 1 with rows), effect 0 or 1, "
                                          "registered 0, 1 or 2 and point_skip >= 1");
-    IM_CUDA(cudaStreamSynchronize(h->stream));
-    h->graph.destroy();   // the launch sequence changes
-    feed_free(h);
+    IM_CUDA(im_stage_reset(h, [h] { feed_free(h); }));
     if (!c) return IMMESH_OK;
     immesh_lio::Feed& f = h->feed;
     f.max_scans = c->max_scans;
@@ -1666,6 +1648,26 @@ int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* c) {
     return IMMESH_OK;
 }
 
+// the common part of the two reads: the wait, counts[2..3], then feed_read of `rings`, its copies and the marks at `started` on the
+// feed's stream (never the handle's)
+static int lio_feed_read(immesh_lio* h, const FeedRings& rings, const long long* started, int64_t since, int wait, int64_t* scans, double* states,
+                         int cap_scans, void* rows, void* second, int64_t cap_rows, int64_t* counts) {
+    immesh_lio::Feed& f = h->feed;
+    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued scan's record, nothing else
+    const long long fin = *(volatile long long*)f.h_done;
+    counts[2] = fin;
+    counts[3] = f.queued;
+    auto copy = [&f](void* dst, const void* src, size_t bytes) {
+        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
+        return IMMESH_OK;
+    };
+    auto marks = [&](long long* m) {
+        IM_CUDA(cudaMemcpyAsync(m, started, 2 * sizeof(long long), cudaMemcpyDeviceToHost, f.stream));
+        IM_CUDA(cudaStreamSynchronize(f.stream));
+        return IMMESH_OK;
+    };
+    return feed_read(rings, since, fin, scans, states, cap_scans, rows, second, cap_rows, counts, copy, marks);
+}
 int immesh_lio_feed(immesh_lio_t* h, int64_t since, int wait, int64_t* scans, double* states, int cap_scans, float* rows, int32_t* row_index, int64_t cap_rows,
                     int64_t* counts) {
     if (!h || !counts || cap_scans < 0 || cap_rows < 0 || (cap_scans > 0 && !scans)) return im_fail(IMMESH_E_INVALID, "bad argument");
@@ -1674,21 +1676,8 @@ int immesh_lio_feed(immesh_lio_t* h, int64_t since, int wait, int64_t* scans, do
     immesh_lio::Feed& f = h->feed;
     if (!f.on) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed: the scan feed is not enabled (immesh_lio_feed_enable)");
     if (since < 0 || since > f.queued) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed: since_scan must be in [0, newest queued scan]");
-    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued scan's record, nothing else
-    const long long fin = *(volatile long long*)f.h_done;
-    counts[2] = fin;
-    counts[3] = f.queued;
     const FeedRings rings{f.max_scans, f.max_rows, f.hdr, f.states, f.rows, f.idx};
-    auto copy = [&](void* dst, const void* src, size_t bytes) {   // on the feed's stream, never the handle's
-        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
-        return IMMESH_OK;
-    };
-    auto marks = [&](long long* m) {
-        IM_CUDA(cudaMemcpyAsync(m, &f.dev->started, 2 * sizeof(long long), cudaMemcpyDeviceToHost, f.stream));
-        IM_CUDA(cudaStreamSynchronize(f.stream));
-        return IMMESH_OK;
-    };
-    const int rc = feed_read(rings, since, fin, scans, states, cap_scans, rows, row_index, cap_rows, counts, copy, marks);
+    const int rc = lio_feed_read(h, rings, &f.dev->started, since, wait, scans, states, cap_scans, rows, row_index, cap_rows, counts);
     if (rc == IMMESH_E_RANGE) return im_fail(rc, "immesh_lio_feed: scans of the range left the rings or were overwritten while they were read; read on from counts[2]");
     if (rc == IMMESH_E_CAPACITY) return im_fail(rc, "immesh_lio_feed: more scans or rows than the caps (counts holds them)");
     return rc;
@@ -1699,9 +1688,7 @@ int immesh_lio_feed_markers_enable(immesh_lio_t* h, int64_t max_rows) {
     immesh_lio::Feed& f = h->feed;
     if (!f.on) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers_enable: the scan feed is not enabled (immesh_lio_feed_enable)");
     if (max_rows < 0 || max_rows > (1LL << 32)) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers_enable: max_rows must be in [0, 2^32] (0: off)");
-    IM_CUDA(cudaStreamSynchronize(h->stream));
-    h->graph.destroy();   // the launch sequence changes
-    markers_free(h);
+    IM_CUDA(im_stage_reset(h, [h] { markers_free(h); }));
     if (max_rows == 0) return IMMESH_OK;
     auto fail = [&](cudaError_t e) { markers_free(h); cudaGetLastError(); return immesh::im_fail_cuda(e, __FILE__, __LINE__); };
     cudaError_t e;
@@ -1721,21 +1708,8 @@ int immesh_lio_feed_markers(immesh_lio_t* h, int64_t since, int wait, int64_t* s
     immesh_lio::Feed& f = h->feed;
     if (!f.on || f.mk_rows == 0) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers: the plane-map markers are not enabled (immesh_lio_feed_markers_enable)");
     if (since < 0 || since > f.queued) return im_fail(IMMESH_E_INVALID, "immesh_lio_feed_markers: since_scan must be in [0, newest queued scan]");
-    if (wait) IM_CUDA(cudaEventSynchronize(f.ev));   // the newest queued scan's record, nothing else
-    const long long fin = *(volatile long long*)f.h_done;
-    counts[2] = fin;
-    counts[3] = f.queued;
     const FeedRings rings = marker_rings(f.max_scans, f.mk_rows, f.mk_hdr, f.mk_ring);
-    auto copy = [&](void* dst, const void* src, size_t bytes) {   // on the feed's stream, never the handle's
-        IM_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, f.stream));
-        return IMMESH_OK;
-    };
-    auto marks = [&](long long* m) {
-        IM_CUDA(cudaMemcpyAsync(m, &f.mk_dev->started, 2 * sizeof(long long), cudaMemcpyDeviceToHost, f.stream));
-        IM_CUDA(cudaStreamSynchronize(f.stream));
-        return IMMESH_OK;
-    };
-    const int rc = feed_read(rings, since, fin, scans, nullptr, cap_scans, rows, nullptr, cap_rows, counts, copy, marks);
+    const int rc = lio_feed_read(h, rings, &f.mk_dev->started, since, wait, scans, nullptr, cap_scans, rows, nullptr, cap_rows, counts);
     if (rc == IMMESH_E_RANGE)
         return im_fail(rc, "immesh_lio_feed_markers: records of the range left the rings, were overwritten while they were read, or predate the enable; read on from counts[2]");
     if (rc == IMMESH_E_CAPACITY) return im_fail(rc, "immesh_lio_feed_markers: more scans or rows than the caps (counts holds them)");

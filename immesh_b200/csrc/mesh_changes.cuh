@@ -1,6 +1,6 @@
 // immesh_b200 -- the mesh's change feed (immesh_mesh_changes_enable / immesh_mesh_changes): per frame, the net difference of the
 // live triangle set and its flips against the state the feed last published, as (a, b, c, code) rows in ascending triple order,
-// appended with a frame header to a device ring.  The bodies below run one thread each in the kernels of mesh_capi.cu (k_chg_*)
+// appended with a frame header to a device ring.  The bodies below run one thread each in the kernels of mesh_feeds.cu (k_chg_*)
 // and in the host emulation of the tests.
 //
 // Touched set of a frame: every slot whose live flag or flip word a writer of the frame changed -- the "existing" branch of

@@ -150,7 +150,7 @@ static_assert(IM_MC_VERTICES < IM_MC_HOST && IM_MC_TRIS_ALLOC < IM_MC_HOST && IM
               IM_MC_STAT_FACETS < IM_MC_HOST && IM_MC_VERT_CHUNKS < IM_MC_HOST, "a slot the host reads lies outside its copy");
 static_assert(IM_MC_BAT_SELECTED < IM_MC_ALLOC, "mesh counter block too small");
 
-// ---- the counter bookkeeping of the frame stages (one thread of the kernels in mesh_capi.cu; the host emulation of the tests)
+// ---- the counter bookkeeping of the frame stages (one thread of the kernels in mesh_capi.cu and mesh_batched.cu; the host emulation of the tests)
 IM_HD void mesh_cnt_init(int* c) {   // create: c holds IM_MC_HOST zeros
     c[IM_MC_BBOX_MIN_X] = c[IM_MC_BBOX_MIN_Y] = c[IM_MC_BBOX_MIN_Z] = 0x7fffffff;
     c[IM_MC_BBOX_MAX_X] = c[IM_MC_BBOX_MAX_Y] = c[IM_MC_BBOX_MAX_Z] = -0x7fffffff;

@@ -1,10 +1,11 @@
-// immesh_b200 -- the one-block scan and the stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, 2048-element tiles;
+// immesh_b200 -- the one-block scan of a buffer and the stable LSD radix sort of (u32 key, u32 value) pairs, 8-bit digits, 2048-element tiles;
 // ranks inside a tile from __match_any_sync (warp) + per-warp digit counts in shared memory.  Used by the pcl::VoxelGrid front-end
 // (cell index -> point), the IMU undistortion (time stamp -> point), the plane-map publisher, the viewer's region buffers, the
 // batched frame and the mesh's change feed.  Include inside an anonymous namespace of a translation unit that includes common_host.hpp (IM_LAUNCH).
 #pragma once
 #define VG_TILE 2048
 #define VG_THREADS 256
+#include "block_scan.cuh"
 
 // ---- stable LSD radix sort, 8-bit digits.  hist is digit-major: hist[d * ntiles + t].  Each kernel has a variant (_dev) that reads
 // the count from the device: block b takes tiles b, b + gridDim.x, ... of the count's tiles, so that any grid gives the same result
@@ -27,30 +28,6 @@ __global__ void __launch_bounds__(VG_THREADS) k_rs_hist(const unsigned int* __re
 __global__ void __launch_bounds__(VG_THREADS) k_rs_hist_dev(const unsigned int* __restrict__ keys, const int* n_dev, int shift, int* hist) {
     const int n = *n_dev, nb = (n + VG_TILE - 1) / VG_TILE;
     for (int t = blockIdx.x; t < nb; t += gridDim.x) rs_hist_tile(keys, n, shift, hist, nb, t);
-}
-// exclusive scan of v over a block of 1024 threads, which all call it: warp shuffle, then a scan of the 32 warp totals in warp 0
-__device__ __forceinline__ int block_scan_1024(int v) {
-    __shared__ int s_warp[32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += u;
-    }
-    if (lane == 31) s_warp[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        int wv = s_warp[lane];
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, wv, o);
-            if (lane >= o) wv += u;
-        }
-        s_warp[lane] = wv;
-    }
-    __syncthreads();
-    return (warp ? s_warp[warp - 1] : 0) + x - v;
 }
 // exclusive scan of `len` ints in place by ONE block (len <= a few 100 k); total -> *total_out if not null
 __device__ __forceinline__ void rs_scan_block(int* a, int len, int* total_out) {

@@ -1,6 +1,6 @@
 // immesh_b200 -- the LiDAR point-cloud reinforcement (src/ImMesh_node.cpp:302-329 with g_if_depth_bind_cam): the depth camera's pose
 // from the last meshed frames (get_last_avr_pose, :169-206) and the depth rasterisation of the live mesh, as __host__ __device__
-// bodies shared by the kernels of mesh_capi.cu and the host emulation of the tests.
+// bodies shared by the kernels of mesh_render.cu and the host emulation of the tests.
 #pragma once
 #include <cuda_runtime.h>
 #include <cmath>

@@ -1,7 +1,7 @@
 // immesh_b200 -- the overlays of the queued mesh view (immesh_mesh_view_overlay, include/immesh_b200.h): what the reference's main
 // loop draws into the viewer's window besides the faces (src/ImMesh_node.cpp:422-470) -- the current scan, the reinforced points,
 // the axis, the ground grid, the wireframe, the sensor's camera frustum and the trajectory -- as __host__ __device__ bodies shared by
-// the kernels of mesh_capi.cu and the host emulation of the tests.  Everything is float64 in the order written, without fused
+// the kernels of mesh_render.cu and the host emulation of the tests.  Everything is float64 in the order written, without fused
 // multiply-adds (the library is built with -fmad=false).
 #pragma once
 #include "reinforce.cuh"

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE (not product code): the host emulation of the mesher (tests/emu/emu_mesh.cpp) with the m_smoothed flags
 // (MeshDev::vsmoothed) attached, plus immesh_mesh_push_frame_batched: the orchestration of the CUDA library's batched frame
-// (mesh_capi.cu, mesh_push_batched) on the same __host__ __device__ bodies, one thread at a time -- append chunks, the activation rule
+// (mesh_batched.cu, mesh_push_batched) on the same __host__ __device__ bodies, one thread at a time -- append chunks, the activation rule
 // after the last chunk, the meshed voxels in key order (rank = flip priority), pass 1 (every dilation's smoothing), pass 2 (dilation
 // lists again, triangulation, pull / commit, the batch's additions), removals after the last batch.  Built as its own library; the
 // per-handle batch state lives beside the handle and is dropped with it.

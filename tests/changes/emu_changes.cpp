@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE (not product code): the host emulation of the mesher with the batched frame (tests/batched/emu_batched.cpp) and
 // the change feed of immesh_mesh_changes_enable / immesh_mesh_changes.  The feed's __host__ __device__ bodies (mesh_changes.cuh, and
-// chg_touch inside apply_face) run one thread at a time in the device's order (mesh_capi.cu, mesh_changes_launch): the touched set
+// chg_touch inside apply_face) run one thread at a time in the device's order (mesh_feeds.cu, mesh_changes_launch): the touched set
 // after the push and before the frame's counter end (or the sweep), the rows against the published bytes, the ring append and the
 // header.  Only the LSD radix sort is replaced by a sort of the rows' triples (the triples of a frame are distinct, so both give the
 // same order).  The read side restates the host logic of immesh_mesh_changes.

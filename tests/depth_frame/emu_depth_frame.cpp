@@ -9,7 +9,7 @@
 
 using namespace immesh;
 
-#define DF_BLOCK 1024   // mesh_capi.cu
+#define DF_BLOCK 1024   // depth_kernels.cuh
 
 extern "C" {
 // img: the device image as the caller passes it (pitch bytes per row); cam = fx fy cx cy z_min z_max depth_scale R[9] t[3].  Writes the

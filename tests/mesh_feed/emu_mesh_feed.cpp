@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE (not product code): the mesh frame feed's rings on the host.  A frame's device work is run in the device's order
-// (mesh_capi.cu: k_mfeed_begin, then k_mfeed_head, k_mfeed_points, k_mfeed_image and k_mfeed_done) in two halves, so that a frame can be
+// (mesh_feeds.cu: k_mfeed_begin, then k_mfeed_head, k_mfeed_points, k_mfeed_image and k_mfeed_done) in two halves, so that a frame can be
 // left in flight: emu_mfeed_head marks the slot, writes the header and places the points and the image with mfeed_head (mesh_feed.cuh),
 // exactly as k_mfeed_head does; emu_mfeed_finish copies the points at mfeed_row_slot and the image at the image slot, refusing a slot
 // outside its ring as the kernels do, and publishes the frame as finished.  The reads are feed_read itself on mfeed_point_rings /
