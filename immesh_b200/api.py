@@ -63,7 +63,8 @@ class _FeedCfg(C.Structure):
 
 FEED_HDR = 12   # IMMESH_LIO_FEED_HDR: the header columns of a recorded scan, in this order
 FEED_HDR_KEYS = ("scan", "kind", "branch", "iters", "matches", "converged", "err", "row_begin", "row_effect_end", "row_end", "source", "rows_lost")
-FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i", "depth")   # IMMESH_FEED_KIND_*
+FEED_KINDS = ("step", "step_dev", "step_async", "step_async_dev_n", "raw", "raw_i", "imu", "imu_i", "depth", "depth_imu")   # IMMESH_FEED_KIND_*
+FEED_BRANCH_DROPPED = 4   # IMMESH_FEED_BRANCH_DROPPED: a step_async_depth_imu frame that sync_packages dropped
 
 
 MARKER_HDR = 10   # IMMESH_LIO_FEED_MARKER_HDR: the header columns of a scan's plane-marker record, in this order
@@ -287,6 +288,8 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_imu_device_points", [vp]),
         ("immesh_imu_get_poses", [vp, dp, C.c_int]),
         ("immesh_imu_init_begin", [vp, C.c_int]),
+        ("immesh_lio_step_async_depth_imu", [vp, vp, vp, dp, C.c_int, C.POINTER(_DepthFrame), vp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_float]),
+        ("immesh_imu_depth_chain_state", [vp, C.POINTER(C.c_int64)]),
         ("immesh_lio_step_async_imu", [vp, vp, vp, dp, C.c_int, vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, ip]),
         ("immesh_voxelgrid_filter_i", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp, ip, ip]),
         ("immesh_lio_step_async_raw_i", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_double, C.c_double, C.c_double]),
@@ -1331,6 +1334,20 @@ class VoxelGrid:
         lio._last_n = cnt
         return br.value
 
+    def step_async_depth_imu(self, lio: "Lio", imu_h: "Imu", batch, depth, cam: DepthCamera, frame_time: float, leaf: float, point_filter_num=1, blind=0.0,
+                             cam_R=np.eye(3), cam_t=np.zeros(3), on_device=False, shape=None, fmt="f32", pitch_bytes=0) -> int:
+        """The IMU-enabled loop on one depth frame (immesh_lio_step_async_depth_imu): batch float64[n_imu,7] (stamp, gyr, acc), the image's
+        cloud of prepare_depth with t = 0 at frame_time.  The drop rule and the branch are decided on the device; nothing is returned
+        about them (Imu.depth_chain_state, the scan feed).  Returns the sampled pixels, the n_max of
+        Mesh.push_frame_from_lio_async_dev_n(lio, input_points(), n_max, input_count())."""
+        im = np.ascontiguousarray(batch, dtype=np.float64).reshape(-1, 7)
+        f, ptr, _keep = Mesh._depth_args(cam, cam_R, cam_t, depth, shape, fmt, pitch_bytes, on_device)
+        _check(self.lib, self.lib.immesh_lio_step_async_depth_imu(lio._h, imu_h._h, self._h, im.ctypes.data_as(C.POINTER(C.c_double)), im.shape[0], C.byref(f), ptr,
+                                                                  1 if on_device else 0, int(point_filter_num), float(blind), float(frame_time), C.c_float(leaf)),
+               "lio_step_async_depth_imu")
+        lio._last_n = _sampled(f)
+        return lio._last_n
+
     def step_async_imu(self, lio: "Lio", imu_h: "Imu", batch, pts, lidar_beg_time: float, leaf: float, calib_laser=False, n=None, on_device=False) -> int:
         """The IMU-enabled scan loop, one queued call per scan (immesh_lio_step_async_imu): batch float64[n_imu,7] (stamp, gyr, acc);
         pts float32[n,4] (x, y, z, curvature ms) host array, or an integer CUDA address with n when on_device.  Returns the branch taken:
@@ -1387,6 +1404,13 @@ class Imu:
     def init_begin(self, max_ini_count: int = 3):
         """Enter the IMU initialisation phase of step_async_imu (first call: a fresh ImuProcess; later calls: the loop's reset)."""
         _check(self.lib, self.lib.immesh_imu_init_begin(self._h, max_ini_count), "imu_init_begin")
+
+    def depth_chain_state(self) -> dict:
+        """VoxelGrid.step_async_depth_imu's counters (immesh_imu_depth_chain_state; blocking)"""
+        out = (C.c_int64 * 8)()
+        _check(self.lib, self.lib.immesh_imu_depth_chain_state(self._h, out), "imu_depth_chain_state")
+        keys = ("calls", "dropped", "branch1", "branch2", "branch3", "carried", "carry_overflows", "init_finished")
+        return dict(zip(keys, (int(v) for v in out)))
 
     def undistort(self, lio: "Lio", imu, pts_xyzt, lidar_beg_time):
         """imu: float64[n_imu,7] (stamp, gyr, acc); pts_xyzt: float32[n,4] (x, y, z, curvature ms).  Returns the time-sorted, compensated cloud."""

@@ -147,6 +147,14 @@ def build_imu_chain(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "imu_chain", "emu_imu_chain.cpp"), EMU_IMU_CHAIN, force)
 
 
+EMU_DEPTH_IMU = os.path.join(_ROOT, "tests", "depth_imu", "libimmesh_emu_depth_imu.so")
+
+
+def build_depth_imu(force=False):
+    """tests/depth_imu: the depth IMU chain's device decision (sync_packages' drop and carry, the branch, IMU_init) built for the host"""
+    return _emu_ext(os.path.join(_ROOT, "tests", "depth_imu", "emu_depth_imu.cpp"), EMU_DEPTH_IMU, force)
+
+
 EMU_REINFORCE = os.path.join(_ROOT, "tests", "reinforce", "libimmesh_emu_reinforce.so")
 
 
@@ -303,6 +311,7 @@ def build_all(force=False):
     build_batched(force)
     build_growth(force)
     build_imu_chain(force)
+    build_depth_imu(force)
     build_reinforce(force)
     build_view(force)
     build_view_overlay(force)

@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -218,6 +219,16 @@ __global__ void __launch_bounds__(VG_THREADS) k_frontend_pack(const float* __res
         if (calib) immesh::kitti_calib_point(&x, &y, &z);
         dst[3 * (size_t)i] = x; dst[3 * (size_t)i + 1] = y; dst[3 * (size_t)i + 2] = z;
         if (dst_i) dst_i[i] = isrc[(size_t)i * istride];
+    }
+}
+// the depth IMU chain's undistorted cloud, x y z t -> packed [n][3]: *n_src points (the cloud in branches 2 and 3, else 0); block 0 sets
+// the ring slot's count to *n_keep (the cloud in branch 3 only: the frame the mesher is handed)
+__global__ void __launch_bounds__(VG_THREADS) k_dimu_pack(const float4* __restrict__ src, const int* n_src, const int* n_keep, float* __restrict__ dst, int* n_dst) {
+    const int n = *n_src;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *n_dst = *n_keep;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const float4 p = src[i];
+        dst[3 * (size_t)i] = p.x; dst[3 * (size_t)i + 1] = p.y; dst[3 * (size_t)i + 2] = p.z;
     }
 }
 
@@ -479,16 +490,23 @@ const int* immesh_voxelgrid_input_count(immesh_voxelgrid_t* h) { return h && h->
 // ---- depth images into the localization (immesh_frontend_prepare_depth, immesh_lio_step_async_depth): the image checked, then the
 // kernels of depth_kernels.cuh queued on st into the next input ring slot -- the filtered sensor-frame cloud and its count, both on the
 // device.  *n_sampled: the sampled pixels, the upper bound of the count.
-static int depth_pack(immesh_voxelgrid* h, const immesh_depth_frame* f, const void* img, int on_device, int point_filter_num, double blind, cudaStream_t st,
-                      int* n_sampled) {
+// The argument checks of a depth frame, nothing queued: *d set up from the image, *n_sampled its sampled pixels.
+static int depth_check(immesh_voxelgrid* h, const immesh_depth_frame* f, const void* img, int point_filter_num, double blind, immesh::DepthFrame* d,
+                       long long* pitch, int* bpp, int* n_sampled) {
     if (point_filter_num < 1) return im_fail(IMMESH_E_INVALID, "depth frame: point_filter_num must be >= 1");
     if (!(blind >= 0.0 && std::isfinite(blind))) return im_fail(IMMESH_E_INVALID, "depth frame: blind must be finite and >= 0");
+    if (const char* bad = immesh::depth_frame_setup(f, img, d, pitch, bpp)) return im_fail(IMMESH_E_INVALID, bad);
+    if ((long long)d->sw * d->sh > h->max_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than the VoxelGrid's max_points");
+    *n_sampled = d->sw * d->sh;
+    return IMMESH_OK;
+}
+// wait_ms (or null): the host time spent waiting for the previous image's copy out of the staging buffer is added there
+static int depth_pack(immesh_voxelgrid* h, const immesh_depth_frame* f, const void* img, int on_device, int point_filter_num, double blind, cudaStream_t st,
+                      int* n_sampled, double* wait_ms = nullptr) {
     immesh::DepthFrame d;
     long long pitch = 0;
-    int bpp = 0;
-    if (const char* bad = immesh::depth_frame_setup(f, img, &d, &pitch, &bpp)) return im_fail(IMMESH_E_INVALID, bad);
-    const int ns = d.sw * d.sh;
-    if ((long long)d.sw * d.sh > h->max_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than the VoxelGrid's max_points");
+    int bpp = 0, ns = 0;
+    if (const int rc = depth_check(h, f, img, point_filter_num, blind, &d, &pitch, &bpp, &ns)) return rc;
     auto& D = h->dep;
     if (!D.d_n) {   // all or nothing: after a failure the handle is as it was
         const size_t nb = (size_t)(h->max_points + DF_BLOCK - 1) / DF_BLOCK;
@@ -509,7 +527,12 @@ static int depth_pack(immesh_voxelgrid* h, const immesh_depth_frame* f, const vo
     const int k = h->in_idx;
     h->d_in = h->d_in_ring[k];
     if (!on_device) {   // the sampled grid, tight, through the pinned staging (sw * sh * bpp <= 4 max_points bytes, within h_raw)
-        if (h->raw_pending) { IM_CUDA(cudaEventSynchronize(h->ev_raw)); h->raw_pending = 0; }   // the previous copy out of the staging buffer
+        if (h->raw_pending) {   // the previous copy out of the staging buffer
+            const auto t0 = std::chrono::steady_clock::now();
+            IM_CUDA(cudaEventSynchronize(h->ev_raw));
+            if (wait_ms) *wait_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+            h->raw_pending = 0;
+        }
         unsigned char* hb = reinterpret_cast<unsigned char*>(h->h_raw);
         immesh::depth_stage_grid(d, static_cast<const unsigned char*>(img), pitch, bpp, hb);
         IM_CUDA(cudaMemcpyAsync(h->d_raw, hb, (size_t)ns * bpp, cudaMemcpyHostToDevice, st));
@@ -680,6 +703,56 @@ const float* immesh_voxelgrid_device_points(immesh_voxelgrid_t* h) { return h ? 
 // cloud -- [calibration] + repack into the input ring (immesh_voxelgrid_input_points), then the build kernels on the packed full scan
 int immesh_voxelgrid_max_points(immesh_voxelgrid_t* h) { return h ? h->max_points : 0; }
 int immesh_voxelmap_build_async_dev(immesh_lio_t* lio, const float* d_body_xyz, int n);   // lio_capi.cu
+// internal (immesh_lio_step_async_depth_imu): the depth frame's checks (*n_sampled: its sampled pixels), and its cloud queued on the
+// localization stream into the next input ring slot (*d_xyz, count *d_n on the device)
+int immesh_frontend_depth_check(immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int point_filter_num, double blind, int* n_sampled) {
+    immesh::DepthFrame d;
+    long long pitch = 0;
+    int bpp = 0;
+    return depth_check(h, f, depth, point_filter_num, blind, &d, &pitch, &bpp, n_sampled);
+}
+int immesh_frontend_depth_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num,
+                                double blind, const float** d_xyz, const int** d_n) {
+    lio->fe_vg = nullptr;
+    int ns = 0;
+    const int rc = depth_pack(h, f, depth, on_device, point_filter_num, blind, lio->stream, &ns, &lio->host_wait_ms);   // staging back-pressure
+    if (rc) return rc;
+    *d_xyz = h->d_in;
+    *d_n = h->dep.d_n + h->in_idx;
+    return IMMESH_OK;
+}
+// internal (immesh_lio_step_async_depth_imu): the chain behind UndistortPcl, every branch launched and every count read on the device.
+// d_xyzt: the undistorted cloud, *d_und points (0 unless branch 2 or 3); *d_b2 / *d_b3: the cloud's count in branch 2 / 3, else 0.
+//   pack        -> back into the input ring slot immesh_frontend_depth_async unprojected into (one slot per call, as on every chain: a
+//                  mesh frame may still read the slot of up to IM_SLOTS + 1 calls ago), its count *d_b3 (the mesher's frame)
+//   voxel_map_init of *d_b2 points (builds nothing unless branch 2; records no scan)
+//   VoxelGrid(leaf) of *d_b3 points -> predict (dt 0: none) + IESKF + map update of the down-sampled cloud: nothing unless branch 3.  Its
+//   scan is the frame's one scan-feed record, with the device branch.
+int immesh_voxelmap_build_async_dev_n(immesh_lio_t* h, const float* d_body_xyz, int n_max, const int* d_n);   // lio_capi.cu
+int immesh_frontend_depth_imu_tail(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_xyzt, int n_max, const int* d_und, const int* d_b2, const int* d_b3,
+                                   const int* d_branch, float leaf) {
+    cudaStream_t st = lio->stream;
+    lio->fe_vg = nullptr;
+    const int k = h->in_idx;   // the k_dimu_expand of the same call has read the unprojected cloud out of it
+    IM_LAUNCH(k_dimu_pack, std::min((n_max + VG_THREADS - 1) / VG_THREADS, h->n_sm * 8), VG_THREADS, 0, st, (const float4*)d_xyzt, d_und, d_b3, h->d_in,
+              h->dep.d_n + k);
+    int rc = immesh_voxelmap_build_async_dev_n(lio, h->d_in, n_max, d_b2);
+    if (rc) return rc;
+    rc = vg_enqueue(h, h->d_in, n_max, leaf, st, nullptr, d_b3);
+    if (rc) return rc;
+    immesh_lio::FeedNext& nx = lio->feed_next;   // the scan feed's full scan (registered source 2): the undistorted cloud, as for the IMU chain
+    nx.kind = IMMESH_FEED_KIND_DEPTH_IMU;
+    nx.branch = 0;
+    nx.branch_dev = d_branch;
+    nx.pts = h->d_in;
+    nx.inten = nullptr;
+    nx.n = n_max;
+    nx.n_dev = d_b3;
+    rc = immesh_lio_step_async_dev_n(lio, h->d_out, n_max < lio->max_scan ? n_max : lio->max_scan, &h->d_grid->m_out, 0.0, 0.0, 0.0);
+    lio->feed_next = immesh_lio::FeedNext();
+    return rc;
+}
+
 int immesh_frontend_build_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_pts, int n, int stride, int calib_laser, const float* d_inten) {
     if (!lio || !h || !d_pts || n < 1 || (stride != 3 && stride != 4)) return im_fail(IMMESH_E_INVALID, "bad argument");
     if (n > h->max_points) return im_fail(IMMESH_E_CAPACITY, "cloud larger than max_points");

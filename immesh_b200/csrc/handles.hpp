@@ -113,6 +113,7 @@ struct immesh_lio {
         const float* pts = nullptr;     // the full scan (registered source 2)
         const float* inten = nullptr;   // its intensity, or null
         const int* n_dev = nullptr;     // its count when that is device resident (n: the upper bound)
+        const int* branch_dev = nullptr;   // the branch when the device decides it (immesh_lio_step_async_depth_imu)
     } feed_next;
     // scan feed (immesh_lio_feed_enable)
     struct Feed {

@@ -10,6 +10,13 @@
 //   k_imu_keys      time-stamp keys (ordered-uint image of the float curvature) for the stable radix sort (radix_sort.cuh)
 //   k_imu_gather    points in time order
 //   k_imu_undistort thread per point: interval lookup + rigid transform into the scan-end frame (16 B in, 16 B out per point)
+// The depth IMU chain (immesh_lio_step_async_depth_imu) decides its branch on the device, from the depth cloud's device count:
+//   k_dimu_branch   one block: sync_packages' drop rule and carry (src/voxel_mapping_common.cpp:393-400), the batch carried + own,
+//                   the branch of Process2 / service_LiDAR_update, and the counts every later kernel of the frame reads
+//   k_dimu_init     branch 1: IMU_init (imu_init_batch, the host chain's code) and the init-end test, on the device
+//   k_dimu_expand   the cloud as x y z t, t = 0 (l515_handler's curvature, src/preprocess.cpp:270): the stable time sort of all-equal
+//                   stamps is the identity, so this is the sorted cloud
+//   k_imu_forward_dn / k_imu_undistort_dn   k_imu_forward / k_imu_undistort with the counts and mean_acc_norm read on the device
 // There is no CPU path.
 #include <cuda_runtime.h>
 
@@ -24,7 +31,7 @@
 #include "handles.hpp"
 #include "imu_core.cuh"
 
-using immesh::im_fail; using immesh::ImuParams; using immesh::ImuStep; using immesh::ImuTime; using immesh::ImuInit;
+using immesh::im_fail; using immesh::ImuParams; using immesh::ImuStep; using immesh::ImuTime; using immesh::ImuInit; using immesh::DepthImu;
 
 namespace {
 
@@ -33,8 +40,8 @@ namespace {
 #define IMU_FWD_THREADS 352
 
 // pts: the scan as given (unsorted), read for its last point's stamp only
-__global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward(ImuParams P, LioCtrl* ctrl, double* run, ImuTime* tm, const double* imu, int n_imu, const float* pts, int n,
-                                                                  double lidar_beg_time, ImuStep* steps, double* poses) {
+__device__ __forceinline__ void imu_forward_block(const ImuParams& P, LioCtrl* ctrl, double* run, ImuTime* tm, const double* imu, int n_imu, const float* pts, int n,
+                                                  double lidar_beg_time, ImuStep* steps, double* poses) {
     __shared__ double Fx[324], T[324];
     __shared__ double s_note, s_dt;
     __shared__ int s_steps;
@@ -50,6 +57,10 @@ __global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward(ImuParams P, Li
     for (int k = 0; k < n_steps; ++k)
         immesh::imu_forward_step(P, ctrl->state, run, steps[k], poses + (size_t)(k + 1) * IM_POSE_DOUBLES, Fx, T, threadIdx.x, blockDim.x);
     if (threadIdx.x == 0) immesh::imu_predict_end(ctrl->state, run, s_note, s_dt);
+}
+__global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward(ImuParams P, LioCtrl* ctrl, double* run, ImuTime* tm, const double* imu, int n_imu, const float* pts, int n,
+                                                                  double lidar_beg_time, ImuStep* steps, double* poses) {
+    imu_forward_block(P, ctrl, run, tm, imu, n_imu, pts, n, lidar_beg_time, steps, poses);
 }
 __global__ void __launch_bounds__(VG_THREADS) k_imu_keys(const float* __restrict__ pts, int n, unsigned int* keys, unsigned int* vals) {
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -76,7 +87,7 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_gather(const float4* __restr
     }
 }
 // the IMUpose count comes from the plan (ImuTime::n_pose); the dynamic shared memory is sized for the batch's upper bound
-__global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm, float* pts, int n) {
+__device__ __forceinline__ void imu_undistort_block(const ImuParams& P, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm, float* pts, int n) {
     extern __shared__ double s_pose[];
     __shared__ double s_end[12];
     const int n_pose = tm->n_pose;
@@ -84,6 +95,48 @@ __global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const
     if (threadIdx.x < 12) s_end[threadIdx.x] = ctrl->state[threadIdx.x];
     __syncthreads();
     for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) immesh::imu_undistort_point(P, s_end, s_pose, n_pose, pts, s);
+}
+__global__ void __launch_bounds__(VG_THREADS) k_imu_undistort(ImuParams P, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm, float* pts, int n) {
+    imu_undistort_block(P, ctrl, poses, tm, pts, n);
+}
+
+// ---- the depth IMU chain: the decision of imu_core.cuh (dimu_decide, dimu_init, dimu_begin) on one thread, in stream order
+static_assert(IM_DIMU_DROPPED == IMMESH_FEED_BRANCH_DROPPED, "the dropped branch is the feed's");
+__global__ void k_dimu_branch(DepthImu* D, const int* d_n, const double* __restrict__ own, int n_own, double* batch, int max_imu, int* err) {
+    __shared__ int s_base;
+    if (threadIdx.x == 0) {
+        int overflow = 0;
+        s_base = immesh::dimu_decide(*D, *d_n, n_own, max_imu, &overflow);
+        if (overflow) atomicOr(err, immesh::IM_ERR_IMU_CARRY);
+    }
+    __syncthreads();
+    const int base = s_base;
+    if (base >= 0)
+        for (int i = threadIdx.x; i < 7 * n_own; i += blockDim.x) batch[7 * (size_t)base + i] = own[i];
+}
+__global__ void k_dimu_init(DepthImu* D, const double* __restrict__ batch, double* state, ImuTime* tm, double frame_time) {
+    if (threadIdx.x == 0) immesh::dimu_init(*D, batch, state, *tm, frame_time);
+}
+__global__ void k_dimu_begin(DepthImu* D, int fresh, int max_ini) {
+    if (threadIdx.x == 0) immesh::dimu_begin(*D, fresh, max_ini);
+}
+__global__ void __launch_bounds__(VG_THREADS) k_dimu_expand(const DepthImu* D, const float* __restrict__ xyz, float4* out) {
+    const int n = D->n_und;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        out[i] = make_float4(xyz[3 * (size_t)i], xyz[3 * (size_t)i + 1], xyz[3 * (size_t)i + 2], 0.0f);
+}
+__global__ void __launch_bounds__(IMU_FWD_THREADS) k_imu_forward_dn(ImuParams P, const DepthImu* D, LioCtrl* ctrl, double* run, ImuTime* tm, const double* imu,
+                                                                     const float* pts, double lidar_beg_time, ImuStep* steps, double* poses) {
+    const int n = D->n_und;
+    if (n <= 0) return;   // block-uniform: branches 2 and 3 only
+    P.mean_acc_norm = D->mean_acc_norm;
+    imu_forward_block(P, ctrl, run, tm, imu, D->n_imu, pts, n, lidar_beg_time, steps, poses);
+}
+__global__ void __launch_bounds__(VG_THREADS) k_imu_undistort_dn(ImuParams P, const DepthImu* D, const LioCtrl* ctrl, const double* __restrict__ poses, const ImuTime* tm,
+                                                                  float* pts) {
+    const int n = D->n_und;
+    if (n <= 0) return;
+    imu_undistort_block(P, ctrl, poses, tm, pts, n);
 }
 
 }  // namespace
@@ -122,6 +175,14 @@ struct immesh_imu {
     float* h_rec = nullptr; // pinned, IM_SLOTS slots of [max_points][rec_stride]
     float* d_in_i = nullptr;   // [max_points] intensity in scan order
     float* d_out_i = nullptr;  // [max_points] intensity in time order (beside d_out)
+    // which chain runs on the handle: 0 none yet, 1 immesh_lio_step_async_imu[_i] (phase on the host), 2 immesh_lio_step_async_depth_imu
+    // (phase on the device, in d_dimu; allocated by its first call with d_own)
+    int chain = 0;
+    DepthImu* d_dimu = nullptr;
+    DepthImu* h_dimu = nullptr;   // pinned: the first call's upload, the state query's read
+    double* d_own = nullptr;      // [max_imu][7] the frame's own samples (d_imu holds the batch)
+    int dimu_begin = 0;           // immesh_imu_init_begin since the last depth call: k_dimu_begin is due
+    int dimu_fresh = 0;           //   and it was the handle's first (a fresh ImuProcess)
     immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // every buffer above
 };
 
@@ -315,10 +376,12 @@ int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count) {
     if (!h || max_ini_count < 0) return im_fail(IMMESH_E_INVALID, "bad argument");
     h->init_phase = 1;
     h->max_ini = max_ini_count;
+    h->dimu_begin = 1;
     immesh::imu_init_reset(h->ini);
     if (!h->began) {   // a fresh ImuProcess: b_first_frame_, zero members
         h->began = 1;
         h->ini.first_frame = 1;
+        h->dimu_fresh = 1;
         h->pending_reset = 2;
     } else {           // the loop's reset (m_flg_reset -> Reset()): b_first_frame_ stays false
         h->pending_reset = std::max(h->pending_reset, 1);
@@ -327,6 +390,21 @@ int immesh_imu_init_begin(immesh_imu_t* h, int max_ini_count) {
 }
 
 }  // extern "C"
+
+// the members immesh_imu_init_begin resets, in stream order ahead of the next scan
+static int imu_pending_reset(immesh_imu* h, cudaStream_t st) {
+    if (h->pending_reset) {
+        if (h->pending_reset == 2) {   // a fresh ImuProcess (last_lidar_end_time_ = 0.0, see the header)
+            IM_CUDA(cudaMemsetAsync(h->d_time, 0, sizeof(ImuTime), st));
+            IM_CUDA(cudaMemsetAsync(h->d_run, 0, 6 * sizeof(double), st));
+        } else {                       // Reset(): last_imu_ and angvel_last; acc_s_last and last_lidar_end_time_ are kept
+            IM_CUDA(cudaMemsetAsync(h->d_time->last_imu, 0, 7 * sizeof(double), st));
+            IM_CUDA(cudaMemsetAsync(h->d_run + 3, 0, 3 * sizeof(double), st));
+        }
+        h->pending_reset = 0;
+    }
+    return IMMESH_OK;
+}
 
 // the loop of immesh_lio_step_async_imu (icol < 0: [n][4] x y z t) and immesh_lio_step_async_imu_i (records of `stride` floats, the time
 // stamp in column tcol, the intensity in icol, carried through the sort, the calibration and the VoxelGrid)
@@ -338,6 +416,7 @@ static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg,
     if (n_imu > h->max_imu) return im_fail(IMMESH_E_CAPACITY, "IMU batch larger than the IMU handle's max_imu");
     if (n > h->max_points || n > immesh_voxelgrid_max_points(vg)) return im_fail(IMMESH_E_CAPACITY, "scan larger than the IMU / VoxelGrid handle's max_points");
     if (n > lio->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than the localization handle's max_scan_points (the map is built from the whole scan, and a scan the VoxelGrid passes through reaches the step whole)");
+    if (h->chain == 2) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_imu: the IMU handle runs immesh_lio_step_async_depth_imu (its phase is on the device)");
     cudaStream_t st = lio->stream;
     lio->fe_vg = nullptr;   // branches 1 and 2 publish nothing (voxel_mapping.cpp:1879, :1903)
     const int feed_kind = icol >= 0 ? IMMESH_FEED_KIND_IMU_I : IMMESH_FEED_KIND_IMU;   // how the scan feed records this scan
@@ -345,16 +424,9 @@ static int imu_chain(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg,
         const int rc = imu_records_alloc(h, on_device ? 0 : stride);
         if (rc) return rc;
     }
-    if (h->pending_reset) {
-        if (h->pending_reset == 2) {   // a fresh ImuProcess (last_lidar_end_time_ = 0.0, see the header)
-            IM_CUDA(cudaMemsetAsync(h->d_time, 0, sizeof(ImuTime), st));
-            IM_CUDA(cudaMemsetAsync(h->d_run, 0, 6 * sizeof(double), st));
-        } else {                       // Reset(): last_imu_ and angvel_last; acc_s_last and last_lidar_end_time_ are kept
-            IM_CUDA(cudaMemsetAsync(h->d_time->last_imu, 0, 7 * sizeof(double), st));
-            IM_CUDA(cudaMemsetAsync(h->d_run + 3, 0, 3 * sizeof(double), st));
-        }
-        h->pending_reset = 0;
-    }
+    h->chain = 1;
+    int prc = imu_pending_reset(h, st);
+    if (prc) return prc;
     const int s = imu_stage_slot(h, lio);
     if (h->init_phase) {
         // branch 1 (Process2 :973-1003): lidar_meas.last_update_time = pcl_end_time; IMU_init on a non-empty batch
@@ -433,6 +505,96 @@ int immesh_lio_step_async_imu_i(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxel
         return im_fail(IMMESH_E_INVALID, "bad records (stride <= 16; time_col and intensity_col distinct, >= 3 and < stride)");
     if (lio && lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_imu_i runs on a single GPU: the localization handle is sharded");
     return imu_chain(lio, h, vg, imu, n_imu, pts, n, stride, time_col, intensity_col, on_device, lidar_beg_time, calib_laser, leaf, branch_out);
+}
+
+// internal entry points of frontend_capi.cu (the depth frame's cloud, and the chain behind UndistortPcl)
+int immesh_frontend_depth_check(immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int point_filter_num, double blind, int* n_sampled);
+int immesh_frontend_depth_async(immesh_lio_t* lio, immesh_voxelgrid_t* h, const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num,
+                                double blind, const float** d_xyz, const int** d_n);
+int immesh_frontend_depth_imu_tail(immesh_lio_t* lio, immesh_voxelgrid_t* h, const float* d_xyzt, int n_max, const int* d_und, const int* d_b2, const int* d_b3,
+                                   const int* d_branch, float leaf);
+
+// The IMU-enabled loop on depth frames: one queued call per frame, every branch decided on the device (see the header).  The host
+// queues the same launches whatever the frame holds; each kernel returns early unless its branch is the one the device took.
+int immesh_lio_step_async_depth_imu(immesh_lio_t* lio, immesh_imu_t* h, immesh_voxelgrid_t* vg, const double* imu, int n_imu, const immesh_depth_frame* f,
+                                    const void* depth, int on_device, int point_filter_num, double blind, double frame_time, float leaf) {
+    if (!lio || !h || !vg || (!imu && n_imu > 0) || n_imu < 0 || !(leaf > 0.f)) return im_fail(IMMESH_E_INVALID, "bad argument");
+    if (lio->P.shard_n > 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_depth_imu runs on a single GPU: the localization handle is sharded");
+    if (h->chain == 1) return im_fail(IMMESH_E_INVALID, "immesh_lio_step_async_depth_imu: the IMU handle runs immesh_lio_step_async_imu (its phase is on the host)");
+    int ns = 0;
+    int rc = immesh_frontend_depth_check(vg, f, depth, point_filter_num, blind, &ns);
+    if (rc) return rc;
+    if (n_imu > h->max_imu) return im_fail(IMMESH_E_CAPACITY, "IMU batch larger than the IMU handle's max_imu");
+    if (ns > h->max_points) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than the IMU handle's max_points");
+    if (ns > lio->max_scan) return im_fail(IMMESH_E_CAPACITY, "depth frame: more sampled pixels than the localization handle's max_scan_points (the map is built from the whole cloud)");
+    cudaStream_t st = lio->stream;
+    if (!h->d_dimu) {   // all or nothing; the device phase starts from the host's (immesh_imu_init_begin before the first call, or none)
+        immesh::MemSet dev, pinned(immesh::MemSet::Pinned);
+        DepthImu *d_dimu, *h_dimu;
+        double* d_own;
+        IM_CUDA(dev.alloc(&d_dimu, 1));
+        IM_CUDA(pinned.alloc(&h_dimu, 1));
+        IM_CUDA(dev.alloc(&d_own, (size_t)h->max_imu * 7));
+        std::memset(h_dimu, 0, sizeof(DepthImu));
+        h_dimu->ini = h->ini;
+        h_dimu->mean_acc_norm = h->P.mean_acc_norm;
+        h_dimu->init_phase = h->init_phase;
+        h_dimu->max_ini = h->max_ini;
+        h_dimu->map_built = h->map_built;
+        IM_CUDA(cudaMemcpyAsync(d_dimu, h_dimu, sizeof(DepthImu), cudaMemcpyHostToDevice, st));
+        h->d_dimu = d_dimu; h->h_dimu = h_dimu; h->d_own = d_own;
+        h->dev.take(std::move(dev));
+        h->pinned.take(std::move(pinned));
+        h->dimu_begin = 0;   // the upload carries the host's phase, b_first_frame_ included
+        h->dimu_fresh = 0;
+    }
+    h->chain = 2;
+    rc = imu_pending_reset(h, st);
+    if (rc) return rc;
+    if (h->dimu_begin) {
+        IM_LAUNCH(k_dimu_begin, 1, 32, 0, st, h->d_dimu, h->dimu_fresh, h->max_ini);
+        h->dimu_begin = 0;
+        h->dimu_fresh = 0;
+    }
+    const float* d_xyz = nullptr;
+    const int* d_n = nullptr;
+    rc = immesh_frontend_depth_async(lio, vg, f, depth, on_device, point_filter_num, blind, &d_xyz, &d_n);
+    if (rc) return rc;
+    const int s = imu_stage_slot(h, lio);
+    if (n_imu > 0) {
+        double* hi = h->h_imu + (size_t)s * h->slot_doubles;
+        std::memcpy(hi, imu, (size_t)n_imu * 7 * sizeof(double));
+        IM_CUDA(cudaMemcpyAsync(h->d_own, hi, (size_t)n_imu * 7 * sizeof(double), cudaMemcpyHostToDevice, st));
+    }
+    rc = imu_stage_release(h, s, st);
+    if (rc) return rc;
+    DepthImu* D = h->d_dimu;
+    const int gs = std::min((ns + VG_THREADS - 1) / VG_THREADS, h->n_sm * 8);
+    IM_LAUNCH(k_dimu_branch, 1, 128, 0, st, D, d_n, (const double*)h->d_own, n_imu, h->d_imu, h->max_imu, lio->d_counters + immesh::IM_LC_ERR);
+    IM_LAUNCH(k_dimu_init, 1, 32, 0, st, D, (const double*)h->d_imu, lio->d_ctrl->state, h->d_time, frame_time);
+    IM_LAUNCH(k_dimu_expand, gs, VG_THREADS, 0, st, (const DepthImu*)D, d_xyz, (float4*)h->d_out);
+    IM_LAUNCH(k_imu_forward_dn, 1, IMU_FWD_THREADS, 0, st, h->P, (const DepthImu*)D, lio->d_ctrl, h->d_run, h->d_time, (const double*)h->d_imu, (const float*)h->d_out,
+              frame_time, h->d_steps, h->d_poses);
+    const size_t smem = (size_t)(h->max_imu + 1) * IM_POSE_DOUBLES * sizeof(double);   // IMUpose holds at most (carried + own) + 1 entries
+    IM_LAUNCH(k_imu_undistort_dn, gs, VG_THREADS, smem, st, h->P, (const DepthImu*)D, (const LioCtrl*)lio->d_ctrl, (const double*)h->d_poses, (const ImuTime*)h->d_time,
+              h->d_out);
+    IM_CUDA(cudaGetLastError());
+    lio->pose_pub_idx = -1;
+    return immesh_frontend_depth_imu_tail(lio, vg, h->d_out, ns, &D->n_und, &D->n_b2, &D->n_b3, &D->branch, leaf);
+}
+
+int immesh_imu_depth_chain_state(immesh_imu_t* h, int64_t out[8]) {
+    if (!h || !out) return im_fail(IMMESH_E_INVALID, "null argument");
+    for (int i = 0; i < 8; ++i) out[i] = 0;
+    if (!h->d_dimu) {
+        out[7] = h->init_phase ? 0 : 1;
+        return IMMESH_OK;
+    }
+    IM_CUDA(cudaDeviceSynchronize());
+    IM_CUDA(cudaMemcpy(h->h_dimu, h->d_dimu, sizeof(DepthImu), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < 7; ++i) out[i] = h->h_dimu->cnt[i];
+    out[7] = h->h_dimu->init_phase ? 0 : 1;
+    return IMMESH_OK;
 }
 
 }  // extern "C"

@@ -2,7 +2,8 @@
 // (/root/reference/src/IMU_Processing.cpp:755-958) and the host part of IMU_init (:188-232).  Split of the work:
 //   imu_plan                : time stamps only -- which IMU intervals are live, their dt / offset, the scan-end dt and sign (one thread
 //                             of k_imu_forward, on the members carried in ImuTime)
-//   imu_init_batch          : IMU_init's running means on the host (the samples are host data)
+//   imu_init_batch          : IMU_init's running means: on the host for immesh_lio_step_async_imu (the samples are host data), on the
+//                             device for immesh_lio_step_async_depth_imu (the batch is assembled there); one implementation for both
 //   imu_forward_step        : one IMU interval: bias / gravity-scale correction, 18x18 covariance propagation F P F^T + Q,
 //                             attitude / velocity / position integration, IMUpose record (block-cooperative, tid / nthreads)
 //   imu_predict_end         : state at the scan end (:881-896)
@@ -69,7 +70,7 @@ IM_HDN inline int imu_plan(ImuTime& tm, const double* imu, int n_imu, float last
     return n_steps;
 }
 
-// IMU_init, StatesGroup version (IMU_Processing.cpp:188-232), on the host: the IMU samples arrive in host memory and nothing else is read.
+// IMU_init, StatesGroup version (IMU_Processing.cpp:188-232): the samples in the reference's order, nothing else read.
 // The covariance lines are commented out in the reference and absent here.
 struct ImuInit {
     double mean_acc[3], mean_gyr[3];
@@ -77,13 +78,13 @@ struct ImuInit {
     int first_frame;   // b_first_frame_
 };
 // ImuProcess::Reset() as far as IMU_init's members go (:73-86)
-inline void imu_init_reset(ImuInit& s) {
+IM_HDN inline void imu_init_reset(ImuInit& s) {
     s.mean_acc[0] = 0.0; s.mean_acc[1] = 0.0; s.mean_acc[2] = -1.0;
     s.mean_gyr[0] = s.mean_gyr[1] = s.mean_gyr[2] = 0.0;
     s.N = 1;
 }
 // one non-empty batch; returns |mean_acc| and gravity = -mean_acc / |mean_acc| * G_m_s2 (rot_end = I, bias_g = 0 are the caller's)
-inline double imu_init_batch(ImuInit& s, const double* imu, int n_imu, double* gravity) {
+IM_HDN inline double imu_init_batch(ImuInit& s, const double* imu, int n_imu, double* gravity) {
     if (s.first_frame) {
         imu_init_reset(s);
         s.first_frame = 0;
@@ -95,9 +96,86 @@ inline double imu_init_batch(ImuInit& s, const double* imu, int n_imu, double* g
         for (int i = 0; i < 3; ++i) { s.mean_acc[i] = s.mean_acc[i] + (m[4 + i] - s.mean_acc[i]) / N; s.mean_gyr[i] = s.mean_gyr[i] + (m[1 + i] - s.mean_gyr[i]) / N; }
         s.N++;
     }
-    const double norm = std::sqrt((s.mean_acc[0] * s.mean_acc[0] + s.mean_acc[1] * s.mean_acc[1]) + s.mean_acc[2] * s.mean_acc[2]);
+    const double norm = sqrt((s.mean_acc[0] * s.mean_acc[0] + s.mean_acc[1] * s.mean_acc[1]) + s.mean_acc[2] * s.mean_acc[2]);
     for (int i = 0; i < 3; ++i) gravity[i] = -s.mean_acc[i] / norm * 9.81;
     return norm;
+}
+
+// ---- the depth IMU chain (immesh_lio_step_async_depth_imu): the device-resident phase of ImuProcess and of the loop around it, and the
+// decision of a frame, which one thread takes on the device (k_dimu_branch, k_dimu_init) and the host emulation restates.
+#define IM_DIMU_DROPPED 4   // IMMESH_FEED_BRANCH_DROPPED
+struct DepthImu {
+    ImuInit ini;           // IMU_init's running means (init_iter_num, b_first_frame_)
+    double mean_acc_norm;  // UndistortPcl's scale: the configured value until IMU_init ends, then |mean_acc|
+    int init_phase;        // imu_need_init_
+    int max_ini;           // MAX_INI_COUNT
+    int map_built;         // m_init_map
+    int carry;             // IMU samples of dropped frames, at the front of the batch buffer
+    int branch;            // this frame's: 1, 2, 3 or IM_DIMU_DROPPED
+    int n;                 // this frame's cloud
+    int n_imu;             // this frame's batch: carried + own samples
+    int n_und, n_b2, n_b3; // the cloud in branches 2 and 3 / 2 / 3, else 0: the counts the later kernels read
+    long long cnt[8];      // calls, dropped, branch-1, -2, -3 frames, carried samples, carry overflows (immesh_imu_depth_chain_state)
+};
+// sync_packages (src/voxel_mapping_common.cpp:393-400): a cloud of <= 1 point is dropped and its IMU samples stay buffered for the next
+// frame, whose meas.imu is then carried + own samples in arrival order.  More than max_imu of them: the frame is dropped and its own
+// samples discarded (*overflow = 1).  Otherwise the branch of Process2 (IMU_Processing.cpp:973-1003) and service_LiDAR_update
+// (voxel_mapping.cpp:1894-1905).  Returns the batch index the frame's own samples go to, or -1 when they are discarded.
+IM_HDN inline int dimu_decide(DepthImu& D, int n, int n_own, int max_imu, int* overflow) {
+    const int carry = D.carry, total = carry + n_own;
+    int br = IM_DIMU_DROPPED, base = carry;
+    *overflow = 0;
+    if (total > max_imu) {
+        *overflow = 1;
+        base = -1;
+        D.cnt[6] += 1;
+    } else if (n <= 1) {
+        D.carry = total;
+    } else {
+        D.carry = 0;
+        D.n_imu = total;
+        br = D.init_phase ? 1 : D.map_built ? 3 : 2;
+        if (br == 2) D.map_built = 1;
+    }
+    D.cnt[0] += 1;
+    D.cnt[br == IM_DIMU_DROPPED ? 1 : 1 + br] += 1;
+    D.cnt[5] = D.carry;
+    D.branch = br;
+    D.n = n;
+    D.n_und = br == 2 || br == 3 ? n : 0;
+    D.n_b2 = br == 2 ? n : 0;
+    D.n_b3 = br == 3 ? n : 0;
+    return base;
+}
+// branch 1 (Process2 :973-1003): lidar_meas.last_update_time = pcl_end_time (frame_time + 0 / 1000: the depth points' curvature is 0);
+// on a non-empty batch IMU_init, rot_end = I, bias_g = 0, gravity, last_imu_ = the batch's last sample, and the init-end test
+// init_iter_num > MAX_INI_COUNT.  state: the 348-double state.  Other branches: nothing.
+IM_HDN inline void dimu_init(DepthImu& D, const double* batch, double* state, ImuTime& tm, double frame_time) {
+    if (D.branch != 1) return;
+    tm.upd_beg = frame_time;
+    tm.upd_curv = 0.0f;
+    const int n_imu = D.n_imu;
+    if (n_imu == 0) return;
+    double grav[3];
+    const double norm = imu_init_batch(D.ini, batch, n_imu, grav);
+    for (int i = 0; i < 9; ++i) state[i] = (i % 4 == 0) ? 1.0 : 0.0;
+    for (int i = 0; i < 3; ++i) { state[15 + i] = 0.0; state[21 + i] = grav[i]; }
+    for (int i = 0; i < 7; ++i) tm.last_imu[i] = batch[7 * (size_t)(n_imu - 1) + i];
+    if (D.ini.N > D.max_ini) {
+        D.init_phase = 0;
+        D.mean_acc_norm = norm;
+    }
+}
+// immesh_imu_init_begin on a handle whose phase is on the device: Reset() of IMU_init's members (IMU_Processing.cpp:73-86) --
+// b_first_frame_ kept, unless fresh (the handle's first immesh_imu_init_begin: a new ImuProcess, b_first_frame_ = true) -- the carry
+// discarded (its samples belong before the reset); the first-map flag, mean_acc_norm and the counters are kept
+IM_HDN inline void dimu_begin(DepthImu& D, int fresh, int max_ini) {
+    imu_init_reset(D.ini);
+    if (fresh) D.ini.first_frame = 1;
+    D.init_phase = 1;
+    D.max_ini = max_ini;
+    D.carry = 0;
+    D.cnt[5] = 0;
 }
 
 IM_HDN inline void imu_write_pose(double* pose, double t, const double* run) {

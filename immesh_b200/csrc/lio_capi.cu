@@ -659,9 +659,11 @@ __global__ void __launch_bounds__(FEED_THREADS) k_feed_head(ScanBuf sb_, const L
     __syncthreads();
     for (int i = threadIdx.x; i < IM_STATE_DOUBLES; i += blockDim.x) states[slot * IM_STATE_DOUBLES + i] = ctrl->state[i];
     if (threadIdx.x == 0) {
-        const int iters = d.lio ? ctrl->iters_run : 0;
+        const int branch = d.branch_dev ? *d.branch_dev : d.branch;
+        const bool lio = d.lio && (!d.branch_dev || branch == 3);
+        const int iters = lio ? ctrl->iters_run : 0;
         long long ne = 0, nr = 0;
-        if (d.lio) {
+        if (lio) {
             if (eff_total) ne = *eff_total;
             const int n = d.src == 2 ? feed_full_n(d) : d.src == 1 ? scan_load_dyn(sb_).n : 0;
             nr = n > 0 ? (n - 1) / skip + 1 : 0;
@@ -669,12 +671,12 @@ __global__ void __launch_bounds__(FEED_THREADS) k_feed_head(ScanBuf sb_, const L
         long long* h = hdr + slot * IMMESH_LIO_FEED_HDR;
         feed_append(*fd, ne, nr, max_rows, h);
         h[IMMESH_FEED_KIND] = d.kind;
-        h[IMMESH_FEED_BRANCH] = d.branch;
+        h[IMMESH_FEED_BRANCH] = branch;
         h[IMMESH_FEED_ITERS] = iters;
         h[IMMESH_FEED_MATCHES] = iters > 0 ? (long long)ctrl->stats[iters - 1].n_match : 0;
         h[IMMESH_FEED_CONVERGED] = iters > 0 ? (long long)ctrl->stats[iters - 1].converged : 0;
         h[IMMESH_FEED_ERR] = counters[IM_LC_ERR];
-        h[IMMESH_FEED_SOURCE] = d.src;
+        h[IMMESH_FEED_SOURCE] = lio ? d.src : 0;
         h[IMMESH_FEED_SCAN] = d.scan;
     }
     __syncthreads();
@@ -1000,6 +1002,7 @@ static int push_dyn(immesh_lio* h, int n, int slot, double dt, double cov_gyr, d
 }
 static int lio_flags_status(int err) {
     if (err & (IM_ERR_NODE_POOL | IM_ERR_CHUNK_POOL | IM_ERR_HASH_FULL | IM_ERR_SEG_POOL)) return im_fail(IMMESH_E_CAPACITY, "device pool overflow (raise the capacities in immesh_lio_config)");
+    if (err & IM_ERR_IMU_CARRY) return im_fail(IMMESH_E_CAPACITY, "immesh_lio_step_async_depth_imu: carried and new IMU samples exceeded max_imu (the frame's samples were dropped)");
     if (err & (IM_ERR_KEY_RANGE | IM_ERR_FX_RANGE)) return im_fail(IMMESH_E_RANGE, "coordinate / normal-equation term outside the representable range");
     if (err & IM_ERR_PEER_TIMEOUT) return im_fail(IMMESH_E_CUDA, "sharded mode: a peer rank did not publish its data in time (peer window epoch flag)");
     return IMMESH_OK;
@@ -1300,6 +1303,7 @@ static int feed_stage(immesh_lio* h, const immesh_lio::FeedNext& nx, int kind, i
     d.n = d.src == 2 ? nx.n : 0;
     d.n_dev = d.src == 2 ? nx.n_dev : nullptr;
     d.pad_ = 0;
+    d.branch_dev = nx.kind >= 0 ? nx.branch_dev : nullptr;
     IM_CUDA(cudaMemcpyAsync(&f.dev->dyn, &d, sizeof(FeedDyn), cudaMemcpyHostToDevice, h->stream));
     return IMMESH_OK;
 }
@@ -1558,12 +1562,15 @@ int immesh_lio_step_async_dev_n(immesh_lio_t* h, const float* d_body_xyz, int n_
     return lio_enqueue(h, d_body_xyz, n_max, 1, dt, cov_gyr, cov_acc, true, IMMESH_FEED_KIND_STEP_ASYNC_DEV_N);
 }
 // voxel_map_init queued like a pipelined step (internal: the first scan after the IMU initialisation, immesh_lio_step_async_imu): the
-// build kernels of immesh_voxelmap_build on a device-resident full scan, behind the staging-slot protocol, without a host wait
-int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, int n) {
+// build kernels of immesh_voxelmap_build on a device-resident full scan, behind the staging-slot protocol, without a host wait.
+// d_n != null: the count is read on the device (n its upper bound; *d_n == 0 builds nothing), and the scan feed records nothing -- the
+// depth IMU chain records its frame once, behind its step.
+static int build_async_dev(immesh_lio_t* h, const float* d_body_xyz, int n, const int* d_n) {
     if (!h || !d_body_xyz || n < 1) return im_fail(IMMESH_E_INVALID, "bad argument");
     const immesh_lio::FeedNext nx = h->feed_next;   // the IMU chain's branch 2 (recorded with its header and state)
     h->feed_next = immesh_lio::FeedNext();
     if (n > h->max_scan) return im_fail(IMMESH_E_CAPACITY, "scan larger than max_scan_points");
+    const bool record = h->feed.on && !d_n;
     int grc = lio_growth_check(h, n);
     if (grc == IMMESH_OK) grc = markers_fit(h);
     if (grc) return grc;
@@ -1576,18 +1583,22 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     }
     ++h->scan_counter;
     ++h->map_steps;
+    h->next_n_dev = d_n;
     int rc = upload_scan(h, d_body_xyz, n, 1, s);
+    // d_n: the depth IMU chain, whose step follows in the same call and takes this scan index again -- one pose-ring slot per call, so
+    // that a mesh frame still reading the pose of up to 7 calls ago keeps it
+    if (d_n) --h->scan_counter;
     if (rc) return rc;
     if (h->lm_on) launch_local_map(h);   // places the box at the building scan's pose
     launch_grow(h, 1);
     h->scan_rows = 0;   // the reference publishes no effect cloud after voxel_map_init
-    if (h->feed.on) {
+    if (record) {
         rc = feed_stage(h, nx, IMMESH_FEED_KIND_IMU, 2, false);
         if (rc) return rc;
         launch_feed(h, false, true);   // voxel_map_init is followed by pubPlaneMap (:1899-1900)
     }
     IM_CUDA(cudaGetLastError());
-    if (h->feed.on) {
+    if (record) {
         rc = feed_commit(h);
         if (rc) return rc;
     }
@@ -1596,8 +1607,13 @@ int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, in
     h->slot_busy[s] = 1;
     h->slot_step[s] = h->map_steps;
     h->timed_last = 0;
-    h->pose_pub_idx = h->scan_counter;
+    if (!d_n) h->pose_pub_idx = h->scan_counter;
     return IMMESH_OK;
+}
+int immesh_voxelmap_build_async_dev(immesh_lio_t* h, const float* d_body_xyz, int n) { return build_async_dev(h, d_body_xyz, n, nullptr); }
+int immesh_voxelmap_build_async_dev_n(immesh_lio_t* h, const float* d_body_xyz, int n_max, const int* d_n) {
+    if (!d_n) return im_fail(IMMESH_E_INVALID, "bad argument");
+    return build_async_dev(h, d_body_xyz, n_max, d_n);
 }
 int immesh_lio_wait(immesh_lio_t* h, double* state_out, int* iters_run) { return lio_wait_impl(h, state_out, iters_run, false); }
 // internal (immesh_lio_step_async_imu, branch 1): record the scan in the feed, header and state only, behind the work queued for it

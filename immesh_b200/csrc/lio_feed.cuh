@@ -28,6 +28,8 @@ struct FeedDyn {
     int src;               // registered source used: 0 none, 1 the down-sampled scan, 2 the full scan
     int lio;               // 1: the scan ran the IESKF (iterations, matches, rows); 0: an IMU branch 1 / 2 scan (header and state only)
     int pad_;
+    const int* branch_dev; // the branch decided on the device (immesh_lio_step_async_depth_imu), or null: then `branch` is the branch, and
+                           // a device branch other than 3 records the scan as lio = 0
 };
 // the points of the full scan (registered source 2)
 IM_HD int feed_full_n(const FeedDyn& d) { return d.n_dev ? *d.n_dev : d.n; }

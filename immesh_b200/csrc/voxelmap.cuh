@@ -115,6 +115,7 @@ enum : int {
     IM_ERR_FX_RANGE = 16,
     IM_ERR_SEG_POOL = 32,
     IM_ERR_PEER_TIMEOUT = 64,   // sharded mode: a peer rank's epoch flag did not arrive (peer_win.cuh)
+    IM_ERR_IMU_CARRY = 128,     // immesh_lio_step_async_depth_imu: carried + own IMU samples exceeded max_imu (the frame's samples dropped)
 };
 
 struct VoxelMapDev {

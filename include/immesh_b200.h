@@ -259,8 +259,9 @@ int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int st
  *   max_scans >= 1: header and state ring; max_rows: row ring (>= 1 when effect or registered is set); effect 0/1; registered 0 (none),
  *   1 (the down-sampled scan, dense_map_en 0) or 2 (the full scan, dense_map_en 1); point_skip >= 1 (publish/pub_point_skip).
  *   Other values, or a sharded handle: IMMESH_E_INVALID.  immesh_lio_shard refuses a handle with the feed on.
- * Every call of immesh_lio_step, _step_dev, _step_async, _step_async_dev_n, _step_async_raw, _raw_i, _imu, _imu_i and _depth records one scan
- * (the IMU chain's branches 1 and 2 too: a header and the state, no rows).  The staged calls record nothing.
+ * Every call of immesh_lio_step, _step_dev, _step_async, _step_async_dev_n, _step_async_raw, _raw_i, _imu, _imu_i, _depth and _depth_imu records
+ * one scan (the IMU chains' branches 1 and 2 too, and _depth_imu's dropped frames: a header and the state, no rows).  The staged calls record
+ * nothing.
  *   header (IMMESH_LIO_FEED_HDR int64): IMMESH_FEED_SCAN number; KIND (IMMESH_FEED_KIND_*); BRANCH (0 LiDAR-only, else the IMU
  *     chain's 1/2/3); ITERS run; MATCHES of the last IESKF iteration (m_effct_feat_num); CONVERGED flag of that iteration; ERR (the
  *     IM_LC_ERR flags); ROW_BEGIN, ROW_EFFECT_END, ROW_END: the scan's effect rows [BEGIN, EFFECT_END) and registered rows
@@ -268,7 +269,7 @@ int immesh_lio_registered_cloud(immesh_lio_t* h, const float* pts, int n, int st
  *   state: the 348 doubles the scan ended with, bit-identical to immesh_lio_wait right after it (branches 1 and 2: the state as the
  *     branch left it).
  *   rows: effect = 1: immesh_lio_effect_cloud right after the scan (row_index = its scan_index).  registered = 1:
- *     immesh_lio_registered_cloud(h, NULL, ..., point_skip); registered = 2: on _raw, _imu and _depth, immesh_lio_registered_cloud of
+ *     immesh_lio_registered_cloud(h, NULL, ..., point_skip); registered = 2: on _raw, _imu, _depth and _depth_imu, immesh_lio_registered_cloud of
  *     immesh_voxelgrid_input_points (stride 3, intensity column -1; _depth: its device count), on _raw_i and _imu_i immesh_lio_frontend_cloud(h, vg, 1,
  *     point_skip), elsewhere (no full scan) source 1.  row_index of a registered row: -1.
  *   A scan whose rows exceed max_rows keeps its header and state and sets ROWS_LOST.  A loss never fails a step or changes the state,
@@ -310,6 +311,9 @@ typedef struct {
 #define IMMESH_FEED_KIND_IMU 6
 #define IMMESH_FEED_KIND_IMU_I 7
 #define IMMESH_FEED_KIND_DEPTH 8   /* immesh_lio_step_async_depth */
+#define IMMESH_FEED_KIND_DEPTH_IMU 9   /* immesh_lio_step_async_depth_imu */
+/* IMMESH_FEED_BRANCH of an immesh_lio_step_async_depth_imu frame that sync_packages dropped (a cloud of <= 1 point, or a carry overflow) */
+#define IMMESH_FEED_BRANCH_DROPPED 4
 int immesh_lio_feed_enable(immesh_lio_t* h, const immesh_lio_feed_config* cfg /* NULL: off */);
 int immesh_lio_feed(immesh_lio_t* h, int64_t since_scan, int wait, int64_t* scans /*[cap_scans][12]*/, double* states /*[cap_scans][348] or NULL*/,
                     int cap_scans, float* rows /*[cap_rows][4] or NULL*/, int32_t* row_index /*[cap_rows] or NULL*/, int64_t cap_rows,
@@ -1060,6 +1064,51 @@ int immesh_lio_step_async_imu(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_vox
 int immesh_lio_step_async_imu_i(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_voxelgrid_t* vg, const double* imu /*[n_imu][7]*/, int n_imu,
                                 const float* pts, int n, int stride, int time_col, int intensity_col, int on_device,
                                 double lidar_beg_time, int calib_laser, float leaf, int* branch_out /*or NULL*/);
+
+/* ---- the IMU-enabled loop on depth frames (L515, D435i, Azure Kinect with imu_en: true): immesh_lio_step_async_imu fed the depth
+ * frame's cloud of immesh_lio_step_async_depth, one queued call per frame, with every decision the reference makes from the cloud made on
+ * the device.  Nothing is read back: the cloud's count exists only on the device, so the host queues the same launches for every frame
+ * and each kernel returns early unless its branch is the one the device took.
+ *   Cloud: that of immesh_frontend_prepare_depth (f, depth, on_device, point_filter_num, blind), as x y z t records with t = 0
+ *     (Preprocess::l515_handler sets curvature = 0, src/preprocess.cpp:270).  lidar_beg_time = frame_time, so pcl_end_time = frame_time.
+ *     The stable time sort of all-equal stamps is the identity.  The KITTI calibration does not apply to depth frames (calib_laser = 0).
+ *   Drop (sync_packages, src/voxel_mapping_common.cpp:393-400): a cloud of <= 1 point is dropped -- no state, last_update_time or
+ *     initialisation change -- and the frame's IMU samples are carried on the device: the next frame's meas.imu is the carried samples,
+ *     then its own, in order.  Carried + own samples beyond max_imu: the frame is dropped and its own samples discarded; the scan feed's
+ *     ERR holds the flag from that frame on, and immesh_lio_wait (and every blocking localization call) returns IMMESH_E_CAPACITY from
+ *     then on: the flag joins the handle's never-reset error word, like a pool overflow.  An overflow does not heal itself: the carry is
+ *     only consumed by a kept frame, and while carry + a frame's samples exceed max_imu every frame is dropped -- size max_imu for the
+ *     longest run of dropped frames, or restart with immesh_imu_init_begin (which discards the carry).
+ *   Otherwise the branch of immesh_lio_step_async_imu, from the device's phase (Process2, src/IMU_Processing.cpp:960-1006;
+ *     src/voxel_mapping.cpp:1820-1905):
+ *     1 initialising: IMU_init (:188-232) on the device, the same code as the host chain's (running means in sample order, no FMA),
+ *       the init-end test init_iter_num > max_ini_count and |mean_acc| on the device; last_update_time = frame_time.
+ *     2 the first frame after it: UndistortPcl, then voxel_map_init from the whole undistorted cloud.
+ *     3 every later frame: UndistortPcl, VoxelGrid(leaf), IESKF on the propagated state and the map update.
+ *   Scan feed: one record per call, KIND = IMMESH_FEED_KIND_DEPTH_IMU, BRANCH = 1, 2, 3 or IMMESH_FEED_BRANCH_DROPPED (header and state
+ *     only unless 3).  Branch 3's full scan (registered = 2) is the undistorted cloud.
+ *   Mesh hand-off, after every call: immesh_mesh_push_frame_from_lio_async_dev_n(mesh, lio, immesh_voxelgrid_input_points(vg), sampled
+ *     pixels, immesh_voxelgrid_input_count(vg)).  The count is the undistorted cloud's in branch 3 and 0 otherwise.  The reference hands
+ *     off nothing for the other frames; here they are mesh frames that add nothing, and the mesh frame feed shows them with N_POINTS = 0.
+ * The call waits for the device only on a busy staging slot (immesh_host_wait_ms counts it: the IMU batch's and the localization's
+ *   slots -- two per call, the build's and the step's -- and, for a host image, the VoxelGrid's image staging) and, with pool growth on,
+ *   where immesh_lio_config's growth needs a drain as on every chain.  Its step replays the captured launch sequence of
+ *   immesh_lio_step_async_dev_n; the direct launches (profiling on) give the same results.
+ * Input and pose rings: one slot of each per call, as on the other chains -- the cloud is unprojected into an input-ring slot and the
+ *   undistorted cloud written back into it, and the build shares the step's scan index.
+ * Handle rules: once this entry point has run on an IMU handle, the handle's phase, first-map flag and carry live on the device;
+ *   immesh_lio_step_async_imu[_i] on it then returns IMMESH_E_INVALID, as this one does on a handle they have run on.
+ *   immesh_imu_init_begin restarts the phase as documented there (the carried samples are discarded: they belong before the reset).
+ * Errors, returned before anything is queued: those of immesh_lio_step_async_depth, IMMESH_E_CAPACITY for n_imu > max_imu, or sampled
+ *   pixels beyond the IMU handle's max_points or the localization handle's max_scan_points; IMMESH_E_INVALID for a sharded handle.
+ *   Exception: a pool growth the localization's build or step then needs can still fail (IMMESH_E_CAPACITY / IMMESH_E_CUDA) after the
+ *   frame's decision is queued: the device phase and carry have then taken the frame without its step.
+ * immesh_imu_depth_chain_state (blocking): out = [calls, dropped, branch-1, branch-2, branch-3 frames, carried samples now, carry
+ *   overflows, initialisation finished (0/1)]. */
+int immesh_lio_step_async_depth_imu(immesh_lio_t* lio, immesh_imu_t* imu_h, immesh_voxelgrid_t* vg, const double* imu /*[n_imu][7]*/, int n_imu,
+                                    const immesh_depth_frame* f, const void* depth, int on_device, int point_filter_num, double blind,
+                                    double frame_time, float leaf);
+int immesh_imu_depth_chain_state(immesh_imu_t* h, int64_t out[8]);
 
 /* optional per-kernel CUDA-event profiler (off by default) and launch accounting, process-wide */
 int immesh_profile_enable(int on);   /* 0 off, 1 per-kernel totals, 2 totals + timeline */
