@@ -43,6 +43,30 @@ EVAL_COUNT_KEYS = ("live_triangles", "degenerate", "samples", "gt_points", "samp
 EVAL_METRIC_KEYS = ("maxmin_deg", "c2se", "accuracy", "completeness", "precision", "recall", "fscore")
 
 
+class _TexCamera(C.Structure):
+    _fields_ = [("width", C.c_int), ("height", C.c_int), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double),
+                ("cam_R", C.c_double * 9), ("cam_t", C.c_double * 3)]
+
+
+class _TexCfg(C.Structure):
+    _fields_ = [("z_near", C.c_double), ("z_far", C.c_double), ("min_cos", C.c_double), ("min_visible_permille", C.c_int), ("two_sided", C.c_int),
+                ("positions", C.c_int), ("pad", C.c_int)]
+
+
+TEXTURE_COUNT_KEYS = ("textured", "untextured", "cameras_used", "pixels")
+
+
+def texture_cameras(cameras):
+    """ctypes array of immesh_texture_camera from (width, height, (fx, fy, cx, cy), cam_R [3, 3], cam_t [3]) tuples: OpenCV axes
+    (x right, y down, z forward), camera to world"""
+    cameras = list(cameras)
+    arr = (_TexCamera * max(len(cameras), 1))()
+    for i, (w, h, K, R, t) in enumerate(cameras):
+        fx, fy, cx, cy = (float(k) for k in K)
+        arr[i] = _TexCamera(int(w), int(h), fx, fy, cx, cy, (C.c_double * 9)(*np.asarray(R, np.float64).reshape(9)), (C.c_double * 3)(*np.asarray(t, np.float64).reshape(3)))
+    return arr, len(cameras)
+
+
 class _ViewStyle(C.Structure):
     _fields_ = [("positions", C.c_int), ("color_by_height", C.c_int), ("z_range", C.c_double * 2)]
 
@@ -266,6 +290,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_evaluate", [vp, vp, C.c_int64, C.c_int, C.POINTER(_EvalCfg), C.POINTER(C.c_int64), dp, C.POINTER(C.c_int32), C.c_int64,
                                   C.POINTER(C.c_int64)]),
         ("immesh_mesh_evaluate_stats", [C.POINTER(C.c_int64)]),
+        ("immesh_mesh_texture_select", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexCfg), C.POINTER(C.c_int32), fp, C.POINTER(C.c_int32), fp, C.c_int64,
+                                        C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+        ("immesh_write_obj_textured", [C.c_char_p, C.c_char_p, fp, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), fp, C.c_int,
+                                       C.POINTER(C.c_int32), C.POINTER(C.c_char_p), C.c_int]),
         ("immesh_mesh_region_stream", [vp, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32), ip]),
         ("immesh_mesh_region_buffers", [vp, C.c_double, C.POINTER(C.c_int32), C.c_int, C.c_double, C.c_int, fp, C.POINTER(C.c_int32), C.c_int,
                                         C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, fp, ip, ip, ip]),
@@ -1141,6 +1169,34 @@ class Mesh:
         out["stats"] = dict(zip(("tiles", "plan_boxes", "scratch_bytes", "table_bytes"), (int(v) for v in st)))
         return out
 
+    def texture_select(self, cameras, *, z_near=0.1, z_far=1000.0, min_cos=0.0, min_visible_permille=0, two_sided=False, positions=0, vertices=True):
+        """The paper's textured mesh (Application-2): per live triangle, in snapshot order, the nearest camera that sees it and its
+        corners' pixel coordinates there.  cameras: (width, height, (fx, fy, cx, cy), cam_R, cam_t) tuples, OpenCV axes, camera to world.
+        positions 1: the smoothed positions where the vertex is smoothed (smooth_all first to match the smoothed PLY).  Returns
+        dict(cam int32[nt] (-1: none), uv float32[nt,6] (u0 v0 u1 v1 u2 v2 of the corners in face order; NaN where cam = -1),
+        px int32[nt,2] (won, covered pixels in the chosen camera), vertices float32[nv,3] (the positions used; with vertices, which
+        first waits for the queued frames so that nv is known; else None), counts {TEXTURE_COUNT_KEYS: int})."""
+        arr, n_cams = texture_cameras(cameras)
+        cfg = _TexCfg(float(z_near), float(z_far), float(min_cos), int(min_visible_permille), 1 if two_sided else 0, int(positions), 0)
+        i32, i64 = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+        nf = C.c_int64(0)
+        counts = np.zeros(4, dtype=np.int64)
+        rc = self.lib.immesh_mesh_texture_select(self._h, arr, n_cams, C.byref(cfg), None, None, None, None, 0, C.byref(nf), None)   # a count query
+        if rc not in (0, -3):
+            _check(self.lib, rc, "mesh_texture_select")
+        if vertices:
+            self.wait()
+        n, nv = nf.value, self.counts()["n_vertices"] if vertices else 0
+        cam = np.zeros(max(n, 1), dtype=np.int32)
+        uv = np.full((max(n, 1), 6), np.nan, dtype=np.float32)
+        px = np.zeros((max(n, 1), 2), dtype=np.int32)
+        verts = np.zeros((max(nv, 1), 3), dtype=np.float32)
+        _check(self.lib, self.lib.immesh_mesh_texture_select(self._h, arr, n_cams, C.byref(cfg), cam.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)),
+                                                             px.ctypes.data_as(i32), verts.ctypes.data_as(C.POINTER(C.c_float)) if vertices else None, n, C.byref(nf),
+                                                             counts.ctypes.data_as(i64)), "mesh_texture_select")
+        return dict(cam=cam[:n].copy(), uv=uv[:n].copy(), px=px[:n].copy(), vertices=verts[:nv].copy() if vertices else None,
+                    counts=dict(zip(TEXTURE_COUNT_KEYS, (int(v) for v in counts))))
+
     def region_stream(self, region_size=10.0, cap=1 << 16):
         """(region_keys int32[nr,3], region_offsets int32[nr+1], triangles int32[nt,3]) -- the viewer's region-bucketed triangle sets."""
         nt = self.counts()["n_triangles"]
@@ -1435,6 +1491,24 @@ def write_ply(path: str, vertices, triangles, flips=None, lib: Optional[C.CDLL] 
     fl = None if flips is None else np.ascontiguousarray(flips, dtype=np.int32)
     _check(lib, lib.immesh_write_ply(path.encode(), v.ctypes.data_as(C.POINTER(C.c_float)), v.shape[0], t.ctypes.data_as(C.POINTER(C.c_int32)),
                                      None if fl is None else fl.ctypes.data_as(C.POINTER(C.c_int32)), t.shape[0]), "write_ply")
+
+
+def write_obj_textured(obj_path: str, mtl_path: str, vertices, triangles, flips, facet_cam, facet_uv, cam_wh, image_files, lib: Optional[C.CDLL] = None):
+    """Wavefront OBJ + MTL of a texture selection: vertices float32[nv,3], triangles int32[nt,3] and flips int32[nt] (a snapshot),
+    facet_cam / facet_uv (Mesh.texture_select's cam / uv), cam_wh int32[n_cams,2] the cameras' image sizes, image_files their paths
+    as the MTL names them (map_Kd).  Texture coordinates are normalised: the images may be larger than the ones selected at."""
+    lib = lib or load_library()
+    v = np.ascontiguousarray(vertices, dtype=np.float32).reshape(-1, 3)
+    t = np.ascontiguousarray(triangles, dtype=np.int32).reshape(-1, 3)
+    fl = None if flips is None else np.ascontiguousarray(flips, dtype=np.int32).reshape(-1)
+    fc = np.ascontiguousarray(facet_cam, dtype=np.int32).reshape(-1)
+    uv = np.ascontiguousarray(facet_uv, dtype=np.float32).reshape(-1, 6)
+    wh = np.ascontiguousarray(cam_wh, dtype=np.int32).reshape(-1, 2)
+    files = (C.c_char_p * max(len(image_files), 1))(*[str(f).encode() for f in image_files])
+    i32 = C.POINTER(C.c_int32)
+    _check(lib, lib.immesh_write_obj_textured(obj_path.encode(), mtl_path.encode(), v.ctypes.data_as(C.POINTER(C.c_float)), v.shape[0], t.ctypes.data_as(i32),
+                                              None if fl is None else fl.ctypes.data_as(i32), fc.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)),
+                                              t.shape[0], wh.ctypes.data_as(i32), files, len(image_files)), "write_obj_textured")
 
 
 def write_pcd(path: str, vertices, lib: Optional[C.CDLL] = None):

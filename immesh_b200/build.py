@@ -172,6 +172,20 @@ def build_view(force=False):
     return _emu_ext(os.path.join(_ROOT, "tests", "view", "emu_view.cpp"), EMU_VIEW, force)
 
 
+EMU_TEXTURE = os.path.join(_ROOT, "tests", "texture", "libimmesh_emu_texture.so")
+
+
+def build_texture(force=False):
+    """tests/texture: the texture selection's bodies (immesh_b200/csrc/texture_core.cuh, with the rasteriser's of reinforce.cuh) in the
+    device chain's orchestration -- binning, tiles, the per-facet test and the rows -- built for the host"""
+    src = os.path.join(_ROOT, "tests", "texture", "emu_texture.cpp")
+    deps = [src] + _sources(CSRC, (".cuh",)) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_TEXTURE, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_TEXTURE, src])
+    return EMU_TEXTURE
+
+
 EMU_VIEW_OVERLAY = os.path.join(_ROOT, "tests", "view_overlay", "libimmesh_emu_view_overlay.so")
 
 
@@ -315,6 +329,7 @@ def build_all(force=False):
     build_reinforce(force)
     build_view(force)
     build_view_overlay(force)
+    build_texture(force)
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)

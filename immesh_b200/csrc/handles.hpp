@@ -355,6 +355,7 @@ int queued_cam_stage(immesh_mesh* h, immesh_mesh::QueuedCam& c, int s);
 void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st);
 void mesh_view_launch(immesh_mesh* h, cudaStream_t st);
 void rf_scan_launch(cudaStream_t st, const int* cnt, int n, int* off);
+void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st, int wire = 0);
 void mesh_changes_launch(immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool batched);
 void mesh_feed_begin_launch(immesh_mesh* h, cudaStream_t st);
 int mesh_feed_stage(immesh_mesh* h, int s, long long frame, long long n, int step, int kind, const double* pose_t, bool rf, bool img);

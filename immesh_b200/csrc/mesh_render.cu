@@ -375,7 +375,7 @@ static cudaError_t rf_image_alloc(immesh::MemSet& dev, int w, int h, int nout, R
     return e;
 }
 // the binning passes of an image: the triangles at positions pos_mode (view_vertex) into the tiles' bins
-static void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st, int wire = 0) {
+void rf_bin_launch(const immesh_mesh* h, const RfImage& im, int pos_mode, cudaStream_t st, int wire) {
     const int g = h->n_sm * 8;
     IM_LAUNCH(k_rf_count, g, 128, 0, st, h->M, pos_mode, wire, (const DepthCam*)im.cam, im.tile_cnt);
     IM_LAUNCH(k_rf_scan, 1, 1024, 0, st, (const int*)im.tile_cnt, im.ntiles, im.tile_off, im.tile_cnt, im.bin_cap, im.misc);

@@ -877,6 +877,73 @@ int immesh_mesh_evaluate(immesh_mesh_t* h, const float* gt_xyz /*[n_gt][3]*/, in
                          int64_t* counts /*[12]*/, double* metrics /*[8]*/, int32_t* facet_rows /*[cap_rows][5] or NULL*/, int64_t cap_rows,
                          int64_t* n_rows /*or NULL*/);
 int immesh_mesh_evaluate_stats(int64_t* out /*[4]*/);
+/* The textured mesh of the paper (ImMesh, Fig. 1(b, c), Fig. 11, Application-2 in section VIII-E: "each facet of the reconstructed mesh
+ * textured by the RGB image captured by the nearest camera frame with the estimated camera pose"): for every live triangle, the
+ * camera that textures it and the pixel coordinates of its corners in that camera's image.  No pixel is resampled: the export
+ * (immesh_write_obj_textured) points at the caller's image files.
+ *   immesh_mesh_texture_select: blocking, on the mesh stream behind the frames already queued (those of
+ *     immesh_mesh_push_frame_from_lio_async included).  It reads the mesh and writes nothing on the handle (no smoothed position,
+ *     m_smoothed flag, counter or change-feed row), as immesh_mesh_render_view.
+ *   Rows: one per live triangle in immesh_mesh_snapshot's order (row i is snapshot triangle i), as immesh_mesh_evaluate's facet rows.
+ *     facet_cam [cap]: the chosen camera, -1 for none; facet_uv [cap][6]: u0 v0 u1 v1 u2 v2 of the corners q0 q1 q2 (below) in the
+ *     chosen camera's pixels, left unwritten where facet_cam = -1; facet_px [cap][2]: won and covered (below) of the chosen camera,
+ *     0 0 where facet_cam = -1; vertices [n_vertices][3]: the positions the rule used (cfg.positions), n_vertices as immesh_mesh_counts
+ *     reports it after immesh_mesh_wait (the call includes the queued frames' vertices).  Each may be NULL.
+ *     *n_facets = the live triangle count; above cap: IMMESH_E_CAPACITY and nothing written (cap = 0: a count query).
+ *     counts [4] (or NULL): facets textured, facets untextured, cameras that texture at least one facet, pixels rasterised (the sum
+ *     of width * height over the cameras).
+ *   Selection rule (defined here), float64 in the order written, without fused multiply-adds.  A facet's corners q0 q1 q2 are its
+ *     stored triple's positions p0 p1 p2 at cfg.positions (immesh_view_style.positions: 0 raw, 1 the smoothed position as float where
+ *     m_smoothed is set) in immesh_write_ply's face order: m_index_flip != 0 p0 p1 p2, else p0 p2 p1.
+ *     1. Camera: the OpenCV camera (x right, y down, z forward; world = cam_R p + cam_t) is the rasteriser's camera of
+ *        immesh_mesh_render_depth with columns 1 and 2 of cam_R negated, an exact conversion.
+ *     2. Visible pixels: immesh_mesh_render_view's visibility rule unchanged at that camera and positions, with cfg's z range: samples
+ *        at integer pixels, the edge-function cover (zero included), 1/z affine, a triangle with a corner outside (z_near, z_far)
+ *        skipped; at each pixel the smaller depth bits win, then the lower (a, b, c) triple.  covered_k(f): the pixels where f has a
+ *        sample; won_k(f): the pixels f wins.
+ *     3. Seen by camera k: every corner projects into [0, w - 1] x [0, h - 1]; won >= 1; 1000 won >= min_visible_permille covered;
+ *        and with g = ((q0 + q1) + q2) / 3, e = cam_t - g, n = (q1 - q0) x (q2 - q0), s = (n0 e0 + n1 e1) + n2 e2: s > 0 (the camera on
+ *        the oriented front side; two_sided: s != 0), and s s >= (min_cos min_cos) (|n|^2 |e|^2), squared norms summed (x^2 + y^2) + z^2.
+ *     4. Nearest: of the cameras that see f, the smallest |e|^2; on a tie the lower camera index.  None: facet_cam = -1.
+ *     5. UVs: the chosen camera's pixel coordinates (u, v) of q0, q1, q2, as (float) of the float64 projection.
+ *     The cameras run one after another in index order and each facet is updated by one thread with a strict <, so the result does
+ *     not depend on atomics or scheduling.
+ *   IMMESH_E_INVALID: NULL h, cams, cfg or n_facets; n_cams < 1; a camera with a size outside [1, 2^26] pixels, non-finite
+ *     intrinsics or pose, or fx or fy = 0; not 0 < z_near < z_far < inf; min_cos outside [0, 1]; min_visible_permille outside
+ *     [0, 1000]; two_sided or positions not 0 / 1; cap < 0; a sharded handle.
+ *   Lens distortion is not modelled: pass rectified images.  Intrinsics scaled to a smaller image select at that resolution; the
+ *   export's normalised coordinates then texture with the full-size images.
+ * immesh_write_obj_textured: host-side only, a Wavefront OBJ + MTL pair of the rows above (vertices, triangles and flips as
+ *   immesh_mesh_snapshot returns them, or the vertices texture_select wrote).  The OBJ: "mtllib <mtl_path's file name>", one "v x y z"
+ *   per vertex (%.9g), three "vt s t" per textured facet with s = (u + 0.5) / W, t = 1 - (v + 0.5) / H of its camera's size (pixel
+ *   centres at integers, so the coordinates do not depend on the resolution selected at), then the faces grouped by "usemtl tex_<k>"
+ *   in ascending k with the rows in order inside a group, each "f a/ta b/tb c/tc" (1-based) with the corners in the face order q0 q1
+ *   q2; the untextured facets last under "usemtl untextured", as "f a b c".  The MTL: "newmtl tex_<k>" with "map_Kd <image_files[k]>"
+ *   for every camera that textures a facet, and "newmtl untextured".  A triangle index outside [0, nv): IMMESH_E_RANGE; facet_cam
+ *   outside [-1, n_cams), a camera size below 1, a NULL image file of a used camera, or a file that cannot be written:
+ *   IMMESH_E_INVALID. */
+typedef struct {
+    int width, height;            /* image size in pixels, [1, 2^26] pixels */
+    double fx, fy, cx, cy;        /* pinhole intrinsics, finite, fx and fy != 0 */
+    double cam_R[9], cam_t[3];    /* camera to world, row-major, OpenCV axes (x right, y down, z forward), as immesh_depth_frame */
+} immesh_texture_camera;
+typedef struct {
+    double z_near, z_far;         /* 0 < z_near < z_far < inf */
+    double min_cos;               /* [0, 1]: the least |cos| between the facet normal and the view ray */
+    int min_visible_permille;     /* [0, 1000]: the least share of the facet's covered pixels it must win */
+    int two_sided;                /* 0: only cameras on the oriented front side; 1: either side */
+    int positions;                /* as immesh_view_style.positions: 0 raw, 1 smoothed where m_smoothed is set */
+    int pad;
+} immesh_texture_config;
+int immesh_mesh_texture_select(immesh_mesh_t* h, const immesh_texture_camera* cams, int n_cams, const immesh_texture_config* cfg,
+                               int32_t* facet_cam /*[cap] or NULL*/, float* facet_uv /*[cap][6] or NULL*/,
+                               int32_t* facet_px /*[cap][2] or NULL: won, covered in the chosen camera*/,
+                               float* vertices /*[n_vertices][3] or NULL: the positions used*/,
+                               int64_t cap, int64_t* n_facets, int64_t* counts /*[4] or NULL: textured, untextured, cameras used, pixels rasterised*/);
+int immesh_write_obj_textured(const char* obj_path, const char* mtl_path, const float* vertices /*[nv][3]*/, int nv,
+                              const int32_t* triangles /*[nt][3]*/, const int32_t* flips /*[nt] or NULL*/, const int32_t* facet_cam /*[nt]*/,
+                              const float* facet_uv /*[nt][6]*/, int nt, const int32_t* cam_wh /*[n_cams][2]*/, const char* const* image_files /*[n_cams]*/,
+                              int n_cams);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
