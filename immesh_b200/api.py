@@ -56,6 +56,46 @@ class _TexCfg(C.Structure):
 TEXTURE_COUNT_KEYS = ("textured", "untextured", "cameras_used", "pixels")
 
 
+class _TexImage(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("width", C.c_int), ("height", C.c_int), ("pitch", C.c_int64)]
+
+
+class _AtlasCfg(C.Structure):
+    _fields_ = [("page_size", C.c_int), ("max_cell", C.c_int), ("max_image_bytes", C.c_int64)]
+
+
+BAKE_COUNT_KEYS = ("textured", "untextured", "cells", "texels")
+
+
+def texture_images(images):
+    """(ctypes array of immesh_texture_image, on_device, keep-alive list) from HxWx3 uint8 numpy arrays or CUDA torch tensors (all one
+    kind; None for a camera no facet uses).  Rows may be padded; pixels must be 3 contiguous bytes."""
+    images = list(images)
+    arr = (_TexImage * max(len(images), 1))()
+    kinds = {type(im).__module__.split(".")[0] for im in images if im is not None}
+    if len(kinds) > 1:
+        raise ValueError("texture images: all numpy arrays or all CUDA torch tensors")
+    on_device = kinds == {"torch"}
+    keep = []
+    for i, im in enumerate(images):
+        if im is None:
+            continue
+        if on_device:
+            if not im.is_cuda or im.dtype.itemsize != 1 or im.dim() != 3 or im.shape[2] != 3 or im.stride(2) != 1 or im.stride(1) != 3:
+                raise ValueError(f"texture image {i}: a CUDA uint8 tensor [H, W, 3] with contiguous pixels")
+            arr[i] = _TexImage(im.data_ptr(), int(im.shape[1]), int(im.shape[0]), int(im.stride(0)))
+        else:
+            a = np.asarray(im)
+            if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.strides[2] != 1 or a.strides[1] != 3:
+                a = np.ascontiguousarray(a, dtype=np.uint8)
+                if a.ndim != 3 or a.shape[2] != 3:
+                    raise ValueError(f"texture image {i}: uint8 [H, W, 3]")
+            keep.append(a)
+            arr[i] = _TexImage(a.ctypes.data, int(a.shape[1]), int(a.shape[0]), int(a.strides[0]))
+        keep.append(im)
+    return arr, int(on_device), keep
+
+
 def texture_cameras(cameras):
     """ctypes array of immesh_texture_camera from (width, height, (fx, fy, cx, cy), cam_R [3, 3], cam_t [3]) tuples: OpenCV axes
     (x right, y down, z forward), camera to world"""
@@ -292,6 +332,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_evaluate_stats", [C.POINTER(C.c_int64)]),
         ("immesh_mesh_texture_select", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexCfg), C.POINTER(C.c_int32), fp, C.POINTER(C.c_int32), fp, C.c_int64,
                                         C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+        ("immesh_mesh_texture_bake", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int, C.POINTER(C.c_int32), fp, C.c_int64,
+                                      C.POINTER(_AtlasCfg), vp, C.c_int, C.POINTER(C.c_int32), fp, ip, C.POINTER(C.c_int64)]),
+        ("immesh_write_png", [C.c_char_p, vp, C.c_int, C.c_int]),
         ("immesh_write_obj_textured", [C.c_char_p, C.c_char_p, fp, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), fp, C.c_int,
                                        C.POINTER(C.c_int32), C.POINTER(C.c_char_p), C.c_int]),
         ("immesh_mesh_region_stream", [vp, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.POINTER(C.c_int32), ip]),
@@ -1197,6 +1240,36 @@ class Mesh:
         return dict(cam=cam[:n].copy(), uv=uv[:n].copy(), px=px[:n].copy(), vertices=verts[:nv].copy() if vertices else None,
                     counts=dict(zip(TEXTURE_COUNT_KEYS, (int(v) for v in counts))))
 
+    def texture_bake(self, sel, cameras, images, *, page_size=4096, max_cell=64, max_image_bytes=0):
+        """The texture atlas of a selection: every textured facet's pixels resampled out of its chosen image into square pages.
+        sel: texture_select's result (cam, uv); cameras: the selection's camera tuples (their width and height rescale uv to each
+        image); images: per camera an HxWx3 uint8 numpy array or CUDA torch tensor (all one kind), None for a camera no facet uses.
+        Blocking, ordered behind the queued frames; writes nothing on the handle.  Returns dict(pages uint8[n_pages, P, P, 3],
+        page int32[nt] (-1: untextured), uv float32[nt,6] (the corners in page texels; NaN where page = -1),
+        counts {BAKE_COUNT_KEYS: int}).  Export: write_obj_textured(..., page, uv, [(P, P)] * n_pages, png_files) after write_png."""
+        arr, n_cams = texture_cameras(cameras)
+        imgs, on_device, keep = texture_images(images)
+        cam = np.ascontiguousarray(sel["cam"], dtype=np.int32).reshape(-1)
+        uv = np.ascontiguousarray(sel["uv"], dtype=np.float32).reshape(-1, 6)
+        n = len(cam)
+        cfg = _AtlasCfg(int(page_size), int(max_cell), int(max_image_bytes))
+        i32 = C.POINTER(C.c_int32)
+        np_ = C.c_int(0)
+        page = np.full(max(n, 1), -1, np.int32)
+        auv = np.full((max(n, 1), 6), np.nan, np.float32)
+        counts = np.zeros(4, np.int64)
+        rc = self.lib.immesh_mesh_texture_bake(self._h, arr, n_cams, imgs, on_device, cam.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)), n,
+                                               C.byref(cfg), None, 0, None, None, C.byref(np_), None)   # a count query
+        _check(self.lib, rc, "mesh_texture_bake")
+        P = int(page_size)
+        pages = np.zeros((np_.value, P, P, 3), np.uint8)
+        _check(self.lib, self.lib.immesh_mesh_texture_bake(self._h, arr, n_cams, imgs, on_device, cam.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)), n,
+                                                           C.byref(cfg), pages.ctypes.data_as(C.c_void_p), pages.shape[0], page.ctypes.data_as(i32),
+                                                           auv.ctypes.data_as(C.POINTER(C.c_float)), C.byref(np_), counts.ctypes.data_as(C.POINTER(C.c_int64))),
+               "mesh_texture_bake")
+        del keep
+        return dict(pages=pages, page=page[:n].copy(), uv=auv[:n].copy(), counts=dict(zip(BAKE_COUNT_KEYS, (int(v) for v in counts))))
+
     def region_stream(self, region_size=10.0, cap=1 << 16):
         """(region_keys int32[nr,3], region_offsets int32[nr+1], triangles int32[nt,3]) -- the viewer's region-bucketed triangle sets."""
         nt = self.counts()["n_triangles"]
@@ -1509,6 +1582,15 @@ def write_obj_textured(obj_path: str, mtl_path: str, vertices, triangles, flips,
     _check(lib, lib.immesh_write_obj_textured(obj_path.encode(), mtl_path.encode(), v.ctypes.data_as(C.POINTER(C.c_float)), v.shape[0], t.ctypes.data_as(i32),
                                               None if fl is None else fl.ctypes.data_as(i32), fc.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)),
                                               t.shape[0], wh.ctypes.data_as(i32), files, len(image_files)), "write_obj_textured")
+
+
+def write_png(path: str, rgb, lib: Optional[C.CDLL] = None):
+    """an uncompressed 8-bit RGB PNG of rgb uint8[H, W, 3] (rows top to bottom), e.g. a page of Mesh.texture_bake"""
+    lib = lib or load_library()
+    a = np.ascontiguousarray(rgb, dtype=np.uint8)
+    if a.ndim != 3 or a.shape[2] != 3:
+        raise ValueError("write_png: rgb must be uint8 [H, W, 3]")
+    _check(lib, lib.immesh_write_png(str(path).encode(), a.ctypes.data_as(C.c_void_p), a.shape[1], a.shape[0]), "write_png")
 
 
 def write_pcd(path: str, vertices, lib: Optional[C.CDLL] = None):

@@ -186,6 +186,20 @@ def build_texture(force=False):
     return EMU_TEXTURE
 
 
+EMU_TEXTURE_BAKE = os.path.join(_ROOT, "tests", "texture_bake", "libimmesh_emu_texture_bake.so")
+
+
+def build_texture_bake(force=False):
+    """tests/texture_bake: the texture atlas's bodies and argument check (immesh_b200/csrc/texture_bake_core.cuh) in the device call's
+    orchestration -- class and key, the stable sort, the class table, placement and the texels of every slot -- built for the host"""
+    src = os.path.join(_ROOT, "tests", "texture_bake", "emu_texture_bake.cpp")
+    deps = [src] + _sources(CSRC, (".cuh",)) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_TEXTURE_BAKE, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-shared",
+                               "-o", EMU_TEXTURE_BAKE, src])
+    return EMU_TEXTURE_BAKE
+
+
 EMU_VIEW_OVERLAY = os.path.join(_ROOT, "tests", "view_overlay", "libimmesh_emu_view_overlay.so")
 
 
@@ -330,6 +344,7 @@ def build_all(force=False):
     build_view(force)
     build_view_overlay(force)
     build_texture(force)
+    build_texture_bake(force)
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)

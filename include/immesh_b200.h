@@ -944,6 +944,66 @@ int immesh_write_obj_textured(const char* obj_path, const char* mtl_path, const 
                               const int32_t* triangles /*[nt][3]*/, const int32_t* flips /*[nt] or NULL*/, const int32_t* facet_cam /*[nt]*/,
                               const float* facet_uv /*[nt][6]*/, int nt, const int32_t* cam_wh /*[n_cams][2]*/, const char* const* image_files /*[n_cams]*/,
                               int n_cams);
+/* The texture atlas of a selection: every textured facet's pixels resampled out of its chosen image into a few square pages, so the
+ * textured mesh ships as one OBJ, one MTL and n_pages images instead of pointing at every source image.
+ *   immesh_mesh_texture_bake: blocking, on the mesh stream behind the frames already queued.  It reads nothing from the mesh: h gives
+ *     the device and the stream, and nothing on the handle is written.  Input: immesh_mesh_texture_select's rows as they are
+ *     (facet_cam [n_facets], facet_uv [n_facets][6] in the selection camera's pixels), cams (only width and height are read) and one
+ *     image per camera (data NULL for a camera no facet uses).  on_device 1: every data pointer is device memory of h's device; 0:
+ *     host memory, uploaded in camera index order in batches of whole images, each batch at most cfg.max_image_bytes bytes (packed
+ *     3 width height), into two alternating device arenas of that size, so the next batch's copy overlaps this batch's bake.
+ *   Outputs: facet_page [n_facets]: the page of the facet's cell, -1 where facet_cam = -1; atlas_uv [n_facets][6]: u0 v0 u1 v1 u2 v2 of
+ *     the corners in page texels (centres at integers), left as the caller had them where facet_cam = -1; pages [n_pages][P][P][3]
+ *     (P = cfg.page_size, rows top to bottom, the images' channel order); *n_pages; counts [4]: textured rows, untextured rows, cells,
+ *     texels written.  pages = NULL: a count query, which lays out the atlas only (facet_page, atlas_uv, *n_pages, counts).
+ *     n_pages > cap_pages with pages != NULL: IMMESH_E_CAPACITY with *n_pages set and nothing written.  Each other output may be NULL.
+ *   Export: immesh_write_obj_textured with facet_page as facet_cam, atlas_uv as facet_uv, (P, P) as every cam_wh and the pages'
+ *     image files (immesh_write_png) as image_files; untextured facets land in its "untextured" material.
+ *   Atlas rule (defined here), float64 in the order written, without fused multiply-adds:
+ *     1. Scale: a textured row's corners in its image (W x H, the selection camera Ws x Hs): u' = ((u + 0.5) W) / Ws - 0.5,
+ *        v' = ((v + 0.5) H) / Hs - 0.5.
+ *     2. Cell: L = the longest of the three edges sqrt(du du + dv dv) of (u', v'); the cell side S is the smallest power of two >= 8
+ *        and >= ceil(L) + 4, or cfg.max_cell if that is smaller.  class = log2 S.
+ *     3. Order: the textured rows sorted stably by (class descending, camera ascending); rows keep their input order inside a key.
+ *        Consecutive rows of a class share a cell: the class's q-th row (from 0) takes cell q / 2, slot q % 2.
+ *     4. Slots: texel (i, j) of a cell (i the column, j the row, 0 <= i, j < S) belongs to slot 0 when i + j <= S - 2, else to slot 1.
+ *        The triangle of slot 0 is (0, 0), (S - 4, 0), (0, S - 4); that of slot 1 is (S - 2, S - 2), (2, S - 2), (S - 2, 2); row
+ *        corner k maps to triangle corner k.  Every texel a bilinear lookup anywhere inside a slot's triangle touches belongs to that
+ *        slot and lies in the cell, so seams do not bleed at the base level (mip-maps may bleed across cells).
+ *     5. Placement: cells in sorted order, class by class; a cell's offset is the exclusive sum of (S / 8)^2 over the cells before it,
+ *        in 8 x 8-texel units.  With U = (P / 8)^2 units per page, the cell is on page offset / U at texel (8 x, 8 y), where x (the even
+ *        bits) and y (the odd bits) are the Morton decode of offset % U.  Sides only shrink, so cells are aligned and none straddles a
+ *        page.  n_pages = ceil(total units / U).  atlas_uv of a row: its cell's origin plus its slot's triangle corners.
+ *     6. Texel (i, j) of a filled slot, T = S - 4: w1 = i / T, w2 = j / T (slot 1: w1 = (S - 2 - i) / T, w2 = (S - 2 - j) / T);
+ *        a = max(w1, 0), b = max(w2, 0); if a + b > 1: s = a + b, a = a / s, b = b / s; w0 = (1 - a) - b.  The source point is
+ *        x = (w0 u'0 + a u'1) + b u'2 and the same for y, clamped to [0, W - 1] x [0, H - 1].  With x0 = floor(x), x1 = min(x0 + 1,
+ *        W - 1), fx = x - x0 (y likewise), each channel is (1 - fy) ((1 - fx) I(x0, y0) + fx I(x1, y0)) + fy ((1 - fx) I(x0, y1) +
+ *        fx I(x1, y1)), written as floor(value + 0.5).  Texels no filled slot owns are 0.
+ *   IMMESH_E_INVALID: NULL h, cams, images, cfg or n_pages; n_cams outside [1, 2^27); n_facets outside [0, 2^31) (or > 0 with NULL
+ *     facet_cam or facet_uv); on_device not 0 / 1; page_size not a power of two in [256, 8192]; max_cell not a power of two in [8, page_size];
+ *     max_image_bytes < 0; a facet_cam outside [-1, n_cams); a textured row with a non-finite uv; a used camera with a NULL image,
+ *     an image or camera size below 1, a pitch below 3 width, or (host images) an image larger than max_image_bytes; cap_pages < 0.
+ * immesh_write_png: host only.  An 8-bit RGB PNG of rgb [height][width][3] (rows top to bottom), uncompressed: stored deflate blocks,
+ *   CRC-32 and Adler-32 computed in place, so no compression library is needed.  IMMESH_E_INVALID: NULL path or rgb, a size below 1,
+ *   or a file that cannot be written. */
+typedef struct {
+    const uint8_t* data;   /* 8-bit, 3 interleaved channels (any order: the pages keep it); NULL for a camera no facet uses */
+    int width, height;     /* may differ from the selection camera's: texture coordinates are rescaled */
+    int64_t pitch;         /* bytes per row, >= 3 * width */
+} immesh_texture_image;
+typedef struct {
+    int page_size;             /* texels per page side: a power of two in [256, 8192] */
+    int max_cell;              /* the largest cell: a power of two in [8, page_size] */
+    int64_t max_image_bytes;   /* host images: device bytes of each of the two upload arenas (0: 512 MiB); must hold the largest used image */
+} immesh_texture_atlas_config;
+int immesh_mesh_texture_bake(immesh_mesh_t* h, const immesh_texture_camera* cams /* the selection's cameras: width, height */, int n_cams,
+                             const immesh_texture_image* images /*[n_cams]*/, int on_device,
+                             const int32_t* facet_cam /*[n]*/, const float* facet_uv /*[n][6]*/, int64_t n_facets,
+                             const immesh_texture_atlas_config* cfg,
+                             uint8_t* pages /*[cap_pages][page][page][3] or NULL*/, int cap_pages,
+                             int32_t* facet_page /*[n] or NULL*/, float* atlas_uv /*[n][6] or NULL*/,
+                             int* n_pages, int64_t* counts /*[4] or NULL: textured, untextured, cells, texels written*/);
+int immesh_write_png(const char* path, const uint8_t* rgb /*[h][w][3]*/, int width, int height);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
