@@ -332,6 +332,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_evaluate_stats", [C.POINTER(C.c_int64)]),
         ("immesh_mesh_texture_select", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexCfg), C.POINTER(C.c_int32), fp, C.POINTER(C.c_int32), fp, C.c_int64,
                                         C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+        ("immesh_mesh_texture_enable", [vp, C.POINTER(_TexCamera), C.POINTER(_TexCfg)]),
+        ("immesh_mesh_texture_pose", [vp, dp, dp]),
+        ("immesh_mesh_texture_rows", [vp, C.POINTER(C.c_int32), fp, C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                      C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_texture_bake", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int, C.POINTER(C.c_int32), fp, C.c_int64,
                                       C.POINTER(_AtlasCfg), vp, C.c_int, C.POINTER(C.c_int32), fp, ip, C.POINTER(C.c_int64)]),
         ("immesh_write_png", [C.c_char_p, vp, C.c_int, C.c_int]),
@@ -1239,6 +1243,51 @@ class Mesh:
                                                              counts.ctypes.data_as(i64)), "mesh_texture_select")
         return dict(cam=cam[:n].copy(), uv=uv[:n].copy(), px=px[:n].copy(), vertices=verts[:nv].copy() if vertices else None,
                     counts=dict(zip(TEXTURE_COUNT_KEYS, (int(v) for v in counts))))
+
+    def texture_enable(self, rig, *, z_near=0.1, z_far=1000.0, min_cos=0.0, min_visible_permille=0, two_sided=False, positions=0):
+        """Texture the mesh behind every queued frame: each triangle record keeps the nearest frame whose camera sees it (texture_select's
+        rule at raw positions).  rig: (width, height, (fx, fy, cx, cy), cam_R, cam_t), the colour camera in the frame's sensor frame
+        (the localization body frame, or the depth camera), OpenCV axes; None turns the texturing off.  Every record starts unobserved."""
+        if rig is None:
+            _check(self.lib, self.lib.immesh_mesh_texture_enable(self._h, None, None), "mesh_texture_enable")
+            return
+        arr, _ = texture_cameras([rig])
+        cfg = _TexCfg(float(z_near), float(z_far), float(min_cos), int(min_visible_permille), 1 if two_sided else 0, int(positions), 0)
+        _check(self.lib, self.lib.immesh_mesh_texture_enable(self._h, arr, C.byref(cfg)), "mesh_texture_enable")
+
+    def texture_pose(self, R=None, t=None):
+        """From the next queued frame on: (R, t) a fixed caller camera (camera to world, OpenCV axes) for every frame; None, None the rig."""
+        dp = C.POINTER(C.c_double)
+        if R is None and t is None:
+            _check(self.lib, self.lib.immesh_mesh_texture_pose(self._h, None, None), "mesh_texture_pose")
+            return
+        R = np.ascontiguousarray(R, dtype=np.float64).reshape(9)
+        t = np.ascontiguousarray(t, dtype=np.float64).reshape(3)
+        _check(self.lib, self.lib.immesh_mesh_texture_pose(self._h, R.ctypes.data_as(dp), t.ctypes.data_as(dp)), "mesh_texture_pose")
+
+    def texture_rows(self, vertices=True):
+        """The queued texturing's rows, ordered behind the queued frames, in texture_select's layout: dict(cam int32[nt] (the frame
+        number, -1: none), uv float32[nt,6] (NaN where cam = -1), px int32[nt,2], vertices float32[nv,3] (the snapshot's raw
+        positions, or None), counts {TEXTURE_COUNT_KEYS: int} (cameras_used: distinct frames
+        of the live rows), frames int32[nf] (ascending frames any record still uses: keep these images, delete the others)).  With the
+        cameras indexed by frame number (None images for the other frames) it goes to texture_bake and write_obj_textured."""
+        i32, i64 = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+        nf, nfr = C.c_int64(0), C.c_int64(0)
+        rc = self.lib.immesh_mesh_texture_rows(self._h, None, None, None, 0, C.byref(nf), None, None, 0, C.byref(nfr))   # a count query
+        if rc not in (0, -3):
+            _check(self.lib, rc, "mesh_texture_rows")
+        n, m = nf.value, nfr.value
+        cam = np.zeros(max(n, 1), dtype=np.int32)
+        uv = np.full((max(n, 1), 6), np.nan, dtype=np.float32)
+        px = np.zeros((max(n, 1), 2), dtype=np.int32)
+        frames = np.zeros(max(m, 1), dtype=np.int32)
+        counts = np.zeros(4, dtype=np.int64)
+        _check(self.lib, self.lib.immesh_mesh_texture_rows(self._h, cam.ctypes.data_as(i32), uv.ctypes.data_as(C.POINTER(C.c_float)), px.ctypes.data_as(i32), n,
+                                                           C.byref(nf), counts.ctypes.data_as(i64), frames.ctypes.data_as(i32), m, C.byref(nfr)),
+               "mesh_texture_rows")
+        verts = self.snapshot()[0] if vertices else None
+        return dict(cam=cam[:n].copy(), uv=uv[:n].copy(), px=px[:n].copy(), vertices=verts, counts=dict(zip(TEXTURE_COUNT_KEYS, (int(v) for v in counts))),
+                    frames=frames[:m].copy())
 
     def texture_bake(self, sel, cameras, images, *, page_size=4096, max_cell=64, max_image_bytes=0):
         """The texture atlas of a selection: every textured facet's pixels resampled out of its chosen image into square pages.

@@ -186,6 +186,21 @@ def build_texture(force=False):
     return EMU_TEXTURE
 
 
+EMU_TEXTURE_ONLINE = os.path.join(_ROOT, "tests", "texture_online", "libimmesh_emu_texture_online.so")
+
+
+def build_texture_online(force=False):
+    """tests/texture_online: the queued texturing's bodies (immesh_b200/csrc/texture_core.cuh, with the rasteriser's of reinforce.cuh)
+    in the device stage's orchestration -- the frame's camera, the per-slot counts, the update, the state's growth, the rows and the
+    frames list -- built for the host"""
+    src = os.path.join(_ROOT, "tests", "texture_online", "emu_texture_online.cpp")
+    deps = [src] + _sources(CSRC, (".cuh",)) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_TEXTURE_ONLINE, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_TEXTURE_ONLINE, src])
+    return EMU_TEXTURE_ONLINE
+
+
 EMU_TEXTURE_BAKE = os.path.join(_ROOT, "tests", "texture_bake", "libimmesh_emu_texture_bake.so")
 
 
@@ -345,6 +360,7 @@ def build_all(force=False):
     build_view_overlay(force)
     build_texture(force)
     build_texture_bake(force)
+    build_texture_online(force)
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)

@@ -12,6 +12,7 @@
 #include "mesh_feed.cuh"
 #include "mesh_voxel.cuh"
 #include "peer_win.cuh"
+#include "texture_core.cuh"
 #include "view_overlay.cuh"
 
 using immesh::LioParams; using immesh::VoxelMapDev; using immesh::ScanBuf; using immesh::LioCtrl;
@@ -293,6 +294,15 @@ struct immesh_mesh {
         immesh::MemSet dev, pinned{immesh::MemSet::Pinned};   // not counted in immesh_mesh_capacity
     } dep;
     int dev_dims_frame = 0;   // newest frame whose n, step and m were set on the device (a depth frame, a device-count hand-off)
+    // texturing queued behind every frame (immesh_mesh_texture_enable, texture_online.cu): the rig's camera at each frame (mode 0) or the
+    // caller's (mode 1, immesh_mesh_texture_pose) into img.cam; the per-record state follows the triangle pool in mesh_grow
+    struct Texture : QueuedCam {
+        immesh_texture_camera rig = {};
+        immesh_texture_config cfg = {};
+        immesh::TxoRecord* rec = nullptr;   // [M.max_t] each triangle record's chosen frame
+        int *won = nullptr, *cov = nullptr; // [M.max_t] the frame's counts, zero between frames
+        long long* pixels = nullptr;        // w * h summed over the frames with a camera since the enable
+    } tx;
 };
 
 // The live triangles in one defined order, for immesh_mesh_snapshot, _region_stream, _region_buffers and immesh_mesh_evaluate
@@ -351,6 +361,7 @@ void mesh_frame_begin_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cu
 void mesh_append_launch(const immesh_mesh* h, const immesh::FrameBuf& F, int g, cudaStream_t st, bool pdl);
 void mesh_dilate_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool pdl);
 int mesh_tri_launch(const immesh_mesh* h, const immesh::FrameBuf& F, cudaStream_t st, bool pdl);
+cudaError_t queued_cam_alloc(immesh_mesh::QueuedCam& c);
 int queued_cam_stage(immesh_mesh* h, immesh_mesh::QueuedCam& c, int s);
 void mesh_reinforce_launch(immesh_mesh* h, cudaStream_t st);
 void mesh_view_launch(immesh_mesh* h, cudaStream_t st);
@@ -364,3 +375,6 @@ cudaError_t mesh_feed_commit(immesh_mesh* h, long long frame);
 void mesh_feed_free(immesh_mesh* h);
 int mesh_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist, const int* n_dev = nullptr);
 size_t mesh_sort_hist_ints(size_t n);
+void mesh_texture_launch(immesh_mesh* h, int src, cudaStream_t st);   // texture_online.cu
+cudaError_t txo_state_alloc(immesh::MemSet& mem, size_t tris, immesh::TxoRecord** rec, int** won, int** cov);
+cudaError_t txo_state_migrate(const immesh_mesh* h, cudaStream_t st, immesh::TxoRecord* rec, int* won, int* cov, int tris, const immesh::TxoRecord* old_rec, int nt);

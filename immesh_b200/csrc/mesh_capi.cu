@@ -620,6 +620,14 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
         pool = "triangle pool (change feed)";
         if ((e = cfresh.alloc(&c_stamp, tris)) == cudaSuccess) e = cfresh.alloc(&c_pub, tris);
     }
+    // and so does the queued texturing's per-record state
+    immesh::MemSet tfresh;
+    immesh::TxoRecord* t_rec = h->tx.rec;
+    int *t_won = h->tx.won, *t_cov = h->tx.cov;
+    if (gt && h->tx.on && e == cudaSuccess) {
+        pool = "triangle pool (texturing)";
+        e = txo_state_alloc(tfresh, (size_t)tris, &t_rec, &t_won, &t_cov);
+    }
     auto fail = [&](cudaError_t err, const char* what) {
         return im_fail_alloc(err, (std::string(what) + ": " + cudaGetErrorString(err) + " during the growth; the handle is unchanged").c_str());
     };
@@ -662,6 +670,7 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
                     MG(cudaMemcpyAsync(c_pub, h->chg.C.pub, (size_t)nt, cudaMemcpyDeviceToDevice, st));
                 }
             }
+            if (t_rec != h->tx.rec) MG(txo_state_migrate(h, st, t_rec, t_won, t_cov, (int)tris, h->tx.rec, nt));
             nm.max_t = (int)tris;
             if (nm.thash != M.thash) {
                 MG(cudaMemsetAsync(nm.thash, 0xFF, tcap * 4, st));
@@ -699,6 +708,11 @@ static int mesh_grow(immesh_mesh* h, long long verts, long long tris, long long 
         h->chg.dev.take(std::move(cfresh));
         h->F.chg_stamp = c_stamp;
         h->chg.C.pub = c_pub;
+    }
+    if (t_rec != h->tx.rec) {
+        for (const void* q : {(const void*)h->tx.rec, (const void*)h->tx.won, (const void*)h->tx.cov}) h->tx.dev.free(q);
+        h->tx.dev.take(std::move(tfresh));
+        h->tx.rec = t_rec; h->tx.won = t_won; h->tx.cov = t_cov;
     }
     if (h->b_fp) {   // batched-frame scratch: allocated again at the new sizes by the next batched frame
         h->batch = immesh::MemSet();
@@ -901,11 +915,12 @@ static int mesh_enqueue(immesh_mesh* h, const FrameSrc& in, int kind, bool allow
         IM_CUDA(cudaMemcpyAsync(h->d_dyn, &d, sizeof(FrameDyn), cudaMemcpyHostToDevice, st));
     }
     // the inputs of the stages queued behind the frame
-    const bool rf_on = h->rf.on != 0, chg_on = h->chg.on != 0, vw_on = h->vw.on != 0;
+    const bool rf_on = h->rf.on != 0, chg_on = h->chg.on != 0, vw_on = h->vw.on != 0, tx_on = h->tx.on != 0;
     const bool fd_on = h->feed.on != 0, fd_img = fd_on && vw_on && h->feed.max_images > 0;
     int rc = rf_on ? queued_cam_stage(h, h->rf, s) : IMMESH_OK;
     if (!rc && fd_on) rc = mesh_feed_stage(h, s, F.frame, dev_dims ? -1 : F.n, F.step, kind, from_lio ? nullptr : in.pose_t, rf_on, fd_img);
     if (!rc && vw_on) rc = queued_cam_stage(h, h->vw, s);
+    if (!rc && tx_on) rc = queued_cam_stage(h, h->tx, s);
     if (rc) return rc;
     // the frame's launch sequence (fixed grids: grid-stride loops over the counts the kernels read on the device)
     bool nccl_failed = false;
@@ -955,6 +970,7 @@ static int mesh_enqueue(immesh_mesh* h, const FrameSrc& in, int kind, bool allow
         IM_LAUNCH_PDL(pdl && !chg_on, k_frame_end, 1, 1, 0, st, h->M);
         if (rf_on) mesh_reinforce_launch(h, st);
         if (vw_on) mesh_view_launch(h, st);
+        if (tx_on) mesh_texture_launch(h, from_lio ? 1 : depth ? 2 : 0, st);
         if (fd_on) mesh_feed_launch(h, st, rf_on, fd_img);
     };
     bool queued = false;
@@ -975,6 +991,7 @@ static int mesh_enqueue(immesh_mesh* h, const FrameSrc& in, int kind, bool allow
     h->timed_last = queued ? 0 : 1;
     if (rf_on) h->rf.last_frame = F.frame;
     if (vw_on) h->vw.last_frame = F.frame;
+    if (tx_on) h->tx.last_frame = F.frame;
     if (chg_on) h->chg.last_frame = F.frame;
     if (depth) h->dep.last_frame = F.frame;
     if (dev_dims) h->dev_dims_frame = F.frame;
@@ -1111,6 +1128,7 @@ int immesh_mesh_shard(immesh_mesh_t* h, int rank, int nranks, const char* unique
     if (h->chg.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the change feed enabled cannot be sharded (immesh_mesh_changes_enable(h, 0, 0) first)");
     if (h->feed.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the frame feed enabled cannot be sharded (immesh_mesh_feed_enable(h, NULL) first)");
     if (h->vw.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the queued view enabled cannot be sharded (immesh_mesh_view_enable(h, NULL, ...) first)");
+    if (h->tx.on) return im_fail(IMMESH_E_INVALID, "a mesh handle with the queued texturing enabled cannot be sharded (immesh_mesh_texture_enable(h, NULL, NULL) first)");
     if (!immesh::nccl().load()) return im_fail(IMMESH_E_CUDA, "libnccl.so.2 not found");
     immesh::nccl_uid_t id;
     std::memcpy(id.internal, unique_id128, 128);

@@ -19,7 +19,6 @@ using namespace immesh;
 // valid pixels in ascending pixel order (k_rf_fcount -> k_rf_scan -> k_rf_emit).  The blocking immesh_mesh_render_depth runs it at the
 // caller's pose; the queued reinforcement (immesh_mesh_reinforce_enable) runs it behind every frame, on the mesh stream and inside its
 // graph, after the camera pose (k_rf_pose), into result buffer (frame & 1).
-struct RfDyn { int mode, pad; double R[9], t[3]; };   // per frame: rf_frame_pose's source (1 = the caller's pose, 2 = the view's follow camera)
 // one block: the frame's camera (sensor-bound or the caller's), the tile counters cleared
 __global__ void __launch_bounds__(256) k_rf_pose(const double (*ring)[12], const int* ring_frame, const FrameDyn* dyn, const RfDyn* rd, int win, DepthCam base,
                                                  DepthCam* cam, RfOut o0, RfOut o1, int* tile_cnt, int ntiles) {
@@ -411,7 +410,7 @@ static bool depth_cam(DepthCam* C, const double* K, int width, int height, doubl
     return true;
 }
 // the per-frame camera source (RfDyn) and its pinned slots; stops at the first failure
-static cudaError_t queued_cam_alloc(immesh_mesh::QueuedCam& c) {
+cudaError_t queued_cam_alloc(immesh_mesh::QueuedCam& c) {
     RfDyn *rd = nullptr, *h_rd = nullptr;
     cudaError_t e = c.dev.alloc(&rd, 1);
     if (e == cudaSuccess) e = c.pinned.alloc(&h_rd, IM_SLOTS, 0);

@@ -277,6 +277,8 @@ IM_HD void rf_avr_pose(const double (*ring)[12], const int* ring_frame, int fram
     rf_quat_mul(q, c, qc);
     rf_quat_to_rot(qc, R);
 }
+// per frame, staged from a pinned slot: rf_frame_pose's source (1 = the caller's pose, 2 = the view's follow camera)
+struct RfDyn { int mode, pad; double R[9], t[3]; };
 // A queued image's camera for frame `frame` by its per-frame source: mode 0 the sensor-bound pose (rf_avr_pose); 1 the caller's
 // (R_in, t_in); 2 the follow camera (g_follow_cam with tracking_camera(Identity, t_last_avr), ImMesh_node.cpp:434-440): the fixed
 // rotation R_in at the window's mean translation plus the offset t_in (a window without a pose: a zero mean translation).

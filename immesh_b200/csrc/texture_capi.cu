@@ -21,8 +21,12 @@ namespace {
 
 // per live record (mesh_tri_order's rec index): this camera's counts, and the best camera so far with its distance and counts
 struct TexFacets { int *won, *cov, *best_cam, *best_won, *best_cov; double* best_e2; };
+// k_tex_tile counts a slot's pixels at its live record's index
+struct TexRowOf {
+    const int* row_of;
+    __device__ __forceinline__ int operator()(int slot) const { return row_of[slot]; }
+};
 
-__device__ __forceinline__ float4 tex_vertex(const MeshDev& M, int pos_mode, int v) { return view_vertex(M.vpos, M.vsmooth, M.vsmoothed, pos_mode, v); }
 __device__ __forceinline__ void tex_facet_corners(const MeshDev& M, int pos_mode, const int4& r, float4* q) {
     tex_corners(tex_vertex(M, pos_mode, r.x), tex_vertex(M, pos_mode, r.y), tex_vertex(M, pos_mode, r.z), (int)(M.tri_flip[r.w] & 1ull), q);
 }
@@ -35,54 +39,6 @@ __global__ void __launch_bounds__(128) k_tex_init(const int4* rec, int n, int* r
         F.best_cam[e] = -1; F.best_won[e] = 0; F.best_cov[e] = 0;
         F.best_e2[e] = INFINITY;
     }
-}
-
-// one block per tile, one thread per pixel (k_view_tile's shape and visibility): the bin's set-ups staged IM_RT_THREADS at a time in
-// shared memory; a covered sample is counted for its facet (ballot per warp, shared sum per block, one atomic per facet and batch), the
-// pixel's winner (depth bits, then the lower triple) gets one won pixel.  Bins over capacity (misc[0]): every triangle slot instead.
-__global__ void __launch_bounds__(IM_RT_THREADS) k_tex_tile(MeshDev M, int pos_mode, const DepthCam* cam, const int* tile_off, const int* bin, const int* misc,
-                                                            const int* row_of, int* won, int* cov) {
-    __shared__ DepthTri S[IM_RT_THREADS];
-    __shared__ int4 Q[IM_RT_THREADS];   // a b c, row
-    __shared__ int s_cov[IM_RT_THREADS];
-    const DepthCam C = *cam;
-    const int ntx = (C.w + IM_RT_TILE - 1) / IM_RT_TILE, lane = threadIdx.x & 31;
-    const int x = (blockIdx.x % ntx) * IM_RT_TILE + (int)(threadIdx.x % IM_RT_TILE), y = (blockIdx.x / ntx) * IM_RT_TILE + (int)(threadIdx.x / IM_RT_TILE);
-    const bool all = misc[0] != 0;
-    const int lo = all ? 0 : tile_off[blockIdx.x], hi = all ? min(M.cnt[IM_MC_TRIS_ALLOC], M.max_t) : tile_off[blockIdx.x + 1];
-    unsigned int best = 0x7f800000u;   // +inf: nothing drawn
-    int ba = INT_MAX, bb = INT_MAX, bc = INT_MAX, brow = -1;
-    for (int b = lo; b < hi; b += IM_RT_THREADS) {
-        const int i = b + (int)threadIdx.x;
-        bool ok = false;
-        if (i < hi) {
-            const int slot = all ? i : bin[i];
-            const int4 r = M.tri[slot];
-            ok = r.w && depth_tri_setup(C, tex_vertex(M, pos_mode, r.x), tex_vertex(M, pos_mode, r.y), tex_vertex(M, pos_mode, r.z), &S[threadIdx.x]);
-            Q[threadIdx.x] = make_int4(r.x, r.y, r.z, ok ? row_of[slot] : -1);
-        }
-        if (!ok) { S[threadIdx.x].x_lo = 1; S[threadIdx.x].x_hi = 0; }   // an empty box
-        s_cov[threadIdx.x] = 0;
-        __syncthreads();
-        const int n = min(IM_RT_THREADS, hi - b);
-        for (int j = 0; j < n; ++j) {   // uniform over the block: every lane reaches the ballot
-            const DepthTri& T = S[j];
-            bool c = false;
-            unsigned int bits = 0;
-            if (x >= T.x_lo && x <= T.x_hi && y >= T.y_lo && y <= T.y_hi) {
-                float zf;
-                if (depth_sample(T, x, y, &zf)) { bits = __float_as_uint(zf); c = bits < 0x7f800000u; }
-            }
-            const unsigned int m = __ballot_sync(0xffffffffu, c);
-            if (lane == 0 && m) atomicAdd(&s_cov[j], __popc(m));
-            const int4 q = Q[j];
-            if (c && view_better(bits, q.x, q.y, q.z, best, ba, bb, bc)) { best = bits; ba = q.x; bb = q.y; bc = q.z; brow = q.w; }
-        }
-        __syncthreads();
-        if ((int)threadIdx.x < n && s_cov[threadIdx.x]) atomicAdd(&cov[Q[threadIdx.x].w], s_cov[threadIdx.x]);
-        __syncthreads();
-    }
-    if (brow >= 0) atomicAdd(&won[brow], 1);
 }
 
 // one thread per facet: camera k's "seen" test on the counts of k_tex_tile, the nearest camera kept with a strict <; the counts cleared
@@ -126,14 +82,6 @@ __global__ void __launch_bounds__(128) k_tex_vertices(MeshDev M, int pos_mode, i
     }
 }
 
-bool tex_camera_ok(const immesh_texture_camera& c) {
-    if (c.width < 1 || c.height < 1 || (long long)c.width * c.height > (1 << 26)) return false;
-    const double k[4] = {c.fx, c.fy, c.cx, c.cy};
-    for (double v : k) if (!std::isfinite(v)) return false;
-    for (double v : c.cam_R) if (!std::isfinite(v)) return false;
-    for (double v : c.cam_t) if (!std::isfinite(v)) return false;
-    return c.fx != 0.0 && c.fy != 0.0;
-}
 int tex_tiles(int w, int h) { return ((w + IM_RT_TILE - 1) / IM_RT_TILE) * ((h + IM_RT_TILE - 1) / IM_RT_TILE); }
 
 }  // namespace
@@ -141,8 +89,7 @@ int tex_tiles(int w, int h) { return ((w + IM_RT_TILE - 1) / IM_RT_TILE) * ((h +
 int immesh_mesh_texture_select(immesh_mesh_t* h, const immesh_texture_camera* cams, int n_cams, const immesh_texture_config* cfg, int32_t* facet_cam,
                                float* facet_uv, int32_t* facet_px, float* vertices, int64_t cap, int64_t* n_facets, int64_t* counts) {
     if (!h || !cams || !cfg || !n_facets || n_cams < 1 || cap < 0) return im_fail(IMMESH_E_INVALID, "texture_select: bad argument (NULL h, cams, cfg or n_facets; n_cams < 1; cap < 0)");
-    if (!(cfg->z_near > 0) || !(cfg->z_far > cfg->z_near) || !std::isfinite(cfg->z_far) || !(cfg->min_cos >= 0.0 && cfg->min_cos <= 1.0) ||
-        cfg->min_visible_permille < 0 || cfg->min_visible_permille > 1000 || (cfg->two_sided != 0 && cfg->two_sided != 1) || (cfg->positions != 0 && cfg->positions != 1))
+    if (!tex_config_ok(*cfg))
         return im_fail(IMMESH_E_INVALID, "texture_select: bad config (0 < z_near < z_far < inf; min_cos in [0, 1]; min_visible_permille in [0, 1000]; two_sided and positions 0 or 1)");
     for (int k = 0; k < n_cams; ++k)
         if (!tex_camera_ok(cams[k]))
@@ -206,8 +153,8 @@ int immesh_mesh_texture_select(immesh_mesh_t* h, const immesh_texture_camera* ca
             ik.ntiles = tex_tiles(cams[k].width, cams[k].height);
             IM_CUDA(cudaMemsetAsync(im.tile_cnt, 0, (size_t)ik.ntiles * sizeof(int), st));
             rf_bin_launch(h, ik, pos, st);
-            IM_LAUNCH(k_tex_tile, ik.ntiles, IM_RT_THREADS, 0, st, h->M, pos, (const DepthCam*)ik.cam, (const int*)im.tile_off, (const int*)im.bin, (const int*)im.misc,
-                      (const int*)row_of, F.won, F.cov);
+            IM_LAUNCH(k_tex_tile<TexRowOf>, ik.ntiles, IM_RT_THREADS, 0, st, h->M, pos, (const DepthCam*)ik.cam, (const int*)im.tile_off, (const int*)im.bin,
+                      (const int*)im.misc, TexRowOf{row_of}, F.won, F.cov);
             IM_LAUNCH(k_tex_facet, mesh_grid(h, n, 128), 128, 0, st, h->M, pos, (const DepthCam*)ik.cam, k, rule, (const int4*)o.rec, n, F);
         }
         IM_LAUNCH(k_tex_rows, mesh_grid(h, n, 128), 128, 0, st, h->M, pos, (const DepthCam*)d_cams, (const int4*)o.rec, o.order, n, F, cam_out, uv_out, px_out, used, cnt);

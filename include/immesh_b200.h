@@ -940,6 +940,44 @@ int immesh_mesh_texture_select(immesh_mesh_t* h, const immesh_texture_camera* ca
                                int32_t* facet_px /*[cap][2] or NULL: won, covered in the chosen camera*/,
                                float* vertices /*[n_vertices][3] or NULL: the positions used*/,
                                int64_t cap, int64_t* n_facets, int64_t* counts /*[4] or NULL: textured, untextured, cameras used, pixels rasterised*/);
+/* Texturing queued behind every frame: each triangle record keeps the nearest frame whose camera sees it, updated on the device at the
+ * end of every queued frame, so a textured mesh can be read at any moment and the images no frame textures any more can be deleted.
+ *   immesh_mesh_texture_enable(h, rig, cfg): rig = the colour camera (immesh_texture_camera: width, height, fx, fy, cx, cy; cam_R, cam_t
+ *     its pose in the frame's sensor frame, OpenCV axes: the localization state's body frame for a frame handed over by a localization
+ *     handle, the depth camera for a depth frame); cfg = immesh_mesh_texture_select's config with positions = 0 (the raw positions).
+ *     As the other queued stages it drains the handle, drops the captured launch sequence and allocates everything once; every triangle
+ *     record starts unobserved (enabling again starts afresh).  rig = NULL turns it off and frees the state; off, nothing is launched,
+ *     captured or allocated.  The state is 48 + 8 bytes per triangle slot of the pool's capacity (1.75 GiB at 32 Mi slots), allocated
+ *     for the current capacity and grown with the triangle pool.
+ *   immesh_mesh_texture_pose(h, cam_R, cam_t): from the next queued frame on, (cam_R, cam_t) (finite, camera to world, OpenCV axes) is the
+ *     camera of every frame, with the rig's size and intrinsics; NULL, NULL returns to the rig (the mode after enable).
+ *   Camera of frame f (f the handle's frame number), float64 in the order written without fused multiply-adds: with the sensor pose
+ *     (R_f, t_f), R = R_f R_rig (each entry (R_f[r][0] R_rig[0][c] + R_f[r][1] R_rig[1][c]) + R_f[r][2] R_rig[2][c]) and
+ *     t = ((R_f[r][0] t_rig0 + R_f[r][1] t_rig1) + R_f[r][2] t_rig2) + t_f[r].  (R_f, t_f) is the converged (rot_end, pos_end) for
+ *     immesh_mesh_push_frame_from_lio, _async and _async_dev_n, and the depth frame's cam_R, cam_t for immesh_mesh_push_depth and
+ *     _async.  World-frame pushes (immesh_mesh_push_frame, _dev, immesh_mesh_reconstruct_from_pointcloud) have no sensor rotation:
+ *     no camera, the frame is not observed, unless a caller camera is set.  Batched frames are never observed.
+ *   Update, at the end of frame f (after its push) when it has a camera C_f: every triangle record live then gets won and covered at
+ *     C_f by immesh_mesh_texture_select's rule (steps 1-3, raw positions, cfg's z range, the record's current flip for the face order
+ *     and the front-side test); when seen with |e|^2 < the record's stored |e|^2 (strict: a tie keeps the earlier frame), the record
+ *     stores (f, |e|^2, won, covered, uv) with uv the corners' pixel coordinates in stored (ascending vertex id) order.  Records that are
+ *     not live keep their state: a record that comes back is the same three vertices, which never move.
+ *   immesh_mesh_texture_rows: blocking, on the mesh stream behind the queued frames; writes nothing on the handle.  One row per live
+ *     triangle in immesh_mesh_snapshot's order, in texture_select's layout: facet_cam = the chosen frame number or -1; facet_uv the
+ *     stored uv in the current face order, unwritten for -1 rows; facet_px won, covered at that frame (0 0 for -1).  counts [4]:
+ *     textured rows, untextured rows, distinct frames of the live rows, pixels rasterised since the enable (w h per frame with a
+ *     camera).  frames [cap_frames]: the ascending distinct frames of every record, live or not (the images still needed), *n_frames
+ *     their number.  *n_facets above cap or (frames given) *n_frames above cap_frames: IMMESH_E_CAPACITY with the counts, nothing else
+ *     written (0: a count query).  The rows go to immesh_mesh_texture_bake and immesh_write_obj_textured with the cameras indexed by
+ *     frame number.
+ *   IMMESH_E_INVALID: NULL h; a rig or cfg texture_select refuses, or positions != 0; cam_R / cam_t or frames / n_frames given one
+ *     without the other; NULL n_facets; cap or cap_frames < 0; texture_pose or texture_rows while off; a sharded handle
+ *     (immesh_mesh_shard refuses a handle with the texturing on). */
+int immesh_mesh_texture_enable(immesh_mesh_t* h, const immesh_texture_camera* rig /* NULL: off */, const immesh_texture_config* cfg);
+int immesh_mesh_texture_pose(immesh_mesh_t* h, const double* cam_R /*[9] or NULL*/, const double* cam_t /*[3] or NULL*/);
+int immesh_mesh_texture_rows(immesh_mesh_t* h, int32_t* facet_cam /*[cap] or NULL*/, float* facet_uv /*[cap][6] or NULL*/,
+                             int32_t* facet_px /*[cap][2] or NULL*/, int64_t cap, int64_t* n_facets, int64_t* counts /*[4] or NULL*/,
+                             int32_t* frames /*[cap_frames] or NULL*/, int64_t cap_frames, int64_t* n_frames /*or NULL*/);
 int immesh_write_obj_textured(const char* obj_path, const char* mtl_path, const float* vertices /*[nv][3]*/, int nv,
                               const int32_t* triangles /*[nt][3]*/, const int32_t* flips /*[nt] or NULL*/, const int32_t* facet_cam /*[nt]*/,
                               const float* facet_uv /*[nt][6]*/, int nt, const int32_t* cam_wh /*[n_cams][2]*/, const char* const* image_files /*[n_cams]*/,
