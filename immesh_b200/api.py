@@ -67,6 +67,16 @@ class _AtlasCfg(C.Structure):
 BAKE_COUNT_KEYS = ("textured", "untextured", "cells", "texels")
 
 
+class _TexViewCfg(C.Structure):
+    _fields_ = [("z_near", C.c_double), ("z_far", C.c_double), ("positions", C.c_int), ("untextured", C.c_uint8 * 3), ("background", C.c_uint8 * 3),
+                ("max_image_bytes", C.c_int64)]
+
+
+# Mesh.render_textured's counts: pixels won by a textured / an untextured row, pixels without a sample, cameras sampled; with a truth
+# image the sums over the textured pixels of the squared difference per channel and of the absolute difference over all channels
+TEXTURE_VIEW_COUNT_KEYS = ("textured", "untextured", "empty", "cameras_sampled", "sse_0", "sse_1", "sse_2", "sad")
+
+
 def texture_images(images):
     """(ctypes array of immesh_texture_image, on_device, keep-alive list) from HxWx3 uint8 numpy arrays or CUDA torch tensors (all one
     kind; None for a camera no facet uses).  Rows may be padded; pixels must be 3 contiguous bytes."""
@@ -338,6 +348,9 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
                                       C.POINTER(C.c_int32), C.c_int64, C.POINTER(C.c_int64)]),
         ("immesh_mesh_texture_bake", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int, C.POINTER(C.c_int32), fp, C.c_int64,
                                       C.POINTER(_AtlasCfg), vp, C.c_int, C.POINTER(C.c_int32), fp, ip, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_render_textured", [vp, C.POINTER(_TexCamera), C.POINTER(_TexViewCfg), C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int,
+                                         C.POINTER(C.c_int32), fp, C.c_int64, C.POINTER(_TexImage), vp, fp, C.POINTER(C.c_int32), vp, C.POINTER(C.c_int64)]),
+        ("immesh_mesh_render_textured_stats", [dp]),
         ("immesh_write_png", [C.c_char_p, vp, C.c_int, C.c_int]),
         ("immesh_write_obj_textured", [C.c_char_p, C.c_char_p, fp, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), fp, C.c_int,
                                        C.POINTER(C.c_int32), C.POINTER(C.c_char_p), C.c_int]),
@@ -1318,6 +1331,65 @@ class Mesh:
                "mesh_texture_bake")
         del keep
         return dict(pages=pages, page=page[:n].copy(), uv=auv[:n].copy(), counts=dict(zip(BAKE_COUNT_KEYS, (int(v) for v in counts))))
+
+    def render_textured(self, view, sel, cameras, images=None, *, truth=None, z_near=0.1, z_far=1000.0, positions=0, untextured=(128, 128, 128),
+                        background=(0, 0, 0), max_image_bytes=0):
+        """The textured mesh rendered at camera view ((width, height, (fx, fy, cx, cy), cam_R, cam_t), OpenCV axes, camera to world), and
+        scored against truth, a photo taken there.  sel: rows of texture_select or texture_rows (cam, uv), or of texture_bake (page, uv);
+        cameras: the rows' camera tuples (only the sizes are read: (P, P) per page for the bake's rows); images: per camera an HxWx3 uint8
+        numpy array or CUDA torch tensor (all one kind, truth too), None for a camera the view does not sample.  images None: the query
+        (depth, facet, needed and the first four counts).  positions: the rows' own setting.  Blocking, ordered behind the queued frames;
+        writes nothing on the handle.  Returns dict(rgb uint8[h,w,3] (None for the query), depth float32[h,w] (render_view's), facet
+        int32[h,w] (the winning snapshot row, -1: no sample), needed uint8[n_cams] (1: the view samples that camera), counts
+        {TEXTURE_VIEW_COUNT_KEYS: int}); with truth also mse = sum sse / (3 n), psnr = 10 log10(255^2 / mse) (inf when mse = 0), mae =
+        sad / (3 n) and coverage = n / (w h), n the textured pixels (mse, psnr and mae NaN when n = 0).  Report coverage beside psnr:
+        texturing fewer pixels can raise psnr."""
+        vw, _ = texture_cameras([view])
+        arr, n_cams = texture_cameras(cameras)
+        keep = []
+        imgs, on_device = None, 0
+        if images is not None:
+            imgs, on_device, keep = texture_images(images)
+        tr = None
+        if truth is not None:
+            if images is None:
+                raise ValueError("render_textured: truth needs images")
+            tr, t_dev, tk = texture_images([truth])
+            if t_dev != on_device and any(im is not None for im in images):
+                raise ValueError("render_textured: truth and images must be the same kind")
+            on_device = t_dev if all(im is None for im in images) else on_device
+            keep += tk
+        cam = np.ascontiguousarray(sel["cam"] if "cam" in sel else sel["page"], dtype=np.int32).reshape(-1)
+        uv = np.ascontiguousarray(sel["uv"], dtype=np.float32).reshape(-1, 6)
+        cfg = _TexViewCfg(float(z_near), float(z_far), int(positions), (C.c_uint8 * 3)(*untextured), (C.c_uint8 * 3)(*background), int(max_image_bytes))
+        w, h = int(view[0]), int(view[1])
+        rgb = np.zeros((h, w, 3), np.uint8) if images is not None else None
+        depth = np.zeros((h, w), np.float32)
+        facet = np.zeros((h, w), np.int32)
+        needed = np.zeros(max(n_cams, 1), np.uint8)
+        counts = np.zeros(8, np.int64)
+        i32 = C.POINTER(C.c_int32)
+        _check(self.lib, self.lib.immesh_mesh_render_textured(self._h, vw, C.byref(cfg), arr, n_cams, imgs, on_device, cam.ctypes.data_as(i32),
+                                                              uv.ctypes.data_as(C.POINTER(C.c_float)), len(cam), tr,
+                                                              None if rgb is None else rgb.ctypes.data_as(C.c_void_p), depth.ctypes.data_as(C.POINTER(C.c_float)),
+                                                              facet.ctypes.data_as(i32), needed.ctypes.data_as(C.c_void_p), counts.ctypes.data_as(C.POINTER(C.c_int64))),
+               "mesh_render_textured")
+        del keep
+        out = dict(rgb=rgb, depth=depth, facet=facet, needed=needed[:n_cams].copy(), counts=dict(zip(TEXTURE_VIEW_COUNT_KEYS, (int(v) for v in counts))))
+        if truth is not None:
+            n = int(counts[0])
+            sse, sad = int(counts[4] + counts[5] + counts[6]), int(counts[7])
+            mse = sse / (3.0 * n) if n else float("nan")
+            out.update(mse=mse, psnr=(float("inf") if mse == 0 else 10.0 * np.log10(255.0 ** 2 / mse)) if n else float("nan"),
+                       mae=sad / (3.0 * n) if n else float("nan"), coverage=n / float(w * h))
+        return out
+
+    def render_textured_stats(self):
+        """the phases of this thread's last render_textured in ms, from CUDA events: dict(pass_a, pass_b (host images: with the uploads
+        it waits for), score)"""
+        ms = np.zeros(3, np.float64)
+        _check(self.lib, self.lib.immesh_mesh_render_textured_stats(ms.ctypes.data_as(C.POINTER(C.c_double))), "mesh_render_textured_stats")
+        return dict(zip(("pass_a", "pass_b", "score"), (float(v) for v in ms)))
 
     def region_stream(self, region_size=10.0, cap=1 << 16):
         """(region_keys int32[nr,3], region_offsets int32[nr+1], triangles int32[nt,3]) -- the viewer's region-bucketed triangle sets."""

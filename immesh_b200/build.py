@@ -215,6 +215,21 @@ def build_texture_bake(force=False):
     return EMU_TEXTURE_BAKE
 
 
+EMU_TEXTURE_RENDER = os.path.join(_ROOT, "tests", "texture_render", "libimmesh_emu_texture_render.so")
+
+
+def build_texture_render(force=False):
+    """tests/texture_render: the textured render's bodies and argument check (immesh_b200/csrc/texture_render_core.cuh, with the bake's
+    scaling, bilinear sample and batch plan and the rasteriser's bodies) in the device call's orchestration -- binning, tiles, the
+    needed check, pass B per host-image batch and the score -- built for the host"""
+    src = os.path.join(_ROOT, "tests", "texture_render", "emu_texture_render.cpp")
+    deps = [src] + _sources(CSRC, (".cuh",)) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_TEXTURE_RENDER, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_TEXTURE_RENDER, src])
+    return EMU_TEXTURE_RENDER
+
+
 EMU_VIEW_OVERLAY = os.path.join(_ROOT, "tests", "view_overlay", "libimmesh_emu_view_overlay.so")
 
 
@@ -361,6 +376,7 @@ def build_all(force=False):
     build_texture(force)
     build_texture_bake(force)
     build_texture_online(force)
+    build_texture_render(force)
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <functional>
+#include <vector>
 
 #include "common_host.hpp"
 #include "depth_frame.cuh"
@@ -376,5 +378,8 @@ void mesh_feed_free(immesh_mesh* h);
 int mesh_sort_passes(cudaStream_t st, unsigned int* const k[2], unsigned int* const v[2], int cur, int n, int passes, int* hist, const int* n_dev = nullptr);
 size_t mesh_sort_hist_ints(size_t n);
 void mesh_texture_launch(immesh_mesh* h, int src, cudaStream_t st);   // texture_online.cu
+namespace immesh { struct BakeImg; }
+int tex_upload_batches(cudaStream_t st, const immesh_texture_image* images, const unsigned char* want, const std::vector<int>& batch_start,   // texture_bake.cu
+                       unsigned char* const arena[2], std::vector<immesh::BakeImg>& himg, immesh::BakeImg* d_img, const std::function<void(int, int)>& run);
 cudaError_t txo_state_alloc(immesh::MemSet& mem, size_t tris, immesh::TxoRecord** rec, int** won, int** cov);
 cudaError_t txo_state_migrate(const immesh_mesh* h, cudaStream_t st, immesh::TxoRecord* rec, int* won, int* cov, int tris, const immesh::TxoRecord* old_rec, int nt);

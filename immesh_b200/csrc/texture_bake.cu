@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -160,6 +161,39 @@ int bake_sort_passes(long long max_key) {
 
 }  // namespace
 
+// Host images in camera order through two alternating device arenas (the batches of bake_batches, batch_start ending with n_cams):
+// each batch's images are copied on an upload stream into arena[batch & 1], their entries of himg / d_img [n_cams] point there
+// (pitch 3 width), and run(first, last) -- the batch's first and last wanted camera -- queues the batch's work on st behind its
+// copies; a copy into an arena waits for the work that last read it.  Shared by immesh_mesh_texture_bake and
+// immesh_mesh_render_textured.
+int tex_upload_batches(cudaStream_t st, const immesh_texture_image* images, const unsigned char* want, const std::vector<int>& batch_start,
+                       unsigned char* const arena[2], std::vector<BakeImg>& himg, BakeImg* d_img, const std::function<void(int, int)>& run) {
+    BakeStreams S;
+    IM_CUDA(S.create());
+    for (size_t bi = 0; bi + 1 < batch_start.size(); ++bi) {
+        const int a = (int)(bi & 1), k0 = batch_start[bi], k1 = batch_start[bi + 1];
+        if (bi >= 2) IM_CUDA(cudaStreamWaitEvent(S.up, S.ev_done[a], 0));   // the work that last read this arena
+        long long off = 0;
+        int first = -1, last = -1;
+        for (int k = k0; k < k1; ++k) {
+            if (!want[k]) continue;
+            const immesh_texture_image& im = images[k];
+            IM_CUDA(cudaMemcpy2DAsync(arena[a] + off, (size_t)im.width * 3, im.data, (size_t)im.pitch, (size_t)im.width * 3, (size_t)im.height,
+                                      cudaMemcpyHostToDevice, S.up));
+            himg[k] = BakeImg{arena[a] + off, im.width, im.height, 3LL * im.width};
+            off += bake_image_bytes(im);
+            if (first < 0) first = k;
+            last = k;
+        }
+        IM_CUDA(cudaMemcpyAsync(d_img + k0, himg.data() + k0, (size_t)(k1 - k0) * sizeof(BakeImg), cudaMemcpyHostToDevice, S.up));
+        IM_CUDA(cudaEventRecord(S.ev_up[a], S.up));
+        IM_CUDA(cudaStreamWaitEvent(st, S.ev_up[a], 0));
+        run(first, last);
+        IM_CUDA(cudaEventRecord(S.ev_done[a], st));
+    }
+    return IMMESH_OK;
+}
+
 int immesh_mesh_texture_bake(immesh_mesh_t* h, const immesh_texture_camera* cams, int n_cams, const immesh_texture_image* images, int on_device,
                              const int32_t* facet_cam, const float* facet_uv, int64_t n_facets, const immesh_texture_atlas_config* cfg, uint8_t* pages,
                              int cap_pages, int32_t* facet_page, float* atlas_uv, int* n_pages, int64_t* counts) {
@@ -247,18 +281,7 @@ int immesh_mesh_texture_bake(immesh_mesh_t* h, const immesh_texture_camera* cams
         // host images: batches of whole used images in camera order, each at most max_image_bytes
         std::vector<int> batch_start;   // the first camera of every batch, then n_cams
         long long arena_bytes = 0;
-        if (!on_device) {
-            const long long cap = bake_arena_bytes(*cfg);
-            long long fill = cap + 1;
-            for (int k = 0; k < n_cams; ++k) {
-                if (!used[k]) continue;
-                const long long b = bake_image_bytes(images[k]);
-                if (fill + b > cap) { batch_start.push_back(k); fill = 0; }
-                fill += b;
-                arena_bytes = std::max(arena_bytes, fill);
-            }
-            batch_start.push_back(n_cams);
-        }
+        if (!on_device) batch_start = bake_batches(images, used.data(), n_cams, bake_arena_bytes(cfg->max_image_bytes), &arena_bytes);
         {
             cudaError_t e = mem.alloc(&d_pages, (size_t)np * page_bytes);
             for (int a = 0; a < 2 && e == cudaSuccess && arena_bytes > 0 && (a == 0 || batch_start.size() > 2); ++a) e = mem.alloc(&arena[a], (size_t)arena_bytes);
@@ -272,30 +295,9 @@ int immesh_mesh_texture_bake(immesh_mesh_t* h, const immesh_texture_camera* cams
         if (on_device) {
             IM_CUDA(cudaMemcpyAsync(d_img, himg.data(), (size_t)n_cams * sizeof(BakeImg), cudaMemcpyHostToDevice, st));
             bake(0, nt);
-        } else {
-            BakeStreams S;
-            IM_CUDA(S.create());
-            for (size_t bi = 0; bi + 1 < batch_start.size(); ++bi) {
-                const int a = (int)(bi & 1), k0 = batch_start[bi], k1 = batch_start[bi + 1];
-                if (bi >= 2) IM_CUDA(cudaStreamWaitEvent(S.up, S.ev_done[a], 0));   // the bake that last read this arena
-                long long off = 0;
-                int first = -1, last = -1;
-                for (int k = k0; k < k1; ++k) {
-                    if (!used[k]) continue;
-                    const immesh_texture_image& im = images[k];
-                    IM_CUDA(cudaMemcpy2DAsync(arena[a] + off, (size_t)im.width * 3, im.data, (size_t)im.pitch, (size_t)im.width * 3, (size_t)im.height,
-                                              cudaMemcpyHostToDevice, S.up));
-                    himg[k] = BakeImg{arena[a] + off, im.width, im.height, 3LL * im.width};
-                    off += bake_image_bytes(im);
-                    if (first < 0) first = k;
-                    last = k;
-                }
-                IM_CUDA(cudaMemcpyAsync(d_img + k0, himg.data() + k0, (size_t)(k1 - k0) * sizeof(BakeImg), cudaMemcpyHostToDevice, S.up));
-                IM_CUDA(cudaEventRecord(S.ev_up[a], S.up));
-                IM_CUDA(cudaStreamWaitEvent(st, S.ev_up[a], 0));
-                bake(hlo[first], hhi[last]);
-                IM_CUDA(cudaEventRecord(S.ev_done[a], st));
-            }
+        } else if (const int rc = tex_upload_batches(st, images, used.data(), batch_start, arena, himg, d_img,
+                                                     [&](int first, int last) { bake(hlo[first], hhi[last]); })) {
+            return rc;
         }
         IM_CUDA(cudaGetLastError());
         IM_CUDA(cudaMemcpyAsync(pages, d_pages, (size_t)np * page_bytes, cudaMemcpyDeviceToHost, st));

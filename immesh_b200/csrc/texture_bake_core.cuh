@@ -4,6 +4,7 @@
 // order (built with -fmad=false on the device and -ffp-contract=off on the host).  Also the call's argument check, host code shared
 // with the emulation so that both refuse the same inputs.
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <string>
 #include <vector>
@@ -70,18 +71,9 @@ IM_HD void bake_morton(long long off, int* x, int* y) {
     *x = ux; *y = uy;
 }
 
-// rule 6: texel (i, j) of slot `slot` in a cell of side S for scaled corners p, sampled bilinearly with clamp to edge from image I
-IM_HD void bake_texel(const BakeImg& I, const double* p, int S, int slot, int i, int j, unsigned char* out) {
-    const double T = (double)(S - 4);
-    const double w1 = (double)(slot ? S - 2 - i : i) / T, w2 = (double)(slot ? S - 2 - j : j) / T;
-    double a = w1 > 0.0 ? w1 : 0.0, b = w2 > 0.0 ? w2 : 0.0;
-    if (a + b > 1.0) {
-        const double s = a + b;
-        a = a / s;
-        b = b / s;
-    }
-    const double w0 = (1.0 - a) - b;
-    double x = (w0 * p[0] + a * p[2]) + b * p[4], y = (w0 * p[1] + a * p[3]) + b * p[5];
+// rule 6's sample: the point (x, y) clamped to [0, W - 1] x [0, H - 1], then each channel bilinear from x0 = floor(x), x1 = min(x0 + 1,
+// W - 1), fx = x - x0 (y likewise), written as floor(value + 0.5)
+IM_HD void bake_bilinear(const BakeImg& I, double x, double y, unsigned char* out) {
     const double xm = (double)(I.w - 1), ym = (double)(I.h - 1);
     x = x < 0.0 ? 0.0 : (x > xm ? xm : x);
     y = y < 0.0 ? 0.0 : (y > ym ? ym : y);
@@ -98,10 +90,68 @@ IM_HD void bake_texel(const BakeImg& I, const double* p, int S, int slot, int i,
     }
 }
 
+// rule 6: texel (i, j) of slot `slot` in a cell of side S for scaled corners p, sampled bilinearly with clamp to edge from image I
+IM_HD void bake_texel(const BakeImg& I, const double* p, int S, int slot, int i, int j, unsigned char* out) {
+    const double T = (double)(S - 4);
+    const double w1 = (double)(slot ? S - 2 - i : i) / T, w2 = (double)(slot ? S - 2 - j : j) / T;
+    double a = w1 > 0.0 ? w1 : 0.0, b = w2 > 0.0 ? w2 : 0.0;
+    if (a + b > 1.0) {
+        const double s = a + b;
+        a = a / s;
+        b = b / s;
+    }
+    const double w0 = (1.0 - a) - b;
+    bake_bilinear(I, (w0 * p[0] + a * p[2]) + b * p[4], (w0 * p[1] + a * p[3]) + b * p[5], out);
+}
+
 // host code
 inline bool bake_pow2_in(long long v, long long lo, long long hi) { return v >= lo && v <= hi && (v & (v - 1)) == 0; }
 inline long long bake_image_bytes(const immesh_texture_image& im) { return 3LL * im.width * im.height; }
-inline long long bake_arena_bytes(const immesh_texture_atlas_config& cfg) { return cfg.max_image_bytes > 0 ? cfg.max_image_bytes : 512LL << 20; }
+inline long long bake_arena_bytes(long long max_image_bytes) { return max_image_bytes > 0 ? max_image_bytes : 512LL << 20; }
+
+// the rows' part of the argument check: facet_cam in [-1, n_cams), finite uv on every textured row.  *n_tex: the textured rows;
+// used [n_cams]: 1 for a camera some row uses.  An empty string when the rows are valid, else the reason.
+inline std::string bake_check_rows(int n_cams, const int32_t* facet_cam, const float* facet_uv, int64_t n_facets, long long* n_tex,
+                                   std::vector<unsigned char>& used) {
+    used.assign((size_t)n_cams, 0);
+    *n_tex = 0;
+    for (int64_t r = 0; r < n_facets; ++r) {
+        const int k = facet_cam[r];
+        if (k < -1 || k >= n_cams) return "facet_cam outside [-1, n_cams) in row " + std::to_string(r);
+        if (k < 0) continue;
+        for (int c = 0; c < 6; ++c)
+            if (!std::isfinite(facet_uv[6 * r + c])) return "a textured row with a non-finite uv: row " + std::to_string(r);
+        used[k] = 1;
+        ++*n_tex;
+    }
+    return std::string();
+}
+// the image part for camera k, which some row uses: an image, image and camera sizes >= 1, a pitch >= 3 width, and for host images
+// at most `arena` bytes
+inline std::string bake_check_image(const immesh_texture_camera* cams, const immesh_texture_image* images, int on_device, long long arena, int k) {
+    const immesh_texture_image& im = images[k];
+    if (!im.data || im.width < 1 || im.height < 1 || im.pitch < 3LL * im.width || cams[k].width < 1 || cams[k].height < 1)
+        return "camera " + std::to_string(k) + " is used: it needs an image, image and camera sizes >= 1 and a pitch >= 3 width";
+    if (!on_device && bake_image_bytes(im) > arena) return "camera " + std::to_string(k) + "'s image is larger than max_image_bytes";
+    return std::string();
+}
+
+// Host images: the cameras with want[k] in index order, batched into whole images of at most `arena` bytes each (packed 3 width
+// height).  Returns the first camera of every batch, then n_cams; *fill_max: the bytes of the largest batch.
+inline std::vector<int> bake_batches(const immesh_texture_image* images, const unsigned char* want, int n_cams, long long arena, long long* fill_max) {
+    std::vector<int> start;
+    long long fill = arena + 1;
+    *fill_max = 0;
+    for (int k = 0; k < n_cams; ++k) {
+        if (!want[k]) continue;
+        const long long b = bake_image_bytes(images[k]);
+        if (fill + b > arena) { start.push_back(k); fill = 0; }
+        fill += b;
+        *fill_max = std::max(*fill_max, fill);
+    }
+    start.push_back(n_cams);
+    return start;
+}
 
 // the argument check of immesh_mesh_texture_bake (everything but h): an empty string when the call may proceed, else the reason.
 // *n_tex: the textured rows.  used [n_cams]: 1 for a camera some row uses.
@@ -114,26 +164,10 @@ inline std::string bake_check(const immesh_texture_camera* cams, int n_cams, con
                "not 0 / 1; cap_pages < 0)";
     if (!bake_pow2_in(cfg->page_size, 256, 8192) || !bake_pow2_in(cfg->max_cell, 8, cfg->page_size) || cfg->max_image_bytes < 0)
         return "bad config (page_size a power of two in [256, 8192]; max_cell a power of two in [8, page_size]; max_image_bytes >= 0)";
-    used.assign((size_t)n_cams, 0);
-    *n_tex = 0;
-    for (int64_t r = 0; r < n_facets; ++r) {
-        const int k = facet_cam[r];
-        if (k < -1 || k >= n_cams) return "facet_cam outside [-1, n_cams) in row " + std::to_string(r);
-        if (k < 0) continue;
-        for (int c = 0; c < 6; ++c)
-            if (!std::isfinite(facet_uv[6 * r + c])) return "a textured row with a non-finite uv: row " + std::to_string(r);
-        used[k] = 1;
-        ++*n_tex;
-    }
-    for (int k = 0; k < n_cams; ++k) {
-        if (!used[k]) continue;
-        const immesh_texture_image& im = images[k];
-        if (!im.data || im.width < 1 || im.height < 1 || im.pitch < 3LL * im.width || cams[k].width < 1 || cams[k].height < 1)
-            return "camera " + std::to_string(k) + " is used: it needs an image, image and camera sizes >= 1 and a pitch >= 3 width";
-        if (!on_device && bake_image_bytes(im) > bake_arena_bytes(*cfg))
-            return "camera " + std::to_string(k) + "'s image is larger than max_image_bytes";
-    }
-    return std::string();
+    std::string why = bake_check_rows(n_cams, facet_cam, facet_uv, n_facets, n_tex, used);
+    for (int k = 0; k < n_cams && why.empty(); ++k)
+        if (used[k]) why = bake_check_image(cams, images, on_device, bake_arena_bytes(cfg->max_image_bytes), k);
+    return why;
 }
 
 }  // namespace immesh

@@ -1042,6 +1042,60 @@ int immesh_mesh_texture_bake(immesh_mesh_t* h, const immesh_texture_camera* cams
                              int32_t* facet_page /*[n] or NULL*/, float* atlas_uv /*[n][6] or NULL*/,
                              int* n_pages, int64_t* counts /*[4] or NULL: textured, untextured, cells, texels written*/);
 int immesh_write_png(const char* path, const uint8_t* rgb /*[h][w][3]*/, int width, int height);
+/* The textured mesh rendered at any camera, and scored against a photo taken there: a preview without a display or an external viewer,
+ * and the photometric measure of texture quality (render at a camera whose photo was held out of the texturing, compare with it).
+ *   immesh_mesh_render_textured: blocking, on the mesh stream behind the frames already queued; it reads the mesh and writes nothing on
+ *     the handle.  Input: rows of any of the three producers, one per live triangle in immesh_mesh_snapshot's order -- texture_select's
+ *     (facet_cam, facet_uv) with its cameras and images; texture_rows' with cameras and images indexed by frame number; or the bake's
+ *     (facet_page, atlas_uv) with (P, P) cameras and the pages as images.  cams: only width and height are read (the size the uv were
+ *     made at); images [n_cams] as immesh_mesh_texture_bake's (on_device 1: device memory of h's device, 0: host memory uploaded in
+ *     camera order through two alternating arenas of cfg.max_image_bytes), but only the cameras the view samples are read: an entry
+ *     may be NULL for any other.  truth (or NULL): a photo at the view's size, in the same memory as the images.
+ *   Outputs, each may be NULL: rgb [h][w][3]; depth [h][w]; facet [h][w] the winning triangle's snapshot row, -1 where no triangle has
+ *     a sample; needed [n_cams] 1 where some pixel samples camera k, else 0; counts [8]: pixels won by a textured row, pixels won by an
+ *     untextured row (facet_cam = -1), pixels without a sample, cameras sampled, then with truth the sums over the textured pixels of
+ *     (rgb - truth)^2 for channels 0, 1 and 2 and of |rgb - truth| over all three channels (0 without truth).  Every count is an integer
+ *     sum, so the result does not depend on atomics or scheduling.
+ *   images = NULL: a query.  It resolves visibility and writes depth, facet, needed and counts [0, 4) (rgb and truth must be NULL): a
+ *     caller whose images live on disk by frame number loads only the needed ones.
+ *   Pixel rule (defined here), float64 in the order written, without fused multiply-adds:
+ *     1. Camera: view is an OpenCV camera, converted to the rasteriser's exactly as texture_select's step 1.
+ *     2. Visibility: immesh_mesh_render_view's rule unchanged at cfg's z range and positions; the nearest depth bits win, then the
+ *        lower (a, b, c) triple.  depth is immesh_mesh_render_view's depth image at that camera bit for bit (-1 at or beyond 0.99 z_far
+ *        or without a sample).
+ *     3. Weights: the winner's set-up with its corners p0 p1 p2 in stored (ascending id) order, w_i = e_i (1 / z_i) from the sample's
+ *        edge functions, as render_view's shading.
+ *     4. Face order: the row's corners are q0 q1 q2 of immesh_write_ply's face order, so o0 = w0, o1 = flip ? w1 : w2,
+ *        o2 = flip ? w2 : w1 with flip the triangle's current m_index_flip.
+ *     5. Source point: the row's uv scaled to image k = facet_cam[row] (W x H, cams[k] Ws x Hs) by the bake's rule 1:
+ *        u'_j = ((u_j + 0.5) W) / Ws - 0.5, v'_j likewise; x = ((o0 u'0 + o1 u'1) + o2 u'2) / ((o0 + o1) + o2), y likewise.  This is
+ *        the perspective-correct interpolation an OBJ viewer applies to immesh_write_obj_textured's output, pixel centres at integers.
+ *     6. Sample: the bake's rule 6 at (x, y): clamped to [0, W - 1] x [0, H - 1], bilinear, each channel floor(value + 0.5).
+ *     7. Colour: a pixel won by a textured row gets its sample; won by an untextured row, cfg.untextured; without a sample,
+ *        cfg.background.  As in render_view, a pixel with a sample is coloured even where its depth is -1 beyond 0.99 z_far.
+ *   IMMESH_E_INVALID, nothing written: NULL h, view, cfg or cams; n_cams < 1; a view texture_select refuses as a camera; not 0 <
+ *     z_near < z_far < inf, positions not 0 / 1 or max_image_bytes < 0; on_device not 0 / 1; n_facets other than the live triangle
+ *     count (rows of another mesh state; their match beyond the count is the caller's contract, as for the bake and the export) or
+ *     > 0 with NULL rows; a facet_cam outside [-1, n_cams) or a textured row with a non-finite uv; a given image of a used camera that
+ *     the bake refuses (size or camera size below 1, pitch below 3 width, a host image larger than max_image_bytes); a NULL image for a
+ *     camera the view samples; a truth image not of the view's size or with a pitch below 3 width; rgb or truth with images = NULL; a
+ *     sharded handle. */
+typedef struct {
+    double z_near, z_far;        /* the view's z range: 0 < z_near < z_far < inf */
+    int positions;               /* 0 raw, 1 the smoothed position where m_smoothed is set: pass the rows' own setting */
+    uint8_t untextured[3];       /* a pixel won by an untextured facet, e.g. (128, 128, 128): the MTL's Kd 0.5 */
+    uint8_t background[3];       /* a pixel without a sample, e.g. (0, 0, 0): the viewer's clear colour */
+    int64_t max_image_bytes;     /* host images: bytes of each of the two upload arenas (0: 512 MiB); must hold the largest needed image */
+} immesh_texture_view_config;
+int immesh_mesh_render_textured(immesh_mesh_t* h, const immesh_texture_camera* view, const immesh_texture_view_config* cfg,
+                                const immesh_texture_camera* cams /* width, height */, int n_cams, const immesh_texture_image* images /*[n_cams] or NULL*/,
+                                int on_device, const int32_t* facet_cam /*[n_facets]*/, const float* facet_uv /*[n_facets][6]*/, int64_t n_facets,
+                                const immesh_texture_image* truth /* or NULL */, uint8_t* rgb /*[h][w][3] or NULL*/, float* depth /*[h][w] or NULL*/,
+                                int32_t* facet /*[h][w] or NULL*/, uint8_t* needed /*[n_cams] or NULL*/, int64_t* counts /*[8] or NULL*/);
+/* The phases of this thread's last successful immesh_mesh_render_textured, in milliseconds from CUDA events on the mesh stream:
+ * ms [3] = pass A (snapshot order, binning, tiles), pass B (with host images the uploads it waits for included), score (with a host
+ * truth image its upload included). */
+int immesh_mesh_render_textured_stats(double* ms /*[3]*/);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
