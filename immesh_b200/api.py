@@ -77,6 +77,15 @@ class _TexViewCfg(C.Structure):
 TEXTURE_VIEW_COUNT_KEYS = ("textured", "untextured", "empty", "cameras_sampled", "sse_0", "sse_1", "sse_2", "sad")
 
 
+class _TexGainsCfg(C.Structure):
+    _fields_ = [("sel", _TexCfg), ("sigma_n", C.c_double), ("sigma_g", C.c_double), ("max_pairs", C.c_int64), ("max_image_bytes", C.c_int64)]
+
+
+# Mesh.texture_gains' counts: pairs (k, c), sample pairs used, sample pairs clipped (a channel at 0 or 255), observer cameras rasterised,
+# cameras left at gain 1 (in no pair), CG iterations (the most over the channels), pixels rasterised, spare
+TEXTURE_GAINS_COUNT_KEYS = ("pairs", "samples", "clipped", "observers", "unpaired", "cg_iterations", "pixels", "spare")
+
+
 def texture_images(images):
     """(ctypes array of immesh_texture_image, on_device, keep-alive list) from HxWx3 uint8 numpy arrays or CUDA torch tensors (all one
     kind; None for a camera no facet uses).  Rows may be padded; pixels must be 3 contiguous bytes."""
@@ -351,6 +360,10 @@ def load_library(path: Optional[str] = None) -> C.CDLL:
         ("immesh_mesh_render_textured", [vp, C.POINTER(_TexCamera), C.POINTER(_TexViewCfg), C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int,
                                          C.POINTER(C.c_int32), fp, C.c_int64, C.POINTER(_TexImage), vp, fp, C.POINTER(C.c_int32), vp, C.POINTER(C.c_int64)]),
         ("immesh_mesh_render_textured_stats", [dp]),
+        ("immesh_mesh_texture_gains", [vp, C.POINTER(_TexCamera), C.c_int, C.POINTER(_TexImage), C.c_int, C.POINTER(C.c_int32), fp, C.c_int64,
+                                       C.POINTER(_TexGainsCfg), dp, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+        ("immesh_mesh_texture_gains_stats", [dp]),
+        ("immesh_texture_apply_gains", [vp, C.POINTER(_TexImage), C.POINTER(_TexImage), C.c_int, C.c_int, dp]),
         ("immesh_write_png", [C.c_char_p, vp, C.c_int, C.c_int]),
         ("immesh_write_obj_textured", [C.c_char_p, C.c_char_p, fp, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), fp, C.c_int,
                                        C.POINTER(C.c_int32), C.POINTER(C.c_char_p), C.c_int]),
@@ -1390,6 +1403,70 @@ class Mesh:
         ms = np.zeros(3, np.float64)
         _check(self.lib, self.lib.immesh_mesh_render_textured_stats(ms.ctypes.data_as(C.POINTER(C.c_double))), "mesh_render_textured_stats")
         return dict(zip(("pass_a", "pass_b", "score"), (float(v) for v in ms)))
+
+    def texture_gains(self, rows, cameras, images, *, z_near=0.1, z_far=1000.0, min_cos=0.0, min_visible_permille=0, two_sided=False, positions=0,
+                      sigma_n=10.0, sigma_g=0.1, max_pairs=1 << 20, max_image_bytes=0, pairs=False):
+        """Colour equalisation between cameras (Brown & Lowe gain compensation): one gain per camera and channel so that cameras agree
+        on the facets several of them see.  rows: texture_select's or texture_rows' result (cam, uv), before any bake; cameras: full
+        camera tuples indexed as the rows index them (by frame number for texture_rows); images: per camera an HxWx3 uint8 numpy array
+        or CUDA torch tensor (all one kind), None for a camera that takes no part (every camera that textures a row needs one).  The
+        select keywords decide whether an observer sees a facet: pass the rows' own.  Blocking, ordered behind the queued frames; writes
+        nothing on the handle.  Returns dict(gains float64[n_cams, 3], counts {TEXTURE_GAINS_COUNT_KEYS: int}) and with pairs=True also
+        pair_cam int32[n_pairs, 2] (observer k, chosen c) and pair_sums int64[n_pairs, 7] (n, S_k[3], S_c[3]).  Correct the images with
+        apply_gains, then bake, render or export them."""
+        arr, n_cams = texture_cameras(cameras)
+        imgs, on_device, keep = texture_images(images)
+        cam = np.ascontiguousarray(rows["cam"], dtype=np.int32).reshape(-1)
+        uv = np.ascontiguousarray(rows["uv"], dtype=np.float32).reshape(-1, 6)
+        sel = _TexCfg(float(z_near), float(z_far), float(min_cos), int(min_visible_permille), 1 if two_sided else 0, int(positions), 0)
+        cfg = _TexGainsCfg(sel, float(sigma_n), float(sigma_g), int(max_pairs), int(max_image_bytes))
+        gains = np.zeros((max(n_cams, 1), 3), np.float64)
+        cap = int(max_pairs) if pairs else 0
+        pc = np.zeros((max(cap, 1), 2), np.int32)
+        ps = np.zeros((max(cap, 1), 7), np.int64)
+        npairs = C.c_int64(0)
+        counts = np.zeros(8, np.int64)
+        i64 = C.POINTER(C.c_int64)
+        _check(self.lib, self.lib.immesh_mesh_texture_gains(self._h, arr, n_cams, imgs, on_device, cam.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                            uv.ctypes.data_as(C.POINTER(C.c_float)), len(cam), C.byref(cfg),
+                                                            gains.ctypes.data_as(C.POINTER(C.c_double)),
+                                                            pc.ctypes.data_as(C.POINTER(C.c_int32)) if pairs else None, ps.ctypes.data_as(i64) if pairs else None,
+                                                            C.byref(npairs), counts.ctypes.data_as(i64)), "mesh_texture_gains")
+        del keep
+        out = dict(gains=gains[:n_cams].copy(), counts=dict(zip(TEXTURE_GAINS_COUNT_KEYS, (int(v) for v in counts))))
+        if pairs:
+            out.update(pair_cam=pc[:npairs.value].copy(), pair_sums=ps[:npairs.value].copy())
+        return out
+
+    def texture_gains_stats(self):
+        """the phases of this thread's last texture_gains in ms: dict(chosen, observers (CUDA events; host images: with the uploads they
+        wait for), solve (host clock, read-back included))"""
+        ms = np.zeros(3, np.float64)
+        _check(self.lib, self.lib.immesh_mesh_texture_gains_stats(ms.ctypes.data_as(C.POINTER(C.c_double))), "mesh_texture_gains_stats")
+        return dict(zip(("chosen", "observers", "solve"), (float(v) for v in ms)))
+
+    def apply_gains(self, images, gains):
+        """The corrected images: each channel min(255, floor(v g + 0.5)) with g = gains[k][ch].  images: HxWx3 uint8 numpy arrays or
+        CUDA torch tensors (all one kind; None stays None); returns new images of the same kind (device images: one kernel on the mesh
+        stream)."""
+        images = list(images)
+        g = np.ascontiguousarray(gains, dtype=np.float64).reshape(-1, 3)
+        if len(g) < len(images):
+            raise ValueError("apply_gains: one gain row per image")
+        outs = []
+        for im in images:
+            if im is None:
+                outs.append(None)
+            elif type(im).__module__.split(".")[0] == "torch":
+                outs.append(im.new_empty(im.shape).contiguous())
+            else:
+                outs.append(np.empty(np.asarray(im).shape, np.uint8))
+        ia, on_device, keep = texture_images(images)
+        oa, _, okeep = texture_images(outs)
+        _check(self.lib, self.lib.immesh_texture_apply_gains(self._h, ia, oa, len(images), on_device, g.ctypes.data_as(C.POINTER(C.c_double))),
+               "texture_apply_gains")
+        del keep, okeep
+        return outs
 
     def region_stream(self, region_size=10.0, cap=1 << 16):
         """(region_keys int32[nr,3], region_offsets int32[nr+1], triangles int32[nt,3]) -- the viewer's region-bucketed triangle sets."""

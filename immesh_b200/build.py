@@ -230,6 +230,21 @@ def build_texture_render(force=False):
     return EMU_TEXTURE_RENDER
 
 
+EMU_TEXTURE_GAINS = os.path.join(_ROOT, "tests", "texture_gains", "libimmesh_emu_texture_gains.so")
+
+
+def build_texture_gains(force=False):
+    """tests/texture_gains: the colour equalisation's bodies, argument check and host solve (immesh_b200/csrc/texture_gains_core.cuh, with
+    the bake's scaling and batch plan, the selection's "seen" test and the rasteriser's bodies) in the device call's orchestration --
+    chosen side, observer passes per host-image batch, compaction and solve -- and the gains' host apply, built for the host"""
+    src = os.path.join(_ROOT, "tests", "texture_gains", "emu_texture_gains.cpp")
+    deps = [src] + _sources(CSRC, (".cuh",)) + [os.path.join(_ROOT, "include", "immesh_b200.h")]
+    if force or _newer(EMU_TEXTURE_GAINS, deps):
+        subprocess.check_call([GXX, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall", "-Wno-unknown-pragmas", "-I/usr/local/cuda/include", "-shared",
+                               "-o", EMU_TEXTURE_GAINS, src])
+    return EMU_TEXTURE_GAINS
+
+
 EMU_VIEW_OVERLAY = os.path.join(_ROOT, "tests", "view_overlay", "libimmesh_emu_view_overlay.so")
 
 
@@ -377,6 +392,7 @@ def build_all(force=False):
     build_texture_bake(force)
     build_texture_online(force)
     build_texture_render(force)
+    build_texture_gains(force)
     build_changes(force)
     build_lio_feed(force)
     build_lio_feed_markers(force)

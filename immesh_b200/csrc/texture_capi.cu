@@ -21,11 +21,6 @@ namespace {
 
 // per live record (mesh_tri_order's rec index): this camera's counts, and the best camera so far with its distance and counts
 struct TexFacets { int *won, *cov, *best_cam, *best_won, *best_cov; double* best_e2; };
-// k_tex_tile counts a slot's pixels at its live record's index
-struct TexRowOf {
-    const int* row_of;
-    __device__ __forceinline__ int operator()(int slot) const { return row_of[slot]; }
-};
 
 __device__ __forceinline__ void tex_facet_corners(const MeshDev& M, int pos_mode, const int4& r, float4* q) {
     tex_corners(tex_vertex(M, pos_mode, r.x), tex_vertex(M, pos_mode, r.y), tex_vertex(M, pos_mode, r.z), (int)(M.tri_flip[r.w] & 1ull), q);

@@ -135,6 +135,12 @@ IM_HD void txo_face_uv(const float* uv_s, int flip, float* uv) {
 
 #ifdef __CUDACC__
 __device__ __forceinline__ float4 tex_vertex(const MeshDev& M, int pos_mode, int v) { return view_vertex(M.vpos, M.vsmooth, M.vsmoothed, pos_mode, v); }
+// k_tex_tile counts a slot's pixels at an index of the caller's (immesh_mesh_texture_select: the live record's; texture_gains: the
+// snapshot row's)
+struct TexRowOf {
+    const int* row_of;
+    __device__ __forceinline__ int operator()(int slot) const { return row_of[slot]; }
+};
 
 // one block per tile, one thread per pixel (k_view_tile's shape and visibility): the bin's set-ups staged IM_RT_THREADS at a time in
 // shared memory; a covered sample is counted for its facet (ballot per warp, shared sum per block, one atomic per facet and batch), the

@@ -1096,6 +1096,63 @@ int immesh_mesh_render_textured(immesh_mesh_t* h, const immesh_texture_camera* v
  * ms [3] = pass A (snapshot order, binning, tiles), pass B (with host images the uploads it waits for included), score (with a host
  * truth image its upload included). */
 int immesh_mesh_render_textured_stats(double* ms /*[3]*/);
+/* Colour equalisation between cameras: each facet takes its colour from one camera, and each camera has its own exposure and white
+ * balance, so the textured mesh shows brightness steps wherever neighbouring facets chose different cameras.  Gain compensation in the
+ * style of Brown & Lowe (panorama stitching, OpenCV's GainCompensator) solves one gain per camera and channel so that cameras agree
+ * where they see the same surface; the mesh gives that overlap exactly: a facet that camera k sees and camera c textures.
+ *   immesh_mesh_texture_gains: blocking, on the mesh stream behind the frames already queued; it reads the mesh and writes nothing on
+ *     the handle.  Input: the rows of texture_select or texture_rows (facet_cam, facet_uv, n_facets = the live triangle count), before
+ *     any bake; cams [n_cams] full cameras indexed as the rows index them (by frame number for texture_rows); images [n_cams] as
+ *     immesh_mesh_texture_bake's (on_device 1: device memory of h's device; 0: host memory uploaded in camera order through two
+ *     alternating arenas of cfg.max_image_bytes); a NULL image: the camera takes no part in the solve.  cfg.sel is the select rule
+ *     that decides whether an observer sees a facet: pass the rows' own positions.
+ *   Outputs: gains [n_cams][3] (float64, channel order of the images); pair_cam [max_pairs][2] (k, c) and pair_sums [max_pairs][7]
+ *     (n, S_k[3], S_c[3]) or NULL; *n_pairs (or NULL); counts [8] (or NULL): pairs, sample pairs used, sample pairs clipped, observer
+ *     cameras rasterised, cameras left at gain 1, CG iterations (the most over the three channels), pixels rasterised (w h summed over
+ *     the observers), 0.  *n_pairs > cfg.max_pairs: IMMESH_E_CAPACITY with *n_pairs and counts set, no gain or pair written.
+ *   Rule (defined here), float64 in the order written, without fused multiply-adds:
+ *     1. Sample points: the 10 barycentric points (b0, b1, b2) = (i / 6, j / 6, l / 6) with i, j, l >= 1, i + j + l = 6, in the order
+ *        i = 1..4, then j = 1..5 - i (l = 6 - i - j), applied to the corners in the row's face order q0 q1 q2.
+ *     2. Chosen side: row f with c = facet_cam[f] >= 0: its uv scaled to image c by the bake's rule 1 (W x H the image, Ws x Hs =
+ *        cams[c]'s size), the point x = (b0 u'0 + b1 u'1) + b2 u'2, y likewise, read at the nearest pixel (floor(x + 0.5), floor(y +
+ *        0.5)) clamped to [0, W - 1] x [0, H - 1]: 10 RGB samples per textured row.
+ *     3. Observer side: every camera k with an image, k != c, that sees f by texture_select's steps 1-3 (cfg.sel's z range, rule and
+ *        positions, f's current flip): select's step-5 uv of f at cams[k], scaled to image k by rule 1, sampled as in 2.
+ *     4. Clipping: a sample pair (I_k, I_c) is dropped when any of its six channel values is 0 or 255.
+ *     5. Pair (k, c): per kept sample pair n += 1, S_k[ch] += I_k[ch], S_c[ch] += I_c[ch]; int64 sums, so exact and independent of
+ *        order.  A pair exists where n >= 1; the list is in ascending (k, c).
+ *     6. Normal equations per channel, K = n_cams unknowns: for each pair (a = k, b = c), A[a][a] += (S_a S_a / n) / sn2 + n / sg2,
+ *        A[b][b] += (S_b S_b / n) / sn2 + n / sg2, A[a][b] and A[b][a] each -= (S_a S_b / n) / sn2, rhs[a] and rhs[b] each += n / sg2
+ *        (sn2 = sigma_n sigma_n, sg2 = sigma_g sigma_g; products of int64 sums as doubles).  A camera in no pair takes the row g = 1
+ *        (A = 1, rhs = 1).  A is symmetric positive definite with off-diagonal entries <= 0, so every gain is > 0.
+ *     7. Solve: Jacobi-preconditioned conjugate gradients on the host from g = 1, dot products summed in camera order, the matrix
+ *        applied as its diagonal then the pairs in list order; stop when |r| <= 1e-12 |rhs| or after max(100, 2 K) iterations.
+ *   IMMESH_E_INVALID, nothing written: NULL h, cams, images, cfg or gains; n_cams < 1; on_device not 0 / 1; n_facets other than the
+ *     live triangle count or > 0 with NULL rows; the bake's row checks (facet_cam in [-1, n_cams), finite uv); a textured row whose
+ *     camera has a NULL image; a given image the bake refuses (sizes below 1, pitch below 3 width, a host image above max_image_bytes);
+ *     a camera with an image that texture_select refuses; a cfg.sel texture_select refuses; sigma_n or sigma_g not finite or not > 0;
+ *     max_pairs < 1; max_image_bytes < 0; a sharded handle.
+ *   Not modelled: blending several views, local seam levelling, bias, gamma or vignetting, lens distortion.
+ * immesh_texture_apply_gains: the corrected images, each channel out = min(255, floor(in g + 0.5)) in float64 with g = gains[k][ch].
+ *   in [n] and out [n] images of equal sizes (out may be in: in place); an entry with NULL in data is skipped.  on_device 1: device
+ *   memory of h's device, one kernel on h's stream, blocking; 0: host memory, a host loop.  The corrected images then go unchanged into
+ *   texture_bake, render_textured and write_png.  IMMESH_E_INVALID, nothing written: NULL h, in, out or gains; n < 0; on_device not
+ *   0 / 1; an entry with a NULL out, a size below 1, sizes that differ or a pitch below 3 width; a gain not finite or < 0. */
+typedef struct {
+    immesh_texture_config sel;   /* the select rule deciding whether an observer sees a facet; positions: the rows' own */
+    double sigma_n, sigma_g;     /* Brown & Lowe's sigmas in 0-255 units: finite, > 0 (OpenCV's defaults: 10 and 0.1) */
+    int64_t max_pairs;           /* >= 1: the capacity of the pair list */
+    int64_t max_image_bytes;     /* host images: bytes of each of the two upload arenas (0: 512 MiB); must hold the largest image */
+} immesh_texture_gains_config;
+int immesh_mesh_texture_gains(immesh_mesh_t* h, const immesh_texture_camera* cams, int n_cams, const immesh_texture_image* images /*[n_cams]*/,
+                              int on_device, const int32_t* facet_cam /*[n_facets]*/, const float* facet_uv /*[n_facets][6]*/, int64_t n_facets,
+                              const immesh_texture_gains_config* cfg, double* gains /*[n_cams][3]*/, int32_t* pair_cam /*[max_pairs][2] or NULL*/,
+                              int64_t* pair_sums /*[max_pairs][7] or NULL*/, int64_t* n_pairs /*or NULL*/, int64_t* counts /*[8] or NULL*/);
+/* The phases of this thread's last immesh_mesh_texture_gains that reached the solve, in milliseconds: ms [3] = chosen samples (CUDA
+ * events; with host images the uploads they wait for), observer passes (CUDA events; likewise), solve (host clock, read-back included). */
+int immesh_mesh_texture_gains_stats(double* ms /*[3]*/);
+int immesh_texture_apply_gains(immesh_mesh_t* h, const immesh_texture_image* in /*[n]*/, const immesh_texture_image* out /*[n]*/, int n, int on_device,
+                               const double* gains /*[n][3]*/);
 /* Voxel_mapping::kitti_log (src/voxel_mapping_common.cpp:43-70): one line "stamp tx ty tz qx qy qz qw\n" of the pose log in the KITTI camera
  * frame for the pose part (rot_end, pos_end) of a state vector.  Host-side only. */
 int immesh_kitti_pose_line(const double* state /*[>=12]*/, double stamp, char* buf, int cap);
